@@ -10,6 +10,7 @@ reference architectures.
     python bench.py --impl reference ...      # the reference networks on the host CPU cores
     python bench.py --impl torch-cuda ...     # GPU STAND-IN for the reference's CUDA build (not the reference arm):
                                               # the oracle port of its networks on CUDA under fp16 autocast
+    python bench.py --dump-outputs DIR ...    # also write the last timed step's outputs as DIR/<name>.npy
 
 A step = one pass of the hot path over one frame.  `value` = hypotheses / step time with the frame,
 mesh and weights resident in HBM (device-timed with CUDA events, max over ranks); `e2e` = the same
@@ -31,6 +32,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
+sys.dont_write_bytecode = True  # the benchmark writes nothing into the source tree (it may be read-only)
 
 N_HYP = 252
 N_ITER = 5
@@ -43,13 +45,16 @@ def load_peaks():
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
             p = json.load(fh)
-        return dict(hbm_gbs=p["hbm_gbs"], tf_burst=p["bf16_tflops"], tf_sustained=p["bf16_tflops_sustained"], source="measured")
+        return dict(hbm_gbs=p["hbm_gbs"], hbm_source="MEASURED_PEAKS.json hbm_gbs (measured)",
+                    tflops=p["bf16_tflops_sustained"], tf_source="MEASURED_PEAKS.json bf16_tflops_sustained (measured)")
     except Exception:
-        return dict(hbm_gbs=6650.0, tf_burst=1590.0, tf_sustained=1400.0, source="fallback")
+        # without a measured file: the data-sheet figures, which bound what a kernel can reach but were not measured
+        return dict(hbm_gbs=3350.0, hbm_source="NVIDIA H100 SXM data sheet: 3.35 TB/s HBM3 at 700 W (not measured)",
+                    tflops=989.0, tf_source="NVIDIA H100 SXM data sheet: 989 TFLOP/s dense FP16 at 700 W (not measured)")
 
 
 class ClockSampler:
-    """SM clock / throttle-reason sampling during the timed region (B200_PROFILING.md): NVML every 20 ms when
+    """SM clock / throttle-reason sampling during the timed region: NVML every 20 ms when
     nvidia-ml-py is importable (an nvidia-smi process per sample is too slow for a 0.3 s loop), else nvidia-smi."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -114,6 +119,18 @@ class ClockSampler:
         reasons = set().union(*[r[2] for r in self.rows])
         return {"sm_mhz": float(np.median([r[0] for r in self.rows])), "sm_max_mhz": float(max(r[1] for r in self.rows)),
                 "reasons": sorted(reasons), "samples": len(self.rows), "source": "nvml" if self._nvml else "nvidia-smi"}
+
+
+def device_info(index):
+    """Name and power limit of the GPU the numbers were measured on (a power-capped card runs at lower clocks)."""
+    info = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=10).stdout.strip()
+        info["power_limit_w"] = float(out)
+    except Exception:
+        pass
+    return info
 
 
 def physical_cores_one_socket():
@@ -245,16 +262,6 @@ def run_reference(args, rank, world):
     })
 
 
-def load_traffic():
-    """DRAM bytes per launch of the roofline kernels, measured by `ncu --set full` and committed by
-    tools/ncu_summary.py as profiles/r02_ncu_traffic.json (kernel-name prefix -> dram read + write bytes of ONE launch)."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")) as fh:
-            return json.load(fh)
-    except Exception:
-        return {}
-
-
 class TorchCudaStandin:
     """GPU STAND-IN for the reference's nvdiffrast + PyTorch CUDA build, which cannot be installed here (SURVEY.md §8d
     last row): the oracle port of the reference networks as plain torch ops on CUDA under fp16 autocast with
@@ -340,6 +347,8 @@ def main():
     ap.add_argument("--no-standin", action="store_true", help="skip the torch-cuda stand-in / parity legs of the native line")
     ap.add_argument("--no-track", action="store_true", help="skip the track_one (BASELINE.json configs[2]) leg")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path returned in its last step (refined poses, scores, best index) as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "native" else args.warmup
 
@@ -444,6 +453,11 @@ def main():
         barrier()
     ms = e0.elapsed_time(e1) / args.steps
     launches = (_lib.launch_count() - launches0) // args.steps
+    if args.dump_outputs and rank == 0:
+        # the seeded synthetic scene, start poses and weights make these comparable between two builds
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t, dt in (("poses", poses_out, np.float32), ("scores", scores, np.float32), ("best_index", best, np.float64)):
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), t.detach().cpu().numpy().astype(dt))
     if world > 1:
         t = torch.tensor([ms], device="cuda")
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -466,26 +480,14 @@ def main():
     _lib.prof_enable(False)
     tf_ach = g_flops / (g_ms * 1e-3) / 1e12 if g_ms > 0 else 0.0
     gb_ach = c_bytes / (c_ms * 1e-3) / 1e9 if c_ms > 0 else 0.0
-    roofline = {"kernel": "tcgen05 implicit-GEMM kernels: gemm_tile_kernel<BN,CG,SLABS,PATCH>, gemm_swap(_patch)_kernel, stem_conv_kernel (15 conv + linear layers)", "bound": "tensor",
-                "achieved": tf_ach, "peak": peaks["tf_sustained"], "unit": "TFLOP/s", "frac": tf_ach / peaks["tf_sustained"],
-                "peak_source": f"MEASURED_PEAKS.json bf16_tflops_sustained ({peaks['source']}); kernel timed inside a long step",
-                "launches_timed": g_n, "avg_launch_ms": g_ms / max(g_n, 1), "share_of_step": (g_ms / 2) / ms,
-                "traffic": None}
-    traffic = load_traffic()  # measured by ncu --set full, committed under profiles/ (never a literal in this file)
-    tg = traffic.get("gemm_tile_kernel")
-    if tg:
-        roofline["traffic"] = tg["dram_bytes"]
-        roofline["traffic_note"] = (f"dram read+write of ONE launch of {tg['kernel']} ({tg.get('what', '')}) from {tg['source']}; "
-                                    f"algorithmic bytes of that launch: {tg.get('algorithmic_bytes')}")
+    roofline = {"kernel": "wgmma implicit-GEMM kernels: gemm_tile_kernel<BN>, stem_conv_kernel (15 conv + linear layers)", "bound": "tensor",
+                "achieved": tf_ach, "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": tf_ach / peaks["tflops"],
+                "peak_source": f"{peaks['tf_source']}; kernel timed inside a long step",
+                "launches_timed": g_n, "avg_launch_ms": g_ms / max(g_n, 1), "share_of_step": (g_ms / 2) / ms}
     roofline_raster = {"kernel": "crop producer: crop_tile_kernel<TILE> (meshlet binning + raster + shade + warp + normalise, one launch per pass)",
                        "bound": "hbm", "achieved": gb_ach, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": gb_ach / peaks["hbm_gbs"],
-                       "launches_timed": c_n, "avg_launch_ms": c_ms / max(c_n, 1), "share_of_step": (c_ms / 2) / ms, "traffic": None}
-    tc = traffic.get("crop_tile_kernel")
-    if tc:
-        roofline_raster["traffic"] = tc["dram_bytes"]
-        roofline_raster["traffic_note"] = f"dram read+write of ONE launch at N = {tc.get('n_hyp')} from {tc['source']}; algorithmic bytes: {tc.get('algorithmic_bytes')}"
-        if tc.get("issue_active_pct") is not None:
-            roofline_raster["issue_active_pct"] = tc["issue_active_pct"]
+                       "peak_source": peaks["hbm_source"],
+                       "launches_timed": c_n, "avg_launch_ms": c_ms / max(c_n, 1), "share_of_step": (c_ms / 2) / ms}
 
     # ---------------------------------------------------------------- ranking margin of this run (SURVEY.md §7 hard part v)
     sc_sorted = torch.sort(scores.float(), descending=True).values
@@ -568,13 +570,14 @@ def main():
                                    "(10242 v / 20480 f, 1024^2 texture), 640x480 synthetic RGB-D, 252 hyp, 5 refine iters + score + argmax",
                        "hypotheses": N_HYP, "refine_iters": N_ITER, "parallelism": f"hyp-shard x{world}",
                        "weights": "seeded random init of RefineNet/ScoreNetMultiPair (no checkpoints offline)",
-                       "l2": "working set per step ~3.5 GB of activations >> 126 MB L2 (no flush needed)"},
+                       "l2": "working set per step ~3.5 GB of activations >> 50 MB L2 (no flush needed)"},
             "whole_path_tflops": flops_step / (ms * 1e-3) / 1e12,
             "e2e": {"value": N_HYP / (e2e_ms * 1e-3), "unit": "hyp/s", "ms_per_step": e2e_ms, "h2d_bytes_per_step": int(h2d),
                     "d2h_bytes_per_step": int(d2h), "api": "FoundationPose.register(K, rgb, depth, ob_mask, iteration=5) with host numpy buffers",
                     "ms_per_step_before_value_loop": e2e_before, "ms_per_step_after_value_loop": e2e_after,
                     "note": "mean of two timed loops of `steps` calls, one before and one after the device-timed loop (the power-capped clock drifts while the die heats up)"},
             "gpu_launches": int(launches),
+            "device": device_info(local_rank),
             "clocks": clk.summary(),
             "roofline": roofline,
             "roofline_raster": roofline_raster,

@@ -1,4 +1,4 @@
-"""In-tree build of libfpose.so (sm_100a only).
+"""In-tree build of libfpose.so (sm_90a only).
 
 `python -m foundationpose_b200.build` or `__graft_entry__.build()`.  nvcc cross-compiles without a
 GPU; the resulting .so is git-ignored but travels to the GPU box with the snapshot.
@@ -15,7 +15,7 @@ LIB = os.path.join(LIBDIR, "libfpose.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",

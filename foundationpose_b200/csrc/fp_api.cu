@@ -577,7 +577,8 @@ int fp_create(fp_ctx** out) {
   FP_CUDA_OK(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   FP_CUDA_OK(cudaGetDeviceProperties(&prop, dev));
-  FP_REQUIRE(prop.major == 10, "libfpose targets sm_100a (B200); device %d is sm_%d%d", dev, prop.major, prop.minor);
+  FP_REQUIRE(prop.major == 9 && prop.minor == 0, "libfpose targets sm_90a (H100); device %d is sm_%d%d", dev, prop.major,
+             prop.minor);
   fp_ctx* c = new fp_ctx();
   c->device = dev;
   const char* ng = getenv("FPOSE_NO_GRAPH");

@@ -112,7 +112,7 @@ int fp_op_attention(const void* qkv, void* out, int B, int impl, void* stream) {
   ap.n_heads = 4;
   ap.scale = 0.08838834764831845f;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  (void)impl;  // one implementation: the tcgen05 kernel
+  (void)impl;  // one implementation: the wgmma kernel
   return fp::attn_tc_launch(ap, st);
 }
 

@@ -25,7 +25,7 @@ namespace fp {
     if (_rc) return _rc; \
   } while (0)
 
-// attention itself lives in fp_attn_tc.cu (tcgen05); this file keeps the SIMT pieces around it
+// attention itself lives in fp_attn_tc.cu (wgmma); this file keeps the SIMT pieces around it
 int attn_core_launch(const AttnParams& p, cudaStream_t stream) { return attn_tc_launch(p, stream); }
 
 // ------------------------------------------------------------------------------------------------
@@ -110,7 +110,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __half* __restrict
 
 int layernorm_launch(const __half* x, __half* y, const float* gamma, const float* beta, int rows, cudaStream_t stream) {
   if (rows == 0) return 0;
-  const int blocks = min((rows + 7) / 8, 148 * 8);
+  const int blocks = min((rows + 7) / 8, num_sms() * 8);
   FP_CUDA_OK(launch_pdl(layernorm_kernel, dim3(blocks), dim3(256), 0, stream, 1, x, y, gamma, beta, rows, 1e-5f));
   note_launches(1);
   FP_CUDA_OK(cudaGetLastError());
@@ -123,7 +123,7 @@ int layernorm_launch(const __half* x, __half* y, const float* gamma, const float
 //   kLN = false: token mean of the attention output -> [512] fp32   (scorer, score_network.py:72-74; the out_proj that
 //                follows is a [N,512] x [512,512] product done by rowwise_linear_kernel for all hypotheses at once)
 // The launch decides who owns the ranges: a CLUSTER of eight CTAs (one range each) at small batches — one CTA per
-// sequence left 32 hypotheses per GPU (8-GPU shards) on 32 of 148 SMs and a single tracked pose on one — or ONE CTA
+// sequence left 32 hypotheses per GPU (8-GPU shards) on 32 of 132 SMs and a single tracked pose on one — or ONE CTA
 // walking the eight ranges at large batches, where 8x the CTAs only add fixed cost.
 // Either way each range's partial sum is built in the same fixed order and the eight partials are added in range
 // order (rank 0 reads its peers' over distributed shared memory): the result is bit-identical for both launches and
@@ -225,8 +225,8 @@ __global__ void __launch_bounds__(kHeadWarps * 32) token_reduce_kernel(const __h
   }
 }
 
-// cluster of eight (the portable maximum) below this many sequences, one CTA per sequence above
-static inline int token_split_for(int B) { return B <= 74 ? kTokSplit : 1; }
+// cluster of eight (the portable maximum) while the eight CTAs per sequence fit four per SM, one CTA per sequence above
+static inline int token_split_for(int B) { return B * kTokSplit <= 4 * num_sms() ? kTokSplit : 1; }
 
 int head_final_launch(const __half* x, const float* gamma, const float* beta, const float* w, const float* bias,
                       float* out, int B, int T, int out_dim, cudaStream_t stream) {

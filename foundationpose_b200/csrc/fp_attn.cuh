@@ -18,7 +18,7 @@ struct AttnParams {
   int B, T, n_heads;
   float scale;  // 1/sqrt(head_dim)
 };
-// the tcgen05 kernel (fp_attn_tc.cu)
+// the wgmma kernel (fp_attn_tc.cu)
 int attn_core_launch(const AttnParams& p, cudaStream_t stream);
 int attn_tc_launch(const AttnParams& p, cudaStream_t stream);
 

@@ -1,24 +1,22 @@
-// fp_attn_tc.cu — softmax(Q K^T / sqrt(128)) V on the 5th-generation tensor cores (tcgen05).
+// fp_attn_tc.cu — softmax(Q K^T / sqrt(128)) V on the Hopper tensor cores (wgmma).
 //
 // Replaces the SDPA inside nn.MultiheadAttention (refine_network.py:56-70 `trans_head` / `rot_head`,
-// score_network.py:53 `att`) for T = 400 tokens and 4 heads of 128.  Persistent CTAs walk the (sequence, head[, group])
-// items; per item:
+// score_network.py:53 `att`) for T = 400 tokens and 4 heads of 128.  Persistent CTAs walk the work units
+// (sequence, head[, group], 128-row query tile); per unit:
 //
-//   smem   K of the head, resident: 2 slabs [400 keys][64 dims] (K-major, 128B swizzle)      100 KB
-//          Q tile, 128 query rows:  2 slabs [128][64]                                          32 KB
-//          V ring, 3 x 80 keys:     2 slabs [80 keys][64 dims] each (MN-major B operand)       60 KB
-//          O staging for the TMA store: 2 slabs [128][64]                                      32 KB
-//   TMEM   S = Q K^T  fp32, columns [0, 400)        (three key ranges: N = 208 + 176 + 16, K = 128)
-//          P = softmax numerators, fp16 pairs, columns [0, 200)   (overwrites S in place)
-//          O = P V    fp32, columns [384, 512)      (A operand = P read straight from TMEM)
-//   warps  0 = TMA producer, 1 = MMA issuer (one thread), 2..5 = softmax + epilogue (thread = query row:
-//          the row maximum / sum need no cross-thread reduction)
+//   smem   Q tile, 128 query rows: 2 slabs [128][64 dims] (K-major, 128B swizzle), 2 stages        64 KB
+//          K and V of 80 keys:     2 + 2 slabs [80 keys][64 dims], 3 stages                         120 KB
+//   warps  thread 0 = TMA producer; warpgroups 1, 2 = query rows [0, 64) and [64, 128) of the tile
 //
-// The four 128-row query tiles of a sequence run back to back; rows >= 400 of the last tile are
-// zero-filled on load and clipped on store by the TMA unit.
+// A consumer warpgroup walks the five 80-key chunks with an online softmax: S = Q K^T (m64n80k16, accumulators in
+// registers), running row maximum, P = exp2(S c - m c) packed to fp16 A fragments in registers, O = O alpha + P V
+// (m64n128k16, V the MN-major B operand straight from the TMA tile), row sum in fp32.  O / l goes to fp16 into the
+// warpgroup's own rows of the Q stage and leaves by TMA store.  Rows >= 400 of the last tile are zero-filled on load
+// and clipped on store by the TMA unit.
 #include "fp_attn.cuh"
 #include "fp_common.cuh"
 #include "fp_gemm.cuh"
+#include "fp_wgmma.cuh"
 
 namespace fp {
 
@@ -30,75 +28,20 @@ namespace {
 
 constexpr int T = 400;
 constexpr int DH = 128;
-constexpr int kKSlab = T * 128;           // bytes of one K slab (400 rows x 128 B)
-constexpr int kQSlab = 128 * 128;         // 16 KB
-constexpr int kVKeys = 80;                // keys per V chunk
-constexpr int kVSlab = kVKeys * 128;      // 10 KB: [80 keys][64 dims]
-constexpr int kVStages = 3;
-constexpr int kOffK = 0;
-constexpr int kOffQ = kOffK + 2 * kKSlab;              // 102400
-constexpr int kOffV = kOffQ + 2 * kQSlab;              // 135168
-constexpr int kOffO = kOffV + kVStages * 2 * kVSlab;   // 196608
-constexpr int kOffBar = kOffO + 2 * kQSlab;            // 229376
+constexpr int kQTiles = (T + 127) / 128;    // 4
+constexpr int kKeys = 80;                   // keys per chunk
+constexpr int kChunks = T / kKeys;          // 5
+constexpr int kKVSlab = kKeys * 128;        // 10 KB: [80 keys][64 dims]
+constexpr int kKVStage = 4 * kKVSlab;       // K dims [0,64), [64,128); V dims [0,64), [64,128)
+constexpr int kKVStages = 3;
+constexpr int kQSlab = 128 * 128;           // 16 KB: [128 rows][64 dims]
+constexpr int kQStage = 2 * kQSlab;
+constexpr int kQStages = 2;
+constexpr int kOffKV = 0;
+constexpr int kOffQ = kOffKV + kKVStages * kKVStage;  // 122880
+constexpr int kOffBar = kOffQ + kQStages * kQStage;   // 188416
 constexpr int kSmem = kOffBar + 256 + 1024;
-constexpr int kTmemCols = 512;
-constexpr uint32_t kColO = 384;
-constexpr int kThreadsTc = 192;
-
-// instruction descriptors (cute::UMMA::InstrDescriptor): fp16 x fp16 -> fp32, M = 128
-__host__ __device__ constexpr uint32_t idesc(uint32_t n, uint32_t b_mn_major) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | (0u << 15) | (b_mn_major << 16) | ((n >> 3) << 17) | ((128u >> 4) << 24);
-}
-
-// B operand, MN-major, 128B swizzle: slab [k rows][64 n-elements]; 8-row groups 1024 B apart (SBO),
-// the two 64-wide n-atoms `lbo_bytes` apart (LBO).
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc_,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc_), "r"(accumulate)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-// 16 packed registers (32 fp16 values of this thread's row) -> 16 TMEM columns
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&v)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(v[0]),
-               "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+constexpr int kThreadsTc = 384;
 
 __device__ __forceinline__ void tma_load_3d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2) {
   asm volatile(
@@ -114,15 +57,6 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void*
                : "memory");
 }
 
-// two softmax numerators: p = exp2(s * c - m * c) in fp32 (MUFU.EX2; an ex2.approx.f16x2 variant was measured: the
-// SASS is two scalar MUFU.EX2.F16, no gain), packed to the fp16 pair that the PV MMA reads from TMEM
-__device__ __forceinline__ uint32_t exp2_pair(uint32_t s0, uint32_t s1, float c, float mc, float& l) {
-  const float p0 = exp2f(fmaf(__uint_as_float(s0), c, -mc));
-  const float p1 = exp2f(fmaf(__uint_as_float(s1), c, -mc));
-  l += p0 + p1;
-  return pack_half2(p0, p1);
-}
-
 struct TcParams {
   int q_col, k_col, v_col;  // column of head 0 inside a qkv row (group offset added per work item)
   int group_col_stride;
@@ -130,332 +64,222 @@ struct TcParams {
   int B, H, G;              // work items: (sequence, head, group)
 };
 
-// Persistent: one CTA per SM walks the (sequence, head, group) items.  Per 128-row query tile
-//   MMA warp    S_a = Q K[0,208)^T | S_b = Q K[208,384)^T | (after the previous tile's O left TMEM) S_c = Q K[384,400)^T
-//               ... P ready ...  O = P V  (5 V chunks)
-//   softmax     max over S_a while S_b is still being computed, max over S_b, S_c; exp pass (P over S in place);
-//               ... O ready ...  O -> registers -> smem -> TMA store
-// O lives in TMEM columns [384, 512): the next tile's S_a / S_b (columns [0, 384)) are issued right behind the PV
-// MMAs, so they run while the softmax warps are still draining O; only the 16-key tail S_c waits for that.
-// K of the next item is fetched as soon as the last S MMA of the current item has retired.
 __global__ void __launch_bounds__(kThreadsTc, 1)
-    attn_tc_kernel(const __grid_constant__ CUtensorMap map_qk,  // (cols, T, B), box (64, 200, 1): K halves
+    attn_tc_kernel(const __grid_constant__ CUtensorMap map_kv,  // (cols, T, B), box (64, 80, 1): K and V chunks
                    const __grid_constant__ CUtensorMap map_q,   // (cols, T, B), box (64, 128, 1)
-                   const __grid_constant__ CUtensorMap map_v,   // (cols, T, B), box (64, 80, 1)
-                   const __grid_constant__ CUtensorMap map_o,   // (512, T, B, G), box (64, 128, 1, 1)
+                   const __grid_constant__ CUtensorMap map_o,   // (512, T, B, G), box (64, 64, 1, 1)
                    const TcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBar);
-  uint64_t* k_full = bars + 0;
-  uint64_t* k_empty = bars + 1;
-  uint64_t* q_full = bars + 2;
-  uint64_t* q_empty = bars + 3;
-  uint64_t* sa_full = bars + 4;
-  uint64_t* sb_full = bars + 5;
-  uint64_t* sc_full = bars + 6;
-  uint64_t* p_ready = bars + 7;               // [3]: keys [0,160), [160,320), [320,400) of P are in TMEM
-  uint64_t* o_full = bars + 10;
-  uint64_t* s_free = bars + 11;
-  uint64_t* v_full = bars + 12;               // [3]
-  uint64_t* v_empty = bars + 12 + kVStages;   // [3]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 12 + 2 * kVStages);
+  uint64_t* q_full = bars;                           // [kQStages]
+  uint64_t* q_empty = bars + kQStages;               // [kQStages]
+  uint64_t* kv_full = bars + 2 * kQStages;           // [kKVStages]
+  uint64_t* kv_empty = bars + 2 * kQStages + kKVStages;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int total = p.B * p.H * p.G;
+  const int total = p.B * p.H * p.G * kQTiles;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&map_qk);
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&map_kv);
     tma_prefetch_desc(&map_q);
-    tma_prefetch_desc(&map_v);
     tma_prefetch_desc(&map_o);
-    mbar_init(k_full, 1);
-    mbar_init(k_empty, 1);
-    mbar_init(q_full, 1);
-    mbar_init(q_empty, 1);
-    mbar_init(sa_full, 1);
-    mbar_init(sb_full, 1);
-    mbar_init(sc_full, 1);
-    for (int i = 0; i < 3; ++i) mbar_init(&p_ready[i], 128);
-    mbar_init(o_full, 1);
-    mbar_init(s_free, 128);
-    for (int i = 0; i < kVStages; ++i) {
-      mbar_init(&v_full[i], 1);
-      mbar_init(&v_empty[i], 1);
+    for (int i = 0; i < kQStages; ++i) {
+      mbar_init(&q_full[i], 1);
+      mbar_init(&q_empty[i], 2);  // one arrival per consumer warpgroup, after its O stores have left the stage
+    }
+    for (int i = 0; i < kKVStages; ++i) {
+      mbar_init(&kv_full[i], 1);
+      mbar_init(&kv_empty[i], 256);
     }
     mbar_fence_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   pdl_trigger();
   pdl_wait();
 
-  auto item = [&](int w, int& b, int& h, int& g, int& gcol) {
+  auto unit = [&](int u, int& b, int& h, int& g, int& gcol, int& qt) {
+    qt = u % kQTiles;
+    const int w = u / kQTiles;
     b = w % p.B;
     h = (w / p.B) % p.H;
     g = w / (p.B * p.H);
     gcol = g * p.group_col_stride + h * DH;
   };
 
-  if (warp == 0) {
-    if (lane == 0) {
-      int vs = 0, vph = 0, it = 0, tc = 0;
-      for (int w = blockIdx.x; w < total; w += gridDim.x, ++it) {
-        int b, h, g, gcol;
-        item(w, b, h, g, gcol);
-        // K of this (sequence, head): 2 dim-slabs x 2 row halves; the buffer is free once the previous item's last
-        // S MMA has retired
-        mbar_wait(k_empty, (it & 1) ^ 1);
-        mbar_expect_tx(k_full, 2 * kKSlab);
+  if (threadIdx.x < 128) {
+    if (threadIdx.x == 0) {
+      int qs = 0, qph = 0, ks = 0, kph = 0;
+      for (int u = blockIdx.x; u < total; u += gridDim.x) {
+        int b, h, g, gcol, qt;
+        unit(u, b, h, g, gcol, qt);
+        mbar_wait(&q_empty[qs], qph ^ 1);
+        mbar_expect_tx(&q_full[qs], kQStage);
         for (int s = 0; s < 2; ++s)
-          for (int half = 0; half < 2; ++half)
-            tma_load_3d(&map_qk, k_full, smem + kOffK + s * kKSlab + half * 200 * 128, gcol + p.k_col + s * 64, half * 200, b);
-        for (int qt = 0; qt < 4; ++qt, ++tc) {
-          mbar_wait(q_empty, (tc & 1) ^ 1);
-          mbar_expect_tx(q_full, 2 * kQSlab);
-          for (int s = 0; s < 2; ++s)
-            tma_load_3d(&map_q, q_full, smem + kOffQ + s * kQSlab, gcol + p.q_col + s * 64, qt * 128, b);
-          for (int c = 0; c < T / kVKeys; ++c) {
-            mbar_wait(&v_empty[vs], vph ^ 1);
-            mbar_expect_tx(&v_full[vs], 2 * kVSlab);
-            for (int s = 0; s < 2; ++s)
-              tma_load_3d(&map_v, &v_full[vs], smem + kOffV + (vs * 2 + s) * kVSlab, gcol + p.v_col + s * 64, c * kVKeys, b);
-            if (++vs == kVStages) {
-              vs = 0;
-              vph ^= 1;
-            }
+          tma_load_3d(&map_q, &q_full[qs], smem + kOffQ + qs * kQStage + s * kQSlab, gcol + p.q_col + s * 64, qt * 128, b);
+        if (++qs == kQStages) {
+          qs = 0;
+          qph ^= 1;
+        }
+        for (int c = 0; c < kChunks; ++c) {
+          mbar_wait(&kv_empty[ks], kph ^ 1);
+          mbar_expect_tx(&kv_full[ks], kKVStage);
+          uint8_t* st = smem + kOffKV + ks * kKVStage;
+          for (int s = 0; s < 2; ++s) {
+            tma_load_3d(&map_kv, &kv_full[ks], st + s * kKVSlab, gcol + p.k_col + s * 64, c * kKeys, b);
+            tma_load_3d(&map_kv, &kv_full[ks], st + (2 + s) * kKVSlab, gcol + p.v_col + s * 64, c * kKeys, b);
+          }
+          if (++ks == kKVStages) {
+            ks = 0;
+            kph ^= 1;
           }
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t id_sa = idesc(208, 0), id_sb = idesc(176, 0), id_sc = idesc(16, 0), id_pv = idesc(128, 1);
-      int vs = 0, vph = 0, it = 0, tc = 0;
-      for (int w = blockIdx.x; w < total; w += gridDim.x, ++it) {
-        mbar_wait(k_full, it & 1);
-        for (int qt = 0; qt < 4; ++qt, ++tc) {
-          mbar_wait(q_full, tc & 1);
-          // P of the previous tile (TMEM columns [0, 200)) is the A operand of its PV MMAs: let them retire before
-          // S_a overwrites those columns
-          if (tc > 0) mbar_wait(o_full, (tc - 1) & 1);
-          tc_fence_after();
-          // S = Q K^T in three key ranges: [0,208), [208,384), [384,400); K = 128 = 2 slabs x 4 k-steps
-          auto s_group = [&](uint32_t key0, uint32_t id) {
-            for (int ks = 0; ks < 8; ++ks) {
-              const int s = ks >> 2, k = ks & 3;
-              const uint64_t da = umma_desc_sw128(smem_u32(smem + kOffQ + s * kQSlab)) + (uint64_t)(2 * k);
-              const uint64_t db = umma_desc_sw128(smem_u32(smem + kOffK + s * kKSlab + key0 * 128)) + (uint64_t)(2 * k);
-              umma_f16(tmem + key0, da, db, id, ks > 0 ? 1u : 0u);
-            }
-          };
-          s_group(0, id_sa);
-          umma_commit(sa_full);
-          s_group(208, id_sb);
-          umma_commit(sb_full);
-          // columns [384, 400) overlap the previous tile's O: wait until the softmax warps have read it out
-          mbar_wait(s_free, (tc & 1) ^ 1);
-          tc_fence_after();
-          s_group(384, id_sc);
-          umma_commit(sc_full);
-          umma_commit(q_empty);               // Q tile consumed
-          if (qt == 3) umma_commit(k_empty);  // K consumed: the next item's K may land
-          // O = P V, P (fp16) read from TMEM columns [0,200), V chunks of 80 keys from the ring
-          for (int c = 0; c < T / kVKeys; ++c) {
-            // the exp pass publishes P in three steps (chunks 0-1, 2-3, 4): PV starts behind it
-            if (c == 0 || c == 2 || c == 4) {
-              mbar_wait(&p_ready[c >> 1], tc & 1);
-              tc_fence_after();
-            }
-            mbar_wait(&v_full[vs], vph);
-            tc_fence_after();
-            const uint32_t vbase = smem_u32(smem + kOffV + vs * 2 * kVSlab);
-            for (int k = 0; k < kVKeys / 16; ++k) {
-              const uint64_t db = umma_desc_mn_sw128(vbase + k * 16 * 128, kVSlab);
-              const uint32_t a_tmem = tmem + (uint32_t)((c * kVKeys + k * 16) >> 1);
-              umma_f16_ts(tmem + kColO, a_tmem, db, id_pv, (c > 0 || k > 0) ? 1u : 0u);
-            }
-            umma_commit(&v_empty[vs]);
-            if (++vs == kVStages) {
-              vs = 0;
-              vph ^= 1;
-            }
-          }
-          umma_commit(o_full);
-        }
-      }
-    }
-  } else {
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
-    const uint32_t lane_base = tmem + ((uint32_t)(quarter * 32) << 16);
-    const bool leader = (warp == 2 && lane == 0);
-    const uint32_t row_off = (uint32_t)row * 128u, sw = (uint32_t)(row & 7);
-    int tc = 0;
-    for (int w = blockIdx.x; w < total; w += gridDim.x) {
-      int b, h, g, gcol;
-      item(w, b, h, g, gcol);
-      for (int qt = 0; qt < 4; ++qt, ++tc) {
-        // pass 1: row maximum, range by range as the S MMAs retire
-        float m = -INFINITY;
-        auto fold32 = [&](const uint32_t (&v)[32]) {
-#pragma unroll
-          for (int i = 0; i < 32; i += 2) m = fmaxf(m, fmaxf(__uint_as_float(v[i]), __uint_as_float(v[i + 1])));
-        };
-        // n chunks of 32 columns from column c0, software-pipelined: the next chunk's load is in flight while the
-        // current one is reduced
-        auto max_range = [&](uint32_t c0, int n) {
-          uint32_t va[32], vb[32];
-          tmem_ld32(lane_base + c0, va);
-          int k = 0;
-#pragma unroll 1
-          for (; k + 1 < n; k += 2) {
-            tmem_ld_wait();
-            tmem_ld32(lane_base + c0 + (uint32_t)(k + 1) * 32u, vb);
-            fold32(va);
-            tmem_ld_wait();
-            if (k + 2 < n) tmem_ld32(lane_base + c0 + (uint32_t)(k + 2) * 32u, va);
-            fold32(vb);
-          }
-          if (k < n) {
-            tmem_ld_wait();
-            fold32(va);
-          }
-        };
-        auto max16 = [&](uint32_t c) {
-          uint32_t v[16];
-          tmem_ld16(lane_base + c, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) m = fmaxf(m, __uint_as_float(v[i]));
-        };
-        mbar_wait(sa_full, tc & 1);
-        tc_fence_after();
-        max_range(0, 6);
-        max16(192);
-        mbar_wait(sb_full, tc & 1);
-        tc_fence_after();
-        max16(208);
-        max_range(224, 5);
-        mbar_wait(sc_full, tc & 1);
-        tc_fence_after();
-        max16(384);
-        const float mc = m * p.scale_log2e;
-        // pass 2: p = exp2(s*c - m*c), row sum, P (fp16 pairs) written over S, chunk by chunk behind the reads.
-        // The 16-key tail (columns [384,400), the only part of S that O's columns overlap) is consumed FIRST and
-        // held in registers, so the PV MMAs of the first keys may start while this pass is still running.
-        float l = 0.f;
-        uint32_t tail[8];
-        {
-          uint32_t v[16];
-          tmem_ld16(lane_base + 384, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 8; ++i) tail[i] = exp2_pair(v[2 * i], v[2 * i + 1], p.scale_log2e, mc, l);
-        }
-        auto publish = [&](int part) {
-          tmem_st_wait();
-          tc_fence_before();
-          mbar_arrive(&p_ready[part]);
-        };
-        // software-pipelined: the load of the next 32 columns is in flight while the current 32 are exponentiated
-        {
-          uint32_t va[32], vb[32], o[16];
-          tmem_ld32(lane_base, va);
-#pragma unroll 1
-          for (int c = 0; c < 384; c += 64) {
-            tmem_ld_wait();
-            tmem_ld32(lane_base + c + 32, vb);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = exp2_pair(va[2 * i], va[2 * i + 1], p.scale_log2e, mc, l);
-            tmem_st16(lane_base + (c >> 1), o);
-            if (c == 128) publish(0);  // keys [0,160)
-            tmem_ld_wait();
-            if (c + 64 < 384) tmem_ld32(lane_base + c + 64, va);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = exp2_pair(vb[2 * i], vb[2 * i + 1], p.scale_log2e, mc, l);
-            tmem_st16(lane_base + (c >> 1) + 16, o);
-            if (c == 256) publish(1);  // keys [160,320)
-          }
-        }
-        tmem_st8(lane_base + 192, tail);
-        publish(2);  // keys [320,400)
-        const float inv_l = 1.f / l;
-
-        // O tile: TMEM -> registers -> fp16 -> swizzled smem slabs -> TMA store
-        mbar_wait(o_full, tc & 1);
-        tc_fence_after();
-        if (leader) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // staging free again
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-#pragma unroll 1
-        for (int s = 0; s < 2; ++s) {
-          uint32_t v0[32], v1[32];
-          tmem_ld32(lane_base + kColO + s * 64, v0);
-          tmem_ld32(lane_base + kColO + s * 64 + 32, v1);
-          tmem_ld_wait();
-          uint8_t* slab = smem + kOffO + s * kQSlab;
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            uint32_t wv[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const float a0 = __uint_as_float(q < 4 ? v0[(q & 3) * 8 + 2 * k] : v1[(q & 3) * 8 + 2 * k]) * inv_l;
-              const float a1 = __uint_as_float(q < 4 ? v0[(q & 3) * 8 + 2 * k + 1] : v1[(q & 3) * 8 + 2 * k + 1]) * inv_l;
-              wv[k] = pack_half2(a0, a1);
-            }
-            *reinterpret_cast<uint4*>(slab + row_off + (((uint32_t)q ^ sw) << 4)) = make_uint4(wv[0], wv[1], wv[2], wv[3]);
-          }
-        }
-        tc_fence_before();
-        mbar_arrive(s_free);  // O has left TMEM: the next tile's S_c may overwrite columns [384, 400)
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (leader) {
-          for (int s = 0; s < 2; ++s) tma_store_4d(&map_o, smem + kOffO + s * kQSlab, h * DH + s * 64, qt * 128, b, g);
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-      }
-    }
-    if (leader) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem, kTmemCols);
+  const int ct = threadIdx.x - 128;
+  const int cw = ct >> 7;  // query rows [64 cw, 64 cw + 64) of the tile
+  const int lane = threadIdx.x & 31;
+  const int r0 = 64 * cw + 16 * ((ct >> 5) & 3) + (lane >> 2);  // this thread's rows: r0, r0 + 8
+  const int cq = 2 * (lane & 3);
+  const bool leader = ((ct & 127) == 0);
+  const float c = p.scale_log2e;
+  float s_acc[kKeys / 2], o[DH / 2];
+#pragma unroll
+  for (int i = 0; i < kKeys / 2; ++i) s_acc[i] = 0.f;
+  int qs = 0, qph = 0, ks = 0, kph = 0;
+  for (int u = blockIdx.x; u < total; u += gridDim.x) {
+    int b, h, g, gcol, qt;
+    unit(u, b, h, g, gcol, qt);
+#pragma unroll
+    for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};  // l: this thread's partial row sums
+    mbar_wait(&q_full[qs], qph);
+    const uint32_t qbase = smem_u32(smem + kOffQ + qs * kQStage) + (uint32_t)cw * 8192u;
+    for (int ch = 0; ch < kChunks; ++ch) {
+      mbar_wait(&kv_full[ks], kph);
+      const uint32_t kvbase = smem_u32(smem + kOffKV + ks * kKVStage);
+      // S = Q K^T over the 80 keys of this chunk; K = 128 dims = 2 slabs x 4 k-steps
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        const int s = kk >> 2, k = kk & 3;
+        Wgmma<kKeys>::ss(s_acc, gmma_desc_sw128(qbase + s * kQSlab) + (uint64_t)(2 * k),
+                         gmma_desc_sw128(kvbase + s * kKVSlab) + (uint64_t)(2 * k), kk > 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(s_acc);
+      // running row maximum (a row's 80 values live in the 4 lanes of a quad)
+      float mx[2] = {m[0], m[1]};
+#pragma unroll
+      for (int j = 0; j < kKeys / 8; ++j) {
+        mx[0] = fmaxf(mx[0], fmaxf(s_acc[4 * j], s_acc[4 * j + 1]));
+        mx[1] = fmaxf(mx[1], fmaxf(s_acc[4 * j + 2], s_acc[4 * j + 3]));
+      }
+      float mc[2], alpha[2];
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+        mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+        alpha[hh] = exp2f((m[hh] - mx[hh]) * c);  // 0 on the first chunk (m = -inf)
+        m[hh] = mx[hh];
+        mc[hh] = mx[hh] * c;
+        l[hh] *= alpha[hh];
+      }
+#pragma unroll
+      for (int j = 0; j < DH / 8; ++j) {
+        o[4 * j] *= alpha[0];
+        o[4 * j + 1] *= alpha[0];
+        o[4 * j + 2] *= alpha[1];
+        o[4 * j + 3] *= alpha[1];
+      }
+      // P = exp2(s c - m c) in fp32 (row sums), packed to the fp16 A fragments of the PV wgmma
+      uint32_t pa[kKeys / 16][4];
+#pragma unroll
+      for (int j = 0; j < kKeys / 8; ++j) {
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const float p0 = exp2f(fmaf(s_acc[4 * j + 2 * hh], c, -mc[hh]));
+          const float p1 = exp2f(fmaf(s_acc[4 * j + 2 * hh + 1], c, -mc[hh]));
+          l[hh] += p0 + p1;
+          pa[j >> 1][(j & 1) * 2 + hh] = pack_half2(p0, p1);
+        }
+      }
+      // O += P V: V chunk [80 keys][128 dims] is the MN-major B operand (dims = N, two 64-dim slabs)
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < kKeys / 16; ++kk)
+        Wgmma<DH>::rs_mn(o, pa[kk], gmma_desc_mn_sw128(kvbase + 2 * kKVSlab + kk * 16 * 128, kKVSlab), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(o);
+      mbar_arrive(&kv_empty[ks]);
+      if (++ks == kKVStages) {
+        ks = 0;
+        kph ^= 1;
+      }
+    }
+    float inv[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
+      l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
+      inv[hh] = 1.f / l[hh];
+    }
+    // O tile -> fp16 -> this warpgroup's own rows of the Q stage (its Q reads have all retired) -> TMA store
+    uint8_t* qst = smem + kOffQ + qs * kQStage;
+#pragma unroll
+    for (int j = 0; j < DH / 8; ++j) {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int row = r0 + 8 * hh;
+        *reinterpret_cast<uint32_t*>(qst + (j >> 3) * kQSlab + row * 128 + ((((uint32_t)j & 7u) ^ (uint32_t)(row & 7)) << 4) +
+                                     cq * 2) = pack_half2(o[4 * j + 2 * hh] * inv[hh], o[4 * j + 2 * hh + 1] * inv[hh]);
+      }
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+    if (leader) {
+      for (int s = 0; s < 2; ++s)
+        tma_store_4d(&map_o, qst + s * kQSlab + cw * 8192, h * DH + s * 64, qt * 128 + 64 * cw, b, g);
+      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+      asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // the stage may be refilled once read out
+      mbar_arrive(&q_empty[qs]);
+    }
+    if (++qs == kQStages) {
+      qs = 0;
+      qph ^= 1;
+    }
   }
+  if (leader) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
 }  // namespace
 
 int attn_tc_launch(const AttnParams& p, cudaStream_t stream) {
-  FP_REQUIRE(p.T == T && p.n_heads == 4, "tcgen05 attention is specialised for T=400, 4 heads of 128");
-  FP_REQUIRE(p.ld_out == 512, "tcgen05 attention writes [*, 512] rows");
+  FP_REQUIRE(p.T == T && p.n_heads == 4, "wgmma attention is specialised for T=400, 4 heads of 128");
+  FP_REQUIRE(p.ld_out == 512, "wgmma attention writes [*, 512] rows");
   static std::atomic<unsigned long long> attr_mask{0};  // per device: the attribute is device state
   if (!device_bit_test(attr_mask)) {
     FP_CUDA_OK(cudaFuncSetAttribute(attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
     device_bit_set(attr_mask);
   }
   if (p.B == 0) return 0;
-  CUtensorMap mk, mq, mv, mo;
+  CUtensorMap mkv, mq, mo;
   const uint64_t E = 2;
   uint64_t d3[3] = {(uint64_t)p.ld, (uint64_t)T, (uint64_t)p.B};
   uint64_t s3[2] = {(uint64_t)p.ld * E, (uint64_t)p.ld * E * T};
-  uint32_t bk[3] = {64, 200, 1}, bq[3] = {64, 128, 1}, bv[3] = {64, (uint32_t)kVKeys, 1};
-  int rc = encode_map_f16(&mk, p.qkv, 3, d3, s3, bk);
+  uint32_t bkv[3] = {64, (uint32_t)kKeys, 1}, bq[3] = {64, 128, 1};
+  int rc = encode_map_f16(&mkv, p.qkv, 3, d3, s3, bkv);
   if (rc) return rc;
   rc = encode_map_f16(&mq, p.qkv, 3, d3, s3, bq);
-  if (rc) return rc;
-  rc = encode_map_f16(&mv, p.qkv, 3, d3, s3, bv);
   if (rc) return rc;
   uint64_t d4[4] = {512, (uint64_t)T, (uint64_t)p.B, (uint64_t)p.n_groups};
   uint64_t s4[3] = {512 * E, 512 * E * T, (uint64_t)p.out_group_stride * E};
   if (p.n_groups == 1) s4[2] = 512 * E * T * p.B;
-  uint32_t bo[4] = {64, 128, 1, 1};
+  uint32_t bo[4] = {64, 64, 1, 1};
   rc = encode_map_f16(&mo, p.out, 4, d4, s4, bo);
   if (rc) return rc;
   TcParams tp;
@@ -467,11 +291,11 @@ int attn_tc_launch(const AttnParams& p, cudaStream_t stream) {
   tp.B = p.B;
   tp.H = p.n_heads;
   tp.G = p.n_groups;
-  const int total = p.B * p.n_heads * p.n_groups;
+  const int total = p.B * p.n_heads * p.n_groups * kQTiles;
   const int sms = num_sms();
   FP_REQUIRE(sms > 0, "no CUDA device");
   dim3 grid(total < sms ? total : sms);
-  FP_CUDA_OK(launch_pdl(attn_tc_kernel, grid, dim3(kThreadsTc), kSmem, stream, 1, mk, mq, mv, mo, tp));
+  FP_CUDA_OK(launch_pdl(attn_tc_kernel, grid, dim3(kThreadsTc), kSmem, stream, 1, mkv, mq, mo, tp));
   note_launches(1);
   FP_CUDA_OK(cudaGetLastError());
   return 0;

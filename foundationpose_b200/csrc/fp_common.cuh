@@ -1,7 +1,7 @@
-// fp_common.cuh — shared device helpers for the sm_100a kernels of libfpose.
+// fp_common.cuh — shared device helpers for the sm_90a kernels of libfpose.
 //
-// Raw PTX wrappers for mbarrier / TMA / tcgen05 (no CUTLASS dependency).
-// Everything here targets sm_100a only; there is no fallback path.
+// Raw PTX wrappers for mbarrier / TMA / wgmma (no CUTLASS dependency).
+// Everything here targets sm_90a only; there is no fallback path.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -58,7 +58,7 @@ void set_last_error(const char* fmt, ...);
 // ----------------------------------------------------------------------------------------------
 // programmatic dependent launch (PDL).  Every kernel of a network pass is launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization: its CTAs may be scheduled (on SMs the previous kernel has
-// already left) and run their prologue — barrier init, TMEM allocation, tensor-map prefetch, loads of constant
+// already left) and run their prologue — barrier init, tensor-map prefetch, loads of constant
 // weights — while the previous kernel's last wave is still draining.  Contract inside a kernel: pdl_trigger()
 // early (lets the NEXT kernel be scheduled once every CTA of this one has started), and pdl_wait() before the
 // first access to global memory that an earlier kernel writes or reads (it returns when all earlier kernels of
@@ -163,9 +163,7 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
 
-// ---- 2-CTA (cta_group::2) variants: the CTA pair of a cluster drives one M=256 MMA; TMA bytes of both
-// CTAs are accounted on the leader's (rank 0) mbarrier, MMA completion is multicast to both.
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // clears the CTA-rank bit of a shared::cluster address
+// ---- clusters
 __device__ __forceinline__ uint32_t cluster_nctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
@@ -180,146 +178,54 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tma_load_5d_2sm(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2,
-                                                int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3),
-      "r"(c4)
-      : "memory");
+
+// wgmma (warpgroup MMA) ------------------------------------------------------------------------
+// fence before the first wgmma of a batch (orders earlier register / shared-memory accesses before it)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// wait until at most N committed groups of this warpgroup are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tma_load_2d_2sm(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-// arrive on the mbarrier at the same smem offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
-      "}" ::"r"(smem_u32(bar)),
-      "r"(rank)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar) & kPeerBitMask),
-      "h"((unsigned short)3)
-      : "memory");
+// read-out of fragment registers only after the wgmma that writes them has been waited for
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// tcgen05 ------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// whole warp
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T ; one thread issues.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once all previously issued MMAs (by this thread) have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 columns of fp32 accumulators -> 32 registers per thread (thread = lane/row)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]),
-        "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]),
-        "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// UMMA shared-memory descriptor: K-major operand, 128-byte swizzle, rows of 64 fp16 (128 B),
-// 8-row core-matrix groups 1024 B apart (SBO), LBO unused.  Layout per cute::UMMA::SmemDescriptor.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);  // start address  [0,14)
-  d |= (uint64_t)0 << 16;                        // leading byte offset (unused for SW128 K-major)
-  d |= (uint64_t)(1024 >> 4) << 32;              // stride byte offset [32,46)
-  d |= (uint64_t)1 << 46;                        // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                        // layout type: SWIZZLE_128B
-  return d;
-}
-// Same layout, arbitrary start row and group stride: tcgen05 applies the 128B swizzle to absolute shared-memory
-// address bits (tools/umma_probe.cu), so `smem_addr` may be any multiple of 128 B and `sbo_bytes` any multiple of
-// 16 B; the base-offset field stays 0.
-__device__ __forceinline__ uint64_t umma_desc_sw128_sbo(uint32_t smem_addr, uint32_t sbo_bytes) {
+// wgmma shared-memory descriptors (sm_90): start address, leading / stride byte offsets (16 B units), layout type in
+// bits [62, 64): 0 = no swizzle, 1 = 128-byte swizzle.
+//
+// K-major operand, 128-byte swizzle: rows of 64 fp16 (128 B), 8-row groups `sbo` bytes apart (1024 for a dense tile),
+// LBO unused.  Advancing 16 fp16 along K inside the swizzle atom is +32 B = +2 on the descriptor.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t sbo = 1024) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(sbo_bytes >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(sbo >> 4) << 32;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// Instruction descriptor for kind::f16, fp16 A/B (K-major both), fp32 accumulate, M=128.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t n, uint32_t m = 128u) {
-  return (1u << 4)               // c_format = F32
-         | (0u << 7)             // a_format = F16
-         | (0u << 10)            // b_format = F16
-         | (0u << 15)            // a K-major
-         | (0u << 16)            // b K-major
-         | ((n >> 3) << 17)      // N >> 3
-         | ((m >> 4) << 24);     // M >> 4
+// MN-major operand, 128-byte swizzle: slab [k rows][64 mn-elements]; 8-row k groups 1024 B apart (SBO), consecutive
+// 64-element mn atoms `lbo` bytes apart (LBO).
+__device__ __forceinline__ uint64_t gmma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
+}
+// K-major operand without swizzle: core matrices of 8 rows x 16 B; the two 8-element K halves of a k-step `lbo` bytes
+// apart, consecutive 8-row groups `sbo` bytes apart.
+__device__ __forceinline__ uint64_t gmma_desc_linear(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)(lbo >> 4) << 16;
+  d |= (uint64_t)(sbo >> 4) << 32;
+  return d;
 }
 
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {

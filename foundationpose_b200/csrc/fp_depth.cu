@@ -299,7 +299,7 @@ int start_poses_launch(const float* depth, const unsigned char* mask, int H, int
                        const float* rot_grid, int N, unsigned int* stats /*6 words of device scratch*/, float* poses_out,
                        float* info, cudaStream_t stream) {
   FP_CUDA_OK(cudaMemsetAsync(stats, 0, 6 * sizeof(unsigned int), stream));
-  mask_stats_kernel<<<148, 256, 0, stream>>>(depth, mask, H, W, stats);
+  mask_stats_kernel<<<num_sms(), 256, 0, stream>>>(depth, mask, H, W, stats);
   start_poses_kernel<<<1, 1024, 0, stream>>>(depth, mask, H, W, fx, fy, cx, cy, rot_grid, N, stats, poses_out, info);
   note_launches(2);
   FP_CUDA_OK(cudaGetLastError());

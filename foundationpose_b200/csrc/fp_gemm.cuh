@@ -1,5 +1,5 @@
 // fp_gemm.cuh — host-side description of one implicit-GEMM layer (conv / linear) for the
-// tcgen05 tile kernel in fp_gemm.cu.
+// wgmma tile kernel in fp_gemm.cu.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>

@@ -1,5 +1,5 @@
-// fp_stem.cu — the 7x7 / stride-2 stem convolution (6 -> 64 channels, 160x160 -> 80x80) as a tcgen05
-// implicit GEMM whose A operand is a *view* of one small shared-memory patch.
+// fp_stem.cu — the 7x7 / stride-2 stem convolution (6 -> 64 channels, 160x160 -> 80x80) as a wgmma implicit GEMM
+// whose A operand is a *view* of one small shared-memory patch.
 //
 // Replaces (reference): learning/models/refine_network.py:34-35 and score_network.py:37-38, the first
 // ConvBNReLU(C_in=6, C_out=64, kernel_size=7, stride=2) of encodeA / encoderA
@@ -12,20 +12,21 @@
 // even columns then odd columns ("EO" layout: [n][166 rows][2][84 column pairs][8 ch] fp16), and the tile
 // is 16 output rows x 8 output columns.  For filter row r and tap pair s (taps 2s, 2s+1) the K = 16 slice of
 // A for output pixel (i, j) is  E[2i + r][j + s] ++ O[2i + r][j + s]  (16 B each), i.e. in shared memory
-//     8 rows (j) at a 16 B pitch, 16 row groups (i) at a constant stride, two K chunks E / O at a constant offset
-// which is exactly tcgen05's un-swizzled K-major canonical layout ((8,m),(8,2)) : ((16 B, SBO), (2 B, LBO)).
-// So ONE 13 KB TMA box (37 rows x 2 x 11 pairs x 16 B) feeds all 7 x 4 = 28 MMAs (M = 128, N = 64, K = 16) of
-// a tile through 28 descriptors that differ only in their start address; the 56 KB of packed weights stay
-// resident in shared memory for the life of the (persistent) CTA.
+//     8 rows (j) at a 16 B pitch, row groups (i) at a constant stride, two K chunks E / O at a constant offset
+// which is exactly wgmma's un-swizzled K-major canonical layout ((8,m),(8,2)) : ((16 B, SBO), (2 B, LBO)).
+// So ONE 13 KB TMA box (37 rows x 2 x 11 pairs x 16 B) feeds all 7 x 4 = 28 k-steps of a tile through
+// descriptors that differ only in their start address; the 56 KB of packed weights stay resident in shared
+// memory for the life of the (persistent) CTA.
 //
-// Roles per CTA (320 threads, one CTA per SM): warp 0 = TMA producer (patch ring), warp 1 = MMA issuer,
-// warps 2..9 = two epilogue warpgroups, one per TMEM accumulator (TMEM -> +bias, ReLU -> fp16 -> 128B-swizzled
-// slab -> TMA tensor store), fp32 accumulators double-buffered in TMEM (2 x 64 columns).
+// Roles per CTA (384 threads, one CTA per SM): thread 0 = TMA producer (patch ring); warpgroups 1 and 2 = output
+// rows [0, 8) and [8, 16) of the tile (M = 64 each, N = 64, fp32 accumulators in registers), each with its own
+// epilogue (+bias, ReLU -> fp16 -> 128B-swizzled slab -> TMA tensor store of its 8 x 8 pixels).
 #include <stdlib.h>
 #include <string.h>
 
 #include "fp_common.cuh"
 #include "fp_gemm.cuh"
+#include "fp_wgmma.cuh"
 
 namespace fp {
 
@@ -37,7 +38,7 @@ int num_sms();
 
 namespace {
 
-constexpr int kThreadsStem = 320;
+constexpr int kThreadsStem = 384;
 constexpr int kTileH = 16, kTileW = 8;                   // output pixels per tile (M = 128)
 constexpr int kPatchRows = 2 * (kTileH - 1) + 7;         // 37 padded input rows
 constexpr int kPatchPairs = kTileW + 3;                  // 11 column pairs
@@ -48,25 +49,14 @@ constexpr int kPatchSlot = 13 * 1024;                    // ring slot (1024-alig
 constexpr int kStagesStem = 6;
 constexpr int kWTileBytes = 2 * 64 * 16;                 // one (r, s) weight tile: [E/O][64 ch][8 ci] fp16
 constexpr int kWBytes = 28 * kWTileBytes;                // 57,344 B
-constexpr int kSlab = 128 * 64 * 2;                      // 16 KB output slab
-constexpr int kStemSmem = kWBytes + kStagesStem * kPatchSlot + 4 * kSlab + 1024 + 256;
+constexpr int kHalfSlab = 64 * 64 * 2;                   // 8 KB: 64 output pixels x 64 channels
+constexpr int kStemSmem = kWBytes + kStagesStem * kPatchSlot + 4 * kHalfSlab + 1024 + 256;
 
 struct StemParams {
   int tiles_w, tiles_h, n_img, total_tiles;
   const float* bias;
   int relu;
 };
-
-// un-swizzled K-major operand: 8 rows at 16 B, row groups `sbo` bytes apart, the two 8-element K chunks
-// `lbo` bytes apart (cute::UMMA::make_umma_desc<Major::K>, LayoutType::INTERLEAVE)
-__device__ __forceinline__ uint64_t umma_desc_linear(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(lbo >> 4) << 16;
-  d |= (uint64_t)(sbo >> 4) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version (sm_100); layout type 0 = no swizzle
-  return d;
-}
 
 __device__ __forceinline__ void bulk_load_1d(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
@@ -83,43 +73,29 @@ __global__ void __launch_bounds__(kThreadsStem, 1)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* wsm = smem;
   uint8_t* ring = smem + kWBytes;
-  uint8_t* staging = ring + S * kPatchSlot;  // [2 groups][2][kSlab], 1024-aligned
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + 4 * kSlab);
-  uint64_t* full = bars;                    // [S]
-  uint64_t* empty = bars + S;               // [S]
-  uint64_t* tmem_full = bars + 2 * S;       // [2]
-  uint64_t* tmem_empty = bars + 2 * S + 2;  // [2]
-  uint64_t* w_full = bars + 2 * S + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * S + 6);
+  uint8_t* staging = ring + S * kPatchSlot;  // [2 warpgroups][2][kHalfSlab], 1024-aligned
+  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + 4 * kHalfSlab);
+  uint64_t* full = bars;       // [S]
+  uint64_t* empty = bars + S;  // [S]
+  uint64_t* w_full = bars + 2 * S;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_in);
     tma_prefetch_desc(&map_out);
     for (int s = 0; s < S; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], 128);
+      mbar_init(&empty[s], 256);
     }
     mbar_init(w_full, 1);
     mbar_fence_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 128);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int tiles_per_img = p.tiles_w * p.tiles_h;
   pdl_trigger();
 
-  if (warp == 0) {
+  if (threadIdx.x < 128) {
     // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
       mbar_expect_tx(w_full, kWBytes);
       bulk_load_1d(wsm, wpack, kWBytes, w_full);  // constant weights: fetched while the previous kernel drains
       pdl_wait();
@@ -137,102 +113,80 @@ __global__ void __launch_bounds__(kThreadsStem, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(64, 128);
-      mbar_wait(w_full, 0);
-      const uint32_t w_addr = smem_u32(wsm);
-      int stage = 0, phase = 0, it = 0;
-      for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x, ++it) {
-        const int acc = it & 1;
-        mbar_wait(&tmem_empty[acc], ((it >> 1) & 1) ^ 1);
-        mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * 64;
-        const uint32_t patch = smem_u32(ring + stage * kPatchSlot);
-#pragma unroll
-        for (int r = 0; r < 7; ++r) {
-#pragma unroll
-          for (int s = 0; s < 4; ++s) {
-            // A: rows j at 16 B from pair j + s of padded row 2i + r; row groups i two padded rows apart
-            const uint64_t da = umma_desc_linear(patch + r * kRowStride + s * 16, kParStride, 2 * kRowStride);
-            // B: [E/O][64 ch][8]: rows (channels) at 16 B, groups of 8 channels 128 B apart, K chunks 1 KB apart
-            const uint64_t db = umma_desc_linear(w_addr + (r * 4 + s) * kWTileBytes, 1024, 128);
-            umma_f16(d_tmem, da, db, idesc, (r | s) ? 1u : 0u);
-          }
-        }
-        umma_commit(&empty[stage]);
-        umma_commit(&tmem_full[acc]);
-        if (++stage == S) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue (warps 2..9)
-    // Two independent warpgroups: group g drains the tiles with (it & 1) == g, i.e. TMEM accumulator g, through its
-    // own pair of staging slabs and its own named barrier, so the per-tile chain (TMEM load -> smem -> TMA store)
-    // of one tile overlaps the next tile's.
-    const int quarter = warp & 3;     // TMEM lanes [32*quarter, +32)
-    const int grp = (warp - 2) >> 2;  // which accumulator / tile parity
-    const int row = quarter * 32 + lane;
-    const bool leader = (quarter == 2 && lane == 0);  // warps 2 and 6
-    const uint32_t row_off = (uint32_t)row * 128u;
-    const uint32_t sw = (uint32_t)(row & 7);
-    const float4* bias4 = reinterpret_cast<const float4*>(p.bias);
-    pdl_wait();  // the output buffer may still be read by an earlier kernel
-    int use = 0;
-    for (int t = blockIdx.x + grp * gridDim.x; t < p.total_tiles; t += 2 * gridDim.x, ++use) {
-      const int n = t / tiles_per_img, rem = t - n * tiles_per_img;
-      const int th = rem / p.tiles_w, tw = rem - th * p.tiles_w;
-      uint8_t* slab = staging + (grp * 2 + (use & 1)) * kSlab;
-      // the TMA store that last used this slab (two of this group's tiles ago) must have finished reading it
-      if (leader) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory");
-      mbar_wait(&tmem_full[grp], use & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + grp * 64 + h * 32, v);
-        tmem_ld_wait();
-        if (h == 1) {
-          tc_fence_before();
-          mbar_arrive(&tmem_empty[grp]);
-        }
-#pragma unroll
-        for (int q4 = 0; q4 < 4; ++q4) {
-          const int q = h * 4 + q4;
-          const float4 b0 = __ldg(bias4 + q * 2), b1 = __ldg(bias4 + q * 2 + 1);
-          const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-          float a[8];
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            a[k] = __uint_as_float(v[q4 * 8 + k]) + bb[k];
-            if (p.relu) a[k] = fmaxf(a[k], 0.f);
-          }
-          *reinterpret_cast<uint4*>(slab + row_off + (((uint32_t)q ^ sw) << 4)) =
-              make_uint4(pack_half2(a[0], a[1]), pack_half2(a[2], a[3]), pack_half2(a[4], a[5]), pack_half2(a[6], a[7]));
-        }
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory");
-      if (leader) {
-        tma_store_5d(&map_out, slab, 0, tw * kTileW, th * kTileH, n, 0);
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-      }
-    }
-    if (leader) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 128);
+  // -------------------------------------------------------------------- consumers (warpgroups 1, 2)
+  const int ct = threadIdx.x - 128;
+  const int cw = ct >> 7;  // output rows [8 cw, 8 cw + 8) of the tile
+  const int lane = threadIdx.x & 31;
+  const int r0 = 16 * ((ct >> 5) & 3) + (lane >> 2);  // this thread's pixels (warpgroup-local rows): r0, r0 + 8
+  const int cq = 2 * (lane & 3);
+  const bool leader = ((ct & 127) == 0);
+  const uint32_t w_addr = smem_u32(wsm);
+  float2 bias[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) bias[j] = __ldg(reinterpret_cast<const float2*>(p.bias + 8 * j + cq));
+  float acc[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+  mbar_wait(w_full, 0);
+  pdl_wait();  // the output buffer may still be read by an earlier kernel
+  int stage = 0, phase = 0, use = 0;
+  for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x, ++use) {
+    const int n = t / tiles_per_img, rem = t - n * tiles_per_img;
+    const int th = rem / p.tiles_w, tw = rem - th * p.tiles_w;
+    mbar_wait(&full[stage], phase);
+    // A: rows j at 16 B from pair j + s of padded row 2i + r; row groups i two padded rows apart; this warpgroup's
+    // first output row is 8 cw
+    const uint32_t patch = smem_u32(ring + stage * kPatchSlot) + (uint32_t)(cw * 8 * 2 * kRowStride);
+    wgmma_fence();
+#pragma unroll
+    for (int r = 0; r < 7; ++r) {
+#pragma unroll
+      for (int s = 0; s < 4; ++s) {
+        const uint64_t da = gmma_desc_linear(patch + r * kRowStride + s * 16, kParStride, 2 * kRowStride);
+        // B: [E/O][64 ch][8]: rows (channels) at 16 B, groups of 8 channels 128 B apart, K chunks 1 KB apart
+        const uint64_t db = gmma_desc_linear(w_addr + (r * 4 + s) * kWTileBytes, 1024, 128);
+        Wgmma<64>::ss(acc, da, db, (r | s) ? 1u : 0u);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(acc);
+    mbar_arrive(&empty[stage]);
+    if (++stage == S) {
+      stage = 0;
+      phase ^= 1;
+    }
+
+    // epilogue: two staging slabs per warpgroup, so one tile's TMA store overlaps the next tile
+    uint8_t* slab = staging + (cw * 2 + (use & 1)) * kHalfSlab;
+    // the TMA store that last used this slab (two tiles ago) must have finished reading it
+    if (leader) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = r0 + 8 * h;
+        float a0 = acc[4 * j + 2 * h] + bias[j].x, a1 = acc[4 * j + 2 * h + 1] + bias[j].y;
+        if (p.relu) {
+          a0 = fmaxf(a0, 0.f);
+          a1 = fmaxf(a1, 0.f);
+        }
+        *reinterpret_cast<uint32_t*>(slab + row * 128 + (((uint32_t)j ^ (uint32_t)(row & 7)) << 4) + cq * 2) =
+            pack_half2(a0, a1);
+      }
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+    if (leader) {
+      tma_store_5d(&map_out, slab, 0, tw * kTileW, th * kTileH + 8 * cw, n, 0);
+      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    }
   }
+  if (leader) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
 }  // namespace
@@ -262,7 +216,7 @@ int stem_conv_launch(const GemmLayer& L, cudaStream_t stream) {
     uint64_t d[5] = {(uint64_t)L.out_ld, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)L.n_img, 1};
     uint64_t s[4] = {(uint64_t)L.out_ld * E, (uint64_t)L.out_ld * E * Wo, (uint64_t)L.out_ld * E * Wo * Ho,
                      (uint64_t)L.out_ld * E * Wo * Ho * L.n_img};
-    uint32_t b[5] = {64, (uint32_t)kTileW, (uint32_t)kTileH, 1, 1};
+    uint32_t b[5] = {64, (uint32_t)kTileW, (uint32_t)kTileH / 2, 1, 1};  // one warpgroup's 8 x 8 pixels
     int rc = encode_map_f16(&mo, L.out, 5, d, s, b);
     if (rc) return rc;
   }

@@ -140,7 +140,7 @@ class Engine:
 
     def __init__(self):
         if not torch.cuda.is_available():
-            raise _lib.FposeError("foundationpose_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise _lib.FposeError("foundationpose_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         h = C.c_void_p()
         _lib.check(lib.fp_create(C.byref(h)), "fp_create")
         self._h = h

@@ -50,7 +50,7 @@ lib.fp_op_attention.restype = C.c_int
 
 
 def attention(qkv, impl=1):
-    """qkv fp16 [B*400, 1536] -> fp16 [B*400, 512]; impl 1 = tcgen05, 0 = mma.sync."""
+    """qkv fp16 [B*400, 1536] -> fp16 [B*400, 512]; `impl` is ignored: one implementation, the wgmma kernel."""
     _require_cuda(qkv)
     assert qkv.dtype == torch.float16 and qkv.shape[1] == 1536 and qkv.shape[0] % 400 == 0
     B = qkv.shape[0] // 400

@@ -1,5 +1,5 @@
 """Host-side weight preparation: fold eval-mode BatchNorm into the convolutions and repack the
-reference `state_dict` tensors into the K-major fp16 layouts the tcgen05 kernels consume.
+reference `state_dict` tensors into the K-major fp16 layouts the wgmma kernels consume.
 
 Reference layouts: learning/models/network_modules.py:37-50 (ConvBNReLU: net.0 = Conv2d, net.1 = BN),
 :73-111 (ResnetBasicBlock: conv1/bn1/conv2/bn2).  BatchNorm2d in eval mode is the per-channel affine
@@ -28,7 +28,7 @@ def pack_conv3(w):
 
 def pack_conv7(w):
     """(Co,Ci<=8,7,7) fp32 -> (7, 4, 2, Co, 8) fp16 = [filter row r][tap pair s][tap 2s + e][Co][8 ch]: one
-    un-swizzled K-major tcgen05 B tile (N = Co, K = 16) per (r, s); tap 7 and channels >= Ci are zero
+    un-swizzled K-major wgmma B tile (N = Co, K = 16) per (r, s); tap 7 and channels >= Ci are zero
     (csrc/fp_stem.cu)."""
     co, ci = w.shape[:2]
     out = torch.zeros(7, 8, co, 8, dtype=torch.float32)  # (r, tap padded to 8, co, c padded to 8)

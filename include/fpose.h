@@ -1,4 +1,4 @@
-/* fpose.h — C ABI of libfpose.so, the B200-native (sm_100a) render-and-compare hot path behind
+/* fpose.h — C ABI of libfpose.so, the H100-native (sm_90a) render-and-compare hot path behind
  * NVlabs/FoundationPose's Python surfaces.
  *
  * Every entry point is `extern "C"`, takes plain pointers and sizes, returns 0 on success or a
@@ -30,7 +30,7 @@ const char* fp_last_error(void);
 unsigned long long fp_launch_count(void);
 
 /* Per-launch device timing of the two roofline kernels (CUDA events on the launching stream):
- * kind 0 = tcgen05 implicit-GEMM kernel (work = algorithmic FLOPs), kind 1 = crop producer
+ * kind 0 = wgmma implicit-GEMM kernel (work = algorithmic FLOPs), kind 1 = crop producer
  * (work = algorithmic output bytes).  fp_prof_collect synchronises the device, returns and clears
  * the sums accumulated since fp_prof_enable(1). */
 int fp_prof_enable(int on);
@@ -40,7 +40,7 @@ int fp_prof_collect(int kind, double* total_ms, double* total_work, int* launche
 /* single operators (parity-test hooks; the product path below calls the same code)           */
 /* ------------------------------------------------------------------------------------------ */
 
-/* kinds of dense layer the tcgen05 implicit-GEMM kernel executes */
+/* kinds of dense layer the wgmma implicit-GEMM kernel executes */
 #define FP_LAYER_LINEAR 0   /* torch.nn.Linear / in_proj / out_proj (refine_network.py:56-70)      */
 #define FP_LAYER_CONV3_S1 1 /* 3x3 s1 p1 conv of ResnetBasicBlock (network_modules.py:73-111)       */
 #define FP_LAYER_CONV3_S2 2 /* 3x3 s2 p1 ConvBNReLU (refine_network.py:37, :45)                      */
@@ -73,7 +73,7 @@ int fp_op_gemm_layer(const fp_gemm_layer_t* layer, void* stream);
 
 /* softmax(Q K^T / sqrt(128)) V of nn.MultiheadAttention (refine_network.py:56-70, score_network.py:53):
  * qkv fp16 [B*400][1536] (q | k | v, 4 heads of 128 each), out fp16 [B*400][512].
- * `impl` is ignored (kept for ABI stability): there is one implementation, the tcgen05 kernel. */
+ * `impl` is ignored (kept for ABI stability): there is one implementation, the wgmma kernel. */
 int fp_op_attention(const void* qkv, void* out, int B, int impl, void* stream);
 
 
@@ -82,7 +82,7 @@ int fp_op_attention(const void* qkv, void* out, int B, int impl, void* stream);
 /* ------------------------------------------------------------------------------------------ */
 typedef struct fp_ctx fp_ctx;
 
-/* Creates a context on the current CUDA device (must be sm_100).  Replaces the implicit global
+/* Creates a context on the current CUDA device (must be sm_90).  Replaces the implicit global
  * state of the reference predictors (`.cuda()` modules, nvdiffrast `RasterizeCudaContext`,
  * estimater.py:29-41, :166-171). */
 int fp_create(fp_ctx** ctx);

@@ -1,6 +1,6 @@
 """CPU: the drop-in module tree (foundationpose_b200/dropin) resolves every name the reference's UNMODIFIED
 run_demo.py uses, the trimesh / imageio stand-ins round-trip the demo-scene files, and the reader parses them."""
-import ast
+import json
 import os
 import subprocess
 import sys
@@ -9,7 +9,8 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DROPIN = os.path.join(ROOT, "foundationpose_b200", "dropin")
-REF_DEMO = "/root/reference/run_demo.py"
+# every name / first-level attribute the reference's driver scripts read (tools/make_golden_drivers.py)
+DRIVERS = json.load(open(os.path.join(ROOT, "tests", "golden", "driver_names.json")))
 
 
 def _env():
@@ -18,30 +19,24 @@ def _env():
     return env
 
 
-@pytest.mark.skipif(not os.path.exists(REF_DEMO), reason="reference tree not present (GPU box)")
-def test_every_name_run_demo_uses_resolves():
-    """Static check against the reference's own driver: all unqualified names and first-level attributes
-    (`trimesh.load`, `dr.RasterizeCudaContext`, `np.stack`, ...) exist after its two star-imports."""
-    import builtins
-
-    tree = ast.parse(open(REF_DEMO).read())
-    assigned, used, attrs = set(), set(), set()
-    for node in ast.walk(tree):
-        if isinstance(node, ast.Name):
-            (assigned if isinstance(node.ctx, ast.Store) else used).add(node.id)
-        elif isinstance(node, ast.Attribute) and isinstance(node.value, ast.Name):
-            attrs.add((node.value.id, node.attr))
-    need = sorted(n for n in used - assigned - set(dir(builtins)) if n != "__file__")
-    assert {"trimesh", "dr", "np", "cv2", "imageio", "logging", "set_seed", "YcbineoatReader", "FoundationPose"} <= set(need)
-    mod_attrs = sorted((m, a) for (m, a) in attrs if m in need and m not in ("args", "parser", "o3d"))
-    code = ("from estimater import *\nfrom datareader import *\nimport argparse\n"
+def _missing(imports, need, mod_attrs, extra=""):
+    code = ("\n".join(imports) + "\n"
             f"missing = [n for n in {need!r} if n not in globals()]\n"
             f"missing += [f'{{m}}.{{a}}' for (m, a) in {mod_attrs!r} if m in globals() and not hasattr(globals()[m], a)]\n"
-            "missing += [] if hasattr(trimesh.bounds, 'oriented_bounds') else ['trimesh.bounds.oriented_bounds']\n"
-            "print('MISSING', missing)\n")
+            + extra + "print('MISSING', missing)\n")
     out = subprocess.run([sys.executable, "-c", code], env=_env(), capture_output=True, text=True, timeout=300)
     assert out.returncode == 0, out.stderr[-2000:]
     assert "MISSING []" in out.stdout, out.stdout[-2000:]
+
+
+def test_every_name_run_demo_uses_resolves():
+    """Static check against the reference's own driver: all unqualified names and first-level attributes
+    (`trimesh.load`, `dr.RasterizeCudaContext`, `np.stack`, ...) exist after its two star-imports."""
+    d = DRIVERS["run_demo.py"]
+    assert {"trimesh", "dr", "np", "cv2", "imageio", "logging", "set_seed", "YcbineoatReader", "FoundationPose"} <= set(d["names"])
+    _missing(["from estimater import *", "from datareader import *", "import argparse"], d["names"],
+             [tuple(x) for x in d["attributes"]],
+             "missing += [] if hasattr(trimesh.bounds, 'oriented_bounds') else ['trimesh.bounds.oriented_bounds']\n")
 
 
 def test_demo_scene_round_trip(tmp_path):
@@ -84,31 +79,9 @@ print('OK')
 def test_every_name_the_dataset_drivers_use_resolves(script):
     """Same static check for the reference's dataset drivers (SURVEY.md §8f N3): replay the script's own import
     statements on top of the drop-in tree, then every unqualified name / first-level attribute must exist."""
-    import builtins
-
-    path = "/root/reference/" + script
-    if not os.path.exists(path):
-        pytest.skip("reference tree not present (GPU box)")
-    tree = ast.parse(open(path).read())
-    imports = [ast.unparse(n) for n in tree.body if isinstance(n, (ast.Import, ast.ImportFrom))]
-    assigned, used, attrs = set(), set(), set()
-    for node in ast.walk(tree):
-        if isinstance(node, ast.Name):
-            (assigned if isinstance(node.ctx, ast.Store) else used).add(node.id)
-        elif isinstance(node, ast.Attribute) and isinstance(node.value, ast.Name):
-            attrs.add((node.value.id, node.attr))
-        elif isinstance(node, (ast.FunctionDef, ast.arg)):
-            assigned.add(node.name if isinstance(node, ast.FunctionDef) else node.arg)
-    need = sorted(n for n in used - assigned - set(dir(builtins)) if n != "__file__")
-    assert {"wp", "NestDict", "make_yaml_dumpable", "dr", "trimesh", "FoundationPose", "set_seed", "argparse"} <= set(need)
-    mod_attrs = sorted((m, a) for (m, a) in attrs if m in need and m not in ("opt", "parser", "o3d", "reader", "reader_tmp", "est"))
-    code = ("\n".join(imports) + "\n"
-            f"missing = [n for n in {need!r} if n not in globals()]\n"
-            f"missing += [f'{{m}}.{{a}}' for (m, a) in {mod_attrs!r} if m in globals() and not hasattr(globals()[m], a)]\n"
-            "print('MISSING', missing)\n")
-    out = subprocess.run([sys.executable, "-c", code], env=_env(), capture_output=True, text=True, timeout=300)
-    assert out.returncode == 0, out.stderr[-2000:]
-    assert "MISSING []" in out.stdout, out.stdout[-2000:]
+    d = DRIVERS[script]
+    assert {"wp", "NestDict", "make_yaml_dumpable", "dr", "trimesh", "FoundationPose", "set_seed", "argparse"} <= set(d["names"])
+    _missing(d["imports"], d["names"], [tuple(x) for x in d["attributes"]])
 
 
 def test_bop_readers_parse_the_synthetic_datasets(tmp_path):

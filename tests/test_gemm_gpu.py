@@ -1,4 +1,4 @@
-"""Parity of the tcgen05 implicit-GEMM kernel (csrc/fp_gemm.cu) against torch fp32 convolutions /
+"""Parity of the wgmma implicit-GEMM kernel (csrc/fp_gemm.cu) against torch fp32 convolutions /
 matmuls evaluated on the same fp16-rounded operands.  Tolerance: fp16 output rounding (rel 2e-3,
 abs 2e-3 on O(1) activations); accumulation is fp32 on both sides.
 """

@@ -1,4 +1,4 @@
-"""GPU parity of the whole network paths (15 tcgen05 conv layers + attention heads) against the fp32
+"""GPU parity of the whole network paths (15 wgmma conv layers + attention heads) against the fp32
 CPU oracle (oracle/nets.py, pinned to the reference classes by tests/test_oracle_golden.py) on
 identical pre-built crops and identical seeded weights.
 
@@ -68,21 +68,26 @@ def test_refine_net_outputs(engine):
 
 
 def test_token_reduction_is_bitwise_the_same_as_cluster_or_single_cta(engine):
-    """fp_attn.cu token_reduce_kernel: a cluster of four CTAs per hypothesis up to 74 hypotheses, one CTA walking the
-    same four token ranges above.  Same partial sums, same order: the read-outs of the first 72 hypotheses must not
-    change by a bit when 8 more are appended (refiner heads and scorer features)."""
+    """fp_attn.cu token_reduce_kernel: a cluster of eight CTAs per hypothesis while B * 8 <= 4 * SMs
+    (token_split_for), one CTA walking the same eight token ranges above.  Same partial sums, same order: the read-outs
+    of the largest batch that takes the cluster launch must not change by a bit when 8 more hypotheses push the batch
+    onto the single-CTA launch (refiner heads and scorer features)."""
     from foundationpose_b200.engine import crops_from_planar
 
     e, _, _ = engine
-    A, B = _crops(80, 21)
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    n_cluster = (4 * sms) // 8  # largest B with B * 8 <= 4 * SMs
+    n_single = n_cluster + 8
+    assert n_cluster * 8 <= 4 * sms < n_single * 8
+    A, B = _crops(n_single, 21)
     big = crops_from_planar(A.cuda(), B.cuda())
-    small = crops_from_planar(A[:72].cuda(), B[:72].cuda())
-    t80, r80 = e.op_refine_net(big, 80)
-    t72, r72 = e.op_refine_net(small, 72)
-    assert torch.equal(t80[:72], t72) and torch.equal(r80[:72], r72)
-    f80 = e.op_score_feats(big, 80)
-    f72 = e.op_score_feats(small, 72)
-    assert torch.equal(f80[:72], f72)
+    small = crops_from_planar(A[:n_cluster].cuda(), B[:n_cluster].cuda())
+    t_big, r_big = e.op_refine_net(big, n_single)
+    t_small, r_small = e.op_refine_net(small, n_cluster)
+    assert torch.equal(t_big[:n_cluster], t_small) and torch.equal(r_big[:n_cluster], r_small)
+    f_big = e.op_score_feats(big, n_single)
+    f_small = e.op_score_feats(small, n_cluster)
+    assert torch.equal(f_big[:n_cluster], f_small)
 
 
 def test_refine_net_golden(engine):

@@ -1,4 +1,4 @@
-"""On-GPU probe of the attention kernels (mma.sync vs tcgen05): error vs torch fp32 + timing at B=252."""
+"""On-GPU probe of the attention kernel: error vs torch fp32 + timing at B=252."""
 import os, sys
 import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
