@@ -28,9 +28,9 @@ struct DevBuf {
 };
 
 // (Re)allocates `b` to at least `bytes`.  `epoch` is the owning context's graph epoch: it is bumped whenever a device
-// pointer or by-value kernel parameter that a captured CUDA graph may hold changes (re-allocation, new mesh /
-// weights / intrinsics), and cached graphs older than it are rebuilt.  Never called while a stream is capturing:
-// every workspace is sized by ensure_capacity / fp_set_mesh / fp_set_frame BEFORE run_graphed.
+// pointer or by-value kernel parameter that a captured CUDA graph may hold changes (re-allocation, new weights /
+// intrinsics), and cached graphs older than it are rebuilt.  Never called while a stream is capturing:
+// every workspace is sized by ensure_capacity / fp_set_mesh_slot / fp_set_frame BEFORE run_graphed.
 static int dev_alloc(unsigned long long& epoch, DevBuf& b, size_t bytes, bool zero = false) {
   if (b.bytes >= bytes && b.p) return 0;
   ++epoch;
@@ -78,18 +78,29 @@ constexpr size_t kCropImg = (size_t)(S + 6) * (S + 8) * 8;  // fp16 elements per
 // boundary: B starts at N rounded up to 4 (up to three never-read pad images).
 static inline int b_img0_of(int N) { return (N + 3) & ~3; }
 
+static_assert(kMaxMeshes == FP_MAX_MESHES, "fp_crop.cuh and fpose.h disagree on the number of mesh slots");
+
+// One mesh of the context (fp_meshlet.cu layout).  Slot 0 is the mesh of every single-object entry point.
+struct MeshSlot {
+  DevBuf vpos, vnrm, vatt, faces, meshlets, ml_verts, ml_tris, tex;
+  int V = 0, F = 0, Ht = 0, Wt = 0, n_meshlets = 0, front_sign = 0, closed = 0;
+  float bs[4] = {0.f, 0.f, 0.f, 0.f};
+  bool has_tex = false, loaded = false;
+  float diameter = 0.f;
+};
+
 }  // namespace fp
 
 struct fp_ctx {
   int device = 0;
   fp::Net net[2];  // 0 = refiner, 1 = scorer
   unsigned long long epoch = 1;  // graph epoch (see dev_alloc)
-  // mesh (fp_meshlet.cu layout)
-  fp::DevBuf vpos, vnrm, vatt, faces, meshlets, ml_verts, ml_tris, tex;
-  int V = 0, F = 0, Ht = 0, Wt = 0, n_meshlets = 0, front_sign = 0, mesh_closed = 0;
-  float mesh_bs[4] = {0.f, 0.f, 0.f, 0.f};
-  bool has_tex = false, has_mesh = false;
-  float diameter = 0.f, rot_normalizer = 0.3490658503988659f;
+  unsigned long long graph_captures = 0;
+  // meshes, and their device table (MeshSlotDev [FP_MAX_MESHES]) that kernels index by slot.  Captured graphs hold only
+  // the table's address: loading a slot rewrites its entry in place and needs no new capture.
+  fp::MeshSlot mesh[fp::kMaxMeshes];
+  fp::DevBuf mesh_table, mesh_of;  // mesh_of: slot id of every object of fp_track_objects
+  float rot_normalizer = 0.3490658503988659f;
   float crop_ratio[2] = {1.2f, 1.2f};  // per predictor: each reads its own config.yml (predict_pose_refine.py:117, predict_score.py:137)
   // frame
   fp::DevBuf rgb_raw, rgba, depth_raw, depth_a, depth_b, xyz;
@@ -130,6 +141,8 @@ struct fp_ctx {
   float* stage_pose = nullptr;
   size_t stage_npix = 0;
   fp::DevBuf track_pose;
+  float* stage_poses = nullptr;  // fp_track_objects: pinned [stage_poses_n][16] pose read-back
+  int stage_poses_n = 0;
 };
 
 namespace fp {
@@ -356,9 +369,53 @@ static int crops_export(fp_ctx* c, void* ext, int N, cudaStream_t st) {
   return 0;
 }
 
+// Entry `s` of the device mesh table, with the expressions the crop producer and the pose update always used.
+static MeshSlotDev mesh_entry(const fp_ctx* c, int s) {
+  const MeshSlot& m = c->mesh[s];
+  MeshSlotDev e;
+  memset(&e, 0, sizeof e);
+  e.mesh.vpos = reinterpret_cast<const float4*>(m.vpos.p);
+  e.mesh.vnrm = reinterpret_cast<const float4*>(m.vnrm.p);
+  e.mesh.vatt = reinterpret_cast<const float4*>(m.vatt.p);
+  e.mesh.faces = reinterpret_cast<const int4*>(m.faces.p);
+  e.mesh.meshlets = reinterpret_cast<const Meshlet*>(m.meshlets.p);
+  e.mesh.ml_verts = reinterpret_cast<const int*>(m.ml_verts.p);
+  e.mesh.ml_tris = reinterpret_cast<const uint2*>(m.ml_tris.p);
+  e.mesh.n_meshlets = m.n_meshlets;
+  e.mesh.V = m.V;
+  e.mesh.F = m.F;
+  e.mesh.front_sign = c->cull_backfaces ? m.front_sign : 0;
+  e.mesh.bs_x = m.bs[0];
+  e.mesh.bs_y = m.bs[1];
+  e.mesh.bs_z = m.bs[2];
+  e.mesh.bs_r = m.bs[3];
+  e.has_tex = m.has_tex ? 1 : 0;
+  e.tex = m.has_tex ? reinterpret_cast<const uchar4*>(m.tex.p) : nullptr;
+  e.Ht = m.Ht;
+  e.Wt = m.Wt;
+  for (int mode = 0; mode < 2; ++mode) e.r3[mode] = (float)((double)m.diameter * (double)c->crop_ratio[mode] / 2.0);
+  e.inv_radius = 1.0f / (m.diameter / 2.0f);
+  e.half_diameter = m.diameter / 2.0f;
+  return e;
+}
+
+// Rewrites the table entries of every loaded slot.  Synchronises: kernels enqueued earlier may be reading the table.
+static int write_mesh_table(fp_ctx* c) {
+  FP_CUDA_OK(cudaDeviceSynchronize());
+  FP_TRY(dev_alloc(c->epoch, c->mesh_table, sizeof(MeshSlotDev) * kMaxMeshes, /*zero=*/true));
+  std::vector<MeshSlotDev> table(kMaxMeshes);
+  memset(table.data(), 0, sizeof(MeshSlotDev) * kMaxMeshes);
+  for (int s = 0; s < kMaxMeshes; ++s)
+    if (c->mesh[s].loaded) table[s] = mesh_entry(c, s);
+  FP_CUDA_OK(cudaMemcpy(c->mesh_table.p, table.data(), sizeof(MeshSlotDev) * kMaxMeshes, cudaMemcpyHostToDevice));
+  FP_CUDA_OK(cudaDeviceSynchronize());
+  return 0;
+}
+
+// mesh_of: [N] device slot ids (validated by the caller), or null = every hypothesis renders slot 0
 static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg, float* win, int* stats,
-                      cudaStream_t st) {
-  FP_REQUIRE(c->has_mesh, "no mesh: call fp_set_mesh first");
+                      cudaStream_t st, const int* mesh_of = nullptr) {
+  FP_REQUIRE(mesh_of || c->mesh[0].loaded, "no mesh: call fp_set_mesh first");
   FP_REQUIRE(c->has_frame, "no frame: call fp_set_frame first");
   // only launches below: this body is also what run_graphed captures (no allocation, no synchronisation)
   CropParams p;
@@ -370,29 +427,10 @@ static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg
   p.cy = c->K[5];
   p.H = c->H;
   p.W = c->W;
-  p.r3 = (float)((double)c->diameter * (double)c->crop_ratio[mode ? 1 : 0] / 2.0);
-  p.inv_radius = 1.0f / (c->diameter / 2.0f);
   p.znear = 0.001f;  // Utils.py:161
   p.zfar = 100.f;
-  p.mesh.vpos = reinterpret_cast<const float4*>(c->vpos.p);
-  p.mesh.vnrm = reinterpret_cast<const float4*>(c->vnrm.p);
-  p.mesh.vatt = reinterpret_cast<const float4*>(c->vatt.p);
-  p.mesh.faces = reinterpret_cast<const int4*>(c->faces.p);
-  p.mesh.meshlets = reinterpret_cast<const Meshlet*>(c->meshlets.p);
-  p.mesh.ml_verts = reinterpret_cast<const int*>(c->ml_verts.p);
-  p.mesh.ml_tris = reinterpret_cast<const uint2*>(c->ml_tris.p);
-  p.mesh.n_meshlets = c->n_meshlets;
-  p.mesh.V = c->V;
-  p.mesh.F = c->F;
-  p.mesh.front_sign = c->cull_backfaces ? c->front_sign : 0;
-  p.mesh.bs_x = c->mesh_bs[0];
-  p.mesh.bs_y = c->mesh_bs[1];
-  p.mesh.bs_z = c->mesh_bs[2];
-  p.mesh.bs_r = c->mesh_bs[3];
-  p.has_tex = c->has_tex ? 1 : 0;
-  p.tex = c->has_tex ? reinterpret_cast<const uchar4*>(c->tex.p) : nullptr;
-  p.Ht = c->Ht;
-  p.Wt = c->Wt;
+  p.slots = reinterpret_cast<const MeshSlotDev*>(c->mesh_table.p);
+  p.mesh_of = mesh_of;
   p.rgb = reinterpret_cast<const uchar4*>(c->rgba.p);
   p.xyz_map = reinterpret_cast<const float4*>(c->xyz.p);
   p.depth = c->depth_cur;
@@ -460,6 +498,7 @@ static int run_graphed(fp_ctx* c, int kind, int N, int iters, cudaStream_t st, B
     FP_CUDA_OK(ie);
     g.epoch = c->epoch;
     c->graph_nodes[key] = (int)n_kernels;
+    ++c->graph_captures;
   }
   FP_CUDA_OK(cudaGraphLaunch(g.exec, st));
   note_launches(c->graph_nodes[key]);
@@ -529,22 +568,50 @@ static int prepare_frame(fp_ctx* c, const float* K, int H, int W, bool need_raw)
   return 0;
 }
 
-static int refine_body(fp_ctx* c, int N, int iterations, cudaStream_t s2) {
+// mesh_of: [N] device slot ids, or null = slot 0 for every hypothesis
+static int refine_body(fp_ctx* c, int N, int iterations, cudaStream_t s2, const int* mesh_of = nullptr) {
   float* cur = reinterpret_cast<float*>(c->poses_a.p);
   float* nxt = reinterpret_cast<float*>(c->poses_b.p);
   const float* ho = reinterpret_cast<const float*>(c->head_out.p);
+  const MeshSlotDev* table = reinterpret_cast<const MeshSlotDev*>(c->mesh_table.p);
   for (int it = 0; it < iterations; ++it) {
-    FP_TRY(make_crops(c, cur, N, 0, nullptr, nullptr, nullptr, s2));
+    FP_TRY(make_crops(c, cur, N, 0, nullptr, nullptr, nullptr, s2, mesh_of));
     FP_TRY(run_encoder(c, c->net[0], reinterpret_cast<const __half*>(c->crops.p), N, s2));
     FP_TRY(run_refine_heads(c, c->net[0], N, s2));
     const bool last = it == iterations - 1;
     FP_TRY(pose_update_launch(cur, ho, ho + (size_t)N * 3, nxt, last ? reinterpret_cast<float*>(c->lt_buf.p) : nullptr,
-                              last ? reinterpret_cast<float*>(c->lr_buf.p) : nullptr, N, c->diameter / 2.0f,
+                              last ? reinterpret_cast<float*>(c->lr_buf.p) : nullptr, N, table, mesh_of, 0.f,
                               c->rot_normalizer, s2));
     float* t = cur;
     cur = nxt;
     nxt = t;
   }
+  return 0;
+}
+
+// pinned host staging of the frame of fp_track / fp_track_objects
+static int alloc_frame_staging(fp_ctx* c, size_t npix) {
+  if (c->stage_npix >= npix) return 0;
+  if (c->stage_rgb) cudaFreeHost(c->stage_rgb);
+  if (c->stage_depth) cudaFreeHost(c->stage_depth);
+  c->stage_rgb = c->stage_depth = nullptr;
+  c->stage_npix = 0;
+  FP_CUDA_OK(cudaMallocHost(&c->stage_rgb, npix * 3));
+  FP_CUDA_OK(cudaMallocHost(&c->stage_depth, npix * 4));
+  c->stage_npix = npix;
+  ++c->epoch;  // the graph's copy nodes hold these addresses
+  return 0;
+}
+
+// The previous frame's graph has finished (both callers synchronise), so the staging buffers are free.  The two
+// uploads are issued as soon as their staging copy is done — the depth DMA runs under the host's rgb copy, the
+// rgb DMA under the graph launch — instead of being nodes of the graph (measured: -40 us per frame)
+static int upload_staged_frame(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, size_t npix,
+                               cudaStream_t st) {
+  memcpy(c->stage_depth, depth_host, npix * 4);
+  FP_CUDA_OK(cudaMemcpyAsync(c->depth_raw.p, c->stage_depth, npix * 4, cudaMemcpyHostToDevice, st));
+  memcpy(c->stage_rgb, rgb_host, npix * 3);
+  FP_CUDA_OK(cudaMemcpyAsync(c->rgb_raw.p, c->stage_rgb, npix * 3, cudaMemcpyHostToDevice, st));
   return 0;
 }
 
@@ -598,8 +665,10 @@ int fp_destroy(fp_ctx* c) {
   cudaDeviceSynchronize();
   for (auto& net : c->net)
     for (auto& kv : net.t) cudaFree(kv.second.p);
-  DevBuf* bufs[] = {&c->vpos, &c->vnrm, &c->vatt, &c->faces, &c->meshlets, &c->ml_verts, &c->ml_tris, &c->tex, &c->rgb_raw,
-                    &c->rgba, &c->depth_raw, &c->depth_a, &c->depth_b, &c->xyz, &c->crops, &c->act0, &c->a1, &c->a2,
+  for (MeshSlot& m : c->mesh)
+    for (DevBuf* b : {&m.vpos, &m.vnrm, &m.vatt, &m.faces, &m.meshlets, &m.ml_verts, &m.ml_tris, &m.tex})
+      if (b->p) cudaFree(b->p);
+  DevBuf* bufs[] = {&c->mesh_table, &c->mesh_of, &c->rgb_raw, &c->rgba, &c->depth_raw, &c->depth_a, &c->depth_b, &c->xyz, &c->crops, &c->act0, &c->a1, &c->a2,
                     &c->a3, &c->ab0, &c->ab1, &c->ab2, &c->c0, &c->c1, &c->c2, &c->tok, &c->qkv, &c->att, &c->x1pre,
                     &c->x1, &c->ff, &c->x2pre, &c->head_out, &c->poses_a, &c->poses_b, &c->feats, &c->tail_qkv,
                     &c->tail_attn, &c->tail_proj, &c->scores, &c->best, &c->lt_buf, &c->lr_buf, &c->feat_buf,
@@ -615,6 +684,7 @@ int fp_destroy(fp_ctx* c) {
   if (c->stage_rgb) cudaFreeHost(c->stage_rgb);
   if (c->stage_depth) cudaFreeHost(c->stage_depth);
   if (c->stage_pose) cudaFreeHost(c->stage_pose);
+  if (c->stage_poses) cudaFreeHost(c->stage_poses);
   delete c;
   return 0;
   FP_API_END
@@ -625,9 +695,11 @@ int fp_set_config(fp_ctx* c, int which, float crop_ratio, float rot_normalizer) 
   FP_REQUIRE(c, "null ctx");
   FP_REQUIRE(which == 0 || which == 1, "fp_set_config: which must be 0 (refiner) or 1 (scorer)");
   FP_REQUIRE(crop_ratio > 0.f, "fp_set_config: crop_ratio must be positive");
+  DeviceGuard dg(c->device);
   c->crop_ratio[which] = crop_ratio;
   if (which == 0) c->rot_normalizer = rot_normalizer;
   ++c->epoch;
+  if (c->mesh_table.p) FP_TRY(write_mesh_table(c));  // the table holds r3 = diameter * crop_ratio / 2
   return 0;
   FP_API_END
 }
@@ -724,28 +796,30 @@ int fp_load_network(fp_ctx* c, int which, const fp_tensor_t* tensors, int n) {
   FP_API_END
 }
 
-int fp_set_mesh(fp_ctx* c, int V, int F, const float* pos, const float* nrm, const float* uv, const float* vcol,
-                const int* faces, const unsigned char* tex_rgb, int Ht, int Wt, float diameter) {
+int fp_set_mesh_slot(fp_ctx* c, int slot, int V, int F, const float* pos, const float* nrm, const float* uv,
+                     const float* vcol, const int* faces, const unsigned char* tex_rgb, int Ht, int Wt, float diameter) {
   FP_API_BEGIN
   FP_REQUIRE(c && pos && nrm && faces, "fp_set_mesh: null argument");
+  FP_REQUIRE(slot >= 0 && slot < kMaxMeshes, "fp_set_mesh_slot: slot %d out of range [0, %d)", slot, kMaxMeshes);
   FP_REQUIRE(V > 0 && F > 0 && diameter > 0.f, "fp_set_mesh: empty mesh");
   FP_REQUIRE((uv && tex_rgb && Ht > 0 && Wt > 0) || vcol, "fp_set_mesh: need (uv + texture) or vertex colours");
   for (int i = 0; i < 3 * F; ++i) FP_REQUIRE(faces[i] >= 0 && faces[i] < V, "fp_set_mesh: face index out of range");
   DeviceGuard dg(c->device);
-  // graphs captured for the previous mesh may still be running on the caller's stream
+  // graphs rendering the previous mesh of this slot may still be running on the caller's stream
   FP_CUDA_OK(cudaDeviceSynchronize());
-  c->has_mesh = false;
+  MeshSlot& m = c->mesh[slot];
+  m.loaded = false;
   const bool has_tex = (uv && tex_rgb);
   MeshHost mh;
   FP_TRY(build_mesh_host(V, F, pos, nrm, has_tex ? uv : vcol, has_tex ? 2 : 3, faces, mh));
-  FP_TRY(upload(c->epoch, c->vpos, mh.vpos));
-  FP_TRY(upload(c->epoch, c->vnrm, mh.vnrm));
-  FP_TRY(upload(c->epoch, c->vatt, mh.vatt));
-  FP_TRY(upload(c->epoch, c->faces, mh.faces));
-  FP_TRY(upload(c->epoch, c->meshlets, mh.meshlets));
-  FP_TRY(upload(c->epoch, c->ml_verts, mh.ml_verts));
-  FP_TRY(upload(c->epoch, c->ml_tris, mh.ml_tris));
-  c->has_tex = has_tex;
+  FP_TRY(upload(c->epoch, m.vpos, mh.vpos));
+  FP_TRY(upload(c->epoch, m.vnrm, mh.vnrm));
+  FP_TRY(upload(c->epoch, m.vatt, mh.vatt));
+  FP_TRY(upload(c->epoch, m.faces, mh.faces));
+  FP_TRY(upload(c->epoch, m.meshlets, mh.meshlets));
+  FP_TRY(upload(c->epoch, m.ml_verts, mh.ml_verts));
+  FP_TRY(upload(c->epoch, m.ml_tris, mh.ml_tris));
+  m.has_tex = has_tex;
   if (has_tex) {
     std::vector<unsigned char> rgba((size_t)Ht * Wt * 4);
     for (size_t i = 0; i < (size_t)Ht * Wt; ++i) {
@@ -754,21 +828,26 @@ int fp_set_mesh(fp_ctx* c, int V, int F, const float* pos, const float* nrm, con
       rgba[4 * i + 2] = tex_rgb[3 * i + 2];
       rgba[4 * i + 3] = 255;
     }
-    FP_TRY(upload(c->epoch, c->tex, rgba));
-    c->Ht = Ht;
-    c->Wt = Wt;
+    FP_TRY(upload(c->epoch, m.tex, rgba));
+    m.Ht = Ht;
+    m.Wt = Wt;
   }
-  c->V = V;
-  c->F = F;
-  c->n_meshlets = (int)mh.meshlets.size();
-  c->front_sign = mh.front_sign;
-  c->mesh_closed = mh.closed;
-  for (int i = 0; i < 4; ++i) c->mesh_bs[i] = mh.bs[i];
-  c->diameter = diameter;
-  c->has_mesh = true;
-  ++c->epoch;
+  m.V = V;
+  m.F = F;
+  m.n_meshlets = (int)mh.meshlets.size();
+  m.front_sign = mh.front_sign;
+  m.closed = mh.closed;
+  for (int i = 0; i < 4; ++i) m.bs[i] = mh.bs[i];
+  m.diameter = diameter;
+  m.loaded = true;
+  FP_TRY(write_mesh_table(c));
   return 0;
   FP_API_END
+}
+
+int fp_set_mesh(fp_ctx* c, int V, int F, const float* pos, const float* nrm, const float* uv, const float* vcol,
+                const int* faces, const unsigned char* tex_rgb, int Ht, int Wt, float diameter) {
+  return fp_set_mesh_slot(c, 0, V, F, pos, nrm, uv, vcol, faces, tex_rgb, Ht, Wt, diameter);
 }
 
 int fp_set_crop_tile(fp_ctx* c, int tile) {
@@ -782,12 +861,13 @@ int fp_set_crop_tile(fp_ctx* c, int tile) {
 
 int fp_mesh_info(fp_ctx* c, int* info) {
   FP_API_BEGIN
-  FP_REQUIRE(c && info && c->has_mesh, "fp_mesh_info: no mesh");
-  info[0] = c->n_meshlets;
-  info[1] = c->mesh_closed;
-  info[2] = c->cull_backfaces ? c->front_sign : 0;
-  info[3] = c->V;
-  info[4] = c->F;
+  FP_REQUIRE(c && info && c->mesh[0].loaded, "fp_mesh_info: no mesh");
+  const MeshSlot& m = c->mesh[0];
+  info[0] = m.n_meshlets;
+  info[1] = m.closed;
+  info[2] = c->cull_backfaces ? m.front_sign : 0;
+  info[3] = m.V;
+  info[4] = m.F;
   return 0;
   FP_API_END
 }
@@ -946,7 +1026,7 @@ int fp_refine(fp_ctx* c, const float* poses_in, int N, int iterations, float* po
   FP_API_BEGIN
   FP_REQUIRE(c && poses_in && poses_out && N >= 0 && iterations >= 0, "fp_refine: bad argument");
   FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
-  FP_REQUIRE(c->has_mesh && c->has_frame, "fp_refine: needs fp_set_mesh and fp_set_frame first");
+  FP_REQUIRE(c->mesh[0].loaded && c->has_frame, "fp_refine: needs fp_set_mesh and fp_set_frame first");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (N == 0) return 0;
@@ -969,7 +1049,7 @@ int fp_score_features(fp_ctx* c, const float* poses, int N, float* feats_out, vo
   FP_API_BEGIN
   FP_REQUIRE(c && poses && feats_out && N >= 0, "fp_score_features: bad argument");
   FP_REQUIRE(c->net[1].loaded, "scorer weights not loaded");
-  FP_REQUIRE(c->has_mesh && c->has_frame, "fp_score_features: needs fp_set_mesh and fp_set_frame first");
+  FP_REQUIRE(c->mesh[0].loaded && c->has_frame, "fp_score_features: needs fp_set_mesh and fp_set_frame first");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (N == 0) return 0;
@@ -1057,36 +1137,20 @@ int fp_track(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, 
   FP_API_BEGIN
   FP_REQUIRE(c && rgb_host && depth_host && K && H > 0 && W > 0 && iterations >= 0, "fp_track: bad argument");
   FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
-  FP_REQUIRE(c->has_mesh, "fp_track: no mesh");
+  FP_REQUIRE(c->mesh[0].loaded, "fp_track: no mesh");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const size_t npix = (size_t)H * W;
   FP_TRY(ensure_capacity(c, 1));
   FP_TRY(prepare_frame(c, K, H, W, true));
   FP_TRY(dev_alloc(c->epoch, c->track_pose, 64));
-  if (c->stage_npix < npix) {
-    if (c->stage_rgb) cudaFreeHost(c->stage_rgb);
-    if (c->stage_depth) cudaFreeHost(c->stage_depth);
-    c->stage_rgb = c->stage_depth = nullptr;
-    c->stage_npix = 0;
-    FP_CUDA_OK(cudaMallocHost(&c->stage_rgb, npix * 3));
-    FP_CUDA_OK(cudaMallocHost(&c->stage_depth, npix * 4));
-    c->stage_npix = npix;
-    ++c->epoch;  // the graph's copy nodes hold these addresses
-  }
+  FP_TRY(alloc_frame_staging(c, (size_t)H * W));
   if (!c->stage_pose) FP_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&c->stage_pose), 64));
   if (pose_in_dev) {
     FP_CUDA_OK(cudaMemcpyAsync(c->track_pose.p, pose_in_dev, 64, cudaMemcpyDeviceToDevice, st));
   } else {
     FP_REQUIRE(c->track_valid, "fp_track: no previous pose in this context: pass pose_in");
   }
-  // the previous frame's graph has finished (fp_track synchronises), so the staging buffers are free.  The two
-  // uploads are issued as soon as their staging copy is done — the depth DMA runs under the host's rgb copy, the
-  // rgb DMA under the graph launch — instead of being nodes of the graph (measured: -40 us per frame)
-  memcpy(c->stage_depth, depth_host, npix * 4);
-  FP_CUDA_OK(cudaMemcpyAsync(c->depth_raw.p, c->stage_depth, npix * 4, cudaMemcpyHostToDevice, st));
-  memcpy(c->stage_rgb, rgb_host, npix * 3);
-  FP_CUDA_OK(cudaMemcpyAsync(c->rgb_raw.p, c->stage_rgb, npix * 3, cudaMemcpyHostToDevice, st));
+  FP_TRY(upload_staged_frame(c, rgb_host, depth_host, (size_t)H * W, st));
   c->has_frame = false;
   float* pa = reinterpret_cast<float*>(c->poses_a.p);
   float* pb = reinterpret_cast<float*>(c->poses_b.p);
@@ -1112,6 +1176,63 @@ int fp_track(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, 
   FP_API_END
 }
 
+int fp_track_objects(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W, int M,
+                     const int* slots_host, const float* poses_in_dev, int iterations, float* poses_out_dev,
+                     float* poses_out_host, void* stream) {
+  FP_API_BEGIN
+  FP_REQUIRE(c && rgb_host && depth_host && K && H > 0 && W > 0 && M > 0 && slots_host && poses_in_dev && iterations >= 0,
+             "fp_track_objects: bad argument");
+  FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
+  // the kernels index the mesh table with these ids unchecked: an empty slot must never reach them
+  for (int i = 0; i < M; ++i) {
+    FP_REQUIRE(slots_host[i] >= 0 && slots_host[i] < kMaxMeshes, "fp_track_objects: object %d: slot %d out of range [0, %d)", i,
+               slots_host[i], kMaxMeshes);
+    FP_REQUIRE(c->mesh[slots_host[i]].loaded, "fp_track_objects: object %d: slot %d holds no mesh", i, slots_host[i]);
+  }
+  DeviceGuard dg(c->device);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(ensure_capacity(c, M));
+  FP_TRY(prepare_frame(c, K, H, W, true));
+  FP_TRY(dev_alloc(c->epoch, c->mesh_of, (size_t)M * sizeof(int)));
+  FP_TRY(alloc_frame_staging(c, (size_t)H * W));
+  if (c->stage_poses_n < M) {
+    if (c->stage_poses) cudaFreeHost(c->stage_poses);
+    c->stage_poses = nullptr;
+    c->stage_poses_n = 0;
+    FP_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&c->stage_poses), (size_t)M * 64));
+    c->stage_poses_n = M;
+    ++c->epoch;  // the graph's read-back node holds this address
+  }
+  float* pa = reinterpret_cast<float*>(c->poses_a.p);
+  float* pb = reinterpret_cast<float*>(c->poses_b.p);
+  const int* mesh_of = reinterpret_cast<const int*>(c->mesh_of.p);
+  // slot ids and start poses go to fixed context buffers ahead of the launch: the graph is keyed on (M, iterations)
+  // alone, so any set or order of objects replays it
+  FP_CUDA_OK(cudaMemcpyAsync(c->mesh_of.p, slots_host, (size_t)M * sizeof(int), cudaMemcpyHostToDevice, st));
+  FP_CUDA_OK(cudaMemcpyAsync(pa, poses_in_dev, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
+  FP_TRY(upload_staged_frame(c, rgb_host, depth_host, (size_t)H * W, st));
+  c->has_frame = false;
+  const float* fin = (iterations % 2 == 0) ? pa : pb;
+  auto body = [&](cudaStream_t s2) -> int {
+    // estimater.py:250-268 for every object at once: one filtered frame, M hypotheses each rendering its own mesh
+    FP_TRY(set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->rgb_raw.p),
+                              reinterpret_cast<const float*>(c->depth_raw.p), FP_FRAME_FILTER_DEPTH, INFINITY, s2));
+    c->has_frame = true;
+    FP_TRY(refine_body(c, M, iterations, s2, mesh_of));
+    FP_CUDA_OK(cudaMemcpyAsync(c->stage_poses, fin, (size_t)M * 64, cudaMemcpyDeviceToHost, s2));
+    return 0;
+  };
+  FP_TRY(run_graphed(c, 3, M, iterations, st, body));
+  c->has_frame = true;
+  if (poses_out_dev) FP_CUDA_OK(cudaMemcpyAsync(poses_out_dev, fin, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
+  FP_CUDA_OK(cudaStreamSynchronize(st));
+  if (poses_out_host) memcpy(poses_out_host, c->stage_poses, (size_t)M * 64);
+  return 0;
+  FP_API_END
+}
+
+unsigned long long fp_graph_captures(fp_ctx* c) { return c ? c->graph_captures : 0ull; }
+
 int fp_op_depth_filter(const float* depth_dev, float* out_dev, int H, int W, int which, void* stream) {
   FP_API_BEGIN
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -1125,8 +1246,8 @@ int fp_op_pose_update(const float* poses_in, const float* trans, const float* ro
                       float mesh_diameter, float rot_normalizer, void* stream) {
   FP_API_BEGIN
   FP_REQUIRE(poses_in && trans && rot && poses_out, "fp_op_pose_update: null argument");
-  return pose_update_launch(poses_in, trans, rot, poses_out, nullptr, nullptr, N, mesh_diameter / 2.0f, rot_normalizer,
-                            reinterpret_cast<cudaStream_t>(stream));
+  return pose_update_launch(poses_in, trans, rot, poses_out, nullptr, nullptr, N, nullptr, nullptr, mesh_diameter / 2.0f,
+                            rot_normalizer, reinterpret_cast<cudaStream_t>(stream));
   FP_API_END
 }
 

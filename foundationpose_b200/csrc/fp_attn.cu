@@ -15,6 +15,7 @@
 #include <stdlib.h>
 
 #include "fp_common.cuh"
+#include "fp_crop.cuh"
 #include "fp_gemm.cuh"
 
 namespace fp {
@@ -423,11 +424,14 @@ int score_tail_launch(const ScoreTailParams& p, cudaStream_t stream) {
 __global__ void pose_update_kernel(const float* __restrict__ pose_in, const float* __restrict__ trans,
                                    const float* __restrict__ rot, float* __restrict__ pose_out,
                                    float* __restrict__ trans_delta_out, float* __restrict__ rot_delta_out, int N,
+                                   const MeshSlotDev* __restrict__ slots, const int* __restrict__ mesh_of,
                                    float trans_scale, float rot_normalizer) {
   pdl_trigger();
   pdl_wait();
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= N) return;
+  // the half-diameter of the hypothesis's own mesh when a mesh table is given (slot 0 without slot ids)
+  if (slots) trans_scale = slots[mesh_of ? mesh_of[n] : 0].half_diameter;
   const float* A = pose_in + (size_t)n * 16;
   // trans_delta = output['trans'] * (mesh_diameter / 2)   (normalize_xyz, predict_pose_refine.py:199,228-229)
   const float td[3] = {trans[n * 3] * trans_scale, trans[n * 3 + 1] * trans_scale, trans[n * 3 + 2] * trans_scale};
@@ -483,11 +487,11 @@ __global__ void pose_update_kernel(const float* __restrict__ pose_in, const floa
 }
 
 int pose_update_launch(const float* pose_in, const float* trans, const float* rot, float* pose_out,
-                       float* trans_delta_out, float* rot_delta_out, int N, float trans_scale, float rot_normalizer,
-                       cudaStream_t stream) {
+                       float* trans_delta_out, float* rot_delta_out, int N, const MeshSlotDev* slots, const int* mesh_of,
+                       float trans_scale, float rot_normalizer, cudaStream_t stream) {
   if (N == 0) return 0;
   FP_CUDA_OK(launch_pdl(pose_update_kernel, dim3((N + 127) / 128), dim3(128), 0, stream, 1, pose_in, trans, rot, pose_out,
-                        trans_delta_out, rot_delta_out, N, trans_scale, rot_normalizer));
+                        trans_delta_out, rot_delta_out, N, slots, mesh_of, trans_scale, rot_normalizer));
   note_launches(1);
   FP_CUDA_OK(cudaGetLastError());
   return 0;

@@ -44,9 +44,12 @@ struct ScoreTailParams {
 };
 int score_tail_launch(const ScoreTailParams& p, cudaStream_t stream);
 
+struct MeshSlotDev;  // fp_crop.cuh
+// trans_scale = mesh_diameter / 2 of every hypothesis; with a mesh table (`slots`, device) each hypothesis takes the
+// half-diameter of its slot mesh_of[n] instead (slot 0 when mesh_of is null)
 int pose_update_launch(const float* pose_in, const float* trans, const float* rot, float* pose_out,
-                       float* trans_delta_out, float* rot_delta_out, int N, float trans_scale, float rot_normalizer,
-                       cudaStream_t stream);
+                       float* trans_delta_out, float* rot_delta_out, int N, const MeshSlotDev* slots, const int* mesh_of,
+                       float trans_scale, float rot_normalizer, cudaStream_t stream);
 int f32_to_f16_launch(const float* x, __half* y, size_t n, cudaStream_t stream);
 
 }  // namespace fp

@@ -1,7 +1,8 @@
 // fp_crop.cu — tiled "pose -> 160x160 network inputs" producer.  ONE kernel; one CTA per (pose hypothesis, TILE x TILE
 // pixel tile of the crop; TILE = 80 / 32 / 16 by batch size); nothing full-frame, nothing fp32 and no intermediate of
-// any kind is materialised in HBM:
-//   1. crop window from the pose                          (Utils.py:577-621 compute_crop_window_tf_batch, 'box_3d')
+// any kind is materialised in HBM.  Each hypothesis renders the mesh of its own slot of the context's mesh table
+// (CropParams::mesh_of), so one launch can crop several objects:
+//   1. crop window from the pose                         (Utils.py:577-621 compute_crop_window_tf_batch, 'box_3d')
 //   2. binning: every MESHLET of the mesh (<= 64 triangles, fp_meshlet.cu) is tested against the tile with its
 //      bounding sphere and — closed meshes — its normal cone; survivors go to a shared-memory list
 //   3. raster: each warp takes meshlets off the list, transforms their <= 64 vertices into shared memory, sets up
@@ -276,7 +277,9 @@ struct TileSmem {
   int list[kListCap];
   int n_list, next;
   int stat[4];
+  MeshSlotDev slot;  // mesh table entry of this CTA's hypothesis
 };
+static_assert(sizeof(MeshSlotDev) % 16 == 0 && sizeof(MeshSlotDev) / 16 <= kThreads, "table entry copied as uint4s");
 
 // one triangle of a meshlet, all three vertices in front of the near plane: coverage inside the tile + depth test
 template <int TILE>
@@ -353,7 +356,7 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
   const int n = blockIdx.y;
   const int tile = blockIdx.x;
   const int ty0 = (tile / TPR) * TILE, tx0 = (tile % TPR) * TILE;
-  const MeshDev& M = p.mesh;
+  const MeshDev& M = sm.slot.mesh;
 
   for (int i = tid; i < TILE * TILE; i += kThreads) sm.zt[i] = 0ull;
   if (tid == 0) {
@@ -361,13 +364,19 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
     sm.next = 0;
     sm.stat[0] = sm.stat[1] = sm.stat[2] = sm.stat[3] = 0;
   }
+  // The mesh table and the slot ids are written by copies that precede the whole launch sequence, never by a kernel
+  // of it: they may be read before the programmatic-dependency wait.
+  if (tid < (int)(sizeof(MeshSlotDev) / 16)) {
+    const int s = p.mesh_of ? __ldg(p.mesh_of + n) : 0;
+    reinterpret_cast<uint4*>(&sm.slot)[tid] = __ldg(reinterpret_cast<const uint4*>(p.slots + s) + tid);
+  }
   pdl_trigger();
   pdl_wait();  // the poses come from the previous iteration's pose update; the crop buffer is read by its stem conv
   if (tid < 16) sm.P[tid] = p.poses[(size_t)n * 16 + tid];
   __syncthreads();
   if (warp == 0) {
     Window w;
-    crop_window_warp(sm.P, p.fx, p.fy, p.cx, p.cy, p.r3, lane, w);
+    crop_window_warp(sm.P, p.fx, p.fy, p.cx, p.cy, sm.slot.r3[p.mode ? 1 : 0], lane, w);
     if (lane == 0) {
       sm.win = w;
       if (p.win_out && tile == 0) {
@@ -571,7 +580,7 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
 
   // ---- shade: a warp resolves 8 x 4-pixel blocks (coverage is coherent in 2-D: fewer warps straddle the silhouette
   // than with 32 x 1 rows, and those are the ones that pay for both the covered and the background path)
-  const float inv_radius = p.inv_radius;
+  const float inv_radius = sm.slot.inv_radius;
   const float tvec[3] = {sm.P[3], sm.P[7], sm.P[11]};
   const float tau = p.mode == 0 ? 0.001f : 0.1f;
   const size_t img_stride = (size_t)(S + 6) * (S + 8) * 8;
@@ -640,24 +649,26 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
       const float Z = w0 * vs[0].Z + w1 * vs[1].Z + w2 * vs[2].Z;
       const float diffuse = w0 * dif[0] + w1 * dif[1] + w2 * dif[2];
       float cr, cg, cb;
-      if (p.has_tex) {
+      if (sm.slot.has_tex) {
+        const int Ht = sm.slot.Ht, Wt = sm.slot.Wt;
+        const uchar4* tex = sm.slot.tex;
         const float tu = w0 * att[0].x + w1 * att[1].x + w2 * att[2].x;
         const float tv = w0 * att[0].y + w1 * att[1].y + w2 * att[2].y;
         // dr.texture(filter_mode='linear', boundary 'wrap'): texel centres at +0.5.  Interpolated uv of a mesh lie in
         // (-1, 2): the wrap is two conditional adds; anything further out takes the general modulo.
-        const float xx = tu * p.Wt - 0.5f, yy = tv * p.Ht - 0.5f;
+        const float xx = tu * Wt - 0.5f, yy = tv * Ht - 0.5f;
         const float xf = floorf(xx), yf = floorf(yy);
         const float ax1 = xx - xf, ay1 = yy - yf;
         int x0 = (int)xf, y0 = (int)yf;
-        if ((unsigned)(x0 + p.Wt) >= (unsigned)(3 * p.Wt)) x0 %= p.Wt;
-        if ((unsigned)(y0 + p.Ht) >= (unsigned)(3 * p.Ht)) y0 %= p.Ht;
-        if (x0 < 0) x0 += p.Wt;
-        if (y0 < 0) y0 += p.Ht;
-        if (x0 >= p.Wt) x0 -= p.Wt;
-        if (y0 >= p.Ht) y0 -= p.Ht;
-        const int x1 = (x0 + 1 == p.Wt) ? 0 : x0 + 1, y1 = (y0 + 1 == p.Ht) ? 0 : y0 + 1;
-        const uchar4 t00 = __ldg(p.tex + (size_t)y0 * p.Wt + x0), t01 = __ldg(p.tex + (size_t)y0 * p.Wt + x1);
-        const uchar4 t10 = __ldg(p.tex + (size_t)y1 * p.Wt + x0), t11 = __ldg(p.tex + (size_t)y1 * p.Wt + x1);
+        if ((unsigned)(x0 + Wt) >= (unsigned)(3 * Wt)) x0 %= Wt;
+        if ((unsigned)(y0 + Ht) >= (unsigned)(3 * Ht)) y0 %= Ht;
+        if (x0 < 0) x0 += Wt;
+        if (y0 < 0) y0 += Ht;
+        if (x0 >= Wt) x0 -= Wt;
+        if (y0 >= Ht) y0 -= Ht;
+        const int x1 = (x0 + 1 == Wt) ? 0 : x0 + 1, y1 = (y0 + 1 == Ht) ? 0 : y0 + 1;
+        const uchar4 t00 = __ldg(tex + (size_t)y0 * Wt + x0), t01 = __ldg(tex + (size_t)y0 * Wt + x1);
+        const uchar4 t10 = __ldg(tex + (size_t)y1 * Wt + x0), t11 = __ldg(tex + (size_t)y1 * Wt + x1);
         const float w00 = (1.f - ax1) * (1.f - ay1), w01 = ax1 * (1.f - ay1), w10 = (1.f - ax1) * ay1, w11 = ax1 * ay1;
         const float k255 = 1.f / 255.f;
         cr = (w00 * t00.x + w01 * t01.x + w10 * t10.x + w11 * t11.x) * k255;

@@ -37,18 +37,29 @@ struct MeshDev {
                    // is a back face, which nvdiffrast shows)
 };
 
+constexpr int kMaxMeshes = 64;  // FP_MAX_MESHES (include/fpose.h)
+
+// One entry of the context's device-side mesh table: everything the crop producer and the pose update read about
+// the mesh a hypothesis renders.  The host fills it with the expressions fp_api.cu used for its by-value kernel
+// parameters, so slot 0 reproduces those values bit for bit.
+struct __align__(16) MeshSlotDev {
+  MeshDev mesh;       // front_sign already 0 when back-face culling is disabled (FPOSE_NO_CULL)
+  const uchar4* tex;  // [Ht][Wt] RGBA8 or null
+  int has_tex;
+  int Ht, Wt;
+  float r3[2];          // mesh_diameter * crop_ratio / 2 (Utils.py:603), [0] refiner, [1] scorer crop ratio
+  float inv_radius;     // 1 / (mesh_diameter / 2)       (h5_dataset.py:96)
+  float half_diameter;  // mesh_diameter / 2             (predict_pose_refine.py:199, pose update)
+};
+
 struct CropParams {
   const float* poses;  // [N][16] row-major ob_in_cam
   int N;
   float fx, fy, cx, cy;
   int H, W;
-  float r3;          // mesh_diameter * crop_ratio / 2 (Utils.py:603)
-  float inv_radius;  // 1 / (mesh_diameter / 2)       (h5_dataset.py:96)
   float znear, zfar; // Utils.py:161 projection_matrix_from_intrinsics(znear=0.001, zfar=100)
-  MeshDev mesh;
-  int has_tex;
-  const uchar4* tex;  // [Ht][Wt] RGBA8 or null
-  int Ht, Wt;
+  const MeshSlotDev* slots;  // [kMaxMeshes] device mesh table
+  const int* mesh_of;        // [N] slot of every hypothesis, device; null = every hypothesis renders slot 0
   // frame (device)
   const uchar4* rgb;      // [H][W] RGBA8
   const float4* xyz_map;  // [H][W] (x, y, z, 0)   (mode 0)

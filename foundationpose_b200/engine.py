@@ -29,8 +29,12 @@ def _proto():
     lib.fp_set_crop_tile.argtypes = [vp, i]
     lib.fp_crop_stats.argtypes = [vp, vp, i, i, C.POINTER(i), vp]
     lib.fp_track.argtypes = [vp, vp, vp, C.POINTER(f), i, i, vp, i, vp, vp, vp]
+    lib.fp_track_objects.argtypes = [vp, vp, vp, C.POINTER(f), i, i, i, C.POINTER(i), vp, i, vp, vp, vp]
+    lib.fp_graph_captures.argtypes = [vp]
+    lib.fp_graph_captures.restype = C.c_ulonglong
     lib.fp_load_network.argtypes = [vp, i, C.POINTER(_FpTensor), i]
     lib.fp_set_mesh.argtypes = [vp, i, i, vp, vp, vp, vp, vp, vp, i, i, f]
+    lib.fp_set_mesh_slot.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp, vp, i, i, f]
     lib.fp_set_frame.argtypes = [vp, vp, vp, C.POINTER(f), i, i, i, f, vp]
     lib.fp_get_depth.argtypes = [vp, vp, vp, vp]
     lib.fp_set_xyz_map.argtypes = [vp, vp, vp]
@@ -46,7 +50,8 @@ def _proto():
     lib.fp_op_tokens.argtypes = [vp, i, vp, i, vp, vp]
     lib.fp_op_depth_filter.argtypes = [vp, vp, i, i, i, vp]
     lib.fp_op_pose_update.argtypes = [vp, vp, vp, vp, i, f, f, vp]
-    for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_crop_stats", "fp_track", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh", "fp_set_frame",
+    for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh",
+                 "fp_set_mesh_slot", "fp_set_frame",
                  "fp_get_depth", "fp_make_crops", "fp_start_poses", "fp_refine", "fp_score", "fp_score_features", "fp_score_tail",
                  "fp_register", "fp_op_refine_net", "fp_op_score_feats", "fp_op_tokens", "fp_op_depth_filter",
                  "fp_op_pose_update"):
@@ -56,6 +61,7 @@ def _proto():
 _proto()
 
 FRAME_ON_DEVICE = 1
+MAX_MESHES = 64  # FP_MAX_MESHES: mesh slots per context
 _NO_PIN = os.environ.get("FPOSE_NO_PIN") == "1"  # A/B: skip the pinned staging of host frames
 FRAME_FILTER_DEPTH = 2
 
@@ -175,8 +181,9 @@ class Engine:
             arr[i] = _FpTensor(name.encode(), a.ctypes.data, 1 if a.dtype == np.float16 else 0, a.size)
         _lib.check(lib.fp_load_network(self._h, 0 if kind == "refine" else 1, arr, len(packed)), "fp_load_network")
 
-    def set_mesh(self, vertices, normals, faces, diameter, uv=None, tex=None, vertex_colors=None):
-        """uv: (V,2) with v already flipped (Utils.py:117); tex: uint8 (Ht,Wt,3); vertex_colors: float 0..1."""
+    def set_mesh(self, vertices, normals, faces, diameter, uv=None, tex=None, vertex_colors=None, slot=0):
+        """uv: (V,2) with v already flipped (Utils.py:117); tex: uint8 (Ht,Wt,3); vertex_colors: float 0..1.
+        slot: 0..MAX_MESHES-1; slot 0 is the mesh of every single-object call, the others are for track_objects."""
         pos = np.ascontiguousarray(vertices, dtype=np.float32)
         nrm = np.ascontiguousarray(normals, dtype=np.float32)
         fc = np.ascontiguousarray(faces, dtype=np.int32)
@@ -189,10 +196,15 @@ class Engine:
         else:
             colp = np.ascontiguousarray(vertex_colors, dtype=np.float32)
         cp = lambda a: None if a is None else C.c_void_p(a.ctypes.data)
-        _lib.check(lib.fp_set_mesh(self._h, len(pos), len(fc), cp(pos), cp(nrm), cp(uvp), cp(colp), cp(fc), cp(texp), Ht, Wt,
-                                   float(diameter)), "fp_set_mesh")
-        self.diameter = float(diameter)
-        self.mesh_key = (len(pos), len(fc), float(diameter))
+        _lib.check(lib.fp_set_mesh_slot(self._h, int(slot), len(pos), len(fc), cp(pos), cp(nrm), cp(uvp), cp(colp), cp(fc), cp(texp),
+                                        Ht, Wt, float(diameter)), "fp_set_mesh")
+        if slot == 0:
+            self.diameter = float(diameter)
+            self.mesh_key = (len(pos), len(fc), float(diameter))
+
+    def graph_captures(self):
+        """Number of CUDA graphs this context has captured (a replay captures none)."""
+        return int(lib.fp_graph_captures(self._h))
 
     def mesh_info(self):
         """dict(meshlets, closed, front_sign, V, F) of the mesh in the context (fp_mesh_info)."""
@@ -228,6 +240,27 @@ class Engine:
                                 int(iterations), _p(pose_out), C.c_void_p(host.ctypes.data), _stream()), "fp_track")
         self.frame_hw = (H, W)
         return pose_out, host
+
+    def track_objects(self, rgb, depth, K, poses_in, slots, iterations):
+        """fp_track_objects: `track` for M objects of one frame in ONE CUDA-graph launch, object i rendering the mesh in
+        slot slots[i] (loaded by set_mesh(..., slot=)).  rgb uint8 (H,W,3) / depth float32 (H,W) HOST arrays; poses_in
+        (M,4,4) CUDA tensor.  Returns (poses CUDA (M,4,4), poses host (M,4,4) float32 numpy)."""
+        rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
+        depth = np.ascontiguousarray(depth, dtype=np.float32)
+        H, W = depth.shape
+        Kf = (C.c_float * 9)(*[float(x) for x in np.asarray(K, dtype=np.float64).reshape(-1)])
+        poses_in = poses_in.reshape(-1, 4, 4).contiguous().float()
+        M = len(poses_in)
+        slots = [int(s) for s in slots]
+        if len(slots) != M:
+            raise ValueError(f"track_objects: {M} poses but {len(slots)} slots")
+        out = torch.empty(M, 4, 4, dtype=torch.float32, device="cuda")
+        host = np.empty((M, 4, 4), dtype=np.float32)
+        _lib.check(lib.fp_track_objects(self._h, C.c_void_p(rgb.ctypes.data), C.c_void_p(depth.ctypes.data), Kf, H, W, M,
+                                        (C.c_int * M)(*slots), _p(poses_in), int(iterations), _p(out),
+                                        C.c_void_p(host.ctypes.data), _stream()), "fp_track_objects")
+        self.frame_hw = (H, W)
+        return out, host
 
     def set_frame(self, rgb, depth, K, filter_depth=True, zfar=float("inf")):
         """rgb uint8 (H,W,3), depth float32 (H,W): numpy / CPU tensors (pinned for async H2D) or CUDA tensors."""

@@ -13,12 +13,13 @@ the one already in the context is uploaded first, a caller-supplied xyz map repl
 """
 import logging
 import os
+import weakref
 
 import numpy as np
 import torch
 
 from . import hypotheses, meshprep, synth, weights
-from .engine import Engine
+from .engine import MAX_MESHES, Engine
 
 
 class _Cfg(dict):
@@ -337,6 +338,68 @@ class FoundationPose:
         pose_dev, pose_host = e.track(rgb, depth, K, self.pose_last.reshape(4, 4), iteration)
         self.pose_last = pose_dev.reshape(1, 4, 4)
         self.refiner.last_trans_update = self.refiner.last_rot_update = None
-        out = pose_host.astype(np.float64)
-        out[:3, 3] -= out[:3, :3] @ np.asarray(self.model_center, dtype=np.float64)  # pose @ T(-model_center), estimater.py:268
-        return out.astype(np.float32)
+        return _uncentre(pose_host, self.model_center)
+
+
+def _uncentre(pose_host, model_center):
+    """pose @ T(-model_center) on the host (estimater.py:268): the pose of the original, un-centred mesh."""
+    out = pose_host.astype(np.float64)
+    out[:3, 3] -= out[:3, :3] @ np.asarray(model_center, dtype=np.float64)
+    return out.astype(np.float32)
+
+
+def _object_slot(est):
+    """The slot of `est`'s mesh in its engine (1..MAX_MESHES-1; slot 0 stays with the single-object calls): assigned at
+    first use, reloaded when reset_object() replaced the estimator's mesh_tensors."""
+    e = est.engine
+    owners = e.__dict__.setdefault("_object_slots", {})  # slot -> weakref to the estimator that owns it
+    slot = getattr(est, "_object_slot", None)
+    if slot is None or slot not in owners or owners[slot]() is not est:
+        for s in [s for s, r in owners.items() if r() is None]:
+            del owners[s]  # the estimator was garbage-collected
+        free = [s for s in range(1, MAX_MESHES) if s not in owners]
+        if not free:
+            raise ValueError(f"track_objects: an engine holds at most {MAX_MESHES - 1} object meshes")
+        slot = free[0]
+        owners[slot] = weakref.ref(est)
+        est._object_slot, est._object_slot_src = slot, None
+    if est._object_slot_src is not est.mesh_tensors:
+        mt = est.mesh_tensors
+        e.set_mesh(mt["pos"], mt["normals"], mt["faces"], est.diameter, uv=mt.get("uv"), tex=mt.get("tex"),
+                   vertex_colors=mt.get("vcolor"), slot=slot)
+        est._object_slot_src = mt
+    return slot
+
+
+def track_objects(estimators, rgb, depth, K, iteration=2):
+    """`[est.track_one(rgb, depth, K, iteration) for est in estimators]` for several objects of one camera stream, as ONE
+    CUDA-graph launch per frame (fp_track_objects): the frame is uploaded and filtered once and the objects' poses are
+    refined as one batch, each rendering its own mesh.  Same poses as the per-object calls; updates every pose_last.
+
+    The estimators must share one engine (the default: get_engine()).  Each one keeps its mesh in a slot of that engine,
+    so alternating objects re-uploads nothing.  Host frames only (uint8 (H,W,3) rgb, float32 (H,W) depth).
+    Returns a list of (4,4) float32 poses of the original meshes."""
+    estimators = list(estimators)
+    if not estimators:
+        return []
+    if torch.is_tensor(rgb) or torch.is_tensor(depth):
+        raise TypeError("track_objects takes host frames (numpy); for device-resident frames call track_one per object")
+    e = estimators[0].engine
+    if any(est.engine is not e for est in estimators):
+        raise ValueError("track_objects: the estimators must share one engine")
+    if len({id(est) for est in estimators}) != len(estimators):
+        raise ValueError("track_objects: an estimator appears more than once")
+    if len(estimators) > MAX_MESHES - 1:
+        raise ValueError(f"track_objects: at most {MAX_MESHES - 1} objects per engine, got {len(estimators)}")
+    if any(est.pose_last is None for est in estimators):
+        logging.info("Please init pose by register first")
+        raise RuntimeError
+    slots = [_object_slot(est) for est in estimators]
+    poses_in = torch.stack([est.pose_last.reshape(4, 4) for est in estimators])
+    poses_dev, poses_host = e.track_objects(rgb, depth, K, poses_in, slots, iteration)
+    out = []
+    for i, est in enumerate(estimators):
+        est.pose_last = poses_dev[i].reshape(1, 4, 4)
+        est.refiner.last_trans_update = est.refiner.last_rot_update = None
+        out.append(_uncentre(poses_host[i], est.model_center))
+    return out

@@ -78,13 +78,24 @@ def make_texture(seed=0, size=1024, block=16):
     return np.ascontiguousarray(np.repeat(np.repeat(low, block, 0), block, 1))
 
 
-def make_mesh(subdivisions=5, tex_seed=0, tex_size=1024):
+def make_mesh(subdivisions=5, tex_seed=0, tex_size=1024, scale=1.0):
+    """Textured icosphere ellipsoid of radii RADII * scale (the object make_multi_scene draws at that scale)."""
     q, f = icosphere(subdivisions)
-    verts = q * RADII
-    nrm = q / RADII
+    radii = RADII * scale
+    verts = q * radii
+    nrm = q / radii
     nrm /= np.linalg.norm(nrm, axis=1, keepdims=True)
     uv = sphere_uv(q)
     return SimpleMesh(verts, f, nrm, uv=uv, texture=make_texture(tex_seed, tex_size))
+
+
+def vertex_coloured(mesh):
+    """The same object with its texture sampled at the vertices: uint8 vertex colours instead of uv + texture."""
+    tex = mesh.visual.image
+    Ht, Wt = tex.shape[:2]
+    tx = np.clip((mesh.visual.uv[:, 0] * Wt).astype(np.int64), 0, Wt - 1)
+    ty = np.clip(((1.0 - mesh.visual.uv[:, 1]) * Ht).astype(np.int64), 0, Ht - 1)
+    return SimpleMesh(mesh.vertices, mesh.faces, mesh.vertex_normals, vertex_colors=tex[ty, tx])
 
 
 def mesh_diameter(vertices):
@@ -110,35 +121,50 @@ def random_rotation(seed):
 def make_scene(mesh_texture, pose, K=DEFAULT_K, H=480, W=640, plane_z=1.2, seed=1, depth_noise=0.001):
     """Analytic RGB-D frame: ellipsoid (radii RADII, texture via spherical UV) at `pose` (4x4 ob_in_cam)
     in front of a textured plane at z = plane_z.  Returns rgb uint8 (H,W,3), depth float32 (H,W), mask bool."""
+    rgb, depth, owner = make_multi_scene([(mesh_texture, pose, 1.0)], K, H, W, plane_z, seed, depth_noise)
+    return rgb, depth, owner == 0
+
+
+def make_multi_scene(objects, K=DEFAULT_K, H=480, W=640, plane_z=1.2, seed=1, depth_noise=0.001):
+    """Analytic RGB-D frame of several ellipsoids in front of the textured plane of make_scene.  objects: sequence of
+    (texture, pose, scale): an ellipsoid of radii RADII * scale (make_mesh(scale=scale)) at `pose` (4x4 ob_in_cam),
+    coloured from `texture` via spherical UV.  On every pixel ray the nearest positive hit wins, so objects occlude
+    each other.  Returns rgb uint8 (H,W,3), depth float32 (H,W) and the index of the object seen at each pixel (-1 =
+    the plane)."""
     rng = np.random.default_rng(seed)
     vs, us = np.meshgrid(np.arange(H), np.arange(W), indexing="ij")
     d = np.stack([(us - K[0, 2]) / K[0, 0], (vs - K[1, 2]) / K[1, 1], np.ones_like(us, dtype=np.float64)], -1)
-    R, t = pose[:3, :3], pose[:3, 3]
-    o_ob = -R.T @ t
-    d_ob = d @ R  # rows: R^T d
-    so, sd = o_ob / RADII, d_ob / RADII
-    a = (sd * sd).sum(-1)
-    b = 2 * (sd * so).sum(-1)
-    c = (so * so).sum() - 1.0
-    disc = b * b - 4 * a * c
-    hit = disc > 0
-    s = np.where(hit, (-b - np.sqrt(np.maximum(disc, 0))) / (2 * a), 0.0)
-    hit &= s > 0
     depth = np.full((H, W), plane_z, dtype=np.float64)
-    depth[hit] = s[hit]
-    # colours
     bg = make_texture(seed + 100, 512, 32)
     bu = ((d[..., 0] * plane_z * 400).astype(np.int64)) % 512
     bv = ((d[..., 1] * plane_z * 400).astype(np.int64)) % 512
     rgb = bg[bv, bu].copy()
-    p_ob = o_ob + d_ob * s[..., None]
-    uv = sphere_uv(p_ob / RADII / np.maximum(np.linalg.norm(p_ob / RADII, axis=-1, keepdims=True), 1e-9))
-    Ht, Wt = mesh_texture.shape[:2]
-    tx = np.clip((uv[..., 0] * Wt).astype(np.int64), 0, Wt - 1)
-    ty = np.clip(((1.0 - uv[..., 1]) * Ht).astype(np.int64), 0, Ht - 1)  # trimesh uv: v = 0 is the image bottom
-    rgb[hit] = mesh_texture[ty, tx][hit]
+    owner = np.full((H, W), -1, dtype=np.int64)
+    nearest = np.full((H, W), np.inf)
+    for k, (texture, pose, scale) in enumerate(objects):
+        radii = RADII * scale
+        R, t = pose[:3, :3], pose[:3, 3]
+        o_ob = -R.T @ t
+        d_ob = d @ R  # rows: R^T d
+        so, sd = o_ob / radii, d_ob / radii
+        a = (sd * sd).sum(-1)
+        b = 2 * (sd * so).sum(-1)
+        c = (so * so).sum() - 1.0
+        disc = b * b - 4 * a * c
+        hit = disc > 0
+        s = np.where(hit, (-b - np.sqrt(np.maximum(disc, 0))) / (2 * a), 0.0)
+        hit &= (s > 0) & (s < nearest)
+        depth[hit] = s[hit]
+        nearest[hit] = s[hit]
+        owner[hit] = k
+        p_ob = o_ob + d_ob * s[..., None]
+        uv = sphere_uv(p_ob / radii / np.maximum(np.linalg.norm(p_ob / radii, axis=-1, keepdims=True), 1e-9))
+        Ht, Wt = texture.shape[:2]
+        tx = np.clip((uv[..., 0] * Wt).astype(np.int64), 0, Wt - 1)
+        ty = np.clip(((1.0 - uv[..., 1]) * Ht).astype(np.int64), 0, Ht - 1)  # trimesh uv: v = 0 is the image bottom
+        rgb[hit] = texture[ty, tx][hit]
     depth = depth + rng.normal(0, depth_noise, size=depth.shape)
-    return rgb.astype(np.uint8), depth.astype(np.float32), hit
+    return rgb.astype(np.uint8), depth.astype(np.float32), owner
 
 
 def default_scene(subdivisions=5, seed=0):

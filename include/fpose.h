@@ -111,7 +111,13 @@ int fp_load_network(fp_ctx* ctx, int which, const fp_tensor_t* tensors, int n);
  * vertex-coloured meshes).  diameter = estimater.py:54. */
 int fp_set_mesh(fp_ctx* ctx, int V, int F, const float* pos, const float* nrm, const float* uv, const float* vcol,
                 const int* faces, const unsigned char* tex_rgb, int Ht, int Wt, float diameter);
-/* What fp_set_mesh derived (test hook): info[5] = {meshlets, mesh is closed and consistently oriented (0/1),
+/* A context holds up to FP_MAX_MESHES meshes, one per slot.  fp_set_mesh is fp_set_mesh_slot(ctx, 0, ...); every
+ * single-object entry point renders slot 0, fp_track_objects renders the slots it is given.  Same arguments and
+ * validation as fp_set_mesh, plus the slot (0 <= slot < FP_MAX_MESHES).  Synchronises the device. */
+#define FP_MAX_MESHES 64
+int fp_set_mesh_slot(fp_ctx* ctx, int slot, int V, int F, const float* pos, const float* nrm, const float* uv,
+                     const float* vcol, const int* faces, const unsigned char* tex_rgb, int Ht, int Wt, float diameter);
+/* What fp_set_mesh derived for slot 0 (test hook): info[5] = {meshlets, mesh is closed and consistently oriented (0/1),
  * front-face winding sign used for back-face culling (0 = both sides are rendered, as nvdiffrast does), V, F}. */
 int fp_mesh_info(fp_ctx* ctx, int* info);
 
@@ -178,6 +184,19 @@ int fp_register(fp_ctx* ctx, const float* poses_host, int N, int iterations, flo
  * previous fp_track produced.  pose_out_dev (DEVICE [16]) / pose_out_host (HOST [16]) are optional.  Synchronises. */
 int fp_track(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
              const float* pose_in_dev, int iterations, float* pose_out_dev, float* pose_out_host, void* stream);
+/* FoundationPose.track_one (estimater.py:250-268) applied to M objects of the same frame, as ONE CUDA-graph launch:
+ * one pinned-staged upload of the frame, one erode_depth + bilateral_filter_depth + depth2xyzmap_batch(zfar = inf),
+ * `iterations` refiner passes over a batch of M hypotheses where hypothesis i renders the mesh in slot slots_host[i],
+ * read-back of the M poses.  slots_host: HOST [M] slot ids, each loaded (checked before anything is enqueued);
+ * poses_in_dev: DEVICE [M][16] ob_in_cam of each centred mesh; poses_out_dev (DEVICE [M][16]) / poses_out_host
+ * (HOST [M][16]) are optional.  Each pose equals what fp_track gives for that object alone.  The slot ids and poses
+ * are copied into the context first, so the cached graph depends on (M, iterations) only.  Leaves fp_track's
+ * continuation pose untouched.  Synchronises. */
+int fp_track_objects(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
+                     int M, const int* slots_host, const float* poses_in_dev, int iterations, float* poses_out_dev,
+                     float* poses_out_host, void* stream);
+/* Number of CUDA graphs this context has captured so far (test hook: a replay captures nothing). */
+unsigned long long fp_graph_captures(fp_ctx* ctx);
 
 /* ------------------------------------------------------------------------------------------ */
 /* one process, several GPUs (the reference's process model: run_demo.py is a single script)  */
