@@ -71,6 +71,11 @@ struct Net {
 
 constexpr int S = 160;
 constexpr int T = 400;
+// fp_register_objects refines and featurises whole objects in passes of at most this many hypotheses (an object above
+// it gets a pass of its own).  ensure_capacity costs ~15.6 MB per hypothesis, so the context keeps ~8 GB of workspace
+// after such a call; the largest buffer (refiner qkv, N * 400 * 3072 fp16) is 1.26 GB, and every element and byte
+// offset inside a buffer stays below 2^31.
+constexpr int kRegisterPassCap = 512;
 constexpr size_t kCropImg = (size_t)(S + 6) * (S + 8) * 8;  // fp16 elements per padded crop image
 // The encoder's first stage runs on the A (rendered) and B (observed) crops as one batch.  The 40x40
 // 128-channel layers tile four images per MMA (gemm_swap_patch_kernel), and the layer that fuses
@@ -143,6 +148,13 @@ struct fp_ctx {
   fp::DevBuf track_pose;
   float* stage_poses = nullptr;  // fp_track_objects: pinned [stage_poses_n][16] pose read-back
   int stage_poses_n = 0;
+  // fp_register_objects: row offsets of the objects' hypotheses [M + 1], their feature rows [sum N][512]; pinned staging
+  // of the masks and of (offsets, per-hypothesis slot ids)
+  fp::DevBuf seg_off, reg_feats;
+  unsigned char* stage_masks = nullptr;
+  size_t stage_masks_n = 0;
+  int* stage_ints = nullptr;
+  size_t stage_ints_n = 0;
 };
 
 namespace fp {
@@ -672,7 +684,8 @@ int fp_destroy(fp_ctx* c) {
                     &c->a3, &c->ab0, &c->ab1, &c->ab2, &c->c0, &c->c1, &c->c2, &c->tok, &c->qkv, &c->att, &c->x1pre,
                     &c->x1, &c->ff, &c->x2pre, &c->head_out, &c->poses_a, &c->poses_b, &c->feats, &c->tail_qkv,
                     &c->tail_attn, &c->tail_proj, &c->scores, &c->best, &c->lt_buf, &c->lr_buf, &c->feat_buf,
-                    &c->pose_stage, &c->mask_buf, &c->mask_stats, &c->crop_stats, &c->track_pose, &c->fold_v, &c->tail_counter, &c->tok_mean};
+                    &c->pose_stage, &c->mask_buf, &c->mask_stats, &c->crop_stats, &c->track_pose, &c->fold_v, &c->tail_counter, &c->tok_mean,
+                    &c->seg_off, &c->reg_feats};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   for (auto& kv : c->graphs)
@@ -685,6 +698,8 @@ int fp_destroy(fp_ctx* c) {
   if (c->stage_depth) cudaFreeHost(c->stage_depth);
   if (c->stage_pose) cudaFreeHost(c->stage_pose);
   if (c->stage_poses) cudaFreeHost(c->stage_poses);
+  if (c->stage_masks) cudaFreeHost(c->stage_masks);
+  if (c->stage_ints) cudaFreeHost(c->stage_ints);
   delete c;
   return 0;
   FP_API_END
@@ -938,7 +953,7 @@ int fp_start_poses(fp_ctx* c, const unsigned char* mask, int mask_on_device, con
     mdev = reinterpret_cast<const unsigned char*>(c->mask_buf.p);
   }
   FP_TRY(dev_alloc(c->epoch, c->mask_stats, 64));
-  return start_poses_launch(c->depth_cur, mdev, c->H, c->W, c->K[0], c->K[4], c->K[2], c->K[5], rot_grid, N,
+  return start_poses_launch(c->depth_cur, mdev, c->H, c->W, c->K[0], c->K[4], c->K[2], c->K[5], rot_grid, N, 1, nullptr,
                             reinterpret_cast<unsigned int*>(c->mask_stats.p), poses_out, info_out, st);
   FP_API_END
 }
@@ -1227,6 +1242,130 @@ int fp_track_objects(fp_ctx* c, const unsigned char* rgb_host, const float* dept
   if (poses_out_dev) FP_CUDA_OK(cudaMemcpyAsync(poses_out_dev, fin, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
   FP_CUDA_OK(cudaStreamSynchronize(st));
   if (poses_out_host) memcpy(poses_out_host, c->stage_poses, (size_t)M * 64);
+  return 0;
+  FP_API_END
+}
+
+int fp_register_objects(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
+                        int M, const int* slots_host, const int* n_hyp_host, const unsigned char* masks_host,
+                        const float* rot_grids_dev, int iterations, float* poses_out_dev, float* scores_out_dev,
+                        int* best_out_dev, float* info_out_dev, void* stream) {
+  FP_API_BEGIN
+  FP_REQUIRE(c && rgb_host && depth_host && K && H > 0 && W > 0 && M > 0 && M <= 65535 && slots_host && n_hyp_host &&
+                 masks_host && rot_grids_dev && iterations >= 0 && poses_out_dev && scores_out_dev && best_out_dev &&
+                 info_out_dev,
+             "fp_register_objects: bad argument");
+  FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
+  FP_REQUIRE(c->net[1].loaded, "scorer weights not loaded");
+  // everything is checked before anything is enqueued: the kernels index the mesh table with these ids unchecked
+  std::vector<int> off(M + 1, 0);
+  int seg_max = 0;
+  for (int i = 0; i < M; ++i) {
+    FP_REQUIRE(slots_host[i] >= 0 && slots_host[i] < kMaxMeshes, "fp_register_objects: object %d: slot %d out of range [0, %d)",
+               i, slots_host[i], kMaxMeshes);
+    FP_REQUIRE(c->mesh[slots_host[i]].loaded, "fp_register_objects: object %d: slot %d holds no mesh", i, slots_host[i]);
+    FP_REQUIRE(n_hyp_host[i] >= 1 && n_hyp_host[i] <= 4096, "fp_register_objects: object %d: %d hypotheses, need 1..4096", i,
+               n_hyp_host[i]);
+    off[i + 1] = off[i] + n_hyp_host[i];
+    seg_max = std::max(seg_max, n_hyp_host[i]);
+  }
+  const int total = off[M];
+  // passes: whole objects in the given order, up to kRegisterPassCap hypotheses; an object above the cap alone
+  std::vector<int> pass_obj(1, 0);  // first object of every pass, then M
+  for (int i = 1; i < M; ++i)
+    if (off[i + 1] - off[pass_obj.back()] > kRegisterPassCap) pass_obj.push_back(i);
+  pass_obj.push_back(M);
+  int max_pass = 0;
+  for (size_t p = 0; p + 1 < pass_obj.size(); ++p) max_pass = std::max(max_pass, off[pass_obj[p + 1]] - off[pass_obj[p]]);
+  DeviceGuard dg(c->device);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const size_t npix = (size_t)H * W;
+  // every workspace is sized for the largest pass here, so no pass bumps the graph epoch
+  FP_TRY(ensure_capacity(c, max_pass));
+  FP_TRY(ensure_tail(c, total));
+  FP_TRY(prepare_frame(c, K, H, W, true));
+  FP_TRY(alloc_frame_staging(c, npix));
+  FP_TRY(dev_alloc(c->epoch, c->mesh_of, (size_t)max_pass * sizeof(int)));
+  FP_TRY(dev_alloc(c->epoch, c->seg_off, (size_t)(M + 1) * sizeof(int)));
+  FP_TRY(dev_alloc(c->epoch, c->reg_feats, (size_t)total * 512 * sizeof(float)));
+  FP_TRY(dev_alloc(c->epoch, c->mask_buf, (size_t)M * npix));
+  FP_TRY(dev_alloc(c->epoch, c->mask_stats, (size_t)M * 6 * sizeof(unsigned int)));
+  FP_TRY(dev_alloc(c->epoch, c->tail_counter, std::max<size_t>(16, (size_t)M * sizeof(unsigned int)), /*zero=*/true));
+  // pinned staging (never read by a captured graph): the copies below leave as soon as they are enqueued
+  if (c->stage_masks_n < (size_t)M * npix) {
+    if (c->stage_masks) cudaFreeHost(c->stage_masks);
+    c->stage_masks = nullptr;
+    c->stage_masks_n = 0;
+    FP_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&c->stage_masks), (size_t)M * npix));
+    c->stage_masks_n = (size_t)M * npix;
+  }
+  if (c->stage_ints_n < (size_t)(M + 1 + total)) {
+    if (c->stage_ints) cudaFreeHost(c->stage_ints);
+    c->stage_ints = nullptr;
+    c->stage_ints_n = 0;
+    FP_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&c->stage_ints), (size_t)(M + 1 + total) * sizeof(int)));
+    c->stage_ints_n = (size_t)(M + 1 + total);
+  }
+  int* slot_of = c->stage_ints + M + 1;  // slot id of every hypothesis
+  memcpy(c->stage_ints, off.data(), (size_t)(M + 1) * sizeof(int));
+  for (int i = 0; i < M; ++i) std::fill(slot_of + off[i], slot_of + off[i + 1], slots_host[i]);
+  memcpy(c->stage_masks, masks_host, (size_t)M * npix);
+  FP_CUDA_OK(cudaMemcpyAsync(c->seg_off.p, c->stage_ints, (size_t)(M + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
+  FP_CUDA_OK(cudaMemcpyAsync(c->mask_buf.p, c->stage_masks, (size_t)M * npix, cudaMemcpyHostToDevice, st));
+  FP_TRY(upload_staged_frame(c, rgb_host, depth_host, npix, st));
+  // estimater.py:173-174, :214 once for every object: erode + bilateral, depth2xyzmap(zfar = inf)
+  c->has_frame = false;
+  FP_TRY(set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->rgb_raw.p), reinterpret_cast<const float*>(c->depth_raw.p),
+                            FP_FRAME_FILTER_DEPTH, INFINITY, st));
+  c->has_frame = true;
+  // estimater.py:137-156, :203-209 for every object in one launch pair; the start poses go to poses_out_dev and are
+  // replaced pass by pass with the refined ones
+  const int* seg = reinterpret_cast<const int*>(c->seg_off.p);
+  FP_TRY(start_poses_launch(c->depth_cur, reinterpret_cast<const unsigned char*>(c->mask_buf.p), H, W, c->K[0], c->K[4], c->K[2],
+                            c->K[5], rot_grids_dev, total, M, seg, reinterpret_cast<unsigned int*>(c->mask_stats.p),
+                            poses_out_dev, info_out_dev, st));
+  float* pa = reinterpret_cast<float*>(c->poses_a.p);
+  float* pb = reinterpret_cast<float*>(c->poses_b.p);
+  float* ps = reinterpret_cast<float*>(c->pose_stage.p);
+  float* fb = reinterpret_cast<float*>(c->feat_buf.p);
+  const int* mesh_of = reinterpret_cast<const int*>(c->mesh_of.p);
+  const float* fin = (iterations % 2 == 0) ? pa : pb;
+  for (size_t p = 0; p + 1 < pass_obj.size(); ++p) {
+    const int row0 = off[pass_obj[p]], n = off[pass_obj[p + 1]] - row0;
+    // the pass's slot ids and start poses go to fixed context buffers and its outputs are copied out after the replays:
+    // the graphs hold no per-pass address and are keyed on (kind, n, iterations) alone
+    FP_CUDA_OK(cudaMemcpyAsync(c->mesh_of.p, slot_of + row0, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+    FP_CUDA_OK(cudaMemcpyAsync(pa, poses_out_dev + (size_t)row0 * 16, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
+    FP_TRY(run_graphed(c, 4, n, iterations, st, [&](cudaStream_t s2) -> int { return refine_body(c, n, iterations, s2, mesh_of); }));
+    FP_CUDA_OK(cudaMemcpyAsync(poses_out_dev + (size_t)row0 * 16, fin, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
+    FP_CUDA_OK(cudaMemcpyAsync(ps, fin, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
+    FP_TRY(run_graphed(c, 5, n, 0, st, [&](cudaStream_t s2) -> int {
+      FP_TRY(make_crops(c, ps, n, 1, nullptr, nullptr, nullptr, s2, mesh_of));
+      FP_TRY(run_encoder(c, c->net[1], reinterpret_cast<const __half*>(c->crops.p), n, s2));
+      return run_score_feats(c, c->net[1], n, fb, s2);
+    }));
+    FP_CUDA_OK(cudaMemcpyAsync(reinterpret_cast<float*>(c->reg_feats.p) + (size_t)row0 * 512, fb, (size_t)n * 2048,
+                               cudaMemcpyDeviceToDevice, st));
+  }
+  // score_network.py:84-88 per object: one tail launch, each object's hypotheses attending only to each other
+  const Net& net = c->net[1];
+  ScoreTailParams tp;
+  tp.feats = reinterpret_cast<const float*>(c->reg_feats.p);
+  tp.L = total;
+  tp.w_in = net.f("cross.in_w");
+  tp.b_in = net.f("cross.in_b");
+  tp.fold_v = reinterpret_cast<const float*>(c->fold_v.p);
+  tp.fold_c = c->fold_c;
+  tp.offset = 100.f;
+  tp.qkv = reinterpret_cast<float*>(c->tail_qkv.p);
+  tp.scores = scores_out_dev;
+  tp.best = best_out_dev;
+  tp.counter = reinterpret_cast<unsigned int*>(c->tail_counter.p);
+  tp.seg = seg;
+  tp.n_seg = M;
+  tp.seg_max = seg_max;
+  FP_TRY(score_tail_launch(tp, st));
+  FP_CUDA_OK(cudaStreamSynchronize(st));
   return 0;
   FP_API_END
 }

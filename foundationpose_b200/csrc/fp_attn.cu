@@ -8,7 +8,7 @@
 //                        hypotheses at once).
 //   cross_attn_score_kernel  scorer: attention across the L pose hypotheses (score_network.py:85-86), out_proj and
 //                        Linear(512,1) folded into one 512-vector, first-max argmax by the last CTA (score_network.py:87-88,
-//                        predict_score.py:196, estimater.py:226).
+//                        predict_score.py:196, estimater.py:226); several objects' hypotheses as independent segments.
 //   pose_update_kernel   predict_pose_refine.py:195-231 + Utils.py:848-855 + pytorch3d so3_exp_map.
 #include "fp_attn.cuh"
 
@@ -303,27 +303,45 @@ __global__ void __launch_bounds__(256) rowwise_linear_kernel(const float* __rest
   }
 }
 
-// One CTA per query hypothesis, one warp per head: attention across the L hypotheses (score_network.py:85-86), then
-// out_proj and Linear(512, 1) (score_network.py:87-88) folded into ONE 512-vector: score = v . attn + c with
-// v = W_out^T w_lin and c = w_lin . b_out + b_lin (both prepared in fp64 by fp_load_network).  The last CTA to
-// finish takes the arg-max (first index of the maximum = ids[0] of estimater.py:226) — two launches for the whole tail.
+// One CTA per query hypothesis, one warp per head: attention across the hypotheses of the query's segment
+// (score_network.py:85-86: one register() call's hypotheses), then out_proj and Linear(512, 1) (score_network.py:87-88)
+// folded into ONE 512-vector: score = v . attn + c with v = W_out^T w_lin and c = w_lin . b_out + b_lin (both prepared
+// in fp64 by fp_load_network).  The last CTA of each segment to finish takes that segment's arg-max (first index of the
+// maximum, relative to the segment = ids[0] of estimater.py:226) — two launches for the whole tail.
+// Segment g is rows [seg[g], seg[g + 1]) (seg = null: one segment of all L rows).  Every loop runs over
+// segment-relative indices (shared scores, the lanes' stride through the exponentials, the key / value order), so a
+// segment's scores are bit-identical to a launch over that segment's rows alone.
 __global__ void __launch_bounds__(128) cross_attn_score_kernel(const float* __restrict__ qkv, const float* __restrict__ fold_v,
                                                                float fold_c, float offset, float* __restrict__ scores,
                                                                int* __restrict__ best, unsigned int* __restrict__ counter,
-                                                               int L, float scale) {
-  extern __shared__ float sc[];  // [4][L]
+                                                               const int* __restrict__ seg, int n_seg, int seg_max, int L,
+                                                               float scale) {
+  extern __shared__ float sc[];  // [4][seg_max]
   __shared__ float part[4];
   __shared__ unsigned int ticket;
   const int q = blockIdx.x, h = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  float* s = sc + h * L;
+  int g = 0, k0 = 0, n = L;
+  if (seg) {  // the segment holding q: seg[g] <= q < seg[g + 1]
+    int lo = 0, hi = n_seg - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (seg[mid] <= q) lo = mid;
+      else hi = mid - 1;
+    }
+    g = lo;
+    k0 = seg[g];
+    n = seg[g + 1] - k0;
+  }
+  const float* keys = qkv + (size_t)k0 * 1536;
+  float* s = sc + h * seg_max;
   const float* qv = qkv + (size_t)q * 1536 + h * 128;
   float qr[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) qr[i] = qv[lane * 4 + i];
   float mx = -INFINITY;
 #pragma unroll 6  // independent key rows: keep several L2 loads in flight (the loop is latency-bound)
-  for (int k = 0; k < L; ++k) {
-    const float4 kv = __ldg(reinterpret_cast<const float4*>(qkv + (size_t)k * 1536 + 512 + h * 128 + lane * 4));
+  for (int k = 0; k < n; ++k) {
+    const float4 kv = __ldg(reinterpret_cast<const float4*>(keys + (size_t)k * 1536 + 512 + h * 128 + lane * 4));
     float d = qr[0] * kv.x + qr[1] * kv.y + qr[2] * kv.z + qr[3] * kv.w;
     d = warp_sum(d) * scale;
     if (lane == 0) s[k] = d;
@@ -331,7 +349,7 @@ __global__ void __launch_bounds__(128) cross_attn_score_kernel(const float* __re
   }
   __syncwarp();
   float sum = 0.f;
-  for (int k = lane; k < L; k += 32) {
+  for (int k = lane; k < n; k += 32) {
     const float e = expf(s[k] - mx);
     s[k] = e;
     sum += e;
@@ -340,9 +358,9 @@ __global__ void __launch_bounds__(128) cross_attn_score_kernel(const float* __re
   __syncwarp();
   float o[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll 6
-  for (int k = 0; k < L; ++k) {
+  for (int k = 0; k < n; ++k) {
     const float pk = s[k];
-    const float4 vv = __ldg(reinterpret_cast<const float4*>(qkv + (size_t)k * 1536 + 1024 + h * 128 + lane * 4));
+    const float4 vv = __ldg(reinterpret_cast<const float4*>(keys + (size_t)k * 1536 + 1024 + h * 128 + lane * 4));
     o[0] += pk * vv.x;
     o[1] += pk * vv.y;
     o[2] += pk * vv.z;
@@ -357,18 +375,18 @@ __global__ void __launch_bounds__(128) cross_attn_score_kernel(const float* __re
   if (threadIdx.x == 0) {
     scores[q] = (((part[0] + part[1]) + part[2]) + part[3]) + fold_c + offset;
     __threadfence();
-    ticket = atomicAdd(counter, 1u);
+    ticket = atomicAdd(counter + g, 1u);
   }
   __syncthreads();
-  if (ticket != (unsigned)(L - 1)) return;
-  // last CTA: every score is visible; first index of the maximum
+  if (ticket != (unsigned)(n - 1)) return;
+  // last CTA of the segment: every score of it is visible; first index of the maximum
   __threadfence();
   __shared__ float sv[128];
   __shared__ int si[128];
   float bv = -INFINITY;
   int bi = 0x7fffffff;
-  for (int l = threadIdx.x; l < L; l += 128) {
-    const float v = __ldcg(scores + l);
+  for (int l = threadIdx.x; l < n; l += 128) {
+    const float v = __ldcg(scores + k0 + l);
     if (v > bv || (v == bv && l < bi)) {
       bv = v;
       bi = l;
@@ -389,8 +407,8 @@ __global__ void __launch_bounds__(128) cross_attn_score_kernel(const float* __re
     __syncthreads();
   }
   if (threadIdx.x == 0) {
-    if (best) *best = si[0];
-    *counter = 0u;  // ready for the next launch (graph replays included)
+    if (best) best[g] = si[0];
+    counter[g] = 0u;  // ready for the next launch (graph replays included)
   }
 }
 
@@ -403,16 +421,18 @@ int rowwise_linear_launch(const float* x, const float* w, const float* bias, flo
 
 int score_tail_launch(const ScoreTailParams& p, cudaStream_t stream) {
   if (p.L == 0) return 0;
-  FP_REQUIRE(p.L <= 4096, "score tail: L=%d too large", p.L);
-  const size_t smem = 4 * (size_t)p.L * sizeof(float);
+  const int seg_max = p.seg ? p.seg_max : p.L;
+  FP_REQUIRE(seg_max <= 4096, "score tail: %d hypotheses in one segment, at most 4096", seg_max);
+  FP_REQUIRE(!p.seg || (p.n_seg >= 1 && seg_max >= 1), "score tail: bad segments");
+  const size_t smem = 4 * (size_t)seg_max * sizeof(float);
   static std::atomic<unsigned long long> attr_mask{0};  // per device: the attribute is device state
   if (!device_bit_test(attr_mask)) {
     FP_CUDA_OK(cudaFuncSetAttribute(cross_attn_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 4096 * 4));
     device_bit_set(attr_mask);
   }
   FP_TRY_RC(rowwise_linear_launch(p.feats, p.w_in, p.b_in, p.qkv, p.L, 1536, stream));
-  cross_attn_score_kernel<<<p.L, 128, smem, stream>>>(p.qkv, p.fold_v, p.fold_c, p.offset, p.scores, p.best, p.counter, p.L,
-                                                      0.08838834764831845f);
+  cross_attn_score_kernel<<<p.L, 128, smem, stream>>>(p.qkv, p.fold_v, p.fold_c, p.offset, p.scores, p.best, p.counter, p.seg,
+                                                      p.n_seg, seg_max, p.L, 0.08838834764831845f);
   note_launches(1);
   FP_CUDA_OK(cudaGetLastError());
   return 0;

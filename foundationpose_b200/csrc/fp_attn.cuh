@@ -39,8 +39,15 @@ struct ScoreTailParams {
   float offset;         // +100 of predict_score.py:207
   float* qkv;           // workspace [L][1536]
   float* scores;        // out [L]
-  int* best;            // out, optional
-  unsigned int* counter;  // device word, zero between launches (the last CTA takes the arg-max and resets it)
+  int* best;            // out, optional: [n_seg] (one segment: [1]) arg-max of each segment, relative to its start
+  unsigned int* counter;  // device words [n_seg], zero between launches (each segment's last CTA takes its arg-max and
+                          // resets its word)
+  // segments: hypotheses of different objects attend only within their own object's rows.  seg: DEVICE [n_seg + 1]
+  // row offsets (seg[0] = 0, seg[n_seg] = L, no empty segment), seg_max: the longest segment (<= 4096).
+  // seg = null: one segment of all L rows.
+  const int* seg = nullptr;
+  int n_seg = 1;
+  int seg_max = 0;
 };
 int score_tail_launch(const ScoreTailParams& p, cudaStream_t stream);
 

@@ -216,12 +216,15 @@ __device__ unsigned int radix_select(const float* __restrict__ depth, const unsi
   return prefix;
 }
 
-// pass 1 (grid-wide): mask bounding box and pixel counts.  All six statistics are max / sum reductions over values
-// that start at 0 (the box minima are stored mirrored), so one 24-byte memset initialises them.
+// pass 1 (grid-wide, one grid row per object): mask bounding box and pixel counts.  All six statistics are max / sum
+// reductions over values that start at 0 (the box minima are stored mirrored), so one memset of 6 words per object
+// initialises them.  Object m reads masks[m] ([H][W]) and writes stats[6 m, 6 m + 6).
 __global__ void __launch_bounds__(256) mask_stats_kernel(const float* __restrict__ depth,
-                                                         const unsigned char* __restrict__ mask, int H, int W,
+                                                         const unsigned char* __restrict__ masks, int H, int W,
                                                          unsigned int* __restrict__ stats) {
   const int npix = H * W;
+  const unsigned char* mask = masks + (size_t)blockIdx.y * npix;
+  stats += 6 * blockIdx.y;
   unsigned int mu0 = 0, u1 = 0, mv0 = 0, v1 = 0, n_mask = 0, n_valid = 0;  // mu0 = W - 1 - umin, mv0 = H - 1 - vmin
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < npix; i += gridDim.x * blockDim.x) {
     if (mask[i]) {
@@ -253,15 +256,26 @@ __global__ void __launch_bounds__(256) mask_stats_kernel(const float* __restrict
   }
 }
 
-// pass 2 (one CTA): exact median over the bounding box, translation, start poses
+// pass 2 (one CTA per object): exact median over the object's bounding box, translation, start poses.  Object m owns
+// rows [off[m], off[m + 1]) of the concatenated rotation grids and start poses (off = null: one object, rows [0, N)),
+// and writes info[4 m, 4 m + 4).
 __global__ void __launch_bounds__(1024) start_poses_kernel(const float* __restrict__ depth,
-                                                           const unsigned char* __restrict__ mask, int H, int W, float fx,
+                                                           const unsigned char* __restrict__ masks, int H, int W, float fx,
                                                            float fy, float cx, float cy, const float* __restrict__ rot_grid,
-                                                           int N, const unsigned int* __restrict__ stats,
+                                                           int N, const int* __restrict__ off,
+                                                           const unsigned int* __restrict__ stats,
                                                            float* __restrict__ poses_out, float* __restrict__ info) {
   __shared__ unsigned int hist[256];
   __shared__ unsigned int sh[2];
   __shared__ float tvec[3];
+  const int m = blockIdx.x;
+  const unsigned char* mask = masks + (size_t)m * H * W;
+  stats += 6 * m;
+  info += 4 * m;
+  const int row0 = off ? off[m] : 0;
+  const int n = off ? off[m + 1] - row0 : N;
+  rot_grid += (size_t)row0 * 16;
+  poses_out += (size_t)row0 * 16;
   const unsigned int nm = stats[4], nv = stats[5];
   // umin, umax, vmin, vmax
   const int bb[4] = {W - (int)stats[0], (int)stats[1] - 1, H - (int)stats[2], (int)stats[3] - 1};
@@ -285,7 +299,7 @@ __global__ void __launch_bounds__(1024) start_poses_kernel(const float* __restri
     info[0] = tvec[0]; info[1] = tvec[1]; info[2] = tvec[2]; info[3] = (float)nv;
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < N * 16; i += blockDim.x) {
+  for (int i = threadIdx.x; i < n * 16; i += blockDim.x) {
     const int e = i & 15;
     float v = rot_grid[i];
     if (e == 3) v = tvec[0];
@@ -295,12 +309,13 @@ __global__ void __launch_bounds__(1024) start_poses_kernel(const float* __restri
   }
 }
 
-int start_poses_launch(const float* depth, const unsigned char* mask, int H, int W, float fx, float fy, float cx, float cy,
-                       const float* rot_grid, int N, unsigned int* stats /*6 words of device scratch*/, float* poses_out,
+int start_poses_launch(const float* depth, const unsigned char* masks, int H, int W, float fx, float fy, float cx, float cy,
+                       const float* rot_grid, int N, int M, const int* off, unsigned int* stats, float* poses_out,
                        float* info, cudaStream_t stream) {
-  FP_CUDA_OK(cudaMemsetAsync(stats, 0, 6 * sizeof(unsigned int), stream));
-  mask_stats_kernel<<<num_sms(), 256, 0, stream>>>(depth, mask, H, W, stats);
-  start_poses_kernel<<<1, 1024, 0, stream>>>(depth, mask, H, W, fx, fy, cx, cy, rot_grid, N, stats, poses_out, info);
+  FP_REQUIRE(M >= 1 && M <= 65535 && (off || M == 1), "start_poses: bad object count %d", M);
+  FP_CUDA_OK(cudaMemsetAsync(stats, 0, (size_t)M * 6 * sizeof(unsigned int), stream));
+  mask_stats_kernel<<<dim3(num_sms(), M), 256, 0, stream>>>(depth, masks, H, W, stats);
+  start_poses_kernel<<<M, 1024, 0, stream>>>(depth, masks, H, W, fx, fy, cx, cy, rot_grid, N, off, stats, poses_out, info);
   note_launches(2);
   FP_CUDA_OK(cudaGetLastError());
   return 0;

@@ -10,7 +10,10 @@ int bilateral_depth_launch(const float* depth, float* out, int H, int W, int rad
 // erode(2) -> bilateral(2) -> back-projection (invalid: z < 0.001 or z > zfar_xyz) + rgb -> rgba, one launch
 int frame_prep_launch(const unsigned char* rgb, const float* depth, uchar4* rgba, float* depth_out, float4* xyz, int H, int W,
                       float fx, float fy, float cx, float cy, float zfar_xyz, cudaStream_t stream);
-int start_poses_launch(const float* depth, const unsigned char* mask, int H, int W, float fx, float fy, float cx, float cy,
-                       const float* rot_grid, int N, unsigned int* stats, float* poses_out, float* info,
-                       cudaStream_t stream);
+// guess_translation + start poses of M objects in two launches: masks [M][H][W]; off [M + 1] device row offsets of
+// each object in rot_grid / poses_out ([off[M]][16]; null when M = 1: rows [0, N)); stats: 6 M words of device
+// scratch; info [M][4] = {tx, ty, tz, n_valid}
+int start_poses_launch(const float* depth, const unsigned char* masks, int H, int W, float fx, float fy, float cx, float cy,
+                       const float* rot_grid, int N, int M, const int* off, unsigned int* stats, float* poses_out,
+                       float* info, cudaStream_t stream);
 }  // namespace fp

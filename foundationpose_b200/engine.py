@@ -30,6 +30,8 @@ def _proto():
     lib.fp_crop_stats.argtypes = [vp, vp, i, i, C.POINTER(i), vp]
     lib.fp_track.argtypes = [vp, vp, vp, C.POINTER(f), i, i, vp, i, vp, vp, vp]
     lib.fp_track_objects.argtypes = [vp, vp, vp, C.POINTER(f), i, i, i, C.POINTER(i), vp, i, vp, vp, vp]
+    lib.fp_register_objects.argtypes = [vp, vp, vp, C.POINTER(f), i, i, i, C.POINTER(i), C.POINTER(i), vp, vp, i, vp, vp, vp,
+                                        vp, vp]
     lib.fp_graph_captures.argtypes = [vp]
     lib.fp_graph_captures.restype = C.c_ulonglong
     lib.fp_load_network.argtypes = [vp, i, C.POINTER(_FpTensor), i]
@@ -50,7 +52,7 @@ def _proto():
     lib.fp_op_tokens.argtypes = [vp, i, vp, i, vp, vp]
     lib.fp_op_depth_filter.argtypes = [vp, vp, i, i, i, vp]
     lib.fp_op_pose_update.argtypes = [vp, vp, vp, vp, i, f, f, vp]
-    for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh",
+    for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_register_objects", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh",
                  "fp_set_mesh_slot", "fp_set_frame",
                  "fp_get_depth", "fp_make_crops", "fp_start_poses", "fp_refine", "fp_score", "fp_score_features", "fp_score_tail",
                  "fp_register", "fp_op_refine_net", "fp_op_score_feats", "fp_op_tokens", "fp_op_depth_filter",
@@ -261,6 +263,39 @@ class Engine:
                                         C.c_void_p(host.ctypes.data), _stream()), "fp_track_objects")
         self.frame_hw = (H, W)
         return out, host
+
+    def register_objects(self, rgb, depth, K, masks, rot_grids, slots, iterations):
+        """fp_register_objects: the register() hot path for M objects of one frame in one call, object i rendering the mesh
+        in slot slots[i].  rgb uint8 (H,W,3) / depth float32 (H,W) / masks (M,H,W) (nonzero = object) HOST arrays;
+        rot_grids: M CUDA float32 (N_i,4,4) rotation grids.  Returns CUDA tensors: poses (sum N_i,4,4) refined, object-major
+        and unranked; scores (sum N_i,); best (M,) int32, each object's first arg-max relative to its own rows; info (M,4)
+        = (tx, ty, tz, n_valid) per object."""
+        rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
+        depth = np.ascontiguousarray(depth, dtype=np.float32)
+        H, W = depth.shape
+        masks = np.ascontiguousarray(masks)
+        M = len(masks)
+        if masks.shape != (M, H, W):
+            raise ValueError(f"register_objects: masks must be (M, {H}, {W}), got {masks.shape}")
+        masks = np.ascontiguousarray(masks > 0, dtype=np.uint8)  # the reference tests `mask > 0` (estimater.py:138, :183)
+        slots = [int(s) for s in slots]
+        rot_grids = [g.reshape(-1, 4, 4) for g in rot_grids]
+        if len(slots) != M or len(rot_grids) != M:
+            raise ValueError(f"register_objects: {M} masks, {len(slots)} slots and {len(rot_grids)} rotation grids")
+        n_hyp = [len(g) for g in rot_grids]
+        grids = torch.cat(rot_grids).to(device="cuda", dtype=torch.float32).contiguous()
+        total = len(grids)
+        Kf = (C.c_float * 9)(*[float(x) for x in np.asarray(K, dtype=np.float64).reshape(-1)])
+        poses = torch.empty(total, 4, 4, dtype=torch.float32, device="cuda")
+        scores = torch.empty(total, dtype=torch.float32, device="cuda")
+        best = torch.empty(M, dtype=torch.int32, device="cuda")
+        info = torch.empty(M, 4, dtype=torch.float32, device="cuda")
+        _lib.check(lib.fp_register_objects(self._h, C.c_void_p(rgb.ctypes.data), C.c_void_p(depth.ctypes.data), Kf, H, W, M,
+                                           (C.c_int * M)(*slots), (C.c_int * M)(*n_hyp), C.c_void_p(masks.ctypes.data), _p(grids),
+                                           int(iterations), _p(poses), _p(scores), _p(best), _p(info), _stream()),
+                   "fp_register_objects")
+        self.frame_hw = (H, W)
+        return poses, scores, best, info
 
     def set_frame(self, rgb, depth, K, filter_depth=True, zfar=float("inf")):
         """rgb uint8 (H,W,3), depth float32 (H,W): numpy / CPU tensors (pinned for async H2D) or CUDA tensors."""

@@ -348,9 +348,10 @@ def _uncentre(pose_host, model_center):
     return out.astype(np.float32)
 
 
-def _object_slot(est):
+def _object_slot(est, caller="track_objects"):
     """The slot of `est`'s mesh in its engine (1..MAX_MESHES-1; slot 0 stays with the single-object calls): assigned at
-    first use, reloaded when reset_object() replaced the estimator's mesh_tensors."""
+    first use, reloaded when reset_object() replaced the estimator's mesh_tensors.  Shared by track_objects and
+    register_objects, so registering and then tracking the same estimators uploads no mesh."""
     e = est.engine
     owners = e.__dict__.setdefault("_object_slots", {})  # slot -> weakref to the estimator that owns it
     slot = getattr(est, "_object_slot", None)
@@ -359,7 +360,7 @@ def _object_slot(est):
             del owners[s]  # the estimator was garbage-collected
         free = [s for s in range(1, MAX_MESHES) if s not in owners]
         if not free:
-            raise ValueError(f"track_objects: an engine holds at most {MAX_MESHES - 1} object meshes")
+            raise ValueError(f"{caller}: an engine holds at most {MAX_MESHES - 1} object meshes")
         slot = free[0]
         owners[slot] = weakref.ref(est)
         est._object_slot, est._object_slot_src = slot, None
@@ -369,6 +370,18 @@ def _object_slot(est):
                    vertex_colors=mt.get("vcolor"), slot=slot)
         est._object_slot_src = mt
     return slot
+
+
+def _shared_engine_of(estimators, caller):
+    """The one engine all `estimators` share; refuses mixed engines, repeated estimators and more objects than slots."""
+    e = estimators[0].engine
+    if any(est.engine is not e for est in estimators):
+        raise ValueError(f"{caller}: the estimators must share one engine")
+    if len({id(est) for est in estimators}) != len(estimators):
+        raise ValueError(f"{caller}: an estimator appears more than once")
+    if len(estimators) > MAX_MESHES - 1:
+        raise ValueError(f"{caller}: at most {MAX_MESHES - 1} objects per engine, got {len(estimators)}")
+    return e
 
 
 def track_objects(estimators, rgb, depth, K, iteration=2):
@@ -384,13 +397,7 @@ def track_objects(estimators, rgb, depth, K, iteration=2):
         return []
     if torch.is_tensor(rgb) or torch.is_tensor(depth):
         raise TypeError("track_objects takes host frames (numpy); for device-resident frames call track_one per object")
-    e = estimators[0].engine
-    if any(est.engine is not e for est in estimators):
-        raise ValueError("track_objects: the estimators must share one engine")
-    if len({id(est) for est in estimators}) != len(estimators):
-        raise ValueError("track_objects: an estimator appears more than once")
-    if len(estimators) > MAX_MESHES - 1:
-        raise ValueError(f"track_objects: at most {MAX_MESHES - 1} objects per engine, got {len(estimators)}")
+    e = _shared_engine_of(estimators, "track_objects")
     if any(est.pose_last is None for est in estimators):
         logging.info("Please init pose by register first")
         raise RuntimeError
@@ -403,3 +410,73 @@ def track_objects(estimators, rgb, depth, K, iteration=2):
         est.refiner.last_trans_update = est.refiner.last_rot_update = None
         out.append(_uncentre(poses_host[i], est.model_center))
     return out
+
+
+def register_objects(estimators, K, rgb, depth, ob_masks, ob_ids=None, iteration=5):
+    """`[est.register(K=K, rgb=rgb, depth=depth, ob_mask=m, ob_id=i, iteration=iteration) for ...]` bit for bit, for
+    several objects of one frame in one fp_register_objects call: the frame is uploaded and filtered once, every object's
+    start poses come from one launch, the objects' hypotheses are refined and featurised together in passes of up to 512
+    (each rendering its own mesh), and one scorer tail keeps every object's hypotheses to themselves.  Each estimator
+    uses its own rotation grid (symmetric objects bring fewer hypotheses) and ends in the state its register() call
+    would leave (pose_last, best_id, poses and scores ranked by descending score, H, W, K, ob_id, ob_mask); an object
+    with fewer than 4 valid masked depth pixels returns the identity rotation with the guessed translation and keeps
+    its previous state.  Everything comes back to the host in one read-back.
+
+    The estimators must share one engine; each keeps its mesh in the same slot track_objects uses, so tracking them
+    afterwards uploads no mesh.  Host frames and masks only (uint8 (H,W,3) rgb, float32 (H,W) depth, (H,W) masks).
+    Returns a list of (4,4) poses of the original meshes."""
+    estimators = list(estimators)
+    if not estimators:
+        return []
+    if torch.is_tensor(rgb) or torch.is_tensor(depth) or any(torch.is_tensor(m) and m.is_cuda for m in ob_masks):
+        raise TypeError("register_objects takes host frames and masks (numpy); for device-resident frames call register per object")
+    e = _shared_engine_of(estimators, "register_objects")
+    ob_masks = list(ob_masks)
+    masks = [m.numpy() if torch.is_tensor(m) else np.asarray(m) for m in ob_masks]
+    M = len(estimators)
+    if len(masks) != M:
+        raise ValueError(f"register_objects: {M} estimators but {len(masks)} masks")
+    H, W = np.shape(depth)[:2]
+    for i, m in enumerate(masks):
+        if m.shape != (H, W):
+            raise ValueError(f"register_objects: mask {i} has shape {m.shape}, the frame is {(H, W)}")
+    ob_ids = [None] * M if ob_ids is None else list(ob_ids)
+    if len(ob_ids) != M:
+        raise ValueError(f"register_objects: {M} estimators but {len(ob_ids)} ob_ids")
+    slots = [_object_slot(est, "register_objects") for est in estimators]
+    poses, scores, _, info = e.register_objects(rgb, depth, K, np.stack(masks), [est.rot_grid for est in estimators], slots,
+                                                iteration)
+    # per object, the ranking and best pose of register(): estimater.py:224-234 on that object's rows
+    ranked, rows, o = [], [], 0
+    for i, est in enumerate(estimators):
+        n = len(est.rot_grid)
+        ids = scores[o:o + n].argsort(descending=True)
+        p, s = poses[o:o + n][ids], scores[o:o + n][ids]
+        best_pose = p[0] @ est.get_tf_to_centered_mesh()
+        ranked.append((ids, p, s))
+        rows.append(torch.cat([info[i], best_pose.reshape(-1)]))
+        o += n
+    out = torch.stack(rows).cpu().numpy()  # the one host synchronisation: (tx, ty, tz, n_valid) and the best pose per object
+    result = []
+    for i, est in enumerate(estimators):
+        early = out[i, 3] < 4
+        est.refiner.last_trans_update = est.refiner.last_rot_update = None
+        if not (early and getattr(est, "strict_early_out", False)):  # register()'s strict path returns before recording the frame
+            est.H, est.W = H, W
+            est.K = K
+            est.ob_id = ob_ids[i]
+            est.ob_mask = ob_masks[i]
+        if early:
+            # estimater.py:183-189: too few valid pixels -> identity rotation, guessed translation, state untouched
+            logging.info("valid too small, return")
+            pose = np.eye(4)
+            pose[:3, 3] = out[i, :3]
+            result.append(pose)
+            continue
+        ids, p, s = ranked[i]
+        est.pose_last = p[0]
+        est.best_id = ids[0]
+        est.poses = p
+        est.scores = s
+        result.append(out[i, 4:].reshape(4, 4).copy())
+    return result

@@ -195,6 +195,26 @@ int fp_track(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host
 int fp_track_objects(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
                      int M, const int* slots_host, const float* poses_in_dev, int iterations, float* poses_out_dev,
                      float* poses_out_host, void* stream);
+/* FoundationPose.register (estimater.py:159-240) applied to M objects of the same frame in one call; object i gives
+ * exactly what fp_set_frame + fp_start_poses + fp_refine + fp_score give for that object alone, bit for bit.
+ *   1. Checks every argument before anything is enqueued: slots_host HOST [M] loaded slot ids (one slot may appear
+ *      more than once: two instances of one object), n_hyp_host HOST [M] hypotheses per object (1..4096), both
+ *      networks loaded.
+ *   2. One pinned-staged upload of the frame (HOST rgb uint8 [H][W][3], depth float32 [H][W]) and of masks_host
+ *      (HOST uint8 [M][H][W], nonzero = object), one erode_depth + bilateral_filter_depth + depth2xyzmap(zfar = inf).
+ *   3. guess_translation + start poses of every object in one launch pair: rot_grids_dev DEVICE [sum N][16], object i's
+ *      n_hyp_host[i] rotations after object i - 1's.
+ *   4. Refines (`iterations` passes) and featurises whole objects in passes of at most 512 hypotheses (an object above
+ *      that alone); hypothesis rows render their own object's slot.
+ *   5. One cross-hypothesis scorer tail in which every object's hypotheses attend only to each other.
+ * Outputs (DEVICE): poses_out_dev [sum N][16] refined poses, object-major, in grid order (not ranked; with iterations = 0
+ * the start poses); scores_out_dev [sum N]; best_out_dev [M] first index of each object's maximum, relative to the
+ * object; info_out_dev [M][4] = {tx, ty, tz, n_valid} as fp_start_poses.  An object with fewer than 4 valid masked
+ * pixels still runs; the caller discards its results (estimater.py:183-189).  Synchronises. */
+int fp_register_objects(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
+                        int M, const int* slots_host, const int* n_hyp_host, const unsigned char* masks_host,
+                        const float* rot_grids_dev, int iterations, float* poses_out_dev, float* scores_out_dev,
+                        int* best_out_dev, float* info_out_dev, void* stream);
 /* Number of CUDA graphs this context has captured so far (test hook: a replay captures nothing). */
 unsigned long long fp_graph_captures(fp_ctx* ctx);
 
