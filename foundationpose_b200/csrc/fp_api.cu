@@ -84,6 +84,7 @@ constexpr size_t kCropImg = (size_t)(S + 6) * (S + 8) * 8;  // fp16 elements per
 static inline int b_img0_of(int N) { return (N + 3) & ~3; }
 
 static_assert(kMaxMeshes == FP_MAX_MESHES, "fp_crop.cuh and fpose.h disagree on the number of mesh slots");
+static_assert(kMaxCameras == FP_MAX_CAMERAS, "fp_crop.cuh and fpose.h disagree on the number of cameras");
 
 // One mesh of the context (fp_meshlet.cu layout).  Slot 0 is the mesh of every single-object entry point.
 struct MeshSlot {
@@ -92,6 +93,15 @@ struct MeshSlot {
   float bs[4] = {0.f, 0.f, 0.f, 0.f};
   bool has_tex = false, loaded = false;
   float diameter = 0.f;
+};
+
+// Frame buffers of cameras 1.. of fp_track_cameras (camera 0 is the context's frame), sized for the largest frame seen,
+// and the pinned staging of their uploads.
+struct CameraBufs {
+  DevBuf rgb_raw, depth_raw, rgba, depth, xyz;
+  void* stage_rgb = nullptr;
+  void* stage_depth = nullptr;
+  size_t stage_npix = 0;
 };
 
 }  // namespace fp
@@ -104,7 +114,7 @@ struct fp_ctx {
   // meshes, and their device table (MeshSlotDev [FP_MAX_MESHES]) that kernels index by slot.  Captured graphs hold only
   // the table's address: loading a slot rewrites its entry in place and needs no new capture.
   fp::MeshSlot mesh[fp::kMaxMeshes];
-  fp::DevBuf mesh_table, mesh_of;  // mesh_of: slot id of every object of fp_track_objects
+  fp::DevBuf mesh_table, mesh_of;  // mesh_of: slot id of every hypothesis of an fp_register_objects pass
   float rot_normalizer = 0.3490658503988659f;
   float crop_ratio[2] = {1.2f, 1.2f};  // per predictor: each reads its own config.yml (predict_pose_refine.py:117, predict_score.py:137)
   // frame
@@ -120,13 +130,16 @@ struct fp_ctx {
   int tail_cap = 0;
   float fold_c = 0.f;      // linear.weight . out_proj.bias + linear.bias (by-value kernel parameter)
   fp::DevBuf fold_v, tail_counter;  // out_proj^T linear.weight [512]; arg-max ticket
-  // CUDA graphs of the launch-bound inner loops, keyed by (kind, N, iterations)
+  // CUDA graphs of the launch-bound inner loops, keyed by (kind, N, iterations, cameras).  K / H / W: the frame
+  // geometry a graph that passes it by value was captured with
   struct GraphEntry {
     cudaGraphExec_t exec = nullptr;
     unsigned long long epoch = 0;
+    float K[9] = {0};
+    int H = 0, W = 0;
   };
-  std::map<std::tuple<int, int, int>, GraphEntry> graphs;
-  std::map<std::tuple<int, int, int>, int> graph_nodes;
+  std::map<std::tuple<int, int, int, int>, GraphEntry> graphs;
+  std::map<std::tuple<int, int, int, int>, int> graph_nodes;
   cudaStream_t cap_stream = nullptr;
   // the refiner's two decoder heads are independent after the shared attention core: at small batches
   // (one linear layer = 1-2 waves of tiles) the second head runs on `side_stream` so that its kernels fill
@@ -155,6 +168,14 @@ struct fp_ctx {
   size_t stage_masks_n = 0;
   int* stage_ints = nullptr;
   size_t stage_ints_n = 0;
+  // fp_track_cameras: buffers of cameras 1..; the per-call arguments (camera table [FP_MAX_CAMERAS], slot ids [M],
+  // camera ids [M]) as one device block and its pinned staging; the frame size its frame-preparation grid covers (the
+  // largest seen)
+  fp::CameraBufs cams[fp::kMaxCameras];
+  fp::DevBuf cam_args;
+  void* stage_args = nullptr;
+  size_t stage_args_n = 0;
+  int cam_grid_h = 0, cam_grid_w = 0;
 };
 
 namespace fp {
@@ -424,9 +445,11 @@ static int write_mesh_table(fp_ctx* c) {
   return 0;
 }
 
-// mesh_of: [N] device slot ids (validated by the caller), or null = every hypothesis renders slot 0
+// mesh_of: [N] device slot ids (validated by the caller), or null = every hypothesis renders slot 0.  cams / camera_of:
+// device camera table and [N] camera ids (fp_track_cameras), or null = the context's frame
 static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg, float* win, int* stats,
-                      cudaStream_t st, const int* mesh_of = nullptr) {
+                      cudaStream_t st, const int* mesh_of = nullptr, const CameraDev* cams = nullptr,
+                      const int* camera_of = nullptr) {
   FP_REQUIRE(mesh_of || c->mesh[0].loaded, "no mesh: call fp_set_mesh first");
   FP_REQUIRE(c->has_frame, "no frame: call fp_set_frame first");
   // only launches below: this body is also what run_graphed captures (no allocation, no synchronisation)
@@ -453,6 +476,8 @@ static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg
   p.win_out = win;
   p.stats = stats;
   p.tile_override = c->crop_tile;
+  p.cams = cams;
+  p.camera_of = camera_of;
   return crop_launch(p, st);
 }
 
@@ -461,17 +486,23 @@ static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg
 // captures + instantiates, later calls replay.  Replay removes ~170 launch + 60 tensor-map-encode host
 // calls per register(), which is what bounds track_one() and small per-GPU shards.  The body never allocates:
 // callers size every workspace first, so a capture after an epoch bump (new mesh, new N) is safe.
+// frame_by_value: the body passes the context's K / H / W to its kernels by value (every body except fp_track_cameras',
+// which reads them from the camera table); such a graph is captured again when they differ from its capture's.  Only
+// that graph: a frame of another size or other intrinsics does not invalidate the others.
 template <class Body>
-static int run_graphed(fp_ctx* c, int kind, int N, int iters, cudaStream_t st, Body body) {
+static int run_graphed(fp_ctx* c, int kind, int N, int iters, cudaStream_t st, Body body, int cameras = 0,
+                       bool frame_by_value = true) {
   if (!c->use_graphs || g_prof_on) return body(st);
-  const auto key = std::make_tuple(kind, N, iters);
+  const auto key = std::make_tuple(kind, N, iters, cameras);
   auto it = c->graphs.find(key);
   if (it == c->graphs.end()) {
     c->graphs[key] = fp_ctx::GraphEntry();  // seen once: next call captures
     return body(st);
   }
   fp_ctx::GraphEntry& g = it->second;
-  if (g.exec == nullptr || g.epoch != c->epoch) {
+  const bool frame_moved =
+      frame_by_value && (g.H != c->H || g.W != c->W || memcmp(g.K, c->K, sizeof g.K) != 0);
+  if (g.exec == nullptr || g.epoch != c->epoch || frame_moved) {
     if (g.exec) {
       cudaGraphExecDestroy(g.exec);
       g.exec = nullptr;
@@ -509,6 +540,9 @@ static int run_graphed(fp_ctx* c, int kind, int N, int iters, cudaStream_t st, B
     cudaGraphDestroy(graph);
     FP_CUDA_OK(ie);
     g.epoch = c->epoch;
+    memcpy(g.K, c->K, sizeof g.K);
+    g.H = c->H;
+    g.W = c->W;
     c->graph_nodes[key] = (int)n_kernels;
     ++c->graph_captures;
   }
@@ -529,16 +563,20 @@ struct DeviceGuard {
   }
 };
 
+// FPOSE_FUSED_PREP=0: the frame filters as four separate launches instead of frame_prep_kernel (A/B)
+static bool fused_prep() {
+  static const bool fused = [] {
+    const char* e = getenv("FPOSE_FUSED_PREP");
+    return !(e && e[0] == '0');
+  }();
+  return fused;
+}
+
 static int set_frame_launches(fp_ctx* c, const unsigned char* rgb_dev, const float* depth_dev, int flags, float zfar,
                               cudaStream_t st) {
   const int H = c->H, W = c->W;
   const size_t npix = (size_t)H * W;
-  static int fused = -1;  // FPOSE_FUSED_PREP=0: the four separate launches (A/B)
-  if (fused < 0) {
-    const char* e = getenv("FPOSE_FUSED_PREP");
-    fused = (e && e[0] == '0') ? 0 : 1;
-  }
-  if ((flags & FP_FRAME_FILTER_DEPTH) && !fused) {
+  if ((flags & FP_FRAME_FILTER_DEPTH) && !fused_prep()) {
     FP_TRY(rgb_to_rgba_launch(rgb_dev, reinterpret_cast<uchar4*>(c->rgba.p), (int)npix, st));
     FP_TRY(erode_depth_launch(depth_dev, reinterpret_cast<float*>(c->depth_a.p), H, W, 2, 0.001f, 0.8f, 100.f, st));
     FP_TRY(bilateral_depth_launch(reinterpret_cast<const float*>(c->depth_a.p), reinterpret_cast<float*>(c->depth_b.p), H,
@@ -560,9 +598,7 @@ static int set_frame_launches(fp_ctx* c, const unsigned char* rgb_dev, const flo
   return 0;
 }
 
-// frame buffers + intrinsics; bumps the epoch when a by-value kernel parameter changes
-static int prepare_frame(fp_ctx* c, const float* K, int H, int W, bool need_raw) {
-  const size_t npix = (size_t)H * W;
+static int alloc_frame_buffers(fp_ctx* c, size_t npix, bool need_raw) {
   FP_TRY(dev_alloc(c->epoch, c->rgba, npix * 4));
   FP_TRY(dev_alloc(c->epoch, c->depth_a, npix * 4));
   FP_TRY(dev_alloc(c->epoch, c->depth_b, npix * 4));
@@ -571,23 +607,32 @@ static int prepare_frame(fp_ctx* c, const float* K, int H, int W, bool need_raw)
     FP_TRY(dev_alloc(c->epoch, c->rgb_raw, npix * 3));
     FP_TRY(dev_alloc(c->epoch, c->depth_raw, npix * 4));
   }
-  bool same = (c->H == H && c->W == W);
-  for (int i = 0; i < 9; ++i) same = same && (c->K[i] == K[i]);
-  if (!same) ++c->epoch;  // intrinsics / frame size are by-value kernel parameters
-  for (int i = 0; i < 9; ++i) c->K[i] = K[i];
-  c->H = H;
-  c->W = W;
   return 0;
 }
 
-// mesh_of: [N] device slot ids, or null = slot 0 for every hypothesis
-static int refine_body(fp_ctx* c, int N, int iterations, cudaStream_t s2, const int* mesh_of = nullptr) {
+// records K / H / W as the context's frame geometry
+static void set_frame_geometry(fp_ctx* c, const float* K, int H, int W) {
+  for (int i = 0; i < 9; ++i) c->K[i] = K[i];
+  c->H = H;
+  c->W = W;
+}
+
+// frame buffers + intrinsics (a graph that holds them by value is captured again when they change, see run_graphed)
+static int prepare_frame(fp_ctx* c, const float* K, int H, int W, bool need_raw) {
+  FP_TRY(alloc_frame_buffers(c, (size_t)H * W, need_raw));
+  set_frame_geometry(c, K, H, W);
+  return 0;
+}
+
+// mesh_of: [N] device slot ids, or null = slot 0 for every hypothesis; cams / camera_of as make_crops
+static int refine_body(fp_ctx* c, int N, int iterations, cudaStream_t s2, const int* mesh_of = nullptr,
+                       const CameraDev* cams = nullptr, const int* camera_of = nullptr) {
   float* cur = reinterpret_cast<float*>(c->poses_a.p);
   float* nxt = reinterpret_cast<float*>(c->poses_b.p);
   const float* ho = reinterpret_cast<const float*>(c->head_out.p);
   const MeshSlotDev* table = reinterpret_cast<const MeshSlotDev*>(c->mesh_table.p);
   for (int it = 0; it < iterations; ++it) {
-    FP_TRY(make_crops(c, cur, N, 0, nullptr, nullptr, nullptr, s2, mesh_of));
+    FP_TRY(make_crops(c, cur, N, 0, nullptr, nullptr, nullptr, s2, mesh_of, cams, camera_of));
     FP_TRY(run_encoder(c, c->net[0], reinterpret_cast<const __half*>(c->crops.p), N, s2));
     FP_TRY(run_refine_heads(c, c->net[0], N, s2));
     const bool last = it == iterations - 1;
@@ -615,15 +660,160 @@ static int alloc_frame_staging(fp_ctx* c, size_t npix) {
   return 0;
 }
 
-// The previous frame's graph has finished (both callers synchronise), so the staging buffers are free.  The two
+// The previous frame's graph has finished (every caller synchronises), so the staging buffers are free.  The two
 // uploads are issued as soon as their staging copy is done — the depth DMA runs under the host's rgb copy, the
-// rgb DMA under the graph launch — instead of being nodes of the graph (measured: -40 us per frame)
+// rgb DMA under the next camera's copies or the graph launch — instead of being nodes of the graph (measured: -40 us
+// per frame)
+static int upload_staged_frame(void* stage_rgb, void* stage_depth, void* rgb_dev, void* depth_dev,
+                               const unsigned char* rgb_host, const float* depth_host, size_t npix, cudaStream_t st) {
+  memcpy(stage_depth, depth_host, npix * 4);
+  FP_CUDA_OK(cudaMemcpyAsync(depth_dev, stage_depth, npix * 4, cudaMemcpyHostToDevice, st));
+  memcpy(stage_rgb, rgb_host, npix * 3);
+  FP_CUDA_OK(cudaMemcpyAsync(rgb_dev, stage_rgb, npix * 3, cudaMemcpyHostToDevice, st));
+  return 0;
+}
 static int upload_staged_frame(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, size_t npix,
                                cudaStream_t st) {
-  memcpy(c->stage_depth, depth_host, npix * 4);
-  FP_CUDA_OK(cudaMemcpyAsync(c->depth_raw.p, c->stage_depth, npix * 4, cudaMemcpyHostToDevice, st));
-  memcpy(c->stage_rgb, rgb_host, npix * 3);
-  FP_CUDA_OK(cudaMemcpyAsync(c->rgb_raw.p, c->stage_rgb, npix * 3, cudaMemcpyHostToDevice, st));
+  return upload_staged_frame(c->stage_rgb, c->stage_depth, c->rgb_raw.p, c->depth_raw.p, rgb_host, depth_host, npix, st);
+}
+
+// fp_track_cameras and fp_track_objects after validation.  Camera 0 is the context's frame (buffers, staging, K / H / W),
+// cameras 1.. have buffers of their own.
+//   by_value = false (fp_track_cameras): every camera's buffers are sized for the largest frame of the call, so a
+//     permutation of the same cameras reallocates nothing.  The camera table, the slot ids and the camera ids go to one
+//     fixed device block in one copy ahead of the launch: the graph holds that block's address, not the frames' sizes,
+//     intrinsics or buffers, and is keyed on (C, M, iterations).  One frame_prep_kernel launch filters every camera
+//     (FPOSE_FUSED_PREP=0 does not apply) and the crops take their frame from the table.
+//   by_value = true (fp_track_objects, C = 1): the context's frame as fp_track sees it; the frame filters and the crop
+//     producer take it by value (the single-camera kernel instantiations), so the graph is captured again when the
+//     frame's size or intrinsics change.  Only the slot ids are copied.
+static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
+                              const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
+                              const float* poses_in_dev, int iterations, float* poses_out_dev, float* poses_out_host,
+                              cudaStream_t st, bool by_value) {
+  size_t npix_max = 0;
+  int H_max = 0, W_max = 0;
+  for (int i = 0; i < C; ++i) {
+    npix_max = std::max(npix_max, (size_t)H[i] * W[i]);
+    H_max = std::max(H_max, H[i]);
+    W_max = std::max(W_max, W[i]);
+  }
+  FP_TRY(ensure_capacity(c, M));
+  FP_TRY(alloc_frame_buffers(c, npix_max, true));
+  FP_TRY(alloc_frame_staging(c, npix_max));
+  set_frame_geometry(c, K, H[0], W[0]);
+  if (!by_value && (H_max > c->cam_grid_h || W_max > c->cam_grid_w)) {
+    // the frame-preparation grid is a by-value launch parameter: it covers the largest frame seen, the blocks outside
+    // a smaller frame return at once
+    ++c->epoch;
+    c->cam_grid_h = std::max(c->cam_grid_h, H_max);
+    c->cam_grid_w = std::max(c->cam_grid_w, W_max);
+  }
+  for (int i = 1; i < C; ++i) {
+    CameraBufs& b = c->cams[i];
+    unsigned long long table_only = 0;  // only the camera table holds these addresses: no graph is affected
+    FP_TRY(dev_alloc(table_only, b.rgb_raw, npix_max * 3));
+    FP_TRY(dev_alloc(table_only, b.depth_raw, npix_max * 4));
+    FP_TRY(dev_alloc(table_only, b.rgba, npix_max * 4));
+    FP_TRY(dev_alloc(table_only, b.depth, npix_max * 4));
+    FP_TRY(dev_alloc(table_only, b.xyz, npix_max * 16));
+    if (b.stage_npix < npix_max) {
+      if (b.stage_rgb) cudaFreeHost(b.stage_rgb);
+      if (b.stage_depth) cudaFreeHost(b.stage_depth);
+      b.stage_rgb = b.stage_depth = nullptr;
+      b.stage_npix = 0;
+      FP_CUDA_OK(cudaMallocHost(&b.stage_rgb, npix_max * 3));
+      FP_CUDA_OK(cudaMallocHost(&b.stage_depth, npix_max * 4));
+      b.stage_npix = npix_max;
+    }
+  }
+  const size_t table_bytes = sizeof(CameraDev) * kMaxCameras;
+  const size_t args_bytes = table_bytes + (size_t)2 * M * sizeof(int);
+  FP_TRY(dev_alloc(c->epoch, c->cam_args, args_bytes));
+  if (c->stage_args_n < args_bytes) {
+    if (c->stage_args) cudaFreeHost(c->stage_args);
+    c->stage_args = nullptr;
+    c->stage_args_n = 0;
+    FP_CUDA_OK(cudaMallocHost(&c->stage_args, args_bytes));
+    c->stage_args_n = args_bytes;
+  }
+  if (c->stage_poses_n < M) {
+    if (c->stage_poses) cudaFreeHost(c->stage_poses);
+    c->stage_poses = nullptr;
+    c->stage_poses_n = 0;
+    FP_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&c->stage_poses), (size_t)M * 64));
+    c->stage_poses_n = M;
+    ++c->epoch;  // the graph's read-back node holds this address
+  }
+  // the per-call arguments: one staged block, one copy
+  int* ints = reinterpret_cast<int*>(reinterpret_cast<char*>(c->stage_args) + table_bytes);
+  memcpy(ints, slots_host, (size_t)M * sizeof(int));
+  if (by_value) {
+    FP_CUDA_OK(cudaMemcpyAsync(reinterpret_cast<char*>(c->cam_args.p) + table_bytes, ints, (size_t)M * sizeof(int),
+                               cudaMemcpyHostToDevice, st));
+  } else {
+    CameraDev* table = reinterpret_cast<CameraDev*>(c->stage_args);
+    memset(table, 0, table_bytes);
+    for (int i = 0; i < C; ++i) {
+      CameraDev& e = table[i];
+      e.rgb_raw = reinterpret_cast<const unsigned char*>(i ? c->cams[i].rgb_raw.p : c->rgb_raw.p);
+      e.depth_raw = reinterpret_cast<const float*>(i ? c->cams[i].depth_raw.p : c->depth_raw.p);
+      e.rgb = reinterpret_cast<uchar4*>(i ? c->cams[i].rgba.p : c->rgba.p);
+      e.depth = reinterpret_cast<float*>(i ? c->cams[i].depth.p : c->depth_b.p);
+      e.xyz_map = reinterpret_cast<float4*>(i ? c->cams[i].xyz.p : c->xyz.p);
+      e.fx = K[9 * i + 0];
+      e.fy = K[9 * i + 4];
+      e.cx = K[9 * i + 2];
+      e.cy = K[9 * i + 5];
+      e.H = H[i];
+      e.W = W[i];
+    }
+    memcpy(ints + M, camera_of, (size_t)M * sizeof(int));
+    FP_CUDA_OK(cudaMemcpyAsync(c->cam_args.p, c->stage_args, args_bytes, cudaMemcpyHostToDevice, st));
+  }
+  const CameraDev* cams_dev = by_value ? nullptr : reinterpret_cast<const CameraDev*>(c->cam_args.p);
+  const int* mesh_of = reinterpret_cast<const int*>(reinterpret_cast<const char*>(c->cam_args.p) + table_bytes);
+  const int* cam_of = by_value ? nullptr : mesh_of + M;
+  float* pa = reinterpret_cast<float*>(c->poses_a.p);
+  float* pb = reinterpret_cast<float*>(c->poses_b.p);
+  FP_CUDA_OK(cudaMemcpyAsync(pa, poses_in_dev, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
+  // camera i's DMA runs while camera i + 1 is copied into its staging on the host
+  for (int i = 0; i < C; ++i) {
+    const size_t npix = (size_t)H[i] * W[i];
+    if (i == 0) {
+      FP_TRY(upload_staged_frame(c, rgb_host[0], depth_host[0], npix, st));
+    } else {
+      CameraBufs& b = c->cams[i];
+      FP_TRY(upload_staged_frame(b.stage_rgb, b.stage_depth, b.rgb_raw.p, b.depth_raw.p, rgb_host[i], depth_host[i], npix, st));
+    }
+  }
+  c->has_frame = false;
+  const float* fin = (iterations % 2 == 0) ? pa : pb;
+  const int grid_h = c->cam_grid_h, grid_w = c->cam_grid_w;
+  auto body = [&](cudaStream_t s2) -> int {
+    // estimater.py:250-268 for every object of every camera at once: each camera's frame filtered once, M hypotheses
+    // each rendering its own mesh and cropping its own camera's frame
+    if (by_value) {
+      FP_TRY(set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->rgb_raw.p),
+                                reinterpret_cast<const float*>(c->depth_raw.p), FP_FRAME_FILTER_DEPTH, INFINITY, s2));
+    } else {
+      c->depth_cur = reinterpret_cast<const float*>(c->depth_b.p);
+      FP_TRY(frame_prep_cameras_launch(cams_dev, C, grid_h, grid_w, INFINITY, s2));
+    }
+    c->has_frame = true;
+    FP_TRY(refine_body(c, M, iterations, s2, mesh_of, cams_dev, cam_of));
+    FP_CUDA_OK(cudaMemcpyAsync(c->stage_poses, fin, (size_t)M * 64, cudaMemcpyDeviceToHost, s2));
+    return 0;
+  };
+  if (by_value) {
+    FP_TRY(run_graphed(c, 3, M, iterations, st, body));
+  } else {
+    FP_TRY(run_graphed(c, 6, M, iterations, st, body, C, /*frame_by_value=*/false));
+  }
+  c->has_frame = true;
+  if (poses_out_dev) FP_CUDA_OK(cudaMemcpyAsync(poses_out_dev, fin, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
+  FP_CUDA_OK(cudaStreamSynchronize(st));
+  if (poses_out_host) memcpy(poses_out_host, c->stage_poses, (size_t)M * 64);
   return 0;
 }
 
@@ -685,9 +875,15 @@ int fp_destroy(fp_ctx* c) {
                     &c->x1, &c->ff, &c->x2pre, &c->head_out, &c->poses_a, &c->poses_b, &c->feats, &c->tail_qkv,
                     &c->tail_attn, &c->tail_proj, &c->scores, &c->best, &c->lt_buf, &c->lr_buf, &c->feat_buf,
                     &c->pose_stage, &c->mask_buf, &c->mask_stats, &c->crop_stats, &c->track_pose, &c->fold_v, &c->tail_counter, &c->tok_mean,
-                    &c->seg_off, &c->reg_feats};
+                    &c->seg_off, &c->reg_feats, &c->cam_args};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
+  for (CameraBufs& cb : c->cams) {
+    for (DevBuf* b : {&cb.rgb_raw, &cb.depth_raw, &cb.rgba, &cb.depth, &cb.xyz})
+      if (b->p) cudaFree(b->p);
+    if (cb.stage_rgb) cudaFreeHost(cb.stage_rgb);
+    if (cb.stage_depth) cudaFreeHost(cb.stage_depth);
+  }
   for (auto& kv : c->graphs)
     if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   if (c->cap_stream) cudaStreamDestroy(c->cap_stream);
@@ -700,6 +896,7 @@ int fp_destroy(fp_ctx* c) {
   if (c->stage_poses) cudaFreeHost(c->stage_poses);
   if (c->stage_masks) cudaFreeHost(c->stage_masks);
   if (c->stage_ints) cudaFreeHost(c->stage_ints);
+  if (c->stage_args) cudaFreeHost(c->stage_args);
   delete c;
   return 0;
   FP_API_END
@@ -1205,44 +1402,38 @@ int fp_track_objects(fp_ctx* c, const unsigned char* rgb_host, const float* dept
     FP_REQUIRE(c->mesh[slots_host[i]].loaded, "fp_track_objects: object %d: slot %d holds no mesh", i, slots_host[i]);
   }
   DeviceGuard dg(c->device);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(ensure_capacity(c, M));
-  FP_TRY(prepare_frame(c, K, H, W, true));
-  FP_TRY(dev_alloc(c->epoch, c->mesh_of, (size_t)M * sizeof(int)));
-  FP_TRY(alloc_frame_staging(c, (size_t)H * W));
-  if (c->stage_poses_n < M) {
-    if (c->stage_poses) cudaFreeHost(c->stage_poses);
-    c->stage_poses = nullptr;
-    c->stage_poses_n = 0;
-    FP_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&c->stage_poses), (size_t)M * 64));
-    c->stage_poses_n = M;
-    ++c->epoch;  // the graph's read-back node holds this address
+  const std::vector<int> camera_of(M, 0);
+  return track_cameras_body(c, 1, &rgb_host, &depth_host, K, &H, &W, M, camera_of.data(), slots_host, poses_in_dev, iterations,
+                            poses_out_dev, poses_out_host, reinterpret_cast<cudaStream_t>(stream), /*by_value=*/true);
+  FP_API_END
+}
+
+int fp_track_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host, const float* K,
+                     const int* H, const int* W, int M, const int* camera_of, const int* slots_host, const float* poses_in_dev,
+                     int iterations, float* poses_out_dev, float* poses_out_host, void* stream) {
+  FP_API_BEGIN
+  FP_REQUIRE(c && rgb_host && depth_host && K && H && W && M > 0 && camera_of && slots_host && poses_in_dev && iterations >= 0,
+             "fp_track_cameras: bad argument");
+  FP_REQUIRE(C >= 1 && C <= kMaxCameras, "fp_track_cameras: %d cameras, need 1..%d", C, kMaxCameras);
+  FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
+  // everything is checked before anything is enqueued: the kernels index the mesh and camera tables unchecked
+  for (int i = 0; i < C; ++i) {
+    FP_REQUIRE(rgb_host[i] && depth_host[i], "fp_track_cameras: camera %d: null frame", i);
+    FP_REQUIRE(H[i] > 0 && W[i] > 0, "fp_track_cameras: camera %d: empty frame (%d x %d)", i, H[i], W[i]);
   }
-  float* pa = reinterpret_cast<float*>(c->poses_a.p);
-  float* pb = reinterpret_cast<float*>(c->poses_b.p);
-  const int* mesh_of = reinterpret_cast<const int*>(c->mesh_of.p);
-  // slot ids and start poses go to fixed context buffers ahead of the launch: the graph is keyed on (M, iterations)
-  // alone, so any set or order of objects replays it
-  FP_CUDA_OK(cudaMemcpyAsync(c->mesh_of.p, slots_host, (size_t)M * sizeof(int), cudaMemcpyHostToDevice, st));
-  FP_CUDA_OK(cudaMemcpyAsync(pa, poses_in_dev, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
-  FP_TRY(upload_staged_frame(c, rgb_host, depth_host, (size_t)H * W, st));
-  c->has_frame = false;
-  const float* fin = (iterations % 2 == 0) ? pa : pb;
-  auto body = [&](cudaStream_t s2) -> int {
-    // estimater.py:250-268 for every object at once: one filtered frame, M hypotheses each rendering its own mesh
-    FP_TRY(set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->rgb_raw.p),
-                              reinterpret_cast<const float*>(c->depth_raw.p), FP_FRAME_FILTER_DEPTH, INFINITY, s2));
-    c->has_frame = true;
-    FP_TRY(refine_body(c, M, iterations, s2, mesh_of));
-    FP_CUDA_OK(cudaMemcpyAsync(c->stage_poses, fin, (size_t)M * 64, cudaMemcpyDeviceToHost, s2));
-    return 0;
-  };
-  FP_TRY(run_graphed(c, 3, M, iterations, st, body));
-  c->has_frame = true;
-  if (poses_out_dev) FP_CUDA_OK(cudaMemcpyAsync(poses_out_dev, fin, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
-  FP_CUDA_OK(cudaStreamSynchronize(st));
-  if (poses_out_host) memcpy(poses_out_host, c->stage_poses, (size_t)M * 64);
-  return 0;
+  std::vector<int> owns(C, 0);
+  for (int i = 0; i < M; ++i) {
+    FP_REQUIRE(camera_of[i] >= 0 && camera_of[i] < C, "fp_track_cameras: object %d: camera %d out of range [0, %d)", i,
+               camera_of[i], C);
+    FP_REQUIRE(slots_host[i] >= 0 && slots_host[i] < kMaxMeshes, "fp_track_cameras: object %d: slot %d out of range [0, %d)", i,
+               slots_host[i], kMaxMeshes);
+    FP_REQUIRE(c->mesh[slots_host[i]].loaded, "fp_track_cameras: object %d: slot %d holds no mesh", i, slots_host[i]);
+    owns[camera_of[i]] = 1;
+  }
+  for (int i = 0; i < C; ++i) FP_REQUIRE(owns[i], "fp_track_cameras: camera %d owns no object", i);
+  DeviceGuard dg(c->device);
+  return track_cameras_body(c, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, poses_in_dev, iterations,
+                            poses_out_dev, poses_out_host, reinterpret_cast<cudaStream_t>(stream), /*by_value=*/false);
   FP_API_END
 }
 

@@ -1,7 +1,8 @@
 // fp_crop.cu — tiled "pose -> 160x160 network inputs" producer.  ONE kernel; one CTA per (pose hypothesis, TILE x TILE
 // pixel tile of the crop; TILE = 80 / 32 / 16 by batch size); nothing full-frame, nothing fp32 and no intermediate of
 // any kind is materialised in HBM.  Each hypothesis renders the mesh of its own slot of the context's mesh table
-// (CropParams::mesh_of), so one launch can crop several objects:
+// (CropParams::mesh_of), and optionally takes its frame from its own entry of a camera table (CropParams::cams,
+// camera_of), so one launch can crop several objects seen by several cameras:
 //   1. crop window from the pose                         (Utils.py:577-621 compute_crop_window_tf_batch, 'box_3d')
 //   2. binning: every MESHLET of the mesh (<= 64 triangles, fp_meshlet.cu) is tested against the tile with its
 //      bounding sphere and — closed meshes — its normal cone; survivors go to a shared-memory list
@@ -278,8 +279,9 @@ struct TileSmem {
   int n_list, next;
   int stat[4];
   MeshSlotDev slot;  // mesh table entry of this CTA's hypothesis
+  CameraDev cam;     // camera table entry of this CTA's hypothesis (kCams)
 };
-static_assert(sizeof(MeshSlotDev) % 16 == 0 && sizeof(MeshSlotDev) / 16 <= kThreads, "table entry copied as uint4s");
+static_assert(sizeof(MeshSlotDev) % 16 == 0 && sizeof(MeshSlotDev) / 16 <= 32, "table entry copied as uint4s by warp 0");
 
 // one triangle of a meshlet, all three vertices in front of the near plane: coverage inside the tile + depth test
 template <int TILE>
@@ -347,7 +349,12 @@ __device__ __forceinline__ float pixel_ray(float idx_plus_half, float origin, fl
   return __fdiv_rn(__fsub_rn(u, c), f);
 }
 
-template <int TILE, bool kStats>
+// kCams: the frame comes from the camera table entry of the hypothesis (p.cams[p.camera_of[n]], copied to shared memory
+// next to the mesh entry) instead of the by-value fields.  A template flag rather than a branch, so that the
+// single-camera instantiations compile to the same code as before the camera table existed.
+// FRAME(f): field f of the frame this hypothesis is cropped from, read where it is used
+#define FRAME(f) (kCams ? sm.cam.f : p.f)
+template <int TILE, bool kStats, bool kCams>
 __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(const CropParams p) {
   constexpr int TPR = S / TILE;
   extern __shared__ __align__(16) unsigned char crop_smem_raw[];
@@ -364,11 +371,16 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
     sm.next = 0;
     sm.stat[0] = sm.stat[1] = sm.stat[2] = sm.stat[3] = 0;
   }
-  // The mesh table and the slot ids are written by copies that precede the whole launch sequence, never by a kernel
-  // of it: they may be read before the programmatic-dependency wait.
+  // The mesh table, the camera table and the slot and camera ids are written by copies that precede the whole launch
+  // sequence, never by a kernel of it: they may be read before the programmatic-dependency wait.  The pixels the camera
+  // entry points to come from frame_prep_kernel of the same sequence and are only read after it.
   if (tid < (int)(sizeof(MeshSlotDev) / 16)) {
     const int s = p.mesh_of ? __ldg(p.mesh_of + n) : 0;
     reinterpret_cast<uint4*>(&sm.slot)[tid] = __ldg(reinterpret_cast<const uint4*>(p.slots + s) + tid);
+  }
+  if (kCams && tid >= 32 && tid < 32 + (int)(sizeof(CameraDev) / 16)) {
+    const int cam = __ldg(p.camera_of + n);
+    reinterpret_cast<uint4*>(&sm.cam)[tid - 32] = __ldg(reinterpret_cast<const uint4*>(p.cams + cam) + tid - 32);
   }
   pdl_trigger();
   pdl_wait();  // the poses come from the previous iteration's pose update; the crop buffer is read by its stem conv
@@ -376,7 +388,7 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
   __syncthreads();
   if (warp == 0) {
     Window w;
-    crop_window_warp(sm.P, p.fx, p.fy, p.cx, p.cy, sm.slot.r3[p.mode ? 1 : 0], lane, w);
+    crop_window_warp(sm.P, FRAME(fx), FRAME(fy), FRAME(cx), FRAME(cy), sm.slot.r3[p.mode ? 1 : 0], lane, w);
     if (lane == 0) {
       sm.win = w;
       if (p.win_out && tile == 0) {
@@ -397,7 +409,7 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
     const int k = is_row ? tid - TILE : tid;
     const int d = (is_row ? ty0 : tx0) + k;
     const float sc = is_row ? W.sy : W.sx, org = is_row ? W.top : W.left;
-    const int size = is_row ? p.H : p.W;
+    const int size = is_row ? FRAME(H) : FRAME(W);
     const float xs = __fadd_rn(__fdiv_rn((float)d, sc), org);
     const float ix = kornia_src_coord(xs, size);
     int un = (int)rintf(ix);
@@ -456,9 +468,10 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
       } else if (Z - r > p.znear) {
         // |delta u| <= fx r (1 + |X| / Z) / (Z - r) for any point of the sphere; crop raster pixels; 1 px of slack
         const float izc = 1.f / Z, izn = 1.f / (Z - r);
-        const float pu = (p.fx * X * izc + p.cx - W.umin) * W.rsx, pv = (p.fy * Y * izc + p.cy - W.vmin) * W.rsy;
-        const float ru = p.fx * W.rsx * r * (1.f + fabsf(X) * izc) * izn + 1.f;
-        const float rv = p.fy * W.rsy * r * (1.f + fabsf(Y) * izc) * izn + 1.f;
+        const float pu = (FRAME(fx) * X * izc + FRAME(cx) - W.umin) * W.rsx;
+        const float pv = (FRAME(fy) * Y * izc + FRAME(cy) - W.vmin) * W.rsy;
+        const float ru = FRAME(fx) * W.rsx * r * (1.f + fabsf(X) * izc) * izn + 1.f;
+        const float rv = FRAME(fy) * W.rsy * r * (1.f + fabsf(Y) * izc) * izn + 1.f;
         keep = pu + ru >= (float)tx0 && pu - ru <= (float)(tx0 + TILE) && pv + rv >= (float)ty0 &&
                pv - rv <= (float)(ty0 + TILE);
       }
@@ -501,7 +514,7 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
           const int gid = __ldg(M.ml_verts + hdr.x + s);
           const float4 q = __ldg(M.vpos + gid);
           VtxScreen o;
-          xform_vertex(sm.P, q.x, q.y, q.z, W, p.fx, p.fy, p.cx, p.cy, o);
+          xform_vertex(sm.P, q.x, q.y, q.z, W, FRAME(fx), FRAME(fy), FRAME(cx), FRAME(cy), o);
           VtxS v;
           v.xi = o.xi; v.yi = o.yi; v.iz = o.iz; v.Z = o.Z;
           sv[s] = v;
@@ -543,15 +556,15 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
             const int gid = __ldg(M.ml_verts + hdr.x + ((packed >> (8 * k)) & 255));
             const float4 q = __ldg(M.vpos + gid);
             VtxScreen o;
-            xform_vertex(sm.P, q.x, q.y, q.z, W, p.fx, p.fy, p.cx, p.cy, o);
+            xform_vertex(sm.P, q.x, q.y, q.z, W, FRAME(fx), FRAME(fy), FRAME(cx), FRAME(cy), o);
             Pc[k][0] = o.X; Pc[k][1] = o.Y; Pc[k][2] = o.Z;
           }
           HomTri ht;
           hom_setup(Pc[0], Pc[1], Pc[2], ht);
           for (int px = lane; px < TILE * TILE; px += 32) {
             const int r = px / TILE, jl = px - r * TILE;
-            const float dx = pixel_ray((float)(tx0 + jl) + 0.5f, W.umin, W.rsx, p.cx, p.fx);
-            const float dy = pixel_ray((float)(ty0 + r) + 0.5f, W.vmin, W.rsy, p.cy, p.fy);
+            const float dx = pixel_ray((float)(tx0 + jl) + 0.5f, W.umin, W.rsx, FRAME(cx), FRAME(fx));
+            const float dy = pixel_ray((float)(ty0 + r) + 0.5f, W.vmin, W.rsy, FRAME(cy), FRAME(fy));
             float l0, l1, l2, iz;
             if (hom_cover(ht, dx, dy, p.znear, p.zfar, l0, l1, l2, iz)) {
               atomicMax(&sm.zt[px], depth_key(iz, face));
@@ -609,7 +622,7 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
         const float4 pp = __ldg(M.vpos + vid[q]);
         const float4 nn = __ldg(M.vnrm + vid[q]);
         att[q] = __ldg(M.vatt + vid[q]);
-        xform_vertex(sm.P, pp.x, pp.y, pp.z, W, p.fx, p.fy, p.cx, p.cy, vs[q]);
+        xform_vertex(sm.P, pp.x, pp.y, pp.z, W, FRAME(fx), FRAME(fy), FRAME(cx), FRAME(cy), vs[q]);
         // diffuse = clip(normalize(R n) . (0,0,-1), 0, 1)   (Utils.py:203-207)
         const float cxn = sm.P[0] * nn.x + sm.P[1] * nn.y + sm.P[2] * nn.z;
         const float cyn = sm.P[4] * nn.x + sm.P[5] * nn.y + sm.P[6] * nn.z;
@@ -638,8 +651,8 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
         const float A3[3] = {vs[0].X, vs[0].Y, vs[0].Z}, B3[3] = {vs[1].X, vs[1].Y, vs[1].Z}, C3[3] = {vs[2].X, vs[2].Y, vs[2].Z};
         HomTri ht;
         hom_setup(A3, B3, C3, ht);
-        const float dx = pixel_ray((float)j + 0.5f, W.umin, W.rsx, p.cx, p.fx);
-        const float dy = pixel_ray((float)r + 0.5f, W.vmin, W.rsy, p.cy, p.fy);
+        const float dx = pixel_ray((float)j + 0.5f, W.umin, W.rsx, FRAME(cx), FRAME(fx));
+        const float dy = pixel_ray((float)r + 0.5f, W.vmin, W.rsy, FRAME(cy), FRAME(fy));
         float iz;
         w0 = w1 = w2 = 0.f;
         hom_cover(ht, dx, dy, p.znear, p.zfar, w0, w1, w2, iz);
@@ -695,8 +708,8 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
       const int x0 = (cxi & 0x80000000) ? x1 : max(x1 - 1, 0), y0 = (ryi & 0x80000000) ? y1 : max(y1 - 1, 0);
       const float wx[2] = {(cxi & 0x40000000) ? 0.f : 1.f - wx1, (cxi & 0x80000000) ? 0.f : wx1};
       const float wy[2] = {(ryi & 0x40000000) ? 0.f : 1.f - wy1, (ryi & 0x80000000) ? 0.f : wy1};
-      const uchar4* row0 = p.rgb + (size_t)y0 * p.W;
-      const uchar4* row1 = p.rgb + (size_t)y1 * p.W;
+      const uchar4* row0 = FRAME(rgb) + (size_t)y0 * FRAME(W);
+      const uchar4* row1 = FRAME(rgb) + (size_t)y1 * FRAME(W);
       const uchar4 t00 = __ldg(row0 + x0), t01 = __ldg(row0 + x1), t10 = __ldg(row1 + x0), t11 = __ldg(row1 + x1);
       const float w00 = wx[0] * wy[0], w01 = wx[1] * wy[0], w10 = wx[0] * wy[1], w11 = wx[1] * wy[1];
       br = w00 * t00.x + w01 * t01.x + w10 * t10.x + w11 * t11.x;
@@ -711,17 +724,17 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
       if (unc >= 0 && vn >= 0) {
         if (p.mode == 0) {
           // refiner: xyz_map (depth2xyzmap, Utils.py:399-438) sampled nearest
-          const float4 q = __ldg(p.xyz_map + (size_t)vn * p.W + unc);
+          const float4 q = __ldg(FRAME(xyz_map) + (size_t)vn * FRAME(W) + unc);
           X = q.x;
           Y = q.y;
           Z = q.z;
         } else {
           const int v2 = sm.rowz[rl];
           float zz = 0.f;
-          if (uzc >= 0 && v2 >= 0) zz = __ldg(p.depth + (size_t)v2 * p.W + uzc);
+          if (uzc >= 0 && v2 >= 0) zz = __ldg(FRAME(depth) + (size_t)v2 * FRAME(W) + uzc);
           if (zz >= 0.001f) {  // depth2xyzmap_batch(zfar=inf): invalid z<0.001 -> 0
-            X = ((float)unc - p.cx) * zz / p.fx;
-            Y = ((float)vn - p.cy) * zz / p.fy;
+            X = ((float)unc - FRAME(cx)) * zz / FRAME(fx);
+            Y = ((float)vn - FRAME(cy)) * zz / FRAME(fy);
             Z = zz;
           }
         }
@@ -744,6 +757,8 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
   }
 }
 
+#undef FRAME
+
 static int g_crop_tile_override = [] {
   const char* e = getenv("FPOSE_CROP_TILE");  // 16 / 32 / 80: force one tile size (A/B measurements)
   const int v = e ? atoi(e) : 0;
@@ -762,21 +777,26 @@ static int launch_tile(const CropParams& p, cudaStream_t stream) {
   const size_t smem = sizeof(TileSmem<TILE>);
   static std::atomic<unsigned long long> attr_mask{0};  // per device
   if (!device_bit_test(attr_mask)) {
-    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     device_bit_set(attr_mask);
   }
   const dim3 grid(TPR * TPR, p.N);
-  if (p.stats) {
-    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, true>, grid, dim3(kThreads), smem, stream, 1, p));
+  if (p.cams) {
+    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, false, true>, grid, dim3(kThreads), smem, stream, 1, p));
+  } else if (p.stats) {
+    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, true, false>, grid, dim3(kThreads), smem, stream, 1, p));
   } else {
-    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, false>, grid, dim3(kThreads), smem, stream, 1, p));
+    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, false, false>, grid, dim3(kThreads), smem, stream, 1, p));
   }
   return 0;
 }
 
 int crop_launch(const CropParams& p, cudaStream_t stream) {
   if (p.N == 0) return 0;
+  FP_REQUIRE(!p.cams == !p.camera_of, "crop_launch: the camera table and the camera ids go together");
+  FP_REQUIRE(!(p.cams && p.stats), "crop_launch: work counters are collected on the single-camera path only");
   // algorithmic bytes: the two 6-channel fp16 crops each hypothesis produces (SURVEY.md §8d)
   prof_mark_begin(1, (double)p.N * 2.0 * 6.0 * S * S * 2.0, stream);
   int tile = p.N >= 64 ? 80 : (p.N >= 4 ? 32 : 16);

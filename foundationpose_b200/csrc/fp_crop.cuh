@@ -52,6 +52,21 @@ struct __align__(16) MeshSlotDev {
   float half_diameter;  // mesh_diameter / 2             (predict_pose_refine.py:199, pose update)
 };
 
+constexpr int kMaxCameras = 16;  // FP_MAX_CAMERAS (include/fpose.h)
+
+// One entry of the camera table of fp_track_cameras: one camera stream's frame buffers (device), size and intrinsics.
+// frame_prep_kernel reads the raw frame and writes the filtered one; the crop producer reads the filtered one.
+struct __align__(16) CameraDev {
+  const unsigned char* rgb_raw;  // [H][W][3] uploaded frame
+  const float* depth_raw;        // [H][W]
+  uchar4* rgb;                   // [H][W] RGBA8
+  float* depth;                  // [H][W] eroded + bilateral-filtered depth
+  float4* xyz_map;               // [H][W] (x, y, z, 0) back-projected filtered depth
+  float fx, fy, cx, cy;
+  int H, W;
+};
+static_assert(sizeof(CameraDev) == 64, "camera table entry: four uint4s");
+
 struct CropParams {
   const float* poses;  // [N][16] row-major ob_in_cam
   int N;
@@ -73,6 +88,10 @@ struct CropParams {
   float* win_out;  // optional [N][4] = (left, top, sx, sy)
   int tile_override;  // 0 = pick by batch size; 16 / 32 / 80 = force (fp_set_crop_tile, A/B tests)
   int* stats;      // optional [4]: meshlet visits, triangles set up, fragments, mixed (near-plane) triangles
+  // optional, device: hypothesis n takes its frame (rgba, xyz, filtered depth, fx fy cx cy, H W) from
+  // cams[camera_of[n]] instead of the by-value frame fields above (fp_track_cameras); both null or both set
+  const CameraDev* cams;
+  const int* camera_of;
 };
 
 int crop_launch(const CropParams& p, cudaStream_t stream);

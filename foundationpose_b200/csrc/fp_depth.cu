@@ -105,20 +105,26 @@ __global__ void bilateral_depth_kernel(const float* __restrict__ depth, float* _
 // a second shared tile (halo pixels are recomputed by the neighbouring blocks, identically) and filters from there:
 // one read of the depth image instead of ~50 per pixel from L1 / L2, three launches fewer per frame (47 -> ~12 us of
 // a 0.97 ms tracked frame).  Same per-pixel code as the stand-alone kernels above: bit-identical.
+// kTable: one launch for several cameras (fp_track_cameras).  blockIdx.z selects the camera's entry of the device table
+// `cams`; the grid covers the largest frame and the blocks outside a smaller one leave at once.  Otherwise the one frame
+// is `one`, passed by value.
 constexpr int kFpW = 32, kFpH = 8, kFpR = 2;
+template <bool kTable>
 __global__ void __launch_bounds__(kFpW* kFpH)
-    frame_prep_kernel(const unsigned char* __restrict__ rgb, const float* __restrict__ depth, uchar4* __restrict__ rgba,
-                      float* __restrict__ depth_out, float4* __restrict__ xyz, int H, int W, float fx, float fy, float cx,
-                      float cy, float zfar_xyz) {
+    frame_prep_kernel(const CameraDev one, const CameraDev* __restrict__ cams, float zfar_xyz) {
   constexpr int RW = kFpW + 4 * kFpR, RH = kFpH + 4 * kFpR;  // raw tile 40 x 16
   constexpr int EW = kFpW + 2 * kFpR, EH = kFpH + 2 * kFpR;  // eroded tile 36 x 12
   __shared__ float raw[RH * RW];
   __shared__ float er[EH * EW];
+  const CameraDev cam = kTable ? cams[blockIdx.z] : one;
+  const int H = cam.H, W = cam.W;
+  const float fx = cam.fx, fy = cam.fy, cx = cam.cx, cy = cam.cy;
   const int w0 = blockIdx.x * kFpW, h0 = blockIdx.y * kFpH;
+  if (kTable && (w0 >= W || h0 >= H)) return;  // the whole block lies outside this camera's (smaller) frame
   const int tid = threadIdx.y * kFpW + threadIdx.x;
   for (int i = tid; i < RH * RW; i += kFpW * kFpH) {
     const int v = h0 - 2 * kFpR + i / RW, u = w0 - 2 * kFpR + i % RW;
-    raw[i] = (v >= 0 && v < H && u >= 0 && u < W) ? depth[v * W + u] : 0.f;  // out-of-image cells are never read
+    raw[i] = (v >= 0 && v < H && u >= 0 && u < W) ? __ldg(cam.depth_raw + v * W + u) : 0.f;  // out-of-image cells are never read
   }
   __syncthreads();
   const TileSrc rsrc{raw, h0 - 2 * kFpR, w0 - 2 * kFpR, RW};
@@ -131,21 +137,41 @@ __global__ void __launch_bounds__(kFpW* kFpH)
   if (w >= W || h >= H) return;
   const float z = bilateral_px(TileSrc{er, h0 - kFpR, w0 - kFpR, EW}, w, h, H, W, kFpR, 100.f, 2.f, 100000.f);
   const int i = h * W + w;
-  depth_out[i] = z;
+  cam.depth[i] = z;
   float X = 0.f, Y = 0.f, Z = 0.f;
   if (!(z < 0.001f) && !(z > zfar_xyz)) {  // depth2xyzmap(_batch): Utils.py:399-438
     X = ((float)w - cx) * z / fx;
     Y = ((float)h - cy) * z / fy;
     Z = z;
   }
-  xyz[i] = make_float4(X, Y, Z, 0.f);
-  rgba[i] = make_uchar4(rgb[3 * i], rgb[3 * i + 1], rgb[3 * i + 2], 255);
+  cam.xyz_map[i] = make_float4(X, Y, Z, 0.f);
+  cam.rgb[i] = make_uchar4(__ldg(cam.rgb_raw + 3 * i), __ldg(cam.rgb_raw + 3 * i + 1), __ldg(cam.rgb_raw + 3 * i + 2), 255);
 }
 
 int frame_prep_launch(const unsigned char* rgb, const float* depth, uchar4* rgba, float* depth_out, float4* xyz, int H, int W,
                       float fx, float fy, float cx, float cy, float zfar_xyz, cudaStream_t stream) {
+  CameraDev one{};
+  one.rgb_raw = rgb;
+  one.depth_raw = depth;
+  one.rgb = rgba;
+  one.depth = depth_out;
+  one.xyz_map = xyz;
+  one.fx = fx;
+  one.fy = fy;
+  one.cx = cx;
+  one.cy = cy;
+  one.H = H;
+  one.W = W;
   dim3 block(kFpW, kFpH), grid((W + kFpW - 1) / kFpW, (H + kFpH - 1) / kFpH);
-  frame_prep_kernel<<<grid, block, 0, stream>>>(rgb, depth, rgba, depth_out, xyz, H, W, fx, fy, cx, cy, zfar_xyz);
+  frame_prep_kernel<false><<<grid, block, 0, stream>>>(one, nullptr, zfar_xyz);
+  note_launches(1);
+  FP_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int frame_prep_cameras_launch(const CameraDev* cams, int C, int max_H, int max_W, float zfar_xyz, cudaStream_t stream) {
+  dim3 block(kFpW, kFpH), grid((max_W + kFpW - 1) / kFpW, (max_H + kFpH - 1) / kFpH, C);
+  frame_prep_kernel<true><<<grid, block, 0, stream>>>(CameraDev{}, cams, zfar_xyz);
   note_launches(1);
   FP_CUDA_OK(cudaGetLastError());
   return 0;

@@ -2,6 +2,8 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include "fp_crop.cuh"  // CameraDev
+
 namespace fp {
 int erode_depth_launch(const float* depth, float* out, int H, int W, int radius, float diff_thres, float ratio_thres,
                        float zfar, cudaStream_t stream);
@@ -10,6 +12,9 @@ int bilateral_depth_launch(const float* depth, float* out, int H, int W, int rad
 // erode(2) -> bilateral(2) -> back-projection (invalid: z < 0.001 or z > zfar_xyz) + rgb -> rgba, one launch
 int frame_prep_launch(const unsigned char* rgb, const float* depth, uchar4* rgba, float* depth_out, float4* xyz, int H, int W,
                       float fx, float fy, float cx, float cy, float zfar_xyz, cudaStream_t stream);
+// the same for C cameras in one launch: cams DEVICE [C] (raw frame in, filtered frame out); max_H x max_W covers the
+// largest of the frames
+int frame_prep_cameras_launch(const CameraDev* cams, int C, int max_H, int max_W, float zfar_xyz, cudaStream_t stream);
 // guess_translation + start poses of M objects in two launches: masks [M][H][W]; off [M + 1] device row offsets of
 // each object in rot_grid / poses_out ([off[M]][16]; null when M = 1: rows [0, N)); stats: 6 M words of device
 // scratch; info [M][4] = {tx, ty, tz, n_valid}

@@ -30,6 +30,8 @@ def _proto():
     lib.fp_crop_stats.argtypes = [vp, vp, i, i, C.POINTER(i), vp]
     lib.fp_track.argtypes = [vp, vp, vp, C.POINTER(f), i, i, vp, i, vp, vp, vp]
     lib.fp_track_objects.argtypes = [vp, vp, vp, C.POINTER(f), i, i, i, C.POINTER(i), vp, i, vp, vp, vp]
+    lib.fp_track_cameras.argtypes = [vp, i, C.POINTER(vp), C.POINTER(vp), C.POINTER(f), C.POINTER(i), C.POINTER(i), i, C.POINTER(i),
+                                     C.POINTER(i), vp, i, vp, vp, vp]
     lib.fp_register_objects.argtypes = [vp, vp, vp, C.POINTER(f), i, i, i, C.POINTER(i), C.POINTER(i), vp, vp, i, vp, vp, vp,
                                         vp, vp]
     lib.fp_graph_captures.argtypes = [vp]
@@ -52,7 +54,7 @@ def _proto():
     lib.fp_op_tokens.argtypes = [vp, i, vp, i, vp, vp]
     lib.fp_op_depth_filter.argtypes = [vp, vp, i, i, i, vp]
     lib.fp_op_pose_update.argtypes = [vp, vp, vp, vp, i, f, f, vp]
-    for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_register_objects", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh",
+    for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_track_cameras", "fp_register_objects", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh",
                  "fp_set_mesh_slot", "fp_set_frame",
                  "fp_get_depth", "fp_make_crops", "fp_start_poses", "fp_refine", "fp_score", "fp_score_features", "fp_score_tail",
                  "fp_register", "fp_op_refine_net", "fp_op_score_feats", "fp_op_tokens", "fp_op_depth_filter",
@@ -64,6 +66,7 @@ _proto()
 
 FRAME_ON_DEVICE = 1
 MAX_MESHES = 64  # FP_MAX_MESHES: mesh slots per context
+MAX_CAMERAS = 16  # FP_MAX_CAMERAS: camera streams per fp_track_cameras call
 _NO_PIN = os.environ.get("FPOSE_NO_PIN") == "1"  # A/B: skip the pinned staging of host frames
 FRAME_FILTER_DEPTH = 2
 
@@ -262,6 +265,31 @@ class Engine:
                                         (C.c_int * M)(*slots), _p(poses_in), int(iterations), _p(out),
                                         C.c_void_p(host.ctypes.data), _stream()), "fp_track_objects")
         self.frame_hw = (H, W)
+        return out, host
+
+    def track_cameras(self, frames, poses_in, camera_of, slots, iterations):
+        """fp_track_cameras: `track_objects` for M objects spread over C camera streams in ONE CUDA-graph launch.  frames: C
+        tuples (rgb uint8 (H,W,3), depth float32 (H,W), K (3,3)) of HOST arrays, one per camera, each with its own size and
+        intrinsics; object i is seen by camera camera_of[i] and renders the mesh in slot slots[i]; poses_in (M,4,4) CUDA
+        tensor.  Returns (poses CUDA (M,4,4), poses host (M,4,4) float32 numpy)."""
+        frames = [(np.ascontiguousarray(rgb, dtype=np.uint8), np.ascontiguousarray(depth, dtype=np.float32), K) for rgb, depth, K in frames]
+        n_cam = len(frames)
+        poses_in = poses_in.reshape(-1, 4, 4).contiguous().float()
+        M = len(poses_in)
+        camera_of, slots = [int(c) for c in camera_of], [int(s) for s in slots]
+        if len(camera_of) != M or len(slots) != M:
+            raise ValueError(f"track_cameras: {M} poses, {len(camera_of)} camera ids and {len(slots)} slots")
+        rgbs = (C.c_void_p * n_cam)(*[rgb.ctypes.data for rgb, _, _ in frames])
+        depths = (C.c_void_p * n_cam)(*[depth.ctypes.data for _, depth, _ in frames])
+        Ks = (C.c_float * (9 * n_cam))(*[float(x) for _, _, K in frames for x in np.asarray(K, dtype=np.float64).reshape(-1)])
+        Hs = (C.c_int * n_cam)(*[depth.shape[0] for _, depth, _ in frames])
+        Ws = (C.c_int * n_cam)(*[depth.shape[1] for _, depth, _ in frames])
+        out = torch.empty(M, 4, 4, dtype=torch.float32, device="cuda")
+        host = np.empty((M, 4, 4), dtype=np.float32)
+        _lib.check(lib.fp_track_cameras(self._h, n_cam, rgbs, depths, Ks, Hs, Ws, M, (C.c_int * M)(*camera_of), (C.c_int * M)(*slots),
+                                        _p(poses_in), int(iterations), _p(out), C.c_void_p(host.ctypes.data), _stream()),
+                   "fp_track_cameras")
+        self.frame_hw = frames[0][1].shape  # camera 0's frame is the context's frame
         return out, host
 
     def register_objects(self, rgb, depth, K, masks, rot_grids, slots, iterations):

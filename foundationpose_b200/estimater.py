@@ -19,7 +19,7 @@ import numpy as np
 import torch
 
 from . import hypotheses, meshprep, synth, weights
-from .engine import MAX_MESHES, Engine
+from .engine import MAX_CAMERAS, MAX_MESHES, Engine
 
 
 class _Cfg(dict):
@@ -410,6 +410,42 @@ def track_objects(estimators, rgb, depth, K, iteration=2):
         est.refiner.last_trans_update = est.refiner.last_rot_update = None
         out.append(_uncentre(poses_host[i], est.model_center))
     return out
+
+
+def track_cameras(views, iteration=2):
+    """`[[est.track_one(rgb, depth, K, iteration) for est in ests] for ests, rgb, depth, K in views]` for objects seen by
+    several camera streams (a multi-camera rig, or several recordings on one GPU), as ONE CUDA-graph launch per call
+    (fp_track_cameras): every camera's frame is uploaded and filtered, and every (object, camera) pair is refined in one
+    batch, each pair tracked independently in its own camera's frame.  Same poses as the per-object calls; updates every
+    pose_last.
+
+    views: one (estimators, rgb, depth, K) per camera, each camera with its own frame size and intrinsics.  All
+    estimators share one engine and none appears twice, across cameras or within one; at most MAX_MESHES - 1 objects and
+    MAX_CAMERAS cameras with objects.  A camera without estimators gives [] and its frame is not uploaded.  Each
+    estimator keeps its mesh in the slot track_objects / register_objects use.  Host frames only (uint8 (H,W,3) rgb,
+    float32 (H,W) depth).  Returns one list of (4,4) float32 poses of the original meshes per camera."""
+    views = [(list(ests), rgb, depth, K) for ests, rgb, depth, K in views]
+    if any(torch.is_tensor(rgb) or torch.is_tensor(depth) for _, rgb, depth, _ in views):
+        raise TypeError("track_cameras takes host frames (numpy); for device-resident frames call track_one per object")
+    used = [v for v in views if v[0]]
+    if not used:
+        return [[] for _ in views]
+    estimators = [est for ests, _, _, _ in used for est in ests]
+    e = _shared_engine_of(estimators, "track_cameras")
+    if len(used) > MAX_CAMERAS:
+        raise ValueError(f"track_cameras: at most {MAX_CAMERAS} cameras with objects, got {len(used)}")
+    if any(est.pose_last is None for est in estimators):
+        logging.info("Please init pose by register first")
+        raise RuntimeError
+    slots = [_object_slot(est, "track_cameras") for est in estimators]
+    camera_of = [c for c, (ests, _, _, _) in enumerate(used) for _ in ests]
+    poses_in = torch.stack([est.pose_last.reshape(4, 4) for est in estimators])
+    poses_dev, poses_host = e.track_cameras([(rgb, depth, K) for _, rgb, depth, K in used], poses_in, camera_of, slots, iteration)
+    for i, est in enumerate(estimators):
+        est.pose_last = poses_dev[i].reshape(1, 4, 4)
+        est.refiner.last_trans_update = est.refiner.last_rot_update = None
+    flat = iter(_uncentre(poses_host[i], est.model_center) for i, est in enumerate(estimators))
+    return [[next(flat) for _ in ests] for ests, _, _, _ in views]
 
 
 def register_objects(estimators, K, rgb, depth, ob_masks, ob_ids=None, iteration=5):

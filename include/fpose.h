@@ -195,6 +195,24 @@ int fp_track(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host
 int fp_track_objects(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
                      int M, const int* slots_host, const float* poses_in_dev, int iterations, float* poses_out_dev,
                      float* poses_out_host, void* stream);
+/* fp_track_objects for M objects spread over C camera streams (1 <= C <= FP_MAX_CAMERAS), each camera with its own
+ * frame size and intrinsics, as ONE CUDA-graph launch: object i is seen by camera camera_of[i] and tracked exactly as
+ * fp_track_objects tracks it in that camera's frame alone, bit for bit.
+ *   rgb_host[c] / depth_host[c]: HOST uint8 [H[c]][W[c]][3] / float32 [H[c]][W[c]] frame of camera c, each uploaded
+ *   through its own pinned staging; K: [C][9] row-major intrinsics; camera_of, slots_host: HOST [M] camera and mesh
+ *   slot of every object; poses_in_dev: DEVICE [M][16]; poses_out_dev (DEVICE [M][16]) / poses_out_host (HOST [M][16])
+ *   are optional.
+ * Everything is checked before anything is enqueued: every camera id in [0, C), every camera owning at least one
+ * object, every slot loaded, non-null frames of positive size.  One frame-preparation launch filters every camera's
+ * depth, then `iterations` refiner passes run over all M objects.  The camera table (buffers, sizes, intrinsics), the
+ * slot ids and the camera ids are copied into the context first, so the cached graph depends on (C, M, iterations)
+ * only: reordering objects or cameras or changing intrinsics replays it.  Camera 0 is the context's frame: afterwards
+ * the context holds camera 0's frame as fp_track_objects leaves it.  Cameras 1.. get buffers of their own, kept at the
+ * largest frame size seen.  Leaves fp_track's continuation pose untouched.  Synchronises. */
+#define FP_MAX_CAMERAS 16
+int fp_track_cameras(fp_ctx* ctx, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
+                     const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
+                     const float* poses_in_dev, int iterations, float* poses_out_dev, float* poses_out_host, void* stream);
 /* FoundationPose.register (estimater.py:159-240) applied to M objects of the same frame in one call; object i gives
  * exactly what fp_set_frame + fp_start_poses + fp_refine + fp_score give for that object alone, bit for bit.
  *   1. Checks every argument before anything is enqueued: slots_host HOST [M] loaded slot ids (one slot may appear
