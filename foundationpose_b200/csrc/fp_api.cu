@@ -8,8 +8,10 @@
 #include <algorithm>
 #include <exception>
 #include <map>
+#include <memory>
 #include <string>
 #include <tuple>
+#include <utility>
 #include <vector>
 
 #include "../../include/fpose.h"
@@ -22,10 +24,32 @@
 namespace fp {
 const char* get_last_error();
 
-struct DevBuf {
+// An allocation that `Free` releases when its owner goes away or grows it.  Move-only: every allocation has one owner,
+// so destroying a context, a mesh slot or a replaced weight tensor frees exactly what it held.  Device memory must be
+// released with its device current.
+template <cudaError_t (*Free)(void*)>
+struct OwnedBuf {
   void* p = nullptr;
   size_t bytes = 0;
+  OwnedBuf() = default;
+  OwnedBuf(OwnedBuf&& o) noexcept : p(std::exchange(o.p, nullptr)), bytes(std::exchange(o.bytes, 0)) {}
+  OwnedBuf& operator=(OwnedBuf&& o) noexcept {
+    if (this != &o) {
+      reset();
+      p = std::exchange(o.p, nullptr);
+      bytes = std::exchange(o.bytes, 0);
+    }
+    return *this;
+  }
+  ~OwnedBuf() { reset(); }
+  void reset() {
+    if (p) Free(p);
+    p = nullptr;
+    bytes = 0;
+  }
 };
+using DevBuf = OwnedBuf<cudaFree>;         // device memory
+using PinnedBuf = OwnedBuf<cudaFreeHost>;  // page-locked host memory
 
 // (Re)allocates `b` to at least `bytes`.  `epoch` is the owning context's graph epoch: it is bumped whenever a device
 // pointer or by-value kernel parameter that a captured CUDA graph may hold changes (re-allocation, new weights /
@@ -34,9 +58,7 @@ struct DevBuf {
 static int dev_alloc(unsigned long long& epoch, DevBuf& b, size_t bytes, bool zero = false) {
   if (b.bytes >= bytes && b.p) return 0;
   ++epoch;
-  if (b.p) cudaFree(b.p);
-  b.p = nullptr;
-  b.bytes = 0;
+  b.reset();
   FP_CUDA_OK(cudaMalloc(&b.p, bytes));
   b.bytes = bytes;
   if (zero) {
@@ -54,8 +76,19 @@ static int upload(unsigned long long& epoch, DevBuf& b, const std::vector<T>& v)
   return 0;
 }
 
+// (Re)allocates pinned `b` to at least `bytes` (cudaHostAlloc `flags`).  `epoch`: the graph epoch of the context whose
+// captured graph holds b's address (a read-back node), bumped when the address changes; null where no graph holds it.
+static int pinned_alloc(unsigned long long* epoch, PinnedBuf& b, size_t bytes, unsigned flags = cudaHostAllocDefault) {
+  if (b.bytes >= bytes && b.p) return 0;
+  if (epoch) ++*epoch;
+  b.reset();
+  FP_CUDA_OK(cudaHostAlloc(&b.p, bytes, flags));
+  b.bytes = bytes;
+  return 0;
+}
+
 struct Tensor {
-  void* p = nullptr;
+  DevBuf buf;
   int dtype = 0;  // 0 = f32, 1 = f16
   long long numel = 0;
 };
@@ -65,8 +98,8 @@ struct Net {
   bool loaded = false;
   // fp_load_network verified that every name the execution plan uses is present; a miss is a programming error
   // and surfaces as an exception that the extern "C" wrappers turn into an error code
-  const __half* h(const char* name) const { return reinterpret_cast<const __half*>(t.at(name).p); }
-  const float* f(const char* name) const { return reinterpret_cast<const float*>(t.at(name).p); }
+  const __half* h(const char* name) const { return reinterpret_cast<const __half*>(t.at(name).buf.p); }
+  const float* f(const char* name) const { return reinterpret_cast<const float*>(t.at(name).buf.p); }
 };
 
 constexpr int S = 160;
@@ -99,9 +132,7 @@ struct MeshSlot {
 // and the pinned staging of their uploads.
 struct CameraBufs {
   DevBuf rgb_raw, depth_raw, rgba, depth, xyz;
-  void* stage_rgb = nullptr;
-  void* stage_depth = nullptr;
-  size_t stage_npix = 0;
+  PinnedBuf stage_rgb, stage_depth;
 };
 
 }  // namespace fp
@@ -154,27 +185,19 @@ struct fp_ctx {
   fp::DevBuf lt_buf, lr_buf, feat_buf, pose_stage, tok_mean;
   fp::DevBuf mask_buf, mask_stats, crop_stats;
   // fp_track: pinned host staging (frame in, pose out) so that the whole frame is ONE graph launch
-  void* stage_rgb = nullptr;
-  void* stage_depth = nullptr;
-  float* stage_pose = nullptr;
-  size_t stage_npix = 0;
+  fp::PinnedBuf stage_rgb, stage_depth, stage_pose;
   fp::DevBuf track_pose;
-  float* stage_poses = nullptr;  // fp_track_objects: pinned [stage_poses_n][16] pose read-back
-  int stage_poses_n = 0;
+  fp::PinnedBuf stage_poses;  // fp_track_objects: pinned [M][16] pose read-back
   // fp_register_objects: row offsets of the objects' hypotheses [M + 1], their feature rows [sum N][512]; pinned staging
   // of the masks and of (offsets, per-hypothesis slot ids)
   fp::DevBuf seg_off, reg_feats;
-  unsigned char* stage_masks = nullptr;
-  size_t stage_masks_n = 0;
-  int* stage_ints = nullptr;
-  size_t stage_ints_n = 0;
+  fp::PinnedBuf stage_masks, stage_ints;
   // fp_track_cameras: buffers of cameras 1..; the per-call arguments (camera table [FP_MAX_CAMERAS], slot ids [M],
   // camera ids [M]) as one device block and its pinned staging; the frame size its frame-preparation grid covers (the
   // largest seen)
   fp::CameraBufs cams[fp::kMaxCameras];
   fp::DevBuf cam_args;
-  void* stage_args = nullptr;
-  size_t stage_args_n = 0;
+  fp::PinnedBuf stage_args;
   int cam_grid_h = 0, cam_grid_w = 0;
 };
 
@@ -481,6 +504,17 @@ static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg
   return crop_launch(p, st);
 }
 
+// The launch sequence a cached graph holds: the first element of its key
+enum class GraphKind {
+  Refine = 0,            // fp_refine
+  ScoreFeatures = 1,     // fp_score_features
+  Track = 2,             // fp_track
+  TrackObjects = 3,      // fp_track_objects
+  RegisterRefine = 4,    // fp_register_objects: one pass's refinement
+  RegisterFeatures = 5,  // fp_register_objects: one pass's scorer features
+  TrackCameras = 6,      // fp_track_cameras
+};
+
 // Runs `body(stream)` — a fixed sequence of kernel launches (and fixed-address copies) on ctx-owned buffers —
 // through a cached CUDA graph: first sight of a key runs eagerly (sets function attributes), the second
 // captures + instantiates, later calls replay.  Replay removes ~170 launch + 60 tensor-map-encode host
@@ -490,10 +524,10 @@ static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg
 // which reads them from the camera table); such a graph is captured again when they differ from its capture's.  Only
 // that graph: a frame of another size or other intrinsics does not invalidate the others.
 template <class Body>
-static int run_graphed(fp_ctx* c, int kind, int N, int iters, cudaStream_t st, Body body, int cameras = 0,
+static int run_graphed(fp_ctx* c, GraphKind kind, int N, int iters, cudaStream_t st, Body body, int cameras = 0,
                        bool frame_by_value = true) {
   if (!c->use_graphs || g_prof_on) return body(st);
-  const auto key = std::make_tuple(kind, N, iters, cameras);
+  const auto key = std::make_tuple(static_cast<int>(kind), N, iters, cameras);
   auto it = c->graphs.find(key);
   if (it == c->graphs.end()) {
     c->graphs[key] = fp_ctx::GraphEntry();  // seen once: next call captures
@@ -646,18 +680,11 @@ static int refine_body(fp_ctx* c, int N, int iterations, cudaStream_t s2, const 
   return 0;
 }
 
-// pinned host staging of the frame of fp_track / fp_track_objects
+// pinned host staging of the context's frame (fp_track, fp_track_objects, fp_track_cameras' camera 0,
+// fp_register_objects).  No graph holds these addresses: upload_staged_frame copies out of them ahead of the launch.
 static int alloc_frame_staging(fp_ctx* c, size_t npix) {
-  if (c->stage_npix >= npix) return 0;
-  if (c->stage_rgb) cudaFreeHost(c->stage_rgb);
-  if (c->stage_depth) cudaFreeHost(c->stage_depth);
-  c->stage_rgb = c->stage_depth = nullptr;
-  c->stage_npix = 0;
-  FP_CUDA_OK(cudaMallocHost(&c->stage_rgb, npix * 3));
-  FP_CUDA_OK(cudaMallocHost(&c->stage_depth, npix * 4));
-  c->stage_npix = npix;
-  ++c->epoch;  // the graph's copy nodes hold these addresses
-  return 0;
+  FP_TRY(pinned_alloc(nullptr, c->stage_rgb, npix * 3));
+  return pinned_alloc(nullptr, c->stage_depth, npix * 4);
 }
 
 // The previous frame's graph has finished (every caller synchronises), so the staging buffers are free.  The two
@@ -674,7 +701,7 @@ static int upload_staged_frame(void* stage_rgb, void* stage_depth, void* rgb_dev
 }
 static int upload_staged_frame(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, size_t npix,
                                cudaStream_t st) {
-  return upload_staged_frame(c->stage_rgb, c->stage_depth, c->rgb_raw.p, c->depth_raw.p, rgb_host, depth_host, npix, st);
+  return upload_staged_frame(c->stage_rgb.p, c->stage_depth.p, c->rgb_raw.p, c->depth_raw.p, rgb_host, depth_host, npix, st);
 }
 
 // fp_track_cameras and fp_track_objects after validation.  Camera 0 is the context's frame (buffers, staging, K / H / W),
@@ -717,42 +744,22 @@ static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_
     FP_TRY(dev_alloc(table_only, b.rgba, npix_max * 4));
     FP_TRY(dev_alloc(table_only, b.depth, npix_max * 4));
     FP_TRY(dev_alloc(table_only, b.xyz, npix_max * 16));
-    if (b.stage_npix < npix_max) {
-      if (b.stage_rgb) cudaFreeHost(b.stage_rgb);
-      if (b.stage_depth) cudaFreeHost(b.stage_depth);
-      b.stage_rgb = b.stage_depth = nullptr;
-      b.stage_npix = 0;
-      FP_CUDA_OK(cudaMallocHost(&b.stage_rgb, npix_max * 3));
-      FP_CUDA_OK(cudaMallocHost(&b.stage_depth, npix_max * 4));
-      b.stage_npix = npix_max;
-    }
+    FP_TRY(pinned_alloc(nullptr, b.stage_rgb, npix_max * 3));
+    FP_TRY(pinned_alloc(nullptr, b.stage_depth, npix_max * 4));
   }
   const size_t table_bytes = sizeof(CameraDev) * kMaxCameras;
   const size_t args_bytes = table_bytes + (size_t)2 * M * sizeof(int);
   FP_TRY(dev_alloc(c->epoch, c->cam_args, args_bytes));
-  if (c->stage_args_n < args_bytes) {
-    if (c->stage_args) cudaFreeHost(c->stage_args);
-    c->stage_args = nullptr;
-    c->stage_args_n = 0;
-    FP_CUDA_OK(cudaMallocHost(&c->stage_args, args_bytes));
-    c->stage_args_n = args_bytes;
-  }
-  if (c->stage_poses_n < M) {
-    if (c->stage_poses) cudaFreeHost(c->stage_poses);
-    c->stage_poses = nullptr;
-    c->stage_poses_n = 0;
-    FP_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&c->stage_poses), (size_t)M * 64));
-    c->stage_poses_n = M;
-    ++c->epoch;  // the graph's read-back node holds this address
-  }
+  FP_TRY(pinned_alloc(nullptr, c->stage_args, args_bytes));
+  FP_TRY(pinned_alloc(&c->epoch, c->stage_poses, (size_t)M * 64));  // the graph's read-back node holds this address
   // the per-call arguments: one staged block, one copy
-  int* ints = reinterpret_cast<int*>(reinterpret_cast<char*>(c->stage_args) + table_bytes);
+  int* ints = reinterpret_cast<int*>(reinterpret_cast<char*>(c->stage_args.p) + table_bytes);
   memcpy(ints, slots_host, (size_t)M * sizeof(int));
   if (by_value) {
     FP_CUDA_OK(cudaMemcpyAsync(reinterpret_cast<char*>(c->cam_args.p) + table_bytes, ints, (size_t)M * sizeof(int),
                                cudaMemcpyHostToDevice, st));
   } else {
-    CameraDev* table = reinterpret_cast<CameraDev*>(c->stage_args);
+    CameraDev* table = reinterpret_cast<CameraDev*>(c->stage_args.p);
     memset(table, 0, table_bytes);
     for (int i = 0; i < C; ++i) {
       CameraDev& e = table[i];
@@ -769,7 +776,7 @@ static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_
       e.W = W[i];
     }
     memcpy(ints + M, camera_of, (size_t)M * sizeof(int));
-    FP_CUDA_OK(cudaMemcpyAsync(c->cam_args.p, c->stage_args, args_bytes, cudaMemcpyHostToDevice, st));
+    FP_CUDA_OK(cudaMemcpyAsync(c->cam_args.p, c->stage_args.p, args_bytes, cudaMemcpyHostToDevice, st));
   }
   const CameraDev* cams_dev = by_value ? nullptr : reinterpret_cast<const CameraDev*>(c->cam_args.p);
   const int* mesh_of = reinterpret_cast<const int*>(reinterpret_cast<const char*>(c->cam_args.p) + table_bytes);
@@ -784,7 +791,7 @@ static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_
       FP_TRY(upload_staged_frame(c, rgb_host[0], depth_host[0], npix, st));
     } else {
       CameraBufs& b = c->cams[i];
-      FP_TRY(upload_staged_frame(b.stage_rgb, b.stage_depth, b.rgb_raw.p, b.depth_raw.p, rgb_host[i], depth_host[i], npix, st));
+      FP_TRY(upload_staged_frame(b.stage_rgb.p, b.stage_depth.p, b.rgb_raw.p, b.depth_raw.p, rgb_host[i], depth_host[i], npix, st));
     }
   }
   c->has_frame = false;
@@ -802,19 +809,48 @@ static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_
     }
     c->has_frame = true;
     FP_TRY(refine_body(c, M, iterations, s2, mesh_of, cams_dev, cam_of));
-    FP_CUDA_OK(cudaMemcpyAsync(c->stage_poses, fin, (size_t)M * 64, cudaMemcpyDeviceToHost, s2));
+    FP_CUDA_OK(cudaMemcpyAsync(c->stage_poses.p, fin, (size_t)M * 64, cudaMemcpyDeviceToHost, s2));
     return 0;
   };
   if (by_value) {
-    FP_TRY(run_graphed(c, 3, M, iterations, st, body));
+    FP_TRY(run_graphed(c, GraphKind::TrackObjects, M, iterations, st, body));
   } else {
-    FP_TRY(run_graphed(c, 6, M, iterations, st, body, C, /*frame_by_value=*/false));
+    FP_TRY(run_graphed(c, GraphKind::TrackCameras, M, iterations, st, body, C, /*frame_by_value=*/false));
   }
   c->has_frame = true;
   if (poses_out_dev) FP_CUDA_OK(cudaMemcpyAsync(poses_out_dev, fin, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
   FP_CUDA_OK(cudaStreamSynchronize(st));
-  if (poses_out_host) memcpy(poses_out_host, c->stage_poses, (size_t)M * 64);
+  if (poses_out_host) memcpy(poses_out_host, c->stage_poses.p, (size_t)M * 64);
   return 0;
+}
+
+// The mesh slot of each of `M` objects.  The kernels index the mesh table with these ids unchecked, so an empty or
+// out-of-range slot must be refused before anything is enqueued.
+static int check_slots(const fp_ctx* c, int M, const int* slots, const char* caller) {
+  for (int i = 0; i < M; ++i) {
+    FP_REQUIRE(slots[i] >= 0 && slots[i] < kMaxMeshes, "%s: object %d: slot %d out of range [0, %d)", caller, i, slots[i],
+               kMaxMeshes);
+    FP_REQUIRE(c->mesh[slots[i]].loaded, "%s: object %d: slot %d holds no mesh", caller, i, slots[i]);
+  }
+  return 0;
+}
+
+// The scorer tail over `L` feature rows as one segment; a segmented launch sets seg / n_seg / seg_max on top.
+static ScoreTailParams score_tail_params(const fp_ctx* c, const float* feats, int L, float* scores, int* best) {
+  const Net& net = c->net[1];
+  ScoreTailParams p;
+  p.feats = feats;
+  p.L = L;
+  p.w_in = net.f("cross.in_w");
+  p.b_in = net.f("cross.in_b");
+  p.fold_v = reinterpret_cast<const float*>(c->fold_v.p);
+  p.fold_c = c->fold_c;
+  p.offset = 100.f;
+  p.qkv = reinterpret_cast<float*>(c->tail_qkv.p);
+  p.scores = scores;
+  p.best = best;
+  p.counter = reinterpret_cast<unsigned int*>(c->tail_counter.p);
+  return p;
 }
 
 }  // namespace fp
@@ -865,39 +901,13 @@ int fp_destroy(fp_ctx* c) {
   if (!c) return 0;
   DeviceGuard dg(c->device);
   cudaDeviceSynchronize();
-  for (auto& net : c->net)
-    for (auto& kv : net.t) cudaFree(kv.second.p);
-  for (MeshSlot& m : c->mesh)
-    for (DevBuf* b : {&m.vpos, &m.vnrm, &m.vatt, &m.faces, &m.meshlets, &m.ml_verts, &m.ml_tris, &m.tex})
-      if (b->p) cudaFree(b->p);
-  DevBuf* bufs[] = {&c->mesh_table, &c->mesh_of, &c->rgb_raw, &c->rgba, &c->depth_raw, &c->depth_a, &c->depth_b, &c->xyz, &c->crops, &c->act0, &c->a1, &c->a2,
-                    &c->a3, &c->ab0, &c->ab1, &c->ab2, &c->c0, &c->c1, &c->c2, &c->tok, &c->qkv, &c->att, &c->x1pre,
-                    &c->x1, &c->ff, &c->x2pre, &c->head_out, &c->poses_a, &c->poses_b, &c->feats, &c->tail_qkv,
-                    &c->tail_attn, &c->tail_proj, &c->scores, &c->best, &c->lt_buf, &c->lr_buf, &c->feat_buf,
-                    &c->pose_stage, &c->mask_buf, &c->mask_stats, &c->crop_stats, &c->track_pose, &c->fold_v, &c->tail_counter, &c->tok_mean,
-                    &c->seg_off, &c->reg_feats, &c->cam_args};
-  for (DevBuf* b : bufs)
-    if (b->p) cudaFree(b->p);
-  for (CameraBufs& cb : c->cams) {
-    for (DevBuf* b : {&cb.rgb_raw, &cb.depth_raw, &cb.rgba, &cb.depth, &cb.xyz})
-      if (b->p) cudaFree(b->p);
-    if (cb.stage_rgb) cudaFreeHost(cb.stage_rgb);
-    if (cb.stage_depth) cudaFreeHost(cb.stage_depth);
-  }
   for (auto& kv : c->graphs)
     if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   if (c->cap_stream) cudaStreamDestroy(c->cap_stream);
   if (c->side_stream) cudaStreamDestroy(c->side_stream);
   if (c->ev_fork) cudaEventDestroy(c->ev_fork);
   if (c->ev_join) cudaEventDestroy(c->ev_join);
-  if (c->stage_rgb) cudaFreeHost(c->stage_rgb);
-  if (c->stage_depth) cudaFreeHost(c->stage_depth);
-  if (c->stage_pose) cudaFreeHost(c->stage_pose);
-  if (c->stage_poses) cudaFreeHost(c->stage_poses);
-  if (c->stage_masks) cudaFreeHost(c->stage_masks);
-  if (c->stage_ints) cudaFreeHost(c->stage_ints);
-  if (c->stage_args) cudaFreeHost(c->stage_args);
-  delete c;
+  delete c;  // the buffers free themselves, with the context's device current
   return 0;
   FP_API_END
 }
@@ -924,7 +934,6 @@ int fp_load_network(fp_ctx* c, int which, const fp_tensor_t* tensors, int n) {
   Net& net = c->net[which];
   ++c->epoch;
   FP_CUDA_OK(cudaDeviceSynchronize());
-  for (auto& kv : net.t) cudaFree(kv.second.p);
   net.t.clear();
   net.loaded = false;
   for (int i = 0; i < n; ++i) {
@@ -934,11 +943,9 @@ int fp_load_network(fp_ctx* c, int which, const fp_tensor_t* tensors, int n) {
     d.dtype = t.dtype;
     d.numel = t.numel;
     const size_t bytes = (size_t)t.numel * (t.dtype == 1 ? 2 : 4);
-    FP_CUDA_OK(cudaMalloc(&d.p, bytes));
-    FP_CUDA_OK(cudaMemcpy(d.p, t.data, bytes, cudaMemcpyHostToDevice));
-    auto old = net.t.find(t.name);
-    if (old != net.t.end()) cudaFree(old->second.p);
-    net.t[t.name] = d;
+    FP_TRY(dev_alloc(c->epoch, d.buf, bytes));
+    FP_CUDA_OK(cudaMemcpy(d.buf.p, t.data, bytes, cudaMemcpyHostToDevice));
+    net.t[t.name] = std::move(d);  // a repeated name frees the earlier tensor
   }
   // verify that everything the execution plan needs is present, with the right size
   std::vector<std::pair<std::string, long long>> need;
@@ -1246,7 +1253,8 @@ int fp_refine(fp_ctx* c, const float* poses_in, int N, int iterations, float* po
   float* pa = reinterpret_cast<float*>(c->poses_a.p);
   float* pb = reinterpret_cast<float*>(c->poses_b.p);
   FP_CUDA_OK(cudaMemcpyAsync(pa, poses_in, (size_t)N * 64, cudaMemcpyDeviceToDevice, st));
-  FP_TRY(run_graphed(c, 0, N, iterations, st, [&](cudaStream_t s2) -> int { return refine_body(c, N, iterations, s2); }));
+  FP_TRY(run_graphed(c, GraphKind::Refine, N, iterations, st,
+                     [&](cudaStream_t s2) -> int { return refine_body(c, N, iterations, s2); }));
   const float* fin = (iterations % 2 == 0) ? pa : pb;
   FP_CUDA_OK(cudaMemcpyAsync(poses_out, fin, (size_t)N * 64, cudaMemcpyDeviceToDevice, st));
   if (iterations > 0) {
@@ -1275,7 +1283,7 @@ int fp_score_features(fp_ctx* c, const float* poses, int N, float* feats_out, vo
     FP_TRY(run_score_feats(c, c->net[1], N, fb, s2));
     return 0;
   };
-  FP_TRY(run_graphed(c, 1, N, 0, st, body));
+  FP_TRY(run_graphed(c, GraphKind::ScoreFeatures, N, 0, st, body));
   // feats_out may live on another GPU of the same process (peer access enabled by fp_group_create): the gather of
   // the sharded register is this copy, device to device over NVLink
   FP_CUDA_OK(cudaMemcpyAsync(feats_out, fb, (size_t)N * 2048, cudaMemcpyDefault, st));
@@ -1291,20 +1299,7 @@ int fp_score_tail(fp_ctx* c, const float* feats, int L, float* scores_out, int* 
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (L == 0) return 0;
   FP_TRY(ensure_tail(c, L));
-  const Net& net = c->net[1];
-  ScoreTailParams p;
-  p.feats = feats;
-  p.L = L;
-  p.w_in = net.f("cross.in_w");
-  p.b_in = net.f("cross.in_b");
-  p.fold_v = reinterpret_cast<const float*>(c->fold_v.p);
-  p.fold_c = c->fold_c;
-  p.offset = 100.f;
-  p.qkv = reinterpret_cast<float*>(c->tail_qkv.p);
-  p.scores = scores_out;
-  p.best = best_out;
-  p.counter = reinterpret_cast<unsigned int*>(c->tail_counter.p);
-  return score_tail_launch(p, st);
+  return score_tail_launch(score_tail_params(c, feats, L, scores_out, best_out), st);
   FP_API_END
 }
 
@@ -1356,7 +1351,7 @@ int fp_track(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, 
   FP_TRY(prepare_frame(c, K, H, W, true));
   FP_TRY(dev_alloc(c->epoch, c->track_pose, 64));
   FP_TRY(alloc_frame_staging(c, (size_t)H * W));
-  if (!c->stage_pose) FP_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&c->stage_pose), 64));
+  FP_TRY(pinned_alloc(&c->epoch, c->stage_pose, 64));  // the graph's read-back node holds this address
   if (pose_in_dev) {
     FP_CUDA_OK(cudaMemcpyAsync(c->track_pose.p, pose_in_dev, 64, cudaMemcpyDeviceToDevice, st));
   } else {
@@ -1375,15 +1370,15 @@ int fp_track(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, 
     FP_TRY(refine_body(c, 1, iterations, s2));
     const float* fin = (iterations % 2 == 0) ? pa : pb;
     FP_CUDA_OK(cudaMemcpyAsync(c->track_pose.p, fin, 64, cudaMemcpyDeviceToDevice, s2));
-    FP_CUDA_OK(cudaMemcpyAsync(c->stage_pose, fin, 64, cudaMemcpyDeviceToHost, s2));
+    FP_CUDA_OK(cudaMemcpyAsync(c->stage_pose.p, fin, 64, cudaMemcpyDeviceToHost, s2));
     return 0;
   };
-  FP_TRY(run_graphed(c, 2, 1, iterations, st, body));
+  FP_TRY(run_graphed(c, GraphKind::Track, 1, iterations, st, body));
   c->has_frame = true;
   c->track_valid = true;
   if (pose_out_dev) FP_CUDA_OK(cudaMemcpyAsync(pose_out_dev, c->track_pose.p, 64, cudaMemcpyDeviceToDevice, st));
   FP_CUDA_OK(cudaStreamSynchronize(st));
-  if (pose_out_host) memcpy(pose_out_host, c->stage_pose, 64);
+  if (pose_out_host) memcpy(pose_out_host, c->stage_pose.p, 64);
   return 0;
   FP_API_END
 }
@@ -1395,12 +1390,7 @@ int fp_track_objects(fp_ctx* c, const unsigned char* rgb_host, const float* dept
   FP_REQUIRE(c && rgb_host && depth_host && K && H > 0 && W > 0 && M > 0 && slots_host && poses_in_dev && iterations >= 0,
              "fp_track_objects: bad argument");
   FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
-  // the kernels index the mesh table with these ids unchecked: an empty slot must never reach them
-  for (int i = 0; i < M; ++i) {
-    FP_REQUIRE(slots_host[i] >= 0 && slots_host[i] < kMaxMeshes, "fp_track_objects: object %d: slot %d out of range [0, %d)", i,
-               slots_host[i], kMaxMeshes);
-    FP_REQUIRE(c->mesh[slots_host[i]].loaded, "fp_track_objects: object %d: slot %d holds no mesh", i, slots_host[i]);
-  }
+  FP_TRY(check_slots(c, M, slots_host, "fp_track_objects"));
   DeviceGuard dg(c->device);
   const std::vector<int> camera_of(M, 0);
   return track_cameras_body(c, 1, &rgb_host, &depth_host, K, &H, &W, M, camera_of.data(), slots_host, poses_in_dev, iterations,
@@ -1425,12 +1415,10 @@ int fp_track_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host, con
   for (int i = 0; i < M; ++i) {
     FP_REQUIRE(camera_of[i] >= 0 && camera_of[i] < C, "fp_track_cameras: object %d: camera %d out of range [0, %d)", i,
                camera_of[i], C);
-    FP_REQUIRE(slots_host[i] >= 0 && slots_host[i] < kMaxMeshes, "fp_track_cameras: object %d: slot %d out of range [0, %d)", i,
-               slots_host[i], kMaxMeshes);
-    FP_REQUIRE(c->mesh[slots_host[i]].loaded, "fp_track_cameras: object %d: slot %d holds no mesh", i, slots_host[i]);
     owns[camera_of[i]] = 1;
   }
   for (int i = 0; i < C; ++i) FP_REQUIRE(owns[i], "fp_track_cameras: camera %d owns no object", i);
+  FP_TRY(check_slots(c, M, slots_host, "fp_track_cameras"));
   DeviceGuard dg(c->device);
   return track_cameras_body(c, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, poses_in_dev, iterations,
                             poses_out_dev, poses_out_host, reinterpret_cast<cudaStream_t>(stream), /*by_value=*/false);
@@ -1448,13 +1436,11 @@ int fp_register_objects(fp_ctx* c, const unsigned char* rgb_host, const float* d
              "fp_register_objects: bad argument");
   FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
   FP_REQUIRE(c->net[1].loaded, "scorer weights not loaded");
-  // everything is checked before anything is enqueued: the kernels index the mesh table with these ids unchecked
+  // everything is checked before anything is enqueued
+  FP_TRY(check_slots(c, M, slots_host, "fp_register_objects"));
   std::vector<int> off(M + 1, 0);
   int seg_max = 0;
   for (int i = 0; i < M; ++i) {
-    FP_REQUIRE(slots_host[i] >= 0 && slots_host[i] < kMaxMeshes, "fp_register_objects: object %d: slot %d out of range [0, %d)",
-               i, slots_host[i], kMaxMeshes);
-    FP_REQUIRE(c->mesh[slots_host[i]].loaded, "fp_register_objects: object %d: slot %d holds no mesh", i, slots_host[i]);
     FP_REQUIRE(n_hyp_host[i] >= 1 && n_hyp_host[i] <= 4096, "fp_register_objects: object %d: %d hypotheses, need 1..4096", i,
                n_hyp_host[i]);
     off[i + 1] = off[i] + n_hyp_host[i];
@@ -1483,26 +1469,15 @@ int fp_register_objects(fp_ctx* c, const unsigned char* rgb_host, const float* d
   FP_TRY(dev_alloc(c->epoch, c->mask_stats, (size_t)M * 6 * sizeof(unsigned int)));
   FP_TRY(dev_alloc(c->epoch, c->tail_counter, std::max<size_t>(16, (size_t)M * sizeof(unsigned int)), /*zero=*/true));
   // pinned staging (never read by a captured graph): the copies below leave as soon as they are enqueued
-  if (c->stage_masks_n < (size_t)M * npix) {
-    if (c->stage_masks) cudaFreeHost(c->stage_masks);
-    c->stage_masks = nullptr;
-    c->stage_masks_n = 0;
-    FP_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&c->stage_masks), (size_t)M * npix));
-    c->stage_masks_n = (size_t)M * npix;
-  }
-  if (c->stage_ints_n < (size_t)(M + 1 + total)) {
-    if (c->stage_ints) cudaFreeHost(c->stage_ints);
-    c->stage_ints = nullptr;
-    c->stage_ints_n = 0;
-    FP_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&c->stage_ints), (size_t)(M + 1 + total) * sizeof(int)));
-    c->stage_ints_n = (size_t)(M + 1 + total);
-  }
-  int* slot_of = c->stage_ints + M + 1;  // slot id of every hypothesis
-  memcpy(c->stage_ints, off.data(), (size_t)(M + 1) * sizeof(int));
+  FP_TRY(pinned_alloc(nullptr, c->stage_masks, (size_t)M * npix));
+  FP_TRY(pinned_alloc(nullptr, c->stage_ints, (size_t)(M + 1 + total) * sizeof(int)));
+  int* ints = reinterpret_cast<int*>(c->stage_ints.p);
+  int* slot_of = ints + M + 1;  // slot id of every hypothesis
+  memcpy(ints, off.data(), (size_t)(M + 1) * sizeof(int));
   for (int i = 0; i < M; ++i) std::fill(slot_of + off[i], slot_of + off[i + 1], slots_host[i]);
-  memcpy(c->stage_masks, masks_host, (size_t)M * npix);
-  FP_CUDA_OK(cudaMemcpyAsync(c->seg_off.p, c->stage_ints, (size_t)(M + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
-  FP_CUDA_OK(cudaMemcpyAsync(c->mask_buf.p, c->stage_masks, (size_t)M * npix, cudaMemcpyHostToDevice, st));
+  memcpy(c->stage_masks.p, masks_host, (size_t)M * npix);
+  FP_CUDA_OK(cudaMemcpyAsync(c->seg_off.p, ints, (size_t)(M + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
+  FP_CUDA_OK(cudaMemcpyAsync(c->mask_buf.p, c->stage_masks.p, (size_t)M * npix, cudaMemcpyHostToDevice, st));
   FP_TRY(upload_staged_frame(c, rgb_host, depth_host, npix, st));
   // estimater.py:173-174, :214 once for every object: erode + bilateral, depth2xyzmap(zfar = inf)
   c->has_frame = false;
@@ -1527,10 +1502,11 @@ int fp_register_objects(fp_ctx* c, const unsigned char* rgb_host, const float* d
     // the graphs hold no per-pass address and are keyed on (kind, n, iterations) alone
     FP_CUDA_OK(cudaMemcpyAsync(c->mesh_of.p, slot_of + row0, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
     FP_CUDA_OK(cudaMemcpyAsync(pa, poses_out_dev + (size_t)row0 * 16, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
-    FP_TRY(run_graphed(c, 4, n, iterations, st, [&](cudaStream_t s2) -> int { return refine_body(c, n, iterations, s2, mesh_of); }));
+    FP_TRY(run_graphed(c, GraphKind::RegisterRefine, n, iterations, st,
+                       [&](cudaStream_t s2) -> int { return refine_body(c, n, iterations, s2, mesh_of); }));
     FP_CUDA_OK(cudaMemcpyAsync(poses_out_dev + (size_t)row0 * 16, fin, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
     FP_CUDA_OK(cudaMemcpyAsync(ps, fin, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
-    FP_TRY(run_graphed(c, 5, n, 0, st, [&](cudaStream_t s2) -> int {
+    FP_TRY(run_graphed(c, GraphKind::RegisterFeatures, n, 0, st, [&](cudaStream_t s2) -> int {
       FP_TRY(make_crops(c, ps, n, 1, nullptr, nullptr, nullptr, s2, mesh_of));
       FP_TRY(run_encoder(c, c->net[1], reinterpret_cast<const __half*>(c->crops.p), n, s2));
       return run_score_feats(c, c->net[1], n, fb, s2);
@@ -1539,19 +1515,7 @@ int fp_register_objects(fp_ctx* c, const unsigned char* rgb_host, const float* d
                                cudaMemcpyDeviceToDevice, st));
   }
   // score_network.py:84-88 per object: one tail launch, each object's hypotheses attending only to each other
-  const Net& net = c->net[1];
-  ScoreTailParams tp;
-  tp.feats = reinterpret_cast<const float*>(c->reg_feats.p);
-  tp.L = total;
-  tp.w_in = net.f("cross.in_w");
-  tp.b_in = net.f("cross.in_b");
-  tp.fold_v = reinterpret_cast<const float*>(c->fold_v.p);
-  tp.fold_c = c->fold_c;
-  tp.offset = 100.f;
-  tp.qkv = reinterpret_cast<float*>(c->tail_qkv.p);
-  tp.scores = scores_out_dev;
-  tp.best = best_out_dev;
-  tp.counter = reinterpret_cast<unsigned int*>(c->tail_counter.p);
+  ScoreTailParams tp = score_tail_params(c, reinterpret_cast<const float*>(c->reg_feats.p), total, scores_out_dev, best_out_dev);
   tp.seg = seg;
   tp.n_seg = M;
   tp.seg_max = seg_max;
@@ -1592,16 +1556,24 @@ int fp_op_pose_update(const float* poses_in, const float* trans, const float* ro
 // collective library); device 0 waits on one event per peer and runs the cross-hypothesis tail once.
 // ------------------------------------------------------------------------------------------------
 struct fp_group {
-  std::vector<fp_ctx*> ctx;
-  std::vector<cudaStream_t> stream;
-  std::vector<cudaEvent_t> done;
-  std::vector<fp::DevBuf> grid, start, info, refined;  // per device: rot grid [N][16], start poses, info[4], refined slice
-  fp::DevBuf feats_all, poses_all, scores, best;       // on device 0
-  void* pin_rgb = nullptr;
-  void* pin_depth = nullptr;
-  void* pin_mask = nullptr;
-  void* pin_grid = nullptr;
-  size_t pin_npix = 0, pin_grid_n = 0;
+  // One device's share: its context, stream and completion event, and register()'s buffers there (rot grid [N][16],
+  // start poses, info[4], refined slice).  Destroyed with its device current.
+  struct Device {
+    fp_ctx* ctx = nullptr;
+    cudaStream_t stream = nullptr;
+    cudaEvent_t done = nullptr;
+    fp::DevBuf grid, start, info, refined;
+    ~Device() {
+      if (stream) cudaStreamDestroy(stream);
+      if (done) cudaEventDestroy(done);
+      fp_destroy(ctx);
+    }
+  };
+  std::vector<std::unique_ptr<Device>> dev;
+  struct Gather {
+    fp::DevBuf feats_all, poses_all, scores, best;
+  } gather;  // on device 0
+  fp::PinnedBuf pin_rgb, pin_depth, pin_mask, pin_grid;  // portable: every device reads them
   unsigned long long epoch = 0;
 };
 
@@ -1610,20 +1582,12 @@ extern "C" {
 int fp_group_destroy(fp_group* g) {
   FP_API_BEGIN
   if (!g) return 0;
-  for (size_t i = 0; i < g->ctx.size(); ++i) {
-    DeviceGuard dg(g->ctx[i]->device);
+  for (size_t i = 0; i < g->dev.size(); ++i) {
+    DeviceGuard dg(g->dev[i]->ctx->device);
     cudaDeviceSynchronize();
-    for (fp::DevBuf* b : {&g->grid[i], &g->start[i], &g->info[i], &g->refined[i]})
-      if (b->p) cudaFree(b->p);
-    if (i == 0)
-      for (fp::DevBuf* b : {&g->feats_all, &g->poses_all, &g->scores, &g->best})
-        if (b->p) cudaFree(b->p);
-    if (g->stream[i]) cudaStreamDestroy(g->stream[i]);
-    if (g->done[i]) cudaEventDestroy(g->done[i]);
-    fp_destroy(g->ctx[i]);
+    if (i == 0) g->gather = fp_group::Gather();
+    g->dev[i].reset();
   }
-  for (void* p : {g->pin_rgb, g->pin_depth, g->pin_mask, g->pin_grid})
-    if (p) cudaFreeHost(p);
   delete g;
   return 0;
   FP_API_END
@@ -1653,25 +1617,20 @@ int fp_group_create(int ndev, const int* dev_ids, fp_group** out) {
       cudaSetDevice(prev);
       return rc;
     }
-    cudaStream_t s = nullptr;
-    cudaEvent_t e = nullptr;
-    cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
-    cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
-    g->ctx.push_back(c);
-    g->stream.push_back(s);
-    g->done.push_back(e);
-    g->grid.emplace_back();
-    g->start.emplace_back();
-    g->info.emplace_back();
-    g->refined.emplace_back();
+    auto d = std::make_unique<fp_group::Device>();
+    d->ctx = c;
+    cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking);
+    cudaEventCreateWithFlags(&d->done, cudaEventDisableTiming);
+    g->dev.push_back(std::move(d));
     if (i > 0) {
       // peers write their feature rows into device 0's buffer: map device 0's memory into this device
+      const int dev0 = g->dev[0]->ctx->device;
       int can = 0;
-      cudaDeviceCanAccessPeer(&can, dev, g->ctx[0]->device);
+      cudaDeviceCanAccessPeer(&can, dev, dev0);
       if (can) {
-        const cudaError_t pe = cudaDeviceEnablePeerAccess(g->ctx[0]->device, 0);
+        const cudaError_t pe = cudaDeviceEnablePeerAccess(dev0, 0);
         if (pe != cudaSuccess && pe != cudaErrorPeerAccessAlreadyEnabled) {
-          set_last_error("fp_group_create: cudaDeviceEnablePeerAccess(%d -> %d): %s", dev, g->ctx[0]->device, cudaGetErrorString(pe));
+          set_last_error("fp_group_create: cudaDeviceEnablePeerAccess(%d -> %d): %s", dev, dev0, cudaGetErrorString(pe));
           fp_group_destroy(g);
           cudaSetDevice(prev);
           return -2;
@@ -1686,14 +1645,14 @@ int fp_group_create(int ndev, const int* dev_ids, fp_group** out) {
   FP_API_END
 }
 
-int fp_group_size(fp_group* g) { return g ? (int)g->ctx.size() : 0; }
+int fp_group_size(fp_group* g) { return g ? (int)g->dev.size() : 0; }
 
-fp_ctx* fp_group_ctx(fp_group* g, int i) { return (g && i >= 0 && i < (int)g->ctx.size()) ? g->ctx[i] : nullptr; }
+fp_ctx* fp_group_ctx(fp_group* g, int i) { return (g && i >= 0 && i < (int)g->dev.size()) ? g->dev[i]->ctx : nullptr; }
 
 int fp_group_load_network(fp_group* g, int which, const fp_tensor_t* tensors, int n) {
   FP_API_BEGIN
   FP_REQUIRE(g, "fp_group_load_network: null group");
-  for (fp_ctx* c : g->ctx) FP_TRY(fp_load_network(c, which, tensors, n));
+  for (auto& d : g->dev) FP_TRY(fp_load_network(d->ctx, which, tensors, n));
   return 0;
   FP_API_END
 }
@@ -1701,7 +1660,7 @@ int fp_group_load_network(fp_group* g, int which, const fp_tensor_t* tensors, in
 int fp_group_set_config(fp_group* g, int which, float crop_ratio, float rot_normalizer) {
   FP_API_BEGIN
   FP_REQUIRE(g, "fp_group_set_config: null group");
-  for (fp_ctx* c : g->ctx) FP_TRY(fp_set_config(c, which, crop_ratio, rot_normalizer));
+  for (auto& d : g->dev) FP_TRY(fp_set_config(d->ctx, which, crop_ratio, rot_normalizer));
   return 0;
   FP_API_END
 }
@@ -1710,7 +1669,7 @@ int fp_group_set_mesh(fp_group* g, int V, int F, const float* pos, const float* 
                       const int* faces, const unsigned char* tex_rgb, int Ht, int Wt, float diameter) {
   FP_API_BEGIN
   FP_REQUIRE(g, "fp_group_set_mesh: null group");
-  for (fp_ctx* c : g->ctx) FP_TRY(fp_set_mesh(c, V, F, pos, nrm, uv, vcol, faces, tex_rgb, Ht, Wt, diameter));
+  for (auto& d : g->dev) FP_TRY(fp_set_mesh(d->ctx, V, F, pos, nrm, uv, vcol, faces, tex_rgb, Ht, Wt, diameter));
   return 0;
   FP_API_END
 }
@@ -1722,75 +1681,63 @@ int fp_group_register(fp_group* g, const unsigned char* rgb_host, const float* d
   FP_REQUIRE(g && rgb_host && depth_host && K && mask_host && rot_grid_host && poses_out_host && scores_out_host &&
                  best_out_host && N > 0 && H > 0 && W > 0,
              "fp_group_register: bad argument");
-  const int G = (int)g->ctx.size();
+  const int G = (int)g->dev.size();
   const size_t npix = (size_t)H * W;
   // pinned staging, filled once, read by every device
-  if (g->pin_npix < npix) {
-    for (void** p : {&g->pin_rgb, &g->pin_depth, &g->pin_mask}) {
-      if (*p) cudaFreeHost(*p);
-      *p = nullptr;
-    }
-    g->pin_npix = 0;
-    FP_CUDA_OK(cudaHostAlloc(&g->pin_rgb, npix * 3, cudaHostAllocPortable));
-    FP_CUDA_OK(cudaHostAlloc(&g->pin_depth, npix * 4, cudaHostAllocPortable));
-    FP_CUDA_OK(cudaHostAlloc(&g->pin_mask, npix, cudaHostAllocPortable));
-    g->pin_npix = npix;
-  }
-  if (g->pin_grid_n < (size_t)N) {
-    if (g->pin_grid) cudaFreeHost(g->pin_grid);
-    g->pin_grid = nullptr;
-    g->pin_grid_n = 0;
-    FP_CUDA_OK(cudaHostAlloc(&g->pin_grid, (size_t)N * 64, cudaHostAllocPortable));
-    g->pin_grid_n = N;
-  }
-  memcpy(g->pin_rgb, rgb_host, npix * 3);
-  memcpy(g->pin_depth, depth_host, npix * 4);
-  memcpy(g->pin_mask, mask_host, npix);
-  memcpy(g->pin_grid, rot_grid_host, (size_t)N * 64);
-  fp_ctx* c0 = g->ctx[0];
+  FP_TRY(pinned_alloc(nullptr, g->pin_rgb, npix * 3, cudaHostAllocPortable));
+  FP_TRY(pinned_alloc(nullptr, g->pin_depth, npix * 4, cudaHostAllocPortable));
+  FP_TRY(pinned_alloc(nullptr, g->pin_mask, npix, cudaHostAllocPortable));
+  FP_TRY(pinned_alloc(nullptr, g->pin_grid, (size_t)N * 64, cudaHostAllocPortable));
+  memcpy(g->pin_rgb.p, rgb_host, npix * 3);
+  memcpy(g->pin_depth.p, depth_host, npix * 4);
+  memcpy(g->pin_mask.p, mask_host, npix);
+  memcpy(g->pin_grid.p, rot_grid_host, (size_t)N * 64);
+  fp_ctx* c0 = g->dev[0]->ctx;
+  fp_group::Gather& ga = g->gather;
   {
     DeviceGuard dg(c0->device);
-    FP_TRY(dev_alloc(g->epoch, g->feats_all, (size_t)N * 2048));
-    FP_TRY(dev_alloc(g->epoch, g->poses_all, (size_t)N * 64));
-    FP_TRY(dev_alloc(g->epoch, g->scores, (size_t)N * 4));
-    FP_TRY(dev_alloc(g->epoch, g->best, 16));
+    FP_TRY(dev_alloc(g->epoch, ga.feats_all, (size_t)N * 2048));
+    FP_TRY(dev_alloc(g->epoch, ga.poses_all, (size_t)N * 64));
+    FP_TRY(dev_alloc(g->epoch, ga.scores, (size_t)N * 4));
+    FP_TRY(dev_alloc(g->epoch, ga.best, 16));
   }
   const int base = N / G, rem = N % G;
   for (int i = 0; i < G; ++i) {
-    fp_ctx* c = g->ctx[i];
+    fp_group::Device& d = *g->dev[i];
+    fp_ctx* c = d.ctx;
     DeviceGuard dg(c->device);
-    cudaStream_t st = g->stream[i];
+    cudaStream_t st = d.stream;
     const int lo = i * base + (i < rem ? i : rem), n = base + (i < rem ? 1 : 0);
-    FP_TRY(dev_alloc(g->epoch, g->grid[i], (size_t)N * 64));
-    FP_TRY(dev_alloc(g->epoch, g->start[i], (size_t)N * 64));
-    FP_TRY(dev_alloc(g->epoch, g->info[i], 16));
-    FP_TRY(dev_alloc(g->epoch, g->refined[i], (size_t)(n > 0 ? n : 1) * 64));
-    FP_TRY(fp_set_frame(c, reinterpret_cast<const unsigned char*>(g->pin_rgb), reinterpret_cast<const float*>(g->pin_depth),
+    FP_TRY(dev_alloc(g->epoch, d.grid, (size_t)N * 64));
+    FP_TRY(dev_alloc(g->epoch, d.start, (size_t)N * 64));
+    FP_TRY(dev_alloc(g->epoch, d.info, 16));
+    FP_TRY(dev_alloc(g->epoch, d.refined, (size_t)(n > 0 ? n : 1) * 64));
+    FP_TRY(fp_set_frame(c, reinterpret_cast<const unsigned char*>(g->pin_rgb.p), reinterpret_cast<const float*>(g->pin_depth.p),
                         K, H, W, FP_FRAME_FILTER_DEPTH, INFINITY, st));
-    FP_CUDA_OK(cudaMemcpyAsync(g->grid[i].p, g->pin_grid, (size_t)N * 64, cudaMemcpyHostToDevice, st));
-    FP_TRY(fp_start_poses(c, reinterpret_cast<const unsigned char*>(g->pin_mask), 0, reinterpret_cast<const float*>(g->grid[i].p),
-                          N, reinterpret_cast<float*>(g->start[i].p), reinterpret_cast<float*>(g->info[i].p), st));
+    FP_CUDA_OK(cudaMemcpyAsync(d.grid.p, g->pin_grid.p, (size_t)N * 64, cudaMemcpyHostToDevice, st));
+    FP_TRY(fp_start_poses(c, reinterpret_cast<const unsigned char*>(g->pin_mask.p), 0, reinterpret_cast<const float*>(d.grid.p),
+                          N, reinterpret_cast<float*>(d.start.p), reinterpret_cast<float*>(d.info.p), st));
     if (n > 0) {
-      float* refined = reinterpret_cast<float*>(g->refined[i].p);
-      FP_TRY(fp_refine(c, reinterpret_cast<const float*>(g->start[i].p) + (size_t)lo * 16, n, iterations, refined, nullptr,
+      float* refined = reinterpret_cast<float*>(d.refined.p);
+      FP_TRY(fp_refine(c, reinterpret_cast<const float*>(d.start.p) + (size_t)lo * 16, n, iterations, refined, nullptr,
                        nullptr, st));
       // the gather: feature rows and refined poses land in device 0's buffers, straight over peer memory
-      FP_TRY(fp_score_features(c, refined, n, reinterpret_cast<float*>(g->feats_all.p) + (size_t)lo * 512, st));
-      FP_CUDA_OK(cudaMemcpyAsync(reinterpret_cast<float*>(g->poses_all.p) + (size_t)lo * 16, refined, (size_t)n * 64,
+      FP_TRY(fp_score_features(c, refined, n, reinterpret_cast<float*>(ga.feats_all.p) + (size_t)lo * 512, st));
+      FP_CUDA_OK(cudaMemcpyAsync(reinterpret_cast<float*>(ga.poses_all.p) + (size_t)lo * 16, refined, (size_t)n * 64,
                                  cudaMemcpyDefault, st));
     }
-    FP_CUDA_OK(cudaEventRecord(g->done[i], st));
+    FP_CUDA_OK(cudaEventRecord(d.done, st));
   }
   {
     DeviceGuard dg(c0->device);
-    cudaStream_t s0 = g->stream[0];
-    for (int i = 1; i < G; ++i) FP_CUDA_OK(cudaStreamWaitEvent(s0, g->done[i], 0));
-    FP_TRY(fp_score_tail(c0, reinterpret_cast<const float*>(g->feats_all.p), N, reinterpret_cast<float*>(g->scores.p),
-                         reinterpret_cast<int*>(g->best.p), s0));
-    FP_CUDA_OK(cudaMemcpyAsync(poses_out_host, g->poses_all.p, (size_t)N * 64, cudaMemcpyDeviceToHost, s0));
-    FP_CUDA_OK(cudaMemcpyAsync(scores_out_host, g->scores.p, (size_t)N * 4, cudaMemcpyDeviceToHost, s0));
-    FP_CUDA_OK(cudaMemcpyAsync(best_out_host, g->best.p, 4, cudaMemcpyDeviceToHost, s0));
-    if (info_out_host) FP_CUDA_OK(cudaMemcpyAsync(info_out_host, g->info[0].p, 16, cudaMemcpyDeviceToHost, s0));
+    cudaStream_t s0 = g->dev[0]->stream;
+    for (int i = 1; i < G; ++i) FP_CUDA_OK(cudaStreamWaitEvent(s0, g->dev[i]->done, 0));
+    FP_TRY(fp_score_tail(c0, reinterpret_cast<const float*>(ga.feats_all.p), N, reinterpret_cast<float*>(ga.scores.p),
+                         reinterpret_cast<int*>(ga.best.p), s0));
+    FP_CUDA_OK(cudaMemcpyAsync(poses_out_host, ga.poses_all.p, (size_t)N * 64, cudaMemcpyDeviceToHost, s0));
+    FP_CUDA_OK(cudaMemcpyAsync(scores_out_host, ga.scores.p, (size_t)N * 4, cudaMemcpyDeviceToHost, s0));
+    FP_CUDA_OK(cudaMemcpyAsync(best_out_host, ga.best.p, 4, cudaMemcpyDeviceToHost, s0));
+    if (info_out_host) FP_CUDA_OK(cudaMemcpyAsync(info_out_host, g->dev[0]->info.p, 16, cudaMemcpyDeviceToHost, s0));
     FP_CUDA_OK(cudaStreamSynchronize(s0));
   }
   return 0;
