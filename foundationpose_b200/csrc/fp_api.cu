@@ -192,6 +192,10 @@ struct fp_ctx {
   // of the masks and of (offsets, per-hypothesis slot ids)
   fp::DevBuf seg_off, reg_feats;
   fp::PinnedBuf stage_masks, stage_ints;
+  // fp_register_cameras: the camera table [FP_MAX_CAMERAS] (fixed size, so its address never changes), the camera id of
+  // every hypothesis of a pass, each object's byte offset into mask_buf, and the pinned staging of the table and offsets
+  fp::DevBuf reg_cams, reg_cam_of, mask_off;
+  fp::PinnedBuf stage_cams;
   // fp_track_cameras: buffers of cameras 1..; the per-call arguments (camera table [FP_MAX_CAMERAS], slot ids [M],
   // camera ids [M]) as one device block and its pinned staging; the frame size its frame-preparation grid covers (the
   // largest seen)
@@ -513,6 +517,8 @@ enum class GraphKind {
   RegisterRefine = 4,    // fp_register_objects: one pass's refinement
   RegisterFeatures = 5,  // fp_register_objects: one pass's scorer features
   TrackCameras = 6,      // fp_track_cameras
+  RegisterCamerasRefine = 7,    // fp_register_cameras: one pass's refinement, frames from the camera table
+  RegisterCamerasFeatures = 8,  // fp_register_cameras: one pass's scorer features, frames from the camera table
 };
 
 // Runs `body(stream)` — a fixed sequence of kernel launches (and fixed-address copies) on ctx-owned buffers —
@@ -704,6 +710,57 @@ static int upload_staged_frame(fp_ctx* c, const unsigned char* rgb_host, const f
   return upload_staged_frame(c->stage_rgb.p, c->stage_depth.p, c->rgb_raw.p, c->depth_raw.p, rgb_host, depth_host, npix, st);
 }
 
+// Frame buffers and pinned staging of cameras 1.. of a multi-camera call, at npix_max pixels each (camera 0 is the
+// context's frame, sized by the caller).  Only the camera table holds these addresses: no graph is affected.
+static int alloc_camera_bufs(fp_ctx* c, int C, size_t npix_max) {
+  for (int i = 1; i < C; ++i) {
+    CameraBufs& b = c->cams[i];
+    unsigned long long table_only = 0;
+    FP_TRY(dev_alloc(table_only, b.rgb_raw, npix_max * 3));
+    FP_TRY(dev_alloc(table_only, b.depth_raw, npix_max * 4));
+    FP_TRY(dev_alloc(table_only, b.rgba, npix_max * 4));
+    FP_TRY(dev_alloc(table_only, b.depth, npix_max * 4));
+    FP_TRY(dev_alloc(table_only, b.xyz, npix_max * 16));
+    FP_TRY(pinned_alloc(nullptr, b.stage_rgb, npix_max * 3));
+    FP_TRY(pinned_alloc(nullptr, b.stage_depth, npix_max * 4));
+  }
+  return 0;
+}
+
+// The camera table of C cameras (entries C.. zeroed): buffers, size and intrinsics (K: [C][9]) of every camera
+static void fill_camera_table(const fp_ctx* c, int C, const float* K, const int* H, const int* W, CameraDev* table) {
+  memset(table, 0, sizeof(CameraDev) * kMaxCameras);
+  for (int i = 0; i < C; ++i) {
+    CameraDev& e = table[i];
+    e.rgb_raw = reinterpret_cast<const unsigned char*>(i ? c->cams[i].rgb_raw.p : c->rgb_raw.p);
+    e.depth_raw = reinterpret_cast<const float*>(i ? c->cams[i].depth_raw.p : c->depth_raw.p);
+    e.rgb = reinterpret_cast<uchar4*>(i ? c->cams[i].rgba.p : c->rgba.p);
+    e.depth = reinterpret_cast<float*>(i ? c->cams[i].depth.p : c->depth_b.p);
+    e.xyz_map = reinterpret_cast<float4*>(i ? c->cams[i].xyz.p : c->xyz.p);
+    e.fx = K[9 * i + 0];
+    e.fy = K[9 * i + 4];
+    e.cx = K[9 * i + 2];
+    e.cy = K[9 * i + 5];
+    e.H = H[i];
+    e.W = W[i];
+  }
+}
+
+// Every camera's frame through its own pinned staging; camera i's DMA runs while camera i + 1 is copied on the host
+static int upload_camera_frames(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
+                                const int* H, const int* W, cudaStream_t st) {
+  for (int i = 0; i < C; ++i) {
+    const size_t npix = (size_t)H[i] * W[i];
+    if (i == 0) {
+      FP_TRY(upload_staged_frame(c, rgb_host[0], depth_host[0], npix, st));
+    } else {
+      CameraBufs& b = c->cams[i];
+      FP_TRY(upload_staged_frame(b.stage_rgb.p, b.stage_depth.p, b.rgb_raw.p, b.depth_raw.p, rgb_host[i], depth_host[i], npix, st));
+    }
+  }
+  return 0;
+}
+
 // fp_track_cameras and fp_track_objects after validation.  Camera 0 is the context's frame (buffers, staging, K / H / W),
 // cameras 1.. have buffers of their own.
 //   by_value = false (fp_track_cameras): every camera's buffers are sized for the largest frame of the call, so a
@@ -736,17 +793,7 @@ static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_
     c->cam_grid_h = std::max(c->cam_grid_h, H_max);
     c->cam_grid_w = std::max(c->cam_grid_w, W_max);
   }
-  for (int i = 1; i < C; ++i) {
-    CameraBufs& b = c->cams[i];
-    unsigned long long table_only = 0;  // only the camera table holds these addresses: no graph is affected
-    FP_TRY(dev_alloc(table_only, b.rgb_raw, npix_max * 3));
-    FP_TRY(dev_alloc(table_only, b.depth_raw, npix_max * 4));
-    FP_TRY(dev_alloc(table_only, b.rgba, npix_max * 4));
-    FP_TRY(dev_alloc(table_only, b.depth, npix_max * 4));
-    FP_TRY(dev_alloc(table_only, b.xyz, npix_max * 16));
-    FP_TRY(pinned_alloc(nullptr, b.stage_rgb, npix_max * 3));
-    FP_TRY(pinned_alloc(nullptr, b.stage_depth, npix_max * 4));
-  }
+  FP_TRY(alloc_camera_bufs(c, C, npix_max));
   const size_t table_bytes = sizeof(CameraDev) * kMaxCameras;
   const size_t args_bytes = table_bytes + (size_t)2 * M * sizeof(int);
   FP_TRY(dev_alloc(c->epoch, c->cam_args, args_bytes));
@@ -759,22 +806,7 @@ static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_
     FP_CUDA_OK(cudaMemcpyAsync(reinterpret_cast<char*>(c->cam_args.p) + table_bytes, ints, (size_t)M * sizeof(int),
                                cudaMemcpyHostToDevice, st));
   } else {
-    CameraDev* table = reinterpret_cast<CameraDev*>(c->stage_args.p);
-    memset(table, 0, table_bytes);
-    for (int i = 0; i < C; ++i) {
-      CameraDev& e = table[i];
-      e.rgb_raw = reinterpret_cast<const unsigned char*>(i ? c->cams[i].rgb_raw.p : c->rgb_raw.p);
-      e.depth_raw = reinterpret_cast<const float*>(i ? c->cams[i].depth_raw.p : c->depth_raw.p);
-      e.rgb = reinterpret_cast<uchar4*>(i ? c->cams[i].rgba.p : c->rgba.p);
-      e.depth = reinterpret_cast<float*>(i ? c->cams[i].depth.p : c->depth_b.p);
-      e.xyz_map = reinterpret_cast<float4*>(i ? c->cams[i].xyz.p : c->xyz.p);
-      e.fx = K[9 * i + 0];
-      e.fy = K[9 * i + 4];
-      e.cx = K[9 * i + 2];
-      e.cy = K[9 * i + 5];
-      e.H = H[i];
-      e.W = W[i];
-    }
+    fill_camera_table(c, C, K, H, W, reinterpret_cast<CameraDev*>(c->stage_args.p));
     memcpy(ints + M, camera_of, (size_t)M * sizeof(int));
     FP_CUDA_OK(cudaMemcpyAsync(c->cam_args.p, c->stage_args.p, args_bytes, cudaMemcpyHostToDevice, st));
   }
@@ -784,16 +816,7 @@ static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_
   float* pa = reinterpret_cast<float*>(c->poses_a.p);
   float* pb = reinterpret_cast<float*>(c->poses_b.p);
   FP_CUDA_OK(cudaMemcpyAsync(pa, poses_in_dev, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
-  // camera i's DMA runs while camera i + 1 is copied into its staging on the host
-  for (int i = 0; i < C; ++i) {
-    const size_t npix = (size_t)H[i] * W[i];
-    if (i == 0) {
-      FP_TRY(upload_staged_frame(c, rgb_host[0], depth_host[0], npix, st));
-    } else {
-      CameraBufs& b = c->cams[i];
-      FP_TRY(upload_staged_frame(b.stage_rgb.p, b.stage_depth.p, b.rgb_raw.p, b.depth_raw.p, rgb_host[i], depth_host[i], npix, st));
-    }
-  }
+  FP_TRY(upload_camera_frames(c, C, rgb_host, depth_host, H, W, st));
   c->has_frame = false;
   const float* fin = (iterations % 2 == 0) ? pa : pb;
   const int grid_h = c->cam_grid_h, grid_w = c->cam_grid_w;
@@ -835,6 +858,24 @@ static int check_slots(const fp_ctx* c, int M, const int* slots, const char* cal
   return 0;
 }
 
+// The frames of C cameras and the camera of each of M objects: non-null frames of positive size, every camera id in
+// [0, C) and every camera owning at least one object.  The kernels index the camera table with these ids unchecked.
+static int check_cameras(int C, const unsigned char* const* rgb_host, const float* const* depth_host, const int* H, const int* W,
+                         int M, const int* camera_of, const char* caller) {
+  FP_REQUIRE(C >= 1 && C <= kMaxCameras, "%s: %d cameras, need 1..%d", caller, C, kMaxCameras);
+  for (int i = 0; i < C; ++i) {
+    FP_REQUIRE(rgb_host[i] && depth_host[i], "%s: camera %d: null frame", caller, i);
+    FP_REQUIRE(H[i] > 0 && W[i] > 0, "%s: camera %d: empty frame (%d x %d)", caller, i, H[i], W[i]);
+  }
+  std::vector<int> owns(C, 0);
+  for (int i = 0; i < M; ++i) {
+    FP_REQUIRE(camera_of[i] >= 0 && camera_of[i] < C, "%s: object %d: camera %d out of range [0, %d)", caller, i, camera_of[i], C);
+    owns[camera_of[i]] = 1;
+  }
+  for (int i = 0; i < C; ++i) FP_REQUIRE(owns[i], "%s: camera %d owns no object", caller, i);
+  return 0;
+}
+
 // The scorer tail over `L` feature rows as one segment; a segmented launch sets seg / n_seg / seg_max on top.
 static ScoreTailParams score_tail_params(const fp_ctx* c, const float* feats, int L, float* scores, int* best) {
   const Net& net = c->net[1];
@@ -851,6 +892,162 @@ static ScoreTailParams score_tail_params(const fp_ctx* c, const float* feats, in
   p.best = best;
   p.counter = reinterpret_cast<unsigned int*>(c->tail_counter.p);
   return p;
+}
+
+// fp_register_cameras and fp_register_objects after validation (n_hyp_host is checked here, before anything is
+// enqueued).  Object i is seen by camera camera_of[i]; its mask is masks_host[i], of its camera's size.  Camera 0 is the
+// context's frame, cameras 1.. have buffers of their own (as track_cameras_body).
+//   by_value = false (fp_register_cameras): every camera's buffers are sized for the largest frame of the call.  One
+//     frame_prep_kernel launch filters every camera and the start-pose kernels read each object's depth, size and
+//     intrinsics from the camera table.  Each pass copies its slot ids and per-hypothesis camera ids into fixed context
+//     buffers and the crops take their frame from the table at its fixed address, so the refine / feature graphs hold
+//     no frame and are keyed on (kind, pass size, iterations) alone: reordering cameras or objects or changing
+//     intrinsics replays them.
+//   by_value = true (fp_register_objects, C = 1): the frame filters, the start-pose kernels and the crop producer take
+//     the context's frame by value (the single-camera kernel instantiations), as fp_register does.
+// Both: whole objects in the given order in passes of up to kRegisterPassCap hypotheses (an object above the cap alone),
+// then one segmented scorer tail over all objects.  Synchronises.
+static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
+                                 const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
+                                 const int* n_hyp_host, const unsigned char* const* masks_host, const float* rot_grids_dev,
+                                 int iterations, float* poses_out_dev, float* scores_out_dev, int* best_out_dev,
+                                 float* info_out_dev, cudaStream_t st, bool by_value) {
+  const char* caller = by_value ? "fp_register_objects" : "fp_register_cameras";
+  std::vector<int> off(M + 1, 0);
+  int seg_max = 0;
+  for (int i = 0; i < M; ++i) {
+    FP_REQUIRE(n_hyp_host[i] >= 1 && n_hyp_host[i] <= 4096, "%s: object %d: %d hypotheses, need 1..4096", caller, i,
+               n_hyp_host[i]);
+    off[i + 1] = off[i] + n_hyp_host[i];
+    seg_max = std::max(seg_max, n_hyp_host[i]);
+  }
+  const int total = off[M];
+  // passes: whole objects in the given order, up to kRegisterPassCap hypotheses; an object above the cap alone
+  std::vector<int> pass_obj(1, 0);  // first object of every pass, then M
+  for (int i = 1; i < M; ++i)
+    if (off[i + 1] - off[pass_obj.back()] > kRegisterPassCap) pass_obj.push_back(i);
+  pass_obj.push_back(M);
+  int max_pass = 0;
+  for (size_t p = 0; p + 1 < pass_obj.size(); ++p) max_pass = std::max(max_pass, off[pass_obj[p + 1]] - off[pass_obj[p]]);
+  // each object's mask at its byte offset of one block
+  size_t npix_max = 0;
+  int H_max = 0, W_max = 0;
+  for (int i = 0; i < C; ++i) {
+    npix_max = std::max(npix_max, (size_t)H[i] * W[i]);
+    H_max = std::max(H_max, H[i]);
+    W_max = std::max(W_max, W[i]);
+  }
+  std::vector<size_t> mask_at(M + 1, 0);
+  for (int i = 0; i < M; ++i) mask_at[i + 1] = mask_at[i] + (size_t)H[camera_of[i]] * W[camera_of[i]];
+  const size_t mask_bytes = mask_at[M];
+  // every workspace is sized for the largest pass here, so no pass bumps the graph epoch
+  FP_TRY(ensure_capacity(c, max_pass));
+  FP_TRY(ensure_tail(c, total));
+  FP_TRY(alloc_frame_buffers(c, npix_max, true));
+  set_frame_geometry(c, K, H[0], W[0]);
+  FP_TRY(alloc_frame_staging(c, npix_max));
+  FP_TRY(alloc_camera_bufs(c, C, npix_max));
+  FP_TRY(dev_alloc(c->epoch, c->mesh_of, (size_t)max_pass * sizeof(int)));
+  FP_TRY(dev_alloc(c->epoch, c->seg_off, (size_t)(2 * M + 1) * sizeof(int)));  // offsets [M + 1], camera ids [M]
+  FP_TRY(dev_alloc(c->epoch, c->reg_feats, (size_t)total * 512 * sizeof(float)));
+  FP_TRY(dev_alloc(c->epoch, c->mask_buf, mask_bytes));
+  FP_TRY(dev_alloc(c->epoch, c->mask_stats, (size_t)M * 6 * sizeof(unsigned int)));
+  FP_TRY(dev_alloc(c->epoch, c->tail_counter, std::max<size_t>(16, (size_t)M * sizeof(unsigned int)), /*zero=*/true));
+  const size_t table_bytes = sizeof(CameraDev) * kMaxCameras;
+  if (!by_value) {
+    FP_TRY(dev_alloc(c->epoch, c->reg_cams, table_bytes));
+    FP_TRY(dev_alloc(c->epoch, c->reg_cam_of, (size_t)max_pass * sizeof(int)));
+    FP_TRY(dev_alloc(c->epoch, c->mask_off, (size_t)M * sizeof(size_t)));
+    FP_TRY(pinned_alloc(nullptr, c->stage_cams, table_bytes + (size_t)M * sizeof(size_t)));
+  }
+  // pinned staging (never read by a captured graph): the copies below leave as soon as they are enqueued
+  FP_TRY(pinned_alloc(nullptr, c->stage_masks, mask_bytes));
+  FP_TRY(pinned_alloc(nullptr, c->stage_ints, (size_t)(2 * M + 1 + 2 * total) * sizeof(int)));
+  // offsets [M + 1], camera of every object [M], slot of every hypothesis [total], camera of every hypothesis [total]
+  int* ints = reinterpret_cast<int*>(c->stage_ints.p);
+  int* slot_of = ints + 2 * M + 1;
+  int* cam_of = slot_of + total;
+  memcpy(ints, off.data(), (size_t)(M + 1) * sizeof(int));
+  memcpy(ints + M + 1, camera_of, (size_t)M * sizeof(int));
+  for (int i = 0; i < M; ++i) {
+    std::fill(slot_of + off[i], slot_of + off[i + 1], slots_host[i]);
+    std::fill(cam_of + off[i], cam_of + off[i + 1], camera_of[i]);
+    memcpy(reinterpret_cast<unsigned char*>(c->stage_masks.p) + mask_at[i], masks_host[i], mask_at[i + 1] - mask_at[i]);
+  }
+  FP_CUDA_OK(cudaMemcpyAsync(c->seg_off.p, ints, (size_t)(2 * M + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
+  FP_CUDA_OK(cudaMemcpyAsync(c->mask_buf.p, c->stage_masks.p, mask_bytes, cudaMemcpyHostToDevice, st));
+  const CameraDev* cams_dev = by_value ? nullptr : reinterpret_cast<const CameraDev*>(c->reg_cams.p);
+  if (!by_value) {
+    char* stage = reinterpret_cast<char*>(c->stage_cams.p);
+    fill_camera_table(c, C, K, H, W, reinterpret_cast<CameraDev*>(stage));
+    memcpy(stage + table_bytes, mask_at.data(), (size_t)M * sizeof(size_t));
+    FP_CUDA_OK(cudaMemcpyAsync(c->reg_cams.p, stage, table_bytes, cudaMemcpyHostToDevice, st));
+    FP_CUDA_OK(cudaMemcpyAsync(c->mask_off.p, stage + table_bytes, (size_t)M * sizeof(size_t), cudaMemcpyHostToDevice, st));
+  }
+  FP_TRY(upload_camera_frames(c, C, rgb_host, depth_host, H, W, st));
+  // estimater.py:173-174, :214 once per camera for every object: erode + bilateral, depth2xyzmap(zfar = inf)
+  c->has_frame = false;
+  if (by_value) {
+    FP_TRY(set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->rgb_raw.p),
+                              reinterpret_cast<const float*>(c->depth_raw.p), FP_FRAME_FILTER_DEPTH, INFINITY, st));
+  } else {
+    c->depth_cur = reinterpret_cast<const float*>(c->depth_b.p);
+    FP_TRY(frame_prep_cameras_launch(cams_dev, C, H_max, W_max, INFINITY, st));
+  }
+  c->has_frame = true;
+  // estimater.py:137-156, :203-209 for every object in one launch pair; the start poses go to poses_out_dev and are
+  // replaced pass by pass with the refined ones
+  const int* seg = reinterpret_cast<const int*>(c->seg_off.p);
+  const unsigned char* masks_dev = reinterpret_cast<const unsigned char*>(c->mask_buf.p);
+  unsigned int* stats = reinterpret_cast<unsigned int*>(c->mask_stats.p);
+  if (by_value) {
+    FP_TRY(start_poses_launch(c->depth_cur, masks_dev, H[0], W[0], c->K[0], c->K[4], c->K[2], c->K[5], rot_grids_dev, total, M,
+                              seg, stats, poses_out_dev, info_out_dev, st));
+  } else {
+    FP_TRY(start_poses_cameras_launch(cams_dev, seg + M + 1, masks_dev, reinterpret_cast<const size_t*>(c->mask_off.p),
+                                      rot_grids_dev, M, seg, stats, poses_out_dev, info_out_dev, st));
+  }
+  float* pa = reinterpret_cast<float*>(c->poses_a.p);
+  float* pb = reinterpret_cast<float*>(c->poses_b.p);
+  float* ps = reinterpret_cast<float*>(c->pose_stage.p);
+  float* fb = reinterpret_cast<float*>(c->feat_buf.p);
+  const int* mesh_of = reinterpret_cast<const int*>(c->mesh_of.p);
+  const int* hyp_cam = by_value ? nullptr : reinterpret_cast<const int*>(c->reg_cam_of.p);
+  const float* fin = (iterations % 2 == 0) ? pa : pb;
+  const GraphKind refine_kind = by_value ? GraphKind::RegisterRefine : GraphKind::RegisterCamerasRefine;
+  const GraphKind feature_kind = by_value ? GraphKind::RegisterFeatures : GraphKind::RegisterCamerasFeatures;
+  for (size_t p = 0; p + 1 < pass_obj.size(); ++p) {
+    const int row0 = off[pass_obj[p]], n = off[pass_obj[p + 1]] - row0;
+    // the pass's slot ids, camera ids and start poses go to fixed context buffers and its outputs are copied out after
+    // the replays: the graphs hold no per-pass address and are keyed on (kind, n, iterations) alone
+    FP_CUDA_OK(cudaMemcpyAsync(c->mesh_of.p, slot_of + row0, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+    if (!by_value)
+      FP_CUDA_OK(cudaMemcpyAsync(c->reg_cam_of.p, cam_of + row0, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+    FP_CUDA_OK(cudaMemcpyAsync(pa, poses_out_dev + (size_t)row0 * 16, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
+    FP_TRY(run_graphed(
+        c, refine_kind, n, iterations, st,
+        [&](cudaStream_t s2) -> int { return refine_body(c, n, iterations, s2, mesh_of, cams_dev, hyp_cam); }, 0, by_value));
+    FP_CUDA_OK(cudaMemcpyAsync(poses_out_dev + (size_t)row0 * 16, fin, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
+    FP_CUDA_OK(cudaMemcpyAsync(ps, fin, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
+    FP_TRY(run_graphed(
+        c, feature_kind, n, 0, st,
+        [&](cudaStream_t s2) -> int {
+          FP_TRY(make_crops(c, ps, n, 1, nullptr, nullptr, nullptr, s2, mesh_of, cams_dev, hyp_cam));
+          FP_TRY(run_encoder(c, c->net[1], reinterpret_cast<const __half*>(c->crops.p), n, s2));
+          return run_score_feats(c, c->net[1], n, fb, s2);
+        },
+        0, by_value));
+    FP_CUDA_OK(cudaMemcpyAsync(reinterpret_cast<float*>(c->reg_feats.p) + (size_t)row0 * 512, fb, (size_t)n * 2048,
+                               cudaMemcpyDeviceToDevice, st));
+  }
+  // score_network.py:84-88 per object: one tail launch, each object's hypotheses attending only to each other
+  ScoreTailParams tp = score_tail_params(c, reinterpret_cast<const float*>(c->reg_feats.p), total, scores_out_dev, best_out_dev);
+  tp.seg = seg;
+  tp.n_seg = M;
+  tp.seg_max = seg_max;
+  FP_TRY(score_tail_launch(tp, st));
+  FP_CUDA_OK(cudaStreamSynchronize(st));
+  return 0;
 }
 
 }  // namespace fp
@@ -1404,20 +1601,9 @@ int fp_track_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host, con
   FP_API_BEGIN
   FP_REQUIRE(c && rgb_host && depth_host && K && H && W && M > 0 && camera_of && slots_host && poses_in_dev && iterations >= 0,
              "fp_track_cameras: bad argument");
-  FP_REQUIRE(C >= 1 && C <= kMaxCameras, "fp_track_cameras: %d cameras, need 1..%d", C, kMaxCameras);
   FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
   // everything is checked before anything is enqueued: the kernels index the mesh and camera tables unchecked
-  for (int i = 0; i < C; ++i) {
-    FP_REQUIRE(rgb_host[i] && depth_host[i], "fp_track_cameras: camera %d: null frame", i);
-    FP_REQUIRE(H[i] > 0 && W[i] > 0, "fp_track_cameras: camera %d: empty frame (%d x %d)", i, H[i], W[i]);
-  }
-  std::vector<int> owns(C, 0);
-  for (int i = 0; i < M; ++i) {
-    FP_REQUIRE(camera_of[i] >= 0 && camera_of[i] < C, "fp_track_cameras: object %d: camera %d out of range [0, %d)", i,
-               camera_of[i], C);
-    owns[camera_of[i]] = 1;
-  }
-  for (int i = 0; i < C; ++i) FP_REQUIRE(owns[i], "fp_track_cameras: camera %d owns no object", i);
+  FP_TRY(check_cameras(C, rgb_host, depth_host, H, W, M, camera_of, "fp_track_cameras"));
   FP_TRY(check_slots(c, M, slots_host, "fp_track_cameras"));
   DeviceGuard dg(c->device);
   return track_cameras_body(c, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, poses_in_dev, iterations,
@@ -1438,90 +1624,36 @@ int fp_register_objects(fp_ctx* c, const unsigned char* rgb_host, const float* d
   FP_REQUIRE(c->net[1].loaded, "scorer weights not loaded");
   // everything is checked before anything is enqueued
   FP_TRY(check_slots(c, M, slots_host, "fp_register_objects"));
-  std::vector<int> off(M + 1, 0);
-  int seg_max = 0;
-  for (int i = 0; i < M; ++i) {
-    FP_REQUIRE(n_hyp_host[i] >= 1 && n_hyp_host[i] <= 4096, "fp_register_objects: object %d: %d hypotheses, need 1..4096", i,
-               n_hyp_host[i]);
-    off[i + 1] = off[i] + n_hyp_host[i];
-    seg_max = std::max(seg_max, n_hyp_host[i]);
-  }
-  const int total = off[M];
-  // passes: whole objects in the given order, up to kRegisterPassCap hypotheses; an object above the cap alone
-  std::vector<int> pass_obj(1, 0);  // first object of every pass, then M
-  for (int i = 1; i < M; ++i)
-    if (off[i + 1] - off[pass_obj.back()] > kRegisterPassCap) pass_obj.push_back(i);
-  pass_obj.push_back(M);
-  int max_pass = 0;
-  for (size_t p = 0; p + 1 < pass_obj.size(); ++p) max_pass = std::max(max_pass, off[pass_obj[p + 1]] - off[pass_obj[p]]);
   DeviceGuard dg(c->device);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const size_t npix = (size_t)H * W;
-  // every workspace is sized for the largest pass here, so no pass bumps the graph epoch
-  FP_TRY(ensure_capacity(c, max_pass));
-  FP_TRY(ensure_tail(c, total));
-  FP_TRY(prepare_frame(c, K, H, W, true));
-  FP_TRY(alloc_frame_staging(c, npix));
-  FP_TRY(dev_alloc(c->epoch, c->mesh_of, (size_t)max_pass * sizeof(int)));
-  FP_TRY(dev_alloc(c->epoch, c->seg_off, (size_t)(M + 1) * sizeof(int)));
-  FP_TRY(dev_alloc(c->epoch, c->reg_feats, (size_t)total * 512 * sizeof(float)));
-  FP_TRY(dev_alloc(c->epoch, c->mask_buf, (size_t)M * npix));
-  FP_TRY(dev_alloc(c->epoch, c->mask_stats, (size_t)M * 6 * sizeof(unsigned int)));
-  FP_TRY(dev_alloc(c->epoch, c->tail_counter, std::max<size_t>(16, (size_t)M * sizeof(unsigned int)), /*zero=*/true));
-  // pinned staging (never read by a captured graph): the copies below leave as soon as they are enqueued
-  FP_TRY(pinned_alloc(nullptr, c->stage_masks, (size_t)M * npix));
-  FP_TRY(pinned_alloc(nullptr, c->stage_ints, (size_t)(M + 1 + total) * sizeof(int)));
-  int* ints = reinterpret_cast<int*>(c->stage_ints.p);
-  int* slot_of = ints + M + 1;  // slot id of every hypothesis
-  memcpy(ints, off.data(), (size_t)(M + 1) * sizeof(int));
-  for (int i = 0; i < M; ++i) std::fill(slot_of + off[i], slot_of + off[i + 1], slots_host[i]);
-  memcpy(c->stage_masks.p, masks_host, (size_t)M * npix);
-  FP_CUDA_OK(cudaMemcpyAsync(c->seg_off.p, ints, (size_t)(M + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
-  FP_CUDA_OK(cudaMemcpyAsync(c->mask_buf.p, c->stage_masks.p, (size_t)M * npix, cudaMemcpyHostToDevice, st));
-  FP_TRY(upload_staged_frame(c, rgb_host, depth_host, npix, st));
-  // estimater.py:173-174, :214 once for every object: erode + bilateral, depth2xyzmap(zfar = inf)
-  c->has_frame = false;
-  FP_TRY(set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->rgb_raw.p), reinterpret_cast<const float*>(c->depth_raw.p),
-                            FP_FRAME_FILTER_DEPTH, INFINITY, st));
-  c->has_frame = true;
-  // estimater.py:137-156, :203-209 for every object in one launch pair; the start poses go to poses_out_dev and are
-  // replaced pass by pass with the refined ones
-  const int* seg = reinterpret_cast<const int*>(c->seg_off.p);
-  FP_TRY(start_poses_launch(c->depth_cur, reinterpret_cast<const unsigned char*>(c->mask_buf.p), H, W, c->K[0], c->K[4], c->K[2],
-                            c->K[5], rot_grids_dev, total, M, seg, reinterpret_cast<unsigned int*>(c->mask_stats.p),
-                            poses_out_dev, info_out_dev, st));
-  float* pa = reinterpret_cast<float*>(c->poses_a.p);
-  float* pb = reinterpret_cast<float*>(c->poses_b.p);
-  float* ps = reinterpret_cast<float*>(c->pose_stage.p);
-  float* fb = reinterpret_cast<float*>(c->feat_buf.p);
-  const int* mesh_of = reinterpret_cast<const int*>(c->mesh_of.p);
-  const float* fin = (iterations % 2 == 0) ? pa : pb;
-  for (size_t p = 0; p + 1 < pass_obj.size(); ++p) {
-    const int row0 = off[pass_obj[p]], n = off[pass_obj[p + 1]] - row0;
-    // the pass's slot ids and start poses go to fixed context buffers and its outputs are copied out after the replays:
-    // the graphs hold no per-pass address and are keyed on (kind, n, iterations) alone
-    FP_CUDA_OK(cudaMemcpyAsync(c->mesh_of.p, slot_of + row0, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
-    FP_CUDA_OK(cudaMemcpyAsync(pa, poses_out_dev + (size_t)row0 * 16, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
-    FP_TRY(run_graphed(c, GraphKind::RegisterRefine, n, iterations, st,
-                       [&](cudaStream_t s2) -> int { return refine_body(c, n, iterations, s2, mesh_of); }));
-    FP_CUDA_OK(cudaMemcpyAsync(poses_out_dev + (size_t)row0 * 16, fin, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
-    FP_CUDA_OK(cudaMemcpyAsync(ps, fin, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
-    FP_TRY(run_graphed(c, GraphKind::RegisterFeatures, n, 0, st, [&](cudaStream_t s2) -> int {
-      FP_TRY(make_crops(c, ps, n, 1, nullptr, nullptr, nullptr, s2, mesh_of));
-      FP_TRY(run_encoder(c, c->net[1], reinterpret_cast<const __half*>(c->crops.p), n, s2));
-      return run_score_feats(c, c->net[1], n, fb, s2);
-    }));
-    FP_CUDA_OK(cudaMemcpyAsync(reinterpret_cast<float*>(c->reg_feats.p) + (size_t)row0 * 512, fb, (size_t)n * 2048,
-                               cudaMemcpyDeviceToDevice, st));
-  }
-  // score_network.py:84-88 per object: one tail launch, each object's hypotheses attending only to each other
-  ScoreTailParams tp = score_tail_params(c, reinterpret_cast<const float*>(c->reg_feats.p), total, scores_out_dev, best_out_dev);
-  tp.seg = seg;
-  tp.n_seg = M;
-  tp.seg_max = seg_max;
-  FP_TRY(score_tail_launch(tp, st));
-  FP_CUDA_OK(cudaStreamSynchronize(st));
-  return 0;
+  std::vector<const unsigned char*> masks(M);
+  for (int i = 0; i < M; ++i) masks[i] = masks_host + (size_t)i * npix;
+  const std::vector<int> camera_of(M, 0);
+  return register_cameras_body(c, 1, &rgb_host, &depth_host, K, &H, &W, M, camera_of.data(), slots_host, n_hyp_host,
+                               masks.data(), rot_grids_dev, iterations, poses_out_dev, scores_out_dev, best_out_dev,
+                               info_out_dev, reinterpret_cast<cudaStream_t>(stream), /*by_value=*/true);
+  FP_API_END
+}
+
+int fp_register_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host, const float* K,
+                        const int* H, const int* W, int M, const int* camera_of, const int* slots_host, const int* n_hyp_host,
+                        const unsigned char* const* masks_host, const float* rot_grids_dev, int iterations,
+                        float* poses_out_dev, float* scores_out_dev, int* best_out_dev, float* info_out_dev, void* stream) {
+  FP_API_BEGIN
+  FP_REQUIRE(c && rgb_host && depth_host && K && H && W && M > 0 && M <= 65535 && camera_of && slots_host && n_hyp_host &&
+                 masks_host && rot_grids_dev && iterations >= 0 && poses_out_dev && scores_out_dev && best_out_dev &&
+                 info_out_dev,
+             "fp_register_cameras: bad argument");
+  FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
+  FP_REQUIRE(c->net[1].loaded, "scorer weights not loaded");
+  // everything is checked before anything is enqueued: the kernels index the mesh and camera tables unchecked
+  FP_TRY(check_cameras(C, rgb_host, depth_host, H, W, M, camera_of, "fp_register_cameras"));
+  for (int i = 0; i < M; ++i) FP_REQUIRE(masks_host[i], "fp_register_cameras: object %d: null mask", i);
+  FP_TRY(check_slots(c, M, slots_host, "fp_register_cameras"));
+  DeviceGuard dg(c->device);
+  return register_cameras_body(c, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, n_hyp_host, masks_host,
+                               rot_grids_dev, iterations, poses_out_dev, scores_out_dev, best_out_dev, info_out_dev,
+                               reinterpret_cast<cudaStream_t>(stream), /*by_value=*/false);
   FP_API_END
 }
 

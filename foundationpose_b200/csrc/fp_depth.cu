@@ -245,11 +245,24 @@ __device__ unsigned int radix_select(const float* __restrict__ depth, const unsi
 // pass 1 (grid-wide, one grid row per object): mask bounding box and pixel counts.  All six statistics are max / sum
 // reductions over values that start at 0 (the box minima are stored mirrored), so one memset of 6 words per object
 // initialises them.  Object m reads masks[m] ([H][W]) and writes stats[6 m, 6 m + 6).
+// kTable (fp_register_cameras): object m is seen by camera camera_of[m] of the device table `cams` and takes its
+// filtered depth and H x W from there; its mask ([H][W] of that camera) starts at byte mask_off[m] of `masks`.  The
+// table arguments follow the by-value ones, so the by-value instantiation reads its parameters where it always did.
+template <bool kTable>
 __global__ void __launch_bounds__(256) mask_stats_kernel(const float* __restrict__ depth,
                                                          const unsigned char* __restrict__ masks, int H, int W,
-                                                         unsigned int* __restrict__ stats) {
+                                                         unsigned int* __restrict__ stats,
+                                                         const CameraDev* __restrict__ cams,
+                                                         const int* __restrict__ camera_of,
+                                                         const size_t* __restrict__ mask_off) {
+  if (kTable) {
+    const CameraDev& cam = cams[camera_of[blockIdx.y]];
+    depth = cam.depth;
+    H = cam.H;
+    W = cam.W;
+  }
   const int npix = H * W;
-  const unsigned char* mask = masks + (size_t)blockIdx.y * npix;
+  const unsigned char* mask = masks + (kTable ? mask_off[blockIdx.y] : (size_t)blockIdx.y * npix);
   stats += 6 * blockIdx.y;
   unsigned int mu0 = 0, u1 = 0, mv0 = 0, v1 = 0, n_mask = 0, n_valid = 0;  // mu0 = W - 1 - umin, mv0 = H - 1 - vmin
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < npix; i += gridDim.x * blockDim.x) {
@@ -284,18 +297,32 @@ __global__ void __launch_bounds__(256) mask_stats_kernel(const float* __restrict
 
 // pass 2 (one CTA per object): exact median over the object's bounding box, translation, start poses.  Object m owns
 // rows [off[m], off[m + 1]) of the concatenated rotation grids and start poses (off = null: one object, rows [0, N)),
-// and writes info[4 m, 4 m + 4).
+// and writes info[4 m, 4 m + 4).  kTable: the object's depth, H x W, fx fy cx cy and mask as in mask_stats_kernel.
+template <bool kTable>
 __global__ void __launch_bounds__(1024) start_poses_kernel(const float* __restrict__ depth,
                                                            const unsigned char* __restrict__ masks, int H, int W, float fx,
                                                            float fy, float cx, float cy, const float* __restrict__ rot_grid,
                                                            int N, const int* __restrict__ off,
                                                            const unsigned int* __restrict__ stats,
-                                                           float* __restrict__ poses_out, float* __restrict__ info) {
+                                                           float* __restrict__ poses_out, float* __restrict__ info,
+                                                           const CameraDev* __restrict__ cams,
+                                                           const int* __restrict__ camera_of,
+                                                           const size_t* __restrict__ mask_off) {
   __shared__ unsigned int hist[256];
   __shared__ unsigned int sh[2];
   __shared__ float tvec[3];
   const int m = blockIdx.x;
-  const unsigned char* mask = masks + (size_t)m * H * W;
+  if (kTable) {
+    const CameraDev& cam = cams[camera_of[m]];
+    depth = cam.depth;
+    H = cam.H;
+    W = cam.W;
+    fx = cam.fx;
+    fy = cam.fy;
+    cx = cam.cx;
+    cy = cam.cy;
+  }
+  const unsigned char* mask = masks + (kTable ? mask_off[m] : (size_t)m * H * W);
   stats += 6 * m;
   info += 4 * m;
   const int row0 = off ? off[m] : 0;
@@ -340,8 +367,22 @@ int start_poses_launch(const float* depth, const unsigned char* masks, int H, in
                        float* info, cudaStream_t stream) {
   FP_REQUIRE(M >= 1 && M <= 65535 && (off || M == 1), "start_poses: bad object count %d", M);
   FP_CUDA_OK(cudaMemsetAsync(stats, 0, (size_t)M * 6 * sizeof(unsigned int), stream));
-  mask_stats_kernel<<<dim3(num_sms(), M), 256, 0, stream>>>(depth, masks, H, W, stats);
-  start_poses_kernel<<<M, 1024, 0, stream>>>(depth, masks, H, W, fx, fy, cx, cy, rot_grid, N, off, stats, poses_out, info);
+  mask_stats_kernel<false><<<dim3(num_sms(), M), 256, 0, stream>>>(depth, masks, H, W, stats, nullptr, nullptr, nullptr);
+  start_poses_kernel<false><<<M, 1024, 0, stream>>>(depth, masks, H, W, fx, fy, cx, cy, rot_grid, N, off, stats, poses_out, info,
+                                                    nullptr, nullptr, nullptr);
+  note_launches(2);
+  FP_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int start_poses_cameras_launch(const CameraDev* cams, const int* camera_of, const unsigned char* masks, const size_t* mask_off,
+                               const float* rot_grid, int M, const int* off, unsigned int* stats, float* poses_out,
+                               float* info, cudaStream_t stream) {
+  FP_REQUIRE(M >= 1 && M <= 65535 && off, "start_poses_cameras: bad object count %d", M);
+  FP_CUDA_OK(cudaMemsetAsync(stats, 0, (size_t)M * 6 * sizeof(unsigned int), stream));
+  mask_stats_kernel<true><<<dim3(num_sms(), M), 256, 0, stream>>>(nullptr, masks, 0, 0, stats, cams, camera_of, mask_off);
+  start_poses_kernel<true><<<M, 1024, 0, stream>>>(nullptr, masks, 0, 0, 0.f, 0.f, 0.f, 0.f, rot_grid, 0, off, stats, poses_out,
+                                                   info, cams, camera_of, mask_off);
   note_launches(2);
   FP_CUDA_OK(cudaGetLastError());
   return 0;

@@ -21,4 +21,10 @@ int frame_prep_cameras_launch(const CameraDev* cams, int C, int max_H, int max_W
 int start_poses_launch(const float* depth, const unsigned char* masks, int H, int W, float fx, float fy, float cx, float cy,
                        const float* rot_grid, int N, int M, const int* off, unsigned int* stats, float* poses_out,
                        float* info, cudaStream_t stream);
+// the same for M objects seen by several cameras (fp_register_cameras): object m takes its filtered depth, H x W and
+// intrinsics from cams[camera_of[m]] (DEVICE table and [M] camera ids) and its mask ([H][W] of that camera) from byte
+// mask_off[m] (DEVICE [M]) of `masks`; off as above, never null
+int start_poses_cameras_launch(const CameraDev* cams, const int* camera_of, const unsigned char* masks, const size_t* mask_off,
+                               const float* rot_grid, int M, const int* off, unsigned int* stats, float* poses_out,
+                               float* info, cudaStream_t stream);
 }  // namespace fp

@@ -7,4 +7,4 @@ from learning.training.predict_score import *  # noqa: F401,F403
 from learning.training.predict_pose_refine import *  # noqa: F401,F403
 import yaml  # noqa: F401
 
-from foundationpose_b200.estimater import FoundationPose, register_objects, track_cameras, track_objects  # noqa: F401,E402
+from foundationpose_b200.estimater import FoundationPose, register_cameras, register_objects, track_cameras, track_objects  # noqa: F401,E402

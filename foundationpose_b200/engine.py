@@ -34,6 +34,8 @@ def _proto():
                                      C.POINTER(i), vp, i, vp, vp, vp]
     lib.fp_register_objects.argtypes = [vp, vp, vp, C.POINTER(f), i, i, i, C.POINTER(i), C.POINTER(i), vp, vp, i, vp, vp, vp,
                                         vp, vp]
+    lib.fp_register_cameras.argtypes = [vp, i, C.POINTER(vp), C.POINTER(vp), C.POINTER(f), C.POINTER(i), C.POINTER(i), i,
+                                        C.POINTER(i), C.POINTER(i), C.POINTER(i), C.POINTER(vp), vp, i, vp, vp, vp, vp, vp]
     lib.fp_graph_captures.argtypes = [vp]
     lib.fp_graph_captures.restype = C.c_ulonglong
     lib.fp_load_network.argtypes = [vp, i, C.POINTER(_FpTensor), i]
@@ -54,7 +56,7 @@ def _proto():
     lib.fp_op_tokens.argtypes = [vp, i, vp, i, vp, vp]
     lib.fp_op_depth_filter.argtypes = [vp, vp, i, i, i, vp]
     lib.fp_op_pose_update.argtypes = [vp, vp, vp, vp, i, f, f, vp]
-    for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_track_cameras", "fp_register_objects", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh",
+    for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_track_cameras", "fp_register_objects", "fp_register_cameras", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh",
                  "fp_set_mesh_slot", "fp_set_frame",
                  "fp_get_depth", "fp_make_crops", "fp_start_poses", "fp_refine", "fp_score", "fp_score_features", "fp_score_tail",
                  "fp_register", "fp_op_refine_net", "fp_op_score_feats", "fp_op_tokens", "fp_op_depth_filter",
@@ -66,7 +68,7 @@ _proto()
 
 FRAME_ON_DEVICE = 1
 MAX_MESHES = 64  # FP_MAX_MESHES: mesh slots per context
-MAX_CAMERAS = 16  # FP_MAX_CAMERAS: camera streams per fp_track_cameras call
+MAX_CAMERAS = 16  # FP_MAX_CAMERAS: camera streams per fp_track_cameras / fp_register_cameras call
 _NO_PIN = os.environ.get("FPOSE_NO_PIN") == "1"  # A/B: skip the pinned staging of host frames
 FRAME_FILTER_DEPTH = 2
 
@@ -323,6 +325,44 @@ class Engine:
                                            int(iterations), _p(poses), _p(scores), _p(best), _p(info), _stream()),
                    "fp_register_objects")
         self.frame_hw = (H, W)
+        return poses, scores, best, info
+
+    def register_cameras(self, frames, masks, rot_grids, camera_of, slots, iterations):
+        """fp_register_cameras: `register_objects` for M objects spread over C camera streams in one call.  frames: C tuples
+        (rgb uint8 (H,W,3), depth float32 (H,W), K (3,3)) of HOST arrays, one per camera, each with its own size and
+        intrinsics; object i is seen by camera camera_of[i], renders the mesh in slot slots[i] and has the HOST mask
+        masks[i] (nonzero = object) of its camera's frame size; rot_grids: M CUDA float32 (N_i,4,4) rotation grids.
+        Returns the CUDA tensors of register_objects: poses (sum N_i,4,4), scores (sum N_i,), best (M,), info (M,4)."""
+        frames = [(np.ascontiguousarray(rgb, dtype=np.uint8), np.ascontiguousarray(depth, dtype=np.float32), K) for rgb, depth, K in frames]
+        n_cam = len(frames)
+        M = len(masks)
+        camera_of, slots = [int(c) for c in camera_of], [int(s) for s in slots]
+        rot_grids = [g.reshape(-1, 4, 4) for g in rot_grids]
+        if len(camera_of) != M or len(slots) != M or len(rot_grids) != M:
+            raise ValueError(f"register_cameras: {M} masks, {len(camera_of)} camera ids, {len(slots)} slots and "
+                             f"{len(rot_grids)} rotation grids")
+        masks = [np.asarray(m) for m in masks]
+        for i, (m, c) in enumerate(zip(masks, camera_of)):
+            if 0 <= c < n_cam and m.shape != frames[c][1].shape:
+                raise ValueError(f"register_cameras: mask {i} has shape {m.shape}, camera {c}'s frame is {frames[c][1].shape}")
+        masks = [np.ascontiguousarray(m > 0, dtype=np.uint8) for m in masks]  # the reference tests `mask > 0` (estimater.py:138, :183)
+        n_hyp = [len(g) for g in rot_grids]
+        grids = torch.cat(rot_grids).to(device="cuda", dtype=torch.float32).contiguous()
+        total = len(grids)
+        rgbs = (C.c_void_p * n_cam)(*[rgb.ctypes.data for rgb, _, _ in frames])
+        depths = (C.c_void_p * n_cam)(*[depth.ctypes.data for _, depth, _ in frames])
+        Ks = (C.c_float * (9 * n_cam))(*[float(x) for _, _, K in frames for x in np.asarray(K, dtype=np.float64).reshape(-1)])
+        Hs = (C.c_int * n_cam)(*[depth.shape[0] for _, depth, _ in frames])
+        Ws = (C.c_int * n_cam)(*[depth.shape[1] for _, depth, _ in frames])
+        poses = torch.empty(total, 4, 4, dtype=torch.float32, device="cuda")
+        scores = torch.empty(total, dtype=torch.float32, device="cuda")
+        best = torch.empty(M, dtype=torch.int32, device="cuda")
+        info = torch.empty(M, 4, dtype=torch.float32, device="cuda")
+        _lib.check(lib.fp_register_cameras(self._h, n_cam, rgbs, depths, Ks, Hs, Ws, M, (C.c_int * M)(*camera_of),
+                                           (C.c_int * M)(*slots), (C.c_int * M)(*n_hyp), (C.c_void_p * M)(*[m.ctypes.data for m in masks]),
+                                           _p(grids), int(iterations), _p(poses), _p(scores), _p(best), _p(info), _stream()),
+                   "fp_register_cameras")
+        self.frame_hw = frames[0][1].shape  # camera 0's frame is the context's frame
         return poses, scores, best, info
 
     def set_frame(self, rgb, depth, K, filter_depth=True, zfar=float("inf")):

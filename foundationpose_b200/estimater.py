@@ -482,6 +482,67 @@ def register_objects(estimators, K, rgb, depth, ob_masks, ob_ids=None, iteration
     slots = [_object_slot(est, "register_objects") for est in estimators]
     poses, scores, _, info = e.register_objects(rgb, depth, K, np.stack(masks), [est.rot_grid for est in estimators], slots,
                                                 iteration)
+    return _finish_register(estimators, poses, scores, info, [(K, H, W)] * M, ob_ids, ob_masks)
+
+
+def register_cameras(views, ob_ids=None, iteration=5):
+    """`[register_objects(ests, K, rgb, depth, ob_masks, ob_ids, iteration) for ests, rgb, depth, K, ob_masks in views]`
+    bit for bit, in the returned poses and in every estimator's state, for objects seen by several camera streams (a
+    multi-camera rig re-acquiring its objects) in one fp_register_cameras call: every camera's frame is uploaded and
+    filtered, every object's start poses come from one launch pair over its own camera's depth and intrinsics, the
+    hypotheses of all objects are refined and featurised together in passes of up to 512 (a pass may mix cameras), and
+    one scorer tail keeps every object's hypotheses to themselves.  Each estimator uses its own rotation grid and keeps
+    its mesh in the slot track_objects / track_cameras use, so tracking them afterwards uploads no mesh.  Everything
+    comes back to the host in one read-back.
+
+    views: one (estimators, rgb, depth, K, ob_masks) per camera, each camera with its own frame size and intrinsics and
+    one (H,W) mask of its frame per estimator.  ob_ids: None, or one list (or None) per view.  All estimators share one
+    engine and none appears twice, across cameras or within one; at most MAX_MESHES - 1 objects and MAX_CAMERAS cameras
+    with objects.  A camera without estimators gives [] and its frame is not uploaded.  Host frames and masks only
+    (uint8 (H,W,3) rgb, float32 (H,W) depth).  Returns one list of (4,4) poses of the original meshes per camera."""
+    views = [(list(ests), rgb, depth, K, list(ob_masks)) for ests, rgb, depth, K, ob_masks in views]
+    ob_ids = [None] * len(views) if ob_ids is None else list(ob_ids)
+    if len(ob_ids) != len(views):
+        raise ValueError(f"register_cameras: {len(views)} views but {len(ob_ids)} ob_ids lists")
+    if any(torch.is_tensor(rgb) or torch.is_tensor(depth) or any(torch.is_tensor(m) and m.is_cuda for m in ms)
+           for _, rgb, depth, _, ms in views):
+        raise TypeError("register_cameras takes host frames and masks (numpy); for device-resident frames call register per object")
+    used = [c for c, v in enumerate(views) if v[0]]
+    if not used:
+        return [[] for _ in views]
+    estimators = [est for c in used for est in views[c][0]]
+    e = _shared_engine_of(estimators, "register_cameras")
+    if len(used) > MAX_CAMERAS:
+        raise ValueError(f"register_cameras: at most {MAX_CAMERAS} cameras with objects, got {len(used)}")
+    masks, ob_masks, ids, frames, camera_of = [], [], [], [], []
+    for j, c in enumerate(used):
+        ests, rgb, depth, K, ms = views[c]
+        H, W = np.shape(depth)[:2]
+        if len(ms) != len(ests):
+            raise ValueError(f"register_cameras: camera {c}: {len(ests)} estimators but {len(ms)} masks")
+        for i, m in enumerate(ms):
+            a = m.numpy() if torch.is_tensor(m) else np.asarray(m)
+            if a.shape != (H, W):
+                raise ValueError(f"register_cameras: camera {c}: mask {i} has shape {a.shape}, the frame is {(H, W)}")
+            masks.append(a)
+        v_ids = [None] * len(ests) if ob_ids[c] is None else list(ob_ids[c])
+        if len(v_ids) != len(ests):
+            raise ValueError(f"register_cameras: camera {c}: {len(ests)} estimators but {len(v_ids)} ob_ids")
+        ob_masks += ms
+        ids += v_ids
+        frames += [(K, H, W)] * len(ests)
+        camera_of += [j] * len(ests)
+    slots = [_object_slot(est, "register_cameras") for est in estimators]
+    poses, scores, _, info = e.register_cameras([views[c][1:4] for c in used], masks, [est.rot_grid for est in estimators],
+                                                camera_of, slots, iteration)
+    flat = iter(_finish_register(estimators, poses, scores, info, frames, ids, ob_masks))
+    return [[next(flat) for _ in ests] for ests, _, _, _, _ in views]
+
+
+def _finish_register(estimators, poses, scores, info, frames, ob_ids, ob_masks):
+    """register()'s ranking, early exit and state updates (estimater.py:181-240) for every estimator, from the object-major
+    outputs of Engine.register_objects / register_cameras.  frames[i] = (K, H, W) of estimator i's camera.  Returns the
+    list of (4,4) poses of the original meshes."""
     # per object, the ranking and best pose of register(): estimater.py:224-234 on that object's rows
     ranked, rows, o = [], [], 0
     for i, est in enumerate(estimators):
@@ -498,8 +559,7 @@ def register_objects(estimators, K, rgb, depth, ob_masks, ob_ids=None, iteration
         early = out[i, 3] < 4
         est.refiner.last_trans_update = est.refiner.last_rot_update = None
         if not (early and getattr(est, "strict_early_out", False)):  # register()'s strict path returns before recording the frame
-            est.H, est.W = H, W
-            est.K = K
+            est.K, est.H, est.W = frames[i]
             est.ob_id = ob_ids[i]
             est.ob_mask = ob_masks[i]
         if early:

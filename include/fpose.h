@@ -233,6 +233,26 @@ int fp_register_objects(fp_ctx* ctx, const unsigned char* rgb_host, const float*
                         int M, const int* slots_host, const int* n_hyp_host, const unsigned char* masks_host,
                         const float* rot_grids_dev, int iterations, float* poses_out_dev, float* scores_out_dev,
                         int* best_out_dev, float* info_out_dev, void* stream);
+/* fp_register_objects for M objects spread over C camera streams (1 <= C <= FP_MAX_CAMERAS), each camera with its own
+ * frame size and intrinsics: object i is seen by camera camera_of[i] and gives exactly what fp_register_objects gives
+ * for it with that camera's frame alone, bit for bit.
+ *   rgb_host[c] / depth_host[c]: HOST uint8 [H[c]][W[c]][3] / float32 [H[c]][W[c]] frame of camera c, each uploaded
+ *   through its own pinned staging; K: [C][9] row-major intrinsics; camera_of, slots_host, n_hyp_host: HOST [M] camera,
+ *   mesh slot and hypothesis count (1..4096) of every object; masks_host[i]: HOST uint8 [H[camera_of[i]]][W[...]]
+ *   (nonzero = object); rot_grids_dev as fp_register_objects.
+ * Everything is checked before anything is enqueued: every camera id in [0, C), every camera owning at least one
+ * object, non-null frames of positive size and non-null masks, every slot loaded, both networks loaded.  All masks go
+ * to the device in one copy; one frame-preparation launch filters every camera's depth and one launch pair computes
+ * every object's start poses, each from its own camera's filtered depth and intrinsics.  Passes and the scorer tail as
+ * fp_register_objects; a pass may mix cameras.  The camera table and each pass's slot and camera ids are copied into
+ * the context first, so the cached graphs depend on the pass sizes and iterations only: reordering objects or cameras
+ * or changing intrinsics replays them.  Camera 0 is the context's frame, as after fp_track_cameras.  Outputs: exactly
+ * fp_register_objects' (object-major, unranked, best relative to the object, info [M][4]).  Synchronises. */
+int fp_register_cameras(fp_ctx* ctx, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
+                        const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
+                        const int* n_hyp_host, const unsigned char* const* masks_host, const float* rot_grids_dev,
+                        int iterations, float* poses_out_dev, float* scores_out_dev, int* best_out_dev, float* info_out_dev,
+                        void* stream);
 /* Number of CUDA graphs this context has captured so far (test hook: a replay captures nothing). */
 unsigned long long fp_graph_captures(fp_ctx* ctx);
 
