@@ -116,11 +116,7 @@ int fp_op_attention(const void* qkv, void* out, int B, int impl, void* stream) {
   return fp::attn_tc_launch(ap, st);
 }
 
-int fp_op_gemm_layer(const fp_gemm_layer_t* l, void* stream) {
-  if (!l) {
-    fp::set_last_error("fp_op_gemm_layer: null layer");
-    return -1;
-  }
+static fp::GemmLayer to_gemm_layer(const fp_gemm_layer_t* l) {
   fp::GemmLayer L;
   L.kind = l->kind;
   L.n_img = l->n_img;
@@ -138,7 +134,23 @@ int fp_op_gemm_layer(const fp_gemm_layer_t* l, void* stream) {
   L.out_split = l->out_split;
   L.post_add = l->post_add;
   L.relu = l->relu;
-  return fp::gemm_layer_launch(L, reinterpret_cast<cudaStream_t>(stream));
+  return L;
+}
+
+int fp_op_gemm_layer(const fp_gemm_layer_t* l, void* stream) {
+  if (!l) {
+    fp::set_last_error("fp_op_gemm_layer: null layer");
+    return -1;
+  }
+  return fp::gemm_layer_launch(to_gemm_layer(l), reinterpret_cast<cudaStream_t>(stream));
+}
+
+int fp_op_gemm_tile_n(const fp_gemm_layer_t* l, int* tile_n) {
+  if (!l || !tile_n) {
+    fp::set_last_error("fp_op_gemm_tile_n: null argument");
+    return -1;
+  }
+  return fp::gemm_layer_tile_n(to_gemm_layer(l), tile_n);
 }
 
 }  // extern "C"

@@ -179,6 +179,17 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
+// ---- register reallocation between warpgroups (setmaxnreg).  Every warp of a warpgroup executes the same call; the
+// kernel must be allocated the register count the releases and requests are balanced against (its launch bound).
+template <uint32_t N>
+__device__ __forceinline__ void regs_release() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void regs_acquire() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+
 // wgmma (warpgroup MMA) ------------------------------------------------------------------------
 // fence before the first wgmma of a batch (orders earlier register / shared-memory accesses before it)
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }

@@ -8,7 +8,8 @@
 //   learning/models/score_network.py:60-74     encoderA / encoderAB / att projections
 //
 // Design (sm_90a, no library GEMM):
-//   * D[128 x BN] tiles (BN = 128, or 64 for 64-channel layers), fp16 operands, fp32 accumulators in registers: two
+//   * D[128 x BN] tiles (BN = 128; 256 for long 3x3 convolutions on tall grids; 64 for 64-channel layers), fp16
+//     operands, fp32 accumulators in registers: two
 //     consumer warpgroups issue m64nBNk16 wgmmas on 64 rows each; one producer thread feeds a ring of TMA stages
 //     (A 16 KB + B BN x 128 B, 128-byte swizzle) through full / empty mbarriers.  Persistent CTAs, one per SM.
 //   * The convolution is an *implicit* GEMM: the A tile for k-block (tap, 64-channel chunk) is one 5-D TMA box over
@@ -143,23 +144,33 @@ constexpr int kTileThreads = 384;               // warpgroup 0: TMA producer; wa
 constexpr int kSlabBytes = kBlockM * 64 * 2;    // 16 KB: one output slab (128 pixels x 64 channels, 128B-swizzled)
 constexpr int kSmemOptIn = 232448;              // 227 KB opt-in shared memory per block
 
-// BN = output channels per tile (64 or 128).  Each consumer warpgroup owns 64 of the tile's 128 pixel rows and keeps
-// its 64 x BN fp32 accumulator in registers (BN / 2 per thread).
+// BN = output channels per tile (64, 128 or 256).  Each consumer warpgroup owns 64 of the tile's 128 pixel rows and
+// keeps its 64 x BN fp32 accumulator in registers (BN / 2 per thread).
+//
+// The 256-wide tile stages its output through kWideSlabs slabs, in BN / 64 / kWideSlabs passes of the epilogue:
+// a stage is 48 KB there, and with two slabs (two 128-channel passes) four stages fit where four slabs leave three.
+constexpr int kWideSlabs = 2;
+constexpr int kWideProducerRegs = 40;   // setmaxnreg of the 256-wide tile: producer warpgroup ...
+constexpr int kWideConsumerRegs = 232;  // ... and the two consumer warpgroups; 128 x 40 + 256 x 232 <= 384 x 168
 template <int BN>
 struct TileCfg {
   static constexpr int kBBytes = BN * kBlockK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStagingBytes = (BN / 64) * kSlabBytes;
+  static constexpr int kSlabs = BN > 128 ? kWideSlabs : BN / 64;  // staging slabs
+  static constexpr int kPasses = BN / 64 / kSlabs;                // epilogue passes through them
+  static constexpr int kStagingBytes = kSlabs * kSlabBytes;
   static constexpr int kRing = kSmemOptIn - kStagingBytes - 1024 /*align slack*/ - 256 /*barriers*/;
   static constexpr int kStages = (kRing / kStageBytes) > 8 ? 8 : (kRing / kStageBytes);
   static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + 1024 + 256;
   static_assert(kSmemBytes <= kSmemOptIn, "tile configuration exceeds the 227 KB opt-in shared memory");
+  static_assert(kPasses * kSlabs * 64 == BN, "the epilogue passes must cover the tile's channels");
 };
 
 // Persistent, warp-specialised: thread 0 streams (A, B) k-blocks through a ring of TMA stages; the two consumer
 // warpgroups issue m64nBNk16 wgmmas from it, then run the epilogue (+bias, +residual, ReLU, +pos.emb. -> fp16 ->
 // 128B-swizzled slabs -> one TMA tensor store per 64-channel slab).  The producer runs ahead into the next tile while
-// the consumers drain this one.
+// the consumers drain this one.  The 256-wide tile moves registers from the producer warpgroup to the consumers
+// (128 accumulators per thread do not fit the 168 a 384-thread CTA gets).
 template <int BN>
 __global__ void __launch_bounds__(kTileThreads, 1)
     gemm_tile_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
@@ -167,7 +178,8 @@ __global__ void __launch_bounds__(kTileThreads, 1)
                      const __grid_constant__ GemmParams p) {
   using Cfg = TileCfg<BN>;
   constexpr int S = Cfg::kStages;
-  constexpr int NSLAB = BN / 64;
+  constexpr int NSLAB = Cfg::kSlabs;
+  constexpr int JP = BN / 8 / Cfg::kPasses;  // 8-column accumulator groups per epilogue pass
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* staging = smem + S * Cfg::kStageBytes;  // [NSLAB][kSlabBytes], 1024-aligned
@@ -205,6 +217,7 @@ __global__ void __launch_bounds__(kTileThreads, 1)
 
   if (threadIdx.x < 128) {
     // ------------------------------------------------------------------ TMA producer
+    if constexpr (BN > 128) regs_release<kWideProducerRegs>();  // all four warps, before three of them leave
     if (threadIdx.x == 0) {
       int stage = 0, phase = 0;
       for (int t = blockIdx.x; t < total; t += gridDim.x) {
@@ -237,6 +250,7 @@ __global__ void __launch_bounds__(kTileThreads, 1)
   }
 
   // -------------------------------------------------------------------- consumers (warpgroups 1, 2)
+  if constexpr (BN > 128) regs_acquire<kWideConsumerRegs>();
   const int ct = threadIdx.x - 128;
   const int cw = ct >> 7;  // rows [64 cw, 64 cw + 64) of the tile
   const int lane = threadIdx.x & 31;
@@ -312,40 +326,55 @@ __global__ void __launch_bounds__(kTileThreads, 1)
         pap[h] = p.post_add + (size_t)(i * p.Wo + j) * p.Cout + n_tile * BN;
       }
     }
-    if (p.has_res) mbar_wait(res_full, (uint32_t)(it & 1));
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int col = 8 * j + cq;
-      const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col));
-      uint8_t* slab = staging + (j >> 3) * kSlabBytes;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = r0 + 8 * h;
-        uint32_t* cell = reinterpret_cast<uint32_t*>(slab + row * 128 + ((((uint32_t)j & 7u) ^ (uint32_t)(row & 7)) << 4) + cq * 2);
-        float a0 = acc[4 * j + 2 * h] + b.x, a1 = acc[4 * j + 2 * h + 1] + b.y;
-        if (p.has_res) {
-          const float2 r = __half22float2(*reinterpret_cast<const __half2*>(cell));
-          a0 += r.x;
-          a1 += r.y;
+    for (int ps = 0; ps < Cfg::kPasses; ++ps) {  // channels [ps * 64 NSLAB, (ps + 1) * 64 NSLAB) of the tile
+      const int c0 = n_tile * BN + ps * NSLAB * 64;
+      if (ps > 0) {
+        // the previous pass's stores have left the slabs: this pass's residual goes into them
+        if (leader) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (leader && p.has_res) {
+          mbar_expect_tx(res_full, NSLAB * kSlabBytes);
+          for (int s = 0; s < NSLAB; ++s)
+            tma_load_5d(&map_res, res_full, staging + s * kSlabBytes, c0 + s * 64, rc[1], rc[2], rc[3], rc[4]);
         }
-        if (p.relu) {
-          a0 = fmaxf(a0, 0.f);
-          a1 = fmaxf(a1, 0.f);
-        }
-        if (pap[h]) {
-          const float2 pe = __ldg(reinterpret_cast<const float2*>(pap[h] + col));
-          a0 += pe.x;
-          a1 += pe.y;
-        }
-        *cell = pack_half2(a0, a1);
       }
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> async proxy
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    if (leader) {
-      for (int s = 0; s < NSLAB; ++s)
-        tma_store_5d(&map_out, staging + s * kSlabBytes, coff + n_tile * BN + s * 64, oc[1], oc[2], oc[3], oc[4]);
-      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+      if (p.has_res) mbar_wait(res_full, (uint32_t)((it * Cfg::kPasses + ps) & 1));
+#pragma unroll
+      for (int jl = 0; jl < JP; ++jl) {
+        const int j = ps * JP + jl;
+        const int col = 8 * j + cq;
+        const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col));
+        uint8_t* slab = staging + (jl >> 3) * kSlabBytes;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = r0 + 8 * h;
+          uint32_t* cell = reinterpret_cast<uint32_t*>(slab + row * 128 + ((((uint32_t)j & 7u) ^ (uint32_t)(row & 7)) << 4) + cq * 2);
+          float a0 = acc[4 * j + 2 * h] + b.x, a1 = acc[4 * j + 2 * h + 1] + b.y;
+          if (p.has_res) {
+            const float2 r = __half22float2(*reinterpret_cast<const __half2*>(cell));
+            a0 += r.x;
+            a1 += r.y;
+          }
+          if (p.relu) {
+            a0 = fmaxf(a0, 0.f);
+            a1 = fmaxf(a1, 0.f);
+          }
+          if (pap[h]) {
+            const float2 pe = __ldg(reinterpret_cast<const float2*>(pap[h] + col));
+            a0 += pe.x;
+            a1 += pe.y;
+          }
+          *cell = pack_half2(a0, a1);
+        }
+      }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> async proxy
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (leader) {
+        for (int s = 0; s < NSLAB; ++s)
+          tma_store_5d(&map_out, staging + s * kSlabBytes, coff + c0 + s * 64, oc[1], oc[2], oc[3], oc[4]);
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+      }
     }
   }
   if (leader) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // smem must outlive the stores
@@ -445,8 +474,15 @@ static int launch_bn(const CUtensorMap& ma, const CUtensorMap& mb, const CUtenso
 
 int stem_conv_launch(const GemmLayer& L, cudaStream_t stream);  // fp_stem.cu
 
-int gemm_layer_launch(const GemmLayer& L, cudaStream_t stream) {
-  if (L.kind == LK_CONV7_S2) return stem_conv_launch(L, stream);
+// Plans the layer and launches it, or, with `tile_n`, only reports the tile width the launch would use.
+static int gemm_layer_plan(const GemmLayer& L, cudaStream_t stream, int* tile_n) {
+  if (L.kind == LK_CONV7_S2) {
+    if (tile_n) {
+      *tile_n = 64;  // the stem kernel's 128-pixel x 64-channel tile
+      return 0;
+    }
+    return stem_conv_launch(L, stream);
+  }
   GemmParams p;
   memset(&p, 0, sizeof(p));
   CUtensorMap ma, mb;
@@ -529,8 +565,21 @@ int gemm_layer_launch(const GemmLayer& L, cudaStream_t stream) {
   p.lg_bw = ilog2(p.bw);
   p.lg_bh = ilog2(p.bh);
 
-  // 128 channels per tile: two 64 x 128 register accumulators per CTA (64 fp32 registers per thread)
-  if (L.Cout % 128 == 0) BN = 128;
+  // 128 channels per tile: two 64 x 128 register accumulators per CTA (64 fp32 registers per thread).  256 channels
+  // when the 256-wide grid still fills kWideMinWaves waves of persistent CTAs and the k-loop is long: the wide tile
+  // reads half the weight bytes per FLOP, but it halves the CTA count, its last, partial wave costs relatively more
+  // on a short grid, and its two-pass epilogue is not hidden behind a short k-loop.  Measured per layer on an H100
+  // SXM at 700 W against the 128-wide tile, the 3x3 convolutions (K = 2304 / 4608) are +7 to +13 % at 9 wide waves,
+  // +16 to +24 % at 12 to 24 (252 hypotheses), even at 6 and about 10 % slower at 3 (a 32-hypothesis shard;
+  // track_one's single image is under one wave); the K = 512 linear layers (8 k-blocks) were no faster at any height.
+  constexpr int kWideMinWaves = 8;
+  constexpr int kWideMinKBlocks = 16;
+  const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
+  if (L.Cout % 256 == 0 && p.num_kb >= kWideMinKBlocks) {
+    const int sms = num_sms();
+    FP_REQUIRE(sms > 0, "no CUDA device");
+    BN = (long long)m_tiles * (L.Cout / 256) >= (long long)kWideMinWaves * sms ? 256 : 128;
+  } else if (L.Cout % 128 == 0) BN = 128;
   else if (L.Cout % 64 == 0) BN = 64;
   else FP_REQUIRE(false, "Cout=%d must be a multiple of 64", L.Cout);
   p.n_tiles_n = L.Cout / BN;
@@ -549,6 +598,10 @@ int gemm_layer_launch(const GemmLayer& L, cudaStream_t stream) {
   FP_REQUIRE(L.out_split == 0 || L.out_split % p.bn == 0,
              "out_split=%d must be a multiple of the tile's image count %d (pad the A/B batch boundary)", L.out_split,
              p.bn);
+  if (tile_n) {
+    *tile_n = BN;
+    return 0;
+  }
   if (p.total_tiles == 0) return 0;
 
   int rc = encode_map(&ma, L.in, 5, dims, str, box);
@@ -595,7 +648,12 @@ int gemm_layer_launch(const GemmLayer& L, cudaStream_t stream) {
       mr = mo;
     }
   }
+  if (BN == 256) return launch_bn<256>(ma, mb, mo, mr, p, stream);
   return BN == 128 ? launch_bn<128>(ma, mb, mo, mr, p, stream) : launch_bn<64>(ma, mb, mo, mr, p, stream);
 }
+
+int gemm_layer_launch(const GemmLayer& L, cudaStream_t stream) { return gemm_layer_plan(L, stream, nullptr); }
+
+int gemm_layer_tile_n(const GemmLayer& L, int* tile_n) { return gemm_layer_plan(L, nullptr, tile_n); }
 
 }  // namespace fp

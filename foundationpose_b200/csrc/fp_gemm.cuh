@@ -39,6 +39,8 @@ struct GemmLayer {
 
 // Enqueue one layer on `stream`.  Returns 0 or a negative error code (fp_last_error() has text).
 int gemm_layer_launch(const GemmLayer& L, cudaStream_t stream);
+// The output channels per tile (64, 128 or 256) gemm_layer_launch would use for L; launches nothing.
+int gemm_layer_tile_n(const GemmLayer& L, int* tile_n);
 
 
 // Optional per-launch device timing (CUDA events on the launching stream) of the two kernels the

@@ -45,6 +45,16 @@ def gemm_layer(kind, x, w_packed, bias, *, n_img, Hin, Win, Cin, Cout, out=None,
     return out
 
 
+def gemm_tile_n(kind, *, n_img, Hin, Win, Cin, Cout, out_split=0):
+    """Output channels per tile (64, 128 or 256) that `gemm_layer` picks for this shape on the current device."""
+    lib.fp_op_gemm_tile_n.argtypes = [C.POINTER(_lib.GemmLayer), C.POINTER(C.c_int)]
+    lib.fp_op_gemm_tile_n.restype = C.c_int
+    L = _lib.GemmLayer(kind, n_img, Hin, Win, Cin, Cout, None, None, None, None, 0, None, Cout, out_split, None, 0)
+    tile_n = C.c_int(0)
+    _lib.check(lib.fp_op_gemm_tile_n(C.byref(L), C.byref(tile_n)), "fp_op_gemm_tile_n")
+    return tile_n.value
+
+
 lib.fp_op_attention.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
 lib.fp_op_attention.restype = C.c_int
 

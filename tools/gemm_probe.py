@@ -94,15 +94,19 @@ def run_case(case):
                   ("conv3s2 64->128 @80 (504)", _lib.LAYER_CONV3_S2, 504, 80, 64, 128, 576),
                   ("conv3 128 @40 (504)", _lib.LAYER_CONV3_S1, 504, 40, 128, 128, 1152),
                   ("conv3 256 @40 (252)", _lib.LAYER_CONV3_S1, 252, 40, 256, 256, 2304),
+                  ("conv3 256 @40 (249, odd M tiles)", _lib.LAYER_CONV3_S1, 249, 40, 256, 256, 2304),
                   ("conv3s2 256->512 @40 (252)", _lib.LAYER_CONV3_S2, 252, 40, 256, 512, 2304),
                   ("conv3 512 @20 (252)", _lib.LAYER_CONV3_S1, 252, 20, 512, 512, 4608),
                   ("linear 512->1536 (100800 rows)", _lib.LAYER_LINEAR, 1, 100800, 512, 1536, 512),
+                  ("linear 512->3072 (100800 rows)", _lib.LAYER_LINEAR, 1, 100800, 512, 3072, 512),
                   ("conv3 128 @40 (504) +res", _lib.LAYER_CONV3_S1, 504, 40, 128, 128, 1152),
                   ("conv3 256 @40 (252) +res", _lib.LAYER_CONV3_S1, 252, 40, 256, 256, 2304),
                   ("conv3 512 @20 (252) +res", _lib.LAYER_CONV3_S1, 252, 20, 512, 512, 4608),
+                  ("conv3 512 @20 (252) +res +pe", _lib.LAYER_CONV3_S1, 252, 20, 512, 512, 4608),
                   ("linear 512->512 (100800) +res", _lib.LAYER_LINEAR, 1, 100800, 512, 512, 512)]
         for name, kind, n, H, Ci, Co, Kreal in shapes:
-            use_res = name.endswith("+res")
+            use_res = "+res" in name
+            use_pe = "+pe" in name
             if kind == _lib.LAYER_LINEAR:
                 x = torch.randn(H, Ci, device=dev).half()
                 w = torch.randn(Co, Ci, device=dev).half()
@@ -123,6 +127,12 @@ def run_case(case):
             out = torch.empty(M * Co, device=dev, dtype=torch.float16)
             if use_res:
                 kw.update(res=torch.randn(M * Co, device=dev).half(), res_ld=Co)
+            if use_pe:
+                kw.update(post_add=torch.randn(Ho * Ho, Co, device=dev))
+            # tile configuration the layer runs with ("-" for a library that predates the query)
+            tile_n = "-"
+            if getattr(_lib.lib, "fp_op_gemm_tile_n", None) is not None:
+                tile_n = f"128x{ops.gemm_tile_n(kind, n_img=kw['n_img'], Hin=kw['Hin'], Win=kw['Win'], Cin=Ci, Cout=Co)}"
             for _ in range(3):
                 ops.gemm_layer(kind, x, w, b, out=out, out_ld=Co, relu=True, **kw)
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -133,7 +143,7 @@ def run_case(case):
             torch.cuda.synchronize()
             ms = e0.elapsed_time(e1) / 10
             fl = 2.0 * M * Co * Kreal
-            print(f"[perf] {name:34s} {ms:8.3f} ms  {fl / ms / 1e9:8.1f} TFLOP/s (algorithmic)")
+            print(f"[perf] {name:34s} tile {tile_n:7s} {ms:8.3f} ms  {fl / ms / 1e9:8.1f} TFLOP/s (algorithmic)")
     print(f"[{case}] {'OK' if ok else 'FAIL'}")
     return ok
 
