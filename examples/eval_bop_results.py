@@ -1,0 +1,131 @@
+"""ADD / ADD-S tables for the result files of the dataset drivers (run_linemod.py -> linemod_res.yml, run_ycb_video.py ->
+ycbv_res.yml, examples/run_linemod_replicas.py), scored on the GPU.
+
+    python examples/eval_bop_results.py --res debug/linemod_res.yml --dataset_dir <LINEMOD root> [--json table.json]
+    python examples/eval_bop_results.py --res debug/ycbv_res.yml --dataset_dir <YCB_Video root> [--kind ycbv]
+
+A result file maps video id -> frame id string -> object id -> 4x4 estimated pose.  The ground truth comes from the
+drop-in readers (`get_gt_pose`), the model points from `get_gt_mesh(ob_id).vertices`; all poses of one object go to
+one `fp_pose_errors` call.  A frame the driver skipped (it writes the identity) counts as a failure: its errors are
+infinite.  An object is symmetric when the reader's `symmetry_tfs[ob_id]` holds more than the identity.  Printed per
+object and overall: the number of poses, ADD and ADD-S AUC (up to 0.1 m in 1 mm steps) and ADD(-S) < 0.1 d (ADD-S for
+symmetric objects, d = `get_model_diameter`).
+"""
+import argparse
+import json
+import os
+import sys
+from collections import defaultdict
+
+import numpy as np
+import yaml
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [os.path.join(ROOT, "foundationpose_b200", "dropin"), ROOT]
+
+from foundationpose_b200 import metrics  # noqa: E402
+
+
+def load_results(path):
+    with open(path) as fh:
+        return yaml.safe_load(fh) or {}
+
+
+def group_by_object(res):
+    """{ob_id: [(video_id, id_str, pose 4x4 float64, skipped)]} in video, frame order."""
+    groups = defaultdict(list)
+    for video_id in sorted(res, key=int):
+        for id_str in sorted(res[video_id], key=str):
+            for ob_id, pose in res[video_id][id_str].items():
+                pose = np.asarray(pose, dtype=np.float64).reshape(4, 4)
+                groups[int(ob_id)].append((int(video_id), str(id_str), pose, bool(np.array_equal(pose, np.eye(4)))))
+    return dict(sorted(groups.items()))
+
+
+def is_symmetric(symmetry_tfs):
+    tfs = np.asarray(symmetry_tfs, dtype=np.float64).reshape(-1, 4, 4)
+    return any(not np.allclose(tf, np.eye(4)) for tf in tfs)
+
+
+def summarize(add, adds, symmetric, diameter):
+    """One table row from per-pose errors (inf for failures)."""
+    add, adds = np.asarray(add, dtype=np.float64), np.asarray(adds, dtype=np.float64)
+    return {"poses": int(len(add)), "add_auc": metrics.auc(add), "adds_auc": metrics.auc(adds),
+            "add_s_recall": metrics.recall(adds if symmetric else add, 0.1 * diameter), "symmetric": bool(symmetric),
+            "diameter": float(diameter)}
+
+
+def summarize_all(rows, errors):
+    """Overall row: AUCs over every pose, ADD(-S) < 0.1 d with each pose's own metric and diameter."""
+    add = np.concatenate([errors[o][0] for o in rows])
+    adds = np.concatenate([errors[o][1] for o in rows])
+    crit = np.concatenate([errors[o][1] if rows[o]["symmetric"] else errors[o][0] for o in rows])
+    thr = np.concatenate([np.full(rows[o]["poses"], 0.1 * rows[o]["diameter"]) for o in rows])
+    return {"poses": int(len(add)), "add_auc": metrics.auc(add), "adds_auc": metrics.auc(adds),
+            "add_s_recall": metrics.recall(crit, thr)}
+
+
+def make_reader_factory(kind, dataset_dir):
+    from datareader import LinemodReader, YcbVideoReader
+
+    cache = {}
+
+    def reader(video_id):
+        if video_id not in cache:
+            if kind == "lm":
+                cache[video_id] = LinemodReader(os.path.join(dataset_dir, "lm_test_all", "test", f"{video_id:06d}"), split=None)
+            else:
+                os.environ.setdefault("YCB_VIDEO_DIR", dataset_dir)
+                cache[video_id] = YcbVideoReader(os.path.join(dataset_dir, "test", f"{video_id:06d}"))
+        return cache[video_id]
+
+    return reader
+
+
+def evaluate(res, kind, dataset_dir):
+    """-> (rows {ob_id: row}, overall row, errors {ob_id: (add [n], adds [n])})."""
+    reader = make_reader_factory(kind, dataset_dir)
+    rows, errors = {}, {}
+    for ob_id, entries in group_by_object(res).items():
+        r0 = reader(entries[0][0])
+        frame = {vid: {s: i for i, s in enumerate(reader(vid).id_strs)} for vid in {e[0] for e in entries}}
+        gt = np.stack([reader(vid).get_gt_pose(frame[vid][id_str], ob_id) for vid, id_str, _, _ in entries])
+        pred = np.stack([e[2] for e in entries])
+        skipped = np.array([e[3] for e in entries])
+        add, adds = metrics.pose_errors(r0.get_gt_mesh(ob_id).vertices, pred, gt)
+        add, adds = add.double().cpu().numpy(), adds.double().cpu().numpy()
+        add[skipped], adds[skipped] = np.inf, np.inf
+        errors[ob_id] = (add, adds)
+        rows[ob_id] = summarize(add, adds, is_symmetric(r0.symmetry_tfs[ob_id]), r0.get_model_diameter(ob_id))
+    return rows, summarize_all(rows, errors) if rows else None, errors
+
+
+def print_table(rows, overall):
+    print(f"{'object':>8} {'poses':>6} {'ADD AUC':>8} {'ADD-S AUC':>10} {'ADD(-S)<0.1d':>13}")
+    for ob_id, r in rows.items():
+        tag = f"{ob_id}{'*' if r['symmetric'] else ''}"
+        print(f"{tag:>8} {r['poses']:6d} {100 * r['add_auc']:8.2f} {100 * r['adds_auc']:10.2f} {100 * r['add_s_recall']:13.2f}")
+    if overall:
+        print(f"{'all':>8} {overall['poses']:6d} {100 * overall['add_auc']:8.2f} {100 * overall['adds_auc']:10.2f} "
+              f"{100 * overall['add_s_recall']:13.2f}")
+    print("(percent; * = symmetric object, scored by ADD-S in the last column)")
+
+
+def main(argv=None):
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--res", required=True, help="linemod_res.yml / ycbv_res.yml written by a dataset driver")
+    ap.add_argument("--dataset_dir", required=True, help="the --linemod_dir / --ycbv_dir the driver ran on")
+    ap.add_argument("--kind", choices=("lm", "ycbv"), default=None, help="default: ycbv if the file name says so, else lm")
+    ap.add_argument("--json", default=None, help="also write the table as JSON here")
+    opt = ap.parse_args(argv)
+    kind = opt.kind or ("ycbv" if "ycbv" in os.path.basename(opt.res) else "lm")
+    rows, overall, _ = evaluate(load_results(opt.res), kind, opt.dataset_dir)
+    print_table(rows, overall)
+    if opt.json:
+        with open(opt.json, "w") as fh:
+            json.dump({"objects": {str(k): v for k, v in rows.items()}, "overall": overall}, fh, indent=1)
+    return rows, overall
+
+
+if __name__ == "__main__":
+    main()

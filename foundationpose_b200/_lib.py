@@ -57,6 +57,9 @@ lib.fp_last_error.restype = C.c_char_p
 lib.fp_launch_count.restype = C.c_ulonglong
 lib.fp_op_gemm_layer.argtypes = [C.POINTER(GemmLayer), C.c_void_p]
 lib.fp_op_gemm_layer.restype = C.c_int
+lib.fp_pose_errors.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                               C.c_void_p]
+lib.fp_pose_errors.restype = C.c_int
 
 
 def check(rc, what=""):

@@ -11,6 +11,30 @@
 namespace fp {
 const char* get_last_error();
 int prof_collect(int kind, double* total_ms, double* total_work, int* launches);
+int pose_errors_launch(const float* pts, int P, const float* pred, int N, const float* gt, int n_gt, float* add_out,
+                       float* adds_out, cudaStream_t stream);
+}
+
+// 0 when `p` is memory a kernel on the current device may read and write, else -1 with the reason in fp_last_error()
+static int check_device_ptr(const void* p, const char* what) {
+  int dev = 0;
+  FP_CUDA_OK(cudaGetDevice(&dev));
+  cudaPointerAttributes a;
+  const cudaError_t e = cudaPointerGetAttributes(&a, p);
+  if (e != cudaSuccess) {
+    cudaGetLastError();  // not sticky; keep it out of the next caller's error check
+    fp::set_last_error("fp_pose_errors: %s: cudaPointerGetAttributes failed (%s)", what, cudaGetErrorString(e));
+    return -1;
+  }
+  if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) {
+    fp::set_last_error("fp_pose_errors: %s is not device memory", what);
+    return -1;
+  }
+  if (a.type == cudaMemoryTypeDevice && a.device != dev) {
+    fp::set_last_error("fp_pose_errors: %s lives on device %d, the current device is %d", what, a.device, dev);
+    return -1;
+  }
+  return 0;
 }
 
 extern "C" {
@@ -151,6 +175,20 @@ int fp_op_gemm_tile_n(const fp_gemm_layer_t* l, int* tile_n) {
     return -1;
   }
   return fp::gemm_layer_tile_n(to_gemm_layer(l), tile_n);
+}
+
+int fp_pose_errors(const float* pts, int P, const float* pred, int N, const float* gt, int n_gt, float* add_out,
+                   float* adds_out, void* stream) {
+  FP_REQUIRE(P >= 1 && P <= FP_METRICS_MAX_POINTS, "fp_pose_errors: P = %d outside [1, %d]", P, FP_METRICS_MAX_POINTS);
+  FP_REQUIRE(N >= 0 && N <= FP_METRICS_MAX_POSES, "fp_pose_errors: N = %d outside [0, %d]", N, FP_METRICS_MAX_POSES);
+  FP_REQUIRE(n_gt == 1 || n_gt == N, "fp_pose_errors: n_gt = %d, must be 1 or N = %d", n_gt, N);
+  if (N == 0) return 0;
+  FP_REQUIRE(pts && pred && gt, "fp_pose_errors: null input pointer");
+  const void* ptrs[5] = {pts, pred, gt, add_out, adds_out};
+  const char* names[5] = {"pts", "pred", "gt", "add_out", "adds_out"};
+  for (int i = 0; i < 5; ++i)
+    if (ptrs[i] && check_device_ptr(ptrs[i], names[i])) return -1;
+  return fp::pose_errors_launch(pts, P, pred, N, gt, n_gt, add_out, adds_out, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -13,6 +13,8 @@ Only the surface the drivers touch is provided (the reference's Utils.py is 1000
   dataset runs   argparse, NestDict (:60-61), make_yaml_dumpable (:996-1020), symmetry_tfs_from_info (:806-834),
                  euler_matrix (the `transformations` package's static-xyz convention), wp (warp stand-in: force_load)
                  — what run_linemod.py / run_ycb_video.py and the BOP readers use unqualified
+  pose accuracy  add_err (:232-240), adds_err (:243-253) — on the GPU (fp_pose_errors), fp32 —, compute_auc_sklearn
+                 (:256-266, without sklearn)
 trimesh and imageio are the real packages when installed, else the minimal stand-ins under _fallback/.
 """
 import argparse  # noqa: F401
@@ -62,6 +64,7 @@ except ImportError:
 
 from foundationpose_b200 import hypotheses as _hyp  # noqa: E402
 from foundationpose_b200 import meshprep as _meshprep  # noqa: E402
+from foundationpose_b200 import metrics as _metrics  # noqa: E402
 from foundationpose_b200.estimater import make_mesh_tensors  # noqa: E402,F401
 
 
@@ -207,6 +210,23 @@ def compute_mesh_diameter(model_pts=None, mesh=None, n_sample=1000):
     to run above 10 000 vertices); this one is exact."""
     pts = np.asarray(mesh.vertices if mesh is not None else model_pts)
     return float(_meshprep.mesh_diameter(pts))
+
+
+def add_err(pred, gt, model_pts, symetry_tfs=np.eye(4)[None]):
+    """ADD: mean distance between the model points under `pred` and under `gt` (4x4 poses, model_pts (P,3)).
+    `symetry_tfs` is accepted and ignored, as in the reference."""
+    add, _ = _metrics.pose_errors(model_pts, pred, gt, add=True, adds=False)
+    return float(add[0])
+
+
+def adds_err(pred, gt, model_pts):
+    """ADD-S: mean over the model points under `gt` of the distance to the nearest model point under `pred`."""
+    _, adds = _metrics.pose_errors(model_pts, pred, gt, add=False, adds=True)
+    return float(adds[0])
+
+
+def compute_auc_sklearn(errs, max_val=0.1, step=0.001):
+    return _metrics.auc(errs, max_val=max_val, step=step)
 
 
 def sample_views_icosphere(n_views, subdivisions=None, radius=1):

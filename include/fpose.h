@@ -81,6 +81,25 @@ int fp_op_attention(const void* qkv, void* out, int B, int impl, void* stream);
 
 
 /* ------------------------------------------------------------------------------------------ */
+/* pose accuracy                                                                              */
+/* ------------------------------------------------------------------------------------------ */
+
+/* Largest model and batch fp_pose_errors accepts: every point coordinate index (3 P) and pose element index (16 N)
+ * stays in `int`, and the grid (8 N CTAs) within the launch limits. */
+#define FP_METRICS_MAX_POINTS 131072
+#define FP_METRICS_MAX_POSES (1 << 24)
+/* ADD / ADD-S (Utils.py:232-253) of N poses against n_gt (1 or N) ground-truth poses over P model points, on the
+ * current device.  pts [P][3], pred [N][16], gt [n_gt][16] row-major, outputs [N]: DEVICE float32.  add_out or
+ * adds_out may be NULL (not computed).  1 <= P <= FP_METRICS_MAX_POINTS, 0 <= N <= FP_METRICS_MAX_POSES.
+ *   ADD   = mean_i |(R_p x_i + t_p) - (R_g x_i + t_g)|      (the reference's unused symetry_tfs is not an argument)
+ *   ADD-S = mean_i min_j |(R_g x_i + t_g) - (R_p x_j + t_p)|   (ground-truth points query the estimated points)
+ * fp32 distances of the transformed points, fp64 means.  Deterministic: a pose's errors do not depend on N, on n_gt
+ * or on the call.  ADD alone costs O(N P); ADD-S O(N P^2).  Every pointer must be device memory of the current device
+ * (cudaPointerGetAttributes); all arguments are checked before anything is enqueued.  Enqueued on `stream`; no sync. */
+int fp_pose_errors(const float* pts, int P, const float* pred, int N, const float* gt, int n_gt,
+                   float* add_out, float* adds_out, void* stream);
+
+/* ------------------------------------------------------------------------------------------ */
 /* product path                                                                               */
 /* ------------------------------------------------------------------------------------------ */
 typedef struct fp_ctx fp_ctx;
