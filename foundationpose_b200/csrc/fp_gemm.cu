@@ -17,8 +17,9 @@
 //     unit, which implements the zero padding.  Stride-2 convolutions use a (2C, W/2, 2, H/2, N) view of the same
 //     memory so that every tap is again a dense box; the 7x7/s2 stem has its own kernel (fp_stem.cu).  No im2col
 //     buffer is ever materialised.
-//   * Epilogue: registers -> +bias/+residual/ReLU/+PE -> fp16 -> 128B-swizzled smem slabs -> TMA tensor store; the
-//     residual tile arrives by TMA into the same slabs while the tile's main loop runs.
+//   * Epilogue: registers -> +bias/+residual/ReLU/+PE -> fp16 -> 128B-swizzled smem slabs -> TMA tensor store, in
+//     64-channel batches; the residual arrives by TMA into the same slabs, as much of it as the slabs hold while the
+//     tile's main loop runs.
 #include "fp_gemm.cuh"
 
 #include <stdarg.h>
@@ -147,8 +148,10 @@ constexpr int kSmemOptIn = 232448;              // 227 KB opt-in shared memory p
 // BN = output channels per tile (64, 128 or 256).  Each consumer warpgroup owns 64 of the tile's 128 pixel rows and
 // keeps its 64 x BN fp32 accumulator in registers (BN / 2 per thread).
 //
-// The 256-wide tile stages its output through kWideSlabs slabs, in BN / 64 / kWideSlabs passes of the epilogue:
-// a stage is 48 KB there, and with two slabs (two 128-channel passes) four stages fit where four slabs leave three.
+// The epilogue converts the tile in 64-channel batches, one staging slab each.  The 64- and 128-wide tiles have a
+// slab per batch and store them all at the end.  The 256-wide tile has two slabs (a stage is 48 KB there, and with
+// two slabs four stages fit where four slabs leave three) and stores each batch as its own pass, alternating between
+// the slabs, so that one slab's store and the next batch's residual load run while the other slab is converted.
 constexpr int kWideSlabs = 2;
 constexpr int kWideProducerRegs = 40;   // setmaxnreg of the 256-wide tile: producer warpgroup ...
 constexpr int kWideConsumerRegs = 232;  // ... and the two consumer warpgroups; 128 x 40 + 256 x 232 <= 384 x 168
@@ -156,14 +159,16 @@ template <int BN>
 struct TileCfg {
   static constexpr int kBBytes = BN * kBlockK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kSlabs = BN > 128 ? kWideSlabs : BN / 64;  // staging slabs
-  static constexpr int kPasses = BN / 64 / kSlabs;                // epilogue passes through them
+  static constexpr int kBatches = BN / 64;                         // 64-channel epilogue batches
+  static constexpr bool kAlternate = BN > 128;                     // one pass per batch, through alternating slabs
+  static constexpr int kSlabs = kAlternate ? kWideSlabs : kBatches;  // staging slabs
   static constexpr int kStagingBytes = kSlabs * kSlabBytes;
   static constexpr int kRing = kSmemOptIn - kStagingBytes - 1024 /*align slack*/ - 256 /*barriers*/;
   static constexpr int kStages = (kRing / kStageBytes) > 8 ? 8 : (kRing / kStageBytes);
   static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + 1024 + 256;
   static_assert(kSmemBytes <= kSmemOptIn, "tile configuration exceeds the 227 KB opt-in shared memory");
-  static_assert(kPasses * kSlabs * 64 == BN, "the epilogue passes must cover the tile's channels");
+  static_assert((2 * kStages + kSlabs) * 8 <= 256, "the mbarriers must fit their 256 bytes");
+  static_assert(kBatches % kSlabs == 0, "every slab must take the same number of batches per tile");
 };
 
 // Persistent, warp-specialised: thread 0 streams (A, B) k-blocks through a ring of TMA stages; the two consumer
@@ -179,14 +184,16 @@ __global__ void __launch_bounds__(kTileThreads, 1)
   using Cfg = TileCfg<BN>;
   constexpr int S = Cfg::kStages;
   constexpr int NSLAB = Cfg::kSlabs;
-  constexpr int JP = BN / 8 / Cfg::kPasses;  // 8-column accumulator groups per epilogue pass
+  constexpr int NB = Cfg::kBatches;
+  constexpr bool kAlt = Cfg::kAlternate;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // offset from the __shared__ array itself, so that the compiler sees every access below as shared memory
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* staging = smem + S * Cfg::kStageBytes;  // [NSLAB][kSlabBytes], 1024-aligned
   uint64_t* bars = reinterpret_cast<uint64_t*>(staging + Cfg::kStagingBytes);
   uint64_t* full = bars;          // [S]
   uint64_t* empty = bars + S;     // [S]
-  uint64_t* res_full = bars + 2 * S;
+  uint64_t* res_full = bars + 2 * S;  // [NSLAB] with kAlt (one per slab), else [1] (all slabs)
 
   const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
   const int total = m_tiles * p.n_tiles_n;
@@ -200,7 +207,7 @@ __global__ void __launch_bounds__(kTileThreads, 1)
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], 256);
     }
-    mbar_init(res_full, 1);
+    for (int s = 0; s < (kAlt ? NSLAB : 1); ++s) mbar_init(&res_full[s], 1);
     mbar_fence_init();
   }
   __syncthreads();
@@ -278,14 +285,16 @@ __global__ void __launch_bounds__(kTileThreads, 1)
       oc[p.odim_n] = n_o0;
       rc[p.odim_n] = n0;
     }
-    // the previous tile's stores have left the staging slabs: fetch this tile's residual into them now, while the
-    // main loop runs
+    // the previous tile's stores have left the staging slabs: fetch the residual of the tile's first NSLAB batches
+    // into them now, while the main loop runs (kAlt: one barrier per slab, else one for all)
     if (leader) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
     asm volatile("bar.sync 1, 256;" ::: "memory");
     if (leader && p.has_res) {
-      mbar_expect_tx(res_full, NSLAB * kSlabBytes);
-      for (int s = 0; s < NSLAB; ++s)
-        tma_load_5d(&map_res, res_full, staging + s * kSlabBytes, n_tile * BN + s * 64, rc[1], rc[2], rc[3], rc[4]);
+      for (int s = 0; s < NSLAB; ++s) {
+        uint64_t* rb = &res_full[kAlt ? s : 0];
+        if (kAlt || s == 0) mbar_expect_tx(rb, kAlt ? kSlabBytes : NSLAB * kSlabBytes);
+        tma_load_5d(&map_res, rb, staging + s * kSlabBytes, n_tile * BN + s * 64, rc[1], rc[2], rc[3], rc[4]);
+      }
     }
 
     // ---- main loop: one wgmma batch (4 x K = 16) per k-block; a stage is released once the NEXT batch is issued
@@ -310,11 +319,9 @@ __global__ void __launch_bounds__(kTileThreads, 1)
         phase ^= 1;
       }
     }
-    wgmma_wait<0>();
-    fence_regs(acc);
-    if (prev >= 0) mbar_arrive(&empty[prev]);
-
-    // ---- epilogue
+    // ---- epilogue: 64-channel batches b, channels [64 b, 64 b + 64) of the tile, each converted into one slab.
+    // Every load of a batch (bias, residual, positional embedding) is issued before the batch's first conversion,
+    // so their latencies overlap instead of adding up element by element.
     const float* bias = p.bias + n_tile * BN;
     const float* pap[2] = {nullptr, nullptr};  // positional-embedding rows of this thread's two pixels
     if (p.post_add) {
@@ -326,54 +333,93 @@ __global__ void __launch_bounds__(kTileThreads, 1)
         pap[h] = p.post_add + (size_t)(i * p.Wo + j) * p.Cout + n_tile * BN;
       }
     }
+    // positional embedding of one batch in registers: batch 0's issued while the last wgmma batch drains, batch
+    // b + 1's as soon as batch b is converted (for the 256-wide tile, ahead of that pass's barrier and store)
+    float2 pe[8][2];
+    auto load_pe = [&](int b) {
 #pragma unroll
-    for (int ps = 0; ps < Cfg::kPasses; ++ps) {  // channels [ps * 64 NSLAB, (ps + 1) * 64 NSLAB) of the tile
-      const int c0 = n_tile * BN + ps * NSLAB * 64;
-      if (ps > 0) {
-        // the previous pass's stores have left the slabs: this pass's residual goes into them
-        if (leader) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (leader && p.has_res) {
-          mbar_expect_tx(res_full, NSLAB * kSlabBytes);
-          for (int s = 0; s < NSLAB; ++s)
-            tma_load_5d(&map_res, res_full, staging + s * kSlabBytes, c0 + s * 64, rc[1], rc[2], rc[3], rc[4]);
+      for (int jl = 0; jl < 8; ++jl)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) pe[jl][h] = __ldg(reinterpret_cast<const float2*>(pap[h] + 64 * b + 8 * jl + cq));
+    };
+    if (p.post_add) load_pe(0);
+    wgmma_wait<0>();
+    fence_regs(acc);
+    if (prev >= 0) mbar_arrive(&empty[prev]);
+
+#pragma unroll
+    for (int b = 0; b < NB; ++b) {
+      const int s = kAlt ? (b & 1) : b;
+      uint8_t* slab = staging + s * kSlabBytes;
+      if (kAlt && p.has_res && b > 0 && b + 1 < NB) {
+        // The other slab's last store (batch b - 1's) has been read out: batch b + 1's residual goes into it now,
+        // and arrives while this batch is converted.  Batches 0 and 1 were fetched during the main loop.
+        if (leader) {
+          asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+          uint64_t* rb = &res_full[(b + 1) & 1];
+          mbar_expect_tx(rb, kSlabBytes);
+          tma_load_5d(&map_res, rb, staging + ((b + 1) & 1) * kSlabBytes, n_tile * BN + (b + 1) * 64, rc[1], rc[2],
+                      rc[3], rc[4]);
         }
       }
-      if (p.has_res) mbar_wait(res_full, (uint32_t)((it * Cfg::kPasses + ps) & 1));
+      // Phase of the barrier that batch b waits on, in the CTA's it-th tile: it completes NB / NSLAB times per tile
+      // (kAlt: res_full[b & 1] twice, for batches b & 1 and (b & 1) + 2; otherwise res_full[0] once, for all slabs),
+      // so this is its completion it * (NB / NSLAB) + b / NSLAB.  Every thread waits each completion before the
+      // leader can start the next fill of the same barrier.
+      if (p.has_res && (kAlt || b == 0))
+        mbar_wait(&res_full[kAlt ? s : 0], (uint32_t)((it * (NB / NSLAB) + b / NSLAB) & 1));
 #pragma unroll
-      for (int jl = 0; jl < JP; ++jl) {
-        const int j = ps * JP + jl;
-        const int col = 8 * j + cq;
-        const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col));
-        uint8_t* slab = staging + (jl >> 3) * kSlabBytes;
+      for (int jh = 0; jh < 8; jh += 4) {  // four 8-column groups at a time: their loads first, then the arithmetic
+        float2 bb[4];
+        __half2 rv[4][2];
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = r0 + 8 * h;
-          uint32_t* cell = reinterpret_cast<uint32_t*>(slab + row * 128 + ((((uint32_t)j & 7u) ^ (uint32_t)(row & 7)) << 4) + cq * 2);
-          float a0 = acc[4 * j + 2 * h] + b.x, a1 = acc[4 * j + 2 * h + 1] + b.y;
+        for (int jl = 0; jl < 4; ++jl) {
+          bb[jl] = __ldg(reinterpret_cast<const float2*>(bias + 64 * b + 8 * (jh + jl) + cq));
           if (p.has_res) {
-            const float2 r = __half22float2(*reinterpret_cast<const __half2*>(cell));
-            a0 += r.x;
-            a1 += r.y;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = r0 + 8 * h;
+              rv[jl][h] = *reinterpret_cast<const __half2*>(slab + row * 128 + (((uint32_t)(jh + jl) ^ (uint32_t)(row & 7)) << 4) + cq * 2);
+            }
           }
-          if (p.relu) {
-            a0 = fmaxf(a0, 0.f);
-            a1 = fmaxf(a1, 0.f);
+        }
+#pragma unroll
+        for (int jl = 0; jl < 4; ++jl) {
+          const int j = 8 * b + jh + jl;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = r0 + 8 * h;
+            uint32_t* cell = reinterpret_cast<uint32_t*>(slab + row * 128 + (((uint32_t)(jh + jl) ^ (uint32_t)(row & 7)) << 4) + cq * 2);
+            float a0 = acc[4 * j + 2 * h] + bb[jl].x, a1 = acc[4 * j + 2 * h + 1] + bb[jl].y;
+            if (p.has_res) {
+              const float2 r = __half22float2(rv[jl][h]);
+              a0 += r.x;
+              a1 += r.y;
+            }
+            if (p.relu) {
+              a0 = fmaxf(a0, 0.f);
+              a1 = fmaxf(a1, 0.f);
+            }
+            if (p.post_add) {
+              a0 += pe[jh + jl][h].x;
+              a1 += pe[jh + jl][h].y;
+            }
+            *cell = pack_half2(a0, a1);
           }
-          if (pap[h]) {
-            const float2 pe = __ldg(reinterpret_cast<const float2*>(pap[h] + col));
-            a0 += pe.x;
-            a1 += pe.y;
-          }
-          *cell = pack_half2(a0, a1);
         }
       }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> async proxy
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (leader) {
-        for (int s = 0; s < NSLAB; ++s)
-          tma_store_5d(&map_out, staging + s * kSlabBytes, coff + c0 + s * 64, oc[1], oc[2], oc[3], oc[4]);
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+      if (p.post_add && b + 1 < NB) load_pe(b + 1);
+      if (kAlt || b == NB - 1) {
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> async proxy
+        // kAlt: the other slab's last store has been read out, so the next batch may convert into it
+        if (kAlt && leader) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (leader) {
+          for (int q = kAlt ? s : 0; q < (kAlt ? s + 1 : NSLAB); ++q)
+            tma_store_5d(&map_out, staging + q * kSlabBytes, coff + n_tile * BN + (kAlt ? 64 * b : 64 * q), oc[1],
+                         oc[2], oc[3], oc[4]);
+          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        }
       }
     }
   }
