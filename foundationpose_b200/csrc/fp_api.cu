@@ -20,6 +20,7 @@
 #include "fp_crop.cuh"
 #include "fp_depth.cuh"
 #include "fp_gemm.cuh"
+#include "fp_vis.cuh"
 
 namespace fp {
 const char* get_last_error();
@@ -203,6 +204,9 @@ struct fp_ctx {
   fp::DevBuf cam_args;
   fp::PinnedBuf stage_args;
   int cam_grid_h = 0, cam_grid_w = 0;
+  // fp_vis: the crop producer's vis record [N][2][160][160] float4 and the per-row depth ranges [N] float2, sized at the
+  // first call for the largest N seen; never allocated by the other entry points
+  fp::DevBuf vis_rec, vis_range;
 };
 
 namespace fp {
@@ -476,7 +480,7 @@ static int write_mesh_table(fp_ctx* c) {
 // device camera table and [N] camera ids (fp_track_cameras), or null = the context's frame
 static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg, float* win, int* stats,
                       cudaStream_t st, const int* mesh_of = nullptr, const CameraDev* cams = nullptr,
-                      const int* camera_of = nullptr) {
+                      const int* camera_of = nullptr, float4* vis = nullptr) {
   FP_REQUIRE(mesh_of || c->mesh[0].loaded, "no mesh: call fp_set_mesh first");
   FP_REQUIRE(c->has_frame, "no frame: call fp_set_frame first");
   // only launches below: this body is also what run_graphed captures (no allocation, no synchronisation)
@@ -505,6 +509,7 @@ static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg
   p.tile_override = c->crop_tile;
   p.cams = cams;
   p.camera_of = camera_of;
+  p.vis = vis;
   return crop_launch(p, st);
 }
 
@@ -1576,6 +1581,73 @@ int fp_track(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, 
   if (pose_out_dev) FP_CUDA_OK(cudaMemcpyAsync(pose_out_dev, c->track_pose.p, 64, cudaMemcpyDeviceToDevice, st));
   FP_CUDA_OK(cudaStreamSynchronize(st));
   if (pose_out_host) memcpy(pose_out_host, c->stage_pose.p, 64);
+  return 0;
+  FP_API_END
+}
+
+int fp_vis_size(int kind, int N, int* hw_out) {
+  FP_API_BEGIN
+  FP_REQUIRE(hw_out, "fp_vis_size: null output");
+  return vis_canvas_size(kind, N, hw_out, hw_out + 1);
+  FP_API_END
+}
+
+int fp_vis_colormap(unsigned char* rgb_out) {
+  FP_API_BEGIN
+  FP_REQUIRE(rgb_out, "fp_vis_colormap: null output");
+  const unsigned* t = vis_colormap();
+  for (int i = 0; i < 256; ++i)
+    for (int ch = 0; ch < 3; ++ch) rgb_out[3 * i + ch] = (unsigned char)(t[i] >> (16 - 8 * ch));
+  return 0;
+  FP_API_END
+}
+
+int fp_vis_crops(fp_ctx* c, const float* poses, int N, int mode, float* rec_out, void* stream) {
+  FP_API_BEGIN
+  FP_REQUIRE(c && poses && rec_out && N > 0 && (mode == 0 || mode == 1), "fp_vis_crops: bad argument");
+  DeviceGuard dg(c->device);
+  FP_TRY(ensure_capacity(c, N));
+  return make_crops(c, poses, N, mode, nullptr, nullptr, nullptr, reinterpret_cast<cudaStream_t>(stream), nullptr, nullptr,
+                    nullptr, reinterpret_cast<float4*>(rec_out));
+  FP_API_END
+}
+
+unsigned long long fp_vis_workspace_bytes(fp_ctx* c) { return c ? (unsigned long long)(c->vis_rec.bytes + c->vis_range.bytes) : 0ull; }
+
+int fp_vis(fp_ctx* c, int kind, const float* poses_a, const float* poses_b, int N, const int* order, unsigned char* canvas_out,
+           int* hw_out, void* stream) {
+  FP_API_BEGIN
+  FP_REQUIRE(c && poses_a && canvas_out && N > 0 && (kind == 0 || kind == 1), "fp_vis: bad argument");
+  FP_REQUIRE(kind == 1 || poses_b, "fp_vis: the refiner canvas needs the refined poses (poses_b)");
+  FP_REQUIRE(kind == 0 || order, "fp_vis: the scorer canvas needs the row order");
+  DeviceGuard dg(c->device);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  int hw[2];
+  FP_TRY(vis_canvas_size(kind, N, hw, hw + 1));
+  if (hw_out) {
+    hw_out[0] = hw[0];
+    hw_out[1] = hw[1];
+  }
+  FP_TRY(ensure_capacity(c, N));
+  // no captured graph holds the vis buffers (fp_vis runs eagerly): growing them must not invalidate the cached graphs
+  unsigned long long no_graph = 0;
+  FP_TRY(dev_alloc(no_graph, c->vis_rec, (size_t)N * 2 * S * S * sizeof(float4)));
+  FP_TRY(dev_alloc(no_graph, c->vis_range, (size_t)N * sizeof(float2)));
+  float4* rec = reinterpret_cast<float4*>(c->vis_rec.p);
+  float2* range = reinterpret_cast<float2*>(c->vis_range.p);
+  if (kind == 0) {
+    // predict_pose_refine.py:241-293: one crop pass at the start poses (left half), one at the refined poses (right)
+    for (int blk = 0; blk < 2; ++blk) {
+      FP_TRY(make_crops(c, blk ? poses_b : poses_a, N, 0, nullptr, nullptr, nullptr, st, nullptr, nullptr, nullptr, rec));
+      FP_TRY(vis_range_launch(rec, N, 2, range, st));
+      FP_TRY(vis_refine_launch(rec, range, N, blk, canvas_out, st));
+    }
+  } else {
+    // predict_score.py:219-224 + :27-52: the scorer's crops, depth range of the rendered image, rows in `order`
+    FP_TRY(make_crops(c, poses_a, N, 1, nullptr, nullptr, nullptr, st, nullptr, nullptr, nullptr, rec));
+    FP_TRY(vis_range_launch(rec, N, 1, range, st));
+    FP_TRY(vis_score_launch(rec, range, order, N, canvas_out, st));
+  }
   return 0;
   FP_API_END
 }

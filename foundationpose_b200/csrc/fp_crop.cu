@@ -354,7 +354,9 @@ __device__ __forceinline__ float pixel_ray(float idx_plus_half, float origin, fl
 // single-camera instantiations compile to the same code as before the camera table existed.
 // FRAME(f): field f of the frame this hypothesis is cropped from, read where it is used
 #define FRAME(f) (kCams ? sm.cam.f : p.f)
-template <int TILE, bool kStats, bool kCams>
+// kVis: also write the fp32 record of every crop pixel to p.vis (fp_vis, the debug canvases).  A template flag for the
+// same reason: the instantiations without it compile to the same code as before the record existed.
+template <int TILE, bool kStats, bool kCams, bool kVis>
 __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(const CropParams p) {
   constexpr int TPR = S / TILE;
   extern __shared__ __align__(16) unsigned char crop_smem_raw[];
@@ -609,6 +611,7 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
     const int unc = sm.coln[jl], uzc = sm.colz[jl];
     // ---- A: rendered crop
     float ar = 0.f, ag = 0.f, ab = 0.f, ax = 0.f, ay = 0.f, az = 0.f;
+    float za = 0.f;  // kVis: rendered camera z
     const unsigned long long key = sm.zt[rl * TILE + jl];
     if (key != 0ull) {
       const int f = (int)(0xFFFFFFFFu - (unsigned)(key & 0xFFFFFFFFull));
@@ -697,9 +700,11 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
       ag = fminf(fmaxf(cg * 0.8f + diffuse * cg * 0.5f, 0.f), 1.f);
       ab = fminf(fmaxf(cb * 0.8f + diffuse * cb * 0.5f, 0.f), 1.f);
       normalise_xyz(X, Y, Z, tvec, inv_radius, tau, ax, ay, az);
+      if (kVis) za = Z;
     }
     // ---- B: observed crop
     float br = 0.f, bg = 0.f, bb = 0.f, bx = 0.f, by = 0.f, bz = 0.f;
+    float zb = 0.f;  // kVis: nearest sample of the filtered depth
     {
       // bilinear rgb, zeros padding: tap indices / weights / validity come from the per-axis tables
       const float wy1 = sm.rowf[rl];
@@ -720,6 +725,7 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
       bb *= (1.f / 255.f);
       // nearest geometry
       const int vn = sm.rown[rl];
+      if (kVis && p.mode == 1 && unc >= 0 && vn >= 0) zb = __ldg(p.depth + (size_t)vn * p.W + unc);
       float X = 0.f, Y = 0.f, Z = 0.f;
       if (unc >= 0 && vn >= 0) {
         if (p.mode == 0) {
@@ -754,6 +760,11 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
       d = p.dbg + (((size_t)n * 2 + 1) * S * S + pix) * 6;
       d[0] = br; d[1] = bg; d[2] = bb; d[3] = bx; d[4] = by; d[5] = bz;
     }
+    if (kVis) {
+      float4* v = p.vis + (size_t)n * 2 * S * S + r * S + j;
+      v[0] = make_float4(ar, ag, ab, p.mode == 0 ? az : za);
+      v[S * S] = make_float4(br, bg, bb, p.mode == 0 ? bz : zb);
+    }
   }
 }
 
@@ -777,18 +788,21 @@ static int launch_tile(const CropParams& p, cudaStream_t stream) {
   const size_t smem = sizeof(TileSmem<TILE>);
   static std::atomic<unsigned long long> attr_mask{0};  // per device
   if (!device_bit_test(attr_mask)) {
-    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     device_bit_set(attr_mask);
   }
   const dim3 grid(TPR * TPR, p.N);
   if (p.cams) {
-    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, false, true>, grid, dim3(kThreads), smem, stream, 1, p));
+    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, false, true, false>, grid, dim3(kThreads), smem, stream, 1, p));
   } else if (p.stats) {
-    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, true, false>, grid, dim3(kThreads), smem, stream, 1, p));
+    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, true, false, false>, grid, dim3(kThreads), smem, stream, 1, p));
+  } else if (p.vis) {
+    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, false, false, true>, grid, dim3(kThreads), smem, stream, 1, p));
   } else {
-    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, false, false>, grid, dim3(kThreads), smem, stream, 1, p));
+    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, false, false, false>, grid, dim3(kThreads), smem, stream, 1, p));
   }
   return 0;
 }
@@ -797,6 +811,7 @@ int crop_launch(const CropParams& p, cudaStream_t stream) {
   if (p.N == 0) return 0;
   FP_REQUIRE(!p.cams == !p.camera_of, "crop_launch: the camera table and the camera ids go together");
   FP_REQUIRE(!(p.cams && p.stats), "crop_launch: work counters are collected on the single-camera path only");
+  FP_REQUIRE(!(p.vis && (p.cams || p.stats)), "crop_launch: the vis record is written on the single-camera path only");
   // algorithmic bytes: the two 6-channel fp16 crops each hypothesis produces (SURVEY.md §8d)
   prof_mark_begin(1, (double)p.N * 2.0 * 6.0 * S * S * 2.0, stream);
   int tile = p.N >= 64 ? 80 : (p.N >= 4 ? 32 : 16);

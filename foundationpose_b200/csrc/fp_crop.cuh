@@ -92,6 +92,10 @@ struct CropParams {
   // cams[camera_of[n]] instead of the by-value frame fields above (fp_track_cameras); both null or both set
   const CameraDev* cams;
   const int* camera_of;
+  // optional, single-camera (fp_vis): [N][2][160][160] fp32 record of every crop pixel, A then B: the r, g, b the
+  // crops hold (0..1) and one depth value — mode 0 the normalised z of the xyz channels, mode 1 the raw depth in metres
+  // (A: rendered camera z, 0 where nothing is covered; B: the nearest sample of the filtered depth, predict_score.py:90)
+  float4* vis;
 };
 
 int crop_launch(const CropParams& p, cudaStream_t stream);

@@ -9,6 +9,8 @@ Only the surface the drivers touch is provided (the reference's Utils.py is 1000
                  glcam_in_cvcam (:66), compute_mesh_diameter (:559-574, exact instead of sampled), sample_views_icosphere
                  (:483-507), make_mesh_tensors (:104-130), erode_depth / bilateral_filter_depth (:304-395, on the GPU)
   drawing        project_3d_to_2d (:667-672), draw_xyz_axis (:675-710), draw_posed_3d_box (:713-750)
+  debug canvases make_grid_image (:293-300), depth_to_vis (:456-479), cv_draw_text (:630-655) — the helpers of the
+                 predictors' get_vis canvases (foundationpose_b200/vis.py)
   clouds         toOpen3dCloud (:280-289) — needs open3d, which only debug >= 2 / 3 paths call
   dataset runs   argparse, NestDict (:60-61), make_yaml_dumpable (:996-1020), symmetry_tfs_from_info (:806-834),
                  euler_matrix (the `transformations` package's static-xyz convention), wp (warp stand-in: force_load)
@@ -66,6 +68,7 @@ from foundationpose_b200 import hypotheses as _hyp  # noqa: E402
 from foundationpose_b200 import meshprep as _meshprep  # noqa: E402
 from foundationpose_b200 import metrics as _metrics  # noqa: E402
 from foundationpose_b200.estimater import make_mesh_tensors  # noqa: E402,F401
+from foundationpose_b200.vis import cv_draw_text, depth_to_vis, make_grid_image  # noqa: E402,F401
 
 
 

@@ -56,11 +56,17 @@ def _proto():
     lib.fp_op_tokens.argtypes = [vp, i, vp, i, vp, vp]
     lib.fp_op_depth_filter.argtypes = [vp, vp, i, i, i, vp]
     lib.fp_op_pose_update.argtypes = [vp, vp, vp, vp, i, f, f, vp]
+    lib.fp_vis.argtypes = [vp, i, vp, vp, i, vp, vp, C.POINTER(i), vp]
+    lib.fp_vis_size.argtypes = [i, i, C.POINTER(i)]
+    lib.fp_vis_colormap.argtypes = [vp]
+    lib.fp_vis_crops.argtypes = [vp, vp, i, i, vp, vp]
+    lib.fp_vis_workspace_bytes.argtypes = [vp]
+    lib.fp_vis_workspace_bytes.restype = C.c_ulonglong
     for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_track_cameras", "fp_register_objects", "fp_register_cameras", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh",
                  "fp_set_mesh_slot", "fp_set_frame",
                  "fp_get_depth", "fp_make_crops", "fp_start_poses", "fp_refine", "fp_score", "fp_score_features", "fp_score_tail",
                  "fp_register", "fp_op_refine_net", "fp_op_score_feats", "fp_op_tokens", "fp_op_depth_filter",
-                 "fp_op_pose_update"):
+                 "fp_op_pose_update", "fp_vis", "fp_vis_size", "fp_vis_colormap", "fp_vis_crops"):
         getattr(lib, name).restype = C.c_int
 
 
@@ -504,6 +510,40 @@ class Engine:
                                    _stream()), "fp_register")
         return out_poses, out_scores, int(best.item())
 
+    # ---- debug canvases
+    def vis(self, kind, poses_a, poses_b=None, order=None):
+        """fp_vis: the get_vis canvas of the context's current frame and mesh, without its text labels, as a CUDA uint8
+        (H, W, 3) tensor.  kind 'refine': the crops at poses_a (the poses predict() received) beside those at poses_b
+        (the refined poses); kind 'score': the scorer's rows of poses_a, row s showing hypothesis order[s]."""
+        k = 0 if kind == "refine" else 1
+        poses_a = self._poses(poses_a)
+        N = len(poses_a)
+        if k == 0:
+            poses_b = self._poses(poses_b)
+            if len(poses_b) != N:
+                raise ValueError(f"vis: {N} start poses but {len(poses_b)} refined poses")
+        else:
+            order = torch.as_tensor(order, device="cuda").to(torch.int32).contiguous()
+            if order.numel() != N:
+                raise ValueError(f"vis: {N} poses but {order.numel()} row indices")
+        H, W = vis_size(kind, N)
+        canvas = torch.empty(H, W, 3, dtype=torch.uint8, device="cuda")
+        _lib.check(lib.fp_vis(self._h, k, _p(poses_a), _p(poses_b) if k == 0 else None, N, _p(order) if k == 1 else None,
+                              _p(canvas), None, _stream()), "fp_vis")
+        return canvas
+
+    def vis_crops(self, poses, mode=0):
+        """The crop pass of vis alone (test hook): (N, 2, 160, 160, 4) CUDA float32 = (r, g, b, depth) of the rendered
+        and the observed crop; depth is the normalised z (mode 0, refiner) or raw metres (mode 1, scorer)."""
+        poses = self._poses(poses)
+        rec = torch.empty(len(poses), 2, 160, 160, 4, dtype=torch.float32, device="cuda")
+        _lib.check(lib.fp_vis_crops(self._h, _p(poses), len(poses), int(mode), _p(rec), _stream()), "fp_vis_crops")
+        return rec
+
+    def vis_workspace_bytes(self):
+        """Device memory the debug canvases hold in this context (0 until the first vis call)."""
+        return int(lib.fp_vis_workspace_bytes(self._h))
+
     # ---- single-operator hooks (tests)
     def op_refine_net(self, crops, N):
         trans = torch.empty(N, 3, dtype=torch.float32, device="cuda")
@@ -520,6 +560,20 @@ class Engine:
         tok = torch.empty(N, 400, 512, dtype=torch.float16, device="cuda")
         _lib.check(lib.fp_op_tokens(self._h, 0 if kind == "refine" else 1, _p(crops), N, _p(tok), _stream()), "fp_op_tokens")
         return tok
+
+
+def vis_size(kind, N):
+    """(H, W) of Engine.vis's canvas for N hypotheses (no GPU needed)."""
+    hw = (C.c_int * 2)()
+    _lib.check(lib.fp_vis_size(0 if kind == "refine" else 1, int(N), hw), "fp_vis_size")
+    return hw[0], hw[1]
+
+
+def vis_colormap():
+    """The canvases' colour map: (256, 3) uint8 RGB (no GPU needed)."""
+    out = np.empty((256, 3), dtype=np.uint8)
+    _lib.check(lib.fp_vis_colormap(C.c_void_p(out.ctypes.data)), "fp_vis_colormap")
+    return out
 
 
 def crops_from_planar(A, B):

@@ -7,7 +7,10 @@ Same names, argument orders and error behaviour as
 so a driver written against the reference (run_demo.py:38-63) only changes its import.
 
 Differences that are deliberate (DESIGN.md §1): no nvdiffrast context is needed (`glctx` is accepted
-and ignored) and visualisation (`get_vis`, debug >= 2 dumps) is not produced.  `predict()` honours the
+and ignored).  Visualisation is what the reference's drivers reach: `predict(get_vis=True)` returns the reference's
+canvases (composed on the device by fp_vis, labelled on the host, foundationpose_b200/vis.py), register() at debug >= 2
+writes color.png, depth.png, ob_mask.png, vis_refiner.png, vis_score.png (and the .ply clouds when open3d imports)
+to debug_dir, and track_one() at debug >= 2 puts the refiner canvas in extra['vis'].  `predict()` honours the
 per-call `mesh` / `mesh_tensors` / `mesh_diameter` / `xyz_map` arguments of the reference: a mesh that is not
 the one already in the context is uploaded first, a caller-supplied xyz map replaces the derived one.
 """
@@ -134,7 +137,8 @@ class PoseRefinePredictor:
     @torch.inference_mode()
     def predict(self, rgb, depth, K, ob_in_cams, xyz_map=None, normal_map=None, get_vis=False, mesh=None, mesh_tensors=None,
                 glctx=None, mesh_diameter=None, iteration=5, _frame_ready=False):
-        """@rgb: (H,W,3) uint8; @ob_in_cams: (N,4,4).  Returns ((N,4,4) cuda tensor, None)."""
+        """@rgb: (H,W,3) uint8; @ob_in_cams: (N,4,4).  Returns ((N,4,4) cuda tensor, canvas): canvas is None, or with
+        get_vis the reference's (N*166+6, 1314, 3) uint8 image of every hypothesis's crops before and after refinement."""
         e = self.engine
         _sync_mesh(e, mesh, mesh_tensors, mesh_diameter)
         if not _frame_ready:
@@ -144,7 +148,11 @@ class PoseRefinePredictor:
         poses, lt, lr = e.refine(ob_in_cams, iteration)
         self.last_trans_update = lt
         self.last_rot_update = lr
-        return poses, None
+        if not get_vis:
+            return poses, None
+        from . import vis  # cv2: only the debug canvases need it
+
+        return poses, vis.refine_canvas(e, ob_in_cams, poses)
 
 
 class ScorePredictor:
@@ -161,13 +169,18 @@ class ScorePredictor:
     @torch.inference_mode()
     def predict(self, rgb, depth, K, ob_in_cams, normal_map=None, get_vis=False, mesh=None, mesh_tensors=None, glctx=None,
                 mesh_diameter=None, _frame_ready=False):
-        """Returns ((N,) cuda tensor of scores = logits + 100, None)."""
+        """Returns ((N,) cuda tensor of scores = logits + 100, canvas): canvas is None, or with get_vis the reference's
+        (N*105, 409, 3) uint8 image of every hypothesis's crops, ranked by descending score."""
         e = self.engine
         _sync_mesh(e, mesh, mesh_tensors, mesh_diameter)
         if not _frame_ready:
             e.set_frame(rgb, depth, K, filter_depth=False)
         scores, _ = e.score(ob_in_cams)
-        return scores, None
+        if not get_vis:
+            return scores, None
+        from . import vis  # cv2: only the debug canvases need it
+
+        return scores, vis.score_canvas(e, ob_in_cams, scores)
 
 
 def make_mesh_tensors(mesh):
@@ -281,6 +294,17 @@ class FoundationPose:
         # translation guess and the start poses, also on the device: nothing synchronises until the result is read
         e.set_frame(rgb, depth, K, filter_depth=True, zfar=float("inf"))
         poses, info = e.start_poses(ob_mask, self.rot_grid)
+        dump = self.debug >= 2
+        if dump:
+            import cv2  # only the debug dumps need it
+
+            # estimater.py:176-180: the filtered frame's cloud and the mask, before the early exit.  The frame may be
+            # device-resident: the dumps take host copies
+            depth_f, xyz = (t.cpu().numpy() for t in e.get_depth())
+            rgb_h = rgb.cpu().numpy() if torch.is_tensor(rgb) else np.asarray(rgb)
+            self._write_cloud("scene_raw.ply", xyz, rgb_h)
+            m = ob_mask.cpu().numpy() if torch.is_tensor(ob_mask) else np.asarray(ob_mask)
+            cv2.imwrite(f"{self.debug_dir}/ob_mask.png", (m * 255.0).clip(0, 255))
         if self.strict_early_out:
             # estimater.py:181-189 returns BEFORE the hypothesis loop when fewer than 4 valid masked pixels remain;
             # knowing that on the host costs one 16-byte read-back (a synchronisation the sync-free path avoids)
@@ -290,16 +314,25 @@ class FoundationPose:
                 pose = np.eye(4)
                 pose[:3, 3] = head[:3]
                 return pose
+        if dump:
+            # estimater.py:191-195
+            cv2.imwrite(f"{self.debug_dir}/color.png", np.ascontiguousarray(rgb_h[..., ::-1]))
+            cv2.imwrite(f"{self.debug_dir}/depth.png", (depth_f * 1000).astype(np.uint16))
+            self._write_cloud("scene_complete.ply", xyz, rgb_h)
         self.H, self.W = depth.shape[:2]
         self.K = K
         self.ob_id = ob_id
         self.ob_mask = ob_mask
-        poses, _ = self.refiner.predict(mesh=self.mesh, mesh_tensors=self.mesh_tensors, rgb=rgb, depth=depth, K=K,
-                                        ob_in_cams=poses, normal_map=None, xyz_map=None, glctx=self.glctx,
-                                        mesh_diameter=self.diameter, iteration=iteration, _frame_ready=True)
-        scores, _ = self.scorer.predict(mesh=self.mesh, rgb=rgb, depth=depth, K=K, ob_in_cams=poses, normal_map=None,
-                                        mesh_tensors=self.mesh_tensors, glctx=self.glctx, mesh_diameter=self.diameter,
-                                        _frame_ready=True)
+        poses, canvas = self.refiner.predict(mesh=self.mesh, mesh_tensors=self.mesh_tensors, rgb=rgb, depth=depth, K=K,
+                                             ob_in_cams=poses, normal_map=None, xyz_map=None, glctx=self.glctx,
+                                             mesh_diameter=self.diameter, iteration=iteration, get_vis=dump, _frame_ready=True)
+        if canvas is not None:
+            cv2.imwrite(f"{self.debug_dir}/vis_refiner.png", canvas[..., ::-1])
+        scores, canvas = self.scorer.predict(mesh=self.mesh, rgb=rgb, depth=depth, K=K, ob_in_cams=poses, normal_map=None,
+                                             mesh_tensors=self.mesh_tensors, glctx=self.glctx, mesh_diameter=self.diameter,
+                                             get_vis=dump, _frame_ready=True)
+        if canvas is not None:
+            cv2.imwrite(f"{self.debug_dir}/vis_score.png", canvas[..., ::-1])
         ids = torch.as_tensor(scores).argsort(descending=True)
         scores = scores[ids]
         poses = poses[ids]
@@ -320,6 +353,20 @@ class FoundationPose:
             return pose
         return out[4:].reshape(4, 4).copy()
 
+    def _write_cloud(self, name, xyz, rgb):
+        """The debug point clouds (estimater.py:178-179, :194-195): valid pixels of the xyz map (host), coloured by the
+        host rgb; only with open3d."""
+        try:
+            import open3d as o3d
+        except ImportError:
+            logging.info(f"open3d is not installed: {name} not written")
+            return
+        valid = xyz[..., 2] >= 0.001
+        pcd = o3d.geometry.PointCloud()
+        pcd.points = o3d.utility.Vector3dVector(xyz[valid].astype(np.float64))
+        pcd.colors = o3d.utility.Vector3dVector(rgb[valid].astype(np.float64) / 255.0)
+        o3d.io.write_point_cloud(f"{self.debug_dir}/{name}", pcd)
+
     def track_one(self, rgb, depth, K, iteration, extra={}):
         if self.pose_last is None:
             logging.info("Please init pose by register first")
@@ -329,13 +376,23 @@ class FoundationPose:
         if torch.is_tensor(rgb) or torch.is_tensor(depth):
             # device-resident frame: enqueue the stages one by one (estimater.py:255-264)
             e.set_frame(rgb, depth, K, filter_depth=True, zfar=float("inf"))
-            pose, _ = self.refiner.predict(mesh=self.mesh, mesh_tensors=self.mesh_tensors, rgb=rgb, depth=depth, K=K,
-                                           ob_in_cams=self.pose_last.reshape(1, 4, 4), normal_map=None, xyz_map=None,
-                                           mesh_diameter=self.diameter, glctx=self.glctx, iteration=iteration, _frame_ready=True)
+            pose, canvas = self.refiner.predict(mesh=self.mesh, mesh_tensors=self.mesh_tensors, rgb=rgb, depth=depth, K=K,
+                                                ob_in_cams=self.pose_last.reshape(1, 4, 4), normal_map=None, xyz_map=None,
+                                                mesh_diameter=self.diameter, glctx=self.glctx, iteration=iteration,
+                                                get_vis=self.debug >= 2, _frame_ready=True)
+            if self.debug >= 2:
+                extra["vis"] = canvas
             self.pose_last = pose
             return (pose @ self.get_tf_to_centered_mesh()).data.cpu().numpy().reshape(4, 4)
         # host frame (what the drivers pass): the whole frame is one CUDA-graph launch (fp_track)
-        pose_dev, pose_host = e.track(rgb, depth, K, self.pose_last.reshape(4, 4), iteration)
+        pose_in = self.pose_last.reshape(4, 4)
+        pose_dev, pose_host = e.track(rgb, depth, K, pose_in, iteration)
+        if self.debug >= 2:
+            # fp_track leaves this frame in the context — its filtered depth and its xyz map with zfar = inf, what the
+            # refiner cropped from — so the canvas pass (estimater.py:263-266) crops the same frame, after the pose is out
+            from . import vis  # cv2: only the debug canvases need it
+
+            extra["vis"] = vis.refine_canvas(e, pose_in, pose_dev)
         self.pose_last = pose_dev.reshape(1, 4, 4)
         self.refiner.last_trans_update = self.refiner.last_rot_update = None
         return _uncentre(pose_host, self.model_center)

@@ -278,6 +278,31 @@ int fp_register_cameras(fp_ctx* ctx, int C, const unsigned char* const* rgb_host
 /* Number of CUDA graphs this context has captured so far (test hook: a replay captures nothing). */
 unsigned long long fp_graph_captures(fp_ctx* ctx);
 
+/* The debug canvases of get_vis, composed on the device from the context's CURRENT frame and mesh slot 0, without the
+ * text labels (the caller draws them: cv_draw_text).  canvas_out: DEVICE uint8 [H][W][3] of the size fp_vis_size
+ * gives; hw_out (HOST [2], optional) receives (H, W).  Asynchronous on `stream`.
+ *   kind 0 replaces predict_pose_refine.py:241-293: N rows of [rgbA | rgbB | depthA | depthB] (make_grid_image,
+ *          padding 2, depth_to_vis of the normalised z over the row's range), crops at poses_a (DEVICE [N][16], the
+ *          poses predict() received) on the left, at poses_b (the refined poses) on the right.
+ *   kind 1 replaces predict_score.py:27-52, :219-224: row s = hypothesis order[s] (DEVICE int [N], e.g. the scores'
+ *          descending argsort) of poses_a: [rgbA | depthA | rgbB | depthB] with 5-pixel gaps, raw depths over the
+ *          rendered depth's range, resized to 100 x 409 by cv2's INTER_LINEAR rule, then 5 rows of 255.
+ * The first call allocates the crop record (819 200 B per hypothesis, 206 MB at N = 252) as the context's high-water
+ * mark; no other entry point does, and no cached graph is invalidated by it. */
+int fp_vis(fp_ctx* ctx, int kind, const float* poses_a, const float* poses_b, int N, const int* order,
+           unsigned char* canvas_out, int* hw_out, void* stream);
+/* Canvas size of fp_vis (no GPU needed): hw_out[2] = (H, W).  Refiner: (166 N + 6, 1314), (168, 1306) for N = 1 (a
+ * one-row grid is not padded); scorer: (105 N, 409). */
+int fp_vis_size(int kind, int N, int* hw_out);
+/* The canvases' 256-entry colour map (cv2.COLORMAP_JET as RGB) into rgb_out [256][3] (no GPU needed). */
+int fp_vis_colormap(unsigned char* rgb_out);
+/* The crop pass of fp_vis alone (test hook): rec_out DEVICE [N][2][160][160][4] fp32 = (r, g, b, depth) of the rendered
+ * and the observed crop at poses (DEVICE [N][16]); depth is the normalised z for mode 0 (refiner), raw metres for mode 1
+ * (scorer: rendered camera z, 0 where nothing is covered; nearest sample of the filtered depth). */
+int fp_vis_crops(fp_ctx* ctx, const float* poses, int N, int mode, float* rec_out, void* stream);
+/* Bytes of device memory fp_vis holds in this context (0 until the first fp_vis call). */
+unsigned long long fp_vis_workspace_bytes(fp_ctx* ctx);
+
 /* ------------------------------------------------------------------------------------------ */
 /* one process, several GPUs (the reference's process model: run_demo.py is a single script)  */
 /* ------------------------------------------------------------------------------------------ */
