@@ -129,8 +129,8 @@ struct MeshSlot {
   float diameter = 0.f;
 };
 
-// Frame buffers of cameras 1.. of fp_track_cameras (camera 0 is the context's frame), sized for the largest frame seen,
-// and the pinned staging of their uploads.
+// One camera's frame: the raw upload, the filtered frame (rgba, depth, xyz) and the pinned staging of the upload.
+// Camera 0 is the context's frame, the one every single-frame entry point reads (see alloc_camera).
 struct CameraBufs {
   DevBuf rgb_raw, depth_raw, rgba, depth, xyz;
   PinnedBuf stage_rgb, stage_depth;
@@ -146,11 +146,13 @@ struct fp_ctx {
   // meshes, and their device table (MeshSlotDev [FP_MAX_MESHES]) that kernels index by slot.  Captured graphs hold only
   // the table's address: loading a slot rewrites its entry in place and needs no new capture.
   fp::MeshSlot mesh[fp::kMaxMeshes];
-  fp::DevBuf mesh_table, mesh_of;  // mesh_of: slot id of every hypothesis of an fp_register_objects pass
+  fp::DevBuf mesh_table;
   float rot_normalizer = 0.3490658503988659f;
   float crop_ratio[2] = {1.2f, 1.2f};  // per predictor: each reads its own config.yml (predict_pose_refine.py:117, predict_score.py:137)
-  // frame
-  fp::DevBuf rgb_raw, rgba, depth_raw, depth_a, depth_b, xyz;
+  // frames: cam[0] is the context's frame, cameras 1.. those of the multi-camera calls; K / H / W are camera 0's.
+  // depth_a: the eroded depth between the separate filter launches of FPOSE_FUSED_PREP=0
+  fp::CameraBufs cam[fp::kMaxCameras];
+  fp::DevBuf depth_a;
   const float* depth_cur = nullptr;
   float K[9] = {0};
   int H = 0, W = 0;
@@ -162,8 +164,8 @@ struct fp_ctx {
   int tail_cap = 0;
   float fold_c = 0.f;      // linear.weight . out_proj.bias + linear.bias (by-value kernel parameter)
   fp::DevBuf fold_v, tail_counter;  // out_proj^T linear.weight [512]; arg-max ticket
-  // CUDA graphs of the launch-bound inner loops, keyed by (kind, N, iterations, cameras).  K / H / W: the frame
-  // geometry a graph that passes it by value was captured with
+  // CUDA graphs of the launch-bound inner loops, keyed by (kind, N, iterations, frame source: see run_graphed).
+  // K / H / W: the frame geometry a graph that passes it by value was captured with
   struct GraphEntry {
     cudaGraphExec_t exec = nullptr;
     unsigned long long epoch = 0;
@@ -185,25 +187,20 @@ struct fp_ctx {
   int crop_tile = 0;
   fp::DevBuf lt_buf, lr_buf, feat_buf, pose_stage, tok_mean;
   fp::DevBuf mask_buf, mask_stats, crop_stats;
-  // fp_track: pinned host staging (frame in, pose out) so that the whole frame is ONE graph launch
-  fp::PinnedBuf stage_rgb, stage_depth, stage_pose;
+  // fp_track: the pose in and out of the graph, and its pinned read-back
+  fp::PinnedBuf stage_pose;
   fp::DevBuf track_pose;
   fp::PinnedBuf stage_poses;  // fp_track_objects: pinned [M][16] pose read-back
-  // fp_register_objects: row offsets of the objects' hypotheses [M + 1], their feature rows [sum N][512]; pinned staging
-  // of the masks and of (offsets, per-hypothesis slot ids)
-  fp::DevBuf seg_off, reg_feats;
-  fp::PinnedBuf stage_masks, stage_ints;
-  // fp_register_cameras: the camera table [FP_MAX_CAMERAS] (fixed size, so its address never changes), the camera id of
-  // every hypothesis of a pass, each object's byte offset into mask_buf, and the pinned staging of the table and offsets
-  fp::DevBuf reg_cams, reg_cam_of, mask_off;
-  fp::PinnedBuf stage_cams;
-  // fp_track_cameras: buffers of cameras 1..; the per-call arguments (camera table [FP_MAX_CAMERAS], slot ids [M],
-  // camera ids [M]) as one device block and its pinned staging; the frame size its frame-preparation grid covers (the
-  // largest seen)
-  fp::CameraBufs cams[fp::kMaxCameras];
-  fp::DevBuf cam_args;
+  // the arguments of a multi-object call or register pass, one device block at a fixed address (a graph holds it) and
+  // its pinned staging: the camera table (CameraDev [FP_MAX_CAMERAS]), the slot ids [n], the camera ids [n]
+  fp::DevBuf args;
   fp::PinnedBuf stage_args;
-  int cam_grid_h = 0, cam_grid_w = 0;
+  int cam_grid_h = 0, cam_grid_w = 0;  // fp_track_cameras' frame-preparation grid: the largest frame seen
+  // fp_register_objects / _cameras: row offsets of the objects' hypotheses [M + 1] and the objects' camera ids [M], the
+  // objects' feature rows [sum N][512], each object's byte offset into mask_buf; pinned staging of the masks and of
+  // (offsets, camera ids, mask offsets)
+  fp::DevBuf seg_off, reg_feats, mask_off;
+  fp::PinnedBuf stage_masks, stage_ints;
   // fp_vis: the crop producer's vis record [N][2][160][160] float4 and the per-row depth ranges [N] float2, sized at the
   // first call for the largest N seen; never allocated by the other entry points
   fp::DevBuf vis_rec, vis_range;
@@ -477,7 +474,7 @@ static int write_mesh_table(fp_ctx* c) {
 }
 
 // mesh_of: [N] device slot ids (validated by the caller), or null = every hypothesis renders slot 0.  cams / camera_of:
-// device camera table and [N] camera ids (fp_track_cameras), or null = the context's frame
+// device camera table and [N] camera ids (the multi-camera calls), or null = the context's frame, by value
 static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg, float* win, int* stats,
                       cudaStream_t st, const int* mesh_of = nullptr, const CameraDev* cams = nullptr,
                       const int* camera_of = nullptr, float4* vis = nullptr) {
@@ -497,8 +494,8 @@ static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg
   p.zfar = 100.f;
   p.slots = reinterpret_cast<const MeshSlotDev*>(c->mesh_table.p);
   p.mesh_of = mesh_of;
-  p.rgb = reinterpret_cast<const uchar4*>(c->rgba.p);
-  p.xyz_map = reinterpret_cast<const float4*>(c->xyz.p);
+  p.rgb = reinterpret_cast<const uchar4*>(c->cam[0].rgba.p);
+  p.xyz_map = reinterpret_cast<const float4*>(c->cam[0].xyz.p);
   p.depth = c->depth_cur;
   p.mode = mode;
   p.crops = reinterpret_cast<__half*>(c->crops.p);
@@ -518,12 +515,9 @@ enum class GraphKind {
   Refine = 0,            // fp_refine
   ScoreFeatures = 1,     // fp_score_features
   Track = 2,             // fp_track
-  TrackObjects = 3,      // fp_track_objects
-  RegisterRefine = 4,    // fp_register_objects: one pass's refinement
-  RegisterFeatures = 5,  // fp_register_objects: one pass's scorer features
-  TrackCameras = 6,      // fp_track_cameras
-  RegisterCamerasRefine = 7,    // fp_register_cameras: one pass's refinement, frames from the camera table
-  RegisterCamerasFeatures = 8,  // fp_register_cameras: one pass's scorer features, frames from the camera table
+  TrackObjects = 3,      // fp_track_objects, fp_track_cameras
+  RegisterRefine = 4,    // fp_register_objects / _cameras: one pass's refinement
+  RegisterFeatures = 5,  // fp_register_objects / _cameras: one pass's scorer features
 };
 
 // Runs `body(stream)` — a fixed sequence of kernel launches (and fixed-address copies) on ctx-owned buffers —
@@ -531,22 +525,22 @@ enum class GraphKind {
 // captures + instantiates, later calls replay.  Replay removes ~170 launch + 60 tensor-map-encode host
 // calls per register(), which is what bounds track_one() and small per-GPU shards.  The body never allocates:
 // callers size every workspace first, so a capture after an epoch bump (new mesh, new N) is safe.
-// frame_by_value: the body passes the context's K / H / W to its kernels by value (every body except fp_track_cameras',
-// which reads them from the camera table); such a graph is captured again when they differ from its capture's.  Only
-// that graph: a frame of another size or other intrinsics does not invalidate the others.
+// frame: where the body's kernels take their frame from, the last element of the key.  -1: the context's K / H / W by
+// value; such a graph is captured again when they differ from its capture's, and only that graph: a frame of another
+// size or other intrinsics does not invalidate the others.  0 or more: the camera table (the camera-table kernel
+// instantiations), which holds every camera's size and intrinsics; fp_track_cameras passes its number of cameras C,
+// which its frame-preparation launch covers, the register passes 0 (their frames are prepared before the passes).
 template <class Body>
-static int run_graphed(fp_ctx* c, GraphKind kind, int N, int iters, cudaStream_t st, Body body, int cameras = 0,
-                       bool frame_by_value = true) {
+static int run_graphed(fp_ctx* c, GraphKind kind, int N, int iters, cudaStream_t st, Body body, int frame = -1) {
   if (!c->use_graphs || g_prof_on) return body(st);
-  const auto key = std::make_tuple(static_cast<int>(kind), N, iters, cameras);
+  const auto key = std::make_tuple(static_cast<int>(kind), N, iters, frame);
   auto it = c->graphs.find(key);
   if (it == c->graphs.end()) {
     c->graphs[key] = fp_ctx::GraphEntry();  // seen once: next call captures
     return body(st);
   }
   fp_ctx::GraphEntry& g = it->second;
-  const bool frame_moved =
-      frame_by_value && (g.H != c->H || g.W != c->W || memcmp(g.K, c->K, sizeof g.K) != 0);
+  const bool frame_moved = frame < 0 && (g.H != c->H || g.W != c->W || memcmp(g.K, c->K, sizeof g.K) != 0);
   if (g.exec == nullptr || g.epoch != c->epoch || frame_moved) {
     if (g.exec) {
       cudaGraphExecDestroy(g.exec);
@@ -621,52 +615,56 @@ static int set_frame_launches(fp_ctx* c, const unsigned char* rgb_dev, const flo
                               cudaStream_t st) {
   const int H = c->H, W = c->W;
   const size_t npix = (size_t)H * W;
+  CameraBufs& f = c->cam[0];
+  uchar4* rgba = reinterpret_cast<uchar4*>(f.rgba.p);
+  float* depth = reinterpret_cast<float*>(f.depth.p);
+  float4* xyz = reinterpret_cast<float4*>(f.xyz.p);
+  c->depth_cur = depth;
   if ((flags & FP_FRAME_FILTER_DEPTH) && !fused_prep()) {
-    FP_TRY(rgb_to_rgba_launch(rgb_dev, reinterpret_cast<uchar4*>(c->rgba.p), (int)npix, st));
+    FP_TRY(rgb_to_rgba_launch(rgb_dev, rgba, (int)npix, st));
     FP_TRY(erode_depth_launch(depth_dev, reinterpret_cast<float*>(c->depth_a.p), H, W, 2, 0.001f, 0.8f, 100.f, st));
-    FP_TRY(bilateral_depth_launch(reinterpret_cast<const float*>(c->depth_a.p), reinterpret_cast<float*>(c->depth_b.p), H,
-                                  W, 2, 100.f, 2.f, 100000.f, st));
-    c->depth_cur = reinterpret_cast<const float*>(c->depth_b.p);
-    return depth_to_xyz_launch(c->depth_cur, reinterpret_cast<float4*>(c->xyz.p), H, W, c->K[0], c->K[4], c->K[2], c->K[5], zfar, st);
+    FP_TRY(bilateral_depth_launch(reinterpret_cast<const float*>(c->depth_a.p), depth, H, W, 2, 100.f, 2.f, 100000.f, st));
+    return depth_to_xyz_launch(depth, xyz, H, W, c->K[0], c->K[4], c->K[2], c->K[5], zfar, st);
   }
   if (flags & FP_FRAME_FILTER_DEPTH) {
     // estimater.py:173-174 erode_depth(radius=2), bilateral_filter_depth(radius=2); :214 depth2xyzmap: one launch
-    c->depth_cur = reinterpret_cast<const float*>(c->depth_b.p);
-    return frame_prep_launch(rgb_dev, depth_dev, reinterpret_cast<uchar4*>(c->rgba.p), reinterpret_cast<float*>(c->depth_b.p),
-                             reinterpret_cast<float4*>(c->xyz.p), H, W, c->K[0], c->K[4], c->K[2], c->K[5], zfar, st);
+    return frame_prep_launch(rgb_dev, depth_dev, rgba, depth, xyz, H, W, c->K[0], c->K[4], c->K[2], c->K[5], zfar, st);
   }
-  FP_TRY(rgb_to_rgba_launch(rgb_dev, reinterpret_cast<uchar4*>(c->rgba.p), (int)npix, st));
-  FP_CUDA_OK(cudaMemcpyAsync(c->depth_b.p, depth_dev, npix * 4, cudaMemcpyDeviceToDevice, st));
-  c->depth_cur = reinterpret_cast<const float*>(c->depth_b.p);
-  FP_TRY(depth_to_xyz_launch(c->depth_cur, reinterpret_cast<float4*>(c->xyz.p), H, W, c->K[0], c->K[4], c->K[2], c->K[5],
-                             zfar, st));
+  FP_TRY(rgb_to_rgba_launch(rgb_dev, rgba, (int)npix, st));
+  FP_CUDA_OK(cudaMemcpyAsync(depth, depth_dev, npix * 4, cudaMemcpyDeviceToDevice, st));
+  return depth_to_xyz_launch(depth, xyz, H, W, c->K[0], c->K[4], c->K[2], c->K[5], zfar, st);
+}
+
+// Sizes camera i's buffers for npix pixels: the filtered frame always, the raw upload if `raw`, its pinned staging if
+// `staged`.  Camera 0's addresses are held by the graphs that take the frame by value, so growing its buffers (or
+// depth_a, which goes with them) bumps the graph epoch.  Cameras 1.. are reached only through the camera table, which
+// every call rewrites: growing them invalidates no graph.  No graph holds the staging: the uploads leave it ahead of
+// the launch.
+static int alloc_camera(fp_ctx* c, int i, size_t npix, bool raw, bool staged) {
+  CameraBufs& b = c->cam[i];
+  unsigned long long table_only = 0;
+  unsigned long long& epoch = i == 0 ? c->epoch : table_only;
+  FP_TRY(dev_alloc(epoch, b.rgba, npix * 4));
+  if (i == 0) FP_TRY(dev_alloc(epoch, c->depth_a, npix * 4));
+  FP_TRY(dev_alloc(epoch, b.depth, npix * 4));
+  FP_TRY(dev_alloc(epoch, b.xyz, npix * 16));
+  if (raw) {
+    FP_TRY(dev_alloc(epoch, b.rgb_raw, npix * 3));
+    FP_TRY(dev_alloc(epoch, b.depth_raw, npix * 4));
+  }
+  if (staged) {
+    FP_TRY(pinned_alloc(nullptr, b.stage_rgb, npix * 3));
+    FP_TRY(pinned_alloc(nullptr, b.stage_depth, npix * 4));
+  }
   return 0;
 }
 
-static int alloc_frame_buffers(fp_ctx* c, size_t npix, bool need_raw) {
-  FP_TRY(dev_alloc(c->epoch, c->rgba, npix * 4));
-  FP_TRY(dev_alloc(c->epoch, c->depth_a, npix * 4));
-  FP_TRY(dev_alloc(c->epoch, c->depth_b, npix * 4));
-  FP_TRY(dev_alloc(c->epoch, c->xyz, npix * 16));
-  if (need_raw) {
-    FP_TRY(dev_alloc(c->epoch, c->rgb_raw, npix * 3));
-    FP_TRY(dev_alloc(c->epoch, c->depth_raw, npix * 4));
-  }
-  return 0;
-}
-
-// records K / H / W as the context's frame geometry
+// records K / H / W as the context's frame geometry (a graph that holds them by value is captured again when they
+// change, see run_graphed)
 static void set_frame_geometry(fp_ctx* c, const float* K, int H, int W) {
   for (int i = 0; i < 9; ++i) c->K[i] = K[i];
   c->H = H;
   c->W = W;
-}
-
-// frame buffers + intrinsics (a graph that holds them by value is captured again when they change, see run_graphed)
-static int prepare_frame(fp_ctx* c, const float* K, int H, int W, bool need_raw) {
-  FP_TRY(alloc_frame_buffers(c, (size_t)H * W, need_raw));
-  set_frame_geometry(c, K, H, W);
-  return 0;
 }
 
 // mesh_of: [N] device slot ids, or null = slot 0 for every hypothesis; cams / camera_of as make_crops
@@ -691,106 +689,91 @@ static int refine_body(fp_ctx* c, int N, int iterations, cudaStream_t s2, const 
   return 0;
 }
 
-// pinned host staging of the context's frame (fp_track, fp_track_objects, fp_track_cameras' camera 0,
-// fp_register_objects).  No graph holds these addresses: upload_staged_frame copies out of them ahead of the launch.
-static int alloc_frame_staging(fp_ctx* c, size_t npix) {
-  FP_TRY(pinned_alloc(nullptr, c->stage_rgb, npix * 3));
-  return pinned_alloc(nullptr, c->stage_depth, npix * 4);
-}
-
 // The previous frame's graph has finished (every caller synchronises), so the staging buffers are free.  The two
 // uploads are issued as soon as their staging copy is done — the depth DMA runs under the host's rgb copy, the
 // rgb DMA under the next camera's copies or the graph launch — instead of being nodes of the graph (measured: -40 us
 // per frame)
-static int upload_staged_frame(void* stage_rgb, void* stage_depth, void* rgb_dev, void* depth_dev,
-                               const unsigned char* rgb_host, const float* depth_host, size_t npix, cudaStream_t st) {
-  memcpy(stage_depth, depth_host, npix * 4);
-  FP_CUDA_OK(cudaMemcpyAsync(depth_dev, stage_depth, npix * 4, cudaMemcpyHostToDevice, st));
-  memcpy(stage_rgb, rgb_host, npix * 3);
-  FP_CUDA_OK(cudaMemcpyAsync(rgb_dev, stage_rgb, npix * 3, cudaMemcpyHostToDevice, st));
-  return 0;
-}
-static int upload_staged_frame(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, size_t npix,
+static int upload_staged_frame(CameraBufs& b, const unsigned char* rgb_host, const float* depth_host, size_t npix,
                                cudaStream_t st) {
-  return upload_staged_frame(c->stage_rgb.p, c->stage_depth.p, c->rgb_raw.p, c->depth_raw.p, rgb_host, depth_host, npix, st);
-}
-
-// Frame buffers and pinned staging of cameras 1.. of a multi-camera call, at npix_max pixels each (camera 0 is the
-// context's frame, sized by the caller).  Only the camera table holds these addresses: no graph is affected.
-static int alloc_camera_bufs(fp_ctx* c, int C, size_t npix_max) {
-  for (int i = 1; i < C; ++i) {
-    CameraBufs& b = c->cams[i];
-    unsigned long long table_only = 0;
-    FP_TRY(dev_alloc(table_only, b.rgb_raw, npix_max * 3));
-    FP_TRY(dev_alloc(table_only, b.depth_raw, npix_max * 4));
-    FP_TRY(dev_alloc(table_only, b.rgba, npix_max * 4));
-    FP_TRY(dev_alloc(table_only, b.depth, npix_max * 4));
-    FP_TRY(dev_alloc(table_only, b.xyz, npix_max * 16));
-    FP_TRY(pinned_alloc(nullptr, b.stage_rgb, npix_max * 3));
-    FP_TRY(pinned_alloc(nullptr, b.stage_depth, npix_max * 4));
-  }
+  memcpy(b.stage_depth.p, depth_host, npix * 4);
+  FP_CUDA_OK(cudaMemcpyAsync(b.depth_raw.p, b.stage_depth.p, npix * 4, cudaMemcpyHostToDevice, st));
+  memcpy(b.stage_rgb.p, rgb_host, npix * 3);
+  FP_CUDA_OK(cudaMemcpyAsync(b.rgb_raw.p, b.stage_rgb.p, npix * 3, cudaMemcpyHostToDevice, st));
   return 0;
 }
 
-// The camera table of C cameras (entries C.. zeroed): buffers, size and intrinsics (K: [C][9]) of every camera
-static void fill_camera_table(const fp_ctx* c, int C, const float* K, const int* H, const int* W, CameraDev* table) {
-  memset(table, 0, sizeof(CameraDev) * kMaxCameras);
+// The uploaded frames filtered for tracking and registration (erode + bilateral, depth2xyzmap with zfar = inf).  cams
+// null: camera 0's frame by value (the single-camera kernels; FPOSE_FUSED_PREP applies).  Otherwise cameras 0..C-1 from
+// the device camera table in one launch over a grid_h x grid_w grid.
+static int prepare_frames(fp_ctx* c, const CameraDev* cams, int C, int grid_h, int grid_w, cudaStream_t st) {
+  if (!cams)
+    return set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->cam[0].rgb_raw.p),
+                              reinterpret_cast<const float*>(c->cam[0].depth_raw.p), FP_FRAME_FILTER_DEPTH, INFINITY, st);
+  c->depth_cur = reinterpret_cast<const float*>(c->cam[0].depth.p);
+  return frame_prep_cameras_launch(cams, C, grid_h, grid_w, INFINITY, st);
+}
+
+constexpr size_t kTableBytes = sizeof(CameraDev) * kMaxCameras;  // the camera table at the head of fp_ctx::args
+
+// The cameras of fp_track_cameras / _objects and fp_register_cameras / _objects, before anything reads a frame.  Every
+// camera's buffers are sized for the largest frame of the call (kept at the largest size seen, so a permutation of the
+// same cameras allocates nothing), camera 0's geometry becomes the context's, the argument block is sized for `rows`
+// slot and camera ids and its staging for `staged_rows`, the staging receives the camera table (buffers, size and
+// intrinsics, K: [C][9]; entries C.. zeroed), and every frame is uploaded through its camera's staging (camera i's DMA
+// runs while camera i + 1 is copied on the host).  H_max / W_max: the largest frame height and width of the call.
+static int setup_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
+                         const float* K, const int* H, const int* W, int rows, int staged_rows, cudaStream_t st,
+                         int& H_max, int& W_max) {
+  size_t npix_max = 0;
+  H_max = W_max = 0;
   for (int i = 0; i < C; ++i) {
+    npix_max = std::max(npix_max, (size_t)H[i] * W[i]);
+    H_max = std::max(H_max, H[i]);
+    W_max = std::max(W_max, W[i]);
+  }
+  for (int i = 0; i < C; ++i) FP_TRY(alloc_camera(c, i, npix_max, /*raw=*/true, /*staged=*/true));
+  set_frame_geometry(c, K, H[0], W[0]);
+  FP_TRY(dev_alloc(c->epoch, c->args, kTableBytes + (size_t)2 * rows * sizeof(int)));
+  FP_TRY(pinned_alloc(nullptr, c->stage_args, kTableBytes + (size_t)2 * staged_rows * sizeof(int)));
+  CameraDev* table = reinterpret_cast<CameraDev*>(c->stage_args.p);
+  memset(table, 0, kTableBytes);
+  for (int i = 0; i < C; ++i) {
+    CameraBufs& b = c->cam[i];
     CameraDev& e = table[i];
-    e.rgb_raw = reinterpret_cast<const unsigned char*>(i ? c->cams[i].rgb_raw.p : c->rgb_raw.p);
-    e.depth_raw = reinterpret_cast<const float*>(i ? c->cams[i].depth_raw.p : c->depth_raw.p);
-    e.rgb = reinterpret_cast<uchar4*>(i ? c->cams[i].rgba.p : c->rgba.p);
-    e.depth = reinterpret_cast<float*>(i ? c->cams[i].depth.p : c->depth_b.p);
-    e.xyz_map = reinterpret_cast<float4*>(i ? c->cams[i].xyz.p : c->xyz.p);
+    e.rgb_raw = reinterpret_cast<const unsigned char*>(b.rgb_raw.p);
+    e.depth_raw = reinterpret_cast<const float*>(b.depth_raw.p);
+    e.rgb = reinterpret_cast<uchar4*>(b.rgba.p);
+    e.depth = reinterpret_cast<float*>(b.depth.p);
+    e.xyz_map = reinterpret_cast<float4*>(b.xyz.p);
     e.fx = K[9 * i + 0];
     e.fy = K[9 * i + 4];
     e.cx = K[9 * i + 2];
     e.cy = K[9 * i + 5];
     e.H = H[i];
     e.W = W[i];
-  }
-}
-
-// Every camera's frame through its own pinned staging; camera i's DMA runs while camera i + 1 is copied on the host
-static int upload_camera_frames(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
-                                const int* H, const int* W, cudaStream_t st) {
-  for (int i = 0; i < C; ++i) {
-    const size_t npix = (size_t)H[i] * W[i];
-    if (i == 0) {
-      FP_TRY(upload_staged_frame(c, rgb_host[0], depth_host[0], npix, st));
-    } else {
-      CameraBufs& b = c->cams[i];
-      FP_TRY(upload_staged_frame(b.stage_rgb.p, b.stage_depth.p, b.rgb_raw.p, b.depth_raw.p, rgb_host[i], depth_host[i], npix, st));
-    }
+    FP_TRY(upload_staged_frame(b, rgb_host[i], depth_host[i], (size_t)H[i] * W[i], st));
   }
   return 0;
 }
 
-// fp_track_cameras and fp_track_objects after validation.  Camera 0 is the context's frame (buffers, staging, K / H / W),
-// cameras 1.. have buffers of their own.
-//   by_value = false (fp_track_cameras): every camera's buffers are sized for the largest frame of the call, so a
-//     permutation of the same cameras reallocates nothing.  The camera table, the slot ids and the camera ids go to one
-//     fixed device block in one copy ahead of the launch: the graph holds that block's address, not the frames' sizes,
-//     intrinsics or buffers, and is keyed on (C, M, iterations).  One frame_prep_kernel launch filters every camera
-//     (FPOSE_FUSED_PREP=0 does not apply) and the crops take their frame from the table.
-//   by_value = true (fp_track_objects, C = 1): the context's frame as fp_track sees it; the frame filters and the crop
+// fp_track_cameras and fp_track_objects after validation.  The camera table, the slot ids and the camera ids go to the
+// argument block in one copy ahead of the launch.
+//   by_value = false (fp_track_cameras): the graph holds the block's address, not the frames' sizes, intrinsics or
+//     buffers, and is keyed on (C, M, iterations): reordering objects or cameras or new intrinsics replay it.  One
+//     frame_prep_kernel launch filters every camera (FPOSE_FUSED_PREP=0 does not apply) and the crops take their frame
+//     from the table.
+//   by_value = true (fp_track_objects, C = 1): camera 0's frame as fp_track sees it; the frame filters and the crop
 //     producer take it by value (the single-camera kernel instantiations), so the graph is captured again when the
-//     frame's size or intrinsics change.  Only the slot ids are copied.
+//     frame's size or intrinsics change.  Its kernels read only the slot ids of the block.
 static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
                               const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
                               const float* poses_in_dev, int iterations, float* poses_out_dev, float* poses_out_host,
                               cudaStream_t st, bool by_value) {
-  size_t npix_max = 0;
-  int H_max = 0, W_max = 0;
-  for (int i = 0; i < C; ++i) {
-    npix_max = std::max(npix_max, (size_t)H[i] * W[i]);
-    H_max = std::max(H_max, H[i]);
-    W_max = std::max(W_max, W[i]);
-  }
   FP_TRY(ensure_capacity(c, M));
-  FP_TRY(alloc_frame_buffers(c, npix_max, true));
-  FP_TRY(alloc_frame_staging(c, npix_max));
-  set_frame_geometry(c, K, H[0], W[0]);
+  FP_TRY(pinned_alloc(&c->epoch, c->stage_poses, (size_t)M * 64));  // the graph's read-back node holds this address
+  c->has_frame = false;
+  int H_max, W_max;
+  FP_TRY(setup_cameras(c, C, rgb_host, depth_host, K, H, W, M, M, st, H_max, W_max));
   if (!by_value && (H_max > c->cam_grid_h || W_max > c->cam_grid_w)) {
     // the frame-preparation grid is a by-value launch parameter: it covers the largest frame seen, the blocks outside
     // a smaller frame return at once
@@ -798,53 +781,29 @@ static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_
     c->cam_grid_h = std::max(c->cam_grid_h, H_max);
     c->cam_grid_w = std::max(c->cam_grid_w, W_max);
   }
-  FP_TRY(alloc_camera_bufs(c, C, npix_max));
-  const size_t table_bytes = sizeof(CameraDev) * kMaxCameras;
-  const size_t args_bytes = table_bytes + (size_t)2 * M * sizeof(int);
-  FP_TRY(dev_alloc(c->epoch, c->cam_args, args_bytes));
-  FP_TRY(pinned_alloc(nullptr, c->stage_args, args_bytes));
-  FP_TRY(pinned_alloc(&c->epoch, c->stage_poses, (size_t)M * 64));  // the graph's read-back node holds this address
-  // the per-call arguments: one staged block, one copy
-  int* ints = reinterpret_cast<int*>(reinterpret_cast<char*>(c->stage_args.p) + table_bytes);
-  memcpy(ints, slots_host, (size_t)M * sizeof(int));
-  if (by_value) {
-    FP_CUDA_OK(cudaMemcpyAsync(reinterpret_cast<char*>(c->cam_args.p) + table_bytes, ints, (size_t)M * sizeof(int),
-                               cudaMemcpyHostToDevice, st));
-  } else {
-    fill_camera_table(c, C, K, H, W, reinterpret_cast<CameraDev*>(c->stage_args.p));
-    memcpy(ints + M, camera_of, (size_t)M * sizeof(int));
-    FP_CUDA_OK(cudaMemcpyAsync(c->cam_args.p, c->stage_args.p, args_bytes, cudaMemcpyHostToDevice, st));
-  }
-  const CameraDev* cams_dev = by_value ? nullptr : reinterpret_cast<const CameraDev*>(c->cam_args.p);
-  const int* mesh_of = reinterpret_cast<const int*>(reinterpret_cast<const char*>(c->cam_args.p) + table_bytes);
+  int* ids = reinterpret_cast<int*>(static_cast<char*>(c->stage_args.p) + kTableBytes);
+  memcpy(ids, slots_host, (size_t)M * sizeof(int));
+  memcpy(ids + M, camera_of, (size_t)M * sizeof(int));
+  FP_CUDA_OK(cudaMemcpyAsync(c->args.p, c->stage_args.p, kTableBytes + (size_t)2 * M * sizeof(int), cudaMemcpyHostToDevice,
+                             st));
+  const CameraDev* cams_dev = by_value ? nullptr : reinterpret_cast<const CameraDev*>(c->args.p);
+  const int* mesh_of = reinterpret_cast<const int*>(static_cast<const char*>(c->args.p) + kTableBytes);
   const int* cam_of = by_value ? nullptr : mesh_of + M;
   float* pa = reinterpret_cast<float*>(c->poses_a.p);
   float* pb = reinterpret_cast<float*>(c->poses_b.p);
   FP_CUDA_OK(cudaMemcpyAsync(pa, poses_in_dev, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
-  FP_TRY(upload_camera_frames(c, C, rgb_host, depth_host, H, W, st));
-  c->has_frame = false;
   const float* fin = (iterations % 2 == 0) ? pa : pb;
   const int grid_h = c->cam_grid_h, grid_w = c->cam_grid_w;
   auto body = [&](cudaStream_t s2) -> int {
     // estimater.py:250-268 for every object of every camera at once: each camera's frame filtered once, M hypotheses
     // each rendering its own mesh and cropping its own camera's frame
-    if (by_value) {
-      FP_TRY(set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->rgb_raw.p),
-                                reinterpret_cast<const float*>(c->depth_raw.p), FP_FRAME_FILTER_DEPTH, INFINITY, s2));
-    } else {
-      c->depth_cur = reinterpret_cast<const float*>(c->depth_b.p);
-      FP_TRY(frame_prep_cameras_launch(cams_dev, C, grid_h, grid_w, INFINITY, s2));
-    }
+    FP_TRY(prepare_frames(c, cams_dev, C, grid_h, grid_w, s2));
     c->has_frame = true;
     FP_TRY(refine_body(c, M, iterations, s2, mesh_of, cams_dev, cam_of));
     FP_CUDA_OK(cudaMemcpyAsync(c->stage_poses.p, fin, (size_t)M * 64, cudaMemcpyDeviceToHost, s2));
     return 0;
   };
-  if (by_value) {
-    FP_TRY(run_graphed(c, GraphKind::TrackObjects, M, iterations, st, body));
-  } else {
-    FP_TRY(run_graphed(c, GraphKind::TrackCameras, M, iterations, st, body, C, /*frame_by_value=*/false));
-  }
+  FP_TRY(run_graphed(c, GraphKind::TrackObjects, M, iterations, st, body, by_value ? -1 : C));
   c->has_frame = true;
   if (poses_out_dev) FP_CUDA_OK(cudaMemcpyAsync(poses_out_dev, fin, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
   FP_CUDA_OK(cudaStreamSynchronize(st));
@@ -900,16 +859,15 @@ static ScoreTailParams score_tail_params(const fp_ctx* c, const float* feats, in
 }
 
 // fp_register_cameras and fp_register_objects after validation (n_hyp_host is checked here, before anything is
-// enqueued).  Object i is seen by camera camera_of[i]; its mask is masks_host[i], of its camera's size.  Camera 0 is the
-// context's frame, cameras 1.. have buffers of their own (as track_cameras_body).
-//   by_value = false (fp_register_cameras): every camera's buffers are sized for the largest frame of the call.  One
-//     frame_prep_kernel launch filters every camera and the start-pose kernels read each object's depth, size and
-//     intrinsics from the camera table.  Each pass copies its slot ids and per-hypothesis camera ids into fixed context
-//     buffers and the crops take their frame from the table at its fixed address, so the refine / feature graphs hold
-//     no frame and are keyed on (kind, pass size, iterations) alone: reordering cameras or objects or changing
-//     intrinsics replays them.
+// enqueued).  Object i is seen by camera camera_of[i]; its mask is masks_host[i], of its camera's size.  Each pass copies
+// its slot ids and per-hypothesis camera ids to the argument block, so the refine / feature graphs hold no per-pass
+// address and are keyed on (kind, pass size, iterations, frame source).
+//   by_value = false (fp_register_cameras): the camera table goes to the argument block once per call.  One
+//     frame_prep_kernel launch filters every camera, the start-pose kernels read each object's depth, size and
+//     intrinsics from the table, and the crops take their frame from it: the graphs hold no frame, so reordering
+//     cameras or objects or changing intrinsics replays them.
 //   by_value = true (fp_register_objects, C = 1): the frame filters, the start-pose kernels and the crop producer take
-//     the context's frame by value (the single-camera kernel instantiations), as fp_register does.
+//     camera 0's frame by value (the single-camera kernel instantiations), as fp_register does.
 // Both: whole objects in the given order in passes of up to kRegisterPassCap hypotheses (an object above the cap alone),
 // then one segmented scorer tail over all objects.  Synchronises.
 static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
@@ -935,70 +893,50 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
   int max_pass = 0;
   for (size_t p = 0; p + 1 < pass_obj.size(); ++p) max_pass = std::max(max_pass, off[pass_obj[p + 1]] - off[pass_obj[p]]);
   // each object's mask at its byte offset of one block
-  size_t npix_max = 0;
-  int H_max = 0, W_max = 0;
-  for (int i = 0; i < C; ++i) {
-    npix_max = std::max(npix_max, (size_t)H[i] * W[i]);
-    H_max = std::max(H_max, H[i]);
-    W_max = std::max(W_max, W[i]);
-  }
   std::vector<size_t> mask_at(M + 1, 0);
   for (int i = 0; i < M; ++i) mask_at[i + 1] = mask_at[i] + (size_t)H[camera_of[i]] * W[camera_of[i]];
   const size_t mask_bytes = mask_at[M];
   // every workspace is sized for the largest pass here, so no pass bumps the graph epoch
   FP_TRY(ensure_capacity(c, max_pass));
   FP_TRY(ensure_tail(c, total));
-  FP_TRY(alloc_frame_buffers(c, npix_max, true));
-  set_frame_geometry(c, K, H[0], W[0]);
-  FP_TRY(alloc_frame_staging(c, npix_max));
-  FP_TRY(alloc_camera_bufs(c, C, npix_max));
-  FP_TRY(dev_alloc(c->epoch, c->mesh_of, (size_t)max_pass * sizeof(int)));
   FP_TRY(dev_alloc(c->epoch, c->seg_off, (size_t)(2 * M + 1) * sizeof(int)));  // offsets [M + 1], camera ids [M]
   FP_TRY(dev_alloc(c->epoch, c->reg_feats, (size_t)total * 512 * sizeof(float)));
   FP_TRY(dev_alloc(c->epoch, c->mask_buf, mask_bytes));
   FP_TRY(dev_alloc(c->epoch, c->mask_stats, (size_t)M * 6 * sizeof(unsigned int)));
   FP_TRY(dev_alloc(c->epoch, c->tail_counter, std::max<size_t>(16, (size_t)M * sizeof(unsigned int)), /*zero=*/true));
-  const size_t table_bytes = sizeof(CameraDev) * kMaxCameras;
-  if (!by_value) {
-    FP_TRY(dev_alloc(c->epoch, c->reg_cams, table_bytes));
-    FP_TRY(dev_alloc(c->epoch, c->reg_cam_of, (size_t)max_pass * sizeof(int)));
-    FP_TRY(dev_alloc(c->epoch, c->mask_off, (size_t)M * sizeof(size_t)));
-    FP_TRY(pinned_alloc(nullptr, c->stage_cams, table_bytes + (size_t)M * sizeof(size_t)));
-  }
-  // pinned staging (never read by a captured graph): the copies below leave as soon as they are enqueued
+  if (!by_value) FP_TRY(dev_alloc(c->epoch, c->mask_off, (size_t)M * sizeof(size_t)));
+  // pinned staging (never read by a captured graph): the copies below leave as soon as they are enqueued.  stage_ints:
+  // offsets [M + 1], camera of every object [M], one int of padding, each object's mask byte offset size_t [M]
   FP_TRY(pinned_alloc(nullptr, c->stage_masks, mask_bytes));
-  FP_TRY(pinned_alloc(nullptr, c->stage_ints, (size_t)(2 * M + 1 + 2 * total) * sizeof(int)));
-  // offsets [M + 1], camera of every object [M], slot of every hypothesis [total], camera of every hypothesis [total]
+  FP_TRY(pinned_alloc(nullptr, c->stage_ints, (size_t)(2 * M + 2) * sizeof(int) + (size_t)M * sizeof(size_t)));
+  c->has_frame = false;
+  int H_max, W_max;
+  FP_TRY(setup_cameras(c, C, rgb_host, depth_host, K, H, W, max_pass, total, st, H_max, W_max));
   int* ints = reinterpret_cast<int*>(c->stage_ints.p);
-  int* slot_of = ints + 2 * M + 1;
-  int* cam_of = slot_of + total;
+  size_t* stage_mask_off = reinterpret_cast<size_t*>(ints + 2 * M + 2);
   memcpy(ints, off.data(), (size_t)(M + 1) * sizeof(int));
   memcpy(ints + M + 1, camera_of, (size_t)M * sizeof(int));
-  for (int i = 0; i < M; ++i) {
-    std::fill(slot_of + off[i], slot_of + off[i + 1], slots_host[i]);
-    std::fill(cam_of + off[i], cam_of + off[i + 1], camera_of[i]);
-    memcpy(reinterpret_cast<unsigned char*>(c->stage_masks.p) + mask_at[i], masks_host[i], mask_at[i + 1] - mask_at[i]);
+  memcpy(stage_mask_off, mask_at.data(), (size_t)M * sizeof(size_t));
+  for (int i = 0; i < M; ++i)
+    memcpy(static_cast<unsigned char*>(c->stage_masks.p) + mask_at[i], masks_host[i], mask_at[i + 1] - mask_at[i]);
+  // the ids of the pass starting at row r0 are staged at 2 * r0 after the table: its slot ids, then its camera ids
+  int* ids = reinterpret_cast<int*>(static_cast<char*>(c->stage_args.p) + kTableBytes);
+  for (size_t p = 0; p + 1 < pass_obj.size(); ++p) {
+    const int row0 = off[pass_obj[p]], n = off[pass_obj[p + 1]] - row0;
+    for (int i = pass_obj[p]; i < pass_obj[p + 1]; ++i) {
+      std::fill(ids + row0 + off[i], ids + row0 + off[i + 1], slots_host[i]);
+      std::fill(ids + row0 + n + off[i], ids + row0 + n + off[i + 1], camera_of[i]);
+    }
   }
   FP_CUDA_OK(cudaMemcpyAsync(c->seg_off.p, ints, (size_t)(2 * M + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
   FP_CUDA_OK(cudaMemcpyAsync(c->mask_buf.p, c->stage_masks.p, mask_bytes, cudaMemcpyHostToDevice, st));
-  const CameraDev* cams_dev = by_value ? nullptr : reinterpret_cast<const CameraDev*>(c->reg_cams.p);
-  if (!by_value) {
-    char* stage = reinterpret_cast<char*>(c->stage_cams.p);
-    fill_camera_table(c, C, K, H, W, reinterpret_cast<CameraDev*>(stage));
-    memcpy(stage + table_bytes, mask_at.data(), (size_t)M * sizeof(size_t));
-    FP_CUDA_OK(cudaMemcpyAsync(c->reg_cams.p, stage, table_bytes, cudaMemcpyHostToDevice, st));
-    FP_CUDA_OK(cudaMemcpyAsync(c->mask_off.p, stage + table_bytes, (size_t)M * sizeof(size_t), cudaMemcpyHostToDevice, st));
+  const CameraDev* cams_dev = by_value ? nullptr : reinterpret_cast<const CameraDev*>(c->args.p);
+  if (cams_dev) {
+    FP_CUDA_OK(cudaMemcpyAsync(c->args.p, c->stage_args.p, kTableBytes, cudaMemcpyHostToDevice, st));
+    FP_CUDA_OK(cudaMemcpyAsync(c->mask_off.p, stage_mask_off, (size_t)M * sizeof(size_t), cudaMemcpyHostToDevice, st));
   }
-  FP_TRY(upload_camera_frames(c, C, rgb_host, depth_host, H, W, st));
   // estimater.py:173-174, :214 once per camera for every object: erode + bilateral, depth2xyzmap(zfar = inf)
-  c->has_frame = false;
-  if (by_value) {
-    FP_TRY(set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->rgb_raw.p),
-                              reinterpret_cast<const float*>(c->depth_raw.p), FP_FRAME_FILTER_DEPTH, INFINITY, st));
-  } else {
-    c->depth_cur = reinterpret_cast<const float*>(c->depth_b.p);
-    FP_TRY(frame_prep_cameras_launch(cams_dev, C, H_max, W_max, INFINITY, st));
-  }
+  FP_TRY(prepare_frames(c, cams_dev, C, H_max, W_max, st));
   c->has_frame = true;
   // estimater.py:137-156, :203-209 for every object in one launch pair; the start poses go to poses_out_dev and are
   // replaced pass by pass with the refined ones
@@ -1016,32 +954,30 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
   float* pb = reinterpret_cast<float*>(c->poses_b.p);
   float* ps = reinterpret_cast<float*>(c->pose_stage.p);
   float* fb = reinterpret_cast<float*>(c->feat_buf.p);
-  const int* mesh_of = reinterpret_cast<const int*>(c->mesh_of.p);
-  const int* hyp_cam = by_value ? nullptr : reinterpret_cast<const int*>(c->reg_cam_of.p);
+  const int* mesh_of = reinterpret_cast<const int*>(static_cast<const char*>(c->args.p) + kTableBytes);
   const float* fin = (iterations % 2 == 0) ? pa : pb;
-  const GraphKind refine_kind = by_value ? GraphKind::RegisterRefine : GraphKind::RegisterCamerasRefine;
-  const GraphKind feature_kind = by_value ? GraphKind::RegisterFeatures : GraphKind::RegisterCamerasFeatures;
+  const int frame = by_value ? -1 : 0;  // from the table: prepared above, outside the graphs
   for (size_t p = 0; p + 1 < pass_obj.size(); ++p) {
     const int row0 = off[pass_obj[p]], n = off[pass_obj[p + 1]] - row0;
-    // the pass's slot ids, camera ids and start poses go to fixed context buffers and its outputs are copied out after
-    // the replays: the graphs hold no per-pass address and are keyed on (kind, n, iterations) alone
-    FP_CUDA_OK(cudaMemcpyAsync(c->mesh_of.p, slot_of + row0, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
-    if (!by_value)
-      FP_CUDA_OK(cudaMemcpyAsync(c->reg_cam_of.p, cam_of + row0, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+    const int* hyp_cam = by_value ? nullptr : mesh_of + n;
+    // the pass's slot and camera ids and its start poses go to fixed context buffers and its outputs are copied out
+    // after the replays: the graphs hold no per-pass address
+    FP_CUDA_OK(cudaMemcpyAsync(static_cast<char*>(c->args.p) + kTableBytes, ids + 2 * row0, (size_t)2 * n * sizeof(int),
+                               cudaMemcpyHostToDevice, st));
     FP_CUDA_OK(cudaMemcpyAsync(pa, poses_out_dev + (size_t)row0 * 16, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
     FP_TRY(run_graphed(
-        c, refine_kind, n, iterations, st,
-        [&](cudaStream_t s2) -> int { return refine_body(c, n, iterations, s2, mesh_of, cams_dev, hyp_cam); }, 0, by_value));
+        c, GraphKind::RegisterRefine, n, iterations, st,
+        [&](cudaStream_t s2) -> int { return refine_body(c, n, iterations, s2, mesh_of, cams_dev, hyp_cam); }, frame));
     FP_CUDA_OK(cudaMemcpyAsync(poses_out_dev + (size_t)row0 * 16, fin, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
     FP_CUDA_OK(cudaMemcpyAsync(ps, fin, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
     FP_TRY(run_graphed(
-        c, feature_kind, n, 0, st,
+        c, GraphKind::RegisterFeatures, n, 0, st,
         [&](cudaStream_t s2) -> int {
           FP_TRY(make_crops(c, ps, n, 1, nullptr, nullptr, nullptr, s2, mesh_of, cams_dev, hyp_cam));
           FP_TRY(run_encoder(c, c->net[1], reinterpret_cast<const __half*>(c->crops.p), n, s2));
           return run_score_feats(c, c->net[1], n, fb, s2);
         },
-        0, by_value));
+        frame));
     FP_CUDA_OK(cudaMemcpyAsync(reinterpret_cast<float*>(c->reg_feats.p) + (size_t)row0 * 512, fb, (size_t)n * 2048,
                                cudaMemcpyDeviceToDevice, st));
   }
@@ -1303,14 +1239,16 @@ int fp_set_frame(fp_ctx* c, const unsigned char* rgb, const float* depth, const 
   const size_t npix = (size_t)H * W;
   c->has_frame = false;
   const bool on_dev = (flags & FP_FRAME_ON_DEVICE) != 0;
-  FP_TRY(prepare_frame(c, K, H, W, !on_dev));
+  FP_TRY(alloc_camera(c, 0, npix, /*raw=*/!on_dev, /*staged=*/false));
+  set_frame_geometry(c, K, H, W);
   const unsigned char* rgb_dev = rgb;
   const float* depth_dev = depth;
   if (!on_dev) {
-    FP_CUDA_OK(cudaMemcpyAsync(c->rgb_raw.p, rgb, npix * 3, cudaMemcpyHostToDevice, st));
-    FP_CUDA_OK(cudaMemcpyAsync(c->depth_raw.p, depth, npix * 4, cudaMemcpyHostToDevice, st));
-    rgb_dev = reinterpret_cast<const unsigned char*>(c->rgb_raw.p);
-    depth_dev = reinterpret_cast<const float*>(c->depth_raw.p);
+    CameraBufs& f = c->cam[0];
+    FP_CUDA_OK(cudaMemcpyAsync(f.rgb_raw.p, rgb, npix * 3, cudaMemcpyHostToDevice, st));
+    FP_CUDA_OK(cudaMemcpyAsync(f.depth_raw.p, depth, npix * 4, cudaMemcpyHostToDevice, st));
+    rgb_dev = reinterpret_cast<const unsigned char*>(f.rgb_raw.p);
+    depth_dev = reinterpret_cast<const float*>(f.depth_raw.p);
   }
   FP_TRY(set_frame_launches(c, rgb_dev, depth_dev, flags, zfar, st));
   c->has_frame = true;
@@ -1325,7 +1263,7 @@ int fp_set_xyz_map(fp_ctx* c, const float* xyz, void* stream) {
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   // [H][W][3] (host or device) -> the float4-per-pixel layout the crop kernel samples
-  FP_CUDA_OK(cudaMemcpy2DAsync(c->xyz.p, 16, xyz, 12, 12, (size_t)c->H * c->W, cudaMemcpyDefault, st));
+  FP_CUDA_OK(cudaMemcpy2DAsync(c->cam[0].xyz.p, 16, xyz, 12, 12, (size_t)c->H * c->W, cudaMemcpyDefault, st));
   return 0;
   FP_API_END
 }
@@ -1339,7 +1277,7 @@ int fp_get_depth(fp_ctx* c, float* depth_out_dev, float* xyz_out_dev, void* stre
   if (depth_out_dev) FP_CUDA_OK(cudaMemcpyAsync(depth_out_dev, c->depth_cur, npix * 4, cudaMemcpyDeviceToDevice, st));
   // internal layout is float4 per pixel; the hook returns the reference's [H][W][3]
   if (xyz_out_dev)
-    FP_CUDA_OK(cudaMemcpy2DAsync(xyz_out_dev, 12, c->xyz.p, 16, 12, npix, cudaMemcpyDeviceToDevice, st));
+    FP_CUDA_OK(cudaMemcpy2DAsync(xyz_out_dev, 12, c->cam[0].xyz.p, 16, 12, npix, cudaMemcpyDeviceToDevice, st));
   return 0;
   FP_API_END
 }
@@ -1550,23 +1488,22 @@ int fp_track(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, 
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   FP_TRY(ensure_capacity(c, 1));
-  FP_TRY(prepare_frame(c, K, H, W, true));
+  FP_TRY(alloc_camera(c, 0, (size_t)H * W, /*raw=*/true, /*staged=*/true));
+  set_frame_geometry(c, K, H, W);
   FP_TRY(dev_alloc(c->epoch, c->track_pose, 64));
-  FP_TRY(alloc_frame_staging(c, (size_t)H * W));
   FP_TRY(pinned_alloc(&c->epoch, c->stage_pose, 64));  // the graph's read-back node holds this address
   if (pose_in_dev) {
     FP_CUDA_OK(cudaMemcpyAsync(c->track_pose.p, pose_in_dev, 64, cudaMemcpyDeviceToDevice, st));
   } else {
     FP_REQUIRE(c->track_valid, "fp_track: no previous pose in this context: pass pose_in");
   }
-  FP_TRY(upload_staged_frame(c, rgb_host, depth_host, (size_t)H * W, st));
+  FP_TRY(upload_staged_frame(c->cam[0], rgb_host, depth_host, (size_t)H * W, st));
   c->has_frame = false;
   float* pa = reinterpret_cast<float*>(c->poses_a.p);
   float* pb = reinterpret_cast<float*>(c->poses_b.p);
   auto body = [&](cudaStream_t s2) -> int {
     // estimater.py:250-268 in one launch sequence: erode + bilateral, depth2xyzmap_batch(zfar=inf), K refiner passes
-    FP_TRY(set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->rgb_raw.p),
-                              reinterpret_cast<const float*>(c->depth_raw.p), FP_FRAME_FILTER_DEPTH, INFINITY, s2));
+    FP_TRY(prepare_frames(c, nullptr, 1, 0, 0, s2));
     FP_CUDA_OK(cudaMemcpyAsync(pa, c->track_pose.p, 64, cudaMemcpyDeviceToDevice, s2));
     c->has_frame = true;
     FP_TRY(refine_body(c, 1, iterations, s2));
