@@ -10,6 +10,14 @@ one `fp_pose_errors` call.  A frame the driver skipped (it writes the identity) 
 infinite.  An object is symmetric when the reader's `symmetry_tfs[ob_id]` holds more than the identity.  Printed per
 object and overall: the number of poses, ADD and ADD-S AUC (up to 0.1 m in 1 mm steps) and ADD(-S) < 0.1 d (ADD-S for
 symmetric objects, d = `get_model_diameter`).
+
+--bop adds BOP's symmetry-aware average recalls, scored by `fp_sym_pose_errors`: AR_MSSD over the thresholds
+0.05 d .. 0.50 d and AR_MSPD over 5 .. 50 px scaled by 640 / image width, both as the mean over the thresholds of the
+share of errors below each.  The symmetries are those of `models_info.json` (`reader.symmetry_info_table`) sampled by
+`metrics.bop_symmetries`, K is `reader.get_K(frame)` and the image width that of the video's frames.  The overall row
+scores every pose with its own object's thresholds.  The errors are taken over the same model vertices as the ADD
+columns, not over BOP's resampled `models_eval` points, so they are not comparable with the BOP leaderboard; and as
+VSD is not computed, no combined BOP AR is printed.
 """
 import argparse
 import json
@@ -65,6 +73,26 @@ def summarize_all(rows, errors):
             "add_s_recall": metrics.recall(crit, thr)}
 
 
+def bop_thresholds(diameter, widths):
+    """([T, n] MSSD, [T, n] MSPD) thresholds of n poses of one object, `widths` the image width of each pose's frame."""
+    widths = np.asarray(widths, dtype=np.float64).reshape(-1)
+    mssd = np.repeat(metrics.mssd_thresholds(diameter)[:, None], len(widths), axis=1)
+    mspd = np.stack([metrics.mspd_thresholds(w) for w in widths], axis=1).reshape(len(metrics.MSPD_STEPS), -1)
+    return mssd, mspd
+
+
+def summarize_bop(mssd, mspd, thresholds):
+    """AR_MSSD and AR_MSPD of one row from per-pose errors (inf for failures) and their [T, n] thresholds."""
+    return {"mssd_ar": metrics.average_recall(mssd, thresholds[0]), "mspd_ar": metrics.average_recall(mspd, thresholds[1])}
+
+
+def summarize_bop_all(errors, thresholds):
+    """Overall AR_MSSD / AR_MSPD: every pose, each with its own object's thresholds."""
+    cat = lambda lists: np.concatenate(lists, axis=-1)  # noqa: E731
+    return summarize_bop(cat([errors[o][2] for o in errors]), cat([errors[o][3] for o in errors]),
+                         (cat([thresholds[o][0] for o in errors]), cat([thresholds[o][1] for o in errors])))
+
+
 def make_reader_factory(kind, dataset_dir):
     from datareader import LinemodReader, YcbVideoReader
 
@@ -82,33 +110,58 @@ def make_reader_factory(kind, dataset_dir):
     return reader
 
 
-def evaluate(res, kind, dataset_dir):
-    """-> (rows {ob_id: row}, overall row, errors {ob_id: (add [n], adds [n])})."""
+def evaluate(res, kind, dataset_dir, bop=False):
+    """-> (rows {ob_id: row}, overall row, errors {ob_id: (add [n], adds [n])}).  With `bop`, every row also holds
+    `mssd_ar` and `mspd_ar`, and errors[ob_id] is (add, adds, mssd [n], mspd [n])."""
     reader = make_reader_factory(kind, dataset_dir)
-    rows, errors = {}, {}
+    rows, errors, thresholds, widths = {}, {}, {}, {}
     for ob_id, entries in group_by_object(res).items():
         r0 = reader(entries[0][0])
         frame = {vid: {s: i for i, s in enumerate(reader(vid).id_strs)} for vid in {e[0] for e in entries}}
         gt = np.stack([reader(vid).get_gt_pose(frame[vid][id_str], ob_id) for vid, id_str, _, _ in entries])
         pred = np.stack([e[2] for e in entries])
         skipped = np.array([e[3] for e in entries])
-        add, adds = metrics.pose_errors(r0.get_gt_mesh(ob_id).vertices, pred, gt)
+        pts = r0.get_gt_mesh(ob_id).vertices
+        add, adds = metrics.pose_errors(pts, pred, gt)
         add, adds = add.double().cpu().numpy(), adds.double().cpu().numpy()
         add[skipped], adds[skipped] = np.inf, np.inf
         errors[ob_id] = (add, adds)
         rows[ob_id] = summarize(add, adds, is_symmetric(r0.symmetry_tfs[ob_id]), r0.get_model_diameter(ob_id))
-    return rows, summarize_all(rows, errors) if rows else None, errors
+        if bop:
+            K = np.stack([reader(vid).get_K(frame[vid][id_str]) for vid, id_str, _, _ in entries])
+            for vid in frame:
+                if vid not in widths:
+                    widths[vid] = reader(vid).get_color(0).shape[1]
+            syms = metrics.bop_symmetries(r0.symmetry_info_table[ob_id])
+            mssd, mspd = metrics.sym_pose_errors(pts, pred, gt, syms, K)
+            mssd, mspd = mssd.double().cpu().numpy(), mspd.double().cpu().numpy()
+            mssd[skipped], mspd[skipped] = np.inf, np.inf
+            errors[ob_id] = (add, adds, mssd, mspd)
+            thresholds[ob_id] = bop_thresholds(r0.get_model_diameter(ob_id), [widths[e[0]] for e in entries])
+            rows[ob_id].update(summarize_bop(mssd, mspd, thresholds[ob_id]))
+    overall = summarize_all(rows, errors) if rows else None
+    if bop and rows:
+        overall.update(summarize_bop_all(errors, thresholds))
+    return rows, overall, errors
 
 
-def print_table(rows, overall):
-    print(f"{'object':>8} {'poses':>6} {'ADD AUC':>8} {'ADD-S AUC':>10} {'ADD(-S)<0.1d':>13}")
-    for ob_id, r in rows.items():
-        tag = f"{ob_id}{'*' if r['symmetric'] else ''}"
-        print(f"{tag:>8} {r['poses']:6d} {100 * r['add_auc']:8.2f} {100 * r['adds_auc']:10.2f} {100 * r['add_s_recall']:13.2f}")
-    if overall:
-        print(f"{'all':>8} {overall['poses']:6d} {100 * overall['add_auc']:8.2f} {100 * overall['adds_auc']:10.2f} "
-              f"{100 * overall['add_s_recall']:13.2f}")
-    print("(percent; * = symmetric object, scored by ADD-S in the last column)")
+def print_table(rows, overall, bop=False):
+    if not bop:
+        print(f"{'object':>8} {'poses':>6} {'ADD AUC':>8} {'ADD-S AUC':>10} {'ADD(-S)<0.1d':>13}")
+        for ob_id, r in rows.items():
+            tag = f"{ob_id}{'*' if r['symmetric'] else ''}"
+            print(f"{tag:>8} {r['poses']:6d} {100 * r['add_auc']:8.2f} {100 * r['adds_auc']:10.2f} {100 * r['add_s_recall']:13.2f}")
+        if overall:
+            print(f"{'all':>8} {overall['poses']:6d} {100 * overall['add_auc']:8.2f} {100 * overall['adds_auc']:10.2f} "
+                  f"{100 * overall['add_s_recall']:13.2f}")
+        print("(percent; * = symmetric object, scored by ADD-S in the last column)")
+        return
+    print(f"{'object':>8} {'poses':>6} {'ADD AUC':>8} {'ADD-S AUC':>10} {'ADD(-S)<0.1d':>13} {'AR MSSD':>8} {'AR MSPD':>8}")
+    for tag, r in [(f"{o}{'*' if r['symmetric'] else ''}", r) for o, r in rows.items()] + ([("all", overall)] if overall else []):
+        print(f"{tag:>8} {r['poses']:6d} {100 * r['add_auc']:8.2f} {100 * r['adds_auc']:10.2f} {100 * r['add_s_recall']:13.2f} "
+              f"{100 * r['mssd_ar']:8.2f} {100 * r['mspd_ar']:8.2f}")
+    print("(percent; * = symmetric object, scored by ADD-S in the fifth column; MSSD / MSPD over the model vertices, "
+          "not BOP's models_eval points, and without VSD, so there is no BOP AR)")
 
 
 def main(argv=None):
@@ -117,10 +170,11 @@ def main(argv=None):
     ap.add_argument("--dataset_dir", required=True, help="the --linemod_dir / --ycbv_dir the driver ran on")
     ap.add_argument("--kind", choices=("lm", "ycbv"), default=None, help="default: ycbv if the file name says so, else lm")
     ap.add_argument("--json", default=None, help="also write the table as JSON here")
+    ap.add_argument("--bop", action="store_true", help="also BOP's symmetry-aware AR_MSSD and AR_MSPD")
     opt = ap.parse_args(argv)
     kind = opt.kind or ("ycbv" if "ycbv" in os.path.basename(opt.res) else "lm")
-    rows, overall, _ = evaluate(load_results(opt.res), kind, opt.dataset_dir)
-    print_table(rows, overall)
+    rows, overall, _ = evaluate(load_results(opt.res), kind, opt.dataset_dir, bop=opt.bop)
+    print_table(rows, overall, bop=opt.bop)
     if opt.json:
         with open(opt.json, "w") as fh:
             json.dump({"objects": {str(k): v for k, v in rows.items()}, "overall": overall}, fh, indent=1)

@@ -60,6 +60,9 @@ lib.fp_op_gemm_layer.restype = C.c_int
 lib.fp_pose_errors.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                C.c_void_p]
 lib.fp_pose_errors.restype = C.c_int
+lib.fp_sym_pose_errors.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
+                                   C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+lib.fp_sym_pose_errors.restype = C.c_int
 
 
 def check(rc, what=""):

@@ -13,25 +13,27 @@ const char* get_last_error();
 int prof_collect(int kind, double* total_ms, double* total_work, int* launches);
 int pose_errors_launch(const float* pts, int P, const float* pred, int N, const float* gt, int n_gt, float* add_out,
                        float* adds_out, cudaStream_t stream);
+int sym_pose_errors_launch(const float* pts, int P, const float* pred, int N, const float* gt, int n_gt, const float* sym,
+                           int S, const float* K, int n_K, float* mssd_out, float* mspd_out, cudaStream_t stream);
 }
 
 // 0 when `p` is memory a kernel on the current device may read and write, else -1 with the reason in fp_last_error()
-static int check_device_ptr(const void* p, const char* what) {
+static int check_device_ptr(const void* p, const char* what, const char* fn = "fp_pose_errors") {
   int dev = 0;
   FP_CUDA_OK(cudaGetDevice(&dev));
   cudaPointerAttributes a;
   const cudaError_t e = cudaPointerGetAttributes(&a, p);
   if (e != cudaSuccess) {
     cudaGetLastError();  // not sticky; keep it out of the next caller's error check
-    fp::set_last_error("fp_pose_errors: %s: cudaPointerGetAttributes failed (%s)", what, cudaGetErrorString(e));
+    fp::set_last_error("%s: %s: cudaPointerGetAttributes failed (%s)", fn, what, cudaGetErrorString(e));
     return -1;
   }
   if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) {
-    fp::set_last_error("fp_pose_errors: %s is not device memory", what);
+    fp::set_last_error("%s: %s is not device memory", fn, what);
     return -1;
   }
   if (a.type == cudaMemoryTypeDevice && a.device != dev) {
-    fp::set_last_error("fp_pose_errors: %s lives on device %d, the current device is %d", what, a.device, dev);
+    fp::set_last_error("%s: %s lives on device %d, the current device is %d", fn, what, a.device, dev);
     return -1;
   }
   return 0;
@@ -189,6 +191,25 @@ int fp_pose_errors(const float* pts, int P, const float* pred, int N, const floa
   for (int i = 0; i < 5; ++i)
     if (ptrs[i] && check_device_ptr(ptrs[i], names[i])) return -1;
   return fp::pose_errors_launch(pts, P, pred, N, gt, n_gt, add_out, adds_out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int fp_sym_pose_errors(const float* pts, int P, const float* pred, int N, const float* gt, int n_gt, const float* sym,
+                       int S, const float* K, int n_K, float* mssd_out, float* mspd_out, void* stream) {
+  FP_REQUIRE(P >= 1 && P <= FP_METRICS_MAX_POINTS, "fp_sym_pose_errors: P = %d outside [1, %d]", P, FP_METRICS_MAX_POINTS);
+  FP_REQUIRE(N >= 0 && N <= FP_METRICS_MAX_POSES, "fp_sym_pose_errors: N = %d outside [0, %d]", N, FP_METRICS_MAX_POSES);
+  FP_REQUIRE(S >= 1 && S <= FP_METRICS_MAX_SYMMETRIES, "fp_sym_pose_errors: S = %d outside [1, %d]", S,
+             FP_METRICS_MAX_SYMMETRIES);
+  FP_REQUIRE(n_gt == 1 || n_gt == N, "fp_sym_pose_errors: n_gt = %d, must be 1 or N = %d", n_gt, N);
+  if (mspd_out) FP_REQUIRE(n_K == 1 || n_K == N, "fp_sym_pose_errors: n_K = %d, must be 1 or N = %d", n_K, N);
+  if (N == 0) return 0;
+  FP_REQUIRE(pts && pred && gt && sym, "fp_sym_pose_errors: null input pointer");
+  FP_REQUIRE(K || !mspd_out, "fp_sym_pose_errors: mspd_out needs K");
+  const void* ptrs[7] = {pts, pred, gt, sym, mspd_out ? K : nullptr, mssd_out, mspd_out};
+  const char* names[7] = {"pts", "pred", "gt", "sym", "K", "mssd_out", "mspd_out"};
+  for (int i = 0; i < 7; ++i)
+    if (ptrs[i] && check_device_ptr(ptrs[i], names[i], "fp_sym_pose_errors")) return -1;
+  return fp::sym_pose_errors_launch(pts, P, pred, N, gt, n_gt, sym, S, K, n_K, mssd_out, mspd_out,
+                                    reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -10,6 +10,17 @@
 //                       Per-query distances are summed in fp64 in a fixed order (slots, warp tree, warps, then the
 //                       eight CTAs in rank order over distributed shared memory), and the launch shape depends on P
 //                       only: a pose's errors are bit-identical across calls and batch sizes.
+//
+//   sym_pose_errors_kernel  BOP's MSSD / MSPD: one CTA per pose.  The model points are staged through shared memory
+//                       in tiles of kSymTile, each with its image under the estimated pose E (and that image's
+//                       projection).  A work item is one symmetry s over one chunk of the tile: the warp composes G s
+//                       in registers, every lane takes a point of the chunk at a time and keeps the largest squared
+//                       distance, and the warp's maximum is merged into s's slot in shared memory by an integer
+//                       atomicMax (squared distances are >= +0, so their bit patterns order as the floats do).  The
+//                       minimum over the slots is taken once at the end.  Max and min are exact and every distance is
+//                       one expression of (point, E, G, s, K), so the results do not depend on the launch shape, on
+//                       the batch or on the order of the symmetries.
+#include "../../include/fpose.h"
 #include "fp_common.cuh"
 
 namespace fp {
@@ -158,6 +169,178 @@ int pose_errors_launch(const float* pts, int P, const float* pred, int N, const 
   else
     e = launch_pdl(pose_errors_kernel<false, true>, grid, block, 0, stream, kMetCluster, pts, P, pred, gt, gt_stride, add_out,
                    adds_out, batches, per_batch);
+  FP_CUDA_OK(e);
+  note_launches(1);
+  FP_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// MSSD / MSPD
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int kSymTile = 1024;    // model points per shared-memory tile
+constexpr int kSymThreads = 256;  // threads per CTA
+constexpr int kSymWarps = kSymThreads / 32;
+
+// NaN-propagating maximum: a NaN distance must win over every number (fmaxf would drop it)
+__device__ __forceinline__ float max_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+// the squared maximum of a work item as an ordered bit pattern: NaN counts as +inf
+__device__ __forceinline__ unsigned worst_bits(float w) { return w == w ? __float_as_uint(w) : 0x7f800000u; }
+
+// [R | t] rows of G s for a row-major 4x4 symmetry s, in fp32.  For s = I every sum is x * 1 + 0 terms: G s = G exactly.
+__device__ __forceinline__ void compose_sym(const float (&g)[12], const float* __restrict__ s, float (&m)[12]) {
+  float a[12];
+#pragma unroll
+  for (int i = 0; i < 12; ++i) a[i] = __ldg(s + i);
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+      m[4 * r + c] = fmaf(g[4 * r], a[c], fmaf(g[4 * r + 1], a[4 + c], g[4 * r + 2] * a[8 + c]));
+    m[4 * r + 3] = fmaf(g[4 * r], a[3], fmaf(g[4 * r + 1], a[7], fmaf(g[4 * r + 2], a[11], g[4 * r + 3])));
+  }
+}
+// rows 0 and 1 of K [R | t]: the numerators of the projection
+__device__ __forceinline__ void compose_k(const float (&k)[9], const float (&m)[12], float (&km)[8]) {
+#pragma unroll
+  for (int r = 0; r < 2; ++r)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) km[4 * r + c] = fmaf(k[3 * r], m[c], fmaf(k[3 * r + 1], m[4 + c], k[3 * r + 2] * m[8 + c]));
+}
+// pi(K, M p) = (K M p)[:2] / (M p)_z, for both poses by the same expression.  z = 0 gives +-inf or NaN, never a number.
+// __fmul_rn keeps the product rounded: contracted into the caller's subtraction it would differ from the staged one.
+__device__ __forceinline__ float2 project(const float (&km)[8], float depth, float x, float y, float z) {
+  const float r = __fdividef(1.f, depth);
+  return make_float2(__fmul_rn(fmaf(km[0], x, fmaf(km[1], y, fmaf(km[2], z, km[3]))), r),
+                     __fmul_rn(fmaf(km[4], x, fmaf(km[5], y, fmaf(km[6], z, km[7]))), r));
+}
+
+// grid = N CTAs of kSymThreads.  Dynamic shared memory: two float4 per tile point, (x y z u_E) and (E p, v_E), then
+// one slot per symmetry and metric.  `chunks` (1, 2, 4 or 8) splits every tile so that small S still fills the warps.
+template <bool kMssd, bool kMspd>
+__global__ void __launch_bounds__(kSymThreads) sym_pose_errors_kernel(const float* __restrict__ pts, int P,
+                                                                      const float* __restrict__ pred,
+                                                                      const float* __restrict__ gt, int gt_stride,
+                                                                      const float* __restrict__ sym, int S,
+                                                                      const float* __restrict__ Kmat, int k_stride,
+                                                                      float* __restrict__ mssd_out,
+                                                                      float* __restrict__ mspd_out, int chunks) {
+  extern __shared__ float4 sym_smem[];
+  float4* tile_a = sym_smem;
+  float4* tile_b = sym_smem + kSymTile;
+  unsigned* worst3 = reinterpret_cast<unsigned*>(sym_smem + 2 * kSymTile);  // [S] squared MSSD candidates
+  unsigned* worst2 = worst3 + (kMssd ? S : 0);                                // [S] squared MSPD candidates
+  __shared__ unsigned warp_best[2][kSymWarps];
+  const int pose = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  pdl_wait();
+  float me[12], mg[12], k[9], ke[8];
+  load_rt(pred + (size_t)pose * 16, me);
+  load_rt(gt + (size_t)pose * gt_stride, mg);
+  if (kMspd) {
+#pragma unroll
+    for (int i = 0; i < 9; ++i) k[i] = __ldg(Kmat + (size_t)pose * k_stride + i);
+    compose_k(k, me, ke);
+  }
+  for (int s = threadIdx.x; s < S * (int(kMssd) + int(kMspd)); s += kSymThreads) worst3[s] = 0u;
+  const int chunk = kSymTile / chunks, items = S * chunks;
+  for (int t0 = 0; t0 < P; t0 += kSymTile) {
+    const int n = min(kSymTile, P - t0);
+    __syncthreads();  // the previous tile has been consumed (and, first time round, the slots are zeroed)
+    for (int j = threadIdx.x; j < kSymTile; j += kSymThreads) {
+      // slots past the end repeat the tile's first point: a repeated pair cannot change a maximum
+      const float* p = pts + 3 * (size_t)(t0 + (j < n ? j : 0));
+      const float x = __ldg(p), y = __ldg(p + 1), z = __ldg(p + 2);
+      const float3 e = xform(me, x, y, z);
+      float2 uv = make_float2(0.f, 0.f);
+      if (kMspd) uv = project(ke, e.z, x, y, z);
+      tile_a[j] = make_float4(x, y, z, uv.x);
+      tile_b[j] = make_float4(e.x, e.y, e.z, uv.y);
+    }
+    __syncthreads();
+    for (int it = warp; it < items; it += kSymWarps) {
+      const int s = it / chunks, j0 = (it - s * chunks) * chunk;
+      if (j0 >= n) continue;  // uniform over the warp
+      float m[12], km[8];
+      compose_sym(mg, sym + (size_t)s * 16, m);
+      if (kMspd) compose_k(k, m, km);
+      float w3 = 0.f, w2 = 0.f;
+      const int j_end = min(j0 + chunk, (n + 31) & ~31);
+#pragma unroll 4
+      for (int j = j0 + lane; j < j_end; j += 32) {
+        const float4 a = tile_a[j], b = tile_b[j];
+        const float3 q = xform(m, a.x, a.y, a.z);
+        if (kMssd) {
+          const float dx = b.x - q.x, dy = b.y - q.y, dz = b.z - q.z;
+          w3 = max_nan(w3, fmaf(dx, dx, fmaf(dy, dy, dz * dz)));
+        }
+        if (kMspd) {
+          const float2 uv = project(km, q.z, a.x, a.y, a.z);
+          const float du = a.w - uv.x, dv = b.w - uv.y;
+          w2 = max_nan(w2, fmaf(du, du, dv * dv));
+        }
+      }
+      if (kMssd) {
+        const unsigned w = __reduce_max_sync(0xffffffffu, worst_bits(w3));
+        if (lane == 0) atomicMax(worst3 + s, w);
+      }
+      if (kMspd) {
+        const unsigned w = __reduce_max_sync(0xffffffffu, worst_bits(w2));
+        if (lane == 0) atomicMax(worst2 + s, w);
+      }
+    }
+  }
+  __syncthreads();
+  unsigned b3 = 0x7f800000u, b2 = 0x7f800000u;
+  for (int s = threadIdx.x; s < S; s += kSymThreads) {
+    if (kMssd) b3 = min(b3, worst3[s]);
+    if (kMspd) b2 = min(b2, worst2[s]);
+  }
+  b3 = __reduce_min_sync(0xffffffffu, b3);
+  b2 = __reduce_min_sync(0xffffffffu, b2);
+  if (lane == 0) {
+    warp_best[0][warp] = b3;
+    warp_best[1][warp] = b2;
+  }
+  __syncthreads();
+  if (threadIdx.x < 2) {
+    unsigned b = 0x7f800000u;
+#pragma unroll
+    for (int w = 0; w < kSymWarps; ++w) b = min(b, warp_best[threadIdx.x][w]);
+    if (threadIdx.x == 0 && kMssd) mssd_out[pose] = sqrtf(__uint_as_float(b));
+    if (threadIdx.x == 1 && kMspd) mspd_out[pose] = sqrtf(__uint_as_float(b));
+  }
+}
+
+// Arguments are checked by fp_sym_pose_errors (fp_api_ops.cu).  The launch shape is a function of S alone.
+int sym_pose_errors_launch(const float* pts, int P, const float* pred, int N, const float* gt, int n_gt, const float* sym,
+                           int S, const float* K, int n_K, float* mssd_out, float* mspd_out, cudaStream_t stream) {
+  if (N == 0 || (!mssd_out && !mspd_out)) return 0;
+  const int chunks = S >= kSymWarps ? 1 : S >= kSymWarps / 2 ? 2 : S >= kSymWarps / 4 ? 4 : 8;
+  const size_t smem = 2 * kSymTile * sizeof(float4) + (size_t)S * ((mssd_out ? 1 : 0) + (mspd_out ? 1 : 0)) * sizeof(unsigned);
+  const int gt_stride = n_gt == 1 ? 0 : 16, k_stride = n_K == 1 ? 0 : 9;
+  const dim3 grid((unsigned)N), block(kSymThreads);
+  static std::atomic<unsigned long long> attr_mask{0};  // per device: the attribute is device state
+  if (!device_bit_test(attr_mask)) {
+    const int most = 2 * kSymTile * (int)sizeof(float4) + 2 * FP_METRICS_MAX_SYMMETRIES * (int)sizeof(unsigned);
+    FP_CUDA_OK(cudaFuncSetAttribute(sym_pose_errors_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
+    FP_CUDA_OK(cudaFuncSetAttribute(sym_pose_errors_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
+    FP_CUDA_OK(cudaFuncSetAttribute(sym_pose_errors_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
+    device_bit_set(attr_mask);
+  }
+  cudaError_t e;
+  if (mssd_out && mspd_out)
+    e = launch_pdl(sym_pose_errors_kernel<true, true>, grid, block, smem, stream, 1, pts, P, pred, gt, gt_stride, sym, S, K,
+                   k_stride, mssd_out, mspd_out, chunks);
+  else if (mssd_out)
+    e = launch_pdl(sym_pose_errors_kernel<true, false>, grid, block, smem, stream, 1, pts, P, pred, gt, gt_stride, sym, S, K,
+                   k_stride, mssd_out, mspd_out, chunks);
+  else
+    e = launch_pdl(sym_pose_errors_kernel<false, true>, grid, block, smem, stream, 1, pts, P, pred, gt, gt_stride, sym, S, K,
+                   k_stride, mssd_out, mspd_out, chunks);
   FP_CUDA_OK(e);
   note_launches(1);
   FP_CUDA_OK(cudaGetLastError());

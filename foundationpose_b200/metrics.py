@@ -1,10 +1,17 @@
 """Pose accuracy: ADD / ADD-S on the GPU (`fp_pose_errors`) and the area-under-curve / recall summaries of
-FoundationPose's evaluation (Utils.py:232-266).
+FoundationPose's evaluation (Utils.py:232-266); BOP's symmetry-aware MSSD / MSPD on the GPU (`fp_sym_pose_errors`) and
+their average recalls.
 
     add, adds = pose_errors(model_pts, pred, gt)   # [N] float32 CUDA tensors, metres
     auc(adds.cpu().numpy())                          # AUC of the accuracy-threshold curve up to 0.1 m
     recall(add.cpu().numpy(), 0.1 * diameter)        # share of poses with ADD < 0.1 d
+
+    syms = bop_symmetries(models_info[str(ob_id)])   # (S, 4, 4) float64, metres, identity first
+    mssd, mspd = sym_pose_errors(model_pts, pred, gt, syms, K)   # [N] float32 CUDA tensors, metres / pixels
+    average_recall(mssd, mssd_thresholds(diameter))  # BOP's AR_MSSD
+    average_recall(mspd, mspd_thresholds(width))     # BOP's AR_MSPD
 """
+import math
 import ctypes as C
 
 import numpy as np
@@ -71,3 +78,106 @@ def recall(errs, threshold):
     """Share of the errors strictly below `threshold` (a scalar, or one threshold per error)."""
     errs = _host(errs)
     return float(np.mean(errs < np.asarray(threshold, dtype=np.float64)))
+
+
+def sym_pose_errors(model_pts, pred, gt, symmetries, K=None, mssd=True, mspd=True):
+    """BOP's MSSD (metres) and MSPD (pixels) of every pose in `pred` against `gt`, computed by libfpose.so:
+
+        MSSD = min_s max_i |E x_i - (G s) x_i|,   MSPD = min_s max_i |pi(K, E x_i) - pi(K, (G s) x_i)|
+
+    with pi(K, x) = (K x)[:2] / x_z.  model_pts: [P, 3]; pred: [N, 4, 4] or one [4, 4]; gt: one [4, 4] pose for every
+    prediction or [N, 4, 4]; symmetries: [S, 4, 4] in metres with the identity among them (`bop_symmetries`); K: one
+    [3, 3] or [N, 3, 3], needed for MSPD only.  numpy arrays or torch tensors (any device, any float dtype).  Returns
+    (mssd, mspd): float32 tensors [N] on the current CUDA device, None for a metric that was not requested.  A point
+    projected from z = 0 makes its symmetry's MSPD infinite.  There is no CPU path: without a CUDA device this raises.
+    """
+    if not torch.cuda.is_available():
+        raise _lib.FposeError("sym_pose_errors needs a CUDA device (there is no CPU path)")
+    if mspd and K is None:
+        raise _lib.FposeError("sym_pose_errors: MSPD needs the intrinsics K")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    pts = _device_f32(model_pts, dev, 3)
+    pred = _device_f32(pred, dev, 16)
+    gt = _device_f32(gt, dev, 16)
+    sym = _device_f32(symmetries, dev, 16)
+    k = _device_f32(K, dev, 9) if mspd else None
+    n = pred.shape[0]
+    mssd_out = torch.empty(n, dtype=torch.float32, device=dev) if mssd else None
+    mspd_out = torch.empty(n, dtype=torch.float32, device=dev) if mspd else None
+
+    def ptr(t):
+        return None if t is None or t.numel() == 0 else C.c_void_p(t.data_ptr())
+
+    rc = lib.fp_sym_pose_errors(ptr(pts), pts.shape[0], ptr(pred), n, ptr(gt), gt.shape[0], ptr(sym), sym.shape[0],
+                                ptr(k), 0 if k is None else k.shape[0], ptr(mssd_out), ptr(mspd_out),
+                                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+    _lib.check(rc, "fp_sym_pose_errors")
+    return mssd_out, mspd_out
+
+
+def _axis_rotation(axis, angle):
+    """Rodrigues: the rotation by `angle` about the unit vector along `axis`."""
+    a = np.asarray(axis, dtype=np.float64).reshape(3)
+    a = a / np.linalg.norm(a)
+    c, s = math.cos(angle), math.sin(angle)
+    cross = np.array([[0.0, -a[2], a[1]], [a[2], 0.0, -a[0]], [-a[1], a[0], 0.0]])
+    return c * np.eye(3) + s * cross + (1.0 - c) * np.outer(a, a)
+
+
+def bop_symmetries(model_info, max_sym_disc_step=0.01):
+    """The symmetry transforms of a BOP `models_info.json` entry, (S, 4, 4) float64 in metres, identity first.
+
+    Discrete: the identity and every `symmetries_discrete` entry (translations mm -> m).  Each continuous symmetry
+    (axis a, offset o in mm) is sampled as n = ceil(pi / max_sym_disc_step) rotations R_i by i 2 pi / n about a,
+    i = 0 .. n-1, with t_i = o - R_i o, so that no model point moves by more than `max_sym_disc_step` diameters between
+    steps.  The set is every continuous step composed with every discrete symmetry, R = R_c R_d, t = R_c t_d + t_c
+    (discrete outer, continuous inner); without continuous symmetries it is the discrete set.  This follows the
+    description of bop_toolkit's misc.get_symmetry_transformations, with step i = 0 included so that the identity is
+    always a member (a pose is never penalised against itself)."""
+    disc = [np.eye(4)]
+    for d in model_info.get("symmetries_discrete", []):
+        d = np.array(d, dtype=np.float64).reshape(4, 4)
+        d[:3, 3] *= 1e-3
+        disc.append(d)
+    cont = []
+    for sym in model_info.get("symmetries_continuous", []):
+        offset = np.asarray(sym["offset"], dtype=np.float64).reshape(3) * 1e-3
+        n = int(math.ceil(math.pi / max_sym_disc_step))
+        for i in range(n):
+            c = np.eye(4)
+            c[:3, :3] = _axis_rotation(sym["axis"], i * 2.0 * math.pi / n)
+            c[:3, 3] = offset - c[:3, :3] @ offset
+            cont.append(c)
+    if not cont:
+        return np.stack(disc)
+    out = []
+    for d in disc:
+        for c in cont:
+            m = np.eye(4)
+            m[:3, :3] = c[:3, :3] @ d[:3, :3]
+            m[:3, 3] = c[:3, :3] @ d[:3, 3] + c[:3, 3]
+            out.append(m)
+    return np.stack(out)
+
+
+MSSD_STEPS = np.arange(1, 11) * 0.05  # x the object diameter: 0.05 d .. 0.50 d
+MSPD_STEPS = np.arange(1, 11) * 5.0   # pixels at an image width of 640: 5 .. 50 px
+
+
+def mssd_thresholds(diameter):
+    """BOP's MSSD thresholds for an object of `diameter` metres."""
+    return MSSD_STEPS * float(diameter)
+
+
+def mspd_thresholds(image_width):
+    """BOP's MSPD thresholds in pixels, scaled from 640-pixel-wide images to `image_width`."""
+    return MSPD_STEPS * (640.0 / float(image_width))
+
+
+def average_recall(errs, thresholds):
+    """Mean over the thresholds of the share of errors strictly below each.  thresholds: [T] (the same for every
+    error) or [T, n] (column j for error j, e.g. each pose with its own object's thresholds)."""
+    errs = _host(errs)
+    thr = np.asarray(thresholds, dtype=np.float64)
+    thr = thr[:, None] if thr.ndim == 1 else thr
+    return float(np.mean(errs[None, :] < thr))

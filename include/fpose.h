@@ -99,6 +99,25 @@ int fp_op_attention(const void* qkv, void* out, int B, int impl, void* stream);
 int fp_pose_errors(const float* pts, int P, const float* pred, int N, const float* gt, int n_gt,
                    float* add_out, float* adds_out, void* stream);
 
+/* Largest symmetry set fp_sym_pose_errors accepts: four discrete symmetries times 315 steps of a continuous one fit
+ * three times over. */
+#define FP_METRICS_MAX_SYMMETRIES 4096
+/* MSSD / MSPD of the BOP Challenge (Hodan et al., "BOP Challenge 2020 on 6D Object Localization", ECCV Workshops
+ * 2020; bop_toolkit's pose_error.mssd / pose_error.mspd) of N poses against n_gt (1 or N) ground-truth poses over P model points and S symmetries, on the current device.
+ * pts [P][3] metres, pred [N][16], gt [n_gt][16], sym [S][16] row-major (metres, the identity included by the caller),
+ * K [n_K][9] row-major intrinsics (n_K 1 or N; needed only for mspd_out), outputs [N]: DEVICE float32.  mssd_out or
+ * mspd_out may be NULL (not computed).  1 <= P <= FP_METRICS_MAX_POINTS, 0 <= N <= FP_METRICS_MAX_POSES,
+ * 1 <= S <= FP_METRICS_MAX_SYMMETRIES.
+ *   MSSD = min_s max_i |E x_i - (G s) x_i|                    metres
+ *   MSPD = min_s max_i |pi(K, E x_i) - pi(K, (G s) x_i)|       pixels, pi(K, x) = (K x)[:2] / x_z
+ * G s is composed in fp32 on the device (for s = I it is G exactly, so a pose scored against itself gives 0); distances
+ * are fp32 differences of the transformed points.  A projection with x_z = 0 gives an infinite MSPD for that symmetry,
+ * never a NaN.  Deterministic: a pose's errors do not depend on N, on n_gt, on n_K or on the order of `sym`.  Costs
+ * O(N S P).  Every pointer must be device memory of the current device (cudaPointerGetAttributes); all arguments are
+ * checked before anything is enqueued.  Enqueued on `stream`; no sync. */
+int fp_sym_pose_errors(const float* pts, int P, const float* pred, int N, const float* gt, int n_gt, const float* sym,
+                       int S, const float* K, int n_K, float* mssd_out, float* mspd_out, void* stream);
+
 /* ------------------------------------------------------------------------------------------ */
 /* product path                                                                               */
 /* ------------------------------------------------------------------------------------------ */
