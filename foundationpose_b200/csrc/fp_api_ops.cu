@@ -179,6 +179,14 @@ int fp_op_gemm_tile_n(const fp_gemm_layer_t* l, int* tile_n) {
   return fp::gemm_layer_tile_n(to_gemm_layer(l), tile_n);
 }
 
+int fp_op_gemm_tile_m(const fp_gemm_layer_t* l, int* tile_m) {
+  if (!l || !tile_m) {
+    fp::set_last_error("fp_op_gemm_tile_m: null argument");
+    return -1;
+  }
+  return fp::gemm_layer_tile_m(to_gemm_layer(l), tile_m);
+}
+
 int fp_pose_errors(const float* pts, int P, const float* pred, int N, const float* gt, int n_gt, float* add_out,
                    float* adds_out, void* stream) {
   FP_REQUIRE(P >= 1 && P <= FP_METRICS_MAX_POINTS, "fp_pose_errors: P = %d outside [1, %d]", P, FP_METRICS_MAX_POINTS);

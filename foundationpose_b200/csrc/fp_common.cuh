@@ -239,6 +239,22 @@ __device__ __forceinline__ uint64_t gmma_desc_linear(uint32_t smem_addr, uint32_
   return d;
 }
 
+// Four 8 x 8 fp16 matrices between shared memory and registers, transposed.  Lane 8 i + r gives the address of row r
+// (16 bytes) of matrix i; register i of lane l holds that matrix's elements (row 2 (l % 4) + e, column l / 4), e = 0, 1.
+// So a memory row of eight consecutive channels of one pixel meets the wgmma accumulator fragment of a tile whose rows
+// are channels and whose columns are pixels.
+__device__ __forceinline__ void ldsm_x4_trans(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
+__device__ __forceinline__ void stsm_x4_trans(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]),
+               "r"(r[1]), "r"(r[2]), "r"(r[3])
+               : "memory");
+}
+
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&h);

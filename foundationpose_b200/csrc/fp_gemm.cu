@@ -8,7 +8,8 @@
 //   learning/models/score_network.py:60-74     encoderA / encoderAB / att projections
 //
 // Design (sm_90a, no library GEMM):
-//   * D[128 x BN] tiles (BN = 128; 256 for long 3x3 convolutions on tall grids; 64 for 64-channel layers), fp16
+//   * D[128 x BN] tiles (BN = 128; 256 for long 3x3 convolutions on tall grids; 64 for 64-channel layers; for the
+//     128-channel 3x3 convolutions on tall grids the swapped D^T[128 x 256 pixels] with the weights as M), fp16
 //     operands, fp32 accumulators in registers: two
 //     consumer warpgroups issue m64nBNk16 wgmmas on 64 rows each; one producer thread feeds a ring of TMA stages
 //     (A 16 KB + B BN x 128 B, 128-byte swizzle) through full / empty mbarriers.  Persistent CTAs, one per SM.
@@ -152,15 +153,23 @@ constexpr int kSmemOptIn = 232448;              // 227 KB opt-in shared memory p
 // slab per batch and store them all at the end.  The 256-wide tile has two slabs (a stage is 48 KB there, and with
 // two slabs four stages fit where four slabs leave three) and stores each batch as its own pass, alternating between
 // the slabs, so that one slab's store and the next batch's residual load run while the other slab is converted.
+//
+// kSwap (BN = 128): the operands trade places, D^T[128 channels x 256 pixels] = W[128 x K] * X^T[K x 256].  The
+// 16 KB M slot of a stage holds the tile's 128 weight rows and the N slot 256 pixels (a 5-D box of four images), so
+// each consumer warpgroup owns 64 channels over all 256 pixels and issues the m64n256k16 wgmmas of the 256-wide tile.
+// Its epilogue moves the transposed fragment through the slabs with ldmatrix / stmatrix .trans: four slabs, one per
+// (128-pixel half, 64-channel half), stored together at the end of the tile like the 64- and 128-wide tiles.
 constexpr int kWideSlabs = 2;
-constexpr int kWideProducerRegs = 40;   // setmaxnreg of the 256-wide tile: producer warpgroup ...
+constexpr int kWideProducerRegs = 40;   // setmaxnreg of the 256-wide tiles: producer warpgroup ...
 constexpr int kWideConsumerRegs = 232;  // ... and the two consumer warpgroups; 128 x 40 + 256 x 232 <= 384 x 168
-template <int BN>
+template <int BN, bool kSwap = false>
 struct TileCfg {
-  static constexpr int kBBytes = BN * kBlockK * 2;
+  static constexpr int kRows = kSwap ? 2 * kBlockM : kBlockM;  // output pixels (or linear rows) per tile
+  static constexpr int kN = kSwap ? kRows : BN;                 // wgmma N: pixels with kSwap, else channels
+  static constexpr int kBBytes = kN * kBlockK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kBatches = BN / 64;                         // 64-channel epilogue batches
-  static constexpr bool kAlternate = BN > 128;                     // one pass per batch, through alternating slabs
+  static constexpr int kBatches = (kRows / kBlockM) * (BN / 64);  // 128-pixel x 64-channel epilogue batches
+  static constexpr bool kAlternate = !kSwap && BN > 128;           // one pass per batch, through alternating slabs
   static constexpr int kSlabs = kAlternate ? kWideSlabs : kBatches;  // staging slabs
   static constexpr int kStagingBytes = kSlabs * kSlabBytes;
   static constexpr int kRing = kSmemOptIn - kStagingBytes - 1024 /*align slack*/ - 256 /*barriers*/;
@@ -175,13 +184,13 @@ struct TileCfg {
 // warpgroups issue m64nBNk16 wgmmas from it, then run the epilogue (+bias, +residual, ReLU, +pos.emb. -> fp16 ->
 // 128B-swizzled slabs -> one TMA tensor store per 64-channel slab).  The producer runs ahead into the next tile while
 // the consumers drain this one.  The 256-wide tile moves registers from the producer warpgroup to the consumers
-// (128 accumulators per thread do not fit the 168 a 384-thread CTA gets).
-template <int BN>
+// (128 accumulators per thread do not fit the 168 a 384-thread CTA gets), and so does the swapped tile.
+template <int BN, bool kSwap = false>
 __global__ void __launch_bounds__(kTileThreads, 1)
     gemm_tile_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                      const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res,
                      const __grid_constant__ GemmParams p) {
-  using Cfg = TileCfg<BN>;
+  using Cfg = TileCfg<BN, kSwap>;
   constexpr int S = Cfg::kStages;
   constexpr int NSLAB = Cfg::kSlabs;
   constexpr int NB = Cfg::kBatches;
@@ -224,7 +233,7 @@ __global__ void __launch_bounds__(kTileThreads, 1)
 
   if (threadIdx.x < 128) {
     // ------------------------------------------------------------------ TMA producer
-    if constexpr (BN > 128) regs_release<kWideProducerRegs>();  // all four warps, before three of them leave
+    if constexpr (Cfg::kN > 128) regs_release<kWideProducerRegs>();  // all four warps, before three of them leave
     if (threadIdx.x == 0) {
       int stage = 0, phase = 0;
       for (int t = blockIdx.x; t < total; t += gridDim.x) {
@@ -239,9 +248,11 @@ __global__ void __launch_bounds__(kTileThreads, 1)
           mbar_wait(&empty[stage], phase ^ 1);
           uint8_t* sa = smem + stage * Cfg::kStageBytes;
           mbar_expect_tx(&full[stage], Cfg::kStageBytes);
-          tma_load_5d(&map_a, &full[stage], sa, base[0] + p.tap_off[tap][0] + chunk * kBlockK, base[1] + p.tap_off[tap][1],
-                      base[2] + p.tap_off[tap][2], base[3] + p.tap_off[tap][3], base[4] + p.tap_off[tap][4]);
-          tma_load_2d(&map_b, &full[stage], sa + kABytes, kb * kBlockK, n_tile * BN);
+          // kSwap: the pixels are the N operand and the weights the M operand
+          tma_load_5d(&map_a, &full[stage], kSwap ? sa + kABytes : sa, base[0] + p.tap_off[tap][0] + chunk * kBlockK,
+                      base[1] + p.tap_off[tap][1], base[2] + p.tap_off[tap][2], base[3] + p.tap_off[tap][3],
+                      base[4] + p.tap_off[tap][4]);
+          tma_load_2d(&map_b, &full[stage], kSwap ? sa : sa + kABytes, kb * kBlockK, n_tile * BN);
           if (++chunk == p.chunks_per_tap) {
             chunk = 0;
             ++tap;
@@ -257,16 +268,20 @@ __global__ void __launch_bounds__(kTileThreads, 1)
   }
 
   // -------------------------------------------------------------------- consumers (warpgroups 1, 2)
-  if constexpr (BN > 128) regs_acquire<kWideConsumerRegs>();
+  if constexpr (Cfg::kN > 128) regs_acquire<kWideConsumerRegs>();
   const int ct = threadIdx.x - 128;
-  const int cw = ct >> 7;  // rows [64 cw, 64 cw + 64) of the tile
+  const int cw = ct >> 7;  // rows [64 cw, 64 cw + 64) of the tile (kSwap: channels, else pixels)
   const int lane = threadIdx.x & 31;
   const int r0 = 64 * cw + 16 * ((ct >> 5) & 3) + (lane >> 2);  // this thread's rows: r0 and r0 + 8
   const int cq = 2 * (lane & 3);                                  // and columns 8 j + cq, 8 j + cq + 1
   const bool leader = (ct == 0);
-  float acc[BN / 2];
+  // slab q of the tile: kSwap: pixel half q >> 1 (images 2 (q >> 1) and 2 (q >> 1) + 1 of the four), channel half q & 1;
+  // otherwise channels [64 q, 64 q + 64).  kSwap runs 3x3 convolutions only, whose image coordinate is 3.
+  auto slab_ch = [](int q) { return kSwap ? 64 * (q & 1) : 64 * q; };
+  auto slab_img = [](int q) { return kSwap ? 2 * (q >> 1) : 0; };
+  float acc[Cfg::kN / 2];
 #pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  for (int i = 0; i < Cfg::kN / 2; ++i) acc[i] = 0.f;
   int stage = 0, phase = 0, it = 0;
   for (int t = blockIdx.x; t < total; t += gridDim.x, ++it) {
     int n_tile, tw, th, tn;
@@ -285,18 +300,6 @@ __global__ void __launch_bounds__(kTileThreads, 1)
       oc[p.odim_n] = n_o0;
       rc[p.odim_n] = n0;
     }
-    // the previous tile's stores have left the staging slabs: fetch the residual of the tile's first NSLAB batches
-    // into them now, while the main loop runs (kAlt: one barrier per slab, else one for all)
-    if (leader) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    if (leader && p.has_res) {
-      for (int s = 0; s < NSLAB; ++s) {
-        uint64_t* rb = &res_full[kAlt ? s : 0];
-        if (kAlt || s == 0) mbar_expect_tx(rb, kAlt ? kSlabBytes : NSLAB * kSlabBytes);
-        tma_load_5d(&map_res, rb, staging + s * kSlabBytes, n_tile * BN + s * 64, rc[1], rc[2], rc[3], rc[4]);
-      }
-    }
-
     // ---- main loop: one wgmma batch (4 x K = 16) per k-block; a stage is released once the NEXT batch is issued
     int prev = -1;
     for (int kb = 0; kb < p.num_kb; ++kb) {
@@ -307,8 +310,23 @@ __global__ void __launch_bounds__(kTileThreads, 1)
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < kBlockK / 16; ++k)
-        Wgmma<BN>::ss(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
+        Wgmma<Cfg::kN>::ss(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
       wgmma_commit();
+      if (kb == 0 && leader) {
+        // The previous tile's stores leave the staging slabs while the first wgmmas run; only the leader waits for
+        // that, and the epilogue's barrier (or its residual wait) tells the other threads.  Then the residual of the
+        // tile's first NSLAB batches goes into the slabs and arrives while the main loop runs (kAlt: one barrier per
+        // slab, else one for all).
+        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+        if (p.has_res) {
+          for (int s = 0; s < NSLAB; ++s) {
+            uint64_t* rb = &res_full[kAlt ? s : 0];
+            if (kAlt || s == 0) mbar_expect_tx(rb, kAlt ? kSlabBytes : NSLAB * kSlabBytes);
+            tma_load_5d(&map_res, rb, staging + s * kSlabBytes, n_tile * BN + slab_ch(s), rc[1], rc[2],
+                        rc[3] + slab_img(s), rc[4]);
+          }
+        }
+      }
       if (prev >= 0) {
         wgmma_wait<1>();
         mbar_arrive(&empty[prev]);
@@ -318,6 +336,63 @@ __global__ void __launch_bounds__(kTileThreads, 1)
         stage = 0;
         phase ^= 1;
       }
+    }
+    if constexpr (kSwap) {
+      // ---- epilogue of the swapped tile: this thread holds channels r0 and r0 + 8 for pixels 8 j + cq (+1), j < 32.
+      // The same fp32 arithmetic as below (bias, residual, ReLU, one fp16 rounding) on each element.  An 8 x 8 block
+      // (column group j, channel half h) is one ldmatrix / stmatrix .trans matrix, whose memory rows are the block's
+      // eight pixels, each 16 bytes of eight consecutive channels: the slabs' swizzle unit.
+      const float bc[2] = {__ldg(p.bias + n_tile * BN + r0), __ldg(p.bias + n_tile * BN + r0 + 8)};
+      wgmma_wait<0>();
+      fence_regs(acc);
+      if (prev >= 0) mbar_arrive(&empty[prev]);
+      // the slabs are free: the residual arrived after the leader saw the previous stores read out, or the barrier
+      // tells every thread that the leader did
+      if (p.has_res) mbar_wait(&res_full[0], (uint32_t)(it & 1));
+      else asm volatile("bar.sync 1, 256;" ::: "memory");
+      // lane 8 i + r addresses row r of matrix i = (column group jl = i >> 1 of a pair, channel half h = i & 1): the
+      // pair's pixel 8 jl + r, 16-byte chunk 2 w + h of the warpgroup's 64 channels, swizzled by the pixel's row & 7
+      const int mi = lane >> 3, mr = lane & 7;
+      const uint32_t lane_off =
+          (uint32_t)(8 * (mi >> 1) + mr) * 128u + ((uint32_t)((2 * ((ct >> 5) & 3) + (mi & 1)) ^ mr) << 4);
+#pragma unroll
+      for (int ph = 0; ph < 2; ++ph) {
+        const uint32_t slab = smem_u32(staging + (2 * ph + cw) * kSlabBytes) + lane_off;
+        uint32_t rv[8][4];
+        if (p.has_res) {
+#pragma unroll
+          for (int g = 0; g < 8; ++g) ldsm_x4_trans(slab + g * 2048u, rv[g]);
+        }
+#pragma unroll
+        for (int g = 0; g < 8; ++g) {  // column groups j = 16 ph + 2 g, 16 ph + 2 g + 1: pixels 16 g .. 16 g + 15
+          uint32_t o[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int j = 16 * ph + 2 * g + (i >> 1), h = i & 1;
+            float a0 = acc[4 * j + 2 * h] + bc[h], a1 = acc[4 * j + 2 * h + 1] + bc[h];
+            if (p.has_res) {
+              const float2 r = __half22float2(*reinterpret_cast<const __half2*>(&rv[g][i]));
+              a0 += r.x;
+              a1 += r.y;
+            }
+            if (p.relu) {
+              a0 = fmaxf(a0, 0.f);
+              a1 = fmaxf(a1, 0.f);
+            }
+            o[i] = pack_half2(a0, a1);
+          }
+          stsm_x4_trans(slab + g * 2048u, o);
+        }
+      }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> async proxy
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (leader) {
+        for (int q = 0; q < NSLAB; ++q)
+          tma_store_5d(&map_out, staging + q * kSlabBytes, coff + n_tile * BN + slab_ch(q), oc[1], oc[2],
+                       oc[3] + slab_img(q), oc[4]);
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+      }
+      continue;
     }
     // ---- epilogue: 64-channel batches b, channels [64 b, 64 b + 64) of the tile, each converted into one slab.
     // Every load of a batch (bias, residual, positional embedding) is issued before the batch's first conversion,
@@ -346,6 +421,9 @@ __global__ void __launch_bounds__(kTileThreads, 1)
     wgmma_wait<0>();
     fence_regs(acc);
     if (prev >= 0) mbar_arrive(&empty[prev]);
+    // Without a residual nothing else tells the threads that the leader saw the previous stores leave the slabs
+    // (with one, batch 0's residual wait does: it arrived after that).
+    if (!p.has_res) asm volatile("bar.sync 1, 256;" ::: "memory");
 
 #pragma unroll
     for (int b = 0; b < NB; ++b) {
@@ -498,20 +576,22 @@ static int ilog2(int v) {
   return l;
 }
 
-template <int BN>
+template <int BN, bool kSwap = false>
 static int launch_bn(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo, const CUtensorMap& mr,
                      const GemmParams& p, cudaStream_t stream) {
-  using Cfg = TileCfg<BN>;
+  using Cfg = TileCfg<BN, kSwap>;
   static std::atomic<unsigned long long> attr_mask{0};  // per device: the attribute is device state
   if (!device_bit_test(attr_mask)) {
-    FP_CUDA_OK(cudaFuncSetAttribute(gemm_tile_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    FP_CUDA_OK(cudaFuncSetAttribute(gemm_tile_kernel<BN, kSwap>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    Cfg::kSmemBytes));
     device_bit_set(attr_mask);
   }
   const int sms = num_sms();
   FP_REQUIRE(sms > 0, "no CUDA device");
   const int grid = p.total_tiles < sms ? p.total_tiles : sms;
   prof_mark_begin(0, p.alg_flops, stream);
-  FP_CUDA_OK(launch_pdl(gemm_tile_kernel<BN>, dim3(grid), dim3(kTileThreads), Cfg::kSmemBytes, stream, 1, ma, mb, mo, mr, p));
+  FP_CUDA_OK(launch_pdl(gemm_tile_kernel<BN, kSwap>, dim3(grid), dim3(kTileThreads), Cfg::kSmemBytes, stream, 1, ma, mb,
+                        mo, mr, p));
   prof_mark_end(stream);
   note_launches(1);
   FP_CUDA_OK(cudaGetLastError());
@@ -520,11 +600,20 @@ static int launch_bn(const CUtensorMap& ma, const CUtensorMap& mb, const CUtenso
 
 int stem_conv_launch(const GemmLayer& L, cudaStream_t stream);  // fp_stem.cu
 
-// Plans the layer and launches it, or, with `tile_n`, only reports the tile width the launch would use.
-static int gemm_layer_plan(const GemmLayer& L, cudaStream_t stream, int* tile_n) {
+// FPOSE_SWAP_TILE=0 keeps the 128-channel convolutions on the 128 x 128 tile.  Read at every plan, so that one process
+// can time and compare both tiles; a captured graph keeps the tiles of its capture.
+static bool swap_tile_enabled() {
+  const char* e = getenv("FPOSE_SWAP_TILE");
+  return !(e && e[0] == '0');
+}
+
+// Plans the layer and launches it, or, with `tile_n` or `tile_m`, only reports the tile the launch would use: its
+// output channels and its output pixels (linear rows).
+static int gemm_layer_plan(const GemmLayer& L, cudaStream_t stream, int* tile_n, int* tile_m) {
   if (L.kind == LK_CONV7_S2) {
-    if (tile_n) {
-      *tile_n = 64;  // the stem kernel's 128-pixel x 64-channel tile
+    if (tile_n || tile_m) {
+      if (tile_n) *tile_n = 64;  // the stem kernel's 128-pixel x 64-channel tile
+      if (tile_m) *tile_m = 128;
       return 0;
     }
     return stem_conv_launch(L, stream);
@@ -618,10 +707,28 @@ static int gemm_layer_plan(const GemmLayer& L, cudaStream_t stream, int* tile_n)
   // SXM at 700 W against the 128-wide tile, the 3x3 convolutions (K = 2304 / 4608) are +7 to +13 % at 9 wide waves,
   // +16 to +24 % at 12 to 24 (252 hypotheses), even at 6 and about 10 % slower at 3 (a 32-hypothesis shard;
   // track_one's single image is under one wave); the K = 512 linear layers (8 k-blocks) were no faster at any height.
+  //
+  // A 3x3 convolution with Cout = 128 cannot take the wide tile; it takes the swapped tile (256 pixels of four 8 x 8
+  // blocks, the weights as the M operand) under the same rule on its 256-pixel grid.  Measured at 504 images (H100 SXM,
+  // 700 W) against the 128 x 128 tile: 128 @ 40 (18 k-blocks) +7 to +10 % without a residual and -2 to +3 % with one;
+  // the stride-2 64 -> 128 layer (9 k-blocks) no faster.
   constexpr int kWideMinWaves = 8;
   constexpr int kWideMinKBlocks = 16;
+  bool swap = false;
+  if (L.Cout == 128 && L.kind != LK_LINEAR && p.bw == 8 && p.num_kb >= kWideMinKBlocks && !L.post_add &&
+      L.out_split % 4 == 0 && swap_tile_enabled()) {
+    const int sms = num_sms();
+    FP_REQUIRE(sms > 0, "no CUDA device");
+    swap = (long long)p.tiles_w * p.tiles_h * ((L.n_img + 3) / 4) >= (long long)kWideMinWaves * sms;
+  }
+  if (swap) {
+    p.bn = 4;
+    box[p.dim_n] = 4;
+    p.tiles_n = (L.n_img + 3) / 4;
+  }
   const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
-  if (L.Cout % 256 == 0 && p.num_kb >= kWideMinKBlocks) {
+  if (swap) BN = 128;
+  else if (L.Cout % 256 == 0 && p.num_kb >= kWideMinKBlocks) {
     const int sms = num_sms();
     FP_REQUIRE(sms > 0, "no CUDA device");
     BN = (long long)m_tiles * (L.Cout / 256) >= (long long)kWideMinWaves * sms ? 256 : 128;
@@ -644,8 +751,9 @@ static int gemm_layer_plan(const GemmLayer& L, cudaStream_t stream, int* tile_n)
   FP_REQUIRE(L.out_split == 0 || L.out_split % p.bn == 0,
              "out_split=%d must be a multiple of the tile's image count %d (pad the A/B batch boundary)", L.out_split,
              p.bn);
-  if (tile_n) {
-    *tile_n = BN;
+  if (tile_n || tile_m) {
+    if (tile_n) *tile_n = BN;
+    if (tile_m) *tile_m = swap ? 256 : 128;
     return 0;
   }
   if (p.total_tiles == 0) return 0;
@@ -678,7 +786,7 @@ static int gemm_layer_plan(const GemmLayer& L, cudaStream_t stream, int* tile_n)
       } else {  // (n, h, w)
         od[1] = (uint64_t)Wo; od[2] = (uint64_t)Ho; od[3] = (uint64_t)nimg;
         os[0] = sw_; os[1] = sh_; os[2] = sn_; os[3] = sn_ * nimg;
-        ob[1] = (uint32_t)p.bw; ob[2] = (uint32_t)p.bh; ob[3] = (uint32_t)p.bn;
+        ob[1] = (uint32_t)p.bw; ob[2] = (uint32_t)p.bh; ob[3] = (uint32_t)(swap ? p.bn / 2 : p.bn);  // 128 pixels
       }
     };
     p.odim_h = lin ? -1 : 2;
@@ -694,12 +802,15 @@ static int gemm_layer_plan(const GemmLayer& L, cudaStream_t stream, int* tile_n)
       mr = mo;
     }
   }
+  if (swap) return launch_bn<128, true>(ma, mb, mo, mr, p, stream);
   if (BN == 256) return launch_bn<256>(ma, mb, mo, mr, p, stream);
   return BN == 128 ? launch_bn<128>(ma, mb, mo, mr, p, stream) : launch_bn<64>(ma, mb, mo, mr, p, stream);
 }
 
-int gemm_layer_launch(const GemmLayer& L, cudaStream_t stream) { return gemm_layer_plan(L, stream, nullptr); }
+int gemm_layer_launch(const GemmLayer& L, cudaStream_t stream) { return gemm_layer_plan(L, stream, nullptr, nullptr); }
 
-int gemm_layer_tile_n(const GemmLayer& L, int* tile_n) { return gemm_layer_plan(L, nullptr, tile_n); }
+int gemm_layer_tile_n(const GemmLayer& L, int* tile_n) { return gemm_layer_plan(L, nullptr, tile_n, nullptr); }
+
+int gemm_layer_tile_m(const GemmLayer& L, int* tile_m) { return gemm_layer_plan(L, nullptr, nullptr, tile_m); }
 
 }  // namespace fp

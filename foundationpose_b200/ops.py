@@ -55,6 +55,16 @@ def gemm_tile_n(kind, *, n_img, Hin, Win, Cin, Cout, out_split=0):
     return tile_n.value
 
 
+def gemm_tile_m(kind, *, n_img, Hin, Win, Cin, Cout, out_split=0):
+    """Output pixels per tile (128, or 256 for the swapped 128-channel tile) that `gemm_layer` picks for this shape."""
+    lib.fp_op_gemm_tile_m.argtypes = [C.POINTER(_lib.GemmLayer), C.POINTER(C.c_int)]
+    lib.fp_op_gemm_tile_m.restype = C.c_int
+    L = _lib.GemmLayer(kind, n_img, Hin, Win, Cin, Cout, None, None, None, None, 0, None, Cout, out_split, None, 0)
+    tile_m = C.c_int(0)
+    _lib.check(lib.fp_op_gemm_tile_m(C.byref(L), C.byref(tile_m)), "fp_op_gemm_tile_m")
+    return tile_m.value
+
+
 lib.fp_op_attention.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
 lib.fp_op_attention.restype = C.c_int
 

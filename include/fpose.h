@@ -73,6 +73,10 @@ int fp_op_gemm_layer(const fp_gemm_layer_t* layer, void* stream);
 /* Output channels per tile (64, 128 or 256) fp_op_gemm_layer would use for `layer`, which depends on the layer's
  * shape and the current device's SM count only.  Launches nothing and dereferences no pointer of the layer. */
 int fp_op_gemm_tile_n(const fp_gemm_layer_t* layer, int* tile_n);
+/* Output pixels (or linear rows) per tile that fp_op_gemm_layer would use for `layer`: 256 where a 128-channel 3x3
+ * convolution runs with the weights as the wgmma M operand (FPOSE_SWAP_TILE=0 turns that tile off), else 128.  Same
+ * rules as fp_op_gemm_tile_n. */
+int fp_op_gemm_tile_m(const fp_gemm_layer_t* layer, int* tile_m);
 
 /* softmax(Q K^T / sqrt(128)) V of nn.MultiheadAttention (refine_network.py:56-70, score_network.py:53):
  * qkv fp16 [B*400][1536] (q | k | v, 4 heads of 128 each), out fp16 [B*400][512].

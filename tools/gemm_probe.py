@@ -89,10 +89,20 @@ def run_case(case):
         ref = F.conv2d(x.float(), w.half().float(), b, stride=2, padding=3).relu().permute(0, 2, 3, 1)
         ok = report(case, out, ref)
     elif case == "perf":
-        # per-layer throughput at the C2 batch (252 hypotheses): CUDA events, 3 warm-up + 10 timed
+        # per-layer throughput at the C2 batch (252 hypotheses): CUDA events, 3 warm-up + 5 windows of 10 timed launches,
+        # the median window reported.  The 128-channel convolutions run both tiles in alternating windows: the 128 x 128
+        # tile (FPOSE_SWAP_TILE=0) and whatever the plan picks by default.
+        name_dev = torch.cuda.get_device_name()
+        try:
+            power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                                    str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout.strip()
+        except (OSError, subprocess.SubprocessError):
+            power = "unknown"
+        print(f"[perf] {name_dev}, power limit {power}")
         shapes = [("conv7 6->64 @160 (504 img)", _lib.LAYER_CONV7_S2, 504, 160, 8, 64, 294),
                   ("conv3s2 64->128 @80 (504)", _lib.LAYER_CONV3_S2, 504, 80, 64, 128, 576),
                   ("conv3 128 @40 (504)", _lib.LAYER_CONV3_S1, 504, 40, 128, 128, 1152),
+                  ("conv3 128 @40 (249+252) +res split", _lib.LAYER_CONV3_S1, 501, 40, 128, 128, 1152),
                   ("conv3 256 @40 (252)", _lib.LAYER_CONV3_S1, 252, 40, 256, 256, 2304),
                   ("conv3 256 @40 (249, odd M tiles)", _lib.LAYER_CONV3_S1, 249, 40, 256, 256, 2304),
                   ("conv3s2 256->512 @40 (252)", _lib.LAYER_CONV3_S2, 252, 40, 256, 512, 2304),
@@ -124,26 +134,49 @@ def run_case(case):
                 M = n * H * H if kind == _lib.LAYER_CONV3_S1 else n * (H // 2) ** 2
             b = torch.zeros(Co, device=dev)
             Ho = 1 if kind == _lib.LAYER_LINEAR else (H if kind == _lib.LAYER_CONV3_S1 else H // 2)
-            out = torch.empty(M * Co, device=dev, dtype=torch.float16)
+            out_ld = Co
+            if "split" in name:  # the last encodeA layer: A images 0..248, B from 252, into the 256-channel concat
+                kw.update(out_split=252)
+                out_ld = 2 * Co
+                out = torch.empty((n - 252) * Ho * Ho * out_ld, device=dev, dtype=torch.float16)
+            else:
+                out = torch.empty(M * Co, device=dev, dtype=torch.float16)
             if use_res:
                 kw.update(res=torch.randn(M * Co, device=dev).half(), res_ld=Co)
             if use_pe:
                 kw.update(post_add=torch.randn(Ho * Ho, Co, device=dev))
-            # tile configuration the layer runs with ("-" for a library that predates the query)
-            tile_n = "-"
-            if getattr(_lib.lib, "fp_op_gemm_tile_n", None) is not None:
-                tile_n = f"128x{ops.gemm_tile_n(kind, n_img=kw['n_img'], Hin=kw['Hin'], Win=kw['Win'], Cin=Ci, Cout=Co)}"
-            for _ in range(3):
-                ops.gemm_layer(kind, x, w, b, out=out, out_ld=Co, relu=True, **kw)
+            q = dict(n_img=kw["n_img"], Hin=kw["Hin"], Win=kw["Win"], Cin=Ci, Cout=Co, out_split=kw.get("out_split", 0))
+            variants = ["1"]
+            if Co == 128 and kind in (_lib.LAYER_CONV3_S1, _lib.LAYER_CONV3_S2):
+                variants = ["0", "1"]
+            times = {v: [] for v in variants}
+            tiles = {}
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(10):
-                ops.gemm_layer(kind, x, w, b, out=out, out_ld=Co, relu=True, **kw)
-            e1.record()
-            torch.cuda.synchronize()
-            ms = e0.elapsed_time(e1) / 10
+            for rep in range(5):
+                for v in variants:
+                    os.environ["FPOSE_SWAP_TILE"] = v
+                    if rep == 0:
+                        # tile configuration the layer runs with ("-" for a library that predates the query)
+                        tile = "-"
+                        if getattr(_lib.lib, "fp_op_gemm_tile_n", None) is not None:
+                            tm = ops.gemm_tile_m(kind, **q) if getattr(_lib.lib, "fp_op_gemm_tile_m", None) else 128
+                            tile = f"{tm}x{ops.gemm_tile_n(kind, **q)}"
+                        tiles[v] = tile
+                        for _ in range(3):
+                            ops.gemm_layer(kind, x, w, b, out=out, out_ld=out_ld, relu=True, **kw)
+                    e0.record()
+                    for _ in range(10):
+                        ops.gemm_layer(kind, x, w, b, out=out, out_ld=out_ld, relu=True, **kw)
+                    e1.record()
+                    torch.cuda.synchronize()
+                    times[v].append(e0.elapsed_time(e1) / 10)
+            os.environ.pop("FPOSE_SWAP_TILE", None)
             fl = 2.0 * M * Co * Kreal
-            print(f"[perf] {name:34s} tile {tile_n:7s} {ms:8.3f} ms  {fl / ms / 1e9:8.1f} TFLOP/s (algorithmic)")
+            for v in variants:
+                ms = sorted(times[v])[len(times[v]) // 2]
+                rates = " ".join(f"{fl / t / 1e9:.0f}" for t in times[v])
+                print(f"[perf] {name:34s} tile {tiles[v]:7s} {ms:8.3f} ms  {fl / ms / 1e9:8.1f} TFLOP/s (algorithmic, "
+                      f"median of 5; windows {rates})")
     print(f"[{case}] {'OK' if ok else 'FAIL'}")
     return ok
 
