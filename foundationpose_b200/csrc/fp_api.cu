@@ -149,11 +149,8 @@ struct fp_ctx {
   fp::DevBuf mesh_table;
   float rot_normalizer = 0.3490658503988659f;
   float crop_ratio[2] = {1.2f, 1.2f};  // per predictor: each reads its own config.yml (predict_pose_refine.py:117, predict_score.py:137)
-  // frames: cam[0] is the context's frame, cameras 1.. those of the multi-camera calls; K / H / W are camera 0's.
-  // depth_a: the eroded depth between the separate filter launches of FPOSE_FUSED_PREP=0
+  // frames: cam[0] is the context's frame, cameras 1.. those of the multi-camera calls; K / H / W are camera 0's
   fp::CameraBufs cam[fp::kMaxCameras];
-  fp::DevBuf depth_a;
-  const float* depth_cur = nullptr;
   float K[9] = {0};
   int H = 0, W = 0;
   bool has_frame = false;
@@ -195,7 +192,7 @@ struct fp_ctx {
   // its pinned staging: the camera table (CameraDev [FP_MAX_CAMERAS]), the slot ids [n], the camera ids [n]
   fp::DevBuf args;
   fp::PinnedBuf stage_args;
-  int cam_grid_h = 0, cam_grid_w = 0;  // fp_track_cameras' frame-preparation grid: the largest frame seen
+  int cam_grid_h = 0, cam_grid_w = 0;  // the tracking calls' frame-preparation grid: the largest frame seen
   // fp_register_objects / _cameras: row offsets of the objects' hypotheses [M + 1] and the objects' camera ids [M], the
   // objects' feature rows [sum N][512], each object's byte offset into mask_buf; pinned staging of the masks and of
   // (offsets, camera ids, mask offsets)
@@ -474,7 +471,8 @@ static int write_mesh_table(fp_ctx* c) {
 }
 
 // mesh_of: [N] device slot ids (validated by the caller), or null = every hypothesis renders slot 0.  cams / camera_of:
-// device camera table and [N] camera ids (the multi-camera calls), or null = the context's frame, by value
+// device camera table and [N] camera ids (the tracking calls, fp_register_cameras), or null = the context's frame
+// (camera 0), by value
 static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg, float* win, int* stats,
                       cudaStream_t st, const int* mesh_of = nullptr, const CameraDev* cams = nullptr,
                       const int* camera_of = nullptr, float4* vis = nullptr) {
@@ -496,7 +494,7 @@ static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg
   p.mesh_of = mesh_of;
   p.rgb = reinterpret_cast<const uchar4*>(c->cam[0].rgba.p);
   p.xyz_map = reinterpret_cast<const float4*>(c->cam[0].xyz.p);
-  p.depth = c->depth_cur;
+  p.depth = reinterpret_cast<const float*>(c->cam[0].depth.p);
   p.mode = mode;
   p.crops = reinterpret_cast<__half*>(c->crops.p);
   p.b_img0 = b_img0_of(N);
@@ -525,11 +523,12 @@ enum class GraphKind {
 // captures + instantiates, later calls replay.  Replay removes ~170 launch + 60 tensor-map-encode host
 // calls per register(), which is what bounds track_one() and small per-GPU shards.  The body never allocates:
 // callers size every workspace first, so a capture after an epoch bump (new mesh, new N) is safe.
-// frame: where the body's kernels take their frame from, the last element of the key.  -1: the context's K / H / W by
-// value; such a graph is captured again when they differ from its capture's, and only that graph: a frame of another
-// size or other intrinsics does not invalidate the others.  0 or more: the camera table (the camera-table kernel
-// instantiations), which holds every camera's size and intrinsics; fp_track_cameras passes its number of cameras C,
-// which its frame-preparation launch covers, the register passes 0 (their frames are prepared before the passes).
+// frame: where the body's kernels take their frame from, the last element of the key.  -1 (the single-object calls,
+// fp_register_objects): the context's K / H / W by value; such a graph is captured again when they differ from its
+// capture's, and only that graph: a frame of another size or other intrinsics does not invalidate the others.  0 or
+// more (the tracking calls, fp_register_cameras): the camera table, which holds every camera's size and intrinsics, so
+// new intrinsics or a smaller frame replay the graph; the tracking calls pass their number of cameras C, which their
+// frame-preparation launch covers, fp_register_cameras' passes 0 (their frames are prepared before the passes).
 template <class Body>
 static int run_graphed(fp_ctx* c, GraphKind kind, int N, int iters, cudaStream_t st, Body body, int frame = -1) {
   if (!c->use_graphs || g_prof_on) return body(st);
@@ -602,15 +601,7 @@ struct DeviceGuard {
   }
 };
 
-// FPOSE_FUSED_PREP=0: the frame filters as four separate launches instead of frame_prep_kernel (A/B)
-static bool fused_prep() {
-  static const bool fused = [] {
-    const char* e = getenv("FPOSE_FUSED_PREP");
-    return !(e && e[0] == '0');
-  }();
-  return fused;
-}
-
+// camera 0's filtered frame from rgb_dev / depth_dev, with the context's K / H / W by value (fp_set_frame, fp_track)
 static int set_frame_launches(fp_ctx* c, const unsigned char* rgb_dev, const float* depth_dev, int flags, float zfar,
                               cudaStream_t st) {
   const int H = c->H, W = c->W;
@@ -619,13 +610,6 @@ static int set_frame_launches(fp_ctx* c, const unsigned char* rgb_dev, const flo
   uchar4* rgba = reinterpret_cast<uchar4*>(f.rgba.p);
   float* depth = reinterpret_cast<float*>(f.depth.p);
   float4* xyz = reinterpret_cast<float4*>(f.xyz.p);
-  c->depth_cur = depth;
-  if ((flags & FP_FRAME_FILTER_DEPTH) && !fused_prep()) {
-    FP_TRY(rgb_to_rgba_launch(rgb_dev, rgba, (int)npix, st));
-    FP_TRY(erode_depth_launch(depth_dev, reinterpret_cast<float*>(c->depth_a.p), H, W, 2, 0.001f, 0.8f, 100.f, st));
-    FP_TRY(bilateral_depth_launch(reinterpret_cast<const float*>(c->depth_a.p), depth, H, W, 2, 100.f, 2.f, 100000.f, st));
-    return depth_to_xyz_launch(depth, xyz, H, W, c->K[0], c->K[4], c->K[2], c->K[5], zfar, st);
-  }
   if (flags & FP_FRAME_FILTER_DEPTH) {
     // estimater.py:173-174 erode_depth(radius=2), bilateral_filter_depth(radius=2); :214 depth2xyzmap: one launch
     return frame_prep_launch(rgb_dev, depth_dev, rgba, depth, xyz, H, W, c->K[0], c->K[4], c->K[2], c->K[5], zfar, st);
@@ -636,16 +620,14 @@ static int set_frame_launches(fp_ctx* c, const unsigned char* rgb_dev, const flo
 }
 
 // Sizes camera i's buffers for npix pixels: the filtered frame always, the raw upload if `raw`, its pinned staging if
-// `staged`.  Camera 0's addresses are held by the graphs that take the frame by value, so growing its buffers (or
-// depth_a, which goes with them) bumps the graph epoch.  Cameras 1.. are reached only through the camera table, which
-// every call rewrites: growing them invalidates no graph.  No graph holds the staging: the uploads leave it ahead of
-// the launch.
+// `staged`.  Camera 0's addresses are held by the graphs that take the frame by value, so growing its buffers bumps the
+// graph epoch.  Cameras 1.. are reached only through the camera table, which every call rewrites: growing them
+// invalidates no graph.  No graph holds the staging: the uploads leave it ahead of the launch.
 static int alloc_camera(fp_ctx* c, int i, size_t npix, bool raw, bool staged) {
   CameraBufs& b = c->cam[i];
   unsigned long long table_only = 0;
   unsigned long long& epoch = i == 0 ? c->epoch : table_only;
   FP_TRY(dev_alloc(epoch, b.rgba, npix * 4));
-  if (i == 0) FP_TRY(dev_alloc(epoch, c->depth_a, npix * 4));
   FP_TRY(dev_alloc(epoch, b.depth, npix * 4));
   FP_TRY(dev_alloc(epoch, b.xyz, npix * 16));
   if (raw) {
@@ -702,17 +684,6 @@ static int upload_staged_frame(CameraBufs& b, const unsigned char* rgb_host, con
   return 0;
 }
 
-// The uploaded frames filtered for tracking and registration (erode + bilateral, depth2xyzmap with zfar = inf).  cams
-// null: camera 0's frame by value (the single-camera kernels; FPOSE_FUSED_PREP applies).  Otherwise cameras 0..C-1 from
-// the device camera table in one launch over a grid_h x grid_w grid.
-static int prepare_frames(fp_ctx* c, const CameraDev* cams, int C, int grid_h, int grid_w, cudaStream_t st) {
-  if (!cams)
-    return set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->cam[0].rgb_raw.p),
-                              reinterpret_cast<const float*>(c->cam[0].depth_raw.p), FP_FRAME_FILTER_DEPTH, INFINITY, st);
-  c->depth_cur = reinterpret_cast<const float*>(c->cam[0].depth.p);
-  return frame_prep_cameras_launch(cams, C, grid_h, grid_w, INFINITY, st);
-}
-
 constexpr size_t kTableBytes = sizeof(CameraDev) * kMaxCameras;  // the camera table at the head of fp_ctx::args
 
 // The cameras of fp_track_cameras / _objects and fp_register_cameras / _objects, before anything reads a frame.  Every
@@ -756,25 +727,20 @@ static int setup_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host,
   return 0;
 }
 
-// fp_track_cameras and fp_track_objects after validation.  The camera table, the slot ids and the camera ids go to the
-// argument block in one copy ahead of the launch.
-//   by_value = false (fp_track_cameras): the graph holds the block's address, not the frames' sizes, intrinsics or
-//     buffers, and is keyed on (C, M, iterations): reordering objects or cameras or new intrinsics replay it.  One
-//     frame_prep_kernel launch filters every camera (FPOSE_FUSED_PREP=0 does not apply) and the crops take their frame
-//     from the table.
-//   by_value = true (fp_track_objects, C = 1): camera 0's frame as fp_track sees it; the frame filters and the crop
-//     producer take it by value (the single-camera kernel instantiations), so the graph is captured again when the
-//     frame's size or intrinsics change.  Its kernels read only the slot ids of the block.
+// fp_track_cameras and fp_track_objects (C = 1) after validation.  The camera table, the slot ids and the camera ids go
+// to the argument block in one copy ahead of the launch.  The graph holds the block's address, not the frames' sizes,
+// intrinsics or buffers, and is keyed on (M, iterations, C): reordering objects or cameras, new intrinsics or a smaller
+// frame replay it.  One frame_prep_kernel launch filters every camera and the crops take their frame from the table.
 static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
                               const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
                               const float* poses_in_dev, int iterations, float* poses_out_dev, float* poses_out_host,
-                              cudaStream_t st, bool by_value) {
+                              cudaStream_t st) {
   FP_TRY(ensure_capacity(c, M));
   FP_TRY(pinned_alloc(&c->epoch, c->stage_poses, (size_t)M * 64));  // the graph's read-back node holds this address
   c->has_frame = false;
   int H_max, W_max;
   FP_TRY(setup_cameras(c, C, rgb_host, depth_host, K, H, W, M, M, st, H_max, W_max));
-  if (!by_value && (H_max > c->cam_grid_h || W_max > c->cam_grid_w)) {
+  if (H_max > c->cam_grid_h || W_max > c->cam_grid_w) {
     // the frame-preparation grid is a by-value launch parameter: it covers the largest frame seen, the blocks outside
     // a smaller frame return at once
     ++c->epoch;
@@ -786,24 +752,25 @@ static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_
   memcpy(ids + M, camera_of, (size_t)M * sizeof(int));
   FP_CUDA_OK(cudaMemcpyAsync(c->args.p, c->stage_args.p, kTableBytes + (size_t)2 * M * sizeof(int), cudaMemcpyHostToDevice,
                              st));
-  const CameraDev* cams_dev = by_value ? nullptr : reinterpret_cast<const CameraDev*>(c->args.p);
+  const CameraDev* cams_dev = reinterpret_cast<const CameraDev*>(c->args.p);
   const int* mesh_of = reinterpret_cast<const int*>(static_cast<const char*>(c->args.p) + kTableBytes);
-  const int* cam_of = by_value ? nullptr : mesh_of + M;
+  const int* cam_of = mesh_of + M;
   float* pa = reinterpret_cast<float*>(c->poses_a.p);
   float* pb = reinterpret_cast<float*>(c->poses_b.p);
   FP_CUDA_OK(cudaMemcpyAsync(pa, poses_in_dev, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
   const float* fin = (iterations % 2 == 0) ? pa : pb;
   const int grid_h = c->cam_grid_h, grid_w = c->cam_grid_w;
   auto body = [&](cudaStream_t s2) -> int {
-    // estimater.py:250-268 for every object of every camera at once: each camera's frame filtered once, M hypotheses
-    // each rendering its own mesh and cropping its own camera's frame
-    FP_TRY(prepare_frames(c, cams_dev, C, grid_h, grid_w, s2));
+    // estimater.py:250-268 for every object of every camera at once: each camera's frame filtered once (erode +
+    // bilateral, depth2xyzmap_batch(zfar = inf)), M hypotheses each rendering its own mesh and cropping its own
+    // camera's frame
+    FP_TRY(frame_prep_cameras_launch(cams_dev, C, grid_h, grid_w, INFINITY, s2));
     c->has_frame = true;
     FP_TRY(refine_body(c, M, iterations, s2, mesh_of, cams_dev, cam_of));
     FP_CUDA_OK(cudaMemcpyAsync(c->stage_poses.p, fin, (size_t)M * 64, cudaMemcpyDeviceToHost, s2));
     return 0;
   };
-  FP_TRY(run_graphed(c, GraphKind::TrackObjects, M, iterations, st, body, by_value ? -1 : C));
+  FP_TRY(run_graphed(c, GraphKind::TrackObjects, M, iterations, st, body, C));
   c->has_frame = true;
   if (poses_out_dev) FP_CUDA_OK(cudaMemcpyAsync(poses_out_dev, fin, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
   FP_CUDA_OK(cudaStreamSynchronize(st));
@@ -866,8 +833,11 @@ static ScoreTailParams score_tail_params(const fp_ctx* c, const float* feats, in
 //     frame_prep_kernel launch filters every camera, the start-pose kernels read each object's depth, size and
 //     intrinsics from the table, and the crops take their frame from it: the graphs hold no frame, so reordering
 //     cameras or objects or changing intrinsics replays them.
-//   by_value = true (fp_register_objects, C = 1): the frame filters, the start-pose kernels and the crop producer take
-//     camera 0's frame by value (the single-camera kernel instantiations), as fp_register does.
+//   by_value = true (fp_register_objects, C = 1): the frame filter, the start-pose kernels and the crop producer take
+//     camera 0's frame by value (the single-camera kernel instantiations), as fp_register does.  Kept for speed: at
+//     252 hypotheses the crop producer's camera-table instantiation runs 3.6 % longer (2.76 against 2.67 ms of crops
+//     per one-object call, H100 80GB HBM3 at 700 W), the one camera-table kernel whose cost shows.  Tracking's few
+//     hypotheses show none, so fp_track_objects shares fp_track_cameras' table path.
 // Both: whole objects in the given order in passes of up to kRegisterPassCap hypotheses (an object above the cap alone),
 // then one segmented scorer tail over all objects.  Synchronises.
 static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
@@ -931,12 +901,15 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
   FP_CUDA_OK(cudaMemcpyAsync(c->seg_off.p, ints, (size_t)(2 * M + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
   FP_CUDA_OK(cudaMemcpyAsync(c->mask_buf.p, c->stage_masks.p, mask_bytes, cudaMemcpyHostToDevice, st));
   const CameraDev* cams_dev = by_value ? nullptr : reinterpret_cast<const CameraDev*>(c->args.p);
-  if (cams_dev) {
+  // estimater.py:173-174, :214 once per camera for every object: erode + bilateral, depth2xyzmap(zfar = inf)
+  if (by_value) {
+    FP_TRY(set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->cam[0].rgb_raw.p),
+                              reinterpret_cast<const float*>(c->cam[0].depth_raw.p), FP_FRAME_FILTER_DEPTH, INFINITY, st));
+  } else {
     FP_CUDA_OK(cudaMemcpyAsync(c->args.p, c->stage_args.p, kTableBytes, cudaMemcpyHostToDevice, st));
     FP_CUDA_OK(cudaMemcpyAsync(c->mask_off.p, stage_mask_off, (size_t)M * sizeof(size_t), cudaMemcpyHostToDevice, st));
+    FP_TRY(frame_prep_cameras_launch(cams_dev, C, H_max, W_max, INFINITY, st));
   }
-  // estimater.py:173-174, :214 once per camera for every object: erode + bilateral, depth2xyzmap(zfar = inf)
-  FP_TRY(prepare_frames(c, cams_dev, C, H_max, W_max, st));
   c->has_frame = true;
   // estimater.py:137-156, :203-209 for every object in one launch pair; the start poses go to poses_out_dev and are
   // replaced pass by pass with the refined ones
@@ -944,8 +917,8 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
   const unsigned char* masks_dev = reinterpret_cast<const unsigned char*>(c->mask_buf.p);
   unsigned int* stats = reinterpret_cast<unsigned int*>(c->mask_stats.p);
   if (by_value) {
-    FP_TRY(start_poses_launch(c->depth_cur, masks_dev, H[0], W[0], c->K[0], c->K[4], c->K[2], c->K[5], rot_grids_dev, total, M,
-                              seg, stats, poses_out_dev, info_out_dev, st));
+    FP_TRY(start_poses_launch(reinterpret_cast<const float*>(c->cam[0].depth.p), masks_dev, H[0], W[0], c->K[0], c->K[4],
+                              c->K[2], c->K[5], rot_grids_dev, total, M, seg, stats, poses_out_dev, info_out_dev, st));
   } else {
     FP_TRY(start_poses_cameras_launch(cams_dev, seg + M + 1, masks_dev, reinterpret_cast<const size_t*>(c->mask_off.p),
                                       rot_grids_dev, M, seg, stats, poses_out_dev, info_out_dev, st));
@@ -1274,7 +1247,7 @@ int fp_get_depth(fp_ctx* c, float* depth_out_dev, float* xyz_out_dev, void* stre
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const size_t npix = (size_t)c->H * c->W;
-  if (depth_out_dev) FP_CUDA_OK(cudaMemcpyAsync(depth_out_dev, c->depth_cur, npix * 4, cudaMemcpyDeviceToDevice, st));
+  if (depth_out_dev) FP_CUDA_OK(cudaMemcpyAsync(depth_out_dev, c->cam[0].depth.p, npix * 4, cudaMemcpyDeviceToDevice, st));
   // internal layout is float4 per pixel; the hook returns the reference's [H][W][3]
   if (xyz_out_dev)
     FP_CUDA_OK(cudaMemcpy2DAsync(xyz_out_dev, 12, c->cam[0].xyz.p, 16, 12, npix, cudaMemcpyDeviceToDevice, st));
@@ -1297,8 +1270,9 @@ int fp_start_poses(fp_ctx* c, const unsigned char* mask, int mask_on_device, con
     mdev = reinterpret_cast<const unsigned char*>(c->mask_buf.p);
   }
   FP_TRY(dev_alloc(c->epoch, c->mask_stats, 64));
-  return start_poses_launch(c->depth_cur, mdev, c->H, c->W, c->K[0], c->K[4], c->K[2], c->K[5], rot_grid, N, 1, nullptr,
-                            reinterpret_cast<unsigned int*>(c->mask_stats.p), poses_out, info_out, st);
+  return start_poses_launch(reinterpret_cast<const float*>(c->cam[0].depth.p), mdev, c->H, c->W, c->K[0], c->K[4], c->K[2],
+                            c->K[5], rot_grid, N, 1, nullptr, reinterpret_cast<unsigned int*>(c->mask_stats.p), poses_out,
+                            info_out, st);
   FP_API_END
 }
 
@@ -1503,7 +1477,8 @@ int fp_track(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, 
   float* pb = reinterpret_cast<float*>(c->poses_b.p);
   auto body = [&](cudaStream_t s2) -> int {
     // estimater.py:250-268 in one launch sequence: erode + bilateral, depth2xyzmap_batch(zfar=inf), K refiner passes
-    FP_TRY(prepare_frames(c, nullptr, 1, 0, 0, s2));
+    FP_TRY(set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->cam[0].rgb_raw.p),
+                              reinterpret_cast<const float*>(c->cam[0].depth_raw.p), FP_FRAME_FILTER_DEPTH, INFINITY, s2));
     FP_CUDA_OK(cudaMemcpyAsync(pa, c->track_pose.p, 64, cudaMemcpyDeviceToDevice, s2));
     c->has_frame = true;
     FP_TRY(refine_body(c, 1, iterations, s2));
@@ -1600,7 +1575,7 @@ int fp_track_objects(fp_ctx* c, const unsigned char* rgb_host, const float* dept
   DeviceGuard dg(c->device);
   const std::vector<int> camera_of(M, 0);
   return track_cameras_body(c, 1, &rgb_host, &depth_host, K, &H, &W, M, camera_of.data(), slots_host, poses_in_dev, iterations,
-                            poses_out_dev, poses_out_host, reinterpret_cast<cudaStream_t>(stream), /*by_value=*/true);
+                            poses_out_dev, poses_out_host, reinterpret_cast<cudaStream_t>(stream));
   FP_API_END
 }
 
@@ -1616,7 +1591,7 @@ int fp_track_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host, con
   FP_TRY(check_slots(c, M, slots_host, "fp_track_cameras"));
   DeviceGuard dg(c->device);
   return track_cameras_body(c, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, poses_in_dev, iterations,
-                            poses_out_dev, poses_out_host, reinterpret_cast<cudaStream_t>(stream), /*by_value=*/false);
+                            poses_out_dev, poses_out_host, reinterpret_cast<cudaStream_t>(stream));
   FP_API_END
 }
 

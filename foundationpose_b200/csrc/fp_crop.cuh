@@ -54,8 +54,8 @@ struct __align__(16) MeshSlotDev {
 
 constexpr int kMaxCameras = 16;  // FP_MAX_CAMERAS (include/fpose.h)
 
-// One entry of the camera table of fp_track_cameras: one camera stream's frame buffers (device), size and intrinsics.
-// frame_prep_kernel reads the raw frame and writes the filtered one; the crop producer reads the filtered one.
+// One entry of the camera table of the tracking calls and fp_register_cameras: one camera stream's frame buffers
+// (device), size and intrinsics.  frame_prep_kernel reads the raw frame and writes the filtered one; the crop producer reads the filtered one.
 struct __align__(16) CameraDev {
   const unsigned char* rgb_raw;  // [H][W][3] uploaded frame
   const float* depth_raw;        // [H][W]
@@ -89,7 +89,8 @@ struct CropParams {
   int tile_override;  // 0 = pick by batch size; 16 / 32 / 80 = force (fp_set_crop_tile, A/B tests)
   int* stats;      // optional [4]: meshlet visits, triangles set up, fragments, mixed (near-plane) triangles
   // optional, device: hypothesis n takes its frame (rgba, xyz, filtered depth, fx fy cx cy, H W) from
-  // cams[camera_of[n]] instead of the by-value frame fields above (fp_track_cameras); both null or both set
+  // cams[camera_of[n]] instead of the by-value frame fields above (the tracking calls, fp_register_cameras); both null
+  // or both set
   const CameraDev* cams;
   const int* camera_of;
   // optional, single-camera (fp_vis): [N][2][160][160] fp32 record of every crop pixel, A then B: the r, g, b the

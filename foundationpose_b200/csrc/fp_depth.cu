@@ -105,7 +105,7 @@ __global__ void bilateral_depth_kernel(const float* __restrict__ depth, float* _
 // a second shared tile (halo pixels are recomputed by the neighbouring blocks, identically) and filters from there:
 // one read of the depth image instead of ~50 per pixel from L1 / L2, three launches fewer per frame (47 -> ~12 us of
 // a 0.97 ms tracked frame).  Same per-pixel code as the stand-alone kernels above: bit-identical.
-// kTable: one launch for several cameras (fp_track_cameras).  blockIdx.z selects the camera's entry of the device table
+// kTable: one launch for several cameras (fp_track_objects / _cameras, fp_register_cameras).  blockIdx.z selects the camera's entry of the device table
 // `cams`; the grid covers the largest frame and the blocks outside a smaller one leave at once.  Otherwise the one frame
 // is `one`, passed by value.
 constexpr int kFpW = 32, kFpH = 8, kFpR = 2;

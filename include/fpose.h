@@ -234,15 +234,15 @@ int fp_track(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host
  * `iterations` refiner passes over a batch of M hypotheses where hypothesis i renders the mesh in slot slots_host[i],
  * read-back of the M poses.  slots_host: HOST [M] slot ids, each loaded (checked before anything is enqueued);
  * poses_in_dev: DEVICE [M][16] ob_in_cam of each centred mesh; poses_out_dev (DEVICE [M][16]) / poses_out_host
- * (HOST [M][16]) are optional.  Each pose equals what fp_track gives for that object alone.  The slot ids and poses
- * are copied into the context first, so the cached graph depends on (M, iterations) only.  Leaves fp_track's
- * continuation pose untouched.  Synchronises. */
+ * (HOST [M][16]) are optional.  Each pose equals what fp_track gives for that object alone.  This is fp_track_cameras
+ * with one camera (C = 1, every object seen by camera 0), and shares its cached graph: new intrinsics or a frame no
+ * larger than one seen before replay it.  Leaves fp_track's continuation pose untouched.  Synchronises. */
 int fp_track_objects(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
                      int M, const int* slots_host, const float* poses_in_dev, int iterations, float* poses_out_dev,
                      float* poses_out_host, void* stream);
 /* fp_track_objects for M objects spread over C camera streams (1 <= C <= FP_MAX_CAMERAS), each camera with its own
  * frame size and intrinsics, as ONE CUDA-graph launch: object i is seen by camera camera_of[i] and tracked exactly as
- * fp_track_objects tracks it in that camera's frame alone, bit for bit.
+ * fp_track_objects tracks it in that camera's frame alone, bit for bit; fp_track_objects is its one-camera case.
  *   rgb_host[c] / depth_host[c]: HOST uint8 [H[c]][W[c]][3] / float32 [H[c]][W[c]] frame of camera c, each uploaded
  *   through its own pinned staging; K: [C][9] row-major intrinsics; camera_of, slots_host: HOST [M] camera and mesh
  *   slot of every object; poses_in_dev: DEVICE [M][16]; poses_out_dev (DEVICE [M][16]) / poses_out_host (HOST [M][16])
@@ -251,9 +251,10 @@ int fp_track_objects(fp_ctx* ctx, const unsigned char* rgb_host, const float* de
  * object, every slot loaded, non-null frames of positive size.  One frame-preparation launch filters every camera's
  * depth, then `iterations` refiner passes run over all M objects.  The camera table (buffers, sizes, intrinsics), the
  * slot ids and the camera ids are copied into the context first, so the cached graph depends on (C, M, iterations)
- * only: reordering objects or cameras or changing intrinsics replays it.  Camera 0 is the context's frame: afterwards
- * the context holds camera 0's frame as fp_track_objects leaves it.  Cameras 1.. get buffers of their own, kept at the
- * largest frame size seen.  Leaves fp_track's continuation pose untouched.  Synchronises. */
+ * only: reordering objects or cameras, changing intrinsics or a frame no larger than one seen before replays it.
+ * Camera 0 is the context's frame: afterwards the context holds camera 0's filtered frame, as fp_track on that frame
+ * leaves it.  Cameras 1.. get buffers of their own, kept at the largest frame size seen.  Leaves fp_track's
+ * continuation pose untouched.  Synchronises. */
 #define FP_MAX_CAMERAS 16
 int fp_track_cameras(fp_ctx* ctx, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
                      const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
@@ -273,7 +274,9 @@ int fp_track_cameras(fp_ctx* ctx, int C, const unsigned char* const* rgb_host, c
  * Outputs (DEVICE): poses_out_dev [sum N][16] refined poses, object-major, in grid order (not ranked; with iterations = 0
  * the start poses); scores_out_dev [sum N]; best_out_dev [M] first index of each object's maximum, relative to the
  * object; info_out_dev [M][4] = {tx, ty, tz, n_valid} as fp_start_poses.  An object with fewer than 4 valid masked
- * pixels still runs; the caller discards its results (estimater.py:183-189).  Synchronises. */
+ * pixels still runs; the caller discards its results (estimater.py:183-189).  The frame filter, the start poses and
+ * the crops take the frame by value, as fp_register does, so the cached graphs are captured again when the frame's
+ * size or intrinsics change.  Synchronises. */
 int fp_register_objects(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
                         int M, const int* slots_host, const int* n_hyp_host, const unsigned char* masks_host,
                         const float* rot_grids_dev, int iterations, float* poses_out_dev, float* scores_out_dev,

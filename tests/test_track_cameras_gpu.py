@@ -94,7 +94,7 @@ def _pairs(cams, order=None):
 
 
 def _alone(e, cam):
-    """fp_track_objects of one camera's objects (the frame and intrinsics passed by value, as fp_track takes them)."""
+    """fp_track_objects of one camera's objects (fp_track_cameras' one-camera case, with that camera as camera 0)."""
     _, host = e.track_objects(cam["rgb"], cam["depth"], cam["K"], torch.from_numpy(cam["start"]).cuda(),
                               [k + 1 for k in cam["seen"]], 2)
     return host

@@ -128,6 +128,24 @@ def test_object_order_and_slot_reuse(rig):
     _, permuted = e.track_objects(rig["rgb"], rig["depth"], K, start[perm], [p + 1 for p in perm], 2)
     assert np.array_equal(permuted, base[perm])
     assert e.graph_captures() == captures, "a different order of the same objects captured a new graph"
+    # other intrinsics, then also a smaller frame whose right edge cuts through object 2 (at u ~ 290 px): the graph reads
+    # the frame from the camera table and replays, each result differs from the one before (the new intrinsics and the
+    # new size are read) and is the same as a fresh context's
+    K2 = K.copy()
+    K2[0, 2] += 3.0
+    K2[1, 1] *= 1.01
+    before = base
+    for rgb, depth in ((rig["rgb"], rig["depth"]), (rig["rgb"][:400, :300], rig["depth"][:400, :300])):
+        _, got = e.track_objects(rgb, depth, K2, start, [1, 2, 3], 2)
+        assert e.graph_captures() == captures, f"a {depth.shape} frame with other intrinsics captured a new graph"
+        assert not np.array_equal(got, before), f"a {depth.shape} frame with other intrinsics changed no pose"
+        fresh = _engine()
+        for k in range(3):
+            _load(fresh, rig["objs"][k][0], k + 1)
+        _, want = fresh.track_objects(rgb, depth, K2, start, [1, 2, 3], 2)
+        fresh.close()
+        assert np.array_equal(got, want), f"{depth.shape} frame: off a fresh context by {np.abs(got - want).max():.2e}"
+        before = got
     # reload slot 2 with object 3's mesh between replays: same as a fresh context holding that set of meshes
     _load(e, rig["objs"][3][0], 2)
     _, swapped = e.track_objects(rig["rgb"], rig["depth"], K, start, [1, 2, 3], 2)
