@@ -318,22 +318,8 @@ static int run_refine_heads(fp_ctx* c, const Net& net, int N, cudaStream_t st) {
   const int M = N * T;
   // both heads' in_proj as one GEMM: [M,512] x [3072,512]^T
   FP_TRY(gemm_layer_launch(mk(LK_LINEAR, 1, 1, M, 512, 3072, c->tok.p, net.h("heads.in_w"), net.f("heads.in_b"), c->qkv.p, 0), st));
-  AttnParams ap;
-  ap.qkv = reinterpret_cast<const __half*>(c->qkv.p);
-  ap.ld = 3072;
-  ap.q_off = 0;
-  ap.k_off = 512;
-  ap.v_off = 1024;
-  ap.group_col_stride = 1536;
-  ap.n_groups = 2;
-  ap.out = reinterpret_cast<__half*>(c->att.p);
-  ap.ld_out = 512;
-  ap.out_group_stride = (size_t)M * 512;
-  ap.B = N;
-  ap.T = T;
-  ap.n_heads = 4;
-  ap.scale = 0.08838834764831845f;
-  FP_TRY(attn_core_launch(ap, st));
+  FP_TRY(attn_core_launch(
+      head_attn_params(reinterpret_cast<const __half*>(c->qkv.p), 3072, 2, reinterpret_cast<__half*>(c->att.p), N), st));
   const bool fork = N <= c->fork_max_n;
   if (fork) {
     if (!c->side_stream) {
@@ -386,22 +372,8 @@ static int run_refine_heads(fp_ctx* c, const Net& net, int N, cudaStream_t st) {
 static int run_score_feats(fp_ctx* c, const Net& net, int N, float* feats, cudaStream_t st) {
   const int M = N * T;
   FP_TRY(gemm_layer_launch(mk(LK_LINEAR, 1, 1, M, 512, 1536, c->tok.p, net.h("att.in_w"), net.f("att.in_b"), c->qkv.p, 0), st));
-  AttnParams ap;
-  ap.qkv = reinterpret_cast<const __half*>(c->qkv.p);
-  ap.ld = 1536;
-  ap.q_off = 0;
-  ap.k_off = 512;
-  ap.v_off = 1024;
-  ap.group_col_stride = 0;
-  ap.n_groups = 1;
-  ap.out = reinterpret_cast<__half*>(c->att.p);
-  ap.ld_out = 512;
-  ap.out_group_stride = 0;
-  ap.B = N;
-  ap.T = T;
-  ap.n_heads = 4;
-  ap.scale = 0.08838834764831845f;
-  FP_TRY(attn_core_launch(ap, st));
+  FP_TRY(attn_core_launch(
+      head_attn_params(reinterpret_cast<const __half*>(c->qkv.p), 1536, 1, reinterpret_cast<__half*>(c->att.p), N), st));
   FP_TRY(token_mean_proj_launch(reinterpret_cast<const __half*>(c->att.p), net.f("att.out_w32"), net.f("att.out_b"),
                                 reinterpret_cast<float*>(c->tok_mean.p), feats, N, T, st));
   return 0;

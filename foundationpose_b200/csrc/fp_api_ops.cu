@@ -122,24 +122,61 @@ int fp_op_attention(const void* qkv, void* out, int B, int impl, void* stream) {
     fp::set_last_error("fp_op_attention: null argument");
     return -1;
   }
-  fp::AttnParams ap;
-  ap.qkv = reinterpret_cast<const __half*>(qkv);
-  ap.ld = 1536;
-  ap.q_off = 0;
-  ap.k_off = 512;
-  ap.v_off = 1024;
-  ap.group_col_stride = 0;
-  ap.n_groups = 1;
-  ap.out = reinterpret_cast<__half*>(out);
-  ap.ld_out = 512;
-  ap.out_group_stride = 0;
-  ap.B = B;
-  ap.T = 400;
-  ap.n_heads = 4;
-  ap.scale = 0.08838834764831845f;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   (void)impl;  // one implementation: the wgmma kernel
-  return fp::attn_tc_launch(ap, st);
+  return fp::attn_tc_launch(
+      fp::head_attn_params(reinterpret_cast<const __half*>(qkv), 1536, 1, reinterpret_cast<__half*>(out), B),
+      reinterpret_cast<cudaStream_t>(stream));
+}
+
+// 0 when `p` is device memory of the current device aligned to the 16 bytes of the kernels' uint4 / float4 loads
+static int check_dev16(const void* p, const char* what, const char* fn) {
+  FP_REQUIRE(p, "%s: %s is null", fn, what);
+  FP_REQUIRE(reinterpret_cast<uintptr_t>(p) % 16 == 0, "%s: %s is not 16-byte aligned", fn, what);
+  return check_device_ptr(p, what, fn);
+}
+
+int fp_op_attention_groups(const void* qkv, int ld, int n_groups, void* out, int B, void* stream) {
+  const char* fn = "fp_op_attention_groups";
+  FP_REQUIRE(n_groups == 1 || n_groups == 2, "%s: n_groups = %d, must be 1 or 2", fn, n_groups);
+  FP_REQUIRE(ld >= 1536 * n_groups && ld % 8 == 0, "%s: ld = %d, must be a multiple of 8 and >= %d", fn, ld, 1536 * n_groups);
+  FP_REQUIRE(B >= 0 && B <= FP_OP_MAX_SEQUENCES, "%s: B = %d outside [0, %d]", fn, B, FP_OP_MAX_SEQUENCES);
+  if (check_dev16(qkv, "qkv", fn) || check_dev16(out, "out", fn)) return -1;
+  return fp::attn_core_launch(
+      fp::head_attn_params(reinterpret_cast<const __half*>(qkv), ld, n_groups, reinterpret_cast<__half*>(out), B),
+      reinterpret_cast<cudaStream_t>(stream));
+}
+
+int fp_op_layernorm(const void* x, void* y, const float* gamma, const float* beta, int rows, void* stream) {
+  const char* fn = "fp_op_layernorm";
+  FP_REQUIRE(rows >= 0 && rows <= FP_OP_MAX_SEQUENCES * 400, "%s: rows = %d outside [0, %d]", fn, rows,
+             FP_OP_MAX_SEQUENCES * 400);
+  if (check_dev16(x, "x", fn) || check_dev16(y, "y", fn) || check_dev16(gamma, "gamma", fn) || check_dev16(beta, "beta", fn))
+    return -1;
+  return fp::layernorm_launch(reinterpret_cast<const __half*>(x), reinterpret_cast<__half*>(y), gamma, beta, rows,
+                              reinterpret_cast<cudaStream_t>(stream));
+}
+
+int fp_op_head_final(const void* x, const float* gamma, const float* beta, const float* w, const float* bias, float* out,
+                     int B, int out_dim, void* stream) {
+  const char* fn = "fp_op_head_final";
+  FP_REQUIRE(B >= 0 && B <= FP_OP_MAX_SEQUENCES, "%s: B = %d outside [0, %d]", fn, B, FP_OP_MAX_SEQUENCES);
+  FP_REQUIRE(out_dim >= 1 && out_dim <= 8, "%s: out_dim = %d outside [1, 8]", fn, out_dim);
+  if (check_dev16(x, "x", fn) || check_dev16(gamma, "gamma", fn) || check_dev16(beta, "beta", fn)) return -1;
+  FP_REQUIRE(w && bias && out, "%s: null w, bias or out", fn);
+  if (check_device_ptr(w, "w", fn) || check_device_ptr(bias, "bias", fn) || check_device_ptr(out, "out", fn)) return -1;
+  return fp::head_final_launch(reinterpret_cast<const __half*>(x), gamma, beta, w, bias, out, B, 400, out_dim,
+                               reinterpret_cast<cudaStream_t>(stream));
+}
+
+int fp_op_token_mean_proj(const void* x, const float* w_f32, const float* bias, float* mean_ws, float* out, int B,
+                          void* stream) {
+  const char* fn = "fp_op_token_mean_proj";
+  FP_REQUIRE(B >= 0 && B <= FP_OP_MAX_SEQUENCES, "%s: B = %d outside [0, %d]", fn, B, FP_OP_MAX_SEQUENCES);
+  if (check_dev16(x, "x", fn) || check_dev16(w_f32, "w_f32", fn) || check_dev16(mean_ws, "mean_ws", fn)) return -1;
+  FP_REQUIRE(bias && out, "%s: null bias or out", fn);
+  if (check_device_ptr(bias, "bias", fn) || check_device_ptr(out, "out", fn)) return -1;
+  return fp::token_mean_proj_launch(reinterpret_cast<const __half*>(x), w_f32, bias, mean_ws, out, B, 400,
+                                    reinterpret_cast<cudaStream_t>(stream));
 }
 
 static fp::GemmLayer to_gemm_layer(const fp_gemm_layer_t* l) {

@@ -18,6 +18,27 @@ struct AttnParams {
   int B, T, n_heads;
   float scale;  // 1/sqrt(head_dim)
 };
+// The heads' attention layout: T = 400 tokens, 4 heads of 128, q / k / v at columns 0 / 512 / 1024 of each group's
+// 1536-column block.  Group g reads columns [1536 g, 1536 g + 1536) of rows of `ld` columns and writes
+// out + g * B * 400 * 512.  Refiner: ld 3072, two groups (trans / rot head); scorer: ld 1536, one group.
+inline AttnParams head_attn_params(const __half* qkv, int ld, int n_groups, __half* out, int B) {
+  AttnParams ap;
+  ap.qkv = qkv;
+  ap.ld = ld;
+  ap.q_off = 0;
+  ap.k_off = 512;
+  ap.v_off = 1024;
+  ap.group_col_stride = 1536;
+  ap.n_groups = n_groups;
+  ap.out = out;
+  ap.ld_out = 512;
+  ap.out_group_stride = (size_t)B * 400 * 512;
+  ap.B = B;
+  ap.T = 400;
+  ap.n_heads = 4;
+  ap.scale = 0.08838834764831845f;
+  return ap;
+}
 // the wgmma kernel (fp_attn_tc.cu)
 int attn_core_launch(const AttnParams& p, cudaStream_t stream);
 int attn_tc_launch(const AttnParams& p, cudaStream_t stream);

@@ -77,3 +77,60 @@ def attention(qkv, impl=1):
     out = torch.empty(qkv.shape[0], 512, dtype=torch.float16, device=qkv.device)
     _lib.check(lib.fp_op_attention(_ptr(qkv), _ptr(out), B, impl, _stream()), "fp_op_attention")
     return out
+
+
+lib.fp_op_attention_groups.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
+lib.fp_op_attention_groups.restype = C.c_int
+lib.fp_op_layernorm.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+lib.fp_op_layernorm.restype = C.c_int
+lib.fp_op_head_final.argtypes = [C.c_void_p] * 6 + [C.c_int, C.c_int, C.c_void_p]
+lib.fp_op_head_final.restype = C.c_int
+lib.fp_op_token_mean_proj.argtypes = [C.c_void_p] * 5 + [C.c_int, C.c_void_p]
+lib.fp_op_token_mean_proj.restype = C.c_int
+
+
+def attention_groups(qkv, B, n_groups, *, ld=None):
+    """Attention of the heads' launch: `qkv` fp16 rows of `ld` elements (default: the tensor's row stride), B * 400 of
+    them from qkv's first element, group g's q | k | v at columns [1536 g, 1536 g + 1536) -> fp16 [n_groups, B*400, 512].
+    `qkv` may be a column slice of a wider tensor (pass ld)."""
+    _require_cuda(qkv)
+    assert qkv.dtype == torch.float16 and qkv.stride(-1) == 1
+    ld = qkv.stride(0) if ld is None else ld
+    out = torch.empty(n_groups, B * 400, 512, dtype=torch.float16, device=qkv.device)
+    _lib.check(lib.fp_op_attention_groups(_ptr(qkv), ld, n_groups, _ptr(out), B, _stream()), "fp_op_attention_groups")
+    return out
+
+
+def layernorm(x, gamma, beta):
+    """fp16 [rows, 512] -> fp16 [rows, 512]: LayerNorm with fp32 gamma / beta, eps 1e-5."""
+    _require_cuda(x, gamma, beta)
+    assert x.dtype == torch.float16 and x.is_contiguous() and x.shape[-1] == 512
+    assert gamma.dtype == torch.float32 and beta.dtype == torch.float32
+    y = torch.empty_like(x)
+    rows = x.numel() // 512
+    _lib.check(lib.fp_op_layernorm(_ptr(x), _ptr(y), _ptr(gamma), _ptr(beta), rows, _stream()), "fp_op_layernorm")
+    return y
+
+
+def head_final(x, gamma, beta, w, bias):
+    """Refiner read-out: fp16 [B, 400, 512] -> fp32 [B, out_dim] = w . mean over tokens of LayerNorm(x) + bias."""
+    _require_cuda(x, gamma, beta, w, bias)
+    assert x.dtype == torch.float16 and x.is_contiguous() and x.shape[1:] == (400, 512)
+    B, out_dim = x.shape[0], w.shape[0]
+    out = torch.empty(B, out_dim, dtype=torch.float32, device=x.device)
+    _lib.check(lib.fp_op_head_final(_ptr(x), _ptr(gamma), _ptr(beta), _ptr(w.contiguous()), _ptr(bias), _ptr(out), B, out_dim,
+                                    _stream()), "fp_op_head_final")
+    return out
+
+
+def token_mean_proj(x, w, bias):
+    """Scorer features: fp16 [B, 400, 512] -> fp32 [B, 512] = w (mean over tokens of x) + bias, w fp32 [512, 512]."""
+    _require_cuda(x, w, bias)
+    assert x.dtype == torch.float16 and x.is_contiguous() and x.shape[1:] == (400, 512)
+    assert w.dtype == torch.float32 and w.is_contiguous() and w.shape == (512, 512)
+    B = x.shape[0]
+    mean_ws = torch.empty(B, 512, dtype=torch.float32, device=x.device)
+    out = torch.empty(B, 512, dtype=torch.float32, device=x.device)
+    _lib.check(lib.fp_op_token_mean_proj(_ptr(x), _ptr(w), _ptr(bias), _ptr(mean_ws), _ptr(out), B, _stream()),
+               "fp_op_token_mean_proj")
+    return out

@@ -83,6 +83,24 @@ int fp_op_gemm_tile_m(const fp_gemm_layer_t* layer, int* tile_m);
  * `impl` is ignored (kept for ABI stability): there is one implementation, the wgmma kernel. */
 int fp_op_attention(const void* qkv, void* out, int B, int impl, void* stream);
 
+/* Transformer-head operators on the launch shapes of the product, for testing each kernel alone.  B sequences of 400
+ * tokens x 512 channels.  Every pointer must be device memory of the current device; fp16 activations, gamma / beta,
+ * w_f32 and mean_ws must be 16-byte aligned.  All arguments are checked before anything is enqueued on `stream`. */
+#define FP_OP_MAX_SEQUENCES 65536
+/* Attention of n_groups (1 or 2) column blocks of 1536 (q | k | v) per row of `ld` columns: qkv fp16 [B*400][ld],
+ * out fp16 [n_groups][B*400][512].  The refiner's heads run ld 3072 with two groups, the scorer ld 1536 with one. */
+int fp_op_attention_groups(const void* qkv, int ld, int n_groups, void* out, int B, void* stream);
+/* LayerNorm over 512 channels (eps 1e-5): x, y fp16 [rows][512], gamma, beta fp32 [512]. */
+int fp_op_layernorm(const void* x, void* y, const float* gamma, const float* beta, int rows, void* stream);
+/* Refiner head read-out: out[b] = w . mean_t LayerNorm(x[b, t]) + bias.  x fp16 [B][400][512], gamma, beta fp32
+ * [512], w fp32 [out_dim][512], bias fp32 [out_dim], out fp32 [B][out_dim], 1 <= out_dim <= 8. */
+int fp_op_head_final(const void* x, const float* gamma, const float* beta, const float* w, const float* bias, float* out,
+                     int B, int out_dim, void* stream);
+/* Scorer features: out[b] = w_f32 mean_t x[b, t] + bias.  x fp16 [B][400][512], w_f32 fp32 [512][512], bias fp32
+ * [512], mean_ws fp32 [B][512] workspace (receives the token means), out fp32 [B][512]. */
+int fp_op_token_mean_proj(const void* x, const float* w_f32, const float* bias, float* mean_ws, float* out, int B,
+                          void* stream);
+
 
 /* ------------------------------------------------------------------------------------------ */
 /* pose accuracy                                                                              */

@@ -15,6 +15,16 @@ def _mods():
     return _lib, ops, packing
 
 
+@pytest.fixture(autouse=True)
+def _fp32_reference():
+    # the references are fp32 convolutions / matmuls: no TF32 inside them
+    conv, mm = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    yield
+    torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = conv, mm
+
+
 def _cmp(got, ref, what, rtol=2e-3, atol=3e-3):
     got = got.float()
     err = (got - ref).abs()
@@ -90,6 +100,37 @@ def test_conv7_s2():
                          Cout=64, relu=True)
     ref = F.conv2d(x.float(), w.half().float(), b, stride=2, padding=3).relu().permute(0, 2, 3, 1)
     _cmp(out, ref, "conv7_s2")
+
+
+_STEM_MAX_IMAGES = 504
+
+
+@pytest.fixture(scope="module")
+def _stem_outputs():
+    """The stem at 3 images, at the 5 of track_one, and at the 501 / 504 of 249 / 252 hypotheses.  Inputs are drawn
+    once at the largest size and sliced, so every batch starts with the same images.  504 images make 25 200 tiles,
+    about 191 per CTA, so the six-stage patch ring wraps and its phase bit flips many times."""
+    _lib, ops, packing = _mods()
+    H = 160
+    x = _rand(_STEM_MAX_IMAGES, 6, H, H, seed=23).half()
+    w = _rand(64, 6, 7, 7, scale=(49 * 6) ** -0.5, seed=24)
+    b = _rand(64, seed=25)
+    w_packed = packing.pack_conv7(w.cpu()).cuda()
+    outs = {}
+    for n in (3, 5, 501, 504):
+        outs[n] = ops.gemm_layer(_lib.LAYER_CONV7_S2, packing.pad_image_c8(x[:n]), w_packed, b, n_img=n, Hin=H, Win=H,
+                                 Cin=8, Cout=64, relu=True)
+    return x, w, b, outs
+
+
+@pytest.mark.parametrize("n", [3, 5, 501, 504])
+def test_conv7_s2_batch_sizes(n, _stem_outputs):
+    """The stem at the image counts the product launches, against fp32 on the same fp16 inputs."""
+    x, w, b, outs = _stem_outputs
+    ref = F.conv2d(x[:n].float(), w.half().float(), b, stride=2, padding=3).relu().permute(0, 2, 3, 1)
+    _cmp(outs[n], ref, "conv7_s2")
+    # a tile's arithmetic does not depend on where in the ring it lands or how many tiles follow it
+    assert torch.equal(outs[n][:3], outs[3]), "images 0..2 differ from the 3-image launch"
 
 
 def test_out_split_concat():

@@ -13,8 +13,7 @@ import torch
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(scope="module")
-def setup():
+def _make_setup():
     from foundationpose_b200 import synth
     from foundationpose_b200.engine import Engine
     from foundationpose_b200.weights import random_state_dict
@@ -39,6 +38,11 @@ def setup():
         poses[i, :3, :3] = synth.random_rotation(10 + i) if i % 2 else poses[i, :3, :3]
         poses[i, :3, 3] += rng.normal(0, 0.01, 3)
     return dict(e=e, mesh=mesh, mt=mt, rgb=rgb, depth=depth, mask=mask, K=synth.DEFAULT_K, d=d, poses=poses, sd_r=sd_r, sd_s=sd_s, gt=pose)
+
+
+@pytest.fixture(scope="module")
+def setup():
+    return _make_setup()
 
 
 def test_refine_one_iteration_matches_oracle(setup):
@@ -205,3 +209,66 @@ def test_decoder_heads_on_two_streams_is_bitwise_serial(setup, monkeypatch):
             assert torch.equal(a, b)
         for a, b in zip(outs["0"][0], outs["0"][call]):
             assert torch.equal(a, b)
+
+
+def _launch_mode_outputs(s, e):
+    """refine(252 grid poses, 2 iterations) then score of the refined poses, three times each (eager, captured, graph
+    replay when graphs are on) -> the third call's (poses, last trans, last rot, scores, best) on the CPU; the three
+    calls must agree bit for bit."""
+    from foundationpose_b200 import hypotheses
+
+    poses = hypotheses.make_rotation_grid()
+    poses[:, :3, 3] = hypotheses.guess_translation(s["depth"], s["mask"], s["K"])
+    runs = []
+    for _ in range(3):
+        p, lt, lr = e.refine(poses, 2)
+        sc, best = e.score(p)
+        runs.append([t.cpu().clone() for t in (p, lt, lr, sc, best)])
+    for run in runs[1:]:
+        assert all(torch.equal(a, b) for a, b in zip(runs[0], run)), "repeated calls differ"
+    return runs[-1]
+
+
+def _write_launch_mode_outputs(path):
+    """Child-process entry of test_launch_modes_agree_at_252: a fresh setup, its outputs saved to `path`."""
+    s = _make_setup()
+    torch.save(_launch_mode_outputs(s, s["e"]), path)
+
+
+def test_launch_modes_agree_at_252(setup, monkeypatch, tmp_path):
+    """The same 252-hypothesis refine + score with CUDA graphs (the default), with eager launches (FPOSE_NO_GRAPH=1,
+    read by fp_create) and, in a child process, without programmatic dependent launch (FPOSE_PDL=0, read once per
+    process).  All three must agree bit for bit: a kernel that touches global memory an earlier kernel writes before
+    its pdl_wait() reads stale data only when it overlaps that kernel, so the PDL run would differ."""
+    import os
+    import subprocess
+    import sys
+
+    from foundationpose_b200.engine import Engine
+
+    s = setup
+    graphs = _launch_mode_outputs(s, s["e"])
+    monkeypatch.setenv("FPOSE_NO_GRAPH", "1")
+    e = Engine()
+    e.load_network("refine", s["sd_r"])
+    e.load_network("score", s["sd_s"])
+    e.set_mesh(s["mt"]["pos"], s["mt"]["normals"], s["mt"]["faces"], s["d"], uv=s["mt"]["uv"], tex=s["mt"]["tex"])
+    e.set_frame(s["rgb"], s["depth"], s["K"], filter_depth=False)
+    eager = _launch_mode_outputs(s, e)
+    e.close()
+    torch.cuda.empty_cache()  # the child process needs its own engine's memory next to this process's
+    monkeypatch.delenv("FPOSE_NO_GRAPH")
+    here = os.path.dirname(os.path.abspath(__file__))
+    out = tmp_path / "no_pdl.pt"
+    env = dict(os.environ, FPOSE_PDL="0")
+    code = ("import sys; sys.path[:0] = [sys.argv[1], sys.argv[2]]; import test_pipeline_gpu as t; "
+            "t._write_launch_mode_outputs(sys.argv[3])")
+    flags = ["-s"] if sys.flags.no_user_site else []
+    r = subprocess.run([sys.executable, *flags, "-c", code, os.path.dirname(here), here, str(out)], env=env,
+                       capture_output=True, text=True, timeout=900)
+    assert r.returncode == 0, f"FPOSE_PDL=0 child failed:\n{r.stdout[-2000:]}\n{r.stderr[-4000:]}"
+    no_pdl = torch.load(out)
+    names = ("poses", "last trans", "last rot", "scores", "best")
+    for name, a, b, c in zip(names, graphs, eager, no_pdl):
+        assert torch.equal(a, b), f"{name}: eager launches differ from graph replay"
+        assert torch.equal(a, c), f"{name}: FPOSE_PDL=0 differs from programmatic dependent launch"
