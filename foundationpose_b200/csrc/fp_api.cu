@@ -134,6 +134,7 @@ struct MeshSlot {
 struct CameraBufs {
   DevBuf rgb_raw, depth_raw, rgba, depth, xyz;
   PinnedBuf stage_rgb, stage_depth;
+  int H = 0, W = 0;  // the frame the last call prepared in this camera (fp_get_depth)
 };
 
 }  // namespace fp
@@ -153,6 +154,7 @@ struct fp_ctx {
   fp::CameraBufs cam[fp::kMaxCameras];
   float K[9] = {0};
   int H = 0, W = 0;
+  int n_frames = 0;  // the last call prepared the frames of cameras 0 .. n_frames - 1
   bool has_frame = false;
   // workspaces (sized for cap_n hypotheses)
   int cap_n = 0;
@@ -184,6 +186,7 @@ struct fp_ctx {
   int crop_tile = 0;
   fp::DevBuf lt_buf, lr_buf, feat_buf, pose_stage, tok_mean;
   fp::DevBuf mask_buf, mask_stats, crop_stats;
+  fp::DevBuf op_mesh_of;  // fp_op_pose_update: the uploaded slot id of every hypothesis
   // fp_track: the pose in and out of the graph, and its pinned read-back
   fp::PinnedBuf stage_pose;
   fp::DevBuf track_pose;
@@ -619,6 +622,9 @@ static void set_frame_geometry(fp_ctx* c, const float* K, int H, int W) {
   for (int i = 0; i < 9; ++i) c->K[i] = K[i];
   c->H = H;
   c->W = W;
+  c->n_frames = 1;
+  c->cam[0].H = H;
+  c->cam[0].W = W;
 }
 
 // mesh_of: [N] device slot ids, or null = slot 0 for every hypothesis; cams / camera_of as make_crops
@@ -676,6 +682,7 @@ static int setup_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host,
   }
   for (int i = 0; i < C; ++i) FP_TRY(alloc_camera(c, i, npix_max, /*raw=*/true, /*staged=*/true));
   set_frame_geometry(c, K, H[0], W[0]);
+  c->n_frames = C;
   FP_TRY(dev_alloc(c->epoch, c->args, kTableBytes + (size_t)2 * rows * sizeof(int)));
   FP_TRY(pinned_alloc(nullptr, c->stage_args, kTableBytes + (size_t)2 * staged_rows * sizeof(int)));
   CameraDev* table = reinterpret_cast<CameraDev*>(c->stage_args.p);
@@ -692,8 +699,8 @@ static int setup_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host,
     e.fy = K[9 * i + 4];
     e.cx = K[9 * i + 2];
     e.cy = K[9 * i + 5];
-    e.H = H[i];
-    e.W = W[i];
+    e.H = b.H = H[i];
+    e.W = b.W = W[i];
     FP_TRY(upload_staged_frame(b, rgb_host[i], depth_host[i], (size_t)H[i] * W[i], st));
   }
   return 0;
@@ -797,6 +804,33 @@ static ScoreTailParams score_tail_params(const fp_ctx* c, const float* feats, in
   return p;
 }
 
+// The scorer tail over n_seg segments of `feats`, segment g being rows [off_host[g], off_host[g + 1]).  Checks the
+// offsets before anything is enqueued (off_host[0] = 0, every segment 1..4096 rows: the kernel's shared memory holds
+// one segment's logits per head), sizes the tail's workspace and its per-segment arg-max tickets, uploads the offsets to
+// seg_off and sets seg / n_seg / seg_max.  `trailing` more ints the caller keeps after the offsets go up in the same copy (the register
+// calls' camera ids).  The register calls and fp_op_score_tail_segments both set their launch up here.
+static int segmented_tail_params(fp_ctx* c, const float* feats, const int* off_host, int n_seg, int trailing, float* scores,
+                                 int* best, cudaStream_t st, const char* caller, ScoreTailParams& p) {
+  FP_REQUIRE(n_seg >= 1, "%s: %d segments, need at least 1", caller, n_seg);
+  FP_REQUIRE(off_host[0] == 0, "%s: the first segment starts at row %d, not 0", caller, off_host[0]);
+  int seg_max = 0;
+  for (int g = 0; g < n_seg; ++g) {
+    const long long n = (long long)off_host[g + 1] - off_host[g];
+    FP_REQUIRE(n >= 1 && n <= 4096, "%s: segment %d has %lld rows, need 1..4096", caller, g, n);
+    seg_max = std::max(seg_max, (int)n);
+  }
+  const size_t ints = (size_t)(n_seg + 1 + trailing);
+  FP_TRY(ensure_tail(c, off_host[n_seg]));
+  FP_TRY(dev_alloc(c->epoch, c->seg_off, ints * sizeof(int)));
+  FP_TRY(dev_alloc(c->epoch, c->tail_counter, std::max<size_t>(16, (size_t)n_seg * sizeof(unsigned int)), /*zero=*/true));
+  FP_CUDA_OK(cudaMemcpyAsync(c->seg_off.p, off_host, ints * sizeof(int), cudaMemcpyHostToDevice, st));
+  p = score_tail_params(c, feats, off_host[n_seg], scores, best);
+  p.seg = reinterpret_cast<const int*>(c->seg_off.p);
+  p.n_seg = n_seg;
+  p.seg_max = seg_max;
+  return 0;
+}
+
 // fp_register_cameras and fp_register_objects after validation (n_hyp_host is checked here, before anything is
 // enqueued).  Object i is seen by camera camera_of[i]; its mask is masks_host[i], of its camera's size.  Each pass copies
 // its slot ids and per-hypothesis camera ids to the argument block, so the refine / feature graphs hold no per-pass
@@ -819,12 +853,10 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
                                  float* info_out_dev, cudaStream_t st, bool by_value) {
   const char* caller = by_value ? "fp_register_objects" : "fp_register_cameras";
   std::vector<int> off(M + 1, 0);
-  int seg_max = 0;
   for (int i = 0; i < M; ++i) {
     FP_REQUIRE(n_hyp_host[i] >= 1 && n_hyp_host[i] <= 4096, "%s: object %d: %d hypotheses, need 1..4096", caller, i,
                n_hyp_host[i]);
     off[i + 1] = off[i] + n_hyp_host[i];
-    seg_max = std::max(seg_max, n_hyp_host[i]);
   }
   const int total = off[M];
   // passes: whole objects in the given order, up to kRegisterPassCap hypotheses; an object above the cap alone
@@ -841,11 +873,9 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
   // every workspace is sized for the largest pass here, so no pass bumps the graph epoch
   FP_TRY(ensure_capacity(c, max_pass));
   FP_TRY(ensure_tail(c, total));
-  FP_TRY(dev_alloc(c->epoch, c->seg_off, (size_t)(2 * M + 1) * sizeof(int)));  // offsets [M + 1], camera ids [M]
   FP_TRY(dev_alloc(c->epoch, c->reg_feats, (size_t)total * 512 * sizeof(float)));
   FP_TRY(dev_alloc(c->epoch, c->mask_buf, mask_bytes));
   FP_TRY(dev_alloc(c->epoch, c->mask_stats, (size_t)M * 6 * sizeof(unsigned int)));
-  FP_TRY(dev_alloc(c->epoch, c->tail_counter, std::max<size_t>(16, (size_t)M * sizeof(unsigned int)), /*zero=*/true));
   if (!by_value) FP_TRY(dev_alloc(c->epoch, c->mask_off, (size_t)M * sizeof(size_t)));
   // pinned staging (never read by a captured graph): the copies below leave as soon as they are enqueued.  stage_ints:
   // offsets [M + 1], camera of every object [M], one int of padding, each object's mask byte offset size_t [M]
@@ -870,7 +900,10 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
       std::fill(ids + row0 + n + off[i], ids + row0 + n + off[i + 1], camera_of[i]);
     }
   }
-  FP_CUDA_OK(cudaMemcpyAsync(c->seg_off.p, ints, (size_t)(2 * M + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
+  // seg_off: the offsets [M + 1], then the camera ids [M]; the scorer tail at the end runs over these segments
+  ScoreTailParams tp;
+  FP_TRY(segmented_tail_params(c, reinterpret_cast<const float*>(c->reg_feats.p), ints, M, /*trailing=*/M, scores_out_dev,
+                               best_out_dev, st, caller, tp));
   FP_CUDA_OK(cudaMemcpyAsync(c->mask_buf.p, c->stage_masks.p, mask_bytes, cudaMemcpyHostToDevice, st));
   const CameraDev* cams_dev = by_value ? nullptr : reinterpret_cast<const CameraDev*>(c->args.p);
   // estimater.py:173-174, :214 once per camera for every object: erode + bilateral, depth2xyzmap(zfar = inf)
@@ -927,10 +960,6 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
                                cudaMemcpyDeviceToDevice, st));
   }
   // score_network.py:84-88 per object: one tail launch, each object's hypotheses attending only to each other
-  ScoreTailParams tp = score_tail_params(c, reinterpret_cast<const float*>(c->reg_feats.p), total, scores_out_dev, best_out_dev);
-  tp.seg = seg;
-  tp.n_seg = M;
-  tp.seg_max = seg_max;
   FP_TRY(score_tail_launch(tp, st));
   FP_CUDA_OK(cudaStreamSynchronize(st));
   return 0;
@@ -1213,16 +1242,22 @@ int fp_set_xyz_map(fp_ctx* c, const float* xyz, void* stream) {
   FP_API_END
 }
 
-int fp_get_depth(fp_ctx* c, float* depth_out_dev, float* xyz_out_dev, void* stream) {
+int fp_get_depth(fp_ctx* c, int camera, float* depth_out_dev, float* xyz_out_dev, int* hw_out, void* stream) {
   FP_API_BEGIN
   FP_REQUIRE(c && c->has_frame, "fp_get_depth: no frame");
+  FP_REQUIRE(camera >= 0 && camera < c->n_frames, "fp_get_depth: camera %d: the last call prepared cameras 0..%d", camera,
+             c->n_frames - 1);
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const size_t npix = (size_t)c->H * c->W;
-  if (depth_out_dev) FP_CUDA_OK(cudaMemcpyAsync(depth_out_dev, c->cam[0].depth.p, npix * 4, cudaMemcpyDeviceToDevice, st));
+  const CameraBufs& b = c->cam[camera];
+  if (hw_out) {
+    hw_out[0] = b.H;
+    hw_out[1] = b.W;
+  }
+  const size_t npix = (size_t)b.H * b.W;
+  if (depth_out_dev) FP_CUDA_OK(cudaMemcpyAsync(depth_out_dev, b.depth.p, npix * 4, cudaMemcpyDeviceToDevice, st));
   // internal layout is float4 per pixel; the hook returns the reference's [H][W][3]
-  if (xyz_out_dev)
-    FP_CUDA_OK(cudaMemcpy2DAsync(xyz_out_dev, 12, c->cam[0].xyz.p, 16, 12, npix, cudaMemcpyDeviceToDevice, st));
+  if (xyz_out_dev) FP_CUDA_OK(cudaMemcpy2DAsync(xyz_out_dev, 12, b.xyz.p, 16, 12, npix, cudaMemcpyDeviceToDevice, st));
   return 0;
   FP_API_END
 }
@@ -1386,6 +1421,22 @@ int fp_score_tail(fp_ctx* c, const float* feats, int L, float* scores_out, int* 
   if (L == 0) return 0;
   FP_TRY(ensure_tail(c, L));
   return score_tail_launch(score_tail_params(c, feats, L, scores_out, best_out), st);
+  FP_API_END
+}
+
+int fp_op_score_tail_segments(fp_ctx* c, const float* feats, int L, const int* seg_host, int n_seg, float* scores_out,
+                              int* best_out, void* stream) {
+  FP_API_BEGIN
+  const char* fn = "fp_op_score_tail_segments";
+  FP_REQUIRE(c && feats && seg_host && scores_out && best_out, "%s: null argument", fn);
+  FP_REQUIRE(c->net[1].loaded, "scorer weights not loaded");
+  FP_REQUIRE(n_seg >= 1, "%s: %d segments, need at least 1", fn, n_seg);
+  FP_REQUIRE(seg_host[n_seg] == L, "%s: the last segment ends at row %d, not at L = %d", fn, seg_host[n_seg], L);
+  DeviceGuard dg(c->device);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  ScoreTailParams p;
+  FP_TRY(segmented_tail_params(c, feats, seg_host, n_seg, /*trailing=*/0, scores_out, best_out, st, fn, p));
+  return score_tail_launch(p, st);
   FP_API_END
 }
 
@@ -1624,12 +1675,25 @@ int fp_op_depth_filter(const float* depth_dev, float* out_dev, int H, int W, int
   FP_API_END
 }
 
-int fp_op_pose_update(const float* poses_in, const float* trans, const float* rot, float* poses_out, int N,
-                      float mesh_diameter, float rot_normalizer, void* stream) {
+int fp_op_pose_update(fp_ctx* c, const float* poses_in, const float* trans, const float* rot, const int* mesh_of_host, int N,
+                      float* poses_out, float* trans_delta_out, float* rot_delta_out, void* stream) {
   FP_API_BEGIN
-  FP_REQUIRE(poses_in && trans && rot && poses_out, "fp_op_pose_update: null argument");
-  return pose_update_launch(poses_in, trans, rot, poses_out, nullptr, nullptr, N, nullptr, nullptr, mesh_diameter / 2.0f,
-                            rot_normalizer, reinterpret_cast<cudaStream_t>(stream));
+  const char* fn = "fp_op_pose_update";
+  FP_REQUIRE(c && poses_in && trans && rot && poses_out && N >= 0, "%s: bad argument", fn);
+  const int slot0 = 0;
+  FP_TRY(check_slots(c, mesh_of_host ? N : 1, mesh_of_host ? mesh_of_host : &slot0, fn));
+  DeviceGuard dg(c->device);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (N == 0) return 0;
+  const int* mesh_of = nullptr;
+  if (mesh_of_host) {
+    FP_TRY(dev_alloc(c->epoch, c->op_mesh_of, (size_t)N * sizeof(int)));
+    FP_CUDA_OK(cudaMemcpyAsync(c->op_mesh_of.p, mesh_of_host, (size_t)N * sizeof(int), cudaMemcpyHostToDevice, st));
+    mesh_of = reinterpret_cast<const int*>(c->op_mesh_of.p);
+  }
+  // as refine_body launches it: each hypothesis's half-diameter from the mesh table, the context's rot_normalizer
+  return pose_update_launch(poses_in, trans, rot, poses_out, trans_delta_out, rot_delta_out, N,
+                            reinterpret_cast<const MeshSlotDev*>(c->mesh_table.p), mesh_of, 0.f, c->rot_normalizer, st);
   FP_API_END
 }
 

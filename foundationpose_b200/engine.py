@@ -42,7 +42,7 @@ def _proto():
     lib.fp_set_mesh.argtypes = [vp, i, i, vp, vp, vp, vp, vp, vp, i, i, f]
     lib.fp_set_mesh_slot.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp, vp, i, i, f]
     lib.fp_set_frame.argtypes = [vp, vp, vp, C.POINTER(f), i, i, i, f, vp]
-    lib.fp_get_depth.argtypes = [vp, vp, vp, vp]
+    lib.fp_get_depth.argtypes = [vp, i, vp, vp, C.POINTER(i), vp]
     lib.fp_set_xyz_map.argtypes = [vp, vp, vp]
     lib.fp_make_crops.argtypes = [vp, vp, i, i, vp, vp, vp, vp]
     lib.fp_start_poses.argtypes = [vp, vp, i, vp, i, vp, vp, vp]
@@ -50,12 +50,13 @@ def _proto():
     lib.fp_score.argtypes = [vp, vp, i, vp, vp, vp]
     lib.fp_score_features.argtypes = [vp, vp, i, vp, vp]
     lib.fp_score_tail.argtypes = [vp, vp, i, vp, vp, vp]
+    lib.fp_op_score_tail_segments.argtypes = [vp, vp, i, C.POINTER(i), i, vp, vp, vp]
     lib.fp_register.argtypes = [vp, vp, i, i, vp, vp, vp, vp]
     lib.fp_op_refine_net.argtypes = [vp, vp, i, vp, vp, vp]
     lib.fp_op_score_feats.argtypes = [vp, vp, i, vp, vp]
     lib.fp_op_tokens.argtypes = [vp, i, vp, i, vp, vp]
     lib.fp_op_depth_filter.argtypes = [vp, vp, i, i, i, vp]
-    lib.fp_op_pose_update.argtypes = [vp, vp, vp, vp, i, f, f, vp]
+    lib.fp_op_pose_update.argtypes = [vp, vp, vp, vp, C.POINTER(i), i, vp, vp, vp, vp]
     lib.fp_vis.argtypes = [vp, i, vp, vp, i, vp, vp, C.POINTER(i), vp]
     lib.fp_vis_size.argtypes = [i, i, C.POINTER(i)]
     lib.fp_vis_colormap.argtypes = [vp]
@@ -65,7 +66,7 @@ def _proto():
     for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_track_cameras", "fp_register_objects", "fp_register_cameras", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh",
                  "fp_set_mesh_slot", "fp_set_frame",
                  "fp_get_depth", "fp_make_crops", "fp_start_poses", "fp_refine", "fp_score", "fp_score_features", "fp_score_tail",
-                 "fp_register", "fp_op_refine_net", "fp_op_score_feats", "fp_op_tokens", "fp_op_depth_filter",
+                 "fp_op_score_tail_segments", "fp_register", "fp_op_refine_net", "fp_op_score_feats", "fp_op_tokens", "fp_op_depth_filter",
                  "fp_op_pose_update", "fp_vis", "fp_vis_size", "fp_vis_colormap", "fp_vis_crops"):
         getattr(lib, name).restype = C.c_int
 
@@ -418,11 +419,15 @@ class Engine:
         self._xyz_keep = x
         _lib.check(lib.fp_set_xyz_map(self._h, _p(x), _stream()), "fp_set_xyz_map")
 
-    def get_depth(self):
-        H, W = self.frame_hw
+    def get_depth(self, camera=0):
+        """Camera `camera`'s filtered depth (H,W) and xyz map (H,W,3) as the last frame-taking call prepared them, at that
+        camera's size (test hook).  Cameras 1.. exist after track_cameras / register_cameras only."""
+        hw = (C.c_int * 2)()
+        _lib.check(lib.fp_get_depth(self._h, int(camera), None, None, hw, _stream()), "fp_get_depth")
+        H, W = hw[0], hw[1]
         d = torch.empty(H, W, dtype=torch.float32, device="cuda")
         x = torch.empty(H, W, 3, dtype=torch.float32, device="cuda")
-        _lib.check(lib.fp_get_depth(self._h, _p(d), _p(x), _stream()), "fp_get_depth")
+        _lib.check(lib.fp_get_depth(self._h, int(camera), _p(d), _p(x), None, _stream()), "fp_get_depth")
         return d, x
 
     def start_poses(self, mask, rot_grid):
@@ -498,6 +503,20 @@ class Engine:
         _lib.check(lib.fp_score_tail(self._h, _p(feats), L, _p(scores), _p(best), _stream()), "fp_score_tail")
         return scores, best
 
+    def score_tail_segments(self, feats, seg, scores=None, best=None):
+        """fp_op_score_tail_segments: the register calls' segmented tail on given features (test hook).  feats (L,512)
+        CUDA; seg: the n_seg + 1 row offsets (0, ..., L).  Returns scores (L,) = logits + 100 and best (n_seg,) int32,
+        each segment's first arg-max relative to its first row, written into `scores` / `best` when given."""
+        feats = feats.contiguous().float()
+        L = feats.shape[0]
+        seg = [int(s) for s in seg]
+        n_seg = len(seg) - 1
+        scores = torch.empty(L, dtype=torch.float32, device="cuda") if scores is None else scores
+        best = torch.empty(max(n_seg, 1), dtype=torch.int32, device="cuda") if best is None else best
+        _lib.check(lib.fp_op_score_tail_segments(self._h, _p(feats), L, (C.c_int * len(seg))(*seg), n_seg, _p(scores), _p(best),
+                                                 _stream()), "fp_op_score_tail_segments")
+        return scores, best
+
     def register_host(self, poses_host, iterations, out_poses=None, out_scores=None):
         """fp_register: pinned host buffers in, host buffers out (synchronous)."""
         poses_host = poses_host if torch.is_tensor(poses_host) else torch.from_numpy(np.ascontiguousarray(poses_host, dtype=np.float32))
@@ -551,6 +570,20 @@ class Engine:
         _lib.check(lib.fp_op_refine_net(self._h, _p(crops), N, _p(trans), _p(rot), _stream()), "fp_op_refine_net")
         return trans, rot
 
+    def op_pose_update(self, poses, trans, rot, mesh_of=None):
+        """fp_op_pose_update: one refine-loop pose update, hypothesis n scaled by the half-diameter of the mesh in slot
+        mesh_of[n] (None = slot 0) and rotated with the context's rot_normalizer.  Returns the new poses (N,4,4), the
+        translation deltas (N,3) and the rotation deltas (N,3,3), CUDA float32."""
+        poses = self._poses(poses)
+        N = len(poses)
+        out = torch.empty_like(poses)
+        td = torch.empty(N, 3, dtype=torch.float32, device="cuda")
+        rd = torch.empty(N, 3, 3, dtype=torch.float32, device="cuda")
+        ids = None if mesh_of is None else (C.c_int * N)(*[int(m) for m in mesh_of])
+        _lib.check(lib.fp_op_pose_update(self._h, _p(poses), _p(trans.contiguous().float()), _p(rot.contiguous().float()), ids, N,
+                                         _p(out), _p(td), _p(rd), _stream()), "fp_op_pose_update")
+        return out, td, rd
+
     def op_score_feats(self, crops, N):
         feats = torch.empty(N, 512, dtype=torch.float32, device="cuda")
         _lib.check(lib.fp_op_score_feats(self._h, _p(crops), N, _p(feats), _stream()), "fp_op_score_feats")
@@ -588,10 +621,3 @@ def op_depth_filter(depth, which):
     _lib.check(lib.fp_op_depth_filter(_p(depth), _p(out), H, W, which, _stream()), "fp_op_depth_filter")
     return out
 
-
-def op_pose_update(poses, trans, rot, mesh_diameter, rot_normalizer):
-    poses = poses.contiguous().float()
-    out = torch.empty_like(poses)
-    _lib.check(lib.fp_op_pose_update(_p(poses), _p(trans.contiguous().float()), _p(rot.contiguous().float()), _p(out),
-                                     len(poses), float(mesh_diameter), float(rot_normalizer), _stream()), "fp_op_pose_update")
-    return out

@@ -194,8 +194,10 @@ int fp_set_frame(fp_ctx* ctx, const unsigned char* rgb, const float* depth, cons
 /* Replaces the xyz map derived by fp_set_frame with the caller's own (PoseRefinePredictor.predict's `xyz_map`
  * argument, predict_pose_refine.py:150,177): float32 [H][W][3], host or device pointer. */
 int fp_set_xyz_map(fp_ctx* ctx, const float* xyz, void* stream);
-/* Copies the filtered depth [H][W] and/or the xyz map [H][W][3] to device buffers (test hook). */
-int fp_get_depth(fp_ctx* ctx, float* depth_out_dev, float* xyz_out_dev, void* stream);
+/* Copies camera `camera`'s filtered depth [H][W] and/or xyz map [H][W][3], as the last frame-taking call prepared
+ * them, to device buffers; hw_out[2] (optional) receives that camera's H and W (test hook).  Refuses a camera the last
+ * call did not prepare (fp_set_frame, fp_track, fp_register_objects: camera 0 only). */
+int fp_get_depth(fp_ctx* ctx, int camera, float* depth_out_dev, float* xyz_out_dev, int* hw_out, void* stream);
 
 /* FoundationPose.guess_translation (estimater.py:137-156: centre of the mask's bounding box, median of the
  * masked valid depths of the CURRENT FILTERED frame) and generate_random_pose_hypo (estimater.py:127-134,
@@ -233,6 +235,12 @@ int fp_score(fp_ctx* ctx, const float* poses, int N, float* scores_out, int* bes
  * cross-hypothesis attention + linear + argmax (score_network.py:84-88). */
 int fp_score_features(fp_ctx* ctx, const float* poses, int N, float* feats_out, void* stream);
 int fp_score_tail(fp_ctx* ctx, const float* feats, int L, float* scores_out, int* best_out, void* stream);
+/* The segmented tail of the register calls (test hook): segment g is feature rows [seg_host[g], seg_host[g + 1]) and
+ * its hypotheses attend only to each other.  seg_host: HOST [n_seg + 1] with seg_host[0] = 0, strictly increasing,
+ * seg_host[n_seg] = L and at most 4096 rows per segment (refused, with nothing enqueued, otherwise).  scores_out DEVICE
+ * [L] (= logits + 100), best_out DEVICE [n_seg]: each segment's first arg-max, relative to its first row. */
+int fp_op_score_tail_segments(fp_ctx* ctx, const float* feats, int L, const int* seg_host, int n_seg, float* scores_out,
+                              int* best_out, void* stream);
 
 /* Hot loop of FoundationPose.register (estimater.py:203-235) with HOST buffers: uploads the N
  * start poses, refines `iterations` times, scores, and returns refined poses [N][16], scores [N]
@@ -383,9 +391,12 @@ int fp_op_build_meshlets(int V, int F, const float* pos, const int* faces, int* 
                          float* meshlets_out /* optional [ceil(F/1)][8]: sphere xyz r, cone axis xyz cutoff */);
 /* which: 0 = erode_depth (Utils.py:359-395), 1 = bilateral_filter_depth (Utils.py:304-356) */
 int fp_op_depth_filter(const float* depth_dev, float* out_dev, int H, int W, int which, void* stream);
-/* egocentric_delta_pose_to_pose with the refiner's output decoding (predict_pose_refine.py:195-231) */
-int fp_op_pose_update(const float* poses_in, const float* trans, const float* rot, float* poses_out, int N,
-                      float mesh_diameter, float rot_normalizer, void* stream);
+/* egocentric_delta_pose_to_pose with the refiner's output decoding (predict_pose_refine.py:195-231), launched as the
+ * refine loop launches it: hypothesis n moves by trans[n] times the half-diameter of the mesh in slot mesh_of_host[n]
+ * (host [N]; null = slot 0; every slot must hold a mesh), rotations use the context's rot_normalizer (fp_set_config).
+ * Device [N][16] poses; trans_delta_out [N][3] / rot_delta_out [N][9] (optional) receive the decoded deltas. */
+int fp_op_pose_update(fp_ctx* ctx, const float* poses_in, const float* trans, const float* rot, const int* mesh_of_host,
+                      int N, float* poses_out, float* trans_delta_out, float* rot_delta_out, void* stream);
 
 #ifdef __cplusplus
 }

@@ -123,7 +123,6 @@ def test_set_frame_filters_and_xyz(scene):
 
 
 def test_pose_update(scene):
-    from foundationpose_b200.engine import op_pose_update
     from oracle import geometry
 
     g = torch.Generator().manual_seed(2)
@@ -131,7 +130,8 @@ def test_pose_update(scene):
     trans = torch.randn(4, 3, generator=g) * 0.3
     rot = torch.randn(4, 3, generator=g)
     rot[0] = 0  # exercises the eps clamp of so3_exp_map
-    out = op_pose_update(poses.cuda(), trans.cuda(), rot.cuda(), scene["d"], 0.3490658503988659)
+    # slot 0 holds the scene's mesh (diameter d); the context keeps the default rot_normalizer
+    out, _, _ = scene["e"].op_pose_update(poses.cuda(), trans.cuda(), rot.cuda())
     ref, _, _ = geometry.pose_update(poses, trans, rot, scene["d"], 0.3490658503988659)
     np.testing.assert_allclose(out.cpu().numpy(), ref.numpy(), atol=2e-6, rtol=0)
 
