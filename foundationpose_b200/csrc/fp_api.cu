@@ -289,30 +289,91 @@ static GemmLayer mk(int kind, int n_img, int H, int W, int Cin, int Cout, const 
     if (_rc) return _rc;     \
   } while (0)
 
-// crops [2N][166][168][8] -> tokens [N][400][512] (+ positional embedding)
-static int run_encoder(fp_ctx* c, const Net& net, const __half* crops, int N, cudaStream_t st) {
+// The encoder's activation buffers, as the layer table names them
+enum EncBuf : int { EB_NONE = -1, EB_CROPS, EB_ACT0, EB_A1, EB_A2, EB_A3, EB_AB0, EB_AB1, EB_AB2, EB_C0, EB_C1, EB_C2, EB_TOK };
+
+// One layer of the encoder (encodeA + encodeAB of refine_network.py:34-50, encoderA + encoderAB of
+// score_network.py:37-51), BatchNorm folded, ReLU after every layer.  Weights "enc.<layer>.w" / "enc.<layer>.b".
+struct EncLayer {
+  int kind;
+  bool ab_batch;    // runs on the M = Np + N images of the A and B crops (Np = b_img0_of(N)), else on the N pairs
+  int H;            // input height = width
+  int Cin, Cout;
+  EncBuf in, out, res;
+  int out_ld;       // 0: Cout
+  bool split;       // out_split = Np: image n < Np -> image n, channels [0, Cout); n >= Np -> image n - Np, [Cout, 2 Cout)
+  bool pe;          // adds the positional embedding "pe" after the ReLU
+};
+
+// The encoder, in launch order: run_encoder, fp_op_encoder and fp_op_encoder_layer all read this table.  Every
+// residual block's second layer adds the block's input, which the buffer rotation keeps until then.
+constexpr int kEncLayers = 15;
+static const EncLayer kEncoder[kEncLayers] = {
+    {LK_CONV7_S2, true, S, 8, 64, EB_CROPS, EB_ACT0, EB_NONE, 0, false, false},
+    {LK_CONV3_S2, true, 80, 64, 128, EB_ACT0, EB_A1, EB_NONE, 0, false, false},
+    {LK_CONV3_S1, true, 40, 128, 128, EB_A1, EB_A2, EB_NONE, 0, false, false},
+    {LK_CONV3_S1, true, 40, 128, 128, EB_A2, EB_A3, EB_A1, 0, false, false},
+    {LK_CONV3_S1, true, 40, 128, 128, EB_A3, EB_A2, EB_NONE, 0, false, false},
+    // the last encodeA layer writes straight into the 256-channel concat buffer (refine_network.py:85)
+    {LK_CONV3_S1, true, 40, 128, 128, EB_A2, EB_AB0, EB_A3, 256, true, false},
+    {LK_CONV3_S1, false, 40, 256, 256, EB_AB0, EB_AB1, EB_NONE, 0, false, false},
+    {LK_CONV3_S1, false, 40, 256, 256, EB_AB1, EB_AB2, EB_AB0, 0, false, false},
+    {LK_CONV3_S1, false, 40, 256, 256, EB_AB2, EB_AB1, EB_NONE, 0, false, false},
+    {LK_CONV3_S1, false, 40, 256, 256, EB_AB1, EB_AB0, EB_AB2, 0, false, false},
+    {LK_CONV3_S2, false, 40, 256, 512, EB_AB0, EB_C0, EB_NONE, 0, false, false},
+    {LK_CONV3_S1, false, 20, 512, 512, EB_C0, EB_C1, EB_NONE, 0, false, false},
+    {LK_CONV3_S1, false, 20, 512, 512, EB_C1, EB_C2, EB_C0, 0, false, false},
+    {LK_CONV3_S1, false, 20, 512, 512, EB_C2, EB_C1, EB_NONE, 0, false, false},
+    {LK_CONV3_S1, false, 20, 512, 512, EB_C1, EB_TOK, EB_C2, 0, false, true},
+};
+
+static void* enc_buf(fp_ctx* c, const __half* crops, EncBuf b) {
+  switch (b) {
+    case EB_CROPS: return const_cast<__half*>(crops);
+    case EB_ACT0: return c->act0.p;
+    case EB_A1: return c->a1.p;
+    case EB_A2: return c->a2.p;
+    case EB_A3: return c->a3.p;
+    case EB_AB0: return c->ab0.p;
+    case EB_AB1: return c->ab1.p;
+    case EB_AB2: return c->ab2.p;
+    case EB_C0: return c->c0.p;
+    case EB_C1: return c->c1.p;
+    case EB_C2: return c->c2.p;
+    case EB_TOK: return c->tok.p;
+    default: return nullptr;
+  }
+}
+
+// Layer k's output buffer as the next layers read it, NHWC: {images, height, width, channels}.  The concat layer's
+// buffer holds N images of [A_i | B_i] (2 Cout channels); the A / B layers' buffers hold all M images, pads included.
+static void enc_out_shape(int k, int N, int shape[4]) {
+  const EncLayer& l = kEncoder[k];
+  shape[0] = (l.ab_batch && !l.split) ? b_img0_of(N) + N : N;
+  shape[1] = shape[2] = l.kind == LK_CONV3_S1 ? l.H : l.H / 2;
+  shape[3] = l.out_ld ? l.out_ld : l.Cout;
+}
+
+// The layer whose output is still in buffer `b` when layer k runs: the last writer before k (-1: the crops)
+static int enc_source(int k, EncBuf b) {
+  for (int j = k - 1; j >= 0; --j)
+    if (kEncoder[j].out == b) return j;
+  return -1;
+}
+
+// crops [2N][166][168][8] -> tokens [N][400][512] (+ positional embedding), or layers 0 .. last only
+static int run_encoder(fp_ctx* c, const Net& net, const __half* crops, int N, cudaStream_t st, int last = kEncLayers - 1) {
   char wn[32], bn[32];
-  auto W = [&](int i) { snprintf(wn, sizeof wn, "enc.%d.w", i); return net.h(wn); };
-  auto B = [&](int i) { snprintf(bn, sizeof bn, "enc.%d.b", i); return net.f(bn); };
   const int Np = b_img0_of(N);
-  const int M = Np + N;
-  FP_TRY(gemm_layer_launch(mk(LK_CONV7_S2, M, S, S, 8, 64, crops, W(0), B(0), c->act0.p, 1), st));
-  FP_TRY(gemm_layer_launch(mk(LK_CONV3_S2, M, 80, 80, 64, 128, c->act0.p, W(1), B(1), c->a1.p, 1), st));
-  FP_TRY(gemm_layer_launch(mk(LK_CONV3_S1, M, 40, 40, 128, 128, c->a1.p, W(2), B(2), c->a2.p, 1), st));
-  FP_TRY(gemm_layer_launch(mk(LK_CONV3_S1, M, 40, 40, 128, 128, c->a2.p, W(3), B(3), c->a3.p, 1, c->a1.p), st));
-  FP_TRY(gemm_layer_launch(mk(LK_CONV3_S1, M, 40, 40, 128, 128, c->a3.p, W(4), B(4), c->a2.p, 1), st));
-  // last encodeA layer writes straight into the 256-channel concat buffer (refine_network.py:85)
-  FP_TRY(gemm_layer_launch(mk(LK_CONV3_S1, M, 40, 40, 128, 128, c->a2.p, W(5), B(5), c->ab0.p, 1, c->a3.p, 256, Np), st));
-  FP_TRY(gemm_layer_launch(mk(LK_CONV3_S1, N, 40, 40, 256, 256, c->ab0.p, W(6), B(6), c->ab1.p, 1), st));
-  FP_TRY(gemm_layer_launch(mk(LK_CONV3_S1, N, 40, 40, 256, 256, c->ab1.p, W(7), B(7), c->ab2.p, 1, c->ab0.p), st));
-  FP_TRY(gemm_layer_launch(mk(LK_CONV3_S1, N, 40, 40, 256, 256, c->ab2.p, W(8), B(8), c->ab1.p, 1), st));
-  FP_TRY(gemm_layer_launch(mk(LK_CONV3_S1, N, 40, 40, 256, 256, c->ab1.p, W(9), B(9), c->ab0.p, 1, c->ab2.p), st));
-  FP_TRY(gemm_layer_launch(mk(LK_CONV3_S2, N, 40, 40, 256, 512, c->ab0.p, W(10), B(10), c->c0.p, 1), st));
-  FP_TRY(gemm_layer_launch(mk(LK_CONV3_S1, N, 20, 20, 512, 512, c->c0.p, W(11), B(11), c->c1.p, 1), st));
-  FP_TRY(gemm_layer_launch(mk(LK_CONV3_S1, N, 20, 20, 512, 512, c->c1.p, W(12), B(12), c->c2.p, 1, c->c0.p), st));
-  FP_TRY(gemm_layer_launch(mk(LK_CONV3_S1, N, 20, 20, 512, 512, c->c2.p, W(13), B(13), c->c1.p, 1), st));
-  FP_TRY(gemm_layer_launch(
-      mk(LK_CONV3_S1, N, 20, 20, 512, 512, c->c1.p, W(14), B(14), c->tok.p, 1, c->c2.p, 0, 0, net.f("pe")), st));
+  for (int k = 0; k <= last; ++k) {
+    const EncLayer& l = kEncoder[k];
+    snprintf(wn, sizeof wn, "enc.%d.w", k);
+    snprintf(bn, sizeof bn, "enc.%d.b", k);
+    FP_TRY(gemm_layer_launch(mk(l.kind, l.ab_batch ? Np + N : N, l.H, l.H, l.Cin, l.Cout, enc_buf(c, crops, l.in),
+                                net.h(wn), net.f(bn), enc_buf(c, crops, l.out), 1, enc_buf(c, crops, l.res), l.out_ld,
+                                l.split ? Np : 0, l.pe ? net.f("pe") : nullptr),
+                             st));
+  }
   return 0;
 }
 
@@ -1346,18 +1407,48 @@ int fp_op_score_feats(fp_ctx* c, const void* crops, int N, float* feats_out, voi
   FP_API_END
 }
 
-int fp_op_tokens(fp_ctx* c, int which, const void* crops, int N, void* tokens_out, void* stream) {
+int fp_op_encoder_layer(int layer, int N, int* info) {
   FP_API_BEGIN
-  FP_REQUIRE(c && crops && tokens_out && (which == 0 || which == 1), "fp_op_tokens: bad argument");
-  FP_REQUIRE(c->net[which].loaded, "weights not loaded");
+  FP_REQUIRE(info, "fp_op_encoder_layer: null info");
+  FP_REQUIRE(layer >= 0 && layer < kEncLayers, "fp_op_encoder_layer: layer = %d outside [0, %d]", layer, kEncLayers - 1);
+  FP_REQUIRE(N >= 0 && N <= kRegisterPassCap, "fp_op_encoder_layer: N = %d outside [0, %d]", N, kRegisterPassCap);
+  const EncLayer& l = kEncoder[layer];
+  const int Np = b_img0_of(N);
+  info[0] = l.kind;
+  info[1] = l.ab_batch ? Np + N : N;
+  info[2] = l.H;
+  info[3] = l.Cin;
+  info[4] = l.Cout;
+  info[5] = enc_source(layer, l.in);
+  info[6] = l.res == EB_NONE ? -1 : enc_source(layer, l.res);
+  info[7] = l.split ? Np : 0;
+  info[8] = l.pe ? 1 : 0;
+  enc_out_shape(layer, N, info + 9);
+  return 0;
+  FP_API_END
+}
+
+long long fp_op_encoder(fp_ctx* c, int which, const void* crops, int N, int last, void* out, void* stream) {
+  FP_API_BEGIN
+  const char* fn = "fp_op_encoder";
+  FP_REQUIRE(c, "%s: null context", fn);
+  FP_REQUIRE(which == 0 || which == 1, "%s: which = %d, must be 0 (refiner) or 1 (scorer)", fn, which);
+  FP_REQUIRE(last >= 0 && last < kEncLayers, "%s: last = %d outside [0, %d]", fn, last, kEncLayers - 1);
+  FP_REQUIRE(N >= 0 && N <= kRegisterPassCap, "%s: N = %d outside [0, %d]", fn, N, kRegisterPassCap);
+  FP_REQUIRE(crops && out, "%s: null crops or out", fn);
+  FP_REQUIRE(c->net[which].loaded, "%s: %s weights not loaded", fn, which == 0 ? "refiner" : "scorer");
   DeviceGuard dg(c->device);
+  if (check_device_ptr(crops, "crops", fn) || check_device_ptr(out, "out", fn)) return -1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (N == 0) return 0;
+  int shape[4];
+  enc_out_shape(last, N, shape);
+  const size_t bytes = (size_t)shape[0] * shape[1] * shape[2] * shape[3] * 2;
   FP_TRY(ensure_capacity(c, N));
   FP_TRY(crops_import(c, crops, N, st));
-  FP_TRY(run_encoder(c, c->net[which], reinterpret_cast<const __half*>(c->crops.p), N, st));
-  FP_CUDA_OK(cudaMemcpyAsync(tokens_out, c->tok.p, (size_t)N * T * 512 * 2, cudaMemcpyDeviceToDevice, st));
-  return 0;
+  FP_TRY(run_encoder(c, c->net[which], reinterpret_cast<const __half*>(c->crops.p), N, st, last));
+  FP_CUDA_OK(cudaMemcpyAsync(out, enc_buf(c, nullptr, kEncoder[last].out), bytes, cudaMemcpyDeviceToDevice, st));
+  return (long long)bytes;
   FP_API_END
 }
 

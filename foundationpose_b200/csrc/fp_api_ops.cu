@@ -15,10 +15,8 @@ int pose_errors_launch(const float* pts, int P, const float* pred, int N, const 
                        float* adds_out, cudaStream_t stream);
 int sym_pose_errors_launch(const float* pts, int P, const float* pred, int N, const float* gt, int n_gt, const float* sym,
                            int S, const float* K, int n_K, float* mssd_out, float* mspd_out, cudaStream_t stream);
-}
 
-// 0 when `p` is memory a kernel on the current device may read and write, else -1 with the reason in fp_last_error()
-static int check_device_ptr(const void* p, const char* what, const char* fn = "fp_pose_errors") {
+int check_device_ptr(const void* p, const char* what, const char* fn) {
   int dev = 0;
   FP_CUDA_OK(cudaGetDevice(&dev));
   cudaPointerAttributes a;
@@ -38,6 +36,9 @@ static int check_device_ptr(const void* p, const char* what, const char* fn = "f
   }
   return 0;
 }
+}  // namespace fp
+
+using fp::check_device_ptr;
 
 extern "C" {
 

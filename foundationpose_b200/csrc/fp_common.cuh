@@ -39,6 +39,9 @@ int num_sms();  // of the current device
 // error plumbing (host)
 // ----------------------------------------------------------------------------------------------
 void set_last_error(const char* fmt, ...);
+// 0 when `p` is memory a kernel on the current device may read and write, else -1 with the reason (prefixed by `fn`)
+// in fp_last_error()
+int check_device_ptr(const void* p, const char* what, const char* fn = "fp_pose_errors");
 #define FP_CUDA_OK(expr)                                                                   \
   do {                                                                                     \
     cudaError_t _e = (expr);                                                               \

@@ -54,7 +54,9 @@ def _proto():
     lib.fp_register.argtypes = [vp, vp, i, i, vp, vp, vp, vp]
     lib.fp_op_refine_net.argtypes = [vp, vp, i, vp, vp, vp]
     lib.fp_op_score_feats.argtypes = [vp, vp, i, vp, vp]
-    lib.fp_op_tokens.argtypes = [vp, i, vp, i, vp, vp]
+    lib.fp_op_encoder.argtypes = [vp, i, vp, i, i, vp, vp]
+    lib.fp_op_encoder.restype = C.c_longlong
+    lib.fp_op_encoder_layer.argtypes = [i, i, C.POINTER(i)]
     lib.fp_op_depth_filter.argtypes = [vp, vp, i, i, i, vp]
     lib.fp_op_pose_update.argtypes = [vp, vp, vp, vp, C.POINTER(i), i, vp, vp, vp, vp]
     lib.fp_vis.argtypes = [vp, i, vp, vp, i, vp, vp, C.POINTER(i), vp]
@@ -66,7 +68,7 @@ def _proto():
     for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_track_cameras", "fp_register_objects", "fp_register_cameras", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh",
                  "fp_set_mesh_slot", "fp_set_frame",
                  "fp_get_depth", "fp_make_crops", "fp_start_poses", "fp_refine", "fp_score", "fp_score_features", "fp_score_tail",
-                 "fp_op_score_tail_segments", "fp_register", "fp_op_refine_net", "fp_op_score_feats", "fp_op_tokens", "fp_op_depth_filter",
+                 "fp_op_score_tail_segments", "fp_register", "fp_op_refine_net", "fp_op_score_feats", "fp_op_encoder_layer", "fp_op_depth_filter",
                  "fp_op_pose_update", "fp_vis", "fp_vis_size", "fp_vis_colormap", "fp_vis_crops"):
         getattr(lib, name).restype = C.c_int
 
@@ -98,19 +100,23 @@ def _bn_of(sd, prefix):
             "running_var": sd[f"{prefix}.running_var"], "eps": 1e-5}
 
 
+def encoder_convs(kind):
+    """State-dict prefixes (convolution, batch norm) of encoder layers 0..14, packed as "enc.<layer>.w" / ".b"."""
+    A, AB = ("encodeA", "encodeAB") if kind == "refine" else ("encoderA", "encoderAB")
+    return [(f"{A}.0.net.0", f"{A}.0.net.1"), (f"{A}.1.net.0", f"{A}.1.net.1"),
+            (f"{A}.2.conv1", f"{A}.2.bn1"), (f"{A}.2.conv2", f"{A}.2.bn2"),
+            (f"{A}.3.conv1", f"{A}.3.bn1"), (f"{A}.3.conv2", f"{A}.3.bn2"),
+            (f"{AB}.0.conv1", f"{AB}.0.bn1"), (f"{AB}.0.conv2", f"{AB}.0.bn2"),
+            (f"{AB}.1.conv1", f"{AB}.1.bn1"), (f"{AB}.1.conv2", f"{AB}.1.bn2"),
+            (f"{AB}.2.net.0", f"{AB}.2.net.1"),
+            (f"{AB}.3.conv1", f"{AB}.3.bn1"), (f"{AB}.3.conv2", f"{AB}.3.bn2"),
+            (f"{AB}.4.conv1", f"{AB}.4.bn1"), (f"{AB}.4.conv2", f"{AB}.4.bn2")]
+
+
 def pack_network(sd, kind):
     """Reference state_dict (learning/models/{refine,score}_network.py layout) -> {name: np.ndarray}."""
-    A, AB = ("encodeA", "encodeAB") if kind == "refine" else ("encoderA", "encoderAB")
-    convs = [(f"{A}.0.net.0", f"{A}.0.net.1"), (f"{A}.1.net.0", f"{A}.1.net.1"),
-             (f"{A}.2.conv1", f"{A}.2.bn1"), (f"{A}.2.conv2", f"{A}.2.bn2"),
-             (f"{A}.3.conv1", f"{A}.3.bn1"), (f"{A}.3.conv2", f"{A}.3.bn2"),
-             (f"{AB}.0.conv1", f"{AB}.0.bn1"), (f"{AB}.0.conv2", f"{AB}.0.bn2"),
-             (f"{AB}.1.conv1", f"{AB}.1.bn1"), (f"{AB}.1.conv2", f"{AB}.1.bn2"),
-             (f"{AB}.2.net.0", f"{AB}.2.net.1"),
-             (f"{AB}.3.conv1", f"{AB}.3.bn1"), (f"{AB}.3.conv2", f"{AB}.3.bn2"),
-             (f"{AB}.4.conv1", f"{AB}.4.bn1"), (f"{AB}.4.conv2", f"{AB}.4.bn2")]
     out = {}
-    for i, (cname, bname) in enumerate(convs):
+    for i, (cname, bname) in enumerate(encoder_convs(kind)):
         w = sd[f"{cname}.weight"]
         if i == 0 and w.shape[1] > 8:
             raise ValueError("stem convolution supports c_in <= 8 (reference configs use 6)")
@@ -589,10 +595,21 @@ class Engine:
         _lib.check(lib.fp_op_score_feats(self._h, _p(crops), N, _p(feats), _stream()), "fp_op_score_feats")
         return feats
 
+    def op_encoder(self, kind, crops, N, last=14):
+        """fp_op_encoder: encoder layers 0..last of network `kind` on the crops ((2N, *CROP_SHAPE) fp16 CUDA) -> layer
+        last's whole output buffer, fp16 NHWC (images, H, W, C) as encoder_layer(last, N)["out_shape"]: all Np + N
+        images for layers 0-4, (N, 40, 40, 256) for layer 5, the tokens (N, 20, 20, 512) for layer 14."""
+        out = torch.empty(*encoder_layer(last, N)["out_shape"], dtype=torch.float16, device="cuda")
+        if N == 0:
+            return out
+        rc = lib.fp_op_encoder(self._h, 0 if kind == "refine" else 1, _p(crops), int(N), int(last), _p(out), _stream())
+        _lib.check(rc if rc < 0 else 0, "fp_op_encoder")
+        assert rc == out.numel() * out.element_size(), f"fp_op_encoder copied {rc} bytes into a {tuple(out.shape)} buffer"
+        return out
+
     def op_tokens(self, kind, crops, N):
-        tok = torch.empty(N, 400, 512, dtype=torch.float16, device="cuda")
-        _lib.check(lib.fp_op_tokens(self._h, 0 if kind == "refine" else 1, _p(crops), N, _p(tok), _stream()), "fp_op_tokens")
-        return tok
+        """The encoder's tokens, fp16 (N, 400, 512): op_encoder(kind, crops, N) with the 20 x 20 token grid flattened."""
+        return self.op_encoder(kind, crops, N).reshape(N, 400, 512)
 
 
 def vis_size(kind, N):
@@ -600,6 +617,17 @@ def vis_size(kind, N):
     hw = (C.c_int * 2)()
     _lib.check(lib.fp_vis_size(0 if kind == "refine" else 1, int(N), hw), "fp_vis_size")
     return hw[0], hw[1]
+
+
+def encoder_layer(k, N):
+    """Encoder layer k (0..14) at N hypotheses, from the layer table run_encoder runs (no GPU needed): dict(kind,
+    n_img (images the layer launches on), H (input height = width), Cin, Cout, src (the layer whose output is its
+    input, -1 = the crops), res (the layer whose output it adds, -1 = none), out_split, pe (adds the positional
+    embedding), out_shape (images, H, W, C) of its output buffer)."""
+    info = (C.c_int * 13)()
+    _lib.check(lib.fp_op_encoder_layer(int(k), int(N), info), "fp_op_encoder_layer")
+    return dict(kind=info[0], n_img=info[1], H=info[2], Cin=info[3], Cout=info[4], src=info[5], res=info[6],
+                out_split=info[7], pe=bool(info[8]), out_shape=tuple(info[9:13]))
 
 
 def vis_colormap():

@@ -382,7 +382,20 @@ int fp_group_register(fp_group* g, const unsigned char* rgb_host, const float* d
 /* parity-test hooks on pre-built crops (fp16 [2N][166][2][84][8], device) */
 int fp_op_refine_net(fp_ctx* ctx, const void* crops, int N, float* trans_out, float* rot_out, void* stream);
 int fp_op_score_feats(fp_ctx* ctx, const void* crops, int N, float* feats_out, void* stream);
-int fp_op_tokens(fp_ctx* ctx, int which, const void* crops, int N, void* tokens_out, void* stream);
+/* The encoder's 15 convolutions, one layer table for the product and these hooks.  N hypotheses, 0 <= N <= 512; the
+ * A and B crops run as one batch of M = Np + N images, B from image Np = N rounded up to 4 (images N .. Np - 1 are
+ * pads, never read by layer 6 on).
+ * fp_op_encoder_layer (no GPU needed): layer `layer` (0 .. 14) at N into info[13] = {kind (fp_gemm_layer_t), launch
+ * images, input height = width, Cin, Cout, the layer whose output is its input (-1: the crops), the layer whose output
+ * is its residual (-1: none), out_split, adds the positional embedding (0 / 1), then the shape of its output buffer
+ * (images, height, width, channels)}.  Layers 0-4 keep all M images; layer 5 writes N images of [A_i | B_{Np+i}]
+ * (256 channels); layer 14's output is the tokens [N][20 x 20][512]. */
+int fp_op_encoder_layer(int layer, int N, int* info);
+/* Runs layers 0 .. last (0 .. 14) of network `which` (0 = refiner, 1 = scorer) on the crops (device, [2N] images as
+ * fp_op_refine_net) and copies layer last's whole output buffer, fp16 NHWC of the shape fp_op_encoder_layer gives,
+ * to `out` (device).  Returns the bytes copied, or a negative error code; every argument is checked before anything
+ * is enqueued on `stream`. */
+long long fp_op_encoder(fp_ctx* ctx, int which, const void* crops, int N, int last, void* out, void* stream);
 /* Host-only hook (no GPU needed) on the mesh preparation fp_set_mesh performs: meshlets of <= 64 triangles / <= 64
  * vertices + closedness / orientation analysis.  info[6] = {meshlets, closed (0/1), front-face winding sign (0 = none),
  * max triangles per meshlet, max vertices per meshlet, total triangles}; face_of_tri_out (optional, [F]) receives the

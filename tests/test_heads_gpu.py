@@ -318,20 +318,20 @@ HEADS_BAR = {"trans": 1.2e-5, "rot": 1.2e-5, "feats": 3e-3}
 @pytest.mark.parametrize("N", [67, 252])
 def test_heads_at_product_n(N, heads_engine):
     """fp_op_refine_net / fp_op_score_feats at N = 252 (the refiner's heads one after the other) and N = 67 (heads
-    forked onto two streams) against oracle.nets' heads run in float64 on the tokens fp_op_tokens returns for the same
+    forked onto two streams) against oracle.nets' heads run in float64 on the tokens fp_op_encoder returns for the same
     crops.  This isolates the glue at product N: the 3072-wide in_proj, the group offsets of run_refine_heads and the
     out_proj -> LayerNorm -> feed-forward -> LayerNorm chain with its fp16 intermediates.  Bars: absolute, HEADS_BAR.
     Probe: a reference whose rot head is fed the trans head's attention output (the rot head's in_proj replaced by the
     trans head's) must fail on more than half of the rot outputs."""
     e, sds = heads_engine
     crops = _random_crops(N, 40 + N)
-    tok = e.op_tokens("refine", crops, N)
+    tok = e.op_encoder("refine", crops, N).reshape(N, 400, 512)
     trans, rot = e.op_refine_net(crops, N)
     sd = sds["refine"]
     ref_t, ref_r = _refine_heads_reference(tok, sd)
     err_t = (trans.double() - ref_t).abs().max().item()
     err_r = (rot.double() - ref_r).abs().max().item()
-    tok_s = e.op_tokens("score", crops, N)
+    tok_s = e.op_encoder("score", crops, N).reshape(N, 400, 512)
     feats = e.op_score_feats(crops, N)
     ref_f = _score_feats_reference(tok_s, sds["score"])
     err_f = (feats.double() - ref_f).abs().max().item()

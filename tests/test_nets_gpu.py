@@ -43,7 +43,7 @@ def test_refine_tokens(engine):
 
     e, sd_r, _ = engine
     A, B = _crops(3, 11)
-    tok = e.op_tokens("refine", crops_from_planar(A.cuda(), B.cuda()), 3).float().cpu()
+    tok = e.op_encoder("refine", crops_from_planar(A.cuda(), B.cuda()), 3).reshape(3, 400, 512).float().cpu()
     # oracle sees the same fp16-rounded inputs
     A16, B16 = A.half().float(), B.half().float()
     x = nets.encode_a(torch.cat([A16, B16], 0), sd_r, "encodeA")

@@ -34,7 +34,7 @@ def main():
     cb = crops_from_planar(A.cuda(), B.cuda())
     A16, B16 = A.half().float(), B.half().float()
 
-    tok = e.op_tokens("refine", cb, n).float().cpu()
+    tok = e.op_encoder("refine", cb, n).reshape(n, 400, 512).float().cpu()
     x = nets.encode_a(torch.cat([A16, B16], 0), sd_r, "encodeA")
     ab = nets.encode_ab(torch.cat((x[:n], x[n:]), 1), sd_r, "encodeAB")
     ref_tok = nets._tokens(ab, sd_r)

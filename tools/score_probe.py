@@ -86,7 +86,7 @@ def outliers():
     ref_depth_f = geometry.bilateral_filter_depth(geometry.erode_depth(depth))
     A, B, _ = pipeline.make_crops(poses[worst], mt, rgb, ref_depth_f, None, synth.DEFAULT_K, d, 1)
     cb = crops_from_planar(A.cuda(), B.cuda())
-    tok = e.op_tokens("score", cb, len(worst)).float().cpu()
+    tok = e.op_encoder("score", cb, len(worst)).reshape(len(worst), 400, 512).float().cpu()
     x = nets.encode_a(torch.cat([A, B], 0), sd_s, "encoderA")
     ab = nets.encode_ab(torch.cat((x[:len(worst)], x[len(worst):]), 1), sd_s, "encoderAB")
     ref_tok = nets._tokens(ab, sd_s)
