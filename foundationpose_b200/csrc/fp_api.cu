@@ -129,12 +129,14 @@ struct MeshSlot {
   float diameter = 0.f;
 };
 
-// One camera's frame: the raw upload, the filtered frame (rgba, depth, xyz) and the pinned staging of the upload.
-// Camera 0 is the context's frame, the one every single-frame entry point reads (see alloc_camera).
+// One camera's frame: the raw upload, the filtered frame (rgba, depth, xyz) and the pinned staging of the upload, and
+// the size and intrinsics of the frame the last call prepared in this camera.  Camera 0 is the context's frame, the one
+// every single-frame entry point reads (see alloc_camera).  camera_dev() makes the kernels' record of it.
 struct CameraBufs {
   DevBuf rgb_raw, depth_raw, rgba, depth, xyz;
   PinnedBuf stage_rgb, stage_depth;
-  int H = 0, W = 0;  // the frame the last call prepared in this camera (fp_get_depth)
+  int H = 0, W = 0;
+  float fx = 0.f, fy = 0.f, cx = 0.f, cy = 0.f;
 };
 
 }  // namespace fp
@@ -150,10 +152,8 @@ struct fp_ctx {
   fp::DevBuf mesh_table;
   float rot_normalizer = 0.3490658503988659f;
   float crop_ratio[2] = {1.2f, 1.2f};  // per predictor: each reads its own config.yml (predict_pose_refine.py:117, predict_score.py:137)
-  // frames: cam[0] is the context's frame, cameras 1.. those of the multi-camera calls; K / H / W are camera 0's
+  // frames: cam[0] is the context's frame, cameras 1.. those of the multi-camera calls
   fp::CameraBufs cam[fp::kMaxCameras];
-  float K[9] = {0};
-  int H = 0, W = 0;
   int n_frames = 0;  // the last call prepared the frames of cameras 0 .. n_frames - 1
   bool has_frame = false;
   // workspaces (sized for cap_n hypotheses)
@@ -164,12 +164,11 @@ struct fp_ctx {
   float fold_c = 0.f;      // linear.weight . out_proj.bias + linear.bias (by-value kernel parameter)
   fp::DevBuf fold_v, tail_counter;  // out_proj^T linear.weight [512]; arg-max ticket
   // CUDA graphs of the launch-bound inner loops, keyed by (kind, N, iterations, frame source: see run_graphed).
-  // K / H / W: the frame geometry a graph that passes it by value was captured with
+  // frame: camera 0's record when the graph was captured (read by a graph that takes the frame by value)
   struct GraphEntry {
     cudaGraphExec_t exec = nullptr;
     unsigned long long epoch = 0;
-    float K[9] = {0};
-    int H = 0, W = 0;
+    fp::CameraDev frame{};
   };
   std::map<std::tuple<int, int, int, int>, GraphEntry> graphs;
   std::map<std::tuple<int, int, int, int>, int> graph_nodes;
@@ -506,6 +505,24 @@ static int write_mesh_table(fp_ctx* c) {
   return 0;
 }
 
+// Camera i's frame as the kernels read it: the by-value frame (camera 0) or camera i's entry of the camera table
+static CameraDev camera_dev(const fp_ctx* c, int i) {
+  const CameraBufs& b = c->cam[i];
+  CameraDev e;
+  e.rgb_raw = static_cast<const unsigned char*>(b.rgb_raw.p);
+  e.depth_raw = static_cast<const float*>(b.depth_raw.p);
+  e.rgb = static_cast<uchar4*>(b.rgba.p);
+  e.depth = static_cast<float*>(b.depth.p);
+  e.xyz_map = static_cast<float4*>(b.xyz.p);
+  e.fx = b.fx;
+  e.fy = b.fy;
+  e.cx = b.cx;
+  e.cy = b.cy;
+  e.H = b.H;
+  e.W = b.W;
+  return e;
+}
+
 // mesh_of: [N] device slot ids (validated by the caller), or null = every hypothesis renders slot 0.  cams / camera_of:
 // device camera table and [N] camera ids (the tracking calls, fp_register_cameras), or null = the context's frame
 // (camera 0), by value
@@ -518,19 +535,11 @@ static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg
   CropParams p;
   p.poses = poses;
   p.N = N;
-  p.fx = c->K[0];
-  p.fy = c->K[4];
-  p.cx = c->K[2];
-  p.cy = c->K[5];
-  p.H = c->H;
-  p.W = c->W;
+  p.frame = camera_dev(c, 0);
   p.znear = 0.001f;  // Utils.py:161
   p.zfar = 100.f;
   p.slots = reinterpret_cast<const MeshSlotDev*>(c->mesh_table.p);
   p.mesh_of = mesh_of;
-  p.rgb = reinterpret_cast<const uchar4*>(c->cam[0].rgba.p);
-  p.xyz_map = reinterpret_cast<const float4*>(c->cam[0].xyz.p);
-  p.depth = reinterpret_cast<const float*>(c->cam[0].depth.p);
   p.mode = mode;
   p.crops = reinterpret_cast<__half*>(c->crops.p);
   p.b_img0 = b_img0_of(N);
@@ -560,8 +569,10 @@ enum class GraphKind {
 // calls per register(), which is what bounds track_one() and small per-GPU shards.  The body never allocates:
 // callers size every workspace first, so a capture after an epoch bump (new mesh, new N) is safe.
 // frame: where the body's kernels take their frame from, the last element of the key.  -1 (the single-object calls,
-// fp_register_objects): the context's K / H / W by value; such a graph is captured again when they differ from its
-// capture's, and only that graph: a frame of another size or other intrinsics does not invalidate the others.  0 or
+// fp_register_objects): camera 0's record (CameraDev) by value; such a graph is captured again when the record differs
+// from its capture's, and only that graph: a frame of another size or other intrinsics does not invalidate the others.
+// The record holds fx fy cx cy, the only entries of K a kernel reads, so a K that differs only in its skew or bottom
+// row replays the graph.  Its buffer addresses change only with the epoch.  0 or
 // more (the tracking calls, fp_register_cameras): the camera table, which holds every camera's size and intrinsics, so
 // new intrinsics or a smaller frame replay the graph; the tracking calls pass their number of cameras C, which their
 // frame-preparation launch covers, fp_register_cameras' passes 0 (their frames are prepared before the passes).
@@ -575,7 +586,8 @@ static int run_graphed(fp_ctx* c, GraphKind kind, int N, int iters, cudaStream_t
     return body(st);
   }
   fp_ctx::GraphEntry& g = it->second;
-  const bool frame_moved = frame < 0 && (g.H != c->H || g.W != c->W || memcmp(g.K, c->K, sizeof g.K) != 0);
+  const CameraDev frame0 = camera_dev(c, 0);
+  const bool frame_moved = frame < 0 && memcmp(&g.frame, &frame0, sizeof frame0) != 0;
   if (g.exec == nullptr || g.epoch != c->epoch || frame_moved) {
     if (g.exec) {
       cudaGraphExecDestroy(g.exec);
@@ -614,9 +626,7 @@ static int run_graphed(fp_ctx* c, GraphKind kind, int N, int iters, cudaStream_t
     cudaGraphDestroy(graph);
     FP_CUDA_OK(ie);
     g.epoch = c->epoch;
-    memcpy(g.K, c->K, sizeof g.K);
-    g.H = c->H;
-    g.W = c->W;
+    g.frame = frame0;
     c->graph_nodes[key] = (int)n_kernels;
     ++c->graph_captures;
   }
@@ -637,22 +647,20 @@ struct DeviceGuard {
   }
 };
 
-// camera 0's filtered frame from rgb_dev / depth_dev, with the context's K / H / W by value (fp_set_frame, fp_track)
+// camera 0's filtered frame from rgb_dev / depth_dev, with camera 0's record by value (fp_set_frame, fp_track)
 static int set_frame_launches(fp_ctx* c, const unsigned char* rgb_dev, const float* depth_dev, int flags, float zfar,
                               cudaStream_t st) {
-  const int H = c->H, W = c->W;
-  const size_t npix = (size_t)H * W;
-  CameraBufs& f = c->cam[0];
-  uchar4* rgba = reinterpret_cast<uchar4*>(f.rgba.p);
-  float* depth = reinterpret_cast<float*>(f.depth.p);
-  float4* xyz = reinterpret_cast<float4*>(f.xyz.p);
+  CameraDev one = camera_dev(c, 0);
+  one.rgb_raw = rgb_dev;  // camera 0's upload buffers, or the caller's device frame (FP_FRAME_ON_DEVICE)
+  one.depth_raw = depth_dev;
   if (flags & FP_FRAME_FILTER_DEPTH) {
     // estimater.py:173-174 erode_depth(radius=2), bilateral_filter_depth(radius=2); :214 depth2xyzmap: one launch
-    return frame_prep_launch(rgb_dev, depth_dev, rgba, depth, xyz, H, W, c->K[0], c->K[4], c->K[2], c->K[5], zfar, st);
+    return frame_prep_launch(one, zfar, st);
   }
-  FP_TRY(rgb_to_rgba_launch(rgb_dev, rgba, (int)npix, st));
-  FP_CUDA_OK(cudaMemcpyAsync(depth, depth_dev, npix * 4, cudaMemcpyDeviceToDevice, st));
-  return depth_to_xyz_launch(depth, xyz, H, W, c->K[0], c->K[4], c->K[2], c->K[5], zfar, st);
+  const size_t npix = (size_t)one.H * one.W;
+  FP_TRY(rgb_to_rgba_launch(rgb_dev, one.rgb, (int)npix, st));
+  FP_CUDA_OK(cudaMemcpyAsync(one.depth, depth_dev, npix * 4, cudaMemcpyDeviceToDevice, st));
+  return depth_to_xyz_launch(one, zfar, st);
 }
 
 // Sizes camera i's buffers for npix pixels: the filtered frame always, the raw upload if `raw`, its pinned staging if
@@ -677,15 +685,16 @@ static int alloc_camera(fp_ctx* c, int i, size_t npix, bool raw, bool staged) {
   return 0;
 }
 
-// records K / H / W as the context's frame geometry (a graph that holds them by value is captured again when they
-// change, see run_graphed)
-static void set_frame_geometry(fp_ctx* c, const float* K, int H, int W) {
-  for (int i = 0; i < 9; ++i) c->K[i] = K[i];
-  c->H = H;
-  c->W = W;
-  c->n_frames = 1;
-  c->cam[0].H = H;
-  c->cam[0].W = W;
+// records camera i's frame size and intrinsics (K: [3][3] row-major).  Camera 0's are the context's frame geometry: a
+// graph that holds them by value is captured again when they change, see run_graphed
+static void set_frame_geometry(fp_ctx* c, int i, const float* K, int H, int W) {
+  CameraBufs& b = c->cam[i];
+  b.fx = K[0];
+  b.fy = K[4];
+  b.cx = K[2];
+  b.cy = K[5];
+  b.H = H;
+  b.W = W;
 }
 
 // mesh_of: [N] device slot ids, or null = slot 0 for every hypothesis; cams / camera_of as make_crops
@@ -727,10 +736,11 @@ constexpr size_t kTableBytes = sizeof(CameraDev) * kMaxCameras;  // the camera t
 
 // The cameras of fp_track_cameras / _objects and fp_register_cameras / _objects, before anything reads a frame.  Every
 // camera's buffers are sized for the largest frame of the call (kept at the largest size seen, so a permutation of the
-// same cameras allocates nothing), camera 0's geometry becomes the context's, the argument block is sized for `rows`
-// slot and camera ids and its staging for `staged_rows`, the staging receives the camera table (buffers, size and
-// intrinsics, K: [C][9]; entries C.. zeroed), and every frame is uploaded through its camera's staging (camera i's DMA
-// runs while camera i + 1 is copied on the host).  H_max / W_max: the largest frame height and width of the call.
+// same cameras allocates nothing), the argument block is sized for `rows` slot and camera ids and its staging for
+// `staged_rows`, every camera records its size and intrinsics (K: [C][9]; camera 0's become the context's frame
+// geometry), the staging receives the camera table (every camera's record; entries C.. zeroed), and every frame is
+// uploaded through its camera's staging (camera i's DMA runs while camera i + 1 is copied on the host).  H_max / W_max:
+// the largest frame height and width of the call.
 static int setup_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
                          const float* K, const int* H, const int* W, int rows, int staged_rows, cudaStream_t st,
                          int& H_max, int& W_max) {
@@ -742,27 +752,15 @@ static int setup_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host,
     W_max = std::max(W_max, W[i]);
   }
   for (int i = 0; i < C; ++i) FP_TRY(alloc_camera(c, i, npix_max, /*raw=*/true, /*staged=*/true));
-  set_frame_geometry(c, K, H[0], W[0]);
   c->n_frames = C;
   FP_TRY(dev_alloc(c->epoch, c->args, kTableBytes + (size_t)2 * rows * sizeof(int)));
   FP_TRY(pinned_alloc(nullptr, c->stage_args, kTableBytes + (size_t)2 * staged_rows * sizeof(int)));
   CameraDev* table = reinterpret_cast<CameraDev*>(c->stage_args.p);
   memset(table, 0, kTableBytes);
   for (int i = 0; i < C; ++i) {
-    CameraBufs& b = c->cam[i];
-    CameraDev& e = table[i];
-    e.rgb_raw = reinterpret_cast<const unsigned char*>(b.rgb_raw.p);
-    e.depth_raw = reinterpret_cast<const float*>(b.depth_raw.p);
-    e.rgb = reinterpret_cast<uchar4*>(b.rgba.p);
-    e.depth = reinterpret_cast<float*>(b.depth.p);
-    e.xyz_map = reinterpret_cast<float4*>(b.xyz.p);
-    e.fx = K[9 * i + 0];
-    e.fy = K[9 * i + 4];
-    e.cx = K[9 * i + 2];
-    e.cy = K[9 * i + 5];
-    e.H = b.H = H[i];
-    e.W = b.W = W[i];
-    FP_TRY(upload_staged_frame(b, rgb_host[i], depth_host[i], (size_t)H[i] * W[i], st));
+    set_frame_geometry(c, i, K + 9 * i, H[i], W[i]);
+    table[i] = camera_dev(c, i);
+    FP_TRY(upload_staged_frame(c->cam[i], rgb_host[i], depth_host[i], (size_t)H[i] * W[i], st));
   }
   return 0;
 }
@@ -901,10 +899,11 @@ static int segmented_tail_params(fp_ctx* c, const float* feats, const int* off_h
 //     intrinsics from the table, and the crops take their frame from it: the graphs hold no frame, so reordering
 //     cameras or objects or changing intrinsics replays them.
 //   by_value = true (fp_register_objects, C = 1): the frame filter, the start-pose kernels and the crop producer take
-//     camera 0's frame by value (the single-camera kernel instantiations), as fp_register does.  Kept for speed: at
-//     252 hypotheses the crop producer's camera-table instantiation runs 3.6 % longer (2.76 against 2.67 ms of crops
-//     per one-object call, H100 80GB HBM3 at 700 W), the one camera-table kernel whose cost shows.  Tracking's few
-//     hypotheses show none, so fp_track_objects shares fp_track_cameras' table path.
+//     camera 0's record by value (the single-camera kernel instantiations), as fp_register does, and its graphs are
+//     captured again when that record changes (run_graphed).  Kept for speed: at 252 hypotheses the crop producer's
+//     camera-table instantiation runs 3.6 % longer (2.76 against 2.67 ms of crops per one-object call, H100 80GB HBM3
+//     at 700 W), the one camera-table kernel whose cost shows.  Tracking's few hypotheses show none, so
+//     fp_track_objects shares fp_track_cameras' table path.
 // Both: whole objects in the given order in passes of up to kRegisterPassCap hypotheses (an object above the cap alone),
 // then one segmented scorer tail over all objects.  Synchronises.
 static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
@@ -982,13 +981,9 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
   const int* seg = reinterpret_cast<const int*>(c->seg_off.p);
   const unsigned char* masks_dev = reinterpret_cast<const unsigned char*>(c->mask_buf.p);
   unsigned int* stats = reinterpret_cast<unsigned int*>(c->mask_stats.p);
-  if (by_value) {
-    FP_TRY(start_poses_launch(reinterpret_cast<const float*>(c->cam[0].depth.p), masks_dev, H[0], W[0], c->K[0], c->K[4],
-                              c->K[2], c->K[5], rot_grids_dev, total, M, seg, stats, poses_out_dev, info_out_dev, st));
-  } else {
-    FP_TRY(start_poses_cameras_launch(cams_dev, seg + M + 1, masks_dev, reinterpret_cast<const size_t*>(c->mask_off.p),
-                                      rot_grids_dev, M, seg, stats, poses_out_dev, info_out_dev, st));
-  }
+  const size_t* mask_off = reinterpret_cast<const size_t*>(c->mask_off.p);
+  FP_TRY(start_poses_launch(camera_dev(c, 0), cams_dev, seg + M + 1, masks_dev, mask_off, rot_grids_dev, total, M, seg, stats,
+                            poses_out_dev, info_out_dev, st));
   float* pa = reinterpret_cast<float*>(c->poses_a.p);
   float* pb = reinterpret_cast<float*>(c->poses_b.p);
   float* ps = reinterpret_cast<float*>(c->pose_stage.p);
@@ -1275,7 +1270,8 @@ int fp_set_frame(fp_ctx* c, const unsigned char* rgb, const float* depth, const 
   c->has_frame = false;
   const bool on_dev = (flags & FP_FRAME_ON_DEVICE) != 0;
   FP_TRY(alloc_camera(c, 0, npix, /*raw=*/!on_dev, /*staged=*/false));
-  set_frame_geometry(c, K, H, W);
+  set_frame_geometry(c, 0, K, H, W);
+  c->n_frames = 1;
   const unsigned char* rgb_dev = rgb;
   const float* depth_dev = depth;
   if (!on_dev) {
@@ -1298,7 +1294,8 @@ int fp_set_xyz_map(fp_ctx* c, const float* xyz, void* stream) {
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   // [H][W][3] (host or device) -> the float4-per-pixel layout the crop kernel samples
-  FP_CUDA_OK(cudaMemcpy2DAsync(c->cam[0].xyz.p, 16, xyz, 12, 12, (size_t)c->H * c->W, cudaMemcpyDefault, st));
+  const CameraBufs& f = c->cam[0];
+  FP_CUDA_OK(cudaMemcpy2DAsync(f.xyz.p, 16, xyz, 12, 12, (size_t)f.H * f.W, cudaMemcpyDefault, st));
   return 0;
   FP_API_END
 }
@@ -1330,7 +1327,8 @@ int fp_start_poses(fp_ctx* c, const unsigned char* mask, int mask_on_device, con
   FP_REQUIRE(c->has_frame, "fp_start_poses: no frame (call fp_set_frame first)");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const size_t npix = (size_t)c->H * c->W;
+  const CameraDev frame = camera_dev(c, 0);
+  const size_t npix = (size_t)frame.H * frame.W;
   const unsigned char* mdev = mask;
   if (!mask_on_device) {
     FP_TRY(dev_alloc(c->epoch, c->mask_buf, npix));
@@ -1338,9 +1336,8 @@ int fp_start_poses(fp_ctx* c, const unsigned char* mask, int mask_on_device, con
     mdev = reinterpret_cast<const unsigned char*>(c->mask_buf.p);
   }
   FP_TRY(dev_alloc(c->epoch, c->mask_stats, 64));
-  return start_poses_launch(reinterpret_cast<const float*>(c->cam[0].depth.p), mdev, c->H, c->W, c->K[0], c->K[4], c->K[2],
-                            c->K[5], rot_grid, N, 1, nullptr, reinterpret_cast<unsigned int*>(c->mask_stats.p), poses_out,
-                            info_out, st);
+  return start_poses_launch(frame, nullptr, nullptr, mdev, nullptr, rot_grid, N, 1, nullptr,
+                            reinterpret_cast<unsigned int*>(c->mask_stats.p), poses_out, info_out, st);
   FP_API_END
 }
 
@@ -1577,7 +1574,8 @@ int fp_track(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, 
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   FP_TRY(ensure_capacity(c, 1));
   FP_TRY(alloc_camera(c, 0, (size_t)H * W, /*raw=*/true, /*staged=*/true));
-  set_frame_geometry(c, K, H, W);
+  set_frame_geometry(c, 0, K, H, W);
+  c->n_frames = 1;
   FP_TRY(dev_alloc(c->epoch, c->track_pose, 64));
   FP_TRY(pinned_alloc(&c->epoch, c->stage_pose, 64));  // the graph's read-back node holds this address
   if (pose_in_dev) {

@@ -350,10 +350,10 @@ __device__ __forceinline__ float pixel_ray(float idx_plus_half, float origin, fl
 }
 
 // kCams: the frame comes from the camera table entry of the hypothesis (p.cams[p.camera_of[n]], copied to shared memory
-// next to the mesh entry) instead of the by-value fields.  A template flag rather than a branch, so that the
-// single-camera instantiations compile to the same code as before the camera table existed.
+// next to the mesh entry) instead of the by-value p.frame.  A template flag rather than a branch, so that the
+// single-camera instantiations carry no camera-table code.
 // FRAME(f): field f of the frame this hypothesis is cropped from, read where it is used
-#define FRAME(f) (kCams ? sm.cam.f : p.f)
+#define FRAME(f) (kCams ? sm.cam.f : p.frame.f)
 // kVis: also write the fp32 record of every crop pixel to p.vis (fp_vis, the debug canvases).  A template flag for the
 // same reason: the instantiations without it compile to the same code as before the record existed.
 template <int TILE, bool kStats, bool kCams, bool kVis>
@@ -725,7 +725,7 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
       bb *= (1.f / 255.f);
       // nearest geometry
       const int vn = sm.rown[rl];
-      if (kVis && p.mode == 1 && unc >= 0 && vn >= 0) zb = __ldg(p.depth + (size_t)vn * p.W + unc);
+      if (kVis && p.mode == 1 && unc >= 0 && vn >= 0) zb = __ldg(FRAME(depth) + (size_t)vn * FRAME(W) + unc);
       float X = 0.f, Y = 0.f, Z = 0.f;
       if (unc >= 0 && vn >= 0) {
         if (p.mode == 0) {
@@ -832,19 +832,18 @@ __global__ void rgb_to_rgba_kernel(const unsigned char* __restrict__ rgb, uchar4
   if (i < npix) out[i] = make_uchar4(rgb[3 * i], rgb[3 * i + 1], rgb[3 * i + 2], 255);
 }
 
-__global__ void depth_to_xyz_kernel(const float* __restrict__ depth, float4* __restrict__ xyz, int H, int W, float fx,
-                                    float fy, float cx, float cy, float zfar) {
+__global__ void depth_to_xyz_kernel(const CameraDev one, float zfar) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= H * W) return;
-  const int v = i / W, u = i - v * W;
-  const float z = depth[i];
+  if (i >= one.H * one.W) return;
+  const int v = i / one.W, u = i - v * one.W;
+  const float z = __ldg(one.depth + i);
   float X = 0.f, Y = 0.f, Z = 0.f;
   if (!(z < 0.001f) && !(z > zfar)) {
-    X = ((float)u - cx) * z / fx;
-    Y = ((float)v - cy) * z / fy;
+    X = ((float)u - one.cx) * z / one.fx;
+    Y = ((float)v - one.cy) * z / one.fy;
     Z = z;
   }
-  xyz[i] = make_float4(X, Y, Z, 0.f);
+  one.xyz_map[i] = make_float4(X, Y, Z, 0.f);
 }
 
 int rgb_to_rgba_launch(const unsigned char* rgb, uchar4* out, int npix, cudaStream_t stream) {
@@ -854,9 +853,8 @@ int rgb_to_rgba_launch(const unsigned char* rgb, uchar4* out, int npix, cudaStre
   return 0;
 }
 
-int depth_to_xyz_launch(const float* depth, float4* xyz, int H, int W, float fx, float fy, float cx, float cy,
-                        float zfar, cudaStream_t stream) {
-  depth_to_xyz_kernel<<<(H * W + 255) / 256, 256, 0, stream>>>(depth, xyz, H, W, fx, fy, cx, cy, zfar);
+int depth_to_xyz_launch(const CameraDev& one, float zfar, cudaStream_t stream) {
+  depth_to_xyz_kernel<<<(one.H * one.W + 255) / 256, 256, 0, stream>>>(one, zfar);
   note_launches(1);
   FP_CUDA_OK(cudaGetLastError());
   return 0;

@@ -40,8 +40,7 @@ struct MeshDev {
 constexpr int kMaxMeshes = 64;  // FP_MAX_MESHES (include/fpose.h)
 
 // One entry of the context's device-side mesh table: everything the crop producer and the pose update read about
-// the mesh a hypothesis renders.  The host fills it with the expressions fp_api.cu used for its by-value kernel
-// parameters, so slot 0 reproduces those values bit for bit.
+// the mesh a hypothesis renders, filled by the host from the slot's buffers and the context's crop ratios.
 struct __align__(16) MeshSlotDev {
   MeshDev mesh;       // front_sign already 0 when back-face culling is disabled (FPOSE_NO_CULL)
   const uchar4* tex;  // [Ht][Wt] RGBA8 or null
@@ -54,8 +53,9 @@ struct __align__(16) MeshSlotDev {
 
 constexpr int kMaxCameras = 16;  // FP_MAX_CAMERAS (include/fpose.h)
 
-// One entry of the camera table of the tracking calls and fp_register_cameras: one camera stream's frame buffers
-// (device), size and intrinsics.  frame_prep_kernel reads the raw frame and writes the filtered one; the crop producer reads the filtered one.
+// One camera's frame: its buffers (device), size and intrinsics.  Kernels take it by value (camera 0, the context's
+// frame) or read it from the camera table of the tracking calls and fp_register_cameras.  frame_prep_kernel reads the
+// raw frame and writes the filtered one; the crop producer and the start poses read the filtered one.
 struct __align__(16) CameraDev {
   const unsigned char* rgb_raw;  // [H][W][3] uploaded frame
   const float* depth_raw;        // [H][W]
@@ -70,16 +70,10 @@ static_assert(sizeof(CameraDev) == 64, "camera table entry: four uint4s");
 struct CropParams {
   const float* poses;  // [N][16] row-major ob_in_cam
   int N;
-  float fx, fy, cx, cy;
-  int H, W;
   float znear, zfar; // Utils.py:161 projection_matrix_from_intrinsics(znear=0.001, zfar=100)
   const MeshSlotDev* slots;  // [kMaxMeshes] device mesh table
   const int* mesh_of;        // [N] slot of every hypothesis, device; null = every hypothesis renders slot 0
-  // frame (device)
-  const uchar4* rgb;      // [H][W] RGBA8
-  const float4* xyz_map;  // [H][W] (x, y, z, 0)   (mode 0)
-  const float* depth;     // [H][W]                (mode 1)
-  int mode;               // 0 = refiner crops, 1 = scorer crops
+  int mode;                  // 0 = refiner crops, 1 = scorer crops
   // outputs
   __half* crops;   // [b_img0 + N][166][2][84][8] fp16 (rows x {even, odd columns} x column pairs x 8 channels, the
                    // "EO" layout of fp_stem.cu): images 0..N-1 = rendered (A), b_img0..b_img0+N-1 = observed (B)
@@ -88,11 +82,12 @@ struct CropParams {
   float* win_out;  // optional [N][4] = (left, top, sx, sy)
   int tile_override;  // 0 = pick by batch size; 16 / 32 / 80 = force (fp_set_crop_tile, A/B tests)
   int* stats;      // optional [4]: meshlet visits, triangles set up, fragments, mixed (near-plane) triangles
-  // optional, device: hypothesis n takes its frame (rgba, xyz, filtered depth, fx fy cx cy, H W) from
-  // cams[camera_of[n]] instead of the by-value frame fields above (the tracking calls, fp_register_cameras); both null
-  // or both set
+  // optional, device: hypothesis n takes its frame from cams[camera_of[n]] instead of `frame` (the tracking calls,
+  // fp_register_cameras); both null or both set
   const CameraDev* cams;
   const int* camera_of;
+  // without `cams`, the frame of every hypothesis: rgb, xyz_map (mode 0), depth (mode 1), fx fy cx cy, H W
+  CameraDev frame;
   // optional, single-camera (fp_vis): [N][2][160][160] fp32 record of every crop pixel, A then B: the r, g, b the
   // crops hold (0..1) and one depth value — mode 0 the normalised z of the xyz channels, mode 1 the raw depth in metres
   // (A: rendered camera z, 0 where nothing is covered; B: the nearest sample of the filtered depth, predict_score.py:90)
@@ -101,8 +96,8 @@ struct CropParams {
 
 int crop_launch(const CropParams& p, cudaStream_t stream);
 int rgb_to_rgba_launch(const unsigned char* rgb, uchar4* out, int npix, cudaStream_t stream);
-int depth_to_xyz_launch(const float* depth, float4* xyz, int H, int W, float fx, float fy, float cx, float cy,
-                        float zfar, cudaStream_t stream);
+// one.xyz_map from one.depth (invalid: z < 0.001 or z > zfar)
+int depth_to_xyz_launch(const CameraDev& one, float zfar, cudaStream_t stream);
 
 // Host-side mesh preparation (fp_meshlet.cu): meshlets + closedness / orientation analysis.
 struct MeshHost {

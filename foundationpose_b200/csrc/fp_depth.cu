@@ -148,21 +148,8 @@ __global__ void __launch_bounds__(kFpW* kFpH)
   cam.rgb[i] = make_uchar4(__ldg(cam.rgb_raw + 3 * i), __ldg(cam.rgb_raw + 3 * i + 1), __ldg(cam.rgb_raw + 3 * i + 2), 255);
 }
 
-int frame_prep_launch(const unsigned char* rgb, const float* depth, uchar4* rgba, float* depth_out, float4* xyz, int H, int W,
-                      float fx, float fy, float cx, float cy, float zfar_xyz, cudaStream_t stream) {
-  CameraDev one{};
-  one.rgb_raw = rgb;
-  one.depth_raw = depth;
-  one.rgb = rgba;
-  one.depth = depth_out;
-  one.xyz_map = xyz;
-  one.fx = fx;
-  one.fy = fy;
-  one.cx = cx;
-  one.cy = cy;
-  one.H = H;
-  one.W = W;
-  dim3 block(kFpW, kFpH), grid((W + kFpW - 1) / kFpW, (H + kFpH - 1) / kFpH);
+int frame_prep_launch(const CameraDev& one, float zfar_xyz, cudaStream_t stream) {
+  dim3 block(kFpW, kFpH), grid((one.W + kFpW - 1) / kFpW, (one.H + kFpH - 1) / kFpH);
   frame_prep_kernel<false><<<grid, block, 0, stream>>>(one, nullptr, zfar_xyz);
   note_launches(1);
   FP_CUDA_OK(cudaGetLastError());
@@ -245,22 +232,17 @@ __device__ unsigned int radix_select(const float* __restrict__ depth, const unsi
 // pass 1 (grid-wide, one grid row per object): mask bounding box and pixel counts.  All six statistics are max / sum
 // reductions over values that start at 0 (the box minima are stored mirrored), so one memset of 6 words per object
 // initialises them.  Object m reads masks[m] ([H][W]) and writes stats[6 m, 6 m + 6).
-// kTable (fp_register_cameras): object m is seen by camera camera_of[m] of the device table `cams` and takes its
-// filtered depth and H x W from there; its mask ([H][W] of that camera) starts at byte mask_off[m] of `masks`.  The
-// table arguments follow the by-value ones, so the by-value instantiation reads its parameters where it always did.
+// The filtered depth and H x W come from `one` (by value), or with kTable (fp_register_cameras) from entry camera_of[m]
+// of the device table `cams`; object m's mask ([H][W] of its camera) then starts at byte mask_off[m] of `masks`.
 template <bool kTable>
-__global__ void __launch_bounds__(256) mask_stats_kernel(const float* __restrict__ depth,
-                                                         const unsigned char* __restrict__ masks, int H, int W,
+__global__ void __launch_bounds__(256) mask_stats_kernel(const CameraDev one, const unsigned char* __restrict__ masks,
                                                          unsigned int* __restrict__ stats,
                                                          const CameraDev* __restrict__ cams,
                                                          const int* __restrict__ camera_of,
                                                          const size_t* __restrict__ mask_off) {
-  if (kTable) {
-    const CameraDev& cam = cams[camera_of[blockIdx.y]];
-    depth = cam.depth;
-    H = cam.H;
-    W = cam.W;
-  }
+  const CameraDev cam = kTable ? cams[camera_of[blockIdx.y]] : one;
+  const float* depth = cam.depth;
+  const int H = cam.H, W = cam.W;
   const int npix = H * W;
   const unsigned char* mask = masks + (kTable ? mask_off[blockIdx.y] : (size_t)blockIdx.y * npix);
   stats += 6 * blockIdx.y;
@@ -297,12 +279,11 @@ __global__ void __launch_bounds__(256) mask_stats_kernel(const float* __restrict
 
 // pass 2 (one CTA per object): exact median over the object's bounding box, translation, start poses.  Object m owns
 // rows [off[m], off[m + 1]) of the concatenated rotation grids and start poses (off = null: one object, rows [0, N)),
-// and writes info[4 m, 4 m + 4).  kTable: the object's depth, H x W, fx fy cx cy and mask as in mask_stats_kernel.
+// and writes info[4 m, 4 m + 4).  The object's frame (depth, H x W, fx fy cx cy) and mask as in mask_stats_kernel.
 template <bool kTable>
-__global__ void __launch_bounds__(1024) start_poses_kernel(const float* __restrict__ depth,
-                                                           const unsigned char* __restrict__ masks, int H, int W, float fx,
-                                                           float fy, float cx, float cy, const float* __restrict__ rot_grid,
-                                                           int N, const int* __restrict__ off,
+__global__ void __launch_bounds__(1024) start_poses_kernel(const CameraDev one, const unsigned char* __restrict__ masks,
+                                                           const float* __restrict__ rot_grid, int N,
+                                                           const int* __restrict__ off,
                                                            const unsigned int* __restrict__ stats,
                                                            float* __restrict__ poses_out, float* __restrict__ info,
                                                            const CameraDev* __restrict__ cams,
@@ -312,16 +293,10 @@ __global__ void __launch_bounds__(1024) start_poses_kernel(const float* __restri
   __shared__ unsigned int sh[2];
   __shared__ float tvec[3];
   const int m = blockIdx.x;
-  if (kTable) {
-    const CameraDev& cam = cams[camera_of[m]];
-    depth = cam.depth;
-    H = cam.H;
-    W = cam.W;
-    fx = cam.fx;
-    fy = cam.fy;
-    cx = cam.cx;
-    cy = cam.cy;
-  }
+  const CameraDev cam = kTable ? cams[camera_of[m]] : one;
+  const float* depth = cam.depth;
+  const int H = cam.H, W = cam.W;
+  const float fx = cam.fx, fy = cam.fy, cx = cam.cx, cy = cam.cy;
   const unsigned char* mask = masks + (kTable ? mask_off[m] : (size_t)m * H * W);
   stats += 6 * m;
   info += 4 * m;
@@ -362,27 +337,15 @@ __global__ void __launch_bounds__(1024) start_poses_kernel(const float* __restri
   }
 }
 
-int start_poses_launch(const float* depth, const unsigned char* masks, int H, int W, float fx, float fy, float cx, float cy,
-                       const float* rot_grid, int N, int M, const int* off, unsigned int* stats, float* poses_out,
-                       float* info, cudaStream_t stream) {
-  FP_REQUIRE(M >= 1 && M <= 65535 && (off || M == 1), "start_poses: bad object count %d", M);
+int start_poses_launch(const CameraDev& one, const CameraDev* cams, const int* camera_of, const unsigned char* masks,
+                       const size_t* mask_off, const float* rot_grid, int N, int M, const int* off, unsigned int* stats,
+                       float* poses_out, float* info, cudaStream_t stream) {
+  FP_REQUIRE(M >= 1 && M <= 65535 && (off || (M == 1 && !cams)), "start_poses: bad object count %d", M);
   FP_CUDA_OK(cudaMemsetAsync(stats, 0, (size_t)M * 6 * sizeof(unsigned int), stream));
-  mask_stats_kernel<false><<<dim3(num_sms(), M), 256, 0, stream>>>(depth, masks, H, W, stats, nullptr, nullptr, nullptr);
-  start_poses_kernel<false><<<M, 1024, 0, stream>>>(depth, masks, H, W, fx, fy, cx, cy, rot_grid, N, off, stats, poses_out, info,
-                                                    nullptr, nullptr, nullptr);
-  note_launches(2);
-  FP_CUDA_OK(cudaGetLastError());
-  return 0;
-}
-
-int start_poses_cameras_launch(const CameraDev* cams, const int* camera_of, const unsigned char* masks, const size_t* mask_off,
-                               const float* rot_grid, int M, const int* off, unsigned int* stats, float* poses_out,
-                               float* info, cudaStream_t stream) {
-  FP_REQUIRE(M >= 1 && M <= 65535 && off, "start_poses_cameras: bad object count %d", M);
-  FP_CUDA_OK(cudaMemsetAsync(stats, 0, (size_t)M * 6 * sizeof(unsigned int), stream));
-  mask_stats_kernel<true><<<dim3(num_sms(), M), 256, 0, stream>>>(nullptr, masks, 0, 0, stats, cams, camera_of, mask_off);
-  start_poses_kernel<true><<<M, 1024, 0, stream>>>(nullptr, masks, 0, 0, 0.f, 0.f, 0.f, 0.f, rot_grid, 0, off, stats, poses_out,
-                                                   info, cams, camera_of, mask_off);
+  const auto stats_kernel = cams ? mask_stats_kernel<true> : mask_stats_kernel<false>;
+  const auto poses_kernel = cams ? start_poses_kernel<true> : start_poses_kernel<false>;
+  stats_kernel<<<dim3(num_sms(), M), 256, 0, stream>>>(one, masks, stats, cams, camera_of, mask_off);
+  poses_kernel<<<M, 1024, 0, stream>>>(one, masks, rot_grid, N, off, stats, poses_out, info, cams, camera_of, mask_off);
   note_launches(2);
   FP_CUDA_OK(cudaGetLastError());
   return 0;

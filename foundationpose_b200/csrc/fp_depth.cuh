@@ -9,22 +9,18 @@ int erode_depth_launch(const float* depth, float* out, int H, int W, int radius,
                        float zfar, cudaStream_t stream);
 int bilateral_depth_launch(const float* depth, float* out, int H, int W, int radius, float zfar, float sigmaD,
                            float sigmaR, cudaStream_t stream);
-// erode(2) -> bilateral(2) -> back-projection (invalid: z < 0.001 or z > zfar_xyz) + rgb -> rgba, one launch
-int frame_prep_launch(const unsigned char* rgb, const float* depth, uchar4* rgba, float* depth_out, float4* xyz, int H, int W,
-                      float fx, float fy, float cx, float cy, float zfar_xyz, cudaStream_t stream);
-// the same for C cameras in one launch: cams DEVICE [C] (raw frame in, filtered frame out); max_H x max_W covers the
-// largest of the frames
+// erode(2) -> bilateral(2) -> back-projection (invalid: z < 0.001 or z > zfar_xyz) + rgb -> rgba of one frame, one
+// launch (raw frame in, filtered frame out)
+int frame_prep_launch(const CameraDev& one, float zfar_xyz, cudaStream_t stream);
+// the same for C cameras in one launch: cams DEVICE [C]; max_H x max_W covers the largest of the frames
 int frame_prep_cameras_launch(const CameraDev* cams, int C, int max_H, int max_W, float zfar_xyz, cudaStream_t stream);
-// guess_translation + start poses of M objects in two launches: masks [M][H][W]; off [M + 1] device row offsets of
-// each object in rot_grid / poses_out ([off[M]][16]; null when M = 1: rows [0, N)); stats: 6 M words of device
-// scratch; info [M][4] = {tx, ty, tz, n_valid}
-int start_poses_launch(const float* depth, const unsigned char* masks, int H, int W, float fx, float fy, float cx, float cy,
-                       const float* rot_grid, int N, int M, const int* off, unsigned int* stats, float* poses_out,
-                       float* info, cudaStream_t stream);
-// the same for M objects seen by several cameras (fp_register_cameras): object m takes its filtered depth, H x W and
-// intrinsics from cams[camera_of[m]] (DEVICE table and [M] camera ids) and its mask ([H][W] of that camera) from byte
-// mask_off[m] (DEVICE [M]) of `masks`; off as above, never null
-int start_poses_cameras_launch(const CameraDev* cams, const int* camera_of, const unsigned char* masks, const size_t* mask_off,
-                               const float* rot_grid, int M, const int* off, unsigned int* stats, float* poses_out,
-                               float* info, cudaStream_t stream);
+// guess_translation + start poses of M objects in two launches; off [M + 1] device row offsets of each object in
+// rot_grid / poses_out ([off[M]][16]; null when M = 1 by value: rows [0, N)); stats: 6 M words of device scratch;
+// info [M][4] = {tx, ty, tz, n_valid}.  cams null: every object is seen in frame `one` (filtered depth, H x W,
+// intrinsics) and its mask is masks[m] ([M][H][W]).  Otherwise (fp_register_cameras) object m is seen in
+// cams[camera_of[m]] (DEVICE table and [M] camera ids) and its mask ([H][W] of that camera) starts at byte mask_off[m]
+// (DEVICE [M]) of `masks`; off is then never null
+int start_poses_launch(const CameraDev& one, const CameraDev* cams, const int* camera_of, const unsigned char* masks,
+                       const size_t* mask_off, const float* rot_grid, int N, int M, const int* off, unsigned int* stats,
+                       float* poses_out, float* info, cudaStream_t stream);
 }  // namespace fp
