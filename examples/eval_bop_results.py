@@ -3,6 +3,7 @@ ycbv_res.yml, examples/run_linemod_replicas.py), scored on the GPU.
 
     python examples/eval_bop_results.py --res debug/linemod_res.yml --dataset_dir <LINEMOD root> [--json table.json]
     python examples/eval_bop_results.py --res debug/ycbv_res.yml --dataset_dir <YCB_Video root> [--kind ycbv]
+    python examples/eval_bop_results.py --res debug/linemod_res.yml --dataset_dir <LINEMOD root> --vsd
 
 A result file maps video id -> frame id string -> object id -> 4x4 estimated pose.  The ground truth comes from the
 drop-in readers (`get_gt_pose`), the model points from `get_gt_mesh(ob_id).vertices`; all poses of one object go to
@@ -16,8 +17,16 @@ symmetric objects, d = `get_model_diameter`).
 share of errors below each.  The symmetries are those of `models_info.json` (`reader.symmetry_info_table`) sampled by
 `metrics.bop_symmetries`, K is `reader.get_K(frame)` and the image width that of the video's frames.  The overall row
 scores every pose with its own object's thresholds.  The errors are taken over the same model vertices as the ADD
-columns, not over BOP's resampled `models_eval` points, so they are not comparable with the BOP leaderboard; and as
-VSD is not computed, no combined BOP AR is printed.
+columns, not over BOP's resampled `models_eval` points, so they are not comparable with the BOP leaderboard; and
+without --vsd no combined BOP AR is printed.
+
+--vsd (implies --bop) adds BOP's visible surface discrepancy, scored by `fp_vsd_errors`: the model (`get_gt_mesh`,
+vertices and faces) is rendered at the estimated and at the ground-truth pose against the test depth
+(`reader.get_depth(frame)`) with delta = 15 mm and the step cost at tau = 0.05 d .. 0.50 d.  AR_VSD is the mean over
+every (tau, threshold 0.05 .. 0.50) pair of the share of poses with an error below the threshold, and BOP AR =
+(AR_VSD + AR_MSSD + AR_MSPD) / 3, per object and overall.  A skipped frame counts as a failure for every tau.  The
+renderer follows the crop producer's coverage rule, not bop_toolkit's OpenGL renderer: the two may differ on silhouette
+pixels.  The models_eval caveat of MSSD / MSPD applies to BOP AR as well.
 """
 import argparse
 import json
@@ -93,6 +102,26 @@ def summarize_bop_all(errors, thresholds):
                          (cat([thresholds[o][0] for o in errors]), cat([thresholds[o][1] for o in errors])))
 
 
+VSD_CHUNK = 64  # poses per fp_vsd_errors call: their test depths are on the device together
+
+
+def vsd_chunks(entries, shapes):
+    """Index ranges [lo, hi) of consecutive entries with the same frame size, at most VSD_CHUNK long."""
+    out, lo = [], 0
+    for i in range(1, len(entries) + 1):
+        if i == len(entries) or i - lo == VSD_CHUNK or shapes[i] != shapes[lo]:
+            out.append((lo, i))
+            lo = i
+    return out
+
+
+def summarize_vsd(vsd, mssd_ar, mspd_ar):
+    """AR_VSD of one row from its per-pose errors [n, T] (inf for failures), and the BOP AR with the row's AR_MSSD and
+    AR_MSPD."""
+    ar = metrics.vsd_average_recall(vsd)
+    return {"vsd_ar": ar, "bop_ar": metrics.bop_ar(ar, mssd_ar, mspd_ar)}
+
+
 def make_reader_factory(kind, dataset_dir):
     from datareader import LinemodReader, YcbVideoReader
 
@@ -110,9 +139,11 @@ def make_reader_factory(kind, dataset_dir):
     return reader
 
 
-def evaluate(res, kind, dataset_dir, bop=False):
+def evaluate(res, kind, dataset_dir, bop=False, vsd=False):
     """-> (rows {ob_id: row}, overall row, errors {ob_id: (add [n], adds [n])}).  With `bop`, every row also holds
-    `mssd_ar` and `mspd_ar`, and errors[ob_id] is (add, adds, mssd [n], mspd [n])."""
+    `mssd_ar` and `mspd_ar`, and errors[ob_id] is (add, adds, mssd [n], mspd [n]).  `vsd` implies `bop`: every row
+    also holds `vsd_ar` and `bop_ar`, and errors[ob_id] gains vsd [n, T]."""
+    bop = bop or vsd
     reader = make_reader_factory(kind, dataset_dir)
     rows, errors, thresholds, widths = {}, {}, {}, {}
     for ob_id, entries in group_by_object(res).items():
@@ -139,13 +170,38 @@ def evaluate(res, kind, dataset_dir, bop=False):
             errors[ob_id] = (add, adds, mssd, mspd)
             thresholds[ob_id] = bop_thresholds(r0.get_model_diameter(ob_id), [widths[e[0]] for e in entries])
             rows[ob_id].update(summarize_bop(mssd, mspd, thresholds[ob_id]))
+        if vsd:
+            mesh = r0.get_gt_mesh(ob_id)
+            diameter = r0.get_model_diameter(ob_id)
+            depths = [None if e[3] else reader(e[0]).get_depth(frame[e[0]][e[1]]) for e in entries]
+            shapes = [None if d is None else d.shape for d in depths]
+            err = np.full((len(entries), len(metrics.VSD_TAUS)), np.inf)
+            for lo, hi in vsd_chunks(entries, shapes):
+                if shapes[lo] is None:
+                    continue  # skipped frames: failures for every tau
+                err[lo:hi] = metrics.vsd_errors(mesh.vertices, mesh.faces, pred[lo:hi], gt[lo:hi], np.stack(depths[lo:hi]),
+                                                K[lo:hi], diameter).double().cpu().numpy()
+            errors[ob_id] = errors[ob_id] + (err,)
+            rows[ob_id].update(summarize_vsd(err, rows[ob_id]["mssd_ar"], rows[ob_id]["mspd_ar"]))
     overall = summarize_all(rows, errors) if rows else None
     if bop and rows:
         overall.update(summarize_bop_all(errors, thresholds))
+    if vsd and rows:
+        overall.update(summarize_vsd(np.concatenate([errors[o][4] for o in rows]), overall["mssd_ar"], overall["mspd_ar"]))
     return rows, overall, errors
 
 
-def print_table(rows, overall, bop=False):
+def print_table(rows, overall, bop=False, vsd=False):
+    if vsd:
+        print(f"{'object':>8} {'poses':>6} {'ADD AUC':>8} {'ADD-S AUC':>10} {'ADD(-S)<0.1d':>13} {'AR MSSD':>8} {'AR MSPD':>8} "
+              f"{'AR VSD':>7} {'BOP AR':>7}")
+        for tag, r in [(f"{o}{'*' if r['symmetric'] else ''}", r) for o, r in rows.items()] + ([("all", overall)] if overall else []):
+            print(f"{tag:>8} {r['poses']:6d} {100 * r['add_auc']:8.2f} {100 * r['adds_auc']:10.2f} {100 * r['add_s_recall']:13.2f} "
+                  f"{100 * r['mssd_ar']:8.2f} {100 * r['mspd_ar']:8.2f} {100 * r['vsd_ar']:7.2f} {100 * r['bop_ar']:7.2f}")
+        print("(percent; * = symmetric object, scored by ADD-S in the fifth column; MSSD / MSPD over the model vertices, "
+              "not BOP's models_eval points; VSD with delta = 15 mm and the step cost, rendered with the crop producer's "
+              "coverage rule; BOP AR = mean of the three ARs)")
+        return
     if not bop:
         print(f"{'object':>8} {'poses':>6} {'ADD AUC':>8} {'ADD-S AUC':>10} {'ADD(-S)<0.1d':>13}")
         for ob_id, r in rows.items():
@@ -164,17 +220,28 @@ def print_table(rows, overall, bop=False):
           "not BOP's models_eval points, and without VSD, so there is no BOP AR)")
 
 
-def main(argv=None):
+def make_parser():
     ap = argparse.ArgumentParser()
     ap.add_argument("--res", required=True, help="linemod_res.yml / ycbv_res.yml written by a dataset driver")
     ap.add_argument("--dataset_dir", required=True, help="the --linemod_dir / --ycbv_dir the driver ran on")
     ap.add_argument("--kind", choices=("lm", "ycbv"), default=None, help="default: ycbv if the file name says so, else lm")
     ap.add_argument("--json", default=None, help="also write the table as JSON here")
     ap.add_argument("--bop", action="store_true", help="also BOP's symmetry-aware AR_MSSD and AR_MSPD")
-    opt = ap.parse_args(argv)
+    ap.add_argument("--vsd", action="store_true", help="also BOP's AR_VSD and the combined BOP AR (implies --bop)")
+    return ap
+
+
+def parse_args(argv=None):
+    opt = make_parser().parse_args(argv)
+    opt.bop = opt.bop or opt.vsd
+    return opt
+
+
+def main(argv=None):
+    opt = parse_args(argv)
     kind = opt.kind or ("ycbv" if "ycbv" in os.path.basename(opt.res) else "lm")
-    rows, overall, _ = evaluate(load_results(opt.res), kind, opt.dataset_dir, bop=opt.bop)
-    print_table(rows, overall, bop=opt.bop)
+    rows, overall, _ = evaluate(load_results(opt.res), kind, opt.dataset_dir, bop=opt.bop, vsd=opt.vsd)
+    print_table(rows, overall, bop=opt.bop, vsd=opt.vsd)
     if opt.json:
         with open(opt.json, "w") as fh:
             json.dump({"objects": {str(k): v for k, v in rows.items()}, "overall": overall}, fh, indent=1)

@@ -63,6 +63,10 @@ lib.fp_pose_errors.restype = C.c_int
 lib.fp_sym_pose_errors.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
                                    C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
 lib.fp_sym_pose_errors.restype = C.c_int
+lib.fp_vsd_errors.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
+                              C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_int,
+                              C.c_void_p, C.c_void_p, C.c_void_p]
+lib.fp_vsd_errors.restype = C.c_int
 
 
 def check(rc, what=""):

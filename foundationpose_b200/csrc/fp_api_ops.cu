@@ -16,6 +16,10 @@ int pose_errors_launch(const float* pts, int P, const float* pred, int N, const 
 int sym_pose_errors_launch(const float* pts, int P, const float* pred, int N, const float* gt, int n_gt, const float* sym,
                            int S, const float* K, int n_K, float* mssd_out, float* mspd_out, cudaStream_t stream);
 
+int vsd_errors_launch(const float* pos, int V, const int* faces, int F, const float* pred, int N, const float* gt,
+                      int n_gt, const float* depth, int n_depth, int H, int W, const float* K, int n_K, float delta,
+                      const float* taus, int T, float* errs_out, int* counts_out, cudaStream_t stream);
+
 int check_device_ptr(const void* p, const char* what, const char* fn) {
   int dev = 0;
   FP_CUDA_OK(cudaGetDevice(&dev));
@@ -256,6 +260,46 @@ int fp_sym_pose_errors(const float* pts, int P, const float* pred, int N, const 
     if (ptrs[i] && check_device_ptr(ptrs[i], names[i], "fp_sym_pose_errors")) return -1;
   return fp::sym_pose_errors_launch(pts, P, pred, N, gt, n_gt, sym, S, K, n_K, mssd_out, mspd_out,
                                     reinterpret_cast<cudaStream_t>(stream));
+}
+
+int fp_vsd_errors(const float* pos, int V, const int* faces, int F, const float* pred, int N, const float* gt, int n_gt,
+                  const float* depth, int n_depth, int H, int W, const float* K, int n_K, float delta, const float* taus,
+                  int T, float* errs_out, int* counts_out, void* stream) {
+  const char* fn = "fp_vsd_errors";
+  FP_REQUIRE(V >= 3 && V <= FP_VSD_MAX_VERTICES, "%s: V = %d outside [3, %d]", fn, V, FP_VSD_MAX_VERTICES);
+  FP_REQUIRE(F >= 1 && F <= FP_VSD_MAX_FACES, "%s: F = %d outside [1, %d]", fn, F, FP_VSD_MAX_FACES);
+  FP_REQUIRE(N >= 0 && N <= FP_METRICS_MAX_POSES, "%s: N = %d outside [0, %d]", fn, N, FP_METRICS_MAX_POSES);
+  FP_REQUIRE(n_gt == 1 || n_gt == N, "%s: n_gt = %d, must be 1 or N = %d", fn, n_gt, N);
+  FP_REQUIRE(n_depth == 1 || n_depth == N, "%s: n_depth = %d, must be 1 or N = %d", fn, n_depth, N);
+  FP_REQUIRE(n_K == 1 || n_K == N, "%s: n_K = %d, must be 1 or N = %d", fn, n_K, N);
+  FP_REQUIRE(H >= 1 && H <= FP_VSD_MAX_DIM && W >= 1 && W <= FP_VSD_MAX_DIM, "%s: H x W = %d x %d outside [1, %d]", fn, H,
+             W, FP_VSD_MAX_DIM);
+  FP_REQUIRE(T >= 1 && T <= FP_VSD_MAX_TAUS, "%s: T = %d outside [1, %d]", fn, T, FP_VSD_MAX_TAUS);
+  FP_REQUIRE(delta >= 0.f && delta < INFINITY, "%s: delta = %g must be finite and >= 0", fn, (double)delta);
+  FP_REQUIRE(pos && faces, "%s: null mesh pointer", fn);
+  {
+    // the mesh comes as host arrays: a device pointer here would be read by the host
+    const void* hp[2] = {pos, faces};
+    const char* hn[2] = {"pos", "faces"};
+    for (int i = 0; i < 2; ++i) {
+      cudaPointerAttributes a;
+      if (cudaPointerGetAttributes(&a, hp[i]) != cudaSuccess) {
+        cudaGetLastError();
+        continue;
+      }
+      FP_REQUIRE(a.type != cudaMemoryTypeDevice, "%s: %s is device memory; the mesh is read on the host", fn, hn[i]);
+    }
+  }
+  for (long long i = 0; i < 3LL * F; ++i)
+    FP_REQUIRE(faces[i] >= 0 && faces[i] < V, "%s: faces[%lld] = %d outside [0, %d)", fn, i / 3, faces[i], V);
+  if (N == 0) return 0;
+  FP_REQUIRE(pred && gt && depth && K && taus && errs_out, "%s: null input or output pointer", fn);
+  const void* ptrs[7] = {pred, gt, depth, K, taus, errs_out, counts_out};
+  const char* names[7] = {"pred", "gt", "depth", "K", "taus", "errs_out", "counts_out"};
+  for (int i = 0; i < 7; ++i)
+    if (ptrs[i] && check_device_ptr(ptrs[i], names[i], fn)) return -1;
+  return fp::vsd_errors_launch(pos, V, faces, F, pred, N, gt, n_gt, depth, n_depth, H, W, K, n_K, delta, taus, T,
+                               errs_out, counts_out, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -110,7 +110,8 @@ struct MeshHost {
   int closed = 0;
   float bs[4] = {0.f, 0.f, 0.f, 0.f};  // bounding sphere of the mesh
 };
-// att: [V][2] uv (n_att = 2) or [V][3] colours (n_att = 3).  Returns 0 or a negative error (fp_last_error()).
+// att: [V][2] uv (n_att = 2) or [V][3] colours (n_att = 3).  nrm or att may be null (zeros: geometry only, fp_vsd.cu).
+// Returns 0 or a negative error (fp_last_error()).
 int build_mesh_host(int V, int F, const float* pos, const float* nrm, const float* att, int n_att, const int* faces,
                     MeshHost& out);
 

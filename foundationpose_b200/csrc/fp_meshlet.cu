@@ -63,9 +63,10 @@ int build_mesh_host(int V, int F, const float* pos, const float* nrm, const floa
   out.vatt.resize(V);
   for (int v = 0; v < V; ++v) {
     out.vpos[v] = make_float4(pos[3 * v], pos[3 * v + 1], pos[3 * v + 2], 0.f);
-    out.vnrm[v] = make_float4(nrm[3 * v], nrm[3 * v + 1], nrm[3 * v + 2], 0.f);
-    out.vatt[v] = n_att == 2 ? make_float4(att[2 * v], att[2 * v + 1], 0.f, 0.f)
-                             : make_float4(att[3 * v], att[3 * v + 1], att[3 * v + 2], 0.f);
+    out.vnrm[v] = nrm ? make_float4(nrm[3 * v], nrm[3 * v + 1], nrm[3 * v + 2], 0.f) : make_float4(0.f, 0.f, 0.f, 0.f);
+    out.vatt[v] = !att ? make_float4(0.f, 0.f, 0.f, 0.f)
+                       : n_att == 2 ? make_float4(att[2 * v], att[2 * v + 1], 0.f, 0.f)
+                                    : make_float4(att[3 * v], att[3 * v + 1], att[3 * v + 2], 0.f);
   }
   out.faces.resize(F);
   for (int f = 0; f < F; ++f) out.faces[f] = make_int4(faces[3 * f], faces[3 * f + 1], faces[3 * f + 2], 0);

@@ -1,6 +1,7 @@
 """Pose accuracy: ADD / ADD-S on the GPU (`fp_pose_errors`) and the area-under-curve / recall summaries of
 FoundationPose's evaluation (Utils.py:232-266); BOP's symmetry-aware MSSD / MSPD on the GPU (`fp_sym_pose_errors`) and
-their average recalls.
+their average recalls; BOP's visible surface discrepancy on the GPU (`fp_vsd_errors`), its average recall and the
+combined BOP AR.
 
     add, adds = pose_errors(model_pts, pred, gt)   # [N] float32 CUDA tensors, metres
     auc(adds.cpu().numpy())                          # AUC of the accuracy-threshold curve up to 0.1 m
@@ -10,6 +11,10 @@ their average recalls.
     mssd, mspd = sym_pose_errors(model_pts, pred, gt, syms, K)   # [N] float32 CUDA tensors, metres / pixels
     average_recall(mssd, mssd_thresholds(diameter))  # BOP's AR_MSSD
     average_recall(mspd, mspd_thresholds(width))     # BOP's AR_MSPD
+
+    vsd = vsd_errors(vertices, faces, pred, gt, depth, K, diameter)   # [N, 10] float32 CUDA tensor
+    ar_vsd = vsd_average_recall(vsd)                                  # BOP's AR_VSD
+    bop_ar(ar_vsd, ar_mssd, ar_mspd)                                  # (AR_VSD + AR_MSSD + AR_MSPD) / 3
 """
 import math
 import ctypes as C
@@ -181,3 +186,67 @@ def average_recall(errs, thresholds):
     thr = np.asarray(thresholds, dtype=np.float64)
     thr = thr[:, None] if thr.ndim == 1 else thr
     return float(np.mean(errs[None, :] < thr))
+
+
+VSD_TAUS = np.arange(1, 11) * 0.05        # misalignment tolerances x the object diameter: 0.05 d .. 0.50 d
+VSD_THRESHOLDS = np.arange(1, 11) * 0.05  # correctness thresholds on the VSD error: 0.05 .. 0.50
+VSD_DELTA = 0.015                         # visibility tolerance, metres (BOP 2019 for LM / YCB-V)
+
+
+def vsd_errors(vertices, faces, pred, gt, depth, K, diameter, delta=VSD_DELTA, taus=VSD_TAUS, return_counts=False):
+    """BOP's VSD (visib_mode 'bop19', cost 'step') of every pose in `pred` against `gt`, computed by libfpose.so: the
+    mesh is rendered at both poses with the crop producer's coverage rule on the full frame, and
+
+        e_t = (|{visG and visE, |distG - distE| >= tau_t d}| + |visG xor visE|) / |visG or visE|   (1 if nothing is visible)
+
+    vertices: [V, 3] metres, faces: [F, 3] (host data; numpy or torch); pred: [N, 4, 4] or one [4, 4]; gt, depth [H, W]
+    (metres, 0 = no measurement) and K [3, 3]: one for every prediction or one per prediction; diameter in metres,
+    `taus` in diameters, `delta` in metres.  Returns float32 [N, T] on the current CUDA device; with `return_counts`
+    also the int32 [N, T + 2] counts (union, intersection, c_0 .. c_{T-1}).  There is no CPU path: without a CUDA
+    device this raises."""
+    if not torch.cuda.is_available():
+        raise _lib.FposeError("vsd_errors needs a CUDA device (there is no CPU path)")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    pos = np.ascontiguousarray(_host_array(vertices), dtype=np.float32).reshape(-1, 3)
+    fcs = np.ascontiguousarray(_host_array(faces), dtype=np.int32).reshape(-1, 3)
+    pred = _device_f32(pred, dev, 16)
+    gt = _device_f32(gt, dev, 16)
+    depth = torch.as_tensor(depth).to(device=dev, dtype=torch.float32)
+    if depth.dim() == 2:
+        depth = depth[None]
+    depth = depth.contiguous()
+    k = _device_f32(K, dev, 9)
+    tau = torch.as_tensor(np.asarray(taus, dtype=np.float64).reshape(-1) * float(diameter), dtype=torch.float32).to(dev)
+    n, T = pred.shape[0], tau.numel()
+    errs = torch.empty(n, T, dtype=torch.float32, device=dev)
+    counts = torch.empty(n, T + 2, dtype=torch.int32, device=dev) if return_counts else None
+
+    def ptr(t):
+        return None if t is None or t.numel() == 0 else C.c_void_p(t.data_ptr())
+
+    rc = lib.fp_vsd_errors(C.c_void_p(pos.ctypes.data), pos.shape[0], C.c_void_p(fcs.ctypes.data), fcs.shape[0],
+                           ptr(pred), n, ptr(gt), gt.shape[0], ptr(depth), depth.shape[0], depth.shape[1], depth.shape[2],
+                           ptr(k), k.shape[0], float(delta), ptr(tau), T, ptr(errs), ptr(counts),
+                           C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+    _lib.check(rc, "fp_vsd_errors")
+    return (errs, counts) if return_counts else errs
+
+
+def _host_array(x):
+    return x.detach().cpu().numpy() if isinstance(x, torch.Tensor) else np.asarray(x)
+
+
+def vsd_average_recall(errs, thresholds=VSD_THRESHOLDS):
+    """BOP's AR_VSD: the mean over every (tau, threshold) pair of the share of poses with e_tau < threshold.
+    errs: [N, T] (one row per pose, one column per tau)."""
+    if isinstance(errs, torch.Tensor):
+        errs = errs.detach().cpu().numpy()
+    errs = np.asarray(errs, dtype=np.float64)
+    errs = errs.reshape(errs.shape[0], -1) if errs.ndim else errs.reshape(1, 1)
+    thr = np.asarray(thresholds, dtype=np.float64).reshape(-1)
+    return float(np.mean(errs[:, :, None] < thr[None, None, :]))
+
+
+def bop_ar(ar_vsd, ar_mssd, ar_mspd):
+    """The BOP Challenge score of one method: (AR_VSD + AR_MSSD + AR_MSPD) / 3."""
+    return (float(ar_vsd) + float(ar_mssd) + float(ar_mspd)) / 3.0

@@ -140,6 +140,35 @@ int fp_pose_errors(const float* pts, int P, const float* pred, int N, const floa
 int fp_sym_pose_errors(const float* pts, int P, const float* pred, int N, const float* gt, int n_gt, const float* sym,
                        int S, const float* K, int n_K, float* mssd_out, float* mspd_out, void* stream);
 
+/* Limits of fp_vsd_errors.  FP_VSD_MAX_TAUS: misalignment tolerances per call (BOP uses 10); the per-CTA counters
+ * live in shared memory.  FP_VSD_MAX_DIM: largest H and W — BOP's largest test frames (T-LESS Canon, 2560 x 1920) fit,
+ * and 1/256-pixel vertex coordinates stay far inside int.  FP_VSD_MAX_VERTICES / FP_VSD_MAX_FACES: mesh size. */
+#define FP_VSD_MAX_TAUS 64
+#define FP_VSD_MAX_DIM 4096
+#define FP_VSD_MAX_VERTICES (1 << 22)
+#define FP_VSD_MAX_FACES (1 << 22)
+/* VSD of the BOP Challenge (Hodan et al., ECCV Workshops 2016; bop_toolkit's pose_error.vsd with visib_mode 'bop19',
+ * cost_type 'step') of N poses against n_gt (1 or N) ground-truth poses, on the current device.
+ * Mesh: HOST arrays pos [V][3] metres and faces [F][3] int32 (meshlets are built and uploaded per call, stream-ordered).
+ * DEVICE arrays: pred [N][16], gt [n_gt][16] row-major, depth [n_depth][H][W] float32 metres (0 = no measurement),
+ * K [n_K][9] row-major, taus [T] metres, errs_out [N][T] float32, and the optional counts_out [N][T + 2] int32 =
+ * (union, intersection, c_0 .. c_{T-1}); n_gt, n_depth, n_K are 1 or N.  1 <= T <= FP_VSD_MAX_TAUS,
+ * 1 <= H, W <= FP_VSD_MAX_DIM, delta >= 0 and finite (metres).
+ *   dE, dG  depth of the mesh rendered at E and at G (0 where not covered): the crop producer's coverage rule on a full
+ *           frame (pixel (u, v) samples (u + 0.5, v + 0.5); 1/256-px snapping, top-left ties, depth test on 1/Z,
+ *           znear 0.001, zfar 100); an OpenGL renderer may differ on silhouette pixels
+ *   dist    d sqrt(((u - cx) / fx)^2 + ((v - cy) / fy)^2 + 1), integer u, v (BOP's depth_im_to_dist_im_fast), fp64
+ *   visG  = (distG - distT <= delta or D = 0) and dG > 0
+ *   visE  = ((distE - distT <= delta or D = 0) and dE > 0) or (visG and dE > 0)
+ *   c_t   = |{visG and visE, |distG - distE| >= taus[t]}|;  e_t = (c_t + |visG or visE| - |visG and visE|) / |visG or visE|,
+ *           1 when nothing is visible.
+ * Counts are integers: a pose's errors and counts do not depend on N, on broadcasting or on the call.  Every device
+ * pointer must be device memory of the current device; all arguments are checked before anything is enqueued.
+ * Enqueued on `stream`; no sync. */
+int fp_vsd_errors(const float* pos, int V, const int* faces, int F, const float* pred, int N, const float* gt, int n_gt,
+                  const float* depth, int n_depth, int H, int W, const float* K, int n_K, float delta, const float* taus,
+                  int T, float* errs_out, int* counts_out, void* stream);
+
 /* ------------------------------------------------------------------------------------------ */
 /* product path                                                                               */
 /* ------------------------------------------------------------------------------------------ */
