@@ -186,10 +186,8 @@ struct fp_ctx {
   fp::DevBuf lt_buf, lr_buf, feat_buf, pose_stage, tok_mean;
   fp::DevBuf mask_buf, mask_stats, crop_stats;
   fp::DevBuf op_mesh_of;  // fp_op_pose_update: the uploaded slot id of every hypothesis
-  // fp_track: the pose in and out of the graph, and its pinned read-back
-  fp::PinnedBuf stage_pose;
-  fp::DevBuf track_pose;
-  fp::PinnedBuf stage_poses;  // fp_track_objects: pinned [M][16] pose read-back
+  fp::DevBuf track_pose;      // fp_track: the pose it produced last, where pose_in = NULL continues from
+  fp::PinnedBuf stage_poses;  // the tracking calls: pinned [M][16] pose read-back
   // the arguments of a multi-object call or register pass, one device block at a fixed address (a graph holds it) and
   // its pinned staging: the camera table (CameraDev [FP_MAX_CAMERAS]), the slot ids [n], the camera ids [n]
   fp::DevBuf args;
@@ -557,10 +555,9 @@ static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg
 enum class GraphKind {
   Refine = 0,            // fp_refine
   ScoreFeatures = 1,     // fp_score_features
-  Track = 2,             // fp_track
-  TrackObjects = 3,      // fp_track_objects, fp_track_cameras
-  RegisterRefine = 4,    // fp_register_objects / _cameras: one pass's refinement
-  RegisterFeatures = 5,  // fp_register_objects / _cameras: one pass's scorer features
+  TrackObjects = 2,      // fp_track, fp_track_objects, fp_track_cameras
+  RegisterRefine = 3,    // fp_register_objects / _cameras: one pass's refinement
+  RegisterFeatures = 4,  // fp_register_objects / _cameras: one pass's scorer features
 };
 
 // Runs `body(stream)` — a fixed sequence of kernel launches (and fixed-address copies) on ctx-owned buffers —
@@ -568,7 +565,7 @@ enum class GraphKind {
 // captures + instantiates, later calls replay.  Replay removes ~170 launch + 60 tensor-map-encode host
 // calls per register(), which is what bounds track_one() and small per-GPU shards.  The body never allocates:
 // callers size every workspace first, so a capture after an epoch bump (new mesh, new N) is safe.
-// frame: where the body's kernels take their frame from, the last element of the key.  -1 (the single-object calls,
+// frame: where the body's kernels take their frame from, the last element of the key.  -1 (fp_refine, fp_score_features,
 // fp_register_objects): camera 0's record (CameraDev) by value; such a graph is captured again when the record differs
 // from its capture's, and only that graph: a frame of another size or other intrinsics does not invalidate the others.
 // The record holds fx fy cx cy, the only entries of K a kernel reads, so a K that differs only in its skew or bottom
@@ -647,7 +644,7 @@ struct DeviceGuard {
   }
 };
 
-// camera 0's filtered frame from rgb_dev / depth_dev, with camera 0's record by value (fp_set_frame, fp_track)
+// camera 0's filtered frame from rgb_dev / depth_dev, with camera 0's record by value (fp_set_frame, fp_register_objects)
 static int set_frame_launches(fp_ctx* c, const unsigned char* rgb_dev, const float* depth_dev, int flags, float zfar,
                               cudaStream_t st) {
   CameraDev one = camera_dev(c, 0);
@@ -765,14 +762,16 @@ static int setup_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host,
   return 0;
 }
 
-// fp_track_cameras and fp_track_objects (C = 1) after validation.  The camera table, the slot ids and the camera ids go
-// to the argument block in one copy ahead of the launch.  The graph holds the block's address, not the frames' sizes,
-// intrinsics or buffers, and is keyed on (M, iterations, C): reordering objects or cameras, new intrinsics or a smaller
-// frame replay it.  One frame_prep_kernel launch filters every camera and the crops take their frame from the table.
+// fp_track_cameras, fp_track_objects (C = 1) and fp_track (C = M = 1) after validation.  The camera table, the slot ids
+// and the camera ids go to the argument block in one copy ahead of the launch.  The graph holds the block's address, not
+// the frames' sizes, intrinsics or buffers, and is keyed on (M, iterations, C): reordering objects or cameras, new
+// intrinsics or a smaller frame replay it.  One frame_prep_kernel launch filters every camera and the crops take their
+// frame from the table.  poses_out_dev, poses_keep_dev (fp_track's continuation pose) and poses_out_host are optional;
+// the device copies are complete when the call returns.
 static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
                               const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
                               const float* poses_in_dev, int iterations, float* poses_out_dev, float* poses_out_host,
-                              cudaStream_t st) {
+                              cudaStream_t st, float* poses_keep_dev = nullptr) {
   FP_TRY(ensure_capacity(c, M));
   FP_TRY(pinned_alloc(&c->epoch, c->stage_poses, (size_t)M * 64));  // the graph's read-back node holds this address
   c->has_frame = false;
@@ -811,6 +810,7 @@ static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_
   FP_TRY(run_graphed(c, GraphKind::TrackObjects, M, iterations, st, body, C));
   c->has_frame = true;
   if (poses_out_dev) FP_CUDA_OK(cudaMemcpyAsync(poses_out_dev, fin, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
+  if (poses_keep_dev) FP_CUDA_OK(cudaMemcpyAsync(poses_keep_dev, fin, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
   FP_CUDA_OK(cudaStreamSynchronize(st));
   if (poses_out_host) memcpy(poses_out_host, c->stage_poses.p, (size_t)M * 64);
   return 0;
@@ -1570,41 +1570,16 @@ int fp_track(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, 
   FP_REQUIRE(c && rgb_host && depth_host && K && H > 0 && W > 0 && iterations >= 0, "fp_track: bad argument");
   FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
   FP_REQUIRE(c->mesh[0].loaded, "fp_track: no mesh");
+  FP_REQUIRE(pose_in_dev || c->track_valid, "fp_track: no previous pose in this context: pass pose_in");
   DeviceGuard dg(c->device);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(ensure_capacity(c, 1));
-  FP_TRY(alloc_camera(c, 0, (size_t)H * W, /*raw=*/true, /*staged=*/true));
-  set_frame_geometry(c, 0, K, H, W);
-  c->n_frames = 1;
-  FP_TRY(dev_alloc(c->epoch, c->track_pose, 64));
-  FP_TRY(pinned_alloc(&c->epoch, c->stage_pose, 64));  // the graph's read-back node holds this address
-  if (pose_in_dev) {
-    FP_CUDA_OK(cudaMemcpyAsync(c->track_pose.p, pose_in_dev, 64, cudaMemcpyDeviceToDevice, st));
-  } else {
-    FP_REQUIRE(c->track_valid, "fp_track: no previous pose in this context: pass pose_in");
-  }
-  FP_TRY(upload_staged_frame(c->cam[0], rgb_host, depth_host, (size_t)H * W, st));
-  c->has_frame = false;
-  float* pa = reinterpret_cast<float*>(c->poses_a.p);
-  float* pb = reinterpret_cast<float*>(c->poses_b.p);
-  auto body = [&](cudaStream_t s2) -> int {
-    // estimater.py:250-268 in one launch sequence: erode + bilateral, depth2xyzmap_batch(zfar=inf), K refiner passes
-    FP_TRY(set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->cam[0].rgb_raw.p),
-                              reinterpret_cast<const float*>(c->cam[0].depth_raw.p), FP_FRAME_FILTER_DEPTH, INFINITY, s2));
-    FP_CUDA_OK(cudaMemcpyAsync(pa, c->track_pose.p, 64, cudaMemcpyDeviceToDevice, s2));
-    c->has_frame = true;
-    FP_TRY(refine_body(c, 1, iterations, s2));
-    const float* fin = (iterations % 2 == 0) ? pa : pb;
-    FP_CUDA_OK(cudaMemcpyAsync(c->track_pose.p, fin, 64, cudaMemcpyDeviceToDevice, s2));
-    FP_CUDA_OK(cudaMemcpyAsync(c->stage_pose.p, fin, 64, cudaMemcpyDeviceToHost, s2));
-    return 0;
-  };
-  FP_TRY(run_graphed(c, GraphKind::Track, 1, iterations, st, body));
-  c->has_frame = true;
+  unsigned long long no_graph = 0;  // the continuation pose is copied outside the graph
+  FP_TRY(dev_alloc(no_graph, c->track_pose, 64));
+  float* keep = reinterpret_cast<float*>(c->track_pose.p);
+  // fp_track_cameras' one-object, one-camera case: object 0 renders slot 0 in camera 0
+  const int zero = 0;
+  FP_TRY(track_cameras_body(c, 1, &rgb_host, &depth_host, K, &H, &W, 1, &zero, &zero, pose_in_dev ? pose_in_dev : keep,
+                            iterations, pose_out_dev, pose_out_host, reinterpret_cast<cudaStream_t>(stream), keep));
   c->track_valid = true;
-  if (pose_out_dev) FP_CUDA_OK(cudaMemcpyAsync(pose_out_dev, c->track_pose.p, 64, cudaMemcpyDeviceToDevice, st));
-  FP_CUDA_OK(cudaStreamSynchronize(st));
-  if (pose_out_host) memcpy(pose_out_host, c->stage_pose.p, 64);
   return 0;
   FP_API_END
 }

@@ -281,7 +281,12 @@ int fp_register(fp_ctx* ctx, const float* poses_host, int N, int iterations, flo
  * uint8 [H][W][3], depth float32 [H][W]; staged through pinned memory owned by the context), erode_depth +
  * bilateral_filter_depth, depth2xyzmap_batch(zfar = inf), `iterations` refiner passes on ONE pose, pose read-back.
  * pose_in_dev: DEVICE [16] ob_in_cam of the centred mesh (pose_last), or NULL = continue from the pose this context's
- * previous fp_track produced.  pose_out_dev (DEVICE [16]) / pose_out_host (HOST [16]) are optional.  Synchronises. */
+ * previous fp_track produced.  pose_out_dev (DEVICE [16]) / pose_out_host (HOST [16]) are optional.  This is the
+ * one-object case of fp_track_cameras (one camera, the mesh in slot 0) and shares its cached graph with
+ * fp_track_objects of one object: the graph takes the frame from the camera table, so new intrinsics or a frame no
+ * larger than one tracked before replay it.  The first tracking call, or one with a larger frame than any tracked
+ * before, captures every cached graph of the context once more (the tracking calls' frame-preparation grid grows).
+ * Synchronises. */
 int fp_track(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
              const float* pose_in_dev, int iterations, float* pose_out_dev, float* pose_out_host, void* stream);
 /* FoundationPose.track_one (estimater.py:250-268) applied to M objects of the same frame, as ONE CUDA-graph launch:
@@ -289,7 +294,8 @@ int fp_track(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host
  * `iterations` refiner passes over a batch of M hypotheses where hypothesis i renders the mesh in slot slots_host[i],
  * read-back of the M poses.  slots_host: HOST [M] slot ids, each loaded (checked before anything is enqueued);
  * poses_in_dev: DEVICE [M][16] ob_in_cam of each centred mesh; poses_out_dev (DEVICE [M][16]) / poses_out_host
- * (HOST [M][16]) are optional.  Each pose equals what fp_track gives for that object alone.  This is fp_track_cameras
+ * (HOST [M][16]) are optional.  Each pose equals what fp_track gives for that object alone, and what fp_set_frame
+ * (FP_FRAME_FILTER_DEPTH, zfar = inf) + fp_refine give for it with its mesh in slot 0.  This is fp_track_cameras
  * with one camera (C = 1, every object seen by camera 0), and shares its cached graph: new intrinsics or a frame no
  * larger than one seen before replay it.  Leaves fp_track's continuation pose untouched.  Synchronises. */
 int fp_track_objects(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,

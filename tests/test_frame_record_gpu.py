@@ -1,6 +1,7 @@
 """The calls that take the context's frame (camera 0) by value keep their CUDA graphs until the frame's size or intrinsics
 change: with warm graphs, a frame with new fx fy cx cy at the same size, then a frame of another size, captures each
-graph the call replays exactly once, and every result equals the same call on a fresh context bit for bit."""
+graph the call replays exactly once, and every result equals the same call on a fresh context bit for bit.  fp_track
+takes the frame from the camera table: the same two frames capture no graph."""
 import numpy as np
 import pytest
 import torch
@@ -67,13 +68,24 @@ def _register(e, f, scene):
     return [t.cpu() for t in (poses, info, refined, scores, best)]
 
 
-# each call and the number of by-value graphs it replays: track's whole frame; one register pass's refinement and
-# scorer features; refine's and score_features'
-CALLS = [(_track, 1), (_register_objects, 2), (_register, 2)]
+# each call and the number of by-value graphs it replays: one register pass's refinement and scorer features; refine's
+# and score_features'
+CALLS = [(_register_objects, 2), (_register, 2)]
 
 
 @pytest.mark.parametrize("call,graphs", CALLS, ids=[c.__name__.lstrip("_") for c, _ in CALLS])
 def test_by_value_graphs_follow_the_frame(scene, call, graphs):
+    _follow_the_frames(scene, call, graphs)
+
+
+def test_track_replays_its_graph_on_a_new_frame(scene):
+    """fp_track is fp_track_cameras with one camera and one object: new intrinsics or a smaller frame replay its graph."""
+    _follow_the_frames(scene, _track, 0)
+
+
+def _follow_the_frames(scene, call, graphs):
+    """Warms every graph of `call` on the first frame, then asserts that new intrinsics, then another frame size, capture
+    `graphs` graphs each and give what a fresh context gives."""
     e = _engine(scene["mesh"])
     first = scene["frames"][0]
     for _ in range(3):  # first sight of every graph runs eagerly, the second captures, the third replays

@@ -1,6 +1,6 @@
-"""fp_track_cameras (objects of several camera streams, ONE graph launch) against fp_track_objects per camera, against the
-CPU oracle (tests/golden/track_cameras.npz, tools/make_golden_track_cameras.py), its graph caching, its refusals, and
-estimater.track_cameras against track_one."""
+"""fp_track_cameras (objects of several camera streams, ONE graph launch) against fp_track_objects per camera, fp_track
+and the by-value fp_set_frame + fp_refine per object, against the CPU oracle (tests/golden/track_cameras.npz,
+tools/make_golden_track_cameras.py), its graph caching, its refusals, and estimater.track_cameras against track_one."""
 import ctypes as C
 import os
 
@@ -101,9 +101,13 @@ def _alone(e, cam):
 
 
 def _single(e, objs, cam, j):
-    """fp_track of object j of a camera alone, its mesh in slot 0."""
+    """Object j of a camera alone, its mesh in slot 0: {path: pose} for fp_track (the camera-table path) and for the
+    by-value path fp_set_frame (filtered, zfar = inf) + fp_refine."""
     _load(e, objs[cam["seen"][j]][0], 0)
-    return e.track(cam["rgb"], cam["depth"], cam["K"], torch.from_numpy(cam["start"][j]).cuda(), 2)[1]
+    start = torch.from_numpy(cam["start"][j]).cuda()
+    tracked = e.track(cam["rgb"], cam["depth"], cam["K"], start, 2)[1]
+    e.set_frame(cam["rgb"], cam["depth"], cam["K"], filter_depth=True, zfar=float("inf"))
+    return {"track": tracked, "set_frame + refine": e.refine(start, 2)[0][0].cpu().numpy()}
 
 
 @pytest.mark.parametrize("C", [1, 2, 4])
@@ -118,8 +122,8 @@ def test_equals_tracking_each_camera_alone(rig, C):
     alone = [_alone(e, cam) for cam in cams]
     for i, (c, j) in enumerate(pairs):
         assert np.array_equal(host[i], alone[c][j]), f"C={C}, camera {c}, object {j}: off by {np.abs(host[i] - alone[c][j]).max():.2e}"
-        single = _single(e, rig["objs"], cams[c], j)
-        assert np.array_equal(host[i], single), f"C={C}, camera {c}, object {j}: off track() by {np.abs(host[i] - single).max():.2e}"
+        for path, single in _single(e, rig["objs"], cams[c], j).items():
+            assert np.array_equal(host[i], single), f"C={C}, camera {c}, object {j}: off {path} by {np.abs(host[i] - single).max():.2e}"
 
 
 def test_the_largest_number_of_cameras(rig):
@@ -137,7 +141,8 @@ def test_the_largest_number_of_cameras(rig):
     _, host = e.track_cameras(frames, start, cam_of, slots, 2)
     for i, (c, j) in enumerate(pairs):
         assert np.array_equal(host[i], _alone(e, cams[c])[j]), f"camera {c}"
-        assert np.array_equal(host[i], _single(e, objs, cams[c], j)), f"camera {c}: track()"
+        for path, single in _single(e, objs, cams[c], j).items():
+            assert np.array_equal(host[i], single), f"camera {c}: {path}"
 
 
 def test_against_the_oracle():

@@ -1,5 +1,6 @@
-"""fp_track_objects (several objects of one frame, ONE graph launch) against fp_track per object, against the CPU oracle
-(tests/golden/track_objects.npz, tools/make_golden_track_objects.py), and through estimater.track_objects."""
+"""fp_track_objects (several objects of one frame, ONE graph launch) against fp_track and the by-value fp_set_frame +
+fp_refine per object, against the CPU oracle (tests/golden/track_objects.npz, tools/make_golden_track_objects.py), and
+through estimater.track_objects."""
 import os
 
 import numpy as np
@@ -70,13 +71,17 @@ def rig():
 
 
 def _single(r, k):
-    """fp_track of object k alone (its mesh in slot 0)."""
+    """Object k alone, its mesh in slot 0: {path: pose} for fp_track (the camera-table path) and for the by-value path
+    fp_set_frame (filtered, zfar = inf) + fp_refine."""
     from foundationpose_b200 import synth
 
     e = r["e"]
     _load(e, r["objs"][k][0], 0)
-    _, host = e.track(r["rgb"], r["depth"], synth.DEFAULT_K, torch.from_numpy(r["start"][k]).cuda(), 2)
-    return host
+    start = torch.from_numpy(r["start"][k]).cuda()
+    _, tracked = e.track(r["rgb"], r["depth"], synth.DEFAULT_K, start, 2)
+    e.set_frame(r["rgb"], r["depth"], synth.DEFAULT_K, filter_depth=True, zfar=float("inf"))
+    refined = e.refine(start, 2)[0][0].cpu().numpy()
+    return {"track": tracked, "set_frame + refine": refined}
 
 
 @pytest.mark.parametrize("M", [1, 2, 3, 5])
@@ -88,8 +93,8 @@ def test_equals_tracking_each_object_alone(rig, M):
                                 list(range(1, M + 1)), 2)
     assert np.array_equal(dev.cpu().numpy(), host), "device and host copies of the poses differ"
     for k in range(M):
-        single = _single(rig, k)
-        assert np.array_equal(host[k], single), f"M={M}, object {k}: off by {np.abs(host[k] - single).max():.2e}"
+        for path, single in _single(rig, k).items():
+            assert np.array_equal(host[k], single), f"M={M}, object {k}: off {path} by {np.abs(host[k] - single).max():.2e}"
 
 
 def test_against_the_oracle():
