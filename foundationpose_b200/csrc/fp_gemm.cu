@@ -599,6 +599,8 @@ static int launch_bn(const CUtensorMap& ma, const CUtensorMap& mb, const CUtenso
 }
 
 int stem_conv_launch(const GemmLayer& L, cudaStream_t stream);  // fp_stem.cu
+bool linear_ws_takes(const GemmLayer& L);                        // fp_linear.cu
+int linear_ws_launch(const GemmLayer& L, cudaStream_t stream);
 
 // FPOSE_SWAP_TILE=0 keeps the 128-channel convolutions on the 128 x 128 tile.  Read at every plan, so that one process
 // can time and compare both tiles; a captured graph keeps the tiles of its capture.
@@ -751,12 +753,15 @@ static int gemm_layer_plan(const GemmLayer& L, cudaStream_t stream, int* tile_n,
   FP_REQUIRE(L.out_split == 0 || L.out_split % p.bn == 0,
              "out_split=%d must be a multiple of the tile's image count %d (pad the A/B batch boundary)", L.out_split,
              p.bn);
+  // the K = 512 linear layers on tall row counts: 64-row x 128-channel tiles of the weight-stationary kernel
+  const bool linear_ws = linear_ws_takes(L);
   if (tile_n || tile_m) {
     if (tile_n) *tile_n = BN;
-    if (tile_m) *tile_m = swap ? 256 : 128;
+    if (tile_m) *tile_m = swap ? 256 : linear_ws ? 64 : 128;
     return 0;
   }
   if (p.total_tiles == 0) return 0;
+  if (linear_ws) return linear_ws_launch(L, stream);
 
   int rc = encode_map(&ma, L.in, 5, dims, str, box);
   if (rc) return rc;

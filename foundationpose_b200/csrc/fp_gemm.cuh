@@ -41,7 +41,8 @@ struct GemmLayer {
 int gemm_layer_launch(const GemmLayer& L, cudaStream_t stream);
 // The output channels per tile (64, 128 or 256) gemm_layer_launch would use for L; launches nothing.
 int gemm_layer_tile_n(const GemmLayer& L, int* tile_n);
-// The output pixels per tile (256 for the swapped 128-channel tile, else 128); launches nothing.
+// The output pixels per tile (256 for the swapped 128-channel tile, 64 for the weight-stationary linear kernel, else
+// 128); launches nothing.
 int gemm_layer_tile_m(const GemmLayer& L, int* tile_m);
 
 

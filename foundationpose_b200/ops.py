@@ -56,7 +56,8 @@ def gemm_tile_n(kind, *, n_img, Hin, Win, Cin, Cout, out_split=0):
 
 
 def gemm_tile_m(kind, *, n_img, Hin, Win, Cin, Cout, out_split=0):
-    """Output pixels per tile (128, or 256 for the swapped 128-channel tile) that `gemm_layer` picks for this shape."""
+    """Output pixels (linear rows) per tile that `gemm_layer` picks for this shape: 128, 256 for the swapped
+    128-channel tile, 64 for the weight-stationary K = 512 linear kernel."""
     lib.fp_op_gemm_tile_m.argtypes = [C.POINTER(_lib.GemmLayer), C.POINTER(C.c_int)]
     lib.fp_op_gemm_tile_m.restype = C.c_int
     L = _lib.GemmLayer(kind, n_img, Hin, Win, Cin, Cout, None, None, None, None, 0, None, Cout, out_split, None, 0)

@@ -74,8 +74,9 @@ int fp_op_gemm_layer(const fp_gemm_layer_t* layer, void* stream);
  * shape and the current device's SM count only.  Launches nothing and dereferences no pointer of the layer. */
 int fp_op_gemm_tile_n(const fp_gemm_layer_t* layer, int* tile_n);
 /* Output pixels (or linear rows) per tile that fp_op_gemm_layer would use for `layer`: 256 where a 128-channel 3x3
- * convolution runs with the weights as the wgmma M operand (FPOSE_SWAP_TILE=0 turns that tile off), else 128.  Same
- * rules as fp_op_gemm_tile_n. */
+ * convolution runs with the weights as the wgmma M operand (FPOSE_SWAP_TILE=0 turns that tile off), 64 where a K = 512
+ * linear layer runs on the weight-stationary kernel (FPOSE_LINEAR_WS=0 turns it off), else 128.  Same rules as
+ * fp_op_gemm_tile_n. */
 int fp_op_gemm_tile_m(const fp_gemm_layer_t* layer, int* tile_m);
 
 /* softmax(Q K^T / sqrt(128)) V of nn.MultiheadAttention (refine_network.py:56-70, score_network.py:53):
