@@ -52,13 +52,39 @@ struct OwnedBuf {
 using DevBuf = OwnedBuf<cudaFree>;         // device memory
 using PinnedBuf = OwnedBuf<cudaFreeHost>;  // page-locked host memory
 
+// A CUDA event (timing disabled), created on first use and destroyed with its owner.  Move-only, as OwnedBuf.
+struct OwnedEvent {
+  cudaEvent_t e = nullptr;
+  OwnedEvent() = default;
+  OwnedEvent(OwnedEvent&& o) noexcept : e(std::exchange(o.e, nullptr)) {}
+  OwnedEvent& operator=(OwnedEvent&& o) noexcept {
+    if (this != &o) {
+      if (e) cudaEventDestroy(e);
+      e = std::exchange(o.e, nullptr);
+    }
+    return *this;
+  }
+  ~OwnedEvent() {
+    if (e) cudaEventDestroy(e);
+  }
+  cudaError_t record(cudaStream_t st) {
+    if (!e) {
+      const cudaError_t ce = cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
+      if (ce != cudaSuccess) return ce;
+    }
+    return cudaEventRecord(e, st);
+  }
+};
+
 // (Re)allocates `b` to at least `bytes`.  `epoch` is the owning context's graph epoch: it is bumped whenever a device
 // pointer or by-value kernel parameter that a captured CUDA graph may hold changes (re-allocation, new weights /
 // intrinsics), and cached graphs older than it are rebuilt.  Never called while a stream is capturing:
-// every workspace is sized by ensure_capacity / fp_set_mesh_slot / fp_set_frame BEFORE run_graphed.
+// every workspace is sized by ensure_capacity / fp_set_mesh_slot / fp_set_frame BEFORE run_graphed.  A tracking call
+// still in flight may be reading the buffer being replaced, so growing one waits for the device first.
 static int dev_alloc(unsigned long long& epoch, DevBuf& b, size_t bytes, bool zero = false) {
   if (b.bytes >= bytes && b.p) return 0;
   ++epoch;
+  if (b.p) FP_CUDA_OK(cudaDeviceSynchronize());
   b.reset();
   FP_CUDA_OK(cudaMalloc(&b.p, bytes));
   b.bytes = bytes;
@@ -129,14 +155,36 @@ struct MeshSlot {
   float diameter = 0.f;
 };
 
-// One camera's frame: the raw upload, the filtered frame (rgba, depth, xyz) and the pinned staging of the upload, and
-// the size and intrinsics of the frame the last call prepared in this camera.  Camera 0 is the context's frame, the one
-// every single-frame entry point reads (see alloc_camera).  camera_dev() makes the kernels' record of it.
+// One camera's frame: the raw upload and the filtered frame (rgba, depth, xyz), and the size and intrinsics of the frame
+// the last call prepared in this camera.  Camera 0 is the context's frame, the one every single-frame entry point reads
+// (see alloc_camera).  camera_dev() makes the kernels' record of it.
 struct CameraBufs {
   DevBuf rgb_raw, depth_raw, rgba, depth, xyz;
-  PinnedBuf stage_rgb, stage_depth;
   int H = 0, W = 0;
   float fx = 0.f, fy = 0.f, cx = 0.f, cy = 0.f;
+};
+
+// The tracking calls keep up to FP_TRACK_MAX_IN_FLIGHT calls in flight, each uploading through a staging set of its
+// own: the host copies the next call's frames while the device still tracks the previous call.  Only the host side is
+// doubled: the device buffers the uploads land in are ordered by the stream.  A set is busy from its call's submit
+// until `uploaded` (recorded after the set's last host-to-device copy) has passed.  The register calls stage through
+// set 0 after draining every set (see drain).
+constexpr int kMaxInFlight = FP_TRACK_MAX_IN_FLIGHT;
+struct StagingSet {
+  PinnedBuf rgb[kMaxCameras], depth[kMaxCameras];
+  PinnedBuf args;  // the camera table, then the slot ids and camera ids (layout of fp_ctx::args)
+  OwnedEvent uploaded;
+  bool busy = false;
+};
+
+// The pose read-back of one submitted tracking call: pinned [M][16] poses, complete once `done` has passed.  Owned by
+// the call's ticket until fp_track_wait collects it (ticket 0: free for the next submit).  A call's read-back outlives
+// its staging set, which the call after next may reuse before this result is collected.
+struct Readback {
+  PinnedBuf poses;
+  OwnedEvent done;
+  unsigned long long ticket = 0;
+  int M = 0;
 };
 
 }  // namespace fp
@@ -187,11 +235,17 @@ struct fp_ctx {
   fp::DevBuf mask_buf, mask_stats, crop_stats;
   fp::DevBuf op_mesh_of;  // fp_op_pose_update: the uploaded slot id of every hypothesis
   fp::DevBuf track_pose;      // fp_track: the pose it produced last, where pose_in = NULL continues from
-  fp::PinnedBuf stage_poses;  // the tracking calls: pinned [M][16] pose read-back
-  // the arguments of a multi-object call or register pass, one device block at a fixed address (a graph holds it) and
-  // its pinned staging: the camera table (CameraDev [FP_MAX_CAMERAS]), the slot ids [n], the camera ids [n]
+  // the tracking calls in flight: their staging sets (used in turn), their read-backs by ticket, the last ticket issued,
+  // and the stream and completion event (after the read-back) of the last call submitted
+  fp::StagingSet sets[fp::kMaxInFlight];
+  int next_set = 0;
+  std::vector<std::unique_ptr<fp::Readback>> readbacks;
+  unsigned long long last_ticket = 0;
+  cudaStream_t last_stream = nullptr;
+  cudaEvent_t last_done = nullptr;  // the last call's Readback::done (a Readback is reused only by a later call)
+  // the arguments of a multi-object call or register pass, one device block at a fixed address (a graph holds it),
+  // staged through a StagingSet: the camera table (CameraDev [FP_MAX_CAMERAS]), the slot ids [n], the camera ids [n]
   fp::DevBuf args;
-  fp::PinnedBuf stage_args;
   int cam_grid_h = 0, cam_grid_w = 0;  // the tracking calls' frame-preparation grid: the largest frame seen
   // fp_register_objects / _cameras: row offsets of the objects' hypotheses [M + 1] and the objects' camera ids [M], the
   // objects' feature rows [sum N][512], each object's byte offset into mask_buf; pinned staging of the masks and of
@@ -660,11 +714,10 @@ static int set_frame_launches(fp_ctx* c, const unsigned char* rgb_dev, const flo
   return depth_to_xyz_launch(one, zfar, st);
 }
 
-// Sizes camera i's buffers for npix pixels: the filtered frame always, the raw upload if `raw`, its pinned staging if
-// `staged`.  Camera 0's addresses are held by the graphs that take the frame by value, so growing its buffers bumps the
-// graph epoch.  Cameras 1.. are reached only through the camera table, which every call rewrites: growing them
-// invalidates no graph.  No graph holds the staging: the uploads leave it ahead of the launch.
-static int alloc_camera(fp_ctx* c, int i, size_t npix, bool raw, bool staged) {
+// Sizes camera i's buffers for npix pixels: the filtered frame always, the raw upload if `raw`.  Camera 0's addresses
+// are held by the graphs that take the frame by value, so growing its buffers bumps the graph epoch.  Cameras 1.. are
+// reached only through the camera table, which every call rewrites: growing them invalidates no graph.
+static int alloc_camera(fp_ctx* c, int i, size_t npix, bool raw) {
   CameraBufs& b = c->cam[i];
   unsigned long long table_only = 0;
   unsigned long long& epoch = i == 0 ? c->epoch : table_only;
@@ -674,10 +727,6 @@ static int alloc_camera(fp_ctx* c, int i, size_t npix, bool raw, bool staged) {
   if (raw) {
     FP_TRY(dev_alloc(epoch, b.rgb_raw, npix * 3));
     FP_TRY(dev_alloc(epoch, b.depth_raw, npix * 4));
-  }
-  if (staged) {
-    FP_TRY(pinned_alloc(nullptr, b.stage_rgb, npix * 3));
-    FP_TRY(pinned_alloc(nullptr, b.stage_depth, npix * 4));
   }
   return 0;
 }
@@ -716,16 +765,29 @@ static int refine_body(fp_ctx* c, int N, int iterations, cudaStream_t s2, const 
   return 0;
 }
 
-// The previous frame's graph has finished (every caller synchronises), so the staging buffers are free.  The two
-// uploads are issued as soon as their staging copy is done — the depth DMA runs under the host's rgb copy, the
-// rgb DMA under the next camera's copies or the graph launch — instead of being nodes of the graph (measured: -40 us
-// per frame)
-static int upload_staged_frame(CameraBufs& b, const unsigned char* rgb_host, const float* depth_host, size_t npix,
-                               cudaStream_t st) {
-  memcpy(b.stage_depth.p, depth_host, npix * 4);
-  FP_CUDA_OK(cudaMemcpyAsync(b.depth_raw.p, b.stage_depth.p, npix * 4, cudaMemcpyHostToDevice, st));
-  memcpy(b.stage_rgb.p, rgb_host, npix * 3);
-  FP_CUDA_OK(cudaMemcpyAsync(b.rgb_raw.p, b.stage_rgb.p, npix * 3, cudaMemcpyHostToDevice, st));
+// Uploads one camera's frame through its staging (free: the set is not busy).  The two uploads are issued as soon as
+// their staging copy is done — the depth DMA runs under the host's rgb copy, the rgb DMA under the next camera's copies
+// or the graph launch — instead of being nodes of the graph (measured: -40 us per frame)
+static int upload_staged_frame(CameraBufs& b, PinnedBuf& stage_rgb, PinnedBuf& stage_depth, const unsigned char* rgb_host,
+                               const float* depth_host, size_t npix, cudaStream_t st) {
+  memcpy(stage_depth.p, depth_host, npix * 4);
+  FP_CUDA_OK(cudaMemcpyAsync(b.depth_raw.p, stage_depth.p, npix * 4, cudaMemcpyHostToDevice, st));
+  memcpy(stage_rgb.p, rgb_host, npix * 3);
+  FP_CUDA_OK(cudaMemcpyAsync(b.rgb_raw.p, stage_rgb.p, npix * 3, cudaMemcpyHostToDevice, st));
+  return 0;
+}
+
+// Waits until every tracking call in flight has moved its uploads out of its staging set, and orders `st` after the
+// last call submitted (its device buffers and the context's frames are then free on `st`).  Every entry point that
+// uses the context's staging, frames or workspaces calls this first; the tracking submits do not, they wait only for
+// the set they reuse.  Results are collected separately (fp_track_wait).
+static int drain(fp_ctx* c, cudaStream_t st) {
+  for (StagingSet& s : c->sets)
+    if (s.busy) {
+      FP_CUDA_OK(cudaEventSynchronize(s.uploaded.e));
+      s.busy = false;
+    }
+  if (c->last_done && st != c->last_stream) FP_CUDA_OK(cudaStreamWaitEvent(st, c->last_done, 0));
   return 0;
 }
 
@@ -737,10 +799,10 @@ constexpr size_t kTableBytes = sizeof(CameraDev) * kMaxCameras;  // the camera t
 // `staged_rows`, every camera records its size and intrinsics (K: [C][9]; camera 0's become the context's frame
 // geometry), the staging receives the camera table (every camera's record; entries C.. zeroed), and every frame is
 // uploaded through its camera's staging (camera i's DMA runs while camera i + 1 is copied on the host).  H_max / W_max:
-// the largest frame height and width of the call.
-static int setup_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
-                         const float* K, const int* H, const int* W, int rows, int staged_rows, cudaStream_t st,
-                         int& H_max, int& W_max) {
+// the largest frame height and width of the call.  `set`: the staging set the call uploads through (not busy).
+static int setup_cameras(fp_ctx* c, StagingSet& set, int C, const unsigned char* const* rgb_host,
+                         const float* const* depth_host, const float* K, const int* H, const int* W, int rows,
+                         int staged_rows, cudaStream_t st, int& H_max, int& W_max) {
   size_t npix_max = 0;
   H_max = W_max = 0;
   for (int i = 0; i < C; ++i) {
@@ -748,35 +810,74 @@ static int setup_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host,
     H_max = std::max(H_max, H[i]);
     W_max = std::max(W_max, W[i]);
   }
-  for (int i = 0; i < C; ++i) FP_TRY(alloc_camera(c, i, npix_max, /*raw=*/true, /*staged=*/true));
+  for (int i = 0; i < C; ++i) {
+    FP_TRY(alloc_camera(c, i, npix_max, /*raw=*/true));
+    FP_TRY(pinned_alloc(nullptr, set.rgb[i], npix_max * 3));
+    FP_TRY(pinned_alloc(nullptr, set.depth[i], npix_max * 4));
+  }
   c->n_frames = C;
   FP_TRY(dev_alloc(c->epoch, c->args, kTableBytes + (size_t)2 * rows * sizeof(int)));
-  FP_TRY(pinned_alloc(nullptr, c->stage_args, kTableBytes + (size_t)2 * staged_rows * sizeof(int)));
-  CameraDev* table = reinterpret_cast<CameraDev*>(c->stage_args.p);
+  FP_TRY(pinned_alloc(nullptr, set.args, kTableBytes + (size_t)2 * staged_rows * sizeof(int)));
+  CameraDev* table = reinterpret_cast<CameraDev*>(set.args.p);
   memset(table, 0, kTableBytes);
   for (int i = 0; i < C; ++i) {
     set_frame_geometry(c, i, K + 9 * i, H[i], W[i]);
     table[i] = camera_dev(c, i);
-    FP_TRY(upload_staged_frame(c->cam[i], rgb_host[i], depth_host[i], (size_t)H[i] * W[i], st));
+    FP_TRY(upload_staged_frame(c->cam[i], set.rgb[i], set.depth[i], rgb_host[i], depth_host[i], (size_t)H[i] * W[i], st));
   }
   return 0;
 }
 
-// fp_track_cameras, fp_track_objects (C = 1) and fp_track (C = M = 1) after validation.  The camera table, the slot ids
-// and the camera ids go to the argument block in one copy ahead of the launch.  The graph holds the block's address, not
-// the frames' sizes, intrinsics or buffers, and is keyed on (M, iterations, C): reordering objects or cameras, new
-// intrinsics or a smaller frame replay it.  One frame_prep_kernel launch filters every camera and the crops take their
-// frame from the table.  poses_out_dev, poses_keep_dev (fp_track's continuation pose) and poses_out_host are optional;
-// the device copies are complete when the call returns.
-static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
-                              const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
-                              const float* poses_in_dev, int iterations, float* poses_out_dev, float* poses_out_host,
-                              cudaStream_t st, float* poses_keep_dev = nullptr) {
+// The staging uploads of one tracking call: the frames, then the camera table, the slot ids and the camera ids in one
+// copy to the argument block.  H_max / W_max as setup_cameras.
+static int stage_track_call(fp_ctx* c, StagingSet& set, int C, const unsigned char* const* rgb_host,
+                            const float* const* depth_host, const float* K, const int* H, const int* W, int M,
+                            const int* camera_of, const int* slots_host, cudaStream_t st, int& H_max, int& W_max) {
+  FP_TRY(setup_cameras(c, set, C, rgb_host, depth_host, K, H, W, M, M, st, H_max, W_max));
+  int* ids = reinterpret_cast<int*>(static_cast<char*>(set.args.p) + kTableBytes);
+  memcpy(ids, slots_host, (size_t)M * sizeof(int));
+  memcpy(ids + M, camera_of, (size_t)M * sizeof(int));
+  FP_CUDA_OK(cudaMemcpyAsync(c->args.p, set.args.p, kTableBytes + (size_t)2 * M * sizeof(int), cudaMemcpyHostToDevice, st));
+  return 0;
+}
+
+// fp_track_cameras_submit, fp_track_objects_submit (C = 1) and fp_track_submit (C = M = 1) after validation, and so
+// every blocking tracking call, which is a submit and its fp_track_wait.  The call stages through the next staging set,
+// waiting first, if that set is still busy, until the uploads of the call that used it have left it.  The camera
+// table, the slot ids and the camera ids go to the argument block in one copy ahead of the launch.  The graph holds the
+// block's address, not the frames' sizes, intrinsics or buffers, and is keyed on (M, iterations, C): reordering objects
+// or cameras, new intrinsics or a smaller frame replay it.  One frame_prep_kernel launch filters every camera and the
+// crops take their frame from the table.  The pose read-back follows the launch outside the graph, into the call's own
+// Readback, so one graph serves every staging set.  poses_out_dev and poses_keep_dev (fp_track's continuation pose)
+// are optional and complete in stream order; *ticket receives the call's ticket.
+static int track_cameras_submit(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
+                                const float* K, const int* H, const int* W, int M, const int* camera_of,
+                                const int* slots_host, const float* poses_in_dev, int iterations, float* poses_out_dev,
+                                cudaStream_t st, unsigned long long* ticket, float* poses_keep_dev = nullptr) {
+  StagingSet& set = c->sets[c->next_set];
+  if (set.busy) {
+    FP_CUDA_OK(cudaEventSynchronize(set.uploaded.e));
+    set.busy = false;
+  }
+  // the context's device buffers are never used by two streams at once
+  if (c->last_done && st != c->last_stream) FP_CUDA_OK(cudaStreamWaitEvent(st, c->last_done, 0));
+  Readback* rb = nullptr;
+  for (auto& r : c->readbacks)
+    if (r->ticket == 0) rb = r.get();
+  if (!rb) {
+    c->readbacks.push_back(std::make_unique<Readback>());
+    rb = c->readbacks.back().get();
+  }
   FP_TRY(ensure_capacity(c, M));
-  FP_TRY(pinned_alloc(&c->epoch, c->stage_poses, (size_t)M * 64));  // the graph's read-back node holds this address
+  FP_TRY(pinned_alloc(nullptr, rb->poses, (size_t)M * 64));
   c->has_frame = false;
-  int H_max, W_max;
-  FP_TRY(setup_cameras(c, C, rgb_host, depth_host, K, H, W, M, M, st, H_max, W_max));
+  int H_max = 0, W_max = 0;
+  const int staged = stage_track_call(c, set, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, st, H_max, W_max);
+  // whatever was staged before a failure is still on its way out: the set stays busy until then
+  FP_CUDA_OK(set.uploaded.record(st));
+  set.busy = true;
+  c->next_set = (c->next_set + 1) % kMaxInFlight;
+  FP_TRY(staged);
   if (H_max > c->cam_grid_h || W_max > c->cam_grid_w) {
     // the frame-preparation grid is a by-value launch parameter: it covers the largest frame seen, the blocks outside
     // a smaller frame return at once
@@ -784,11 +885,6 @@ static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_
     c->cam_grid_h = std::max(c->cam_grid_h, H_max);
     c->cam_grid_w = std::max(c->cam_grid_w, W_max);
   }
-  int* ids = reinterpret_cast<int*>(static_cast<char*>(c->stage_args.p) + kTableBytes);
-  memcpy(ids, slots_host, (size_t)M * sizeof(int));
-  memcpy(ids + M, camera_of, (size_t)M * sizeof(int));
-  FP_CUDA_OK(cudaMemcpyAsync(c->args.p, c->stage_args.p, kTableBytes + (size_t)2 * M * sizeof(int), cudaMemcpyHostToDevice,
-                             st));
   const CameraDev* cams_dev = reinterpret_cast<const CameraDev*>(c->args.p);
   const int* mesh_of = reinterpret_cast<const int*>(static_cast<const char*>(c->args.p) + kTableBytes);
   const int* cam_of = mesh_of + M;
@@ -803,16 +899,32 @@ static int track_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_
     // camera's frame
     FP_TRY(frame_prep_cameras_launch(cams_dev, C, grid_h, grid_w, INFINITY, s2));
     c->has_frame = true;
-    FP_TRY(refine_body(c, M, iterations, s2, mesh_of, cams_dev, cam_of));
-    FP_CUDA_OK(cudaMemcpyAsync(c->stage_poses.p, fin, (size_t)M * 64, cudaMemcpyDeviceToHost, s2));
-    return 0;
+    return refine_body(c, M, iterations, s2, mesh_of, cams_dev, cam_of);
   };
   FP_TRY(run_graphed(c, GraphKind::TrackObjects, M, iterations, st, body, C));
   c->has_frame = true;
   if (poses_out_dev) FP_CUDA_OK(cudaMemcpyAsync(poses_out_dev, fin, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
   if (poses_keep_dev) FP_CUDA_OK(cudaMemcpyAsync(poses_keep_dev, fin, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
-  FP_CUDA_OK(cudaStreamSynchronize(st));
-  if (poses_out_host) memcpy(poses_out_host, c->stage_poses.p, (size_t)M * 64);
+  FP_CUDA_OK(cudaMemcpyAsync(rb->poses.p, fin, (size_t)M * 64, cudaMemcpyDeviceToHost, st));
+  FP_CUDA_OK(rb->done.record(st));
+  c->last_done = rb->done.e;
+  c->last_stream = st;
+  rb->M = M;
+  rb->ticket = ++c->last_ticket;
+  *ticket = rb->ticket;
+  return 0;
+}
+
+// fp_track_wait: waits for ticket's read-back and copies its poses out (poses_out_host may be null: the result is
+// dropped).  The ticket is collected whatever the outcome, so an asynchronous error is reported once.
+static int track_wait(fp_ctx* c, unsigned long long ticket, float* poses_out_host) {
+  Readback* rb = nullptr;
+  for (auto& r : c->readbacks)
+    if (ticket != 0 && r->ticket == ticket) rb = r.get();
+  FP_REQUIRE(rb, "fp_track_wait: ticket %llu is unknown or already collected", ticket);
+  rb->ticket = 0;
+  FP_CUDA_OK(cudaEventSynchronize(rb->done.e));
+  if (poses_out_host) memcpy(poses_out_host, rb->poses.p, (size_t)rb->M * 64);
   return 0;
 }
 
@@ -943,7 +1055,8 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
   FP_TRY(pinned_alloc(nullptr, c->stage_ints, (size_t)(2 * M + 2) * sizeof(int) + (size_t)M * sizeof(size_t)));
   c->has_frame = false;
   int H_max, W_max;
-  FP_TRY(setup_cameras(c, C, rgb_host, depth_host, K, H, W, max_pass, total, st, H_max, W_max));
+  StagingSet& set = c->sets[0];  // free: the entry point drained every set
+  FP_TRY(setup_cameras(c, set, C, rgb_host, depth_host, K, H, W, max_pass, total, st, H_max, W_max));
   int* ints = reinterpret_cast<int*>(c->stage_ints.p);
   size_t* stage_mask_off = reinterpret_cast<size_t*>(ints + 2 * M + 2);
   memcpy(ints, off.data(), (size_t)(M + 1) * sizeof(int));
@@ -952,7 +1065,7 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
   for (int i = 0; i < M; ++i)
     memcpy(static_cast<unsigned char*>(c->stage_masks.p) + mask_at[i], masks_host[i], mask_at[i + 1] - mask_at[i]);
   // the ids of the pass starting at row r0 are staged at 2 * r0 after the table: its slot ids, then its camera ids
-  int* ids = reinterpret_cast<int*>(static_cast<char*>(c->stage_args.p) + kTableBytes);
+  int* ids = reinterpret_cast<int*>(static_cast<char*>(set.args.p) + kTableBytes);
   for (size_t p = 0; p + 1 < pass_obj.size(); ++p) {
     const int row0 = off[pass_obj[p]], n = off[pass_obj[p + 1]] - row0;
     for (int i = pass_obj[p]; i < pass_obj[p + 1]; ++i) {
@@ -971,7 +1084,7 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
     FP_TRY(set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->cam[0].rgb_raw.p),
                               reinterpret_cast<const float*>(c->cam[0].depth_raw.p), FP_FRAME_FILTER_DEPTH, INFINITY, st));
   } else {
-    FP_CUDA_OK(cudaMemcpyAsync(c->args.p, c->stage_args.p, kTableBytes, cudaMemcpyHostToDevice, st));
+    FP_CUDA_OK(cudaMemcpyAsync(c->args.p, set.args.p, kTableBytes, cudaMemcpyHostToDevice, st));
     FP_CUDA_OK(cudaMemcpyAsync(c->mask_off.p, stage_mask_off, (size_t)M * sizeof(size_t), cudaMemcpyHostToDevice, st));
     FP_TRY(frame_prep_cameras_launch(cams_dev, C, H_max, W_max, INFINITY, st));
   }
@@ -1068,7 +1181,7 @@ int fp_destroy(fp_ctx* c) {
   FP_API_BEGIN
   if (!c) return 0;
   DeviceGuard dg(c->device);
-  cudaDeviceSynchronize();
+  cudaDeviceSynchronize();  // calls still in flight finish; their uncollected read-backs are freed with the context
   for (auto& kv : c->graphs)
     if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   if (c->cap_stream) cudaStreamDestroy(c->cap_stream);
@@ -1266,10 +1379,11 @@ int fp_set_frame(fp_ctx* c, const unsigned char* rgb, const float* depth, const 
   FP_REQUIRE(H > 0 && W > 0, "fp_set_frame: empty frame");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(drain(c, st));
   const size_t npix = (size_t)H * W;
   c->has_frame = false;
   const bool on_dev = (flags & FP_FRAME_ON_DEVICE) != 0;
-  FP_TRY(alloc_camera(c, 0, npix, /*raw=*/!on_dev, /*staged=*/false));
+  FP_TRY(alloc_camera(c, 0, npix, /*raw=*/!on_dev));
   set_frame_geometry(c, 0, K, H, W);
   c->n_frames = 1;
   const unsigned char* rgb_dev = rgb;
@@ -1293,6 +1407,7 @@ int fp_set_xyz_map(fp_ctx* c, const float* xyz, void* stream) {
   FP_REQUIRE(c->has_frame, "fp_set_xyz_map: no frame (call fp_set_frame first)");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(drain(c, st));
   // [H][W][3] (host or device) -> the float4-per-pixel layout the crop kernel samples
   const CameraBufs& f = c->cam[0];
   FP_CUDA_OK(cudaMemcpy2DAsync(f.xyz.p, 16, xyz, 12, 12, (size_t)f.H * f.W, cudaMemcpyDefault, st));
@@ -1307,6 +1422,7 @@ int fp_get_depth(fp_ctx* c, int camera, float* depth_out_dev, float* xyz_out_dev
              c->n_frames - 1);
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(drain(c, st));
   const CameraBufs& b = c->cam[camera];
   if (hw_out) {
     hw_out[0] = b.H;
@@ -1327,6 +1443,7 @@ int fp_start_poses(fp_ctx* c, const unsigned char* mask, int mask_on_device, con
   FP_REQUIRE(c->has_frame, "fp_start_poses: no frame (call fp_set_frame first)");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(drain(c, st));
   const CameraDev frame = camera_dev(c, 0);
   const size_t npix = (size_t)frame.H * frame.W;
   const unsigned char* mdev = mask;
@@ -1348,6 +1465,7 @@ int fp_make_crops(fp_ctx* c, const float* poses, int N, int mode, void* crops_ou
   FP_REQUIRE(mode == 0 || mode == 1, "fp_make_crops: mode must be 0 (refiner) or 1 (scorer)");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(drain(c, st));
   if (N == 0) return 0;
   FP_TRY(ensure_capacity(c, N));
   FP_TRY(make_crops(c, poses, N, mode, dbg_out, win_out, nullptr, st));
@@ -1361,6 +1479,7 @@ int fp_crop_stats(fp_ctx* c, const float* poses, int N, int mode, int* stats_out
   FP_REQUIRE(c && poses && stats_out_host && N > 0, "fp_crop_stats: bad argument");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(drain(c, st));
   FP_TRY(ensure_capacity(c, N));
   FP_TRY(dev_alloc(c->epoch, c->crop_stats, 16));
   FP_CUDA_OK(cudaMemsetAsync(c->crop_stats.p, 0, 16, st));
@@ -1377,6 +1496,7 @@ int fp_op_refine_net(fp_ctx* c, const void* crops, int N, float* trans_out, floa
   FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(drain(c, st));
   if (N == 0) return 0;
   FP_TRY(ensure_capacity(c, N));
   FP_TRY(crops_import(c, crops, N, st));
@@ -1395,6 +1515,7 @@ int fp_op_score_feats(fp_ctx* c, const void* crops, int N, float* feats_out, voi
   FP_REQUIRE(c->net[1].loaded, "scorer weights not loaded");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(drain(c, st));
   if (N == 0) return 0;
   FP_TRY(ensure_capacity(c, N));
   FP_TRY(crops_import(c, crops, N, st));
@@ -1437,6 +1558,7 @@ long long fp_op_encoder(fp_ctx* c, int which, const void* crops, int N, int last
   DeviceGuard dg(c->device);
   if (check_device_ptr(crops, "crops", fn) || check_device_ptr(out, "out", fn)) return -1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(drain(c, st));
   if (N == 0) return 0;
   int shape[4];
   enc_out_shape(last, N, shape);
@@ -1457,6 +1579,7 @@ int fp_refine(fp_ctx* c, const float* poses_in, int N, int iterations, float* po
   FP_REQUIRE(c->mesh[0].loaded && c->has_frame, "fp_refine: needs fp_set_mesh and fp_set_frame first");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(drain(c, st));
   if (N == 0) return 0;
   FP_TRY(ensure_capacity(c, N));
   float* pa = reinterpret_cast<float*>(c->poses_a.p);
@@ -1481,6 +1604,7 @@ int fp_score_features(fp_ctx* c, const float* poses, int N, float* feats_out, vo
   FP_REQUIRE(c->mesh[0].loaded && c->has_frame, "fp_score_features: needs fp_set_mesh and fp_set_frame first");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(drain(c, st));
   if (N == 0) return 0;
   FP_TRY(ensure_capacity(c, N));
   float* ps = reinterpret_cast<float*>(c->pose_stage.p);
@@ -1506,6 +1630,7 @@ int fp_score_tail(fp_ctx* c, const float* feats, int L, float* scores_out, int* 
   FP_REQUIRE(c->net[1].loaded, "scorer weights not loaded");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(drain(c, st));
   if (L == 0) return 0;
   FP_TRY(ensure_tail(c, L));
   return score_tail_launch(score_tail_params(c, feats, L, scores_out, best_out), st);
@@ -1522,6 +1647,7 @@ int fp_op_score_tail_segments(fp_ctx* c, const float* feats, int L, const int* s
   FP_REQUIRE(seg_host[n_seg] == L, "%s: the last segment ends at row %d, not at L = %d", fn, seg_host[n_seg], L);
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(drain(c, st));
   ScoreTailParams p;
   FP_TRY(segmented_tail_params(c, feats, seg_host, n_seg, /*trailing=*/0, scores_out, best_out, st, fn, p));
   return score_tail_launch(p, st);
@@ -1545,6 +1671,7 @@ int fp_register(fp_ctx* c, const float* poses_host, int N, int iterations, float
   FP_REQUIRE(c && poses_host && poses_out_host && scores_out_host && best_out_host && N > 0, "fp_register: bad argument");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(drain(c, st));
   FP_TRY(ensure_capacity(c, N));
   FP_TRY(ensure_tail(c, N));
   // poses_b is the loop's ping-pong partner; stage the input in `feats`' neighbour: use tail_proj as scratch
@@ -1564,10 +1691,10 @@ int fp_register(fp_ctx* c, const float* poses_host, int N, int iterations, float
   FP_API_END
 }
 
-int fp_track(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
-             const float* pose_in_dev, int iterations, float* pose_out_dev, float* pose_out_host, void* stream) {
+int fp_track_submit(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
+                    const float* pose_in_dev, int iterations, float* pose_out_dev, void* stream, unsigned long long* ticket) {
   FP_API_BEGIN
-  FP_REQUIRE(c && rgb_host && depth_host && K && H > 0 && W > 0 && iterations >= 0, "fp_track: bad argument");
+  FP_REQUIRE(c && rgb_host && depth_host && K && H > 0 && W > 0 && iterations >= 0 && ticket, "fp_track: bad argument");
   FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
   FP_REQUIRE(c->mesh[0].loaded, "fp_track: no mesh");
   FP_REQUIRE(pose_in_dev || c->track_valid, "fp_track: no previous pose in this context: pass pose_in");
@@ -1577,10 +1704,25 @@ int fp_track(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, 
   float* keep = reinterpret_cast<float*>(c->track_pose.p);
   // fp_track_cameras' one-object, one-camera case: object 0 renders slot 0 in camera 0
   const int zero = 0;
-  FP_TRY(track_cameras_body(c, 1, &rgb_host, &depth_host, K, &H, &W, 1, &zero, &zero, pose_in_dev ? pose_in_dev : keep,
-                            iterations, pose_out_dev, pose_out_host, reinterpret_cast<cudaStream_t>(stream), keep));
+  FP_TRY(track_cameras_submit(c, 1, &rgb_host, &depth_host, K, &H, &W, 1, &zero, &zero, pose_in_dev ? pose_in_dev : keep,
+                              iterations, pose_out_dev, reinterpret_cast<cudaStream_t>(stream), ticket, keep));
   c->track_valid = true;
   return 0;
+  FP_API_END
+}
+
+int fp_track(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
+             const float* pose_in_dev, int iterations, float* pose_out_dev, float* pose_out_host, void* stream) {
+  unsigned long long ticket = 0;
+  const int rc = fp_track_submit(c, rgb_host, depth_host, K, H, W, pose_in_dev, iterations, pose_out_dev, stream, &ticket);
+  return rc ? rc : fp_track_wait(c, ticket, pose_out_host);
+}
+
+int fp_track_wait(fp_ctx* c, unsigned long long ticket, float* poses_out_host) {
+  FP_API_BEGIN
+  FP_REQUIRE(c, "fp_track_wait: null ctx");
+  DeviceGuard dg(c->device);
+  return track_wait(c, ticket, poses_out_host);
   FP_API_END
 }
 
@@ -1605,6 +1747,7 @@ int fp_vis_crops(fp_ctx* c, const float* poses, int N, int mode, float* rec_out,
   FP_API_BEGIN
   FP_REQUIRE(c && poses && rec_out && N > 0 && (mode == 0 || mode == 1), "fp_vis_crops: bad argument");
   DeviceGuard dg(c->device);
+  FP_TRY(drain(c, reinterpret_cast<cudaStream_t>(stream)));
   FP_TRY(ensure_capacity(c, N));
   return make_crops(c, poses, N, mode, nullptr, nullptr, nullptr, reinterpret_cast<cudaStream_t>(stream), nullptr, nullptr,
                     nullptr, reinterpret_cast<float4*>(rec_out));
@@ -1621,6 +1764,7 @@ int fp_vis(fp_ctx* c, int kind, const float* poses_a, const float* poses_b, int 
   FP_REQUIRE(kind == 0 || order, "fp_vis: the scorer canvas needs the row order");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(drain(c, st));
   int hw[2];
   FP_TRY(vis_canvas_size(kind, N, hw, hw + 1));
   if (hw_out) {
@@ -1651,35 +1795,56 @@ int fp_vis(fp_ctx* c, int kind, const float* poses_a, const float* poses_b, int 
   FP_API_END
 }
 
-int fp_track_objects(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W, int M,
-                     const int* slots_host, const float* poses_in_dev, int iterations, float* poses_out_dev,
-                     float* poses_out_host, void* stream) {
+int fp_track_objects_submit(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
+                            int M, const int* slots_host, const float* poses_in_dev, int iterations, float* poses_out_dev,
+                            void* stream, unsigned long long* ticket) {
   FP_API_BEGIN
-  FP_REQUIRE(c && rgb_host && depth_host && K && H > 0 && W > 0 && M > 0 && slots_host && poses_in_dev && iterations >= 0,
+  FP_REQUIRE(c && rgb_host && depth_host && K && H > 0 && W > 0 && M > 0 && slots_host && poses_in_dev && iterations >= 0 &&
+                 ticket,
              "fp_track_objects: bad argument");
   FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
   FP_TRY(check_slots(c, M, slots_host, "fp_track_objects"));
   DeviceGuard dg(c->device);
   const std::vector<int> camera_of(M, 0);
-  return track_cameras_body(c, 1, &rgb_host, &depth_host, K, &H, &W, M, camera_of.data(), slots_host, poses_in_dev, iterations,
-                            poses_out_dev, poses_out_host, reinterpret_cast<cudaStream_t>(stream));
+  return track_cameras_submit(c, 1, &rgb_host, &depth_host, K, &H, &W, M, camera_of.data(), slots_host, poses_in_dev,
+                              iterations, poses_out_dev, reinterpret_cast<cudaStream_t>(stream), ticket);
   FP_API_END
 }
 
-int fp_track_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host, const float* K,
-                     const int* H, const int* W, int M, const int* camera_of, const int* slots_host, const float* poses_in_dev,
-                     int iterations, float* poses_out_dev, float* poses_out_host, void* stream) {
+int fp_track_objects(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W, int M,
+                     const int* slots_host, const float* poses_in_dev, int iterations, float* poses_out_dev,
+                     float* poses_out_host, void* stream) {
+  unsigned long long ticket = 0;
+  const int rc = fp_track_objects_submit(c, rgb_host, depth_host, K, H, W, M, slots_host, poses_in_dev, iterations,
+                                         poses_out_dev, stream, &ticket);
+  return rc ? rc : fp_track_wait(c, ticket, poses_out_host);
+}
+
+int fp_track_cameras_submit(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
+                            const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
+                            const float* poses_in_dev, int iterations, float* poses_out_dev, void* stream,
+                            unsigned long long* ticket) {
   FP_API_BEGIN
-  FP_REQUIRE(c && rgb_host && depth_host && K && H && W && M > 0 && camera_of && slots_host && poses_in_dev && iterations >= 0,
+  FP_REQUIRE(c && rgb_host && depth_host && K && H && W && M > 0 && camera_of && slots_host && poses_in_dev && iterations >= 0 &&
+                 ticket,
              "fp_track_cameras: bad argument");
   FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
   // everything is checked before anything is enqueued: the kernels index the mesh and camera tables unchecked
   FP_TRY(check_cameras(C, rgb_host, depth_host, H, W, M, camera_of, "fp_track_cameras"));
   FP_TRY(check_slots(c, M, slots_host, "fp_track_cameras"));
   DeviceGuard dg(c->device);
-  return track_cameras_body(c, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, poses_in_dev, iterations,
-                            poses_out_dev, poses_out_host, reinterpret_cast<cudaStream_t>(stream));
+  return track_cameras_submit(c, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, poses_in_dev, iterations,
+                              poses_out_dev, reinterpret_cast<cudaStream_t>(stream), ticket);
   FP_API_END
+}
+
+int fp_track_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host, const float* K,
+                     const int* H, const int* W, int M, const int* camera_of, const int* slots_host, const float* poses_in_dev,
+                     int iterations, float* poses_out_dev, float* poses_out_host, void* stream) {
+  unsigned long long ticket = 0;
+  const int rc = fp_track_cameras_submit(c, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, poses_in_dev,
+                                         iterations, poses_out_dev, stream, &ticket);
+  return rc ? rc : fp_track_wait(c, ticket, poses_out_host);
 }
 
 int fp_register_objects(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
@@ -1696,6 +1861,7 @@ int fp_register_objects(fp_ctx* c, const unsigned char* rgb_host, const float* d
   // everything is checked before anything is enqueued
   FP_TRY(check_slots(c, M, slots_host, "fp_register_objects"));
   DeviceGuard dg(c->device);
+  FP_TRY(drain(c, reinterpret_cast<cudaStream_t>(stream)));
   const size_t npix = (size_t)H * W;
   std::vector<const unsigned char*> masks(M);
   for (int i = 0; i < M; ++i) masks[i] = masks_host + (size_t)i * npix;
@@ -1722,6 +1888,7 @@ int fp_register_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host, 
   for (int i = 0; i < M; ++i) FP_REQUIRE(masks_host[i], "fp_register_cameras: object %d: null mask", i);
   FP_TRY(check_slots(c, M, slots_host, "fp_register_cameras"));
   DeviceGuard dg(c->device);
+  FP_TRY(drain(c, reinterpret_cast<cudaStream_t>(stream)));
   return register_cameras_body(c, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, n_hyp_host, masks_host,
                                rot_grids_dev, iterations, poses_out_dev, scores_out_dev, best_out_dev, info_out_dev,
                                reinterpret_cast<cudaStream_t>(stream), /*by_value=*/false);
@@ -1748,6 +1915,7 @@ int fp_op_pose_update(fp_ctx* c, const float* poses_in, const float* trans, cons
   FP_TRY(check_slots(c, mesh_of_host ? N : 1, mesh_of_host ? mesh_of_host : &slot0, fn));
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(drain(c, st));
   if (N == 0) return 0;
   const int* mesh_of = nullptr;
   if (mesh_of_host) {

@@ -6,6 +6,7 @@ computation on the hot path happens inside the C-ABI library.
 """
 import ctypes as C
 import os
+import weakref
 
 import numpy as np
 import torch
@@ -36,6 +37,12 @@ def _proto():
                                         vp, vp]
     lib.fp_register_cameras.argtypes = [vp, i, C.POINTER(vp), C.POINTER(vp), C.POINTER(f), C.POINTER(i), C.POINTER(i), i,
                                         C.POINTER(i), C.POINTER(i), C.POINTER(i), C.POINTER(vp), vp, i, vp, vp, vp, vp, vp]
+    lib.fp_track_submit.argtypes = [vp, vp, vp, C.POINTER(f), i, i, vp, i, vp, vp, C.POINTER(C.c_ulonglong)]
+    lib.fp_track_objects_submit.argtypes = [vp, vp, vp, C.POINTER(f), i, i, i, C.POINTER(i), vp, i, vp, vp,
+                                            C.POINTER(C.c_ulonglong)]
+    lib.fp_track_cameras_submit.argtypes = [vp, i, C.POINTER(vp), C.POINTER(vp), C.POINTER(f), C.POINTER(i), C.POINTER(i), i,
+                                            C.POINTER(i), C.POINTER(i), vp, i, vp, vp, C.POINTER(C.c_ulonglong)]
+    lib.fp_track_wait.argtypes = [vp, C.c_ulonglong, vp]
     lib.fp_graph_captures.argtypes = [vp]
     lib.fp_graph_captures.restype = C.c_ulonglong
     lib.fp_load_network.argtypes = [vp, i, C.POINTER(_FpTensor), i]
@@ -65,7 +72,8 @@ def _proto():
     lib.fp_vis_crops.argtypes = [vp, vp, i, i, vp, vp]
     lib.fp_vis_workspace_bytes.argtypes = [vp]
     lib.fp_vis_workspace_bytes.restype = C.c_ulonglong
-    for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_track_cameras", "fp_register_objects", "fp_register_cameras", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh",
+    for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_track_cameras", "fp_track_submit", "fp_track_objects_submit",
+                 "fp_track_cameras_submit", "fp_track_wait", "fp_register_objects", "fp_register_cameras", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh",
                  "fp_set_mesh_slot", "fp_set_frame",
                  "fp_get_depth", "fp_make_crops", "fp_start_poses", "fp_refine", "fp_score", "fp_score_features", "fp_score_tail",
                  "fp_op_score_tail_segments", "fp_register", "fp_op_refine_net", "fp_op_score_feats", "fp_op_encoder_layer", "fp_op_depth_filter",
@@ -78,6 +86,7 @@ _proto()
 FRAME_ON_DEVICE = 1
 MAX_MESHES = 64  # FP_MAX_MESHES: mesh slots per context
 MAX_CAMERAS = 16  # FP_MAX_CAMERAS: camera streams per fp_track_cameras / fp_register_cameras call
+MAX_IN_FLIGHT = 2  # FP_TRACK_MAX_IN_FLIGHT: tracking calls in flight per context (its staging sets)
 _NO_PIN = os.environ.get("FPOSE_NO_PIN") == "1"  # A/B: skip the pinned staging of host frames
 FRAME_FILTER_DEPTH = 2
 
@@ -161,6 +170,24 @@ def pack_network(sd, kind):
     return out
 
 
+class PendingPoses:
+    """The host poses of one tracking call submitted with wait=False.  result() waits for the call's read-back (once; later
+    calls return the same array) and returns what the blocking call returns as its host poses.  A handle dropped without
+    result() is collected by its engine at a later submit or at close, so its ticket never leaks."""
+
+    def __init__(self, engine, ticket, shape):
+        self._engine, self.ticket, self._shape, self._host = engine, ticket, shape, None
+        self._dropped = weakref.finalize(self, engine._dropped.append, ticket)
+
+    def result(self):
+        if self._host is None:
+            self._dropped.detach()
+            host = np.empty(self._shape, dtype=np.float32)
+            self._engine._wait(self.ticket, host)
+            self._host = host
+        return self._host
+
+
 class Engine:
     """One fp_ctx on the current CUDA device."""
 
@@ -173,9 +200,12 @@ class Engine:
         self.device_index = torch.cuda.current_device()
         self.diameter = None
         self.frame_hw = None
+        self._dropped = []  # tickets of PendingPoses dropped without result()
+        self._last_ticket = 0
 
     def close(self):
         if getattr(self, "_h", None):
+            self._collect_dropped(0)
             lib.fp_destroy(self._h)
             self._h = None
 
@@ -243,10 +273,38 @@ class Engine:
         _lib.check(lib.fp_crop_stats(self._h, _p(poses), len(poses), mode, st, _stream()), "fp_crop_stats")
         return dict(meshlet_visits=st[0], triangles=st[1], fragments=st[2], near_plane_triangles=st[3])
 
-    def track(self, rgb, depth, K, pose_in, iterations, pose_out=None):
+    # ---- tracking: every call is a submit and, with wait=True, its fp_track_wait
+    def _collect_dropped(self, keep):
+        """Collects the dropped handles' tickets except those of the last `keep` submits (still running, most likely)."""
+        for t in [t for t in self._dropped if t <= self._last_ticket - keep]:
+            self._dropped.remove(t)
+            _lib.check(lib.fp_track_wait(self._h, t, None), "fp_track_wait")
+
+    def _submit(self, fn, args, what, out, shape, wait):
+        """Submits one tracking call (`fn(ctx, *args, stream, &ticket)`).  Returns (out, host poses) with wait, else (out,
+        PendingPoses)."""
+        if not getattr(self, "_h", None):
+            raise _lib.FposeError(f"{what}: the engine is closed")
+        self._collect_dropped(MAX_IN_FLIGHT)
+        ticket = C.c_ulonglong()
+        _lib.check(fn(self._h, *args, _stream(), C.byref(ticket)), what)
+        self._last_ticket = ticket.value
+        if not wait:
+            return out, PendingPoses(self, ticket.value, shape)
+        host = np.empty(shape, dtype=np.float32)
+        self._wait(ticket.value, host)
+        return out, host
+
+    def _wait(self, ticket, host):
+        if not getattr(self, "_h", None):
+            raise _lib.FposeError("fp_track_wait: the engine is closed")
+        _lib.check(lib.fp_track_wait(self._h, ticket, C.c_void_p(host.ctypes.data)), "fp_track_wait")
+
+    def track(self, rgb, depth, K, pose_in, iterations, pose_out=None, wait=True):
         """fp_track: one CUDA-graph launch per frame (upload + depth filters + xyz map + refiner passes + read-back).
         rgb uint8 (H,W,3) / depth float32 (H,W) HOST arrays; pose_in (4,4) CUDA tensor or None (continue).
-        Returns (pose_out CUDA (4,4), pose host (4,4) float32 numpy)."""
+        Returns (pose_out CUDA (4,4), pose host (4,4) float32 numpy).  wait=False returns as soon as the call is
+        submitted (the host arrays may then be reused): (pose_out, PendingPoses), pose_out complete in stream order."""
         rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
         depth = np.ascontiguousarray(depth, dtype=np.float32)
         H, W = depth.shape
@@ -255,16 +313,15 @@ class Engine:
             pose_in = pose_in.reshape(4, 4).contiguous().float()
         if pose_out is None:
             pose_out = torch.empty(4, 4, dtype=torch.float32, device="cuda")
-        host = np.empty((4, 4), dtype=np.float32)
-        _lib.check(lib.fp_track(self._h, C.c_void_p(rgb.ctypes.data), C.c_void_p(depth.ctypes.data), Kf, H, W, _p(pose_in),
-                                int(iterations), _p(pose_out), C.c_void_p(host.ctypes.data), _stream()), "fp_track")
+        out = self._submit(lib.fp_track_submit, (C.c_void_p(rgb.ctypes.data), C.c_void_p(depth.ctypes.data), Kf, H, W,
+                                                 _p(pose_in), int(iterations), _p(pose_out)), "fp_track", pose_out, (4, 4), wait)
         self.frame_hw = (H, W)
-        return pose_out, host
+        return out
 
-    def track_objects(self, rgb, depth, K, poses_in, slots, iterations):
+    def track_objects(self, rgb, depth, K, poses_in, slots, iterations, wait=True):
         """fp_track_objects: `track` for M objects of one frame in ONE CUDA-graph launch, object i rendering the mesh in
         slot slots[i] (loaded by set_mesh(..., slot=)).  rgb uint8 (H,W,3) / depth float32 (H,W) HOST arrays; poses_in
-        (M,4,4) CUDA tensor.  Returns (poses CUDA (M,4,4), poses host (M,4,4) float32 numpy)."""
+        (M,4,4) CUDA tensor.  Returns (poses CUDA (M,4,4), poses host (M,4,4) float32 numpy); wait=False as `track`."""
         rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
         depth = np.ascontiguousarray(depth, dtype=np.float32)
         H, W = depth.shape
@@ -275,18 +332,17 @@ class Engine:
         if len(slots) != M:
             raise ValueError(f"track_objects: {M} poses but {len(slots)} slots")
         out = torch.empty(M, 4, 4, dtype=torch.float32, device="cuda")
-        host = np.empty((M, 4, 4), dtype=np.float32)
-        _lib.check(lib.fp_track_objects(self._h, C.c_void_p(rgb.ctypes.data), C.c_void_p(depth.ctypes.data), Kf, H, W, M,
-                                        (C.c_int * M)(*slots), _p(poses_in), int(iterations), _p(out),
-                                        C.c_void_p(host.ctypes.data), _stream()), "fp_track_objects")
+        res = self._submit(lib.fp_track_objects_submit, (C.c_void_p(rgb.ctypes.data), C.c_void_p(depth.ctypes.data), Kf, H, W, M,
+                                                         (C.c_int * M)(*slots), _p(poses_in), int(iterations), _p(out)),
+                           "fp_track_objects", out, (M, 4, 4), wait)
         self.frame_hw = (H, W)
-        return out, host
+        return res
 
-    def track_cameras(self, frames, poses_in, camera_of, slots, iterations):
+    def track_cameras(self, frames, poses_in, camera_of, slots, iterations, wait=True):
         """fp_track_cameras: `track_objects` for M objects spread over C camera streams in ONE CUDA-graph launch.  frames: C
         tuples (rgb uint8 (H,W,3), depth float32 (H,W), K (3,3)) of HOST arrays, one per camera, each with its own size and
         intrinsics; object i is seen by camera camera_of[i] and renders the mesh in slot slots[i]; poses_in (M,4,4) CUDA
-        tensor.  Returns (poses CUDA (M,4,4), poses host (M,4,4) float32 numpy)."""
+        tensor.  Returns (poses CUDA (M,4,4), poses host (M,4,4) float32 numpy); wait=False as `track`."""
         frames = [(np.ascontiguousarray(rgb, dtype=np.uint8), np.ascontiguousarray(depth, dtype=np.float32), K) for rgb, depth, K in frames]
         n_cam = len(frames)
         poses_in = poses_in.reshape(-1, 4, 4).contiguous().float()
@@ -300,12 +356,11 @@ class Engine:
         Hs = (C.c_int * n_cam)(*[depth.shape[0] for _, depth, _ in frames])
         Ws = (C.c_int * n_cam)(*[depth.shape[1] for _, depth, _ in frames])
         out = torch.empty(M, 4, 4, dtype=torch.float32, device="cuda")
-        host = np.empty((M, 4, 4), dtype=np.float32)
-        _lib.check(lib.fp_track_cameras(self._h, n_cam, rgbs, depths, Ks, Hs, Ws, M, (C.c_int * M)(*camera_of), (C.c_int * M)(*slots),
-                                        _p(poses_in), int(iterations), _p(out), C.c_void_p(host.ctypes.data), _stream()),
-                   "fp_track_cameras")
+        res = self._submit(lib.fp_track_cameras_submit, (n_cam, rgbs, depths, Ks, Hs, Ws, M, (C.c_int * M)(*camera_of),
+                                                         (C.c_int * M)(*slots), _p(poses_in), int(iterations), _p(out)),
+                           "fp_track_cameras", out, (M, 4, 4), wait)
         self.frame_hw = frames[0][1].shape  # camera 0's frame is the context's frame
-        return out, host
+        return res
 
     def register_objects(self, rgb, depth, K, masks, rot_grids, slots, iterations):
         """fp_register_objects: the register() hot path for M objects of one frame in one call, object i rendering the mesh

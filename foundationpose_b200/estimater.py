@@ -441,17 +441,33 @@ def _shared_engine_of(estimators, caller):
     return e
 
 
-def track_objects(estimators, rgb, depth, K, iteration=2):
+class PendingTrack:
+    """A tracking call submitted with wait=False (track_objects, track_cameras).  Every estimator's pose_last already holds
+    its pending device pose, so the next call can be submitted at once; result() waits for this call and returns exactly
+    the list the blocking call returns (the same list on every call)."""
+
+    def __init__(self, pending, finish):
+        self._pending, self._finish, self._out = pending, finish, None
+
+    def result(self):
+        if self._out is None:
+            self._out = self._finish(None if self._pending is None else self._pending.result())
+        return self._out
+
+
+def track_objects(estimators, rgb, depth, K, iteration=2, wait=True):
     """`[est.track_one(rgb, depth, K, iteration) for est in estimators]` for several objects of one camera stream, as ONE
     CUDA-graph launch per frame (fp_track_objects): the frame is uploaded and filtered once and the objects' poses are
     refined as one batch, each rendering its own mesh.  Same poses as the per-object calls; updates every pose_last.
 
     The estimators must share one engine (the default: get_engine()).  Each one keeps its mesh in a slot of that engine,
     so alternating objects re-uploads nothing.  Host frames only (uint8 (H,W,3) rgb, float32 (H,W) depth).
-    Returns a list of (4,4) float32 poses of the original meshes."""
+    Returns a list of (4,4) float32 poses of the original meshes.  wait=False returns a PendingTrack as soon as the call
+    is submitted (the frame arrays may then be reused) with every pose_last already set, so the next frame can be
+    submitted while the device tracks this one."""
     estimators = list(estimators)
     if not estimators:
-        return []
+        return [] if wait else PendingTrack(None, lambda _: [])
     if torch.is_tensor(rgb) or torch.is_tensor(depth):
         raise TypeError("track_objects takes host frames (numpy); for device-resident frames call track_one per object")
     e = _shared_engine_of(estimators, "track_objects")
@@ -460,16 +476,19 @@ def track_objects(estimators, rgb, depth, K, iteration=2):
         raise RuntimeError
     slots = [_object_slot(est) for est in estimators]
     poses_in = torch.stack([est.pose_last.reshape(4, 4) for est in estimators])
-    poses_dev, poses_host = e.track_objects(rgb, depth, K, poses_in, slots, iteration)
-    out = []
+    if wait:
+        poses_dev, poses_host = e.track_objects(rgb, depth, K, poses_in, slots, iteration)
+    else:
+        poses_dev, pending = e.track_objects(rgb, depth, K, poses_in, slots, iteration, wait=False)
     for i, est in enumerate(estimators):
         est.pose_last = poses_dev[i].reshape(1, 4, 4)
         est.refiner.last_trans_update = est.refiner.last_rot_update = None
-        out.append(_uncentre(poses_host[i], est.model_center))
-    return out
+    centers = [est.model_center for est in estimators]
+    finish = lambda host: [_uncentre(host[i], c) for i, c in enumerate(centers)]
+    return finish(poses_host) if wait else PendingTrack(pending, finish)
 
 
-def track_cameras(views, iteration=2):
+def track_cameras(views, iteration=2, wait=True):
     """`[[est.track_one(rgb, depth, K, iteration) for est in ests] for ests, rgb, depth, K in views]` for objects seen by
     several camera streams (a multi-camera rig, or several recordings on one GPU), as ONE CUDA-graph launch per call
     (fp_track_cameras): every camera's frame is uploaded and filtered, and every (object, camera) pair is refined in one
@@ -480,13 +499,15 @@ def track_cameras(views, iteration=2):
     estimators share one engine and none appears twice, across cameras or within one; at most MAX_MESHES - 1 objects and
     MAX_CAMERAS cameras with objects.  A camera without estimators gives [] and its frame is not uploaded.  Each
     estimator keeps its mesh in the slot track_objects / register_objects use.  Host frames only (uint8 (H,W,3) rgb,
-    float32 (H,W) depth).  Returns one list of (4,4) float32 poses of the original meshes per camera."""
+    float32 (H,W) depth).  Returns one list of (4,4) float32 poses of the original meshes per camera.  wait=False returns
+    a PendingTrack as track_objects does."""
     views = [(list(ests), rgb, depth, K) for ests, rgb, depth, K in views]
     if any(torch.is_tensor(rgb) or torch.is_tensor(depth) for _, rgb, depth, _ in views):
         raise TypeError("track_cameras takes host frames (numpy); for device-resident frames call track_one per object")
     used = [v for v in views if v[0]]
     if not used:
-        return [[] for _ in views]
+        empty = [[] for _ in views]
+        return empty if wait else PendingTrack(None, lambda _: empty)
     estimators = [est for ests, _, _, _ in used for est in ests]
     e = _shared_engine_of(estimators, "track_cameras")
     if len(used) > MAX_CAMERAS:
@@ -497,12 +518,22 @@ def track_cameras(views, iteration=2):
     slots = [_object_slot(est, "track_cameras") for est in estimators]
     camera_of = [c for c, (ests, _, _, _) in enumerate(used) for _ in ests]
     poses_in = torch.stack([est.pose_last.reshape(4, 4) for est in estimators])
-    poses_dev, poses_host = e.track_cameras([(rgb, depth, K) for _, rgb, depth, K in used], poses_in, camera_of, slots, iteration)
+    frames = [(rgb, depth, K) for _, rgb, depth, K in used]
+    if wait:
+        poses_dev, poses_host = e.track_cameras(frames, poses_in, camera_of, slots, iteration)
+    else:
+        poses_dev, pending = e.track_cameras(frames, poses_in, camera_of, slots, iteration, wait=False)
     for i, est in enumerate(estimators):
         est.pose_last = poses_dev[i].reshape(1, 4, 4)
         est.refiner.last_trans_update = est.refiner.last_rot_update = None
-    flat = iter(_uncentre(poses_host[i], est.model_center) for i, est in enumerate(estimators))
-    return [[next(flat) for _ in ests] for ests, _, _, _ in views]
+    centers = [est.model_center for est in estimators]
+    counts = [len(ests) for ests, _, _, _ in views]
+
+    def finish(host):
+        flat = iter(_uncentre(host[i], c) for i, c in enumerate(centers))
+        return [[next(flat) for _ in range(n)] for n in counts]
+
+    return finish(poses_host) if wait else PendingTrack(pending, finish)
 
 
 def register_objects(estimators, K, rgb, depth, ob_masks, ob_ids=None, iteration=5):

@@ -321,6 +321,36 @@ int fp_track_objects(fp_ctx* ctx, const unsigned char* rgb_host, const float* de
 int fp_track_cameras(fp_ctx* ctx, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
                      const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
                      const float* poses_in_dev, int iterations, float* poses_out_dev, float* poses_out_host, void* stream);
+
+/* Non-blocking tracking: the host stages and submits the next call while the device still tracks the previous one.
+ * Each blocking tracking call is its submit followed by fp_track_wait on its ticket.
+ *   fp_track_cameras_submit / fp_track_objects_submit / fp_track_submit take the arguments of fp_track_cameras /
+ *   fp_track_objects / fp_track except poses_out_host / pose_out_host, and check them the same way: a refused call
+ *   enqueues nothing.  Each copies the host frames into pinned staging on the calling thread and enqueues the uploads,
+ *   the graph launch and the pose read-back on `stream`, then writes the call's ticket to *ticket.  Once it returns the
+ *   caller may reuse its host frame buffers; poses_out_dev (and fp_track's continuation pose) are complete in stream
+ *   order, so the next call may read them as its poses_in_dev without any host synchronisation.
+ *   The context has FP_TRACK_MAX_IN_FLIGHT staging sets, used in turn.  A submit that finds its set still in use
+ *   blocks only until the uploads of the call that used it have left it, not until that call's result is ready.
+ *   A submit on a stream other than the previous submit's makes its stream wait for the previous call first: the
+ *   context's device buffers are never used by two streams at once.
+ * fp_track_wait waits for the call's read-back and copies its poses (HOST [M][16], or [16] for fp_track) to
+ * poses_out_host (NULL: the result is dropped).  Tickets may be collected in any order, each once: an unknown or
+ * already collected ticket is refused and the context stays usable.  Asynchronous CUDA errors of the call are reported
+ * here.  Every other entry point that uses the context's staging, frames or workspaces first waits for the staging of
+ * the calls in flight to drain and orders its stream after the last submitted call; results stay pending until
+ * collected.  fp_destroy waits for calls in flight and frees uncollected results. */
+#define FP_TRACK_MAX_IN_FLIGHT 2
+int fp_track_cameras_submit(fp_ctx* ctx, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
+                            const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
+                            const float* poses_in_dev, int iterations, float* poses_out_dev, void* stream,
+                            unsigned long long* ticket);
+int fp_track_objects_submit(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host, const float* K, int H,
+                            int W, int M, const int* slots_host, const float* poses_in_dev, int iterations,
+                            float* poses_out_dev, void* stream, unsigned long long* ticket);
+int fp_track_submit(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
+                    const float* pose_in_dev, int iterations, float* pose_out_dev, void* stream, unsigned long long* ticket);
+int fp_track_wait(fp_ctx* ctx, unsigned long long ticket, float* poses_out_host);
 /* FoundationPose.register (estimater.py:159-240) applied to M objects of the same frame in one call; object i gives
  * exactly what fp_set_frame + fp_start_poses + fp_refine + fp_score give for that object alone, bit for bit.
  *   1. Checks every argument before anything is enqueued: slots_host HOST [M] loaded slot ids (one slot may appear
