@@ -164,15 +164,18 @@ struct CameraBufs {
   float fx = 0.f, fy = 0.f, cx = 0.f, cy = 0.f;
 };
 
-// The tracking calls keep up to FP_TRACK_MAX_IN_FLIGHT calls in flight, each uploading through a staging set of its
-// own: the host copies the next call's frames while the device still tracks the previous call.  Only the host side is
-// doubled: the device buffers the uploads land in are ordered by the stream.  A set is busy from its call's submit
-// until `uploaded` (recorded after the set's last host-to-device copy) has passed.  The register calls stage through
-// set 0 after draining every set (see drain).
+// All pinned staging of host inputs.  The tracking calls keep up to FP_TRACK_MAX_IN_FLIGHT calls in flight, each
+// uploading through a staging set of its own: the host copies the next call's frames while the device still tracks the
+// previous call.  Only the host side is doubled: the device buffers the uploads land in are ordered by the stream.
+// Every call that stages pageable host memory takes the next set in turn (take_set) and marks it busy after its last
+// copy out of it (set_busy): a set is busy until `uploaded`, recorded after that copy, has passed.
 constexpr int kMaxInFlight = FP_TRACK_MAX_IN_FLIGHT;
 struct StagingSet {
   PinnedBuf rgb[kMaxCameras], depth[kMaxCameras];
   PinnedBuf args;  // the camera table, then the slot ids and camera ids (layout of fp_ctx::args)
+  // the register calls' masks of every object at its byte offset, and their (offsets [M + 1], camera ids [M], one int of
+  // padding, each object's mask byte offset size_t [M]); fp_start_poses' mask; fp_register's start poses
+  PinnedBuf masks, ints, poses;
   OwnedEvent uploaded;
   bool busy = false;
 };
@@ -207,7 +210,7 @@ struct fp_ctx {
   // workspaces (sized for cap_n hypotheses)
   int cap_n = 0;
   fp::DevBuf crops, act0, a1, a2, a3, ab0, ab1, ab2, c0, c1, c2, tok, qkv, att, x1pre, x1, ff, x2pre;
-  fp::DevBuf head_out, poses_a, poses_b, feats, tail_qkv, tail_attn, tail_proj, scores, best;
+  fp::DevBuf head_out, poses_a, poses_b, feats, tail_qkv, tail_attn, scores, best;
   int tail_cap = 0;
   float fold_c = 0.f;      // linear.weight . out_proj.bias + linear.bias (by-value kernel parameter)
   fp::DevBuf fold_v, tail_counter;  // out_proj^T linear.weight [512]; arg-max ticket
@@ -248,10 +251,8 @@ struct fp_ctx {
   fp::DevBuf args;
   int cam_grid_h = 0, cam_grid_w = 0;  // the tracking calls' frame-preparation grid: the largest frame seen
   // fp_register_objects / _cameras: row offsets of the objects' hypotheses [M + 1] and the objects' camera ids [M], the
-  // objects' feature rows [sum N][512], each object's byte offset into mask_buf; pinned staging of the masks and of
-  // (offsets, camera ids, mask offsets)
+  // objects' feature rows [sum N][512], each object's byte offset into mask_buf
   fp::DevBuf seg_off, reg_feats, mask_off;
-  fp::PinnedBuf stage_masks, stage_ints;
   // fp_vis: the crop producer's vis record [N][2][160][160] float4 and the per-row depth ranges [N] float2, sized at the
   // first call for the largest N seen; never allocated by the other entry points
   fp::DevBuf vis_rec, vis_range;
@@ -303,7 +304,6 @@ static int ensure_tail(fp_ctx* c, int L) {
   int rc = 0;
   rc |= dev_alloc(c->epoch, c->tail_qkv, (size_t)L * 1536 * 4);
   rc |= dev_alloc(c->epoch, c->tail_attn, (size_t)L * 512 * 4);
-  rc |= dev_alloc(c->epoch, c->tail_proj, (size_t)L * 512 * 4);
   rc |= dev_alloc(c->epoch, c->scores, (size_t)L * 4);
   rc |= dev_alloc(c->epoch, c->best, 16);
   if (rc) return -2;
@@ -765,28 +765,74 @@ static int refine_body(fp_ctx* c, int N, int iterations, cudaStream_t s2, const 
   return 0;
 }
 
+// Copies `bytes` of host memory `src` into the pinned `stage` (grown as needed) and enqueues its upload to `dst`: the
+// caller's memory is free again once this returns.
+static int stage_copy(void* dst, PinnedBuf& stage, const void* src, size_t bytes, cudaStream_t st) {
+  FP_TRY(pinned_alloc(nullptr, stage, bytes));
+  memcpy(stage.p, src, bytes);
+  FP_CUDA_OK(cudaMemcpyAsync(dst, stage.p, bytes, cudaMemcpyHostToDevice, st));
+  return 0;
+}
+
 // Uploads one camera's frame through its staging (free: the set is not busy).  The two uploads are issued as soon as
 // their staging copy is done — the depth DMA runs under the host's rgb copy, the rgb DMA under the next camera's copies
 // or the graph launch — instead of being nodes of the graph (measured: -40 us per frame)
 static int upload_staged_frame(CameraBufs& b, PinnedBuf& stage_rgb, PinnedBuf& stage_depth, const unsigned char* rgb_host,
                                const float* depth_host, size_t npix, cudaStream_t st) {
-  memcpy(stage_depth.p, depth_host, npix * 4);
-  FP_CUDA_OK(cudaMemcpyAsync(b.depth_raw.p, stage_depth.p, npix * 4, cudaMemcpyHostToDevice, st));
-  memcpy(stage_rgb.p, rgb_host, npix * 3);
-  FP_CUDA_OK(cudaMemcpyAsync(b.rgb_raw.p, stage_rgb.p, npix * 3, cudaMemcpyHostToDevice, st));
+  FP_TRY(stage_copy(b.depth_raw.p, stage_depth, depth_host, npix * 4, st));
+  return stage_copy(b.rgb_raw.p, stage_rgb, rgb_host, npix * 3, st);
+}
+
+// The one place that decides which staging set a call uses: the next one in turn, waited for first, if it is still
+// busy, until the uploads of the call that used it have left it.
+static int take_set(fp_ctx* c, StagingSet*& set) {
+  set = &c->sets[c->next_set];
+  if (set->busy) {
+    FP_CUDA_OK(cudaEventSynchronize(set->uploaded.e));
+    set->busy = false;
+  }
+  c->next_set = (c->next_set + 1) % kMaxInFlight;
   return 0;
 }
 
-// Waits until every tracking call in flight has moved its uploads out of its staging set, and orders `st` after the
-// last call submitted (its device buffers and the context's frames are then free on `st`).  Every entry point that
-// uses the context's staging, frames or workspaces calls this first; the tracking submits do not, they wait only for
-// the set they reuse.  Results are collected separately (fp_track_wait).
-static int drain(fp_ctx* c, cudaStream_t st) {
-  for (StagingSet& s : c->sets)
-    if (s.busy) {
-      FP_CUDA_OK(cudaEventSynchronize(s.uploaded.e));
-      s.busy = false;
-    }
+// After a call's last copy out of `set`: the set stays busy until `st` has passed that copy.
+static int set_busy(StagingSet& set, cudaStream_t st) {
+  FP_CUDA_OK(set.uploaded.record(st));
+  set.busy = true;
+  return 0;
+}
+
+// Host memory that the device cannot read in place, so a copy from it may wait on the stream.  Page-locked (and device
+// or managed) memory is anything cudaPointerGetAttributes knows.
+static bool pageable(const void* p) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();  // not sticky; keep it out of the next caller's error check
+    return true;
+  }
+  return a.type == cudaMemoryTypeUnregistered;
+}
+
+// Uploads `bytes` of the caller's host memory `src` to `dst` on `st`.  Page-locked memory is copied straight from the
+// caller's buffer, which must stay untouched until `st` has passed the copy; pageable memory goes through `stage` of the
+// next staging set, so the caller may reuse it once this returns and the host does not wait on the stream for it.
+static int upload_host(fp_ctx* c, void* dst, const void* src, size_t bytes, PinnedBuf StagingSet::*stage, cudaStream_t st) {
+  if (!pageable(src)) {
+    FP_CUDA_OK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st));
+    return 0;
+  }
+  StagingSet* set;
+  FP_TRY(take_set(c, set));
+  const int staged = stage_copy(dst, set->*stage, src, bytes, st);
+  FP_TRY(set_busy(*set, st));  // after a failure too: a copy may have been enqueued
+  return staged;
+}
+
+// Orders `st` after the last tracking call submitted: its device buffers and the context's frames are then free on `st`
+// (a call on the same stream is ordered already).  Every entry point that uses the context's frames or workspaces
+// calls this first.  It never waits on the host: a staging set is waited for only by the call that takes it again
+// (take_set), and results are collected separately (fp_track_wait).
+static int order_after_track(fp_ctx* c, cudaStream_t st) {
   if (c->last_done && st != c->last_stream) FP_CUDA_OK(cudaStreamWaitEvent(st, c->last_done, 0));
   return 0;
 }
@@ -854,13 +900,9 @@ static int track_cameras_submit(fp_ctx* c, int C, const unsigned char* const* rg
                                 const float* K, const int* H, const int* W, int M, const int* camera_of,
                                 const int* slots_host, const float* poses_in_dev, int iterations, float* poses_out_dev,
                                 cudaStream_t st, unsigned long long* ticket, float* poses_keep_dev = nullptr) {
-  StagingSet& set = c->sets[c->next_set];
-  if (set.busy) {
-    FP_CUDA_OK(cudaEventSynchronize(set.uploaded.e));
-    set.busy = false;
-  }
-  // the context's device buffers are never used by two streams at once
-  if (c->last_done && st != c->last_stream) FP_CUDA_OK(cudaStreamWaitEvent(st, c->last_done, 0));
+  StagingSet* set;
+  FP_TRY(take_set(c, set));
+  FP_TRY(order_after_track(c, st));  // the context's device buffers are never used by two streams at once
   Readback* rb = nullptr;
   for (auto& r : c->readbacks)
     if (r->ticket == 0) rb = r.get();
@@ -872,11 +914,9 @@ static int track_cameras_submit(fp_ctx* c, int C, const unsigned char* const* rg
   FP_TRY(pinned_alloc(nullptr, rb->poses, (size_t)M * 64));
   c->has_frame = false;
   int H_max = 0, W_max = 0;
-  const int staged = stage_track_call(c, set, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, st, H_max, W_max);
+  const int staged = stage_track_call(c, *set, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, st, H_max, W_max);
   // whatever was staged before a failure is still on its way out: the set stays busy until then
-  FP_CUDA_OK(set.uploaded.record(st));
-  set.busy = true;
-  c->next_set = (c->next_set + 1) % kMaxInFlight;
+  FP_TRY(set_busy(*set, st));
   FP_TRY(staged);
   if (H_max > c->cam_grid_h || W_max > c->cam_grid_w) {
     // the frame-preparation grid is a by-value launch parameter: it covers the largest frame seen, the blocks outside
@@ -1049,23 +1089,29 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
   FP_TRY(dev_alloc(c->epoch, c->mask_buf, mask_bytes));
   FP_TRY(dev_alloc(c->epoch, c->mask_stats, (size_t)M * 6 * sizeof(unsigned int)));
   if (!by_value) FP_TRY(dev_alloc(c->epoch, c->mask_off, (size_t)M * sizeof(size_t)));
-  // pinned staging (never read by a captured graph): the copies below leave as soon as they are enqueued.  stage_ints:
-  // offsets [M + 1], camera of every object [M], one int of padding, each object's mask byte offset size_t [M]
-  FP_TRY(pinned_alloc(nullptr, c->stage_masks, mask_bytes));
-  FP_TRY(pinned_alloc(nullptr, c->stage_ints, (size_t)(2 * M + 2) * sizeof(int) + (size_t)M * sizeof(size_t)));
+  // pinned staging (never read by a captured graph): the copies below leave as soon as they are enqueued
+  StagingSet* set;
+  FP_TRY(take_set(c, set));
+  // every return from here on, a failure's included, leaves the set busy until the copies enqueued from it have left it
+  struct MarkBusy {
+    StagingSet& set;
+    cudaStream_t st;
+    ~MarkBusy() { set_busy(set, st); }
+  } mark_busy{*set, st};
+  FP_TRY(pinned_alloc(nullptr, set->masks, mask_bytes));
+  FP_TRY(pinned_alloc(nullptr, set->ints, (size_t)(2 * M + 2) * sizeof(int) + (size_t)M * sizeof(size_t)));
   c->has_frame = false;
   int H_max, W_max;
-  StagingSet& set = c->sets[0];  // free: the entry point drained every set
-  FP_TRY(setup_cameras(c, set, C, rgb_host, depth_host, K, H, W, max_pass, total, st, H_max, W_max));
-  int* ints = reinterpret_cast<int*>(c->stage_ints.p);
+  FP_TRY(setup_cameras(c, *set, C, rgb_host, depth_host, K, H, W, max_pass, total, st, H_max, W_max));
+  int* ints = reinterpret_cast<int*>(set->ints.p);
   size_t* stage_mask_off = reinterpret_cast<size_t*>(ints + 2 * M + 2);
   memcpy(ints, off.data(), (size_t)(M + 1) * sizeof(int));
   memcpy(ints + M + 1, camera_of, (size_t)M * sizeof(int));
   memcpy(stage_mask_off, mask_at.data(), (size_t)M * sizeof(size_t));
   for (int i = 0; i < M; ++i)
-    memcpy(static_cast<unsigned char*>(c->stage_masks.p) + mask_at[i], masks_host[i], mask_at[i + 1] - mask_at[i]);
+    memcpy(static_cast<unsigned char*>(set->masks.p) + mask_at[i], masks_host[i], mask_at[i + 1] - mask_at[i]);
   // the ids of the pass starting at row r0 are staged at 2 * r0 after the table: its slot ids, then its camera ids
-  int* ids = reinterpret_cast<int*>(static_cast<char*>(set.args.p) + kTableBytes);
+  int* ids = reinterpret_cast<int*>(static_cast<char*>(set->args.p) + kTableBytes);
   for (size_t p = 0; p + 1 < pass_obj.size(); ++p) {
     const int row0 = off[pass_obj[p]], n = off[pass_obj[p + 1]] - row0;
     for (int i = pass_obj[p]; i < pass_obj[p + 1]; ++i) {
@@ -1077,14 +1123,14 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
   ScoreTailParams tp;
   FP_TRY(segmented_tail_params(c, reinterpret_cast<const float*>(c->reg_feats.p), ints, M, /*trailing=*/M, scores_out_dev,
                                best_out_dev, st, caller, tp));
-  FP_CUDA_OK(cudaMemcpyAsync(c->mask_buf.p, c->stage_masks.p, mask_bytes, cudaMemcpyHostToDevice, st));
+  FP_CUDA_OK(cudaMemcpyAsync(c->mask_buf.p, set->masks.p, mask_bytes, cudaMemcpyHostToDevice, st));
   const CameraDev* cams_dev = by_value ? nullptr : reinterpret_cast<const CameraDev*>(c->args.p);
   // estimater.py:173-174, :214 once per camera for every object: erode + bilateral, depth2xyzmap(zfar = inf)
   if (by_value) {
     FP_TRY(set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->cam[0].rgb_raw.p),
                               reinterpret_cast<const float*>(c->cam[0].depth_raw.p), FP_FRAME_FILTER_DEPTH, INFINITY, st));
   } else {
-    FP_CUDA_OK(cudaMemcpyAsync(c->args.p, set.args.p, kTableBytes, cudaMemcpyHostToDevice, st));
+    FP_CUDA_OK(cudaMemcpyAsync(c->args.p, set->args.p, kTableBytes, cudaMemcpyHostToDevice, st));
     FP_CUDA_OK(cudaMemcpyAsync(c->mask_off.p, stage_mask_off, (size_t)M * sizeof(size_t), cudaMemcpyHostToDevice, st));
     FP_TRY(frame_prep_cameras_launch(cams_dev, C, H_max, W_max, INFINITY, st));
   }
@@ -1379,7 +1425,7 @@ int fp_set_frame(fp_ctx* c, const unsigned char* rgb, const float* depth, const 
   FP_REQUIRE(H > 0 && W > 0, "fp_set_frame: empty frame");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(drain(c, st));
+  FP_TRY(order_after_track(c, st));
   const size_t npix = (size_t)H * W;
   c->has_frame = false;
   const bool on_dev = (flags & FP_FRAME_ON_DEVICE) != 0;
@@ -1390,8 +1436,17 @@ int fp_set_frame(fp_ctx* c, const unsigned char* rgb, const float* depth, const 
   const float* depth_dev = depth;
   if (!on_dev) {
     CameraBufs& f = c->cam[0];
-    FP_CUDA_OK(cudaMemcpyAsync(f.rgb_raw.p, rgb, npix * 3, cudaMemcpyHostToDevice, st));
-    FP_CUDA_OK(cudaMemcpyAsync(f.depth_raw.p, depth, npix * 4, cudaMemcpyHostToDevice, st));
+    if (pageable(rgb) || pageable(depth)) {
+      StagingSet* set;
+      FP_TRY(take_set(c, set));
+      const int staged = upload_staged_frame(f, set->rgb[0], set->depth[0], rgb, depth, npix, st);
+      FP_TRY(set_busy(*set, st));
+      FP_TRY(staged);
+    } else {
+      // page-locked frames, fp_group_register's among them, are read in place: one host copy fewer
+      FP_CUDA_OK(cudaMemcpyAsync(f.rgb_raw.p, rgb, npix * 3, cudaMemcpyHostToDevice, st));
+      FP_CUDA_OK(cudaMemcpyAsync(f.depth_raw.p, depth, npix * 4, cudaMemcpyHostToDevice, st));
+    }
     rgb_dev = reinterpret_cast<const unsigned char*>(f.rgb_raw.p);
     depth_dev = reinterpret_cast<const float*>(f.depth_raw.p);
   }
@@ -1407,7 +1462,7 @@ int fp_set_xyz_map(fp_ctx* c, const float* xyz, void* stream) {
   FP_REQUIRE(c->has_frame, "fp_set_xyz_map: no frame (call fp_set_frame first)");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(drain(c, st));
+  FP_TRY(order_after_track(c, st));
   // [H][W][3] (host or device) -> the float4-per-pixel layout the crop kernel samples
   const CameraBufs& f = c->cam[0];
   FP_CUDA_OK(cudaMemcpy2DAsync(f.xyz.p, 16, xyz, 12, 12, (size_t)f.H * f.W, cudaMemcpyDefault, st));
@@ -1422,7 +1477,7 @@ int fp_get_depth(fp_ctx* c, int camera, float* depth_out_dev, float* xyz_out_dev
              c->n_frames - 1);
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(drain(c, st));
+  FP_TRY(order_after_track(c, st));
   const CameraBufs& b = c->cam[camera];
   if (hw_out) {
     hw_out[0] = b.H;
@@ -1443,13 +1498,13 @@ int fp_start_poses(fp_ctx* c, const unsigned char* mask, int mask_on_device, con
   FP_REQUIRE(c->has_frame, "fp_start_poses: no frame (call fp_set_frame first)");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(drain(c, st));
+  FP_TRY(order_after_track(c, st));
   const CameraDev frame = camera_dev(c, 0);
   const size_t npix = (size_t)frame.H * frame.W;
   const unsigned char* mdev = mask;
   if (!mask_on_device) {
     FP_TRY(dev_alloc(c->epoch, c->mask_buf, npix));
-    FP_CUDA_OK(cudaMemcpyAsync(c->mask_buf.p, mask, npix, cudaMemcpyHostToDevice, st));
+    FP_TRY(upload_host(c, c->mask_buf.p, mask, npix, &StagingSet::masks, st));
     mdev = reinterpret_cast<const unsigned char*>(c->mask_buf.p);
   }
   FP_TRY(dev_alloc(c->epoch, c->mask_stats, 64));
@@ -1465,7 +1520,7 @@ int fp_make_crops(fp_ctx* c, const float* poses, int N, int mode, void* crops_ou
   FP_REQUIRE(mode == 0 || mode == 1, "fp_make_crops: mode must be 0 (refiner) or 1 (scorer)");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(drain(c, st));
+  FP_TRY(order_after_track(c, st));
   if (N == 0) return 0;
   FP_TRY(ensure_capacity(c, N));
   FP_TRY(make_crops(c, poses, N, mode, dbg_out, win_out, nullptr, st));
@@ -1479,7 +1534,7 @@ int fp_crop_stats(fp_ctx* c, const float* poses, int N, int mode, int* stats_out
   FP_REQUIRE(c && poses && stats_out_host && N > 0, "fp_crop_stats: bad argument");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(drain(c, st));
+  FP_TRY(order_after_track(c, st));
   FP_TRY(ensure_capacity(c, N));
   FP_TRY(dev_alloc(c->epoch, c->crop_stats, 16));
   FP_CUDA_OK(cudaMemsetAsync(c->crop_stats.p, 0, 16, st));
@@ -1496,7 +1551,7 @@ int fp_op_refine_net(fp_ctx* c, const void* crops, int N, float* trans_out, floa
   FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(drain(c, st));
+  FP_TRY(order_after_track(c, st));
   if (N == 0) return 0;
   FP_TRY(ensure_capacity(c, N));
   FP_TRY(crops_import(c, crops, N, st));
@@ -1515,7 +1570,7 @@ int fp_op_score_feats(fp_ctx* c, const void* crops, int N, float* feats_out, voi
   FP_REQUIRE(c->net[1].loaded, "scorer weights not loaded");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(drain(c, st));
+  FP_TRY(order_after_track(c, st));
   if (N == 0) return 0;
   FP_TRY(ensure_capacity(c, N));
   FP_TRY(crops_import(c, crops, N, st));
@@ -1558,7 +1613,7 @@ long long fp_op_encoder(fp_ctx* c, int which, const void* crops, int N, int last
   DeviceGuard dg(c->device);
   if (check_device_ptr(crops, "crops", fn) || check_device_ptr(out, "out", fn)) return -1;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(drain(c, st));
+  FP_TRY(order_after_track(c, st));
   if (N == 0) return 0;
   int shape[4];
   enc_out_shape(last, N, shape);
@@ -1579,7 +1634,7 @@ int fp_refine(fp_ctx* c, const float* poses_in, int N, int iterations, float* po
   FP_REQUIRE(c->mesh[0].loaded && c->has_frame, "fp_refine: needs fp_set_mesh and fp_set_frame first");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(drain(c, st));
+  FP_TRY(order_after_track(c, st));
   if (N == 0) return 0;
   FP_TRY(ensure_capacity(c, N));
   float* pa = reinterpret_cast<float*>(c->poses_a.p);
@@ -1604,7 +1659,7 @@ int fp_score_features(fp_ctx* c, const float* poses, int N, float* feats_out, vo
   FP_REQUIRE(c->mesh[0].loaded && c->has_frame, "fp_score_features: needs fp_set_mesh and fp_set_frame first");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(drain(c, st));
+  FP_TRY(order_after_track(c, st));
   if (N == 0) return 0;
   FP_TRY(ensure_capacity(c, N));
   float* ps = reinterpret_cast<float*>(c->pose_stage.p);
@@ -1630,7 +1685,7 @@ int fp_score_tail(fp_ctx* c, const float* feats, int L, float* scores_out, int* 
   FP_REQUIRE(c->net[1].loaded, "scorer weights not loaded");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(drain(c, st));
+  FP_TRY(order_after_track(c, st));
   if (L == 0) return 0;
   FP_TRY(ensure_tail(c, L));
   return score_tail_launch(score_tail_params(c, feats, L, scores_out, best_out), st);
@@ -1647,7 +1702,7 @@ int fp_op_score_tail_segments(fp_ctx* c, const float* feats, int L, const int* s
   FP_REQUIRE(seg_host[n_seg] == L, "%s: the last segment ends at row %d, not at L = %d", fn, seg_host[n_seg], L);
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(drain(c, st));
+  FP_TRY(order_after_track(c, st));
   ScoreTailParams p;
   FP_TRY(segmented_tail_params(c, feats, seg_host, n_seg, /*trailing=*/0, scores_out, best_out, st, fn, p));
   return score_tail_launch(p, st);
@@ -1671,17 +1726,16 @@ int fp_register(fp_ctx* c, const float* poses_host, int N, int iterations, float
   FP_REQUIRE(c && poses_host && poses_out_host && scores_out_host && best_out_host && N > 0, "fp_register: bad argument");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(drain(c, st));
+  FP_TRY(order_after_track(c, st));
   FP_TRY(ensure_capacity(c, N));
   FP_TRY(ensure_tail(c, N));
-  // poses_b is the loop's ping-pong partner; stage the input in `feats`' neighbour: use tail_proj as scratch
-  float* pin = reinterpret_cast<float*>(c->tail_proj.p);  // >= N*512 floats
-  float* pout = pin + (size_t)N * 16;
-  FP_CUDA_OK(cudaMemcpyAsync(pin, poses_host, (size_t)N * 64, cudaMemcpyHostToDevice, st));
-  FP_TRY(fp_refine(c, pin, N, iterations, pout, nullptr, nullptr, stream));
-  // keep the refined poses out of the tail's scratch: copy to poses_b's idle half (poses_a/b are free now)
+  // the start poses go up to pose_stage, which fp_refine reads before its loop and takes its result back into; the
+  // refined poses then move to poses_b (idle after the loop), since fp_score stages its input in pose_stage
+  float* ps = reinterpret_cast<float*>(c->pose_stage.p);
+  FP_TRY(upload_host(c, ps, poses_host, (size_t)N * 64, &StagingSet::poses, st));
+  FP_TRY(fp_refine(c, ps, N, iterations, ps, nullptr, nullptr, stream));
   float* refined = reinterpret_cast<float*>(c->poses_b.p);
-  FP_CUDA_OK(cudaMemcpyAsync(refined, pout, (size_t)N * 64, cudaMemcpyDeviceToDevice, st));
+  FP_CUDA_OK(cudaMemcpyAsync(refined, ps, (size_t)N * 64, cudaMemcpyDeviceToDevice, st));
   FP_TRY(fp_score(c, refined, N, reinterpret_cast<float*>(c->scores.p), reinterpret_cast<int*>(c->best.p), stream));
   FP_CUDA_OK(cudaMemcpyAsync(poses_out_host, refined, (size_t)N * 64, cudaMemcpyDeviceToHost, st));
   FP_CUDA_OK(cudaMemcpyAsync(scores_out_host, c->scores.p, (size_t)N * 4, cudaMemcpyDeviceToHost, st));
@@ -1747,7 +1801,7 @@ int fp_vis_crops(fp_ctx* c, const float* poses, int N, int mode, float* rec_out,
   FP_API_BEGIN
   FP_REQUIRE(c && poses && rec_out && N > 0 && (mode == 0 || mode == 1), "fp_vis_crops: bad argument");
   DeviceGuard dg(c->device);
-  FP_TRY(drain(c, reinterpret_cast<cudaStream_t>(stream)));
+  FP_TRY(order_after_track(c, reinterpret_cast<cudaStream_t>(stream)));
   FP_TRY(ensure_capacity(c, N));
   return make_crops(c, poses, N, mode, nullptr, nullptr, nullptr, reinterpret_cast<cudaStream_t>(stream), nullptr, nullptr,
                     nullptr, reinterpret_cast<float4*>(rec_out));
@@ -1764,7 +1818,7 @@ int fp_vis(fp_ctx* c, int kind, const float* poses_a, const float* poses_b, int 
   FP_REQUIRE(kind == 0 || order, "fp_vis: the scorer canvas needs the row order");
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(drain(c, st));
+  FP_TRY(order_after_track(c, st));
   int hw[2];
   FP_TRY(vis_canvas_size(kind, N, hw, hw + 1));
   if (hw_out) {
@@ -1861,7 +1915,7 @@ int fp_register_objects(fp_ctx* c, const unsigned char* rgb_host, const float* d
   // everything is checked before anything is enqueued
   FP_TRY(check_slots(c, M, slots_host, "fp_register_objects"));
   DeviceGuard dg(c->device);
-  FP_TRY(drain(c, reinterpret_cast<cudaStream_t>(stream)));
+  FP_TRY(order_after_track(c, reinterpret_cast<cudaStream_t>(stream)));
   const size_t npix = (size_t)H * W;
   std::vector<const unsigned char*> masks(M);
   for (int i = 0; i < M; ++i) masks[i] = masks_host + (size_t)i * npix;
@@ -1888,7 +1942,7 @@ int fp_register_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host, 
   for (int i = 0; i < M; ++i) FP_REQUIRE(masks_host[i], "fp_register_cameras: object %d: null mask", i);
   FP_TRY(check_slots(c, M, slots_host, "fp_register_cameras"));
   DeviceGuard dg(c->device);
-  FP_TRY(drain(c, reinterpret_cast<cudaStream_t>(stream)));
+  FP_TRY(order_after_track(c, reinterpret_cast<cudaStream_t>(stream)));
   return register_cameras_body(c, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, n_hyp_host, masks_host,
                                rot_grids_dev, iterations, poses_out_dev, scores_out_dev, best_out_dev, info_out_dev,
                                reinterpret_cast<cudaStream_t>(stream), /*by_value=*/false);
@@ -1915,7 +1969,7 @@ int fp_op_pose_update(fp_ctx* c, const float* poses_in, const float* trans, cons
   FP_TRY(check_slots(c, mesh_of_host ? N : 1, mesh_of_host ? mesh_of_host : &slot0, fn));
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(drain(c, st));
+  FP_TRY(order_after_track(c, st));
   if (N == 0) return 0;
   const int* mesh_of = nullptr;
   if (mesh_of_host) {

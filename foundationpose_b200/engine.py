@@ -5,7 +5,6 @@ torch is used for device memory, streams and (in parallel.py) torch.distributed 
 computation on the hot path happens inside the C-ABI library.
 """
 import ctypes as C
-import os
 import weakref
 
 import numpy as np
@@ -87,7 +86,6 @@ FRAME_ON_DEVICE = 1
 MAX_MESHES = 64  # FP_MAX_MESHES: mesh slots per context
 MAX_CAMERAS = 16  # FP_MAX_CAMERAS: camera streams per fp_track_cameras / fp_register_cameras call
 MAX_IN_FLIGHT = 2  # FP_TRACK_MAX_IN_FLIGHT: tracking calls in flight per context (its staging sets)
-_NO_PIN = os.environ.get("FPOSE_NO_PIN") == "1"  # A/B: skip the pinned staging of host frames
 FRAME_FILTER_DEPTH = 2
 
 
@@ -434,7 +432,8 @@ class Engine:
         return poses, scores, best, info
 
     def set_frame(self, rgb, depth, K, filter_depth=True, zfar=float("inf")):
-        """rgb uint8 (H,W,3), depth float32 (H,W): numpy / CPU tensors (pinned for async H2D) or CUDA tensors."""
+        """rgb uint8 (H,W,3), depth float32 (H,W): numpy / CPU tensors or CUDA tensors.  Pageable host frames are staged
+        by the library and may be reused once this returns."""
         Kf = (C.c_float * 9)(*[float(x) for x in np.asarray(K, dtype=np.float64).reshape(-1)])
         flags = FRAME_FILTER_DEPTH if filter_depth else 0
         if torch.is_tensor(rgb) and rgb.is_cuda:
@@ -443,33 +442,17 @@ class Engine:
             depth = depth.contiguous().float()
             assert rgb.dtype == torch.uint8
             flags |= FRAME_ON_DEVICE
-            H, W = depth.shape
-            rp, dp = _p(rgb), _p(depth)
         else:
             rgb = rgb if torch.is_tensor(rgb) else torch.from_numpy(np.ascontiguousarray(rgb, dtype=np.uint8))
             depth = depth if torch.is_tensor(depth) else torch.from_numpy(np.ascontiguousarray(depth, dtype=np.float32))
             rgb = rgb.contiguous()
             depth = depth.contiguous()
             assert rgb.dtype == torch.uint8 and depth.dtype == torch.float32
-            H, W = depth.shape
-            if not rgb.is_pinned() and not _NO_PIN:
-                # pageable host memory makes cudaMemcpyAsync synchronous and staged by the driver: stage through a
-                # pinned buffer owned by the engine (the previous frame's copy has been consumed: same stream)
-                pin = getattr(self, "_pin", None)
-                if pin is None or pin[0].shape != rgb.shape or pin[1].shape != depth.shape:
-                    torch.cuda.current_stream().synchronize()
-                    pin = self._pin = (torch.empty(rgb.shape, dtype=torch.uint8).pin_memory(), torch.empty(depth.shape, dtype=torch.float32).pin_memory(),
-                                       torch.cuda.Event())
-                else:
-                    pin[2].synchronize()
-                pin[0].copy_(rgb)
-                pin[1].copy_(depth)
-                rgb, depth = pin[0], pin[1]
-            rp, dp = _p(rgb), _p(depth)
-        self._frame_keep = (rgb, depth)
-        _lib.check(lib.fp_set_frame(self._h, rp, dp, Kf, H, W, flags, float(zfar), _stream()), "fp_set_frame")
-        if getattr(self, "_pin", None) is not None and rgb is self._pin[0]:
-            self._pin[2].record()  # the staging buffers may be overwritten once this point of the stream has passed
+        H, W = depth.shape
+        # device and page-locked frames are read in place after the call returns, in stream order: keep them until then
+        in_place = rgb.is_cuda or (rgb.is_pinned() and depth.is_pinned())
+        self._frame_keep = (rgb, depth) if in_place else None
+        _lib.check(lib.fp_set_frame(self._h, _p(rgb), _p(depth), Kf, H, W, flags, float(zfar), _stream()), "fp_set_frame")
         self.frame_hw = (H, W)
 
     def set_xyz_map(self, xyz_map):
@@ -503,7 +486,9 @@ class Engine:
             mask = torch.as_tensor(np.ascontiguousarray(mask))
         m = (mask if mask.dtype == torch.bool else (mask > 0)).to(torch.uint8).contiguous()
         on_dev = 1 if m.is_cuda else 0
-        self._mask_keep = m
+        # a device mask is read after the call returns, in stream order; the library stages a host mask (a new,
+        # pageable tensor) before it returns
+        self._mask_keep = m if on_dev else None
         poses = torch.empty(N, 4, 4, dtype=torch.float32, device="cuda")
         info = torch.empty(4, dtype=torch.float32, device="cuda")
         _lib.check(lib.fp_start_poses(self._h, _p(m), on_dev, _p(rot_grid), N, _p(poses), _p(info), _stream()), "fp_start_poses")
@@ -579,12 +564,12 @@ class Engine:
         return scores, best
 
     def register_host(self, poses_host, iterations, out_poses=None, out_scores=None):
-        """fp_register: pinned host buffers in, host buffers out (synchronous)."""
+        """fp_register: host buffers in and out (synchronous)."""
         poses_host = poses_host if torch.is_tensor(poses_host) else torch.from_numpy(np.ascontiguousarray(poses_host, dtype=np.float32))
         poses_host = poses_host.reshape(-1, 4, 4).contiguous()
         N = len(poses_host)
-        out_poses = torch.empty(N, 4, 4, dtype=torch.float32).pin_memory() if out_poses is None else out_poses
-        out_scores = torch.empty(N, dtype=torch.float32).pin_memory() if out_scores is None else out_scores
+        out_poses = torch.empty(N, 4, 4, dtype=torch.float32) if out_poses is None else out_poses
+        out_scores = torch.empty(N, dtype=torch.float32) if out_scores is None else out_scores
         best = torch.zeros(1, dtype=torch.int32)
         _lib.check(lib.fp_register(self._h, _p(poses_host), N, int(iterations), _p(out_poses), _p(out_scores), _p(best),
                                    _stream()), "fp_register")

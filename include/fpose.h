@@ -214,6 +214,10 @@ int fp_set_mesh_slot(fp_ctx* ctx, int slot, int V, int F, const float* pos, cons
  * front-face winding sign used for back-face culling (0 = both sides are rendered, as nvdiffrast does), V, F}. */
 int fp_mesh_info(fp_ctx* ctx, int* info);
 
+/* Host inputs of fp_set_frame, fp_start_poses and fp_register.  Pageable host memory is copied into the context's
+ * pinned staging before the call returns: the caller may reuse it at once, and the call does not wait on `stream` for
+ * it.  Page-locked memory (cudaHostAlloc, cudaHostRegister) is copied straight from the caller's buffer on `stream`:
+ * the caller keeps it unchanged until `stream` has passed the call. */
 #define FP_FRAME_ON_DEVICE 1    /* rgb/depth are device pointers (default: host, copied on `stream`) */
 #define FP_FRAME_FILTER_DEPTH 2 /* erode_depth + bilateral_filter_depth (estimater.py:173-174, :257-258) */
 /* Uploads one RGB-D frame (rgb uint8 [H][W][3], depth float32 [H][W] metres, K row-major 3x3), runs
@@ -337,9 +341,9 @@ int fp_track_cameras(fp_ctx* ctx, int C, const unsigned char* const* rgb_host, c
  * fp_track_wait waits for the call's read-back and copies its poses (HOST [M][16], or [16] for fp_track) to
  * poses_out_host (NULL: the result is dropped).  Tickets may be collected in any order, each once: an unknown or
  * already collected ticket is refused and the context stays usable.  Asynchronous CUDA errors of the call are reported
- * here.  Every other entry point that uses the context's staging, frames or workspaces first waits for the staging of
- * the calls in flight to drain and orders its stream after the last submitted call; results stay pending until
- * collected.  fp_destroy waits for calls in flight and frees uncollected results. */
+ * here.  Every other entry point that uses the context's frames or workspaces first orders its stream after the last
+ * submitted call, on the device: it does not wait on the host.  A staging set is waited for only by the call that
+ * takes it again.  Results stay pending until collected.  fp_destroy waits for calls in flight and frees uncollected results. */
 #define FP_TRACK_MAX_IN_FLIGHT 2
 int fp_track_cameras_submit(fp_ctx* ctx, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
                             const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
