@@ -1,518 +1,25 @@
-// fp_api.cu — the product C ABI (include/fpose.h): context, weights, mesh, frame, and the per-frame
-// hot loop (crops -> encoder -> heads -> pose update, K times; then scoring) enqueued on one stream
-// with no host synchronisation.
+// fp_api.cu — the product C ABI (include/fpose.h): context, meshes, frames, and the per-frame hot loop (crops ->
+// encoder -> heads -> pose update, K times; then scoring) enqueued on one stream with no host synchronisation.  The
+// network plan the loop launches is in fp_net.cu, the operator hooks in fp_api_ops.cu, fp_group in fp_group.cu.
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
-#include <exception>
-#include <map>
 #include <memory>
-#include <string>
 #include <tuple>
-#include <utility>
 #include <vector>
 
 #include "../../include/fpose.h"
 #include "fp_attn.cuh"
 #include "fp_common.cuh"
 #include "fp_crop.cuh"
+#include "fp_ctx.cuh"
 #include "fp_depth.cuh"
 #include "fp_gemm.cuh"
 #include "fp_vis.cuh"
 
 namespace fp {
-const char* get_last_error();
-
-// An allocation that `Free` releases when its owner goes away or grows it.  Move-only: every allocation has one owner,
-// so destroying a context, a mesh slot or a replaced weight tensor frees exactly what it held.  Device memory must be
-// released with its device current.
-template <cudaError_t (*Free)(void*)>
-struct OwnedBuf {
-  void* p = nullptr;
-  size_t bytes = 0;
-  OwnedBuf() = default;
-  OwnedBuf(OwnedBuf&& o) noexcept : p(std::exchange(o.p, nullptr)), bytes(std::exchange(o.bytes, 0)) {}
-  OwnedBuf& operator=(OwnedBuf&& o) noexcept {
-    if (this != &o) {
-      reset();
-      p = std::exchange(o.p, nullptr);
-      bytes = std::exchange(o.bytes, 0);
-    }
-    return *this;
-  }
-  ~OwnedBuf() { reset(); }
-  void reset() {
-    if (p) Free(p);
-    p = nullptr;
-    bytes = 0;
-  }
-};
-using DevBuf = OwnedBuf<cudaFree>;         // device memory
-using PinnedBuf = OwnedBuf<cudaFreeHost>;  // page-locked host memory
-
-// A CUDA event (timing disabled), created on first use and destroyed with its owner.  Move-only, as OwnedBuf.
-struct OwnedEvent {
-  cudaEvent_t e = nullptr;
-  OwnedEvent() = default;
-  OwnedEvent(OwnedEvent&& o) noexcept : e(std::exchange(o.e, nullptr)) {}
-  OwnedEvent& operator=(OwnedEvent&& o) noexcept {
-    if (this != &o) {
-      if (e) cudaEventDestroy(e);
-      e = std::exchange(o.e, nullptr);
-    }
-    return *this;
-  }
-  ~OwnedEvent() {
-    if (e) cudaEventDestroy(e);
-  }
-  cudaError_t record(cudaStream_t st) {
-    if (!e) {
-      const cudaError_t ce = cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
-      if (ce != cudaSuccess) return ce;
-    }
-    return cudaEventRecord(e, st);
-  }
-};
-
-// (Re)allocates `b` to at least `bytes`.  `epoch` is the owning context's graph epoch: it is bumped whenever a device
-// pointer or by-value kernel parameter that a captured CUDA graph may hold changes (re-allocation, new weights /
-// intrinsics), and cached graphs older than it are rebuilt.  Never called while a stream is capturing:
-// every workspace is sized by ensure_capacity / fp_set_mesh_slot / fp_set_frame BEFORE run_graphed.  A tracking call
-// still in flight may be reading the buffer being replaced, so growing one waits for the device first.
-static int dev_alloc(unsigned long long& epoch, DevBuf& b, size_t bytes, bool zero = false) {
-  if (b.bytes >= bytes && b.p) return 0;
-  ++epoch;
-  if (b.p) FP_CUDA_OK(cudaDeviceSynchronize());
-  b.reset();
-  FP_CUDA_OK(cudaMalloc(&b.p, bytes));
-  b.bytes = bytes;
-  if (zero) {
-    // legacy-stream memset + full synchronisation: the consumers run on the caller's (possibly non-blocking) stream
-    FP_CUDA_OK(cudaMemset(b.p, 0, bytes));
-    FP_CUDA_OK(cudaDeviceSynchronize());
-  }
-  return 0;
-}
-template <class T>
-static int upload(unsigned long long& epoch, DevBuf& b, const std::vector<T>& v) {
-  const size_t bytes = std::max<size_t>(v.size() * sizeof(T), 16);
-  if (dev_alloc(epoch, b, bytes)) return -2;
-  if (!v.empty()) FP_CUDA_OK(cudaMemcpy(b.p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-  return 0;
-}
-
-// (Re)allocates pinned `b` to at least `bytes` (cudaHostAlloc `flags`).  `epoch`: the graph epoch of the context whose
-// captured graph holds b's address (a read-back node), bumped when the address changes; null where no graph holds it.
-static int pinned_alloc(unsigned long long* epoch, PinnedBuf& b, size_t bytes, unsigned flags = cudaHostAllocDefault) {
-  if (b.bytes >= bytes && b.p) return 0;
-  if (epoch) ++*epoch;
-  b.reset();
-  FP_CUDA_OK(cudaHostAlloc(&b.p, bytes, flags));
-  b.bytes = bytes;
-  return 0;
-}
-
-struct Tensor {
-  DevBuf buf;
-  int dtype = 0;  // 0 = f32, 1 = f16
-  long long numel = 0;
-};
-
-struct Net {
-  std::map<std::string, Tensor> t;
-  bool loaded = false;
-  // fp_load_network verified that every name the execution plan uses is present; a miss is a programming error
-  // and surfaces as an exception that the extern "C" wrappers turn into an error code
-  const __half* h(const char* name) const { return reinterpret_cast<const __half*>(t.at(name).buf.p); }
-  const float* f(const char* name) const { return reinterpret_cast<const float*>(t.at(name).buf.p); }
-};
-
-constexpr int S = 160;
-constexpr int T = 400;
-// fp_register_objects refines and featurises whole objects in passes of at most this many hypotheses (an object above
-// it gets a pass of its own).  ensure_capacity costs ~15.6 MB per hypothesis, so the context keeps ~8 GB of workspace
-// after such a call; the largest buffer (refiner qkv, N * 400 * 3072 fp16) is 1.26 GB, and every element and byte
-// offset inside a buffer stays below 2^31.
-constexpr int kRegisterPassCap = 512;
-constexpr size_t kCropImg = (size_t)(S + 6) * (S + 8) * 8;  // fp16 elements per padded crop image
-// The encoder's first stage runs on the A (rendered) and B (observed) crops as one batch.  The 40x40
-// 128-channel layers tile four images per MMA (gemm_swap_patch_kernel), and the layer that fuses
-// torch.cat((a, b), 1) stores A and B tiles to different channel halves, so the A/B boundary must fall on a tile
-// boundary: B starts at N rounded up to 4 (up to three never-read pad images).
-static inline int b_img0_of(int N) { return (N + 3) & ~3; }
-
-static_assert(kMaxMeshes == FP_MAX_MESHES, "fp_crop.cuh and fpose.h disagree on the number of mesh slots");
-static_assert(kMaxCameras == FP_MAX_CAMERAS, "fp_crop.cuh and fpose.h disagree on the number of cameras");
-
-// One mesh of the context (fp_meshlet.cu layout).  Slot 0 is the mesh of every single-object entry point.
-struct MeshSlot {
-  DevBuf vpos, vnrm, vatt, faces, meshlets, ml_verts, ml_tris, tex;
-  int V = 0, F = 0, Ht = 0, Wt = 0, n_meshlets = 0, front_sign = 0, closed = 0;
-  float bs[4] = {0.f, 0.f, 0.f, 0.f};
-  bool has_tex = false, loaded = false;
-  float diameter = 0.f;
-};
-
-// One camera's frame: the raw upload and the filtered frame (rgba, depth, xyz), and the size and intrinsics of the frame
-// the last call prepared in this camera.  Camera 0 is the context's frame, the one every single-frame entry point reads
-// (see alloc_camera).  camera_dev() makes the kernels' record of it.
-struct CameraBufs {
-  DevBuf rgb_raw, depth_raw, rgba, depth, xyz;
-  int H = 0, W = 0;
-  float fx = 0.f, fy = 0.f, cx = 0.f, cy = 0.f;
-};
-
-// All pinned staging of host inputs.  The tracking calls keep up to FP_TRACK_MAX_IN_FLIGHT calls in flight, each
-// uploading through a staging set of its own: the host copies the next call's frames while the device still tracks the
-// previous call.  Only the host side is doubled: the device buffers the uploads land in are ordered by the stream.
-// Every call that stages pageable host memory takes the next set in turn (take_set) and marks it busy after its last
-// copy out of it (set_busy): a set is busy until `uploaded`, recorded after that copy, has passed.
-constexpr int kMaxInFlight = FP_TRACK_MAX_IN_FLIGHT;
-struct StagingSet {
-  PinnedBuf rgb[kMaxCameras], depth[kMaxCameras];
-  PinnedBuf args;  // the camera table, then the slot ids and camera ids (layout of fp_ctx::args)
-  // the register calls' masks of every object at its byte offset, and their (offsets [M + 1], camera ids [M], one int of
-  // padding, each object's mask byte offset size_t [M]); fp_start_poses' mask; fp_register's start poses
-  PinnedBuf masks, ints, poses;
-  OwnedEvent uploaded;
-  bool busy = false;
-};
-
-// The pose read-back of one submitted tracking call: pinned [M][16] poses, complete once `done` has passed.  Owned by
-// the call's ticket until fp_track_wait collects it (ticket 0: free for the next submit).  A call's read-back outlives
-// its staging set, which the call after next may reuse before this result is collected.
-struct Readback {
-  PinnedBuf poses;
-  OwnedEvent done;
-  unsigned long long ticket = 0;
-  int M = 0;
-};
-
-}  // namespace fp
-
-struct fp_ctx {
-  int device = 0;
-  fp::Net net[2];  // 0 = refiner, 1 = scorer
-  unsigned long long epoch = 1;  // graph epoch (see dev_alloc)
-  unsigned long long graph_captures = 0;
-  // meshes, and their device table (MeshSlotDev [FP_MAX_MESHES]) that kernels index by slot.  Captured graphs hold only
-  // the table's address: loading a slot rewrites its entry in place and needs no new capture.
-  fp::MeshSlot mesh[fp::kMaxMeshes];
-  fp::DevBuf mesh_table;
-  float rot_normalizer = 0.3490658503988659f;
-  float crop_ratio[2] = {1.2f, 1.2f};  // per predictor: each reads its own config.yml (predict_pose_refine.py:117, predict_score.py:137)
-  // frames: cam[0] is the context's frame, cameras 1.. those of the multi-camera calls
-  fp::CameraBufs cam[fp::kMaxCameras];
-  int n_frames = 0;  // the last call prepared the frames of cameras 0 .. n_frames - 1
-  bool has_frame = false;
-  // workspaces (sized for cap_n hypotheses)
-  int cap_n = 0;
-  fp::DevBuf crops, act0, a1, a2, a3, ab0, ab1, ab2, c0, c1, c2, tok, qkv, att, x1pre, x1, ff, x2pre;
-  fp::DevBuf head_out, poses_a, poses_b, feats, tail_qkv, tail_attn, scores, best;
-  int tail_cap = 0;
-  float fold_c = 0.f;      // linear.weight . out_proj.bias + linear.bias (by-value kernel parameter)
-  fp::DevBuf fold_v, tail_counter;  // out_proj^T linear.weight [512]; arg-max ticket
-  // CUDA graphs of the launch-bound inner loops, keyed by (kind, N, iterations, frame source: see run_graphed).
-  // frame: camera 0's record when the graph was captured (read by a graph that takes the frame by value)
-  struct GraphEntry {
-    cudaGraphExec_t exec = nullptr;
-    unsigned long long epoch = 0;
-    fp::CameraDev frame{};
-  };
-  std::map<std::tuple<int, int, int, int>, GraphEntry> graphs;
-  std::map<std::tuple<int, int, int, int>, int> graph_nodes;
-  cudaStream_t cap_stream = nullptr;
-  // the refiner's two decoder heads are independent after the shared attention core: at small batches
-  // (one linear layer = 1-2 waves of tiles) the second head runs on `side_stream` so that its kernels fill
-  // the SMs the first head's tail wave leaves idle.  Fork / join are events, captured into the graph.
-  cudaStream_t side_stream = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  int fork_max_n = 128;  // FPOSE_FORK_MAX_N; 0 disables.  Measured (profiles/r02_fork_probe.log): -5 % at 32, -1 % at 126, +1 % at 252 hypotheses
-  bool use_graphs = true;
-  bool cull_backfaces = true;  // FPOSE_NO_CULL=1: render both sides even for closed meshes (A/B checks)
-  bool track_valid = false;
-  int crop_tile = 0;
-  fp::DevBuf lt_buf, lr_buf, feat_buf, pose_stage, tok_mean;
-  fp::DevBuf mask_buf, mask_stats, crop_stats;
-  fp::DevBuf op_mesh_of;  // fp_op_pose_update: the uploaded slot id of every hypothesis
-  fp::DevBuf track_pose;      // fp_track: the pose it produced last, where pose_in = NULL continues from
-  // the tracking calls in flight: their staging sets (used in turn), their read-backs by ticket, the last ticket issued,
-  // and the stream and completion event (after the read-back) of the last call submitted
-  fp::StagingSet sets[fp::kMaxInFlight];
-  int next_set = 0;
-  std::vector<std::unique_ptr<fp::Readback>> readbacks;
-  unsigned long long last_ticket = 0;
-  cudaStream_t last_stream = nullptr;
-  cudaEvent_t last_done = nullptr;  // the last call's Readback::done (a Readback is reused only by a later call)
-  // the arguments of a multi-object call or register pass, one device block at a fixed address (a graph holds it),
-  // staged through a StagingSet: the camera table (CameraDev [FP_MAX_CAMERAS]), the slot ids [n], the camera ids [n]
-  fp::DevBuf args;
-  int cam_grid_h = 0, cam_grid_w = 0;  // the tracking calls' frame-preparation grid: the largest frame seen
-  // fp_register_objects / _cameras: row offsets of the objects' hypotheses [M + 1] and the objects' camera ids [M], the
-  // objects' feature rows [sum N][512], each object's byte offset into mask_buf
-  fp::DevBuf seg_off, reg_feats, mask_off;
-  // fp_vis: the crop producer's vis record [N][2][160][160] float4 and the per-row depth ranges [N] float2, sized at the
-  // first call for the largest N seen; never allocated by the other entry points
-  fp::DevBuf vis_rec, vis_range;
-};
-
-namespace fp {
-
-static int ensure_capacity(fp_ctx* c, int N) {
-  if (N <= c->cap_n) return 0;
-  const size_t n = (size_t)N;
-  int rc = 0;
-  // the crop buffer is zeroed once: the 3-pixel border is never written afterwards
-  const size_t m = 2 * n + 3;  // A + pad + B images
-  rc |= dev_alloc(c->epoch, c->crops, m * kCropImg * 2, true);
-  rc |= dev_alloc(c->epoch, c->act0, m * 80 * 80 * 64 * 2);
-  rc |= dev_alloc(c->epoch, c->a1, m * 1600 * 128 * 2);
-  rc |= dev_alloc(c->epoch, c->a2, m * 1600 * 128 * 2);
-  rc |= dev_alloc(c->epoch, c->a3, m * 1600 * 128 * 2);
-  rc |= dev_alloc(c->epoch, c->ab0, n * 1600 * 256 * 2);
-  rc |= dev_alloc(c->epoch, c->ab1, n * 1600 * 256 * 2);
-  rc |= dev_alloc(c->epoch, c->ab2, n * 1600 * 256 * 2);
-  rc |= dev_alloc(c->epoch, c->c0, n * T * 512 * 2);
-  rc |= dev_alloc(c->epoch, c->c1, n * T * 512 * 2);
-  rc |= dev_alloc(c->epoch, c->c2, n * T * 512 * 2);
-  rc |= dev_alloc(c->epoch, c->tok, n * T * 512 * 2);
-  rc |= dev_alloc(c->epoch, c->qkv, n * T * 3072 * 2);
-  rc |= dev_alloc(c->epoch, c->att, 2 * n * T * 512 * 2);
-  // x 2: one set per decoder head (they may run concurrently, see run_refine_heads)
-  rc |= dev_alloc(c->epoch, c->x1pre, 2 * n * T * 512 * 2);
-  rc |= dev_alloc(c->epoch, c->x1, 2 * n * T * 512 * 2);
-  rc |= dev_alloc(c->epoch, c->ff, 2 * n * T * 512 * 2);
-  rc |= dev_alloc(c->epoch, c->x2pre, 2 * n * T * 512 * 2);
-  rc |= dev_alloc(c->epoch, c->head_out, 2 * n * 3 * 4);
-  rc |= dev_alloc(c->epoch, c->poses_a, n * 16 * 4);
-  rc |= dev_alloc(c->epoch, c->poses_b, n * 16 * 4);
-  rc |= dev_alloc(c->epoch, c->feats, n * 512 * 4);
-  rc |= dev_alloc(c->epoch, c->lt_buf, n * 3 * 4);
-  rc |= dev_alloc(c->epoch, c->lr_buf, n * 9 * 4);
-  rc |= dev_alloc(c->epoch, c->feat_buf, n * 512 * 4);
-  rc |= dev_alloc(c->epoch, c->pose_stage, n * 16 * 4);
-  rc |= dev_alloc(c->epoch, c->tok_mean, n * 512 * 4);
-  if (rc) return -2;
-  c->cap_n = N;
-  return 0;
-}
-
-static int ensure_tail(fp_ctx* c, int L) {
-  if (L <= c->tail_cap) return 0;
-  int rc = 0;
-  rc |= dev_alloc(c->epoch, c->tail_qkv, (size_t)L * 1536 * 4);
-  rc |= dev_alloc(c->epoch, c->tail_attn, (size_t)L * 512 * 4);
-  rc |= dev_alloc(c->epoch, c->scores, (size_t)L * 4);
-  rc |= dev_alloc(c->epoch, c->best, 16);
-  if (rc) return -2;
-  c->tail_cap = L;
-  return 0;
-}
-
-static GemmLayer mk(int kind, int n_img, int H, int W, int Cin, int Cout, const void* in, const __half* w,
-                    const float* b, void* out, int relu, const void* res = nullptr, int out_ld = 0, int out_split = 0,
-                    const float* post_add = nullptr) {
-  GemmLayer L;
-  L.kind = kind;
-  L.n_img = n_img;
-  L.Hin = H;
-  L.Win = W;
-  L.Cin = Cin;
-  L.Cout = Cout;
-  L.in = in;
-  L.w = w;
-  L.bias = b;
-  L.res = res;
-  L.res_ld = Cout;
-  L.out = out;
-  L.out_ld = out_ld ? out_ld : Cout;
-  L.out_split = out_split;
-  L.post_add = post_add;
-  L.relu = relu;
-  return L;
-}
-
-#define FP_TRY(expr)         \
-  do {                       \
-    int _rc = (expr);        \
-    if (_rc) return _rc;     \
-  } while (0)
-
-// The encoder's activation buffers, as the layer table names them
-enum EncBuf : int { EB_NONE = -1, EB_CROPS, EB_ACT0, EB_A1, EB_A2, EB_A3, EB_AB0, EB_AB1, EB_AB2, EB_C0, EB_C1, EB_C2, EB_TOK };
-
-// One layer of the encoder (encodeA + encodeAB of refine_network.py:34-50, encoderA + encoderAB of
-// score_network.py:37-51), BatchNorm folded, ReLU after every layer.  Weights "enc.<layer>.w" / "enc.<layer>.b".
-struct EncLayer {
-  int kind;
-  bool ab_batch;    // runs on the M = Np + N images of the A and B crops (Np = b_img0_of(N)), else on the N pairs
-  int H;            // input height = width
-  int Cin, Cout;
-  EncBuf in, out, res;
-  int out_ld;       // 0: Cout
-  bool split;       // out_split = Np: image n < Np -> image n, channels [0, Cout); n >= Np -> image n - Np, [Cout, 2 Cout)
-  bool pe;          // adds the positional embedding "pe" after the ReLU
-};
-
-// The encoder, in launch order: run_encoder, fp_op_encoder and fp_op_encoder_layer all read this table.  Every
-// residual block's second layer adds the block's input, which the buffer rotation keeps until then.
-constexpr int kEncLayers = 15;
-static const EncLayer kEncoder[kEncLayers] = {
-    {LK_CONV7_S2, true, S, 8, 64, EB_CROPS, EB_ACT0, EB_NONE, 0, false, false},
-    {LK_CONV3_S2, true, 80, 64, 128, EB_ACT0, EB_A1, EB_NONE, 0, false, false},
-    {LK_CONV3_S1, true, 40, 128, 128, EB_A1, EB_A2, EB_NONE, 0, false, false},
-    {LK_CONV3_S1, true, 40, 128, 128, EB_A2, EB_A3, EB_A1, 0, false, false},
-    {LK_CONV3_S1, true, 40, 128, 128, EB_A3, EB_A2, EB_NONE, 0, false, false},
-    // the last encodeA layer writes straight into the 256-channel concat buffer (refine_network.py:85)
-    {LK_CONV3_S1, true, 40, 128, 128, EB_A2, EB_AB0, EB_A3, 256, true, false},
-    {LK_CONV3_S1, false, 40, 256, 256, EB_AB0, EB_AB1, EB_NONE, 0, false, false},
-    {LK_CONV3_S1, false, 40, 256, 256, EB_AB1, EB_AB2, EB_AB0, 0, false, false},
-    {LK_CONV3_S1, false, 40, 256, 256, EB_AB2, EB_AB1, EB_NONE, 0, false, false},
-    {LK_CONV3_S1, false, 40, 256, 256, EB_AB1, EB_AB0, EB_AB2, 0, false, false},
-    {LK_CONV3_S2, false, 40, 256, 512, EB_AB0, EB_C0, EB_NONE, 0, false, false},
-    {LK_CONV3_S1, false, 20, 512, 512, EB_C0, EB_C1, EB_NONE, 0, false, false},
-    {LK_CONV3_S1, false, 20, 512, 512, EB_C1, EB_C2, EB_C0, 0, false, false},
-    {LK_CONV3_S1, false, 20, 512, 512, EB_C2, EB_C1, EB_NONE, 0, false, false},
-    {LK_CONV3_S1, false, 20, 512, 512, EB_C1, EB_TOK, EB_C2, 0, false, true},
-};
-
-static void* enc_buf(fp_ctx* c, const __half* crops, EncBuf b) {
-  switch (b) {
-    case EB_CROPS: return const_cast<__half*>(crops);
-    case EB_ACT0: return c->act0.p;
-    case EB_A1: return c->a1.p;
-    case EB_A2: return c->a2.p;
-    case EB_A3: return c->a3.p;
-    case EB_AB0: return c->ab0.p;
-    case EB_AB1: return c->ab1.p;
-    case EB_AB2: return c->ab2.p;
-    case EB_C0: return c->c0.p;
-    case EB_C1: return c->c1.p;
-    case EB_C2: return c->c2.p;
-    case EB_TOK: return c->tok.p;
-    default: return nullptr;
-  }
-}
-
-// Layer k's output buffer as the next layers read it, NHWC: {images, height, width, channels}.  The concat layer's
-// buffer holds N images of [A_i | B_i] (2 Cout channels); the A / B layers' buffers hold all M images, pads included.
-static void enc_out_shape(int k, int N, int shape[4]) {
-  const EncLayer& l = kEncoder[k];
-  shape[0] = (l.ab_batch && !l.split) ? b_img0_of(N) + N : N;
-  shape[1] = shape[2] = l.kind == LK_CONV3_S1 ? l.H : l.H / 2;
-  shape[3] = l.out_ld ? l.out_ld : l.Cout;
-}
-
-// The layer whose output is still in buffer `b` when layer k runs: the last writer before k (-1: the crops)
-static int enc_source(int k, EncBuf b) {
-  for (int j = k - 1; j >= 0; --j)
-    if (kEncoder[j].out == b) return j;
-  return -1;
-}
-
-// crops [2N][166][168][8] -> tokens [N][400][512] (+ positional embedding), or layers 0 .. last only
-static int run_encoder(fp_ctx* c, const Net& net, const __half* crops, int N, cudaStream_t st, int last = kEncLayers - 1) {
-  char wn[32], bn[32];
-  const int Np = b_img0_of(N);
-  for (int k = 0; k <= last; ++k) {
-    const EncLayer& l = kEncoder[k];
-    snprintf(wn, sizeof wn, "enc.%d.w", k);
-    snprintf(bn, sizeof bn, "enc.%d.b", k);
-    FP_TRY(gemm_layer_launch(mk(l.kind, l.ab_batch ? Np + N : N, l.H, l.H, l.Cin, l.Cout, enc_buf(c, crops, l.in),
-                                net.h(wn), net.f(bn), enc_buf(c, crops, l.out), 1, enc_buf(c, crops, l.res), l.out_ld,
-                                l.split ? Np : 0, l.pe ? net.f("pe") : nullptr),
-                             st));
-  }
-  return 0;
-}
-
-// tokens -> (trans, rot) raw network outputs, [2][N][3] fp32 in head_out
-static int run_refine_heads(fp_ctx* c, const Net& net, int N, cudaStream_t st) {
-  const int M = N * T;
-  // both heads' in_proj as one GEMM: [M,512] x [3072,512]^T
-  FP_TRY(gemm_layer_launch(mk(LK_LINEAR, 1, 1, M, 512, 3072, c->tok.p, net.h("heads.in_w"), net.f("heads.in_b"), c->qkv.p, 0), st));
-  FP_TRY(attn_core_launch(
-      head_attn_params(reinterpret_cast<const __half*>(c->qkv.p), 3072, 2, reinterpret_cast<__half*>(c->att.p), N), st));
-  const bool fork = N <= c->fork_max_n;
-  if (fork) {
-    if (!c->side_stream) {
-      FP_CUDA_OK(cudaStreamCreateWithFlags(&c->side_stream, cudaStreamNonBlocking));
-      FP_CUDA_OK(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
-      FP_CUDA_OK(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
-    }
-    FP_CUDA_OK(cudaEventRecord(c->ev_fork, st));
-    FP_CUDA_OK(cudaStreamWaitEvent(c->side_stream, c->ev_fork, 0));
-  }
-  for (int g = 0; g < 2; ++g) {
-    cudaStream_t sg = (fork && g == 1) ? c->side_stream : st;
-    char nm[48];
-    auto H = [&](const char* s) { snprintf(nm, sizeof nm, "head%d.%s", g, s); return net.h(nm); };
-    auto Fp = [&](const char* s) { snprintf(nm, sizeof nm, "head%d.%s", g, s); return net.f(nm); };
-    const size_t off = (size_t)g * M * 512;
-    const __half* att_g = reinterpret_cast<const __half*>(c->att.p) + off;
-    __half* x1pre = reinterpret_cast<__half*>(c->x1pre.p) + off;
-    __half* x1 = reinterpret_cast<__half*>(c->x1.p) + off;
-    __half* ff = reinterpret_cast<__half*>(c->ff.p) + off;
-    __half* x2pre = reinterpret_cast<__half*>(c->x2pre.p) + off;
-    const __half* w;
-    const float* b;
-    w = H("out_w"); b = Fp("out_b");
-    // the first kernel behind an event wait has a full (not programmatic) dependency
-    if (fork && g == 1) pdl_skip_next();
-    FP_TRY(gemm_layer_launch(mk(LK_LINEAR, 1, 1, M, 512, 512, att_g, w, b, x1pre, 0, c->tok.p), sg));
-    const float* g1 = Fp("ln1_g");
-    const float* b1 = Fp("ln1_b");
-    FP_TRY(layernorm_launch(x1pre, x1, g1, b1, M, sg));
-    w = H("ff1_w"); b = Fp("ff1_b");
-    FP_TRY(gemm_layer_launch(mk(LK_LINEAR, 1, 1, M, 512, 512, x1, w, b, ff, 1), sg));
-    w = H("ff2_w"); b = Fp("ff2_b");
-    FP_TRY(gemm_layer_launch(mk(LK_LINEAR, 1, 1, M, 512, 512, ff, w, b, x2pre, 0, x1), sg));
-    const float* g2 = Fp("ln2_g");
-    const float* b2 = Fp("ln2_b");
-    const float* fw = Fp("fin_w");
-    const float* fb = Fp("fin_b");
-    FP_TRY(head_final_launch(x2pre, g2, b2, fw, fb, reinterpret_cast<float*>(c->head_out.p) + (size_t)g * N * 3, N, T, 3, sg));
-  }
-  if (fork) {
-    FP_CUDA_OK(cudaEventRecord(c->ev_join, c->side_stream));
-    FP_CUDA_OK(cudaStreamWaitEvent(st, c->ev_join, 0));
-    pdl_skip_next();  // the consumer of head_out joins two streams
-  }
-  return 0;
-}
-
-// tokens -> per-hypothesis 512-d features (score_network.py:72-74)
-static int run_score_feats(fp_ctx* c, const Net& net, int N, float* feats, cudaStream_t st) {
-  const int M = N * T;
-  FP_TRY(gemm_layer_launch(mk(LK_LINEAR, 1, 1, M, 512, 1536, c->tok.p, net.h("att.in_w"), net.f("att.in_b"), c->qkv.p, 0), st));
-  FP_TRY(attn_core_launch(
-      head_attn_params(reinterpret_cast<const __half*>(c->qkv.p), 1536, 1, reinterpret_cast<__half*>(c->att.p), N), st));
-  FP_TRY(token_mean_proj_launch(reinterpret_cast<const __half*>(c->att.p), net.f("att.out_w32"), net.f("att.out_b"),
-                                reinterpret_cast<float*>(c->tok_mean.p), feats, N, T, st));
-  return 0;
-}
-
-// external crop layout of the test hooks: [2N] images, A then B, contiguous
-static int crops_import(fp_ctx* c, const void* ext, int N, cudaStream_t st) {
-  const size_t img = kCropImg * 2;
-  __half* dst = reinterpret_cast<__half*>(c->crops.p);
-  const char* src = reinterpret_cast<const char*>(ext);
-  FP_CUDA_OK(cudaMemcpyAsync(dst, src, (size_t)N * img, cudaMemcpyDeviceToDevice, st));
-  FP_CUDA_OK(cudaMemcpyAsync(dst + (size_t)b_img0_of(N) * kCropImg, src + (size_t)N * img, (size_t)N * img,
-                             cudaMemcpyDeviceToDevice, st));
-  return 0;
-}
-static int crops_export(fp_ctx* c, void* ext, int N, cudaStream_t st) {
-  const size_t img = kCropImg * 2;
-  const __half* src = reinterpret_cast<const __half*>(c->crops.p);
-  char* dst = reinterpret_cast<char*>(ext);
-  FP_CUDA_OK(cudaMemcpyAsync(dst, src, (size_t)N * img, cudaMemcpyDeviceToDevice, st));
-  FP_CUDA_OK(cudaMemcpyAsync(dst + (size_t)N * img, src + (size_t)b_img0_of(N) * kCropImg, (size_t)N * img,
-                             cudaMemcpyDeviceToDevice, st));
-  return 0;
-}
 
 // Entry `s` of the device mesh table, with the expressions the crop producer and the pose update always used.
 static MeshSlotDev mesh_entry(const fp_ctx* c, int s) {
@@ -547,7 +54,7 @@ static MeshSlotDev mesh_entry(const fp_ctx* c, int s) {
 // Rewrites the table entries of every loaded slot.  Synchronises: kernels enqueued earlier may be reading the table.
 static int write_mesh_table(fp_ctx* c) {
   FP_CUDA_OK(cudaDeviceSynchronize());
-  FP_TRY(dev_alloc(c->epoch, c->mesh_table, sizeof(MeshSlotDev) * kMaxMeshes, /*zero=*/true));
+  FP_TRY(dev_alloc(&c->epoch, c->mesh_table, sizeof(MeshSlotDev) * kMaxMeshes, /*zero=*/true));
   std::vector<MeshSlotDev> table(kMaxMeshes);
   memset(table.data(), 0, sizeof(MeshSlotDev) * kMaxMeshes);
   for (int s = 0; s < kMaxMeshes; ++s)
@@ -686,18 +193,6 @@ static int run_graphed(fp_ctx* c, GraphKind kind, int N, int iters, cudaStream_t
   return 0;
 }
 
-// RAII: make the context's device current for the duration of an entry point
-struct DeviceGuard {
-  int prev = -1;
-  bool switched = false;
-  explicit DeviceGuard(int dev) {
-    if (cudaGetDevice(&prev) == cudaSuccess && prev != dev) switched = cudaSetDevice(dev) == cudaSuccess;
-  }
-  ~DeviceGuard() {
-    if (switched) cudaSetDevice(prev);
-  }
-};
-
 // camera 0's filtered frame from rgb_dev / depth_dev, with camera 0's record by value (fp_set_frame, fp_register_objects)
 static int set_frame_launches(fp_ctx* c, const unsigned char* rgb_dev, const float* depth_dev, int flags, float zfar,
                               cudaStream_t st) {
@@ -719,8 +214,7 @@ static int set_frame_launches(fp_ctx* c, const unsigned char* rgb_dev, const flo
 // reached only through the camera table, which every call rewrites: growing them invalidates no graph.
 static int alloc_camera(fp_ctx* c, int i, size_t npix, bool raw) {
   CameraBufs& b = c->cam[i];
-  unsigned long long table_only = 0;
-  unsigned long long& epoch = i == 0 ? c->epoch : table_only;
+  unsigned long long* epoch = i == 0 ? &c->epoch : nullptr;
   FP_TRY(dev_alloc(epoch, b.rgba, npix * 4));
   FP_TRY(dev_alloc(epoch, b.depth, npix * 4));
   FP_TRY(dev_alloc(epoch, b.xyz, npix * 16));
@@ -832,7 +326,7 @@ static int upload_host(fp_ctx* c, void* dst, const void* src, size_t bytes, Pinn
 // (a call on the same stream is ordered already).  Every entry point that uses the context's frames or workspaces
 // calls this first.  It never waits on the host: a staging set is waited for only by the call that takes it again
 // (take_set), and results are collected separately (fp_track_wait).
-static int order_after_track(fp_ctx* c, cudaStream_t st) {
+int order_after_track(fp_ctx* c, cudaStream_t st) {
   if (c->last_done && st != c->last_stream) FP_CUDA_OK(cudaStreamWaitEvent(st, c->last_done, 0));
   return 0;
 }
@@ -862,7 +356,7 @@ static int setup_cameras(fp_ctx* c, StagingSet& set, int C, const unsigned char*
     FP_TRY(pinned_alloc(nullptr, set.depth[i], npix_max * 4));
   }
   c->n_frames = C;
-  FP_TRY(dev_alloc(c->epoch, c->args, kTableBytes + (size_t)2 * rows * sizeof(int)));
+  FP_TRY(dev_alloc(&c->epoch, c->args, kTableBytes + (size_t)2 * rows * sizeof(int)));
   FP_TRY(pinned_alloc(nullptr, set.args, kTableBytes + (size_t)2 * staged_rows * sizeof(int)));
   CameraDev* table = reinterpret_cast<CameraDev*>(set.args.p);
   memset(table, 0, kTableBytes);
@@ -970,7 +464,7 @@ static int track_wait(fp_ctx* c, unsigned long long ticket, float* poses_out_hos
 
 // The mesh slot of each of `M` objects.  The kernels index the mesh table with these ids unchecked, so an empty or
 // out-of-range slot must be refused before anything is enqueued.
-static int check_slots(const fp_ctx* c, int M, const int* slots, const char* caller) {
+int check_slots(const fp_ctx* c, int M, const int* slots, const char* caller) {
   for (int i = 0; i < M; ++i) {
     FP_REQUIRE(slots[i] >= 0 && slots[i] < kMaxMeshes, "%s: object %d: slot %d out of range [0, %d)", caller, i, slots[i],
                kMaxMeshes);
@@ -994,51 +488,6 @@ static int check_cameras(int C, const unsigned char* const* rgb_host, const floa
     owns[camera_of[i]] = 1;
   }
   for (int i = 0; i < C; ++i) FP_REQUIRE(owns[i], "%s: camera %d owns no object", caller, i);
-  return 0;
-}
-
-// The scorer tail over `L` feature rows as one segment; a segmented launch sets seg / n_seg / seg_max on top.
-static ScoreTailParams score_tail_params(const fp_ctx* c, const float* feats, int L, float* scores, int* best) {
-  const Net& net = c->net[1];
-  ScoreTailParams p;
-  p.feats = feats;
-  p.L = L;
-  p.w_in = net.f("cross.in_w");
-  p.b_in = net.f("cross.in_b");
-  p.fold_v = reinterpret_cast<const float*>(c->fold_v.p);
-  p.fold_c = c->fold_c;
-  p.offset = 100.f;
-  p.qkv = reinterpret_cast<float*>(c->tail_qkv.p);
-  p.scores = scores;
-  p.best = best;
-  p.counter = reinterpret_cast<unsigned int*>(c->tail_counter.p);
-  return p;
-}
-
-// The scorer tail over n_seg segments of `feats`, segment g being rows [off_host[g], off_host[g + 1]).  Checks the
-// offsets before anything is enqueued (off_host[0] = 0, every segment 1..4096 rows: the kernel's shared memory holds
-// one segment's logits per head), sizes the tail's workspace and its per-segment arg-max tickets, uploads the offsets to
-// seg_off and sets seg / n_seg / seg_max.  `trailing` more ints the caller keeps after the offsets go up in the same copy (the register
-// calls' camera ids).  The register calls and fp_op_score_tail_segments both set their launch up here.
-static int segmented_tail_params(fp_ctx* c, const float* feats, const int* off_host, int n_seg, int trailing, float* scores,
-                                 int* best, cudaStream_t st, const char* caller, ScoreTailParams& p) {
-  FP_REQUIRE(n_seg >= 1, "%s: %d segments, need at least 1", caller, n_seg);
-  FP_REQUIRE(off_host[0] == 0, "%s: the first segment starts at row %d, not 0", caller, off_host[0]);
-  int seg_max = 0;
-  for (int g = 0; g < n_seg; ++g) {
-    const long long n = (long long)off_host[g + 1] - off_host[g];
-    FP_REQUIRE(n >= 1 && n <= 4096, "%s: segment %d has %lld rows, need 1..4096", caller, g, n);
-    seg_max = std::max(seg_max, (int)n);
-  }
-  const size_t ints = (size_t)(n_seg + 1 + trailing);
-  FP_TRY(ensure_tail(c, off_host[n_seg]));
-  FP_TRY(dev_alloc(c->epoch, c->seg_off, ints * sizeof(int)));
-  FP_TRY(dev_alloc(c->epoch, c->tail_counter, std::max<size_t>(16, (size_t)n_seg * sizeof(unsigned int)), /*zero=*/true));
-  FP_CUDA_OK(cudaMemcpyAsync(c->seg_off.p, off_host, ints * sizeof(int), cudaMemcpyHostToDevice, st));
-  p = score_tail_params(c, feats, off_host[n_seg], scores, best);
-  p.seg = reinterpret_cast<const int*>(c->seg_off.p);
-  p.n_seg = n_seg;
-  p.seg_max = seg_max;
   return 0;
 }
 
@@ -1085,10 +534,10 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
   // every workspace is sized for the largest pass here, so no pass bumps the graph epoch
   FP_TRY(ensure_capacity(c, max_pass));
   FP_TRY(ensure_tail(c, total));
-  FP_TRY(dev_alloc(c->epoch, c->reg_feats, (size_t)total * 512 * sizeof(float)));
-  FP_TRY(dev_alloc(c->epoch, c->mask_buf, mask_bytes));
-  FP_TRY(dev_alloc(c->epoch, c->mask_stats, (size_t)M * 6 * sizeof(unsigned int)));
-  if (!by_value) FP_TRY(dev_alloc(c->epoch, c->mask_off, (size_t)M * sizeof(size_t)));
+  FP_TRY(dev_alloc(&c->epoch, c->reg_feats, (size_t)total * 512 * sizeof(float)));
+  FP_TRY(dev_alloc(&c->epoch, c->mask_buf, mask_bytes));
+  FP_TRY(dev_alloc(&c->epoch, c->mask_stats, (size_t)M * 6 * sizeof(unsigned int)));
+  if (!by_value) FP_TRY(dev_alloc(&c->epoch, c->mask_off, (size_t)M * sizeof(size_t)));
   // pinned staging (never read by a captured graph): the copies below leave as soon as they are enqueued
   StagingSet* set;
   FP_TRY(take_set(c, set));
@@ -1184,19 +633,6 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
 
 using namespace fp;
 
-// every entry point: exceptions never cross the C boundary, the context's device is current inside
-#define FP_API_BEGIN try {
-#define FP_API_END                                                        \
-  }                                                                       \
-  catch (const std::exception& e) {                                       \
-    fp::set_last_error("%s: exception: %s", __func__, e.what());          \
-    return -3;                                                            \
-  }                                                                       \
-  catch (...) {                                                           \
-    fp::set_last_error("%s: unknown exception", __func__);                \
-    return -3;                                                            \
-  }
-
 extern "C" {
 
 int fp_create(fp_ctx** out) {
@@ -1253,95 +689,6 @@ int fp_set_config(fp_ctx* c, int which, float crop_ratio, float rot_normalizer) 
   FP_API_END
 }
 
-int fp_load_network(fp_ctx* c, int which, const fp_tensor_t* tensors, int n) {
-  FP_API_BEGIN
-  FP_REQUIRE(c && tensors, "fp_load_network: null argument");
-  FP_REQUIRE(which == 0 || which == 1, "fp_load_network: which must be 0 (refiner) or 1 (scorer)");
-  DeviceGuard dg(c->device);
-  Net& net = c->net[which];
-  ++c->epoch;
-  FP_CUDA_OK(cudaDeviceSynchronize());
-  net.t.clear();
-  net.loaded = false;
-  for (int i = 0; i < n; ++i) {
-    const fp_tensor_t& t = tensors[i];
-    FP_REQUIRE(t.name && t.data && t.numel > 0, "fp_load_network: bad tensor #%d", i);
-    Tensor d;
-    d.dtype = t.dtype;
-    d.numel = t.numel;
-    const size_t bytes = (size_t)t.numel * (t.dtype == 1 ? 2 : 4);
-    FP_TRY(dev_alloc(c->epoch, d.buf, bytes));
-    FP_CUDA_OK(cudaMemcpy(d.buf.p, t.data, bytes, cudaMemcpyHostToDevice));
-    net.t[t.name] = std::move(d);  // a repeated name frees the earlier tensor
-  }
-  // verify that everything the execution plan needs is present, with the right size
-  std::vector<std::pair<std::string, long long>> need;
-  const int cin[15] = {0, 64, 128, 128, 128, 128, 256, 256, 256, 256, 256, 512, 512, 512, 512};
-  const int cout[15] = {64, 128, 128, 128, 128, 128, 256, 256, 256, 256, 512, 512, 512, 512, 512};
-  for (int i = 0; i < 15; ++i) {
-    const long long k = i == 0 ? 7 * 64 : 9LL * cin[i];
-    need.push_back({"enc." + std::to_string(i) + ".w", k * cout[i]});
-    need.push_back({"enc." + std::to_string(i) + ".b", cout[i]});
-  }
-  need.push_back({"pe", 400LL * 512});
-  if (which == 0) {
-    need.push_back({"heads.in_w", 3072LL * 512});
-    need.push_back({"heads.in_b", 3072});
-    for (int g = 0; g < 2; ++g) {
-      const std::string h = "head" + std::to_string(g) + ".";
-      for (const char* s : {"out_w", "ff1_w", "ff2_w"}) need.push_back({h + s, 512LL * 512});
-      for (const char* s : {"out_b", "ff1_b", "ff2_b", "ln1_g", "ln1_b", "ln2_g", "ln2_b"}) need.push_back({h + s, 512});
-      need.push_back({h + "fin_w", 3LL * 512});
-      need.push_back({h + "fin_b", 3});
-    }
-  } else {
-    need.push_back({"att.in_w", 1536LL * 512});
-    need.push_back({"att.in_b", 1536});
-    need.push_back({"att.out_w32", 512LL * 512});
-    need.push_back({"att.out_b", 512});
-    need.push_back({"cross.in_w", 1536LL * 512});
-    need.push_back({"cross.in_b", 1536});
-    need.push_back({"cross.out_w", 512LL * 512});
-    need.push_back({"cross.out_b", 512});
-    need.push_back({"lin.w", 512});
-    need.push_back({"lin.b", 1});
-  }
-  for (auto& nd : need) {
-    auto it = net.t.find(nd.first);
-    FP_REQUIRE(it != net.t.end(), "fp_load_network: tensor '%s' missing", nd.first.c_str());
-    FP_REQUIRE(it->second.numel == nd.second, "fp_load_network: tensor '%s' has %lld elements, expected %lld",
-               nd.first.c_str(), it->second.numel, nd.second);
-  }
-  if (which == 1) {
-    // score = linear(out_proj(a)) = (W_out^T w_lin) . a + (w_lin . b_out + b_lin): fold once, in fp64
-    const float *wo = nullptr, *bo = nullptr, *wl = nullptr, *bl = nullptr;
-    for (int i = 0; i < n; ++i) {
-      const std::string nm = tensors[i].name;
-      const float* d = reinterpret_cast<const float*>(tensors[i].data);
-      if (tensors[i].dtype != 0) continue;
-      if (nm == "cross.out_w") wo = d;
-      else if (nm == "cross.out_b") bo = d;
-      else if (nm == "lin.w") wl = d;
-      else if (nm == "lin.b") bl = d;
-    }
-    FP_REQUIRE(wo && bo && wl && bl, "fp_load_network: the scorer tail tensors must be float32");
-    std::vector<float> v(512);
-    for (int i = 0; i < 512; ++i) {
-      double acc = 0.0;
-      for (int o = 0; o < 512; ++o) acc += (double)wl[o] * (double)wo[(size_t)o * 512 + i];
-      v[i] = (float)acc;
-    }
-    double cc = (double)bl[0];
-    for (int o = 0; o < 512; ++o) cc += (double)wl[o] * (double)bo[o];
-    c->fold_c = (float)cc;
-    FP_TRY(upload(c->epoch, c->fold_v, v));
-    FP_TRY(dev_alloc(c->epoch, c->tail_counter, 16, /*zero=*/true));
-  }
-  net.loaded = true;
-  return 0;
-  FP_API_END
-}
-
 int fp_set_mesh_slot(fp_ctx* c, int slot, int V, int F, const float* pos, const float* nrm, const float* uv,
                      const float* vcol, const int* faces, const unsigned char* tex_rgb, int Ht, int Wt, float diameter) {
   FP_API_BEGIN
@@ -1358,13 +705,13 @@ int fp_set_mesh_slot(fp_ctx* c, int slot, int V, int F, const float* pos, const 
   const bool has_tex = (uv && tex_rgb);
   MeshHost mh;
   FP_TRY(build_mesh_host(V, F, pos, nrm, has_tex ? uv : vcol, has_tex ? 2 : 3, faces, mh));
-  FP_TRY(upload(c->epoch, m.vpos, mh.vpos));
-  FP_TRY(upload(c->epoch, m.vnrm, mh.vnrm));
-  FP_TRY(upload(c->epoch, m.vatt, mh.vatt));
-  FP_TRY(upload(c->epoch, m.faces, mh.faces));
-  FP_TRY(upload(c->epoch, m.meshlets, mh.meshlets));
-  FP_TRY(upload(c->epoch, m.ml_verts, mh.ml_verts));
-  FP_TRY(upload(c->epoch, m.ml_tris, mh.ml_tris));
+  FP_TRY(upload(&c->epoch, m.vpos, mh.vpos));
+  FP_TRY(upload(&c->epoch, m.vnrm, mh.vnrm));
+  FP_TRY(upload(&c->epoch, m.vatt, mh.vatt));
+  FP_TRY(upload(&c->epoch, m.faces, mh.faces));
+  FP_TRY(upload(&c->epoch, m.meshlets, mh.meshlets));
+  FP_TRY(upload(&c->epoch, m.ml_verts, mh.ml_verts));
+  FP_TRY(upload(&c->epoch, m.ml_tris, mh.ml_tris));
   m.has_tex = has_tex;
   if (has_tex) {
     std::vector<unsigned char> rgba((size_t)Ht * Wt * 4);
@@ -1374,7 +721,7 @@ int fp_set_mesh_slot(fp_ctx* c, int slot, int V, int F, const float* pos, const 
       rgba[4 * i + 2] = tex_rgb[3 * i + 2];
       rgba[4 * i + 3] = 255;
     }
-    FP_TRY(upload(c->epoch, m.tex, rgba));
+    FP_TRY(upload(&c->epoch, m.tex, rgba));
     m.Ht = Ht;
     m.Wt = Wt;
   }
@@ -1503,11 +850,11 @@ int fp_start_poses(fp_ctx* c, const unsigned char* mask, int mask_on_device, con
   const size_t npix = (size_t)frame.H * frame.W;
   const unsigned char* mdev = mask;
   if (!mask_on_device) {
-    FP_TRY(dev_alloc(c->epoch, c->mask_buf, npix));
+    FP_TRY(dev_alloc(&c->epoch, c->mask_buf, npix));
     FP_TRY(upload_host(c, c->mask_buf.p, mask, npix, &StagingSet::masks, st));
     mdev = reinterpret_cast<const unsigned char*>(c->mask_buf.p);
   }
-  FP_TRY(dev_alloc(c->epoch, c->mask_stats, 64));
+  FP_TRY(dev_alloc(&c->epoch, c->mask_stats, 64));
   return start_poses_launch(frame, nullptr, nullptr, mdev, nullptr, rot_grid, N, 1, nullptr,
                             reinterpret_cast<unsigned int*>(c->mask_stats.p), poses_out, info_out, st);
   FP_API_END
@@ -1536,93 +883,12 @@ int fp_crop_stats(fp_ctx* c, const float* poses, int N, int mode, int* stats_out
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   FP_TRY(order_after_track(c, st));
   FP_TRY(ensure_capacity(c, N));
-  FP_TRY(dev_alloc(c->epoch, c->crop_stats, 16));
+  FP_TRY(dev_alloc(&c->epoch, c->crop_stats, 16));
   FP_CUDA_OK(cudaMemsetAsync(c->crop_stats.p, 0, 16, st));
   FP_TRY(make_crops(c, poses, N, mode, nullptr, nullptr, reinterpret_cast<int*>(c->crop_stats.p), st));
   FP_CUDA_OK(cudaMemcpyAsync(stats_out_host, c->crop_stats.p, 16, cudaMemcpyDeviceToHost, st));
   FP_CUDA_OK(cudaStreamSynchronize(st));
   return 0;
-  FP_API_END
-}
-
-int fp_op_refine_net(fp_ctx* c, const void* crops, int N, float* trans_out, float* rot_out, void* stream) {
-  FP_API_BEGIN
-  FP_REQUIRE(c && crops && trans_out && rot_out, "fp_op_refine_net: null argument");
-  FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
-  DeviceGuard dg(c->device);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(order_after_track(c, st));
-  if (N == 0) return 0;
-  FP_TRY(ensure_capacity(c, N));
-  FP_TRY(crops_import(c, crops, N, st));
-  FP_TRY(run_encoder(c, c->net[0], reinterpret_cast<const __half*>(c->crops.p), N, st));
-  FP_TRY(run_refine_heads(c, c->net[0], N, st));
-  const float* ho = reinterpret_cast<const float*>(c->head_out.p);
-  FP_CUDA_OK(cudaMemcpyAsync(trans_out, ho, (size_t)N * 12, cudaMemcpyDeviceToDevice, st));
-  FP_CUDA_OK(cudaMemcpyAsync(rot_out, ho + (size_t)N * 3, (size_t)N * 12, cudaMemcpyDeviceToDevice, st));
-  return 0;
-  FP_API_END
-}
-
-int fp_op_score_feats(fp_ctx* c, const void* crops, int N, float* feats_out, void* stream) {
-  FP_API_BEGIN
-  FP_REQUIRE(c && crops && feats_out, "fp_op_score_feats: null argument");
-  FP_REQUIRE(c->net[1].loaded, "scorer weights not loaded");
-  DeviceGuard dg(c->device);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(order_after_track(c, st));
-  if (N == 0) return 0;
-  FP_TRY(ensure_capacity(c, N));
-  FP_TRY(crops_import(c, crops, N, st));
-  FP_TRY(run_encoder(c, c->net[1], reinterpret_cast<const __half*>(c->crops.p), N, st));
-  FP_TRY(run_score_feats(c, c->net[1], N, feats_out, st));
-  return 0;
-  FP_API_END
-}
-
-int fp_op_encoder_layer(int layer, int N, int* info) {
-  FP_API_BEGIN
-  FP_REQUIRE(info, "fp_op_encoder_layer: null info");
-  FP_REQUIRE(layer >= 0 && layer < kEncLayers, "fp_op_encoder_layer: layer = %d outside [0, %d]", layer, kEncLayers - 1);
-  FP_REQUIRE(N >= 0 && N <= kRegisterPassCap, "fp_op_encoder_layer: N = %d outside [0, %d]", N, kRegisterPassCap);
-  const EncLayer& l = kEncoder[layer];
-  const int Np = b_img0_of(N);
-  info[0] = l.kind;
-  info[1] = l.ab_batch ? Np + N : N;
-  info[2] = l.H;
-  info[3] = l.Cin;
-  info[4] = l.Cout;
-  info[5] = enc_source(layer, l.in);
-  info[6] = l.res == EB_NONE ? -1 : enc_source(layer, l.res);
-  info[7] = l.split ? Np : 0;
-  info[8] = l.pe ? 1 : 0;
-  enc_out_shape(layer, N, info + 9);
-  return 0;
-  FP_API_END
-}
-
-long long fp_op_encoder(fp_ctx* c, int which, const void* crops, int N, int last, void* out, void* stream) {
-  FP_API_BEGIN
-  const char* fn = "fp_op_encoder";
-  FP_REQUIRE(c, "%s: null context", fn);
-  FP_REQUIRE(which == 0 || which == 1, "%s: which = %d, must be 0 (refiner) or 1 (scorer)", fn, which);
-  FP_REQUIRE(last >= 0 && last < kEncLayers, "%s: last = %d outside [0, %d]", fn, last, kEncLayers - 1);
-  FP_REQUIRE(N >= 0 && N <= kRegisterPassCap, "%s: N = %d outside [0, %d]", fn, N, kRegisterPassCap);
-  FP_REQUIRE(crops && out, "%s: null crops or out", fn);
-  FP_REQUIRE(c->net[which].loaded, "%s: %s weights not loaded", fn, which == 0 ? "refiner" : "scorer");
-  DeviceGuard dg(c->device);
-  if (check_device_ptr(crops, "crops", fn) || check_device_ptr(out, "out", fn)) return -1;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(order_after_track(c, st));
-  if (N == 0) return 0;
-  int shape[4];
-  enc_out_shape(last, N, shape);
-  const size_t bytes = (size_t)shape[0] * shape[1] * shape[2] * shape[3] * 2;
-  FP_TRY(ensure_capacity(c, N));
-  FP_TRY(crops_import(c, crops, N, st));
-  FP_TRY(run_encoder(c, c->net[which], reinterpret_cast<const __half*>(c->crops.p), N, st, last));
-  FP_CUDA_OK(cudaMemcpyAsync(out, enc_buf(c, nullptr, kEncoder[last].out), bytes, cudaMemcpyDeviceToDevice, st));
-  return (long long)bytes;
   FP_API_END
 }
 
@@ -1692,23 +958,6 @@ int fp_score_tail(fp_ctx* c, const float* feats, int L, float* scores_out, int* 
   FP_API_END
 }
 
-int fp_op_score_tail_segments(fp_ctx* c, const float* feats, int L, const int* seg_host, int n_seg, float* scores_out,
-                              int* best_out, void* stream) {
-  FP_API_BEGIN
-  const char* fn = "fp_op_score_tail_segments";
-  FP_REQUIRE(c && feats && seg_host && scores_out && best_out, "%s: null argument", fn);
-  FP_REQUIRE(c->net[1].loaded, "scorer weights not loaded");
-  FP_REQUIRE(n_seg >= 1, "%s: %d segments, need at least 1", fn, n_seg);
-  FP_REQUIRE(seg_host[n_seg] == L, "%s: the last segment ends at row %d, not at L = %d", fn, seg_host[n_seg], L);
-  DeviceGuard dg(c->device);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(order_after_track(c, st));
-  ScoreTailParams p;
-  FP_TRY(segmented_tail_params(c, feats, seg_host, n_seg, /*trailing=*/0, scores_out, best_out, st, fn, p));
-  return score_tail_launch(p, st);
-  FP_API_END
-}
-
 int fp_score(fp_ctx* c, const float* poses, int N, float* scores_out, int* best_out, void* stream) {
   FP_API_BEGIN
   FP_REQUIRE(c && poses && scores_out && N >= 0, "fp_score: bad argument");
@@ -1753,8 +1002,7 @@ int fp_track_submit(fp_ctx* c, const unsigned char* rgb_host, const float* depth
   FP_REQUIRE(c->mesh[0].loaded, "fp_track: no mesh");
   FP_REQUIRE(pose_in_dev || c->track_valid, "fp_track: no previous pose in this context: pass pose_in");
   DeviceGuard dg(c->device);
-  unsigned long long no_graph = 0;  // the continuation pose is copied outside the graph
-  FP_TRY(dev_alloc(no_graph, c->track_pose, 64));
+  FP_TRY(dev_alloc(nullptr, c->track_pose, 64));  // the continuation pose is copied outside the graph
   float* keep = reinterpret_cast<float*>(c->track_pose.p);
   // fp_track_cameras' one-object, one-camera case: object 0 renders slot 0 in camera 0
   const int zero = 0;
@@ -1827,9 +1075,8 @@ int fp_vis(fp_ctx* c, int kind, const float* poses_a, const float* poses_b, int 
   }
   FP_TRY(ensure_capacity(c, N));
   // no captured graph holds the vis buffers (fp_vis runs eagerly): growing them must not invalidate the cached graphs
-  unsigned long long no_graph = 0;
-  FP_TRY(dev_alloc(no_graph, c->vis_rec, (size_t)N * 2 * S * S * sizeof(float4)));
-  FP_TRY(dev_alloc(no_graph, c->vis_range, (size_t)N * sizeof(float2)));
+  FP_TRY(dev_alloc(nullptr, c->vis_rec, (size_t)N * 2 * S * S * sizeof(float4)));
+  FP_TRY(dev_alloc(nullptr, c->vis_range, (size_t)N * sizeof(float2)));
   float4* rec = reinterpret_cast<float4*>(c->vis_rec.p);
   float2* range = reinterpret_cast<float2*>(c->vis_range.p);
   if (kind == 0) {
@@ -1950,236 +1197,5 @@ int fp_register_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host, 
 }
 
 unsigned long long fp_graph_captures(fp_ctx* c) { return c ? c->graph_captures : 0ull; }
-
-int fp_op_depth_filter(const float* depth_dev, float* out_dev, int H, int W, int which, void* stream) {
-  FP_API_BEGIN
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_REQUIRE(depth_dev && out_dev && H > 0 && W > 0, "fp_op_depth_filter: bad argument");
-  if (which == 0) return erode_depth_launch(depth_dev, out_dev, H, W, 2, 0.001f, 0.8f, 100.f, st);
-  return bilateral_depth_launch(depth_dev, out_dev, H, W, 2, 100.f, 2.f, 100000.f, st);
-  FP_API_END
-}
-
-int fp_op_pose_update(fp_ctx* c, const float* poses_in, const float* trans, const float* rot, const int* mesh_of_host, int N,
-                      float* poses_out, float* trans_delta_out, float* rot_delta_out, void* stream) {
-  FP_API_BEGIN
-  const char* fn = "fp_op_pose_update";
-  FP_REQUIRE(c && poses_in && trans && rot && poses_out && N >= 0, "%s: bad argument", fn);
-  const int slot0 = 0;
-  FP_TRY(check_slots(c, mesh_of_host ? N : 1, mesh_of_host ? mesh_of_host : &slot0, fn));
-  DeviceGuard dg(c->device);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  FP_TRY(order_after_track(c, st));
-  if (N == 0) return 0;
-  const int* mesh_of = nullptr;
-  if (mesh_of_host) {
-    FP_TRY(dev_alloc(c->epoch, c->op_mesh_of, (size_t)N * sizeof(int)));
-    FP_CUDA_OK(cudaMemcpyAsync(c->op_mesh_of.p, mesh_of_host, (size_t)N * sizeof(int), cudaMemcpyHostToDevice, st));
-    mesh_of = reinterpret_cast<const int*>(c->op_mesh_of.p);
-  }
-  // as refine_body launches it: each hypothesis's half-diameter from the mesh table, the context's rot_normalizer
-  return pose_update_launch(poses_in, trans, rot, poses_out, trans_delta_out, rot_delta_out, N,
-                            reinterpret_cast<const MeshSlotDev*>(c->mesh_table.p), mesh_of, 0.f, c->rot_normalizer, st);
-  FP_API_END
-}
-
-}  // extern "C"
-
-// ------------------------------------------------------------------------------------------------
-// fp_group: ONE process (one host thread) driving several GPUs — the reference's process model (run_demo.py is one
-// script).  One fp_ctx per device, each with its own stream; register() shards the hypothesis list contiguously,
-// every device filters the frame, derives the start poses and refines / featurises its slice; the only exchange is
-// the per-hypothesis feature rows (+ refined poses), written by each device DIRECTLY into device 0's gather buffer
-// over NVLink peer memory (cudaMemcpyAsync device-to-device on the producing device's stream: no host staging, no
-// collective library); device 0 waits on one event per peer and runs the cross-hypothesis tail once.
-// ------------------------------------------------------------------------------------------------
-struct fp_group {
-  // One device's share: its context, stream and completion event, and register()'s buffers there (rot grid [N][16],
-  // start poses, info[4], refined slice).  Destroyed with its device current.
-  struct Device {
-    fp_ctx* ctx = nullptr;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t done = nullptr;
-    fp::DevBuf grid, start, info, refined;
-    ~Device() {
-      if (stream) cudaStreamDestroy(stream);
-      if (done) cudaEventDestroy(done);
-      fp_destroy(ctx);
-    }
-  };
-  std::vector<std::unique_ptr<Device>> dev;
-  struct Gather {
-    fp::DevBuf feats_all, poses_all, scores, best;
-  } gather;  // on device 0
-  fp::PinnedBuf pin_rgb, pin_depth, pin_mask, pin_grid;  // portable: every device reads them
-  unsigned long long epoch = 0;
-};
-
-extern "C" {
-
-int fp_group_destroy(fp_group* g) {
-  FP_API_BEGIN
-  if (!g) return 0;
-  for (size_t i = 0; i < g->dev.size(); ++i) {
-    DeviceGuard dg(g->dev[i]->ctx->device);
-    cudaDeviceSynchronize();
-    if (i == 0) g->gather = fp_group::Gather();
-    g->dev[i].reset();
-  }
-  delete g;
-  return 0;
-  FP_API_END
-}
-
-int fp_group_create(int ndev, const int* dev_ids, fp_group** out) {
-  FP_API_BEGIN
-  FP_REQUIRE(out && ndev > 0, "fp_group_create: bad argument");
-  int visible = 0;
-  FP_CUDA_OK(cudaGetDeviceCount(&visible));
-  fp_group* g = new fp_group();
-  int prev = 0;
-  cudaGetDevice(&prev);
-  for (int i = 0; i < ndev; ++i) {
-    const int dev = dev_ids ? dev_ids[i] : i;
-    if (dev < 0 || dev >= visible) {
-      fp_group_destroy(g);
-      set_last_error("fp_group_create: device %d not visible (%d devices)", dev, visible);
-      cudaSetDevice(prev);
-      return -1;
-    }
-    cudaSetDevice(dev);
-    fp_ctx* c = nullptr;
-    const int rc = fp_create(&c);
-    if (rc) {
-      fp_group_destroy(g);
-      cudaSetDevice(prev);
-      return rc;
-    }
-    auto d = std::make_unique<fp_group::Device>();
-    d->ctx = c;
-    cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking);
-    cudaEventCreateWithFlags(&d->done, cudaEventDisableTiming);
-    g->dev.push_back(std::move(d));
-    if (i > 0) {
-      // peers write their feature rows into device 0's buffer: map device 0's memory into this device
-      const int dev0 = g->dev[0]->ctx->device;
-      int can = 0;
-      cudaDeviceCanAccessPeer(&can, dev, dev0);
-      if (can) {
-        const cudaError_t pe = cudaDeviceEnablePeerAccess(dev0, 0);
-        if (pe != cudaSuccess && pe != cudaErrorPeerAccessAlreadyEnabled) {
-          set_last_error("fp_group_create: cudaDeviceEnablePeerAccess(%d -> %d): %s", dev, dev0, cudaGetErrorString(pe));
-          fp_group_destroy(g);
-          cudaSetDevice(prev);
-          return -2;
-        }
-        cudaGetLastError();
-      }
-    }
-  }
-  cudaSetDevice(prev);
-  *out = g;
-  return 0;
-  FP_API_END
-}
-
-int fp_group_size(fp_group* g) { return g ? (int)g->dev.size() : 0; }
-
-fp_ctx* fp_group_ctx(fp_group* g, int i) { return (g && i >= 0 && i < (int)g->dev.size()) ? g->dev[i]->ctx : nullptr; }
-
-int fp_group_load_network(fp_group* g, int which, const fp_tensor_t* tensors, int n) {
-  FP_API_BEGIN
-  FP_REQUIRE(g, "fp_group_load_network: null group");
-  for (auto& d : g->dev) FP_TRY(fp_load_network(d->ctx, which, tensors, n));
-  return 0;
-  FP_API_END
-}
-
-int fp_group_set_config(fp_group* g, int which, float crop_ratio, float rot_normalizer) {
-  FP_API_BEGIN
-  FP_REQUIRE(g, "fp_group_set_config: null group");
-  for (auto& d : g->dev) FP_TRY(fp_set_config(d->ctx, which, crop_ratio, rot_normalizer));
-  return 0;
-  FP_API_END
-}
-
-int fp_group_set_mesh(fp_group* g, int V, int F, const float* pos, const float* nrm, const float* uv, const float* vcol,
-                      const int* faces, const unsigned char* tex_rgb, int Ht, int Wt, float diameter) {
-  FP_API_BEGIN
-  FP_REQUIRE(g, "fp_group_set_mesh: null group");
-  for (auto& d : g->dev) FP_TRY(fp_set_mesh(d->ctx, V, F, pos, nrm, uv, vcol, faces, tex_rgb, Ht, Wt, diameter));
-  return 0;
-  FP_API_END
-}
-
-int fp_group_register(fp_group* g, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
-                      const unsigned char* mask_host, const float* rot_grid_host, int N, int iterations,
-                      float* poses_out_host, float* scores_out_host, int* best_out_host, float* info_out_host) {
-  FP_API_BEGIN
-  FP_REQUIRE(g && rgb_host && depth_host && K && mask_host && rot_grid_host && poses_out_host && scores_out_host &&
-                 best_out_host && N > 0 && H > 0 && W > 0,
-             "fp_group_register: bad argument");
-  const int G = (int)g->dev.size();
-  const size_t npix = (size_t)H * W;
-  // pinned staging, filled once, read by every device
-  FP_TRY(pinned_alloc(nullptr, g->pin_rgb, npix * 3, cudaHostAllocPortable));
-  FP_TRY(pinned_alloc(nullptr, g->pin_depth, npix * 4, cudaHostAllocPortable));
-  FP_TRY(pinned_alloc(nullptr, g->pin_mask, npix, cudaHostAllocPortable));
-  FP_TRY(pinned_alloc(nullptr, g->pin_grid, (size_t)N * 64, cudaHostAllocPortable));
-  memcpy(g->pin_rgb.p, rgb_host, npix * 3);
-  memcpy(g->pin_depth.p, depth_host, npix * 4);
-  memcpy(g->pin_mask.p, mask_host, npix);
-  memcpy(g->pin_grid.p, rot_grid_host, (size_t)N * 64);
-  fp_ctx* c0 = g->dev[0]->ctx;
-  fp_group::Gather& ga = g->gather;
-  {
-    DeviceGuard dg(c0->device);
-    FP_TRY(dev_alloc(g->epoch, ga.feats_all, (size_t)N * 2048));
-    FP_TRY(dev_alloc(g->epoch, ga.poses_all, (size_t)N * 64));
-    FP_TRY(dev_alloc(g->epoch, ga.scores, (size_t)N * 4));
-    FP_TRY(dev_alloc(g->epoch, ga.best, 16));
-  }
-  const int base = N / G, rem = N % G;
-  for (int i = 0; i < G; ++i) {
-    fp_group::Device& d = *g->dev[i];
-    fp_ctx* c = d.ctx;
-    DeviceGuard dg(c->device);
-    cudaStream_t st = d.stream;
-    const int lo = i * base + (i < rem ? i : rem), n = base + (i < rem ? 1 : 0);
-    FP_TRY(dev_alloc(g->epoch, d.grid, (size_t)N * 64));
-    FP_TRY(dev_alloc(g->epoch, d.start, (size_t)N * 64));
-    FP_TRY(dev_alloc(g->epoch, d.info, 16));
-    FP_TRY(dev_alloc(g->epoch, d.refined, (size_t)(n > 0 ? n : 1) * 64));
-    FP_TRY(fp_set_frame(c, reinterpret_cast<const unsigned char*>(g->pin_rgb.p), reinterpret_cast<const float*>(g->pin_depth.p),
-                        K, H, W, FP_FRAME_FILTER_DEPTH, INFINITY, st));
-    FP_CUDA_OK(cudaMemcpyAsync(d.grid.p, g->pin_grid.p, (size_t)N * 64, cudaMemcpyHostToDevice, st));
-    FP_TRY(fp_start_poses(c, reinterpret_cast<const unsigned char*>(g->pin_mask.p), 0, reinterpret_cast<const float*>(d.grid.p),
-                          N, reinterpret_cast<float*>(d.start.p), reinterpret_cast<float*>(d.info.p), st));
-    if (n > 0) {
-      float* refined = reinterpret_cast<float*>(d.refined.p);
-      FP_TRY(fp_refine(c, reinterpret_cast<const float*>(d.start.p) + (size_t)lo * 16, n, iterations, refined, nullptr,
-                       nullptr, st));
-      // the gather: feature rows and refined poses land in device 0's buffers, straight over peer memory
-      FP_TRY(fp_score_features(c, refined, n, reinterpret_cast<float*>(ga.feats_all.p) + (size_t)lo * 512, st));
-      FP_CUDA_OK(cudaMemcpyAsync(reinterpret_cast<float*>(ga.poses_all.p) + (size_t)lo * 16, refined, (size_t)n * 64,
-                                 cudaMemcpyDefault, st));
-    }
-    FP_CUDA_OK(cudaEventRecord(d.done, st));
-  }
-  {
-    DeviceGuard dg(c0->device);
-    cudaStream_t s0 = g->dev[0]->stream;
-    for (int i = 1; i < G; ++i) FP_CUDA_OK(cudaStreamWaitEvent(s0, g->dev[i]->done, 0));
-    FP_TRY(fp_score_tail(c0, reinterpret_cast<const float*>(ga.feats_all.p), N, reinterpret_cast<float*>(ga.scores.p),
-                         reinterpret_cast<int*>(ga.best.p), s0));
-    FP_CUDA_OK(cudaMemcpyAsync(poses_out_host, ga.poses_all.p, (size_t)N * 64, cudaMemcpyDeviceToHost, s0));
-    FP_CUDA_OK(cudaMemcpyAsync(scores_out_host, ga.scores.p, (size_t)N * 4, cudaMemcpyDeviceToHost, s0));
-    FP_CUDA_OK(cudaMemcpyAsync(best_out_host, ga.best.p, 4, cudaMemcpyDeviceToHost, s0));
-    if (info_out_host) FP_CUDA_OK(cudaMemcpyAsync(info_out_host, g->dev[0]->info.p, 16, cudaMemcpyDeviceToHost, s0));
-    FP_CUDA_OK(cudaStreamSynchronize(s0));
-  }
-  return 0;
-  FP_API_END
-}
 
 }  // extern "C"

@@ -20,12 +20,6 @@
 
 namespace fp {
 
-#define FP_TRY_RC(expr)  \
-  do {                   \
-    int _rc = (expr);    \
-    if (_rc) return _rc; \
-  } while (0)
-
 // attention itself lives in fp_attn_tc.cu (wgmma); this file keeps the SIMT pieces around it
 int attn_core_launch(const AttnParams& p, cudaStream_t stream) { return attn_tc_launch(p, stream); }
 
@@ -430,7 +424,7 @@ int score_tail_launch(const ScoreTailParams& p, cudaStream_t stream) {
     FP_CUDA_OK(cudaFuncSetAttribute(cross_attn_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 4096 * 4));
     device_bit_set(attr_mask);
   }
-  FP_TRY_RC(rowwise_linear_launch(p.feats, p.w_in, p.b_in, p.qkv, p.L, 1536, stream));
+  FP_TRY(rowwise_linear_launch(p.feats, p.w_in, p.b_in, p.qkv, p.L, 1536, stream));
   cross_attn_score_kernel<<<p.L, 128, smem, stream>>>(p.qkv, p.fold_v, p.fold_c, p.offset, p.scores, p.best, p.counter, p.seg,
                                                       p.n_seg, seg_max, p.L, 0.08838834764831845f);
   note_launches(1);

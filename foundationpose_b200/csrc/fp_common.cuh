@@ -57,6 +57,12 @@ int check_device_ptr(const void* p, const char* what, const char* fn = "fp_pose_
       return -1;                                                                           \
     }                                                                                      \
   } while (0)
+// returns the status of a call that failed (nonzero)
+#define FP_TRY(expr)     \
+  do {                   \
+    int _rc = (expr);    \
+    if (_rc) return _rc; \
+  } while (0)
 
 // ----------------------------------------------------------------------------------------------
 // programmatic dependent launch (PDL).  Every kernel of a network pass is launched with

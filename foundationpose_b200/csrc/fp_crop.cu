@@ -542,12 +542,6 @@ static int g_crop_tile_override = [] {
   return (v == 16 || v == 32 || v == 80) ? v : 0;
 }();
 
-#define FP_TRY_RC(expr)  \
-  do {                   \
-    int _rc = (expr);    \
-    if (_rc) return _rc; \
-  } while (0)
-
 template <int TILE>
 static int launch_tile(const CropParams& p, cudaStream_t stream) {
   constexpr int TPR = S / TILE;
@@ -583,7 +577,7 @@ int crop_launch(const CropParams& p, cudaStream_t stream) {
   int tile = p.N >= 64 ? 80 : (p.N >= 4 ? 32 : 16);
   if (g_crop_tile_override) tile = g_crop_tile_override;
   if (p.tile_override == 16 || p.tile_override == 32 || p.tile_override == 80) tile = p.tile_override;
-  FP_TRY_RC(tile == 80 ? launch_tile<80>(p, stream) : (tile == 32 ? launch_tile<32>(p, stream) : launch_tile<16>(p, stream)));
+  FP_TRY(tile == 80 ? launch_tile<80>(p, stream) : (tile == 32 ? launch_tile<32>(p, stream) : launch_tile<16>(p, stream)));
   prof_mark_end(stream);
   note_launches(1);
   FP_CUDA_OK(cudaGetLastError());

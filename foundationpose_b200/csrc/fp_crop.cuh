@@ -77,7 +77,7 @@ struct CropParams {
   // outputs
   __half* crops;   // [b_img0 + N][166][2][84][8] fp16 (rows x {even, odd columns} x column pairs x 8 channels, the
                    // "EO" layout of fp_stem.cu): images 0..N-1 = rendered (A), b_img0..b_img0+N-1 = observed (B)
-  int b_img0;      // first B image (N rounded up to the conv tile's image count, see fp_api.cu)
+  int b_img0;      // first B image (N rounded up to the conv tile's image count, see b_img0_of in fp_ctx.cuh)
   float* dbg;      // optional [N][2][160][160][6] fp32 copy of the normalised crops
   float* win_out;  // optional [N][4] = (left, top, sx, sy)
   int tile_override;  // 0 = pick by batch size; 16 / 32 / 80 = force (fp_set_crop_tile, A/B tests)

@@ -168,6 +168,36 @@ def pack_network(sd, kind):
     return out
 
 
+def _tensor_array(packed):
+    """{name: np.ndarray} -> (fp_tensor_t array, the arrays it points into: keep them alive until the call returns)."""
+    arr = (_FpTensor * len(packed))()
+    keep = []
+    for i, (name, a) in enumerate(packed.items()):
+        a = np.ascontiguousarray(a)
+        keep.append(a)
+        arr[i] = _FpTensor(name.encode(), a.ctypes.data, 1 if a.dtype == np.float16 else 0, a.size)
+    return arr, keep
+
+
+def _mesh_args(vertices, normals, faces, uv=None, tex=None, vertex_colors=None):
+    """The (V, F, pos, nrm, uv, vcol, faces, tex_rgb, Ht, Wt) arguments of fp_set_mesh*, and the arrays the pointers point
+    into: keep them alive until the call returns."""
+    pos = np.ascontiguousarray(vertices, dtype=np.float32)
+    nrm = np.ascontiguousarray(normals, dtype=np.float32)
+    fc = np.ascontiguousarray(faces, dtype=np.int32)
+    uvp = texp = colp = None
+    Ht = Wt = 0
+    if uv is not None and tex is not None:
+        uvp = np.ascontiguousarray(uv, dtype=np.float32)
+        texp = np.ascontiguousarray(tex[..., :3], dtype=np.uint8)
+        Ht, Wt = texp.shape[:2]
+    else:
+        colp = np.ascontiguousarray(vertex_colors, dtype=np.float32)
+    cp = lambda a: None if a is None else C.c_void_p(a.ctypes.data)
+    keep = (pos, nrm, uvp, colp, fc, texp)
+    return (len(pos), len(fc), cp(pos), cp(nrm), cp(uvp), cp(colp), cp(fc), cp(texp), Ht, Wt), keep
+
+
 class PendingPoses:
     """The host poses of one tracking call submitted with wait=False.  result() waits for the call's read-back (once; later
     calls return the same array) and returns what the blocking call returns as its host poses.  A handle dropped without
@@ -220,35 +250,17 @@ class Engine:
         _lib.check(lib.fp_set_config(self._h, which, float(crop_ratio), float(rot_normalizer)), "fp_set_config")
 
     def load_network(self, kind, state_dict):
-        packed = pack_network(state_dict, kind)
-        arr = (_FpTensor * len(packed))()
-        keep = []
-        for i, (name, a) in enumerate(packed.items()):
-            a = np.ascontiguousarray(a)
-            keep.append(a)
-            arr[i] = _FpTensor(name.encode(), a.ctypes.data, 1 if a.dtype == np.float16 else 0, a.size)
-        _lib.check(lib.fp_load_network(self._h, 0 if kind == "refine" else 1, arr, len(packed)), "fp_load_network")
+        arr, keep = _tensor_array(pack_network(state_dict, kind))
+        _lib.check(lib.fp_load_network(self._h, 0 if kind == "refine" else 1, arr, len(arr)), "fp_load_network")
 
     def set_mesh(self, vertices, normals, faces, diameter, uv=None, tex=None, vertex_colors=None, slot=0):
         """uv: (V,2) with v already flipped (Utils.py:117); tex: uint8 (Ht,Wt,3); vertex_colors: float 0..1.
         slot: 0..MAX_MESHES-1; slot 0 is the mesh of every single-object call, the others are for track_objects."""
-        pos = np.ascontiguousarray(vertices, dtype=np.float32)
-        nrm = np.ascontiguousarray(normals, dtype=np.float32)
-        fc = np.ascontiguousarray(faces, dtype=np.int32)
-        uvp = texp = colp = None
-        Ht = Wt = 0
-        if uv is not None and tex is not None:
-            uvp = np.ascontiguousarray(uv, dtype=np.float32)
-            texp = np.ascontiguousarray(tex[..., :3], dtype=np.uint8)
-            Ht, Wt = texp.shape[:2]
-        else:
-            colp = np.ascontiguousarray(vertex_colors, dtype=np.float32)
-        cp = lambda a: None if a is None else C.c_void_p(a.ctypes.data)
-        _lib.check(lib.fp_set_mesh_slot(self._h, int(slot), len(pos), len(fc), cp(pos), cp(nrm), cp(uvp), cp(colp), cp(fc), cp(texp),
-                                        Ht, Wt, float(diameter)), "fp_set_mesh")
+        args, keep = _mesh_args(vertices, normals, faces, uv, tex, vertex_colors)
+        _lib.check(lib.fp_set_mesh_slot(self._h, int(slot), *args, float(diameter)), "fp_set_mesh")
         if slot == 0:
             self.diameter = float(diameter)
-            self.mesh_key = (len(pos), len(fc), float(diameter))
+            self.mesh_key = (args[0], args[1], float(diameter))
 
     def graph_captures(self):
         """Number of CUDA graphs this context has captured (a replay captures none)."""

@@ -13,7 +13,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import lib
-from .engine import _FpTensor, pack_network
+from .engine import _FpTensor, _mesh_args, _tensor_array, pack_network
 
 vp, i32, f32 = C.c_void_p, C.c_int, C.c_float
 lib.fp_group_create.argtypes = [i32, C.POINTER(i32), C.POINTER(vp)]
@@ -54,33 +54,15 @@ class EngineGroup:
         return len(self.device_ids)
 
     def load_network(self, kind, state_dict):
-        packed = pack_network(state_dict, kind)
-        arr = (_FpTensor * len(packed))()
-        keep = []
-        for k, (name, a) in enumerate(packed.items()):
-            a = np.ascontiguousarray(a)
-            keep.append(a)
-            arr[k] = _FpTensor(name.encode(), a.ctypes.data, 1 if a.dtype == np.float16 else 0, a.size)
-        _lib.check(lib.fp_group_load_network(self._h, 0 if kind == "refine" else 1, arr, len(packed)), "fp_group_load_network")
+        arr, keep = _tensor_array(pack_network(state_dict, kind))
+        _lib.check(lib.fp_group_load_network(self._h, 0 if kind == "refine" else 1, arr, len(arr)), "fp_group_load_network")
 
     def set_config(self, kind, crop_ratio=1.2, rot_normalizer=0.3490658503988659):
         _lib.check(lib.fp_group_set_config(self._h, 0 if kind == "refine" else 1, float(crop_ratio), float(rot_normalizer)), "fp_group_set_config")
 
     def set_mesh(self, vertices, normals, faces, diameter, uv=None, tex=None, vertex_colors=None):
-        pos = np.ascontiguousarray(vertices, dtype=np.float32)
-        nrm = np.ascontiguousarray(normals, dtype=np.float32)
-        fc = np.ascontiguousarray(faces, dtype=np.int32)
-        uvp = texp = colp = None
-        Ht = Wt = 0
-        if uv is not None and tex is not None:
-            uvp = np.ascontiguousarray(uv, dtype=np.float32)
-            texp = np.ascontiguousarray(tex[..., :3], dtype=np.uint8)
-            Ht, Wt = texp.shape[:2]
-        else:
-            colp = np.ascontiguousarray(vertex_colors, dtype=np.float32)
-        cp = lambda a: None if a is None else vp(a.ctypes.data)
-        _lib.check(lib.fp_group_set_mesh(self._h, len(pos), len(fc), cp(pos), cp(nrm), cp(uvp), cp(colp), cp(fc), cp(texp), Ht, Wt,
-                                         float(diameter)), "fp_group_set_mesh")
+        args, keep = _mesh_args(vertices, normals, faces, uv, tex, vertex_colors)
+        _lib.check(lib.fp_group_set_mesh(self._h, *args, float(diameter)), "fp_group_set_mesh")
 
     def register(self, rgb, depth, K, mask, rot_grid, iterations=5):
         """HOST numpy in, HOST numpy out: refined poses (N,4,4), scores (N,), best index, info (tx, ty, tz, n_valid)."""

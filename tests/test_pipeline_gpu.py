@@ -190,7 +190,7 @@ def test_predict_honours_per_call_arguments(setup):
 
 
 def test_decoder_heads_on_two_streams_is_bitwise_serial(setup, monkeypatch):
-    """The two refiner decoder heads run on two streams at small batches (fp_api.cu run_refine_heads, fork / join
+    """The two refiner decoder heads run on two streams at small batches (fp_net.cu run_refine_heads, fork / join
     captured into the graph).  Same kernels on the same data: the poses must be bit-identical to the serial order,
     eagerly (first call), while capturing (second) and on graph replay (third)."""
     from foundationpose_b200.engine import Engine
