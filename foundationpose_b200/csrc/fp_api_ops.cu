@@ -123,6 +123,26 @@ int fp_op_build_meshlets(int V, int F, const float* pos, const int* faces, int* 
   FP_API_END
 }
 
+int fp_op_meshlet_sizes(int V, int F, const float* pos, const int* faces, int* tris_of_meshlet_out) {
+  FP_API_BEGIN
+  if (!pos || !faces || !tris_of_meshlet_out || V <= 0 || F <= 0) {
+    fp::set_last_error("fp_op_meshlet_sizes: bad argument");
+    return -1;
+  }
+  for (int i = 0; i < 3 * F; ++i)
+    if (faces[i] < 0 || faces[i] >= V) {
+      fp::set_last_error("fp_op_meshlet_sizes: face index out of range");
+      return -1;
+    }
+  std::vector<float> nrm((size_t)V * 3, 0.f), att((size_t)V * 3, 0.f);
+  fp::MeshHost mh;
+  int rc = fp::build_mesh_host(V, F, pos, nrm.data(), att.data(), 3, faces, mh);
+  if (rc) return rc;
+  for (size_t i = 0; i < mh.meshlets.size(); ++i) tris_of_meshlet_out[i] = mh.meshlets[i].n_tris;
+  return (int)mh.meshlets.size();
+  FP_API_END
+}
+
 int fp_op_attention(const void* qkv, void* out, int B, int impl, void* stream) {
   FP_API_BEGIN
   if (!qkv || !out) {

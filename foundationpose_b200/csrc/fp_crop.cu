@@ -214,12 +214,10 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
   const float oz = -(sm.P[2] * sm.P[3] + sm.P[6] * sm.P[7] + sm.P[10] * sm.P[11]);
   const float iz_far = 1.f / p.zfar;
   int n_vis = 0, n_tri = 0, n_frag = 0, n_mixed = 0;
-  // back faces may only be skipped when the camera centre is outside the solid (bounding sphere: conservative)
+  // back faces may only be skipped when the near plane clips nothing of the solid: a front face cut away by it uncovers
+  // the back faces behind it.  Bounding sphere, conservative; it also rules out a camera centre inside the solid.
   int front_sign = M.front_sign;
-  {
-    const float bx = ox - M.bs_x, by = oy - M.bs_y, bz = oz - M.bs_z;
-    if (bx * bx + by * by + bz * bz <= M.bs_r * M.bs_r) front_sign = 0;
-  }
+  if (sm.P[8] * M.bs_x + sm.P[9] * M.bs_y + sm.P[10] * M.bs_z + sm.P[11] - M.bs_r <= p.znear) front_sign = 0;
 
   for (int base = 0; base < M.n_meshlets; base += kListCap) {
     // ---- binning: meshlet bounding sphere vs this tile, normal cone vs the camera

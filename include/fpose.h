@@ -472,6 +472,10 @@ long long fp_op_encoder(fp_ctx* ctx, int which, const void* crops, int N, int la
  * original face id of every meshlet triangle.  Verifies internally that every meshlet triangle maps back to its face. */
 int fp_op_build_meshlets(int V, int F, const float* pos, const int* faces, int* info, int* face_of_tri_out,
                          float* meshlets_out /* optional [ceil(F/1)][8]: sphere xyz r, cone axis xyz cutoff */);
+/* Host-only hook on the same mesh preparation: writes the number of triangles of each meshlet, in the order the crop
+ * producer bins them (and fp_op_build_meshlets' face_of_tri_out lists their faces), to tris_of_meshlet_out ([F]
+ * suffices).  Returns the number of meshlets, or a negative error code. */
+int fp_op_meshlet_sizes(int V, int F, const float* pos, const int* faces, int* tris_of_meshlet_out);
 /* which: 0 = erode_depth (Utils.py:359-395), 1 = bilateral_filter_depth (Utils.py:304-356) */
 int fp_op_depth_filter(const float* depth_dev, float* out_dev, int H, int W, int which, void* stream);
 /* egocentric_delta_pose_to_pose with the refiner's output decoding (predict_pose_refine.py:195-231), launched as the
