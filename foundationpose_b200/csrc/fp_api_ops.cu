@@ -426,6 +426,42 @@ long long fp_op_encoder(fp_ctx* c, int which, const void* crops, int N, int last
   FP_API_END
 }
 
+long long fp_op_heads(fp_ctx* c, int which, const void* tok, int N, int stage, void* out, void* stream) {
+  FP_API_BEGIN
+  const char* fn = "fp_op_heads";
+  FP_REQUIRE(c, "%s: null context", fn);
+  FP_REQUIRE(which == 0 || which == 1, "%s: which = %d, must be 0 (refiner) or 1 (scorer)", fn, which);
+  const int stages = which == 0 ? 7 : 4;
+  FP_REQUIRE(stage >= 0 && stage < stages, "%s: stage = %d outside [0, %d]", fn, stage, stages - 1);
+  FP_REQUIRE(N >= 1 && N <= kRegisterPassCap, "%s: N = %d outside [1, %d]", fn, N, kRegisterPassCap);
+  FP_REQUIRE(tok && out, "%s: null tok or out", fn);
+  FP_REQUIRE(c->net[which].loaded, "%s: %s weights not loaded", fn, which == 0 ? "refiner" : "scorer");
+  DeviceGuard dg(c->device);
+  if (check_device_ptr(tok, "tok", fn) || check_device_ptr(out, "out", fn)) return -1;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  FP_TRY(order_after_track(c, st));
+  FP_TRY(ensure_capacity(c, N));  // may reallocate: the buffers are looked up after it
+  const size_t M = (size_t)N * T;
+  FP_CUDA_OK(cudaMemcpyAsync(c->tok.p, tok, M * 512 * 2, cudaMemcpyDeviceToDevice, st));
+  const void* src;
+  size_t bytes;
+  if (which == 0) {
+    FP_TRY(run_refine_heads(c, c->net[0], N, st));
+    const size_t act = 2 * M * 512 * 2;  // [2][M][512] fp16
+    const void* bufs[7] = {c->qkv.p, c->att.p, c->x1pre.p, c->x1.p, c->ff.p, c->x2pre.p, c->head_out.p};
+    const size_t sizes[7] = {M * 3072 * 2, act, act, act, act, act, (size_t)2 * N * 3 * 4};
+    src = bufs[stage], bytes = sizes[stage];
+  } else {
+    FP_TRY(run_score_feats(c, c->net[1], N, reinterpret_cast<float*>(c->feats.p), st));
+    const void* bufs[4] = {c->qkv.p, c->att.p, c->tok_mean.p, c->feats.p};
+    const size_t sizes[4] = {M * 1536 * 2, M * 512 * 2, (size_t)N * 512 * 4, (size_t)N * 512 * 4};
+    src = bufs[stage], bytes = sizes[stage];
+  }
+  FP_CUDA_OK(cudaMemcpyAsync(out, src, bytes, cudaMemcpyDeviceToDevice, st));
+  return (long long)bytes;
+  FP_API_END
+}
+
 int fp_op_score_tail_segments(fp_ctx* c, const float* feats, int L, const int* seg_host, int n_seg, float* scores_out,
                               int* best_out, void* stream) {
   FP_API_BEGIN

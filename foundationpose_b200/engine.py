@@ -62,6 +62,8 @@ def _proto():
     lib.fp_op_score_feats.argtypes = [vp, vp, i, vp, vp]
     lib.fp_op_encoder.argtypes = [vp, i, vp, i, i, vp, vp]
     lib.fp_op_encoder.restype = C.c_longlong
+    lib.fp_op_heads.argtypes = [vp, i, vp, i, i, vp, vp]
+    lib.fp_op_heads.restype = C.c_longlong
     lib.fp_op_encoder_layer.argtypes = [i, i, C.POINTER(i)]
     lib.fp_op_depth_filter.argtypes = [vp, vp, i, i, i, vp]
     lib.fp_op_pose_update.argtypes = [vp, vp, vp, vp, C.POINTER(i), i, vp, vp, vp, vp]
@@ -657,6 +659,30 @@ class Engine:
         rc = lib.fp_op_encoder(self._h, 0 if kind == "refine" else 1, _p(crops), int(N), int(last), _p(out), _stream())
         _lib.check(rc if rc < 0 else 0, "fp_op_encoder")
         assert rc == out.numel() * out.element_size(), f"fp_op_encoder copied {rc} bytes into a {tuple(out.shape)} buffer"
+        return out
+
+    # fp_op_heads: the buffer each stage leaves, as (dtype, shape at N hypotheses of 400 tokens)
+    HEAD_STAGES = {
+        "refine": [(torch.float16, lambda N: (N * 400, 3072))]
+        + [(torch.float16, lambda N: (2, N * 400, 512))] * 5 + [(torch.float32, lambda N: (2, N, 3))],
+        "score": [(torch.float16, lambda N: (N * 400, 1536)), (torch.float16, lambda N: (N * 400, 512)),
+                  (torch.float32, lambda N: (N, 512)), (torch.float32, lambda N: (N, 512))],
+    }
+
+    def op_heads(self, kind, tok, N, stage):
+        """fp_op_heads: the heads of network `kind` (run_refine_heads / run_score_feats) on the tokens (fp16 CUDA, N x 400
+        x 512 contiguous) -> the buffer of stage `stage`.  Refiner: 0 qkv (M, 3072), 1 att, 2 x1pre, 3 x1, 4 ff, 5 x2pre
+        (each (2, M, 512) fp16, one block per head), 6 head_out (2, N, 3) fp32; scorer: 0 qkv (M, 1536), 1 att (M, 512),
+        2 the token mean of att (N, 512) fp32, 3 the features (N, 512) fp32.  M = 400 N."""
+        stages = self.HEAD_STAGES[kind]
+        if not 0 <= stage < len(stages):
+            raise ValueError(f"op_heads: {kind} has stages 0..{len(stages) - 1}, not {stage}")
+        assert tok.dtype == torch.float16 and tok.is_contiguous() and tok.numel() == N * 400 * 512
+        dtype, shape = stages[stage]
+        out = torch.empty(*shape(N), dtype=dtype, device="cuda")
+        rc = lib.fp_op_heads(self._h, 0 if kind == "refine" else 1, _p(tok), int(N), int(stage), _p(out), _stream())
+        _lib.check(rc if rc < 0 else 0, "fp_op_heads")
+        assert rc == out.numel() * out.element_size(), f"fp_op_heads copied {rc} bytes into a {tuple(out.shape)} buffer"
         return out
 
     def op_tokens(self, kind, crops, N):

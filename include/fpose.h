@@ -466,6 +466,14 @@ int fp_op_encoder_layer(int layer, int N, int* info);
  * to `out` (device).  Returns the bytes copied, or a negative error code; every argument is checked before anything
  * is enqueued on `stream`. */
 long long fp_op_encoder(fp_ctx* ctx, int which, const void* crops, int N, int last, void* out, void* stream);
+/* Runs the heads of network `which` (0 = refiner: run_refine_heads, 1 = scorer: run_score_feats) on given tokens `tok`
+ * (device, fp16 [N][400][512], 1 <= N <= 512) and copies one of the workspace buffers they leave to `out` (device).
+ * M = 400 N rows; fp16 unless marked fp32; [2] = the two refiner heads (0 trans, 1 rot):
+ *   refiner  0 qkv [M][3072], 1 att [2][M][512], 2 x1pre = out_proj(att) + tok, 3 x1 = LayerNorm1(x1pre),
+ *            4 ff = relu(linear1(x1)), 5 x2pre = linear2(ff) + x1 (2-5 each [2][M][512]), 6 head_out fp32 [2][N][3]
+ *   scorer   0 qkv [M][1536], 1 att [M][512], 2 token mean of att fp32 [N][512], 3 features fp32 [N][512]
+ * Returns the bytes copied, or a negative error code; every argument is checked before anything is enqueued. */
+long long fp_op_heads(fp_ctx* ctx, int which, const void* tok, int N, int stage, void* out, void* stream);
 /* Host-only hook (no GPU needed) on the mesh preparation fp_set_mesh performs: meshlets of <= 64 triangles / <= 64
  * vertices + closedness / orientation analysis.  info[6] = {meshlets, closed (0/1), front-face winding sign (0 = none),
  * max triangles per meshlet, max vertices per meshlet, total triangles}; face_of_tri_out (optional, [F]) receives the

@@ -88,12 +88,14 @@ def conv_terms(x, w, kind, H, shift=False):
     return acc, mag, tap22
 
 
-def epilogue(acc, b, res=None, pe=None):
-    """relu(acc + b + res) + pe in float64; b (Co,), res like acc, pe (Ho, Wo, Co)."""
+def epilogue(acc, b, res=None, pe=None, relu=True):
+    """relu(acc + b + res) + pe in float64; b (Co,), res like acc, pe (Ho, Wo, Co).  relu=False: the linear layers
+    without ReLU (tests/heads_reference.py)."""
     y = acc + b.double()
     if res is not None:
         y = y + res.double()
-    y = y.clamp_min(0.0)
+    if relu:
+        y = y.clamp_min(0.0)
     if pe is not None:
         y = y + pe.double()
     return y

@@ -15,11 +15,9 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-pytestmark = pytest.mark.gpu
+import heads_reference as ref
 
-U16 = 2.0 ** -11  # unit roundoff of fp16
-U32 = 2.0 ** -24  # unit roundoff of fp32
-SCALE = 1.0 / math.sqrt(128)
+pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(autouse=True)
@@ -60,41 +58,15 @@ def _attn_inputs(B, G, seed):
     return x.reshape(B * 400, G * 1536)
 
 
-def _attn_reference(qkv, B, G, g, b0, b1):
-    """float64 attention of sequences [b0, b1) of group g from the same fp16 q, k, v -> [b, 400, 4, 128] tensors:
-    o_ref, P_ref @ |V| (row-normalised), the subnormal term, and the two probes (o with the last 80 keys dropped for
-    query tile 3, o with P rounded through bfloat16)."""
-    x = qkv.view(B, 400, G, 3, 4, 128)[b0:b1, :, g].double().permute(2, 0, 3, 1, 4)  # [3, b, head, 400, 128]
-    q, k, v = x[0], x[1], x[2]
-    s = (q @ k.transpose(-1, -2)) * SCALE
-    p = torch.exp(s - s.amax(-1, keepdim=True))
-    l = p.sum(-1, keepdim=True)
-    o = p @ v / l
-    pv_abs = p @ v.abs() / l
-    sub = 2.0 ** -25 * v.abs().sum(-2, keepdim=True) / l + 2.0 ** -24
-    o_bf16 = p.to(torch.bfloat16).double() @ v / l
-    s3 = s[:, :, 384:, :320]  # query tile 3 (rows 384..399) without the last 80-key chunk
-    p3 = torch.exp(s3 - s3.amax(-1, keepdim=True))
-    o_drop = o.clone()
-    o_drop[:, :, 384:] = p3 @ v[:, :, :320] / p3.sum(-1, keepdim=True)
-    t = lambda a: a.permute(0, 2, 1, 3)  # -> [b, 400, head, 128]
-    return t(o), t(pv_abs), t(sub.expand_as(o)), t(o_drop), t(o_bf16)
-
-
 @pytest.mark.parametrize("G", [1, 2], ids=lambda g: f"G{g}")
 @pytest.mark.parametrize("B", [1, 3, 66, 67, 249, 252], ids=lambda b: f"B{b}")
 def test_attention_groups(B, G):
     """attn_tc_kernel (fp_attn_tc.cu) through fp_op_attention_groups, the launch of run_refine_heads (G = 2, ld 3072)
     and run_score_feats (G = 1, ld 1536), against float64 softmax(q k^T / sqrt(128)) v on the same fp16 q, k, v.
 
-    Error bound per output element.  S = q k^T is exact products summed in fp32; P = exp(S - m) is kept in fp32 for
-    the row sum l, but packed to fp16 (relative error <= u = 2^-11, or <= 2^-25 absolute below fp16's normal range)
-    before P V, which accumulates in fp32.  So O / l = sum_k p~_k v_k with |p~_k - p_k| <= u p_k + 2^-25 / l, hence
-    |O / l - o_ref| <= u (P_ref @ |V|) + 2^-25 sum_k |v_k| / l.  The output is rounded to fp16: another u |o|
-    (<= u |o_ref| + u^2 (...)), or 2^-24 absolute for subnormal outputs.  Together
-        |o - o_ref| <= u (|o_ref| + P_ref @ |V|) + 2^-25 sum_k |v_k| / l + 2^-24.
-    The fp32 parts (S, exp2f, alpha rescales, the sums) are a few 2^-24 relative to the same magnitudes; the safety
-    factor 1.25 on the u term covers them.  Measured on an H100: at most 0.75 of this bar over the whole grid.
+    Error bound per output element: heads_reference.attention_bar,
+        |o - o_ref| <= 1.25 u (|o_ref| + P_ref @ |V|) + 2^-25 sum_k |v_k| / l + 2^-24,
+    derived there.  Measured on an H100: at most 0.75 of this bar over the whole grid.
 
     Probes: dropping the last 80-key chunk for query tile 3 must fail on more than half of tile 3's elements (81 to 89 %
     measured); rounding P through bfloat16 (4x fp16's rounding) must fail on more than 1 % of all elements (3.6 to
@@ -116,8 +88,8 @@ def test_attention_groups(B, G):
         got = out[g].view(B, 400, 4, 128)
         for b0 in range(0, B, chunk):
             b1 = min(B, b0 + chunk)
-            o_ref, pv_abs, sub, o_drop, o_bf16 = _attn_reference(qkv, B, G, g, b0, b1)
-            bar = 1.25 * U16 * (o_ref.abs() + pv_abs) + sub
+            o_ref, pv_abs, sub, o_drop, o_bf16 = ref.attention(qkv, B, G, g, b0, b1)
+            bar = ref.attention_bar(o_ref, pv_abs, sub)
             o = got[b0:b1].double()
             err = (o - o_ref).abs()
             bad = err > bar
@@ -148,11 +120,9 @@ def test_layernorm(rows):
     Edge rows: row 1 is constant (mean exact, variance 0: the output must be beta rounded to fp16, exactly); row 2 has
     mean ~1000 and spread ~1 (cancellation); row 3 has values near +-6e4 (squares near 4e9).
 
-    Error bound: the mean is an fp32 sum of 512 values in a chain 21 deep (16 in-lane adds, 5 shuffles), so
-    |dmean| <= 21 u32 mean|x|; the variance sum the same, relative; rsqrtf is within 2 ulp; the affine step adds a few
-    roundings.  With z = (x - mean) rstd:  |y - y_ref| <= u16 |y_ref| + |gamma| (|z| 32 u32 + rstd |dmean|) +
-    |beta| 2 u32 + 2^-24, and a safety factor 1.25.  Probe: the variance divided by 511 instead of 512 (z off by
-    1/1022, about 2 u16) must fail on more than half of the elements (88 % measured; at most 0.80 of the bar reached)."""
+    Error bound: heads_reference.layernorm, derived there.  Probe: the variance divided by 511 instead of 512 (z off
+    by 1/1022, about 2 u16) must fail on more than half of the elements (88 % measured; at most 0.80 of the bar
+    reached)."""
     from foundationpose_b200 import ops
 
     gen = torch.Generator(device="cuda").manual_seed(rows)
@@ -165,18 +135,11 @@ def test_layernorm(rows):
     x16 = x.half()
     y = ops.layernorm(x16, gamma, beta).double()
     assert torch.equal(y[1], beta.half().double()), "a constant row must give beta rounded to fp16"
-    xd, g, b = x16.double(), gamma.double(), beta.double()
-    ref = F.layer_norm(xd, (512,), g, b, 1e-5)
-    mean = xd.mean(-1, keepdim=True)
-    var = xd.var(-1, unbiased=False, keepdim=True)
-    rstd = (var + 1e-5).rsqrt()
-    z = (xd - mean) * rstd
-    dmean = 21 * U32 * xd.abs().mean(-1, keepdim=True)
-    bar = 1.25 * (U16 * ref.abs() + g.abs() * (z.abs() * 32 * U32 + rstd * dmean) + b.abs() * 2 * U32) + 2.0 ** -24
-    err = (y - ref).abs()
+    y_ref, bar = ref.layernorm(x16, gamma, beta)
+    err = (y - y_ref).abs()
     ratio = _report(f"layernorm rows={rows}", err, bar)
     assert ratio <= 1.0, f"layernorm rows={rows}: {int((err > bar).sum())} elements over the bar, first row {int((err > bar).any(-1).nonzero()[0])}"
-    probe = (xd - mean) * (var * 512 / 511 + 1e-5).rsqrt() * g + b
+    probe = ref.layernorm_var511(x16, gamma, beta)
     frac = _probe_fraction((y - probe).abs(), bar)
     print(f"layernorm rows={rows}: variance/511 probe fails {frac:.2%}")
     assert frac > 0.5, "the bar does not see the variance divided by 511"
@@ -193,10 +156,8 @@ def _tokens(B, seed):
     return (base + 0.5 * torch.randn(B, 400, 512, generator=gen, device="cuda")).half()
 
 
-# Both reductions sum 400 tokens in fp32 chains about 23 deep (per-warp rows, eight warps, eight token ranges), divide
-# by 400 and take a dot product over 512 channels 21 deep; the LayerNorm before it costs about 35 u32 relative.  The
-# bound is therefore below 80 u32 of the L1 magnitude M_j = sum_c |W_jc| mean_t |x_tc| + |b_j|; the bar is 128 u32 M.
-TOKEN_BAR_U32 = 128
+# Both reductions are held to heads_reference.TOKEN_BAR_U32 u32 of the L1 magnitude M_j = sum_c |W_jc| mean_t |x_tc| +
+# |b_j| (derived there).
 
 
 @pytest.mark.parametrize("B", [1, 66, 67, 252])
@@ -217,13 +178,10 @@ def test_head_final(B):
     bias = 0.01 * torch.randn(3, generator=gen, device="cuda")
     out = ops.head_final(x, gamma, beta, w, bias).double()
     ln = F.layer_norm(x.double(), (512,), gamma.double(), beta.double(), 1e-5)
-    wd, bd = w.double(), bias.double()
-    ref = ln.mean(1) @ wd.t() + bd
-    mag = ln.abs().mean(1) @ wd.abs().t() + bd.abs()
-    bar = TOKEN_BAR_U32 * U32 * mag
-    err = (out - ref).abs()
+    y_ref, bar = ref.token_readout(ln, w, bias)
+    err = (out - y_ref).abs()
     assert _report(f"head_final B={B}", err, bar) <= 1.0
-    probe = ln.sum(1) / 399 @ wd.t() + bd
+    probe, _ = ref.token_readout(ln, w, bias, tokens=399)
     frac = _probe_fraction((out - probe).abs(), bar)
     print(f"head_final B={B}: 399-token probe fails {frac:.2%}")
     assert frac > 0.6, "the bar does not see a mean over 399 tokens"
@@ -241,13 +199,10 @@ def test_token_mean_proj(B):
     w = torch.randn(512, 512, generator=gen, device="cuda") / math.sqrt(512)
     bias = 0.01 * torch.randn(512, generator=gen, device="cuda")
     out = ops.token_mean_proj(x, w, bias).double()
-    xd, wd, bd = x.double(), w.double(), bias.double()
-    ref = xd.mean(1) @ wd.t() + bd
-    mag = xd.abs().mean(1) @ wd.abs().t() + bd.abs()
-    bar = TOKEN_BAR_U32 * U32 * mag
-    err = (out - ref).abs()
+    y_ref, bar = ref.token_readout(x, w, bias)
+    err = (out - y_ref).abs()
     assert _report(f"token_mean_proj B={B}", err, bar) <= 1.0
-    probe = xd.sum(1) / 399 @ wd.t() + bd
+    probe, _ = ref.token_readout(x, w, bias, tokens=399)
     frac = _probe_fraction((out - probe).abs(), bar)
     print(f"token_mean_proj B={B}: 399-token probe fails {frac:.2%}")
     assert frac > 0.6, "the bar does not see a mean over 399 tokens"
