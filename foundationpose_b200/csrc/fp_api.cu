@@ -296,22 +296,53 @@ static int set_busy(StagingSet& set, cudaStream_t st) {
   return 0;
 }
 
-// Host memory that the device cannot read in place, so a copy from it may wait on the stream.  Page-locked (and device
-// or managed) memory is anything cudaPointerGetAttributes knows.
-static bool pageable(const void* p) {
+// Where one of the caller's input buffers lives, as cudaPointerGetAttributes sees it
+enum class Residence {
+  Pageable,     // host memory the device cannot read in place: a copy from it may wait on the stream
+  HostLocked,   // page-locked or managed memory: host memory the device can also read
+  Device,       // device memory of the context's device: the kernels can read it in place
+  OtherDevice,  // device memory of another device: refused where a call would read it in place
+};
+static Residence residence(const fp_ctx* c, const void* p) {
   cudaPointerAttributes a;
   if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
     cudaGetLastError();  // not sticky; keep it out of the next caller's error check
-    return true;
+    return Residence::Pageable;
   }
-  return a.type == cudaMemoryTypeUnregistered;
+  if (a.type == cudaMemoryTypeUnregistered) return Residence::Pageable;
+  if (a.type == cudaMemoryTypeDevice) return a.device == c->device ? Residence::Device : Residence::OtherDevice;
+  return Residence::HostLocked;  // cudaMemoryTypeHost, cudaMemoryTypeManaged
+}
+
+// Whether the caller's frame or mask buffer `p` of a tracking or register call is read in place (device memory of the
+// context's device) or staged (host memory).  Device memory of another device is refused.  what / i name the buffer.
+static int read_in_place(const fp_ctx* c, const void* p, bool& in_place, const char* caller, const char* what, int i) {
+  const Residence r = residence(c, p);
+  FP_REQUIRE(r != Residence::OtherDevice, "%s: %s %d is device memory of another device than the context's (device %d)",
+             caller, what, i, c->device);
+  in_place = r == Residence::Device;
+  return 0;
+}
+
+// Which frame buffers of a call's C cameras are read in place (see read_in_place), each camera's rgb and depth on
+// their own.  Classified before anything is enqueued.
+struct FrameSources {
+  bool rgb[kMaxCameras] = {}, depth[kMaxCameras] = {};
+};
+static int frame_sources(const fp_ctx* c, int C, const unsigned char* const* rgb, const float* const* depth, FrameSources& on_dev,
+                         const char* caller) {
+  for (int i = 0; i < C; ++i) {
+    FP_TRY(read_in_place(c, rgb[i], on_dev.rgb[i], caller, "the rgb frame of camera", i));
+    FP_TRY(read_in_place(c, depth[i], on_dev.depth[i], caller, "the depth frame of camera", i));
+  }
+  return 0;
 }
 
 // Uploads `bytes` of the caller's host memory `src` to `dst` on `st`.  Page-locked memory is copied straight from the
 // caller's buffer, which must stay untouched until `st` has passed the copy; pageable memory goes through `stage` of the
 // next staging set, so the caller may reuse it once this returns and the host does not wait on the stream for it.
 static int upload_host(fp_ctx* c, void* dst, const void* src, size_t bytes, PinnedBuf StagingSet::*stage, cudaStream_t st) {
-  if (!pageable(src)) {
+  if (residence(c, src) != Residence::Pageable) {
     FP_CUDA_OK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st));
     return 0;
   }
@@ -337,12 +368,15 @@ constexpr size_t kTableBytes = sizeof(CameraDev) * kMaxCameras;  // the camera t
 // camera's buffers are sized for the largest frame of the call (kept at the largest size seen, so a permutation of the
 // same cameras allocates nothing), the argument block is sized for `rows` slot and camera ids and its staging for
 // `staged_rows`, every camera records its size and intrinsics (K: [C][9]; camera 0's become the context's frame
-// geometry), the staging receives the camera table (every camera's record; entries C.. zeroed), and every frame is
-// uploaded through its camera's staging (camera i's DMA runs while camera i + 1 is copied on the host).  H_max / W_max:
-// the largest frame height and width of the call.  `set`: the staging set the call uploads through (not busy).
-static int setup_cameras(fp_ctx* c, StagingSet& set, int C, const unsigned char* const* rgb_host,
-                         const float* const* depth_host, const float* K, const int* H, const int* W, int rows,
-                         int staged_rows, cudaStream_t st, int& H_max, int& W_max) {
+// geometry), the staging receives the camera table (every camera's record; entries C.. zeroed), and every host frame is
+// uploaded through its camera's staging (camera i's DMA runs while camera i + 1 is copied on the host).  A frame buffer
+// on the device (on_dev) is read in place: its table entry points at the caller's buffer, and nothing is staged or
+// uploaded for it.  Every camera still gets its raw upload buffers, so where a frame lives never changes an allocation
+// or the graph epoch.  H_max / W_max: the largest frame height and width of the call.  `set`: the staging set the call
+// uploads through (not busy).
+static int setup_cameras(fp_ctx* c, StagingSet& set, int C, const unsigned char* const* rgb, const float* const* depth,
+                         const FrameSources& on_dev, const float* K, const int* H, const int* W, int rows, int staged_rows,
+                         cudaStream_t st, int& H_max, int& W_max) {
   size_t npix_max = 0;
   H_max = W_max = 0;
   for (int i = 0; i < C; ++i) {
@@ -352,8 +386,8 @@ static int setup_cameras(fp_ctx* c, StagingSet& set, int C, const unsigned char*
   }
   for (int i = 0; i < C; ++i) {
     FP_TRY(alloc_camera(c, i, npix_max, /*raw=*/true));
-    FP_TRY(pinned_alloc(nullptr, set.rgb[i], npix_max * 3));
-    FP_TRY(pinned_alloc(nullptr, set.depth[i], npix_max * 4));
+    if (!on_dev.rgb[i]) FP_TRY(pinned_alloc(nullptr, set.rgb[i], npix_max * 3));
+    if (!on_dev.depth[i]) FP_TRY(pinned_alloc(nullptr, set.depth[i], npix_max * 4));
   }
   c->n_frames = C;
   FP_TRY(dev_alloc(&c->epoch, c->args, kTableBytes + (size_t)2 * rows * sizeof(int)));
@@ -363,17 +397,22 @@ static int setup_cameras(fp_ctx* c, StagingSet& set, int C, const unsigned char*
   for (int i = 0; i < C; ++i) {
     set_frame_geometry(c, i, K + 9 * i, H[i], W[i]);
     table[i] = camera_dev(c, i);
-    FP_TRY(upload_staged_frame(c->cam[i], set.rgb[i], set.depth[i], rgb_host[i], depth_host[i], (size_t)H[i] * W[i], st));
+    if (on_dev.rgb[i]) table[i].rgb_raw = rgb[i];
+    if (on_dev.depth[i]) table[i].depth_raw = depth[i];
+    // the order of upload_staged_frame: depth, then rgb
+    const size_t npix = (size_t)H[i] * W[i];
+    if (!on_dev.depth[i]) FP_TRY(stage_copy(c->cam[i].depth_raw.p, set.depth[i], depth[i], npix * 4, st));
+    if (!on_dev.rgb[i]) FP_TRY(stage_copy(c->cam[i].rgb_raw.p, set.rgb[i], rgb[i], npix * 3, st));
   }
   return 0;
 }
 
 // The staging uploads of one tracking call: the frames, then the camera table, the slot ids and the camera ids in one
 // copy to the argument block.  H_max / W_max as setup_cameras.
-static int stage_track_call(fp_ctx* c, StagingSet& set, int C, const unsigned char* const* rgb_host,
-                            const float* const* depth_host, const float* K, const int* H, const int* W, int M,
+static int stage_track_call(fp_ctx* c, StagingSet& set, int C, const unsigned char* const* rgb, const float* const* depth,
+                            const FrameSources& on_dev, const float* K, const int* H, const int* W, int M,
                             const int* camera_of, const int* slots_host, cudaStream_t st, int& H_max, int& W_max) {
-  FP_TRY(setup_cameras(c, set, C, rgb_host, depth_host, K, H, W, M, M, st, H_max, W_max));
+  FP_TRY(setup_cameras(c, set, C, rgb, depth, on_dev, K, H, W, M, M, st, H_max, W_max));
   int* ids = reinterpret_cast<int*>(static_cast<char*>(set.args.p) + kTableBytes);
   memcpy(ids, slots_host, (size_t)M * sizeof(int));
   memcpy(ids + M, camera_of, (size_t)M * sizeof(int));
@@ -388,12 +427,16 @@ static int stage_track_call(fp_ctx* c, StagingSet& set, int C, const unsigned ch
 // block's address, not the frames' sizes, intrinsics or buffers, and is keyed on (M, iterations, C): reordering objects
 // or cameras, new intrinsics or a smaller frame replay it.  One frame_prep_kernel launch filters every camera and the
 // crops take their frame from the table.  The pose read-back follows the launch outside the graph, into the call's own
-// Readback, so one graph serves every staging set.  poses_out_dev and poses_keep_dev (fp_track's continuation pose)
-// are optional and complete in stream order; *ticket receives the call's ticket.
-static int track_cameras_submit(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
-                                const float* K, const int* H, const int* W, int M, const int* camera_of,
-                                const int* slots_host, const float* poses_in_dev, int iterations, float* poses_out_dev,
-                                cudaStream_t st, unsigned long long* ticket, float* poses_keep_dev = nullptr) {
+// Readback, so one graph serves every staging set.  Frames on the device are read in place through the camera table
+// (setup_cameras), so where a frame lives changes neither the graph nor its key.  poses_out_dev and poses_keep_dev
+// (fp_track's continuation pose) are optional and complete in stream order; *ticket receives the call's ticket.
+static int track_cameras_submit(fp_ctx* c, const char* caller, int C, const unsigned char* const* rgb,
+                                const float* const* depth, const float* K, const int* H, const int* W, int M,
+                                const int* camera_of, const int* slots_host, const float* poses_in_dev, int iterations,
+                                float* poses_out_dev, cudaStream_t st, unsigned long long* ticket,
+                                float* poses_keep_dev = nullptr) {
+  FrameSources on_dev;
+  FP_TRY(frame_sources(c, C, rgb, depth, on_dev, caller));  // refused before anything is enqueued
   StagingSet* set;
   FP_TRY(take_set(c, set));
   FP_TRY(order_after_track(c, st));  // the context's device buffers are never used by two streams at once
@@ -408,7 +451,7 @@ static int track_cameras_submit(fp_ctx* c, int C, const unsigned char* const* rg
   FP_TRY(pinned_alloc(nullptr, rb->poses, (size_t)M * 64));
   c->has_frame = false;
   int H_max = 0, W_max = 0;
-  const int staged = stage_track_call(c, *set, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, st, H_max, W_max);
+  const int staged = stage_track_call(c, *set, C, rgb, depth, on_dev, K, H, W, M, camera_of, slots_host, st, H_max, W_max);
   // whatever was staged before a failure is still on its way out: the set stays busy until then
   FP_TRY(set_busy(*set, st));
   FP_TRY(staged);
@@ -475,11 +518,11 @@ int check_slots(const fp_ctx* c, int M, const int* slots, const char* caller) {
 
 // The frames of C cameras and the camera of each of M objects: non-null frames of positive size, every camera id in
 // [0, C) and every camera owning at least one object.  The kernels index the camera table with these ids unchecked.
-static int check_cameras(int C, const unsigned char* const* rgb_host, const float* const* depth_host, const int* H, const int* W,
+static int check_cameras(int C, const unsigned char* const* rgb, const float* const* depth, const int* H, const int* W,
                          int M, const int* camera_of, const char* caller) {
   FP_REQUIRE(C >= 1 && C <= kMaxCameras, "%s: %d cameras, need 1..%d", caller, C, kMaxCameras);
   for (int i = 0; i < C; ++i) {
-    FP_REQUIRE(rgb_host[i] && depth_host[i], "%s: camera %d: null frame", caller, i);
+    FP_REQUIRE(rgb[i] && depth[i], "%s: camera %d: null frame", caller, i);
     FP_REQUIRE(H[i] > 0 && W[i] > 0, "%s: camera %d: empty frame (%d x %d)", caller, i, H[i], W[i]);
   }
   std::vector<int> owns(C, 0);
@@ -492,7 +535,9 @@ static int check_cameras(int C, const unsigned char* const* rgb_host, const floa
 }
 
 // fp_register_cameras and fp_register_objects after validation (n_hyp_host is checked here, before anything is
-// enqueued).  Object i is seen by camera camera_of[i]; its mask is masks_host[i], of its camera's size.  Each pass copies
+// enqueued).  Object i is seen by camera camera_of[i]; its mask is masks[i], of its camera's size.  Frames and masks on
+// the context's device are read in place (frames through the camera table or camera 0's record, masks by device copies
+// into mask_buf), host ones are staged; fp_register_objects' masks are one block, classified once.  Each pass copies
 // its slot ids and per-hypothesis camera ids to the argument block, so the refine / feature graphs hold no per-pass
 // address and are keyed on (kind, pass size, iterations, frame source).
 //   by_value = false (fp_register_cameras): the camera table goes to the argument block once per call.  One
@@ -507,9 +552,9 @@ static int check_cameras(int C, const unsigned char* const* rgb_host, const floa
 //     fp_track_objects shares fp_track_cameras' table path.
 // Both: whole objects in the given order in passes of up to kRegisterPassCap hypotheses (an object above the cap alone),
 // then one segmented scorer tail over all objects.  Synchronises.
-static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
+static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* rgb, const float* const* depth,
                                  const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
-                                 const int* n_hyp_host, const unsigned char* const* masks_host, const float* rot_grids_dev,
+                                 const int* n_hyp_host, const unsigned char* const* masks, const float* rot_grids_dev,
                                  int iterations, float* poses_out_dev, float* scores_out_dev, int* best_out_dev,
                                  float* info_out_dev, cudaStream_t st, bool by_value) {
   const char* caller = by_value ? "fp_register_objects" : "fp_register_cameras";
@@ -519,6 +564,19 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
                n_hyp_host[i]);
     off[i + 1] = off[i] + n_hyp_host[i];
   }
+  FrameSources on_dev;
+  FP_TRY(frame_sources(c, C, rgb, depth, on_dev, caller));
+  std::vector<char> mask_on_dev(M, 0);
+  for (int i = 0; i < M; ++i) {
+    bool d = false;
+    if (by_value && i > 0)
+      d = mask_on_dev[0];
+    else
+      FP_TRY(read_in_place(c, masks[i], d, caller, by_value ? "the mask block starting at object" : "the mask of object", i));
+    mask_on_dev[i] = d;
+  }
+  const bool staged_masks = std::find(mask_on_dev.begin(), mask_on_dev.end(), 0) != mask_on_dev.end();
+  FP_TRY(order_after_track(c, st));
   const int total = off[M];
   // passes: whole objects in the given order, up to kRegisterPassCap hypotheses; an object above the cap alone
   std::vector<int> pass_obj(1, 0);  // first object of every pass, then M
@@ -547,18 +605,19 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
     cudaStream_t st;
     ~MarkBusy() { set_busy(set, st); }
   } mark_busy{*set, st};
-  FP_TRY(pinned_alloc(nullptr, set->masks, mask_bytes));
+  if (staged_masks) FP_TRY(pinned_alloc(nullptr, set->masks, mask_bytes));
   FP_TRY(pinned_alloc(nullptr, set->ints, (size_t)(2 * M + 2) * sizeof(int) + (size_t)M * sizeof(size_t)));
   c->has_frame = false;
   int H_max, W_max;
-  FP_TRY(setup_cameras(c, *set, C, rgb_host, depth_host, K, H, W, max_pass, total, st, H_max, W_max));
+  FP_TRY(setup_cameras(c, *set, C, rgb, depth, on_dev, K, H, W, max_pass, total, st, H_max, W_max));
   int* ints = reinterpret_cast<int*>(set->ints.p);
   size_t* stage_mask_off = reinterpret_cast<size_t*>(ints + 2 * M + 2);
   memcpy(ints, off.data(), (size_t)(M + 1) * sizeof(int));
   memcpy(ints + M + 1, camera_of, (size_t)M * sizeof(int));
   memcpy(stage_mask_off, mask_at.data(), (size_t)M * sizeof(size_t));
   for (int i = 0; i < M; ++i)
-    memcpy(static_cast<unsigned char*>(set->masks.p) + mask_at[i], masks_host[i], mask_at[i + 1] - mask_at[i]);
+    if (!mask_on_dev[i])
+      memcpy(static_cast<unsigned char*>(set->masks.p) + mask_at[i], masks[i], mask_at[i + 1] - mask_at[i]);
   // the ids of the pass starting at row r0 are staged at 2 * r0 after the table: its slot ids, then its camera ids
   int* ids = reinterpret_cast<int*>(static_cast<char*>(set->args.p) + kTableBytes);
   for (size_t p = 0; p + 1 < pass_obj.size(); ++p) {
@@ -572,12 +631,24 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
   ScoreTailParams tp;
   FP_TRY(segmented_tail_params(c, reinterpret_cast<const float*>(c->reg_feats.p), ints, M, /*trailing=*/M, scores_out_dev,
                                best_out_dev, st, caller, tp));
-  FP_CUDA_OK(cudaMemcpyAsync(c->mask_buf.p, set->masks.p, mask_bytes, cudaMemcpyHostToDevice, st));
+  // the masks into mask_buf: every run of staged masks in one copy (all of them in one when every mask is on the host),
+  // every run of device masks that follow each other in the caller's memory in one device-to-device copy
+  for (int i = 0, j; i < M; i = j) {
+    for (j = i + 1; j < M && mask_on_dev[j] == mask_on_dev[i]; ++j)
+      if (mask_on_dev[j] && masks[j] != masks[j - 1] + (mask_at[j] - mask_at[j - 1])) break;
+    unsigned char* dst = static_cast<unsigned char*>(c->mask_buf.p) + mask_at[i];
+    const size_t bytes = mask_at[j] - mask_at[i];
+    if (mask_on_dev[i])
+      FP_CUDA_OK(cudaMemcpyAsync(dst, masks[i], bytes, cudaMemcpyDeviceToDevice, st));
+    else
+      FP_CUDA_OK(cudaMemcpyAsync(dst, static_cast<unsigned char*>(set->masks.p) + mask_at[i], bytes, cudaMemcpyHostToDevice, st));
+  }
   const CameraDev* cams_dev = by_value ? nullptr : reinterpret_cast<const CameraDev*>(c->args.p);
   // estimater.py:173-174, :214 once per camera for every object: erode + bilateral, depth2xyzmap(zfar = inf)
   if (by_value) {
-    FP_TRY(set_frame_launches(c, reinterpret_cast<const unsigned char*>(c->cam[0].rgb_raw.p),
-                              reinterpret_cast<const float*>(c->cam[0].depth_raw.p), FP_FRAME_FILTER_DEPTH, INFINITY, st));
+    const unsigned char* rgb0 = on_dev.rgb[0] ? rgb[0] : static_cast<const unsigned char*>(c->cam[0].rgb_raw.p);
+    const float* depth0 = on_dev.depth[0] ? depth[0] : static_cast<const float*>(c->cam[0].depth_raw.p);
+    FP_TRY(set_frame_launches(c, rgb0, depth0, FP_FRAME_FILTER_DEPTH, INFINITY, st));
   } else {
     FP_CUDA_OK(cudaMemcpyAsync(c->args.p, set->args.p, kTableBytes, cudaMemcpyHostToDevice, st));
     FP_CUDA_OK(cudaMemcpyAsync(c->mask_off.p, stage_mask_off, (size_t)M * sizeof(size_t), cudaMemcpyHostToDevice, st));
@@ -783,7 +854,7 @@ int fp_set_frame(fp_ctx* c, const unsigned char* rgb, const float* depth, const 
   const float* depth_dev = depth;
   if (!on_dev) {
     CameraBufs& f = c->cam[0];
-    if (pageable(rgb) || pageable(depth)) {
+    if (residence(c, rgb) == Residence::Pageable || residence(c, depth) == Residence::Pageable) {
       StagingSet* set;
       FP_TRY(take_set(c, set));
       const int staged = upload_staged_frame(f, set->rgb[0], set->depth[0], rgb, depth, npix, st);
@@ -994,10 +1065,10 @@ int fp_register(fp_ctx* c, const float* poses_host, int N, int iterations, float
   FP_API_END
 }
 
-int fp_track_submit(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
+int fp_track_submit(fp_ctx* c, const unsigned char* rgb, const float* depth, const float* K, int H, int W,
                     const float* pose_in_dev, int iterations, float* pose_out_dev, void* stream, unsigned long long* ticket) {
   FP_API_BEGIN
-  FP_REQUIRE(c && rgb_host && depth_host && K && H > 0 && W > 0 && iterations >= 0 && ticket, "fp_track: bad argument");
+  FP_REQUIRE(c && rgb && depth && K && H > 0 && W > 0 && iterations >= 0 && ticket, "fp_track: bad argument");
   FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
   FP_REQUIRE(c->mesh[0].loaded, "fp_track: no mesh");
   FP_REQUIRE(pose_in_dev || c->track_valid, "fp_track: no previous pose in this context: pass pose_in");
@@ -1006,17 +1077,17 @@ int fp_track_submit(fp_ctx* c, const unsigned char* rgb_host, const float* depth
   float* keep = reinterpret_cast<float*>(c->track_pose.p);
   // fp_track_cameras' one-object, one-camera case: object 0 renders slot 0 in camera 0
   const int zero = 0;
-  FP_TRY(track_cameras_submit(c, 1, &rgb_host, &depth_host, K, &H, &W, 1, &zero, &zero, pose_in_dev ? pose_in_dev : keep,
+  FP_TRY(track_cameras_submit(c, "fp_track", 1, &rgb, &depth, K, &H, &W, 1, &zero, &zero, pose_in_dev ? pose_in_dev : keep,
                               iterations, pose_out_dev, reinterpret_cast<cudaStream_t>(stream), ticket, keep));
   c->track_valid = true;
   return 0;
   FP_API_END
 }
 
-int fp_track(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
+int fp_track(fp_ctx* c, const unsigned char* rgb, const float* depth, const float* K, int H, int W,
              const float* pose_in_dev, int iterations, float* pose_out_dev, float* pose_out_host, void* stream) {
   unsigned long long ticket = 0;
-  const int rc = fp_track_submit(c, rgb_host, depth_host, K, H, W, pose_in_dev, iterations, pose_out_dev, stream, &ticket);
+  const int rc = fp_track_submit(c, rgb, depth, K, H, W, pose_in_dev, iterations, pose_out_dev, stream, &ticket);
   return rc ? rc : fp_track_wait(c, ticket, pose_out_host);
 }
 
@@ -1096,65 +1167,65 @@ int fp_vis(fp_ctx* c, int kind, const float* poses_a, const float* poses_b, int 
   FP_API_END
 }
 
-int fp_track_objects_submit(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
+int fp_track_objects_submit(fp_ctx* c, const unsigned char* rgb, const float* depth, const float* K, int H, int W,
                             int M, const int* slots_host, const float* poses_in_dev, int iterations, float* poses_out_dev,
                             void* stream, unsigned long long* ticket) {
   FP_API_BEGIN
-  FP_REQUIRE(c && rgb_host && depth_host && K && H > 0 && W > 0 && M > 0 && slots_host && poses_in_dev && iterations >= 0 &&
+  FP_REQUIRE(c && rgb && depth && K && H > 0 && W > 0 && M > 0 && slots_host && poses_in_dev && iterations >= 0 &&
                  ticket,
              "fp_track_objects: bad argument");
   FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
   FP_TRY(check_slots(c, M, slots_host, "fp_track_objects"));
   DeviceGuard dg(c->device);
   const std::vector<int> camera_of(M, 0);
-  return track_cameras_submit(c, 1, &rgb_host, &depth_host, K, &H, &W, M, camera_of.data(), slots_host, poses_in_dev,
+  return track_cameras_submit(c, "fp_track_objects", 1, &rgb, &depth, K, &H, &W, M, camera_of.data(), slots_host, poses_in_dev,
                               iterations, poses_out_dev, reinterpret_cast<cudaStream_t>(stream), ticket);
   FP_API_END
 }
 
-int fp_track_objects(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W, int M,
+int fp_track_objects(fp_ctx* c, const unsigned char* rgb, const float* depth, const float* K, int H, int W, int M,
                      const int* slots_host, const float* poses_in_dev, int iterations, float* poses_out_dev,
                      float* poses_out_host, void* stream) {
   unsigned long long ticket = 0;
-  const int rc = fp_track_objects_submit(c, rgb_host, depth_host, K, H, W, M, slots_host, poses_in_dev, iterations,
+  const int rc = fp_track_objects_submit(c, rgb, depth, K, H, W, M, slots_host, poses_in_dev, iterations,
                                          poses_out_dev, stream, &ticket);
   return rc ? rc : fp_track_wait(c, ticket, poses_out_host);
 }
 
-int fp_track_cameras_submit(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
+int fp_track_cameras_submit(fp_ctx* c, int C, const unsigned char* const* rgb, const float* const* depth,
                             const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
                             const float* poses_in_dev, int iterations, float* poses_out_dev, void* stream,
                             unsigned long long* ticket) {
   FP_API_BEGIN
-  FP_REQUIRE(c && rgb_host && depth_host && K && H && W && M > 0 && camera_of && slots_host && poses_in_dev && iterations >= 0 &&
+  FP_REQUIRE(c && rgb && depth && K && H && W && M > 0 && camera_of && slots_host && poses_in_dev && iterations >= 0 &&
                  ticket,
              "fp_track_cameras: bad argument");
   FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
   // everything is checked before anything is enqueued: the kernels index the mesh and camera tables unchecked
-  FP_TRY(check_cameras(C, rgb_host, depth_host, H, W, M, camera_of, "fp_track_cameras"));
+  FP_TRY(check_cameras(C, rgb, depth, H, W, M, camera_of, "fp_track_cameras"));
   FP_TRY(check_slots(c, M, slots_host, "fp_track_cameras"));
   DeviceGuard dg(c->device);
-  return track_cameras_submit(c, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, poses_in_dev, iterations,
+  return track_cameras_submit(c, "fp_track_cameras", C, rgb, depth, K, H, W, M, camera_of, slots_host, poses_in_dev, iterations,
                               poses_out_dev, reinterpret_cast<cudaStream_t>(stream), ticket);
   FP_API_END
 }
 
-int fp_track_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host, const float* K,
+int fp_track_cameras(fp_ctx* c, int C, const unsigned char* const* rgb, const float* const* depth, const float* K,
                      const int* H, const int* W, int M, const int* camera_of, const int* slots_host, const float* poses_in_dev,
                      int iterations, float* poses_out_dev, float* poses_out_host, void* stream) {
   unsigned long long ticket = 0;
-  const int rc = fp_track_cameras_submit(c, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, poses_in_dev,
+  const int rc = fp_track_cameras_submit(c, C, rgb, depth, K, H, W, M, camera_of, slots_host, poses_in_dev,
                                          iterations, poses_out_dev, stream, &ticket);
   return rc ? rc : fp_track_wait(c, ticket, poses_out_host);
 }
 
-int fp_register_objects(fp_ctx* c, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
-                        int M, const int* slots_host, const int* n_hyp_host, const unsigned char* masks_host,
+int fp_register_objects(fp_ctx* c, const unsigned char* rgb, const float* depth, const float* K, int H, int W,
+                        int M, const int* slots_host, const int* n_hyp_host, const unsigned char* masks,
                         const float* rot_grids_dev, int iterations, float* poses_out_dev, float* scores_out_dev,
                         int* best_out_dev, float* info_out_dev, void* stream) {
   FP_API_BEGIN
-  FP_REQUIRE(c && rgb_host && depth_host && K && H > 0 && W > 0 && M > 0 && M <= 65535 && slots_host && n_hyp_host &&
-                 masks_host && rot_grids_dev && iterations >= 0 && poses_out_dev && scores_out_dev && best_out_dev &&
+  FP_REQUIRE(c && rgb && depth && K && H > 0 && W > 0 && M > 0 && M <= 65535 && slots_host && n_hyp_host &&
+                 masks && rot_grids_dev && iterations >= 0 && poses_out_dev && scores_out_dev && best_out_dev &&
                  info_out_dev,
              "fp_register_objects: bad argument");
   FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
@@ -1162,35 +1233,33 @@ int fp_register_objects(fp_ctx* c, const unsigned char* rgb_host, const float* d
   // everything is checked before anything is enqueued
   FP_TRY(check_slots(c, M, slots_host, "fp_register_objects"));
   DeviceGuard dg(c->device);
-  FP_TRY(order_after_track(c, reinterpret_cast<cudaStream_t>(stream)));
   const size_t npix = (size_t)H * W;
-  std::vector<const unsigned char*> masks(M);
-  for (int i = 0; i < M; ++i) masks[i] = masks_host + (size_t)i * npix;
+  std::vector<const unsigned char*> mask_of(M);
+  for (int i = 0; i < M; ++i) mask_of[i] = masks + (size_t)i * npix;
   const std::vector<int> camera_of(M, 0);
-  return register_cameras_body(c, 1, &rgb_host, &depth_host, K, &H, &W, M, camera_of.data(), slots_host, n_hyp_host,
-                               masks.data(), rot_grids_dev, iterations, poses_out_dev, scores_out_dev, best_out_dev,
+  return register_cameras_body(c, 1, &rgb, &depth, K, &H, &W, M, camera_of.data(), slots_host, n_hyp_host,
+                               mask_of.data(), rot_grids_dev, iterations, poses_out_dev, scores_out_dev, best_out_dev,
                                info_out_dev, reinterpret_cast<cudaStream_t>(stream), /*by_value=*/true);
   FP_API_END
 }
 
-int fp_register_cameras(fp_ctx* c, int C, const unsigned char* const* rgb_host, const float* const* depth_host, const float* K,
+int fp_register_cameras(fp_ctx* c, int C, const unsigned char* const* rgb, const float* const* depth, const float* K,
                         const int* H, const int* W, int M, const int* camera_of, const int* slots_host, const int* n_hyp_host,
-                        const unsigned char* const* masks_host, const float* rot_grids_dev, int iterations,
+                        const unsigned char* const* masks, const float* rot_grids_dev, int iterations,
                         float* poses_out_dev, float* scores_out_dev, int* best_out_dev, float* info_out_dev, void* stream) {
   FP_API_BEGIN
-  FP_REQUIRE(c && rgb_host && depth_host && K && H && W && M > 0 && M <= 65535 && camera_of && slots_host && n_hyp_host &&
-                 masks_host && rot_grids_dev && iterations >= 0 && poses_out_dev && scores_out_dev && best_out_dev &&
+  FP_REQUIRE(c && rgb && depth && K && H && W && M > 0 && M <= 65535 && camera_of && slots_host && n_hyp_host &&
+                 masks && rot_grids_dev && iterations >= 0 && poses_out_dev && scores_out_dev && best_out_dev &&
                  info_out_dev,
              "fp_register_cameras: bad argument");
   FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
   FP_REQUIRE(c->net[1].loaded, "scorer weights not loaded");
   // everything is checked before anything is enqueued: the kernels index the mesh and camera tables unchecked
-  FP_TRY(check_cameras(C, rgb_host, depth_host, H, W, M, camera_of, "fp_register_cameras"));
-  for (int i = 0; i < M; ++i) FP_REQUIRE(masks_host[i], "fp_register_cameras: object %d: null mask", i);
+  FP_TRY(check_cameras(C, rgb, depth, H, W, M, camera_of, "fp_register_cameras"));
+  for (int i = 0; i < M; ++i) FP_REQUIRE(masks[i], "fp_register_cameras: object %d: null mask", i);
   FP_TRY(check_slots(c, M, slots_host, "fp_register_cameras"));
   DeviceGuard dg(c->device);
-  FP_TRY(order_after_track(c, reinterpret_cast<cudaStream_t>(stream)));
-  return register_cameras_body(c, C, rgb_host, depth_host, K, H, W, M, camera_of, slots_host, n_hyp_host, masks_host,
+  return register_cameras_body(c, C, rgb, depth, K, H, W, M, camera_of, slots_host, n_hyp_host, masks,
                                rot_grids_dev, iterations, poses_out_dev, scores_out_dev, best_out_dev, info_out_dev,
                                reinterpret_cast<cudaStream_t>(stream), /*by_value=*/false);
   FP_API_END

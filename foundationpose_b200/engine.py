@@ -99,6 +99,64 @@ def _p(t):
     return None if t is None else C.c_void_p(t.data_ptr())
 
 
+def _on_device(x):
+    return torch.is_tensor(x) and x.is_cuda
+
+
+def _ptr(x):
+    """Address of a host array or a CUDA tensor."""
+    return C.c_void_p(x.data_ptr() if torch.is_tensor(x) else x.ctypes.data)
+
+
+def _frame(rgb, depth, what):
+    """One camera's frame as the tracking and register calls take it: (rgb, depth, (H, W)).  Each buffer is a host array
+    (made a contiguous uint8 / float32 numpy array, staged by the library) or a CUDA tensor on the engine's device, read
+    in place in stream order: rgb uint8 (H,W,3), depth (H,W) converted to float32, both made contiguous."""
+    if _on_device(depth):
+        if depth.dim() != 2:
+            raise ValueError(f"{what}: depth must be (H, W), got {tuple(depth.shape)}")
+        depth = depth.contiguous().float()
+    else:
+        depth = np.ascontiguousarray(depth, dtype=np.float32)
+    H, W = depth.shape
+    if _on_device(rgb):
+        if rgb.dtype != torch.uint8:
+            raise ValueError(f"{what}: a CUDA rgb frame must be uint8, got {rgb.dtype}")
+        if tuple(rgb.shape) != (H, W, 3):
+            raise ValueError(f"{what}: rgb must be ({H}, {W}, 3) to match depth, got {tuple(rgb.shape)}")
+        rgb = rgb.contiguous()
+    else:
+        rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
+    return rgb, depth, (int(H), int(W))
+
+
+def _device_mask(m):
+    """A CUDA mask (bool, uint8 or float) as the library reads it: contiguous uint8, 1 where `m > 0` (the reference's
+    test, estimater.py:138, :183), binarised on the device."""
+    return (m > 0).to(torch.uint8).contiguous()
+
+
+def _hold(bufs):
+    """The CUDA tensors among `bufs`, each recorded on the current stream: the library reads them in that stream's order,
+    so the caching allocator must not hand their memory to another stream before it has passed the call."""
+    held = [b for b in bufs if _on_device(b)]
+    st = torch.cuda.current_stream()
+    for b in held:
+        b.record_stream(st)
+    return held
+
+
+def _camera_args(frames):
+    """The (rgb pointers, depth pointers, K [C][9], H, W) arguments of the multi-camera calls for frames made by _frame."""
+    n_cam = len(frames)
+    rgbs = (C.c_void_p * n_cam)(*[_ptr(rgb).value for rgb, _, _ in frames])
+    depths = (C.c_void_p * n_cam)(*[_ptr(depth).value for _, depth, _ in frames])
+    Ks = (C.c_float * (9 * n_cam))(*[float(x) for _, _, K in frames for x in np.asarray(K, dtype=np.float64).reshape(-1)])
+    Hs = (C.c_int * n_cam)(*[int(depth.shape[0]) for _, depth, _ in frames])
+    Ws = (C.c_int * n_cam)(*[int(depth.shape[1]) for _, depth, _ in frames])
+    return rgbs, depths, Ks, Hs, Ws
+
+
 # ---------------------------------------------------------------------------------------------
 # checkpoint -> packed tensors
 # ---------------------------------------------------------------------------------------------
@@ -203,10 +261,11 @@ def _mesh_args(vertices, normals, faces, uv=None, tex=None, vertex_colors=None):
 class PendingPoses:
     """The host poses of one tracking call submitted with wait=False.  result() waits for the call's read-back (once; later
     calls return the same array) and returns what the blocking call returns as its host poses.  A handle dropped without
-    result() is collected by its engine at a later submit or at close, so its ticket never leaks."""
+    result() is collected by its engine at a later submit or at close, so its ticket never leaks.  It holds the call's
+    device frames until result() has collected the call."""
 
-    def __init__(self, engine, ticket, shape):
-        self._engine, self.ticket, self._shape, self._host = engine, ticket, shape, None
+    def __init__(self, engine, ticket, shape, held=()):
+        self._engine, self.ticket, self._shape, self._host, self._held = engine, ticket, shape, None, list(held)
         self._dropped = weakref.finalize(self, engine._dropped.append, ticket)
 
     def result(self):
@@ -215,6 +274,7 @@ class PendingPoses:
             host = np.empty(self._shape, dtype=np.float32)
             self._engine._wait(self.ticket, host)
             self._host = host
+            self._held = []
         return self._host
 
 
@@ -292,9 +352,9 @@ class Engine:
             self._dropped.remove(t)
             _lib.check(lib.fp_track_wait(self._h, t, None), "fp_track_wait")
 
-    def _submit(self, fn, args, what, out, shape, wait):
-        """Submits one tracking call (`fn(ctx, *args, stream, &ticket)`).  Returns (out, host poses) with wait, else (out,
-        PendingPoses)."""
+    def _submit(self, fn, args, what, out, shape, wait, bufs=()):
+        """Submits one tracking call (`fn(ctx, *args, stream, &ticket)`) on the frame buffers `bufs`.  Returns (out, host
+        poses) with wait, else (out, PendingPoses), which holds the device buffers among `bufs` until it is collected."""
         if not getattr(self, "_h", None):
             raise _lib.FposeError(f"{what}: the engine is closed")
         self._collect_dropped(MAX_IN_FLIGHT)
@@ -302,7 +362,7 @@ class Engine:
         _lib.check(fn(self._h, *args, _stream(), C.byref(ticket)), what)
         self._last_ticket = ticket.value
         if not wait:
-            return out, PendingPoses(self, ticket.value, shape)
+            return out, PendingPoses(self, ticket.value, shape, _hold(bufs))
         host = np.empty(shape, dtype=np.float32)
         self._wait(ticket.value, host)
         return out, host
@@ -314,29 +374,27 @@ class Engine:
 
     def track(self, rgb, depth, K, pose_in, iterations, pose_out=None, wait=True):
         """fp_track: one CUDA-graph launch per frame (upload + depth filters + xyz map + refiner passes + read-back).
-        rgb uint8 (H,W,3) / depth float32 (H,W) HOST arrays; pose_in (4,4) CUDA tensor or None (continue).
+        rgb uint8 (H,W,3) / depth float32 (H,W): host arrays, or CUDA tensors on the engine's device, read in place in the
+        current stream's order (see _frame); pose_in (4,4) CUDA tensor or None (continue).
         Returns (pose_out CUDA (4,4), pose host (4,4) float32 numpy).  wait=False returns as soon as the call is
         submitted (the host arrays may then be reused): (pose_out, PendingPoses), pose_out complete in stream order."""
-        rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
-        depth = np.ascontiguousarray(depth, dtype=np.float32)
-        H, W = depth.shape
+        rgb, depth, (H, W) = _frame(rgb, depth, "track")
         Kf = (C.c_float * 9)(*[float(x) for x in np.asarray(K, dtype=np.float64).reshape(-1)])
         if pose_in is not None:
             pose_in = pose_in.reshape(4, 4).contiguous().float()
         if pose_out is None:
             pose_out = torch.empty(4, 4, dtype=torch.float32, device="cuda")
-        out = self._submit(lib.fp_track_submit, (C.c_void_p(rgb.ctypes.data), C.c_void_p(depth.ctypes.data), Kf, H, W,
-                                                 _p(pose_in), int(iterations), _p(pose_out)), "fp_track", pose_out, (4, 4), wait)
+        out = self._submit(lib.fp_track_submit, (_ptr(rgb), _ptr(depth), Kf, H, W, _p(pose_in), int(iterations), _p(pose_out)),
+                           "fp_track", pose_out, (4, 4), wait, (rgb, depth))
         self.frame_hw = (H, W)
         return out
 
     def track_objects(self, rgb, depth, K, poses_in, slots, iterations, wait=True):
         """fp_track_objects: `track` for M objects of one frame in ONE CUDA-graph launch, object i rendering the mesh in
-        slot slots[i] (loaded by set_mesh(..., slot=)).  rgb uint8 (H,W,3) / depth float32 (H,W) HOST arrays; poses_in
-        (M,4,4) CUDA tensor.  Returns (poses CUDA (M,4,4), poses host (M,4,4) float32 numpy); wait=False as `track`."""
-        rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
-        depth = np.ascontiguousarray(depth, dtype=np.float32)
-        H, W = depth.shape
+        slot slots[i] (loaded by set_mesh(..., slot=)).  rgb uint8 (H,W,3) / depth float32 (H,W): host arrays or CUDA
+        tensors, as `track`; poses_in (M,4,4) CUDA tensor.  Returns (poses CUDA (M,4,4), poses host (M,4,4) float32
+        numpy); wait=False as `track`."""
+        rgb, depth, (H, W) = _frame(rgb, depth, "track_objects")
         Kf = (C.c_float * 9)(*[float(x) for x in np.asarray(K, dtype=np.float64).reshape(-1)])
         poses_in = poses_in.reshape(-1, 4, 4).contiguous().float()
         M = len(poses_in)
@@ -344,50 +402,51 @@ class Engine:
         if len(slots) != M:
             raise ValueError(f"track_objects: {M} poses but {len(slots)} slots")
         out = torch.empty(M, 4, 4, dtype=torch.float32, device="cuda")
-        res = self._submit(lib.fp_track_objects_submit, (C.c_void_p(rgb.ctypes.data), C.c_void_p(depth.ctypes.data), Kf, H, W, M,
-                                                         (C.c_int * M)(*slots), _p(poses_in), int(iterations), _p(out)),
-                           "fp_track_objects", out, (M, 4, 4), wait)
+        res = self._submit(lib.fp_track_objects_submit, (_ptr(rgb), _ptr(depth), Kf, H, W, M, (C.c_int * M)(*slots), _p(poses_in),
+                                                         int(iterations), _p(out)),
+                           "fp_track_objects", out, (M, 4, 4), wait, (rgb, depth))
         self.frame_hw = (H, W)
         return res
 
     def track_cameras(self, frames, poses_in, camera_of, slots, iterations, wait=True):
         """fp_track_cameras: `track_objects` for M objects spread over C camera streams in ONE CUDA-graph launch.  frames: C
-        tuples (rgb uint8 (H,W,3), depth float32 (H,W), K (3,3)) of HOST arrays, one per camera, each with its own size and
-        intrinsics; object i is seen by camera camera_of[i] and renders the mesh in slot slots[i]; poses_in (M,4,4) CUDA
-        tensor.  Returns (poses CUDA (M,4,4), poses host (M,4,4) float32 numpy); wait=False as `track`."""
-        frames = [(np.ascontiguousarray(rgb, dtype=np.uint8), np.ascontiguousarray(depth, dtype=np.float32), K) for rgb, depth, K in frames]
+        tuples (rgb uint8 (H,W,3), depth float32 (H,W), K (3,3)), one per camera, each with its own size and intrinsics and
+        each buffer a host array or a CUDA tensor, as `track` (one call may mix them); object i is seen by camera
+        camera_of[i] and renders the mesh in slot slots[i]; poses_in (M,4,4) CUDA tensor.  Returns (poses CUDA (M,4,4),
+        poses host (M,4,4) float32 numpy); wait=False as `track`."""
+        frames = [(*_frame(rgb, depth, f"track_cameras: camera {c}")[:2], K) for c, (rgb, depth, K) in enumerate(frames)]
         n_cam = len(frames)
         poses_in = poses_in.reshape(-1, 4, 4).contiguous().float()
         M = len(poses_in)
         camera_of, slots = [int(c) for c in camera_of], [int(s) for s in slots]
         if len(camera_of) != M or len(slots) != M:
             raise ValueError(f"track_cameras: {M} poses, {len(camera_of)} camera ids and {len(slots)} slots")
-        rgbs = (C.c_void_p * n_cam)(*[rgb.ctypes.data for rgb, _, _ in frames])
-        depths = (C.c_void_p * n_cam)(*[depth.ctypes.data for _, depth, _ in frames])
-        Ks = (C.c_float * (9 * n_cam))(*[float(x) for _, _, K in frames for x in np.asarray(K, dtype=np.float64).reshape(-1)])
-        Hs = (C.c_int * n_cam)(*[depth.shape[0] for _, depth, _ in frames])
-        Ws = (C.c_int * n_cam)(*[depth.shape[1] for _, depth, _ in frames])
+        rgbs, depths, Ks, Hs, Ws = _camera_args(frames)
         out = torch.empty(M, 4, 4, dtype=torch.float32, device="cuda")
         res = self._submit(lib.fp_track_cameras_submit, (n_cam, rgbs, depths, Ks, Hs, Ws, M, (C.c_int * M)(*camera_of),
                                                          (C.c_int * M)(*slots), _p(poses_in), int(iterations), _p(out)),
-                           "fp_track_cameras", out, (M, 4, 4), wait)
-        self.frame_hw = frames[0][1].shape  # camera 0's frame is the context's frame
+                           "fp_track_cameras", out, (M, 4, 4), wait, [b for rgb, depth, _ in frames for b in (rgb, depth)])
+        self.frame_hw = tuple(frames[0][1].shape)  # camera 0's frame is the context's frame
         return res
 
     def register_objects(self, rgb, depth, K, masks, rot_grids, slots, iterations):
         """fp_register_objects: the register() hot path for M objects of one frame in one call, object i rendering the mesh
-        in slot slots[i].  rgb uint8 (H,W,3) / depth float32 (H,W) / masks (M,H,W) (nonzero = object) HOST arrays;
-        rot_grids: M CUDA float32 (N_i,4,4) rotation grids.  Returns CUDA tensors: poses (sum N_i,4,4) refined, object-major
-        and unranked; scores (sum N_i,); best (M,) int32, each object's first arg-max relative to its own rows; info (M,4)
-        = (tx, ty, tz, n_valid) per object."""
-        rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
-        depth = np.ascontiguousarray(depth, dtype=np.float32)
-        H, W = depth.shape
-        masks = np.ascontiguousarray(masks)
+        in slot slots[i].  rgb uint8 (H,W,3) / depth float32 (H,W): host arrays or CUDA tensors, as `track`; masks
+        (M,H,W) (nonzero = object): a host array, or a CUDA bool / uint8 / float tensor (or a sequence of M CUDA (H,W)
+        masks) binarised on the device; rot_grids: M CUDA float32 (N_i,4,4) rotation grids.  Returns CUDA tensors: poses
+        (sum N_i,4,4) refined, object-major and unranked; scores (sum N_i,); best (M,) int32, each object's first arg-max
+        relative to its own rows; info (M,4) = (tx, ty, tz, n_valid) per object."""
+        rgb, depth, (H, W) = _frame(rgb, depth, "register_objects")
+        if not _on_device(masks) and len(masks) and all(_on_device(m) for m in masks):
+            masks = torch.stack(list(masks))
+        masks = masks if _on_device(masks) else np.ascontiguousarray(masks)
         M = len(masks)
-        if masks.shape != (M, H, W):
-            raise ValueError(f"register_objects: masks must be (M, {H}, {W}), got {masks.shape}")
-        masks = np.ascontiguousarray(masks > 0, dtype=np.uint8)  # the reference tests `mask > 0` (estimater.py:138, :183)
+        if tuple(masks.shape) != (M, H, W):
+            raise ValueError(f"register_objects: masks must be (M, {H}, {W}), got {tuple(masks.shape)}")
+        if _on_device(masks):
+            masks = _device_mask(masks)
+        else:
+            masks = np.ascontiguousarray(masks > 0, dtype=np.uint8)  # the reference tests `mask > 0` (estimater.py:138, :183)
         slots = [int(s) for s in slots]
         rot_grids = [g.reshape(-1, 4, 4) for g in rot_grids]
         if len(slots) != M or len(rot_grids) != M:
@@ -400,20 +459,21 @@ class Engine:
         scores = torch.empty(total, dtype=torch.float32, device="cuda")
         best = torch.empty(M, dtype=torch.int32, device="cuda")
         info = torch.empty(M, 4, dtype=torch.float32, device="cuda")
-        _lib.check(lib.fp_register_objects(self._h, C.c_void_p(rgb.ctypes.data), C.c_void_p(depth.ctypes.data), Kf, H, W, M,
-                                           (C.c_int * M)(*slots), (C.c_int * M)(*n_hyp), C.c_void_p(masks.ctypes.data), _p(grids),
-                                           int(iterations), _p(poses), _p(scores), _p(best), _p(info), _stream()),
-                   "fp_register_objects")
+        _lib.check(lib.fp_register_objects(self._h, _ptr(rgb), _ptr(depth), Kf, H, W, M, (C.c_int * M)(*slots), (C.c_int * M)(*n_hyp),
+                                           _ptr(masks), _p(grids), int(iterations), _p(poses), _p(scores), _p(best), _p(info),
+                                           _stream()),
+                   "fp_register_objects")  # synchronises its stream: the device inputs are free again on return
         self.frame_hw = (H, W)
         return poses, scores, best, info
 
     def register_cameras(self, frames, masks, rot_grids, camera_of, slots, iterations):
         """fp_register_cameras: `register_objects` for M objects spread over C camera streams in one call.  frames: C tuples
-        (rgb uint8 (H,W,3), depth float32 (H,W), K (3,3)) of HOST arrays, one per camera, each with its own size and
-        intrinsics; object i is seen by camera camera_of[i], renders the mesh in slot slots[i] and has the HOST mask
-        masks[i] (nonzero = object) of its camera's frame size; rot_grids: M CUDA float32 (N_i,4,4) rotation grids.
+        (rgb uint8 (H,W,3), depth float32 (H,W), K (3,3)), one per camera, each with its own size and intrinsics and each
+        buffer a host array or a CUDA tensor, as `track`; object i is seen by camera camera_of[i], renders the mesh in slot
+        slots[i] and has the mask masks[i] (nonzero = object) of its camera's frame size, a host array or a CUDA bool /
+        uint8 / float tensor binarised on the device; rot_grids: M CUDA float32 (N_i,4,4) rotation grids.
         Returns the CUDA tensors of register_objects: poses (sum N_i,4,4), scores (sum N_i,), best (M,), info (M,4)."""
-        frames = [(np.ascontiguousarray(rgb, dtype=np.uint8), np.ascontiguousarray(depth, dtype=np.float32), K) for rgb, depth, K in frames]
+        frames = [(*_frame(rgb, depth, f"register_cameras: camera {c}")[:2], K) for c, (rgb, depth, K) in enumerate(frames)]
         n_cam = len(frames)
         M = len(masks)
         camera_of, slots = [int(c) for c in camera_of], [int(s) for s in slots]
@@ -421,28 +481,26 @@ class Engine:
         if len(camera_of) != M or len(slots) != M or len(rot_grids) != M:
             raise ValueError(f"register_cameras: {M} masks, {len(camera_of)} camera ids, {len(slots)} slots and "
                              f"{len(rot_grids)} rotation grids")
-        masks = [np.asarray(m) for m in masks]
+        masks = [m if _on_device(m) else np.asarray(m) for m in masks]
         for i, (m, c) in enumerate(zip(masks, camera_of)):
-            if 0 <= c < n_cam and m.shape != frames[c][1].shape:
-                raise ValueError(f"register_cameras: mask {i} has shape {m.shape}, camera {c}'s frame is {frames[c][1].shape}")
-        masks = [np.ascontiguousarray(m > 0, dtype=np.uint8) for m in masks]  # the reference tests `mask > 0` (estimater.py:138, :183)
+            if 0 <= c < n_cam and tuple(m.shape) != tuple(frames[c][1].shape):
+                raise ValueError(f"register_cameras: mask {i} has shape {tuple(m.shape)}, camera {c}'s frame is "
+                                 f"{tuple(frames[c][1].shape)}")
+        # the reference tests `mask > 0` (estimater.py:138, :183)
+        masks = [_device_mask(m) if _on_device(m) else np.ascontiguousarray(m > 0, dtype=np.uint8) for m in masks]
         n_hyp = [len(g) for g in rot_grids]
         grids = torch.cat(rot_grids).to(device="cuda", dtype=torch.float32).contiguous()
         total = len(grids)
-        rgbs = (C.c_void_p * n_cam)(*[rgb.ctypes.data for rgb, _, _ in frames])
-        depths = (C.c_void_p * n_cam)(*[depth.ctypes.data for _, depth, _ in frames])
-        Ks = (C.c_float * (9 * n_cam))(*[float(x) for _, _, K in frames for x in np.asarray(K, dtype=np.float64).reshape(-1)])
-        Hs = (C.c_int * n_cam)(*[depth.shape[0] for _, depth, _ in frames])
-        Ws = (C.c_int * n_cam)(*[depth.shape[1] for _, depth, _ in frames])
+        rgbs, depths, Ks, Hs, Ws = _camera_args(frames)
         poses = torch.empty(total, 4, 4, dtype=torch.float32, device="cuda")
         scores = torch.empty(total, dtype=torch.float32, device="cuda")
         best = torch.empty(M, dtype=torch.int32, device="cuda")
         info = torch.empty(M, 4, dtype=torch.float32, device="cuda")
         _lib.check(lib.fp_register_cameras(self._h, n_cam, rgbs, depths, Ks, Hs, Ws, M, (C.c_int * M)(*camera_of),
-                                           (C.c_int * M)(*slots), (C.c_int * M)(*n_hyp), (C.c_void_p * M)(*[m.ctypes.data for m in masks]),
+                                           (C.c_int * M)(*slots), (C.c_int * M)(*n_hyp), (C.c_void_p * M)(*[_ptr(m).value for m in masks]),
                                            _p(grids), int(iterations), _p(poses), _p(scores), _p(best), _p(info), _stream()),
-                   "fp_register_cameras")
-        self.frame_hw = frames[0][1].shape  # camera 0's frame is the context's frame
+                   "fp_register_cameras")  # synchronises its stream: the device inputs are free again on return
+        self.frame_hw = tuple(frames[0][1].shape)  # camera 0's frame is the context's frame
         return poses, scores, best, info
 
     def set_frame(self, rgb, depth, K, filter_depth=True, zfar=float("inf")):

@@ -217,7 +217,17 @@ int fp_mesh_info(fp_ctx* ctx, int* info);
 /* Host inputs of fp_set_frame, fp_start_poses and fp_register.  Pageable host memory is copied into the context's
  * pinned staging before the call returns: the caller may reuse it at once, and the call does not wait on `stream` for
  * it.  Page-locked memory (cudaHostAlloc, cudaHostRegister) is copied straight from the caller's buffer on `stream`:
- * the caller keeps it unchanged until `stream` has passed the call. */
+ * the caller keeps it unchanged until `stream` has passed the call.
+ * Frames and masks of the tracking calls (fp_track, fp_track_objects, fp_track_cameras and their _submit variants),
+ * fp_register_objects and fp_register_cameras: each buffer (each camera's rgb, each camera's depth, each mask;
+ * fp_register_objects' mask block as one buffer) may be host or device memory, classified on its own with
+ * cudaPointerGetAttributes, and one call may mix them.  Host memory, pageable, page-locked or managed, is copied into the
+ * context's pinned staging before the call returns: the caller may reuse it at once.  Device memory of the context's
+ * device is read in place: nothing is staged or uploaded for it (a device mask is copied into the context on the
+ * device), and the kernels read it in stream order on `stream`.  The caller keeps it allocated and unchanged until
+ * `stream` has passed the call; for a submit, until its ticket's work is done, so a producer that writes the next frame
+ * into the same buffer on the same stream after the submit is safe.  Device memory of another device is refused before
+ * anything is enqueued. */
 #define FP_FRAME_ON_DEVICE 1    /* rgb/depth are device pointers (default: host, copied on `stream`) */
 #define FP_FRAME_FILTER_DEPTH 2 /* erode_depth + bilateral_filter_depth (estimater.py:173-174, :257-258) */
 /* Uploads one RGB-D frame (rgb uint8 [H][W][3], depth float32 [H][W] metres, K row-major 3x3), runs
@@ -282,8 +292,9 @@ int fp_op_score_tail_segments(fp_ctx* ctx, const float* feats, int L, const int*
 int fp_register(fp_ctx* ctx, const float* poses_host, int N, int iterations, float* poses_out_host,
                 float* scores_out_host, int* best_out_host, void* stream);
 
-/* FoundationPose.track_one (estimater.py:250-268) as ONE CUDA-graph launch per frame: upload of the frame (HOST rgb
- * uint8 [H][W][3], depth float32 [H][W]; staged through pinned memory owned by the context), erode_depth +
+/* FoundationPose.track_one (estimater.py:250-268) as ONE CUDA-graph launch per frame: the frame (rgb uint8 [H][W][3],
+ * depth float32 [H][W], host or device: a host frame is staged through pinned memory owned by the context and uploaded,
+ * a device frame is read in place, see above), erode_depth +
  * bilateral_filter_depth, depth2xyzmap_batch(zfar = inf), `iterations` refiner passes on ONE pose, pose read-back.
  * pose_in_dev: DEVICE [16] ob_in_cam of the centred mesh (pose_last), or NULL = continue from the pose this context's
  * previous fp_track produced.  pose_out_dev (DEVICE [16]) / pose_out_host (HOST [16]) are optional.  This is the
@@ -292,10 +303,10 @@ int fp_register(fp_ctx* ctx, const float* poses_host, int N, int iterations, flo
  * larger than one tracked before replay it.  The first tracking call, or one with a larger frame than any tracked
  * before, captures every cached graph of the context once more (the tracking calls' frame-preparation grid grows).
  * Synchronises. */
-int fp_track(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
+int fp_track(fp_ctx* ctx, const unsigned char* rgb, const float* depth, const float* K, int H, int W,
              const float* pose_in_dev, int iterations, float* pose_out_dev, float* pose_out_host, void* stream);
 /* FoundationPose.track_one (estimater.py:250-268) applied to M objects of the same frame, as ONE CUDA-graph launch:
- * one pinned-staged upload of the frame, one erode_depth + bilateral_filter_depth + depth2xyzmap_batch(zfar = inf),
+ * the frame (host or device, as fp_track), one erode_depth + bilateral_filter_depth + depth2xyzmap_batch(zfar = inf),
  * `iterations` refiner passes over a batch of M hypotheses where hypothesis i renders the mesh in slot slots_host[i],
  * read-back of the M poses.  slots_host: HOST [M] slot ids, each loaded (checked before anything is enqueued);
  * poses_in_dev: DEVICE [M][16] ob_in_cam of each centred mesh; poses_out_dev (DEVICE [M][16]) / poses_out_host
@@ -303,26 +314,28 @@ int fp_track(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host
  * (FP_FRAME_FILTER_DEPTH, zfar = inf) + fp_refine give for it with its mesh in slot 0.  This is fp_track_cameras
  * with one camera (C = 1, every object seen by camera 0), and shares its cached graph: new intrinsics or a frame no
  * larger than one seen before replay it.  Leaves fp_track's continuation pose untouched.  Synchronises. */
-int fp_track_objects(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
+int fp_track_objects(fp_ctx* ctx, const unsigned char* rgb, const float* depth, const float* K, int H, int W,
                      int M, const int* slots_host, const float* poses_in_dev, int iterations, float* poses_out_dev,
                      float* poses_out_host, void* stream);
 /* fp_track_objects for M objects spread over C camera streams (1 <= C <= FP_MAX_CAMERAS), each camera with its own
  * frame size and intrinsics, as ONE CUDA-graph launch: object i is seen by camera camera_of[i] and tracked exactly as
  * fp_track_objects tracks it in that camera's frame alone, bit for bit; fp_track_objects is its one-camera case.
- *   rgb_host[c] / depth_host[c]: HOST uint8 [H[c]][W[c]][3] / float32 [H[c]][W[c]] frame of camera c, each uploaded
- *   through its own pinned staging; K: [C][9] row-major intrinsics; camera_of, slots_host: HOST [M] camera and mesh
+ *   rgb[c] / depth[c]: host or device uint8 [H[c]][W[c]][3] / float32 [H[c]][W[c]] frame of camera c, each host buffer
+ *   uploaded through its camera's pinned staging, each device buffer read in place through the camera table (see above);
+ *   K: [C][9] row-major intrinsics; camera_of, slots_host: HOST [M] camera and mesh
  *   slot of every object; poses_in_dev: DEVICE [M][16]; poses_out_dev (DEVICE [M][16]) / poses_out_host (HOST [M][16])
  *   are optional.
  * Everything is checked before anything is enqueued: every camera id in [0, C), every camera owning at least one
  * object, every slot loaded, non-null frames of positive size.  One frame-preparation launch filters every camera's
  * depth, then `iterations` refiner passes run over all M objects.  The camera table (buffers, sizes, intrinsics), the
  * slot ids and the camera ids are copied into the context first, so the cached graph depends on (C, M, iterations)
- * only: reordering objects or cameras, changing intrinsics or a frame no larger than one seen before replays it.
+ * only: reordering objects or cameras, changing intrinsics, a frame no larger than one seen before, or frames at other
+ * addresses, on the host or on the device, replay it.
  * Camera 0 is the context's frame: afterwards the context holds camera 0's filtered frame, as fp_track on that frame
  * leaves it.  Cameras 1.. get buffers of their own, kept at the largest frame size seen.  Leaves fp_track's
  * continuation pose untouched.  Synchronises. */
 #define FP_MAX_CAMERAS 16
-int fp_track_cameras(fp_ctx* ctx, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
+int fp_track_cameras(fp_ctx* ctx, int C, const unsigned char* const* rgb, const float* const* depth,
                      const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
                      const float* poses_in_dev, int iterations, float* poses_out_dev, float* poses_out_host, void* stream);
 
@@ -332,8 +345,9 @@ int fp_track_cameras(fp_ctx* ctx, int C, const unsigned char* const* rgb_host, c
  *   fp_track_objects / fp_track except poses_out_host / pose_out_host, and check them the same way: a refused call
  *   enqueues nothing.  Each copies the host frames into pinned staging on the calling thread and enqueues the uploads,
  *   the graph launch and the pose read-back on `stream`, then writes the call's ticket to *ticket.  Once it returns the
- *   caller may reuse its host frame buffers; poses_out_dev (and fp_track's continuation pose) are complete in stream
- *   order, so the next call may read them as its poses_in_dev without any host synchronisation.
+ *   caller may reuse its host frame buffers (device frames: once the ticket's work is done); poses_out_dev (and
+ *   fp_track's continuation pose) are complete in stream order, so the next call may read them as its poses_in_dev
+ *   without any host synchronisation.
  *   The context has FP_TRACK_MAX_IN_FLIGHT staging sets, used in turn.  A submit that finds its set still in use
  *   blocks only until the uploads of the call that used it have left it, not until that call's result is ready.
  *   A submit on a stream other than the previous submit's makes its stream wait for the previous call first: the
@@ -345,14 +359,14 @@ int fp_track_cameras(fp_ctx* ctx, int C, const unsigned char* const* rgb_host, c
  * submitted call, on the device: it does not wait on the host.  A staging set is waited for only by the call that
  * takes it again.  Results stay pending until collected.  fp_destroy waits for calls in flight and frees uncollected results. */
 #define FP_TRACK_MAX_IN_FLIGHT 2
-int fp_track_cameras_submit(fp_ctx* ctx, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
+int fp_track_cameras_submit(fp_ctx* ctx, int C, const unsigned char* const* rgb, const float* const* depth,
                             const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
                             const float* poses_in_dev, int iterations, float* poses_out_dev, void* stream,
                             unsigned long long* ticket);
-int fp_track_objects_submit(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host, const float* K, int H,
+int fp_track_objects_submit(fp_ctx* ctx, const unsigned char* rgb, const float* depth, const float* K, int H,
                             int W, int M, const int* slots_host, const float* poses_in_dev, int iterations,
                             float* poses_out_dev, void* stream, unsigned long long* ticket);
-int fp_track_submit(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
+int fp_track_submit(fp_ctx* ctx, const unsigned char* rgb, const float* depth, const float* K, int H, int W,
                     const float* pose_in_dev, int iterations, float* pose_out_dev, void* stream, unsigned long long* ticket);
 int fp_track_wait(fp_ctx* ctx, unsigned long long ticket, float* poses_out_host);
 /* FoundationPose.register (estimater.py:159-240) applied to M objects of the same frame in one call; object i gives
@@ -360,8 +374,9 @@ int fp_track_wait(fp_ctx* ctx, unsigned long long ticket, float* poses_out_host)
  *   1. Checks every argument before anything is enqueued: slots_host HOST [M] loaded slot ids (one slot may appear
  *      more than once: two instances of one object), n_hyp_host HOST [M] hypotheses per object (1..4096), both
  *      networks loaded.
- *   2. One pinned-staged upload of the frame (HOST rgb uint8 [H][W][3], depth float32 [H][W]) and of masks_host
- *      (HOST uint8 [M][H][W], nonzero = object), one erode_depth + bilateral_filter_depth + depth2xyzmap(zfar = inf).
+ *   2. The frame (rgb uint8 [H][W][3], depth float32 [H][W]) and masks (uint8 [M][H][W], nonzero = object), each host
+ *      or device as the tracking calls' frames (host buffers pinned-staged and uploaded, device ones read in place, the
+ *      masks by one device copy), one erode_depth + bilateral_filter_depth + depth2xyzmap(zfar = inf).
  *   3. guess_translation + start poses of every object in one launch pair: rot_grids_dev DEVICE [sum N][16], object i's
  *      n_hyp_host[i] rotations after object i - 1's.
  *   4. Refines (`iterations` passes) and featurises whole objects in passes of at most 512 hypotheses (an object above
@@ -372,29 +387,31 @@ int fp_track_wait(fp_ctx* ctx, unsigned long long ticket, float* poses_out_host)
  * object; info_out_dev [M][4] = {tx, ty, tz, n_valid} as fp_start_poses.  An object with fewer than 4 valid masked
  * pixels still runs; the caller discards its results (estimater.py:183-189).  The frame filter, the start poses and
  * the crops take the frame by value, as fp_register does, so the cached graphs are captured again when the frame's
- * size or intrinsics change.  Synchronises. */
-int fp_register_objects(fp_ctx* ctx, const unsigned char* rgb_host, const float* depth_host, const float* K, int H, int W,
-                        int M, const int* slots_host, const int* n_hyp_host, const unsigned char* masks_host,
+ * size or intrinsics change (not when it moves between host and device: the graphs hold the context's filtered frame,
+ * prepared outside them).  Synchronises. */
+int fp_register_objects(fp_ctx* ctx, const unsigned char* rgb, const float* depth, const float* K, int H, int W,
+                        int M, const int* slots_host, const int* n_hyp_host, const unsigned char* masks,
                         const float* rot_grids_dev, int iterations, float* poses_out_dev, float* scores_out_dev,
                         int* best_out_dev, float* info_out_dev, void* stream);
 /* fp_register_objects for M objects spread over C camera streams (1 <= C <= FP_MAX_CAMERAS), each camera with its own
  * frame size and intrinsics: object i is seen by camera camera_of[i] and gives exactly what fp_register_objects gives
  * for it with that camera's frame alone, bit for bit.
- *   rgb_host[c] / depth_host[c]: HOST uint8 [H[c]][W[c]][3] / float32 [H[c]][W[c]] frame of camera c, each uploaded
- *   through its own pinned staging; K: [C][9] row-major intrinsics; camera_of, slots_host, n_hyp_host: HOST [M] camera,
- *   mesh slot and hypothesis count (1..4096) of every object; masks_host[i]: HOST uint8 [H[camera_of[i]]][W[...]]
- *   (nonzero = object); rot_grids_dev as fp_register_objects.
+ *   rgb[c] / depth[c]: host or device uint8 [H[c]][W[c]][3] / float32 [H[c]][W[c]] frame of camera c, as
+ *   fp_track_cameras; K: [C][9] row-major intrinsics; camera_of, slots_host, n_hyp_host: HOST [M] camera, mesh slot and
+ *   hypothesis count (1..4096) of every object; masks[i]: host or device uint8 [H[camera_of[i]]][W[...]] (nonzero =
+ *   object); rot_grids_dev as fp_register_objects.
  * Everything is checked before anything is enqueued: every camera id in [0, C), every camera owning at least one
- * object, non-null frames of positive size and non-null masks, every slot loaded, both networks loaded.  All masks go
- * to the device in one copy; one frame-preparation launch filters every camera's depth and one launch pair computes
+ * object, non-null frames of positive size and non-null masks, every slot loaded, both networks loaded.  The host masks
+ * go to the device in one copy per run of consecutive host masks (one copy when all are on the host), the device masks
+ * by device copies; one frame-preparation launch filters every camera's depth and one launch pair computes
  * every object's start poses, each from its own camera's filtered depth and intrinsics.  Passes and the scorer tail as
  * fp_register_objects; a pass may mix cameras.  The camera table and each pass's slot and camera ids are copied into
  * the context first, so the cached graphs depend on the pass sizes and iterations only: reordering objects or cameras
  * or changing intrinsics replays them.  Camera 0 is the context's frame, as after fp_track_cameras.  Outputs: exactly
  * fp_register_objects' (object-major, unranked, best relative to the object, info [M][4]).  Synchronises. */
-int fp_register_cameras(fp_ctx* ctx, int C, const unsigned char* const* rgb_host, const float* const* depth_host,
+int fp_register_cameras(fp_ctx* ctx, int C, const unsigned char* const* rgb, const float* const* depth,
                         const float* K, const int* H, const int* W, int M, const int* camera_of, const int* slots_host,
-                        const int* n_hyp_host, const unsigned char* const* masks_host, const float* rot_grids_dev,
+                        const int* n_hyp_host, const unsigned char* const* masks, const float* rot_grids_dev,
                         int iterations, float* poses_out_dev, float* scores_out_dev, int* best_out_dev, float* info_out_dev,
                         void* stream);
 /* Number of CUDA graphs this context has captured so far (test hook: a replay captures nothing). */
