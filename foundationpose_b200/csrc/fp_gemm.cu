@@ -126,6 +126,10 @@ struct GemmParams {
   int lg_bw, lg_bh;  // tile rows m -> (nn, ii, jj): jj = m & (bw-1), ii = (m >> lg_bw) & (bh-1)
   int bw, bh, bn;
   int tiles_w, tiles_h, tiles_n, n_tiles_n, total_tiles;
+  // Packing of the last, partial image group (conv3, non-swapped tiles): tiles_n counts the full groups only, and
+  // every m-tile after them holds up to `pack` spatial blocks of the last group's n_img % bn images, block q at tile
+  // rows [q pack_rows, (q + 1) pack_rows).  pack = 0: no packing, the last group is one zero-filled box per block.
+  int pack, pack_rows;
   int num_kb, chunks_per_tap;
   int dim_w, dim_h, dim_n;
   short tap_off[9][5];
@@ -185,11 +189,16 @@ struct TileCfg {
 // 128B-swizzled slabs -> one TMA tensor store per 64-channel slab).  The producer runs ahead into the next tile while
 // the consumers drain this one.  The 256-wide tile moves registers from the producer warpgroup to the consumers
 // (128 accumulators per thread do not fit the 168 a 384-thread CTA gets), and so does the swapped tile.
+//
+// Packed tiles (p.pack > 0) read, store and take the residual of each spatial block as its own box of the last
+// group's images (the *_pk maps, whose image box is n_img % bn), at the block's rows of the A slot and of every
+// slab; tile rows that no block fills are computed but never stored.
 template <int BN, bool kSwap = false>
 __global__ void __launch_bounds__(kTileThreads, 1)
     gemm_tile_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                      const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res,
-                     const __grid_constant__ GemmParams p) {
+                     const __grid_constant__ CUtensorMap map_a_pk, const __grid_constant__ CUtensorMap map_out_pk,
+                     const __grid_constant__ CUtensorMap map_res_pk, const __grid_constant__ GemmParams p) {
   using Cfg = TileCfg<BN, kSwap>;
   constexpr int S = Cfg::kStages;
   constexpr int NSLAB = Cfg::kSlabs;
@@ -204,14 +213,19 @@ __global__ void __launch_bounds__(kTileThreads, 1)
   uint64_t* empty = bars + S;     // [S]
   uint64_t* res_full = bars + 2 * S;  // [NSLAB] with kAlt (one per slab), else [1] (all slabs)
 
-  const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
-  const int total = m_tiles * p.n_tiles_n;
+  const int full_m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
+  const int total = p.total_tiles;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
     tma_prefetch_desc(&map_out);
     if (p.has_res) tma_prefetch_desc(&map_res);
+    if (p.pack) {
+      tma_prefetch_desc(&map_a_pk);
+      tma_prefetch_desc(&map_out_pk);
+      if (p.has_res) tma_prefetch_desc(&map_res_pk);
+    }
     for (int s = 0; s < S; ++s) {
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], 256);
@@ -223,9 +237,20 @@ __global__ void __launch_bounds__(kTileThreads, 1)
   pdl_trigger();
   pdl_wait();  // everything above overlapped the previous kernel's tail; activations are touched only from here on
 
-  auto decode = [&](int t, int& n_tile, int& tw, int& th, int& tn) {
+  // nsub = 0: a full tile at block (tw, th) of image group tn.  Otherwise a packed tile (m-tiles past the full
+  // groups): nsub blocks of the last group tn, from (tw, th) on in row-major block order.
+  auto decode = [&](int t, int& n_tile, int& tw, int& th, int& tn, int& nsub) {
     n_tile = t % p.n_tiles_n;
     const int m_tile = t / p.n_tiles_n;
+    if (!kSwap && m_tile >= full_m_tiles) {
+      const int blk = (m_tile - full_m_tiles) * p.pack;
+      nsub = min(p.pack, p.tiles_w * p.tiles_h - blk);
+      tw = blk % p.tiles_w;
+      th = blk / p.tiles_w;
+      tn = p.tiles_n;
+      return;
+    }
+    nsub = 0;
     tw = m_tile % p.tiles_w;
     th = (m_tile / p.tiles_w) % p.tiles_h;
     tn = m_tile / (p.tiles_w * p.tiles_h);
@@ -237,8 +262,8 @@ __global__ void __launch_bounds__(kTileThreads, 1)
     if (threadIdx.x == 0) {
       int stage = 0, phase = 0;
       for (int t = blockIdx.x; t < total; t += gridDim.x) {
-        int n_tile, tw, th, tn;
-        decode(t, n_tile, tw, th, tn);
+        int n_tile, tw, th, tn, nsub;
+        decode(t, n_tile, tw, th, tn, nsub);
         int base[5] = {0, 0, 0, 0, 0};
         base[p.dim_w] += tw * p.bw;
         if (p.dim_h >= 0) base[p.dim_h] += th * p.bh;
@@ -247,11 +272,28 @@ __global__ void __launch_bounds__(kTileThreads, 1)
         for (int kb = 0; kb < p.num_kb; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
           uint8_t* sa = smem + stage * Cfg::kStageBytes;
-          mbar_expect_tx(&full[stage], Cfg::kStageBytes);
-          // kSwap: the pixels are the N operand and the weights the M operand
-          tma_load_5d(&map_a, &full[stage], kSwap ? sa + kABytes : sa, base[0] + p.tap_off[tap][0] + chunk * kBlockK,
-                      base[1] + p.tap_off[tap][1], base[2] + p.tap_off[tap][2], base[3] + p.tap_off[tap][3],
-                      base[4] + p.tap_off[tap][4]);
+          if (kSwap || nsub == 0) {
+            mbar_expect_tx(&full[stage], Cfg::kStageBytes);
+            // kSwap: the pixels are the N operand and the weights the M operand
+            tma_load_5d(&map_a, &full[stage], kSwap ? sa + kABytes : sa, base[0] + p.tap_off[tap][0] + chunk * kBlockK,
+                        base[1] + p.tap_off[tap][1], base[2] + p.tap_off[tap][2], base[3] + p.tap_off[tap][3],
+                        base[4] + p.tap_off[tap][4]);
+          } else {
+            // one box of the last group's images per block, into the block's rows of the A slot
+            mbar_expect_tx(&full[stage], Cfg::kBBytes + nsub * p.pack_rows * 128);
+            for (int q = 0, x = tw, y = th; q < nsub; ++q) {
+              // block q's displacement from the tile's first block, along w (dimension 1 of both conv3 views) and h
+              const int dw = (x - tw) * p.bw, dh = (y - th) * p.bh;
+              tma_load_5d(&map_a_pk, &full[stage], sa + q * p.pack_rows * 128,
+                          base[0] + p.tap_off[tap][0] + chunk * kBlockK, base[1] + p.tap_off[tap][1] + dw,
+                          base[2] + p.tap_off[tap][2] + (p.dim_h == 2 ? dh : 0),
+                          base[3] + p.tap_off[tap][3] + (p.dim_h == 3 ? dh : 0), base[4] + p.tap_off[tap][4]);
+              if (++x == p.tiles_w) {
+                x = 0;
+                ++y;
+              }
+            }
+          }
           tma_load_2d(&map_b, &full[stage], kSwap ? sa : sa + kABytes, kb * kBlockK, n_tile * BN);
           if (++chunk == p.chunks_per_tap) {
             chunk = 0;
@@ -284,8 +326,8 @@ __global__ void __launch_bounds__(kTileThreads, 1)
   for (int i = 0; i < Cfg::kN / 2; ++i) acc[i] = 0.f;
   int stage = 0, phase = 0, it = 0;
   for (int t = blockIdx.x; t < total; t += gridDim.x, ++it) {
-    int n_tile, tw, th, tn;
-    decode(t, n_tile, tw, th, tn);
+    int n_tile, tw, th, tn, nsub;
+    decode(t, n_tile, tw, th, tn, nsub);
     const int n0 = tn * p.bn;
     int n_o0 = n0, coff = 0;
     if (p.out_split > 0) {
@@ -300,6 +342,25 @@ __global__ void __launch_bounds__(kTileThreads, 1)
       oc[p.odim_n] = n_o0;
       rc[p.odim_n] = n0;
     }
+    // A packed tile's output / residual boxes: f(row byte offset in a slab, x, y) for each of its blocks, whose
+    // images are those of the last group (the *_pk maps; conv3 only, so the coordinates are (c, w, h, n)).
+    auto for_blocks = [&](auto&& f) {
+      for (int q = 0, x = tw, y = th; q < nsub; ++q) {
+        f((uint32_t)(q * p.pack_rows * 128), x * p.bw, y * p.bh);
+        if (++x == p.tiles_w) {
+          x = 0;
+          ++y;
+        }
+      }
+    };
+    // the residual of 64 channels from `ch` (kSwap: and images from `img` on) into slab `dst`, on barrier rb
+    auto load_res = [&](uint64_t* rb, uint8_t* dst, int ch, int img) {
+      if (nsub == 0)
+        tma_load_5d(&map_res, rb, dst, ch, rc[1], rc[2], rc[3] + img, rc[4]);
+      else
+        for_blocks([&](uint32_t off, int x, int y) { tma_load_5d(&map_res_pk, rb, dst + off, ch, x, y, n0, 0); });
+    };
+    auto slab_bytes = [&]() -> uint32_t { return nsub ? nsub * p.pack_rows * 128 : kSlabBytes; };  // a slab's boxes
     // ---- main loop: one wgmma batch (4 x K = 16) per k-block; a stage is released once the NEXT batch is issued
     int prev = -1;
     for (int kb = 0; kb < p.num_kb; ++kb) {
@@ -321,9 +382,8 @@ __global__ void __launch_bounds__(kTileThreads, 1)
         if (p.has_res) {
           for (int s = 0; s < NSLAB; ++s) {
             uint64_t* rb = &res_full[kAlt ? s : 0];
-            if (kAlt || s == 0) mbar_expect_tx(rb, kAlt ? kSlabBytes : NSLAB * kSlabBytes);
-            tma_load_5d(&map_res, rb, staging + s * kSlabBytes, n_tile * BN + slab_ch(s), rc[1], rc[2],
-                        rc[3] + slab_img(s), rc[4]);
+            if (kAlt || s == 0) mbar_expect_tx(rb, (kAlt ? 1 : NSLAB) * slab_bytes());
+            load_res(rb, staging + s * kSlabBytes, n_tile * BN + slab_ch(s), slab_img(s));
           }
         }
       }
@@ -404,7 +464,13 @@ __global__ void __launch_bounds__(kTileThreads, 1)
       for (int h = 0; h < 2; ++h) {
         const int row = r0 + 8 * h;
         const int jj = row & (p.bw - 1), ii = (row >> p.lg_bw) & (p.bh - 1);
-        const int i = th * p.bh + ii, j = min(tw * p.bw + jj, p.Wo - 1);
+        int bx = tw, by = th;  // the row's spatial block; in a packed tile, that of its block q (rows no block fills
+        if (nsub) {            // take the last block's)
+          const int blk = th * p.tiles_w + tw + min(row / p.pack_rows, nsub - 1);
+          bx = blk % p.tiles_w;
+          by = blk / p.tiles_w;
+        }
+        const int i = by * p.bh + ii, j = min(bx * p.bw + jj, p.Wo - 1);
         pap[h] = p.post_add + (size_t)(i * p.Wo + j) * p.Cout + n_tile * BN;
       }
     }
@@ -435,9 +501,8 @@ __global__ void __launch_bounds__(kTileThreads, 1)
         if (leader) {
           asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
           uint64_t* rb = &res_full[(b + 1) & 1];
-          mbar_expect_tx(rb, kSlabBytes);
-          tma_load_5d(&map_res, rb, staging + ((b + 1) & 1) * kSlabBytes, n_tile * BN + (b + 1) * 64, rc[1], rc[2],
-                      rc[3], rc[4]);
+          mbar_expect_tx(rb, slab_bytes());
+          load_res(rb, staging + ((b + 1) & 1) * kSlabBytes, n_tile * BN + (b + 1) * 64, 0);
         }
       }
       // Phase of the barrier that batch b waits on, in the CTA's it-th tile: it completes NB / NSLAB times per tile
@@ -493,9 +558,15 @@ __global__ void __launch_bounds__(kTileThreads, 1)
         if (kAlt && leader) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
         asm volatile("bar.sync 1, 256;" ::: "memory");
         if (leader) {
-          for (int q = kAlt ? s : 0; q < (kAlt ? s + 1 : NSLAB); ++q)
-            tma_store_5d(&map_out, staging + q * kSlabBytes, coff + n_tile * BN + (kAlt ? 64 * b : 64 * q), oc[1],
-                         oc[2], oc[3], oc[4]);
+          for (int q = kAlt ? s : 0; q < (kAlt ? s + 1 : NSLAB); ++q) {
+            const int ch = coff + n_tile * BN + (kAlt ? 64 * b : 64 * q);
+            if (nsub == 0)
+              tma_store_5d(&map_out, staging + q * kSlabBytes, ch, oc[1], oc[2], oc[3], oc[4]);
+            else
+              for_blocks([&](uint32_t off, int x, int y) {
+                tma_store_5d(&map_out_pk, staging + q * kSlabBytes + off, ch, x, y, n_o0, 0);
+              });
+          }
           asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         }
       }
@@ -578,7 +649,8 @@ static int ilog2(int v) {
 
 template <int BN, bool kSwap = false>
 static int launch_bn(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo, const CUtensorMap& mr,
-                     const GemmParams& p, cudaStream_t stream) {
+                     const CUtensorMap& ma_pk, const CUtensorMap& mo_pk, const CUtensorMap& mr_pk, const GemmParams& p,
+                     cudaStream_t stream) {
   using Cfg = TileCfg<BN, kSwap>;
   static std::atomic<unsigned long long> attr_mask{0};  // per device: the attribute is device state
   if (!device_bit_test(attr_mask)) {
@@ -591,7 +663,7 @@ static int launch_bn(const CUtensorMap& ma, const CUtensorMap& mb, const CUtenso
   const int grid = p.total_tiles < sms ? p.total_tiles : sms;
   prof_mark_begin(0, p.alg_flops, stream);
   FP_CUDA_OK(launch_pdl(gemm_tile_kernel<BN, kSwap>, dim3(grid), dim3(kTileThreads), Cfg::kSmemBytes, stream, 1, ma, mb,
-                        mo, mr, p));
+                        mo, mr, ma_pk, mo_pk, mr_pk, p));
   prof_mark_end(stream);
   note_launches(1);
   FP_CUDA_OK(cudaGetLastError());
@@ -728,7 +800,19 @@ static int gemm_layer_plan(const GemmLayer& L, cudaStream_t stream, int* tile_n,
     box[p.dim_n] = 4;
     p.tiles_n = (L.n_img + 3) / 4;
   }
-  const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
+  // The last image group holds r = n_img % bn images.  As one box per spatial block it would leave bn - r of the
+  // tile's bn images to the TMA unit's zero fill; instead, k = bn / r >= 2 of its blocks share a tile, each as a box
+  // of r images at rows q * bw * bh * r (a multiple of the 1024-byte swizzle atom).  Every output element keeps its
+  // k-order and epilogue arithmetic.  At 252 hypotheses the 20 x 20 layers' 4 x 4 x 8 tiles go from 25 x 32 to
+  // 25 x 31 + 13 m-tiles: 1576 instead of 1600 tiles of 256 channels, 12 rounds of 132 persistent CTAs instead of 13.
+  // A grid of one round or less gains nothing (its time is one tile's): there, packing would only put the same work
+  // on fewer SMs (packing track_one's layers, one to five images, took its p50 from 1.2-1.3 ms to 1.5 ms on an H100
+  // SXM at 700 W).  The tile width is chosen from the packed count; packing itself is decided below, against the SM
+  // count, after the tile queries have returned.
+  const int last_n = L.n_img % p.bn;
+  const int pack = (!swap && last_n > 0) ? p.bn / last_n : 0;
+  const int blocks = p.tiles_w * p.tiles_h;
+  int m_tiles = pack >= 2 ? blocks * (L.n_img / p.bn) + (blocks + pack - 1) / pack : blocks * p.tiles_n;
   if (swap) BN = 128;
   else if (L.Cout % 256 == 0 && p.num_kb >= kWideMinKBlocks) {
     const int sms = num_sms();
@@ -738,7 +822,6 @@ static int gemm_layer_plan(const GemmLayer& L, cudaStream_t stream, int* tile_n,
   else if (L.Cout % 64 == 0) BN = 64;
   else FP_REQUIRE(false, "Cout=%d must be a multiple of 64", L.Cout);
   p.n_tiles_n = L.Cout / BN;
-  p.total_tiles = p.tiles_w * p.tiles_h * p.tiles_n * p.n_tiles_n;
   p.Ho = Ho; p.Wo = Wo; p.n_img = L.n_img; p.Cout = L.Cout;
   p.bias = L.bias;
   p.has_res = L.res != nullptr;
@@ -760,11 +843,30 @@ static int gemm_layer_plan(const GemmLayer& L, cudaStream_t stream, int* tile_n,
     if (tile_m) *tile_m = swap ? 256 : linear_ws ? 64 : 128;
     return 0;
   }
+  if (pack >= 2) {
+    const int sms = num_sms();
+    FP_REQUIRE(sms > 0, "no CUDA device");
+    if ((long long)blocks * p.tiles_n * p.n_tiles_n > sms) {
+      p.pack = pack;
+      p.pack_rows = p.bw * p.bh * last_n;
+      p.tiles_n = L.n_img / p.bn;
+    } else {
+      m_tiles = blocks * p.tiles_n;
+    }
+  }
+  p.total_tiles = m_tiles * p.n_tiles_n;
   if (p.total_tiles == 0) return 0;
   if (linear_ws) return linear_ws_launch(L, stream);
 
   int rc = encode_map(&ma, L.in, 5, dims, str, box);
   if (rc) return rc;
+  // packed tiles: the same maps with a box of the last group's images (unused copies without packing)
+  CUtensorMap ma_pk = ma, mo_pk, mr_pk;
+  if (p.pack) {
+    box[p.dim_n] = (uint32_t)last_n;
+    rc = encode_map(&ma_pk, L.in, 5, dims, str, box);
+    if (rc) return rc;
+  }
   uint64_t wd[2] = {(uint64_t)ktot, (uint64_t)L.Cout};
   uint64_t ws[1] = {(uint64_t)ktot * E};
   uint32_t wb[2] = {64, (uint32_t)BN};
@@ -796,20 +898,32 @@ static int gemm_layer_plan(const GemmLayer& L, cudaStream_t stream, int* tile_n,
     };
     p.odim_h = lin ? -1 : 2;
     p.odim_n = lin ? -1 : 3;
+    // the map of 128-pixel boxes and its packed-tile twin, whose box holds the last group's images
+    auto encode_out = [&](CUtensorMap* m, CUtensorMap* m_pk, const void* base) {
+      int e = encode_map(m, base, 5, od, os, ob);
+      if (e || !p.pack) {
+        *m_pk = *m;
+        return e;
+      }
+      ob[3] = (uint32_t)last_n;
+      return encode_map(m_pk, base, 5, od, os, ob);
+    };
     fill(L.out_ld, n_out);
-    rc = encode_map(&mo, L.out, 5, od, os, ob);
+    rc = encode_out(&mo, &mo_pk, L.out);
     if (rc) return rc;
     if (L.res) {
       fill(L.res_ld, L.n_img);
-      rc = encode_map(&mr, L.res, 5, od, os, ob);
+      rc = encode_out(&mr, &mr_pk, L.res);
       if (rc) return rc;
     } else {
       mr = mo;
+      mr_pk = mo_pk;
     }
   }
-  if (swap) return launch_bn<128, true>(ma, mb, mo, mr, p, stream);
-  if (BN == 256) return launch_bn<256>(ma, mb, mo, mr, p, stream);
-  return BN == 128 ? launch_bn<128>(ma, mb, mo, mr, p, stream) : launch_bn<64>(ma, mb, mo, mr, p, stream);
+  if (swap) return launch_bn<128, true>(ma, mb, mo, mr, ma_pk, mo_pk, mr_pk, p, stream);
+  if (BN == 256) return launch_bn<256>(ma, mb, mo, mr, ma_pk, mo_pk, mr_pk, p, stream);
+  return BN == 128 ? launch_bn<128>(ma, mb, mo, mr, ma_pk, mo_pk, mr_pk, p, stream)
+                   : launch_bn<64>(ma, mb, mo, mr, ma_pk, mo_pk, mr_pk, p, stream);
 }
 
 int gemm_layer_launch(const GemmLayer& L, cudaStream_t stream) { return gemm_layer_plan(L, stream, nullptr, nullptr); }
