@@ -84,10 +84,11 @@ static CameraDev camera_dev(const fp_ctx* c, int i) {
 
 // mesh_of: [N] device slot ids (validated by the caller), or null = every hypothesis renders slot 0.  cams / camera_of:
 // device camera table and [N] camera ids (the tracking calls, fp_register_cameras), or null = the context's frame
-// (camera 0), by value
+// (camera 0), by value.  fit / fit_delta: the fit pass of the tracking calls (CropParams::fit), no crops
 static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg, float* win, int* stats,
                       cudaStream_t st, const int* mesh_of = nullptr, const CameraDev* cams = nullptr,
-                      const int* camera_of = nullptr, float4* vis = nullptr) {
+                      const int* camera_of = nullptr, float4* vis = nullptr, int* fit = nullptr,
+                      const float* fit_delta = nullptr) {
   FP_REQUIRE(mesh_of || c->mesh[0].loaded, "no mesh: call fp_set_mesh first");
   FP_REQUIRE(c->has_frame, "no frame: call fp_set_frame first");
   // only launches below: this body is also what run_graphed captures (no allocation, no synchronisation)
@@ -109,6 +110,8 @@ static int make_crops(fp_ctx* c, const float* poses, int N, int mode, float* dbg
   p.cams = cams;
   p.camera_of = camera_of;
   p.vis = vis;
+  p.fit = fit;
+  p.fit_delta = fit_delta;
   return crop_launch(p, st);
 }
 
@@ -119,6 +122,7 @@ enum class GraphKind {
   TrackObjects = 2,      // fp_track, fp_track_objects, fp_track_cameras
   RegisterRefine = 3,    // fp_register_objects / _cameras: one pass's refinement
   RegisterFeatures = 4,  // fp_register_objects / _cameras: one pass's scorer features
+  TrackObjectsFit = 5,   // fp_track_cameras_fit_submit: TrackObjects, then the fit pass at the returned poses
 };
 
 // Runs `body(stream)` — a fixed sequence of kernel launches (and fixed-address copies) on ctx-owned buffers —
@@ -363,6 +367,8 @@ int order_after_track(fp_ctx* c, cudaStream_t st) {
 }
 
 constexpr size_t kTableBytes = sizeof(CameraDev) * kMaxCameras;  // the camera table at the head of fp_ctx::args
+// fp_ctx::args (and its staging) for `rows` slot and camera ids: the table, the ids, and a tracking call's fit threshold
+static size_t args_bytes(int rows) { return kTableBytes + (size_t)2 * rows * sizeof(int) + sizeof(float); }
 
 // The cameras of fp_track_cameras / _objects and fp_register_cameras / _objects, before anything reads a frame.  Every
 // camera's buffers are sized for the largest frame of the call (kept at the largest size seen, so a permutation of the
@@ -390,8 +396,8 @@ static int setup_cameras(fp_ctx* c, StagingSet& set, int C, const unsigned char*
     if (!on_dev.depth[i]) FP_TRY(pinned_alloc(nullptr, set.depth[i], npix_max * 4));
   }
   c->n_frames = C;
-  FP_TRY(dev_alloc(&c->epoch, c->args, kTableBytes + (size_t)2 * rows * sizeof(int)));
-  FP_TRY(pinned_alloc(nullptr, set.args, kTableBytes + (size_t)2 * staged_rows * sizeof(int)));
+  FP_TRY(dev_alloc(&c->epoch, c->args, args_bytes(rows)));
+  FP_TRY(pinned_alloc(nullptr, set.args, args_bytes(staged_rows)));
   CameraDev* table = reinterpret_cast<CameraDev*>(set.args.p);
   memset(table, 0, kTableBytes);
   for (int i = 0; i < C; ++i) {
@@ -407,16 +413,19 @@ static int setup_cameras(fp_ctx* c, StagingSet& set, int C, const unsigned char*
   return 0;
 }
 
-// The staging uploads of one tracking call: the frames, then the camera table, the slot ids and the camera ids in one
-// copy to the argument block.  H_max / W_max as setup_cameras.
+// The staging uploads of one tracking call: the frames, then the camera table, the slot ids, the camera ids and, with a
+// fit (delta non-null), its threshold in one copy to the argument block.  H_max / W_max as setup_cameras.
 static int stage_track_call(fp_ctx* c, StagingSet& set, int C, const unsigned char* const* rgb, const float* const* depth,
                             const FrameSources& on_dev, const float* K, const int* H, const int* W, int M,
-                            const int* camera_of, const int* slots_host, cudaStream_t st, int& H_max, int& W_max) {
+                            const int* camera_of, const int* slots_host, const float* delta, cudaStream_t st, int& H_max,
+                            int& W_max) {
   FP_TRY(setup_cameras(c, set, C, rgb, depth, on_dev, K, H, W, M, M, st, H_max, W_max));
   int* ids = reinterpret_cast<int*>(static_cast<char*>(set.args.p) + kTableBytes);
   memcpy(ids, slots_host, (size_t)M * sizeof(int));
   memcpy(ids + M, camera_of, (size_t)M * sizeof(int));
-  FP_CUDA_OK(cudaMemcpyAsync(c->args.p, set.args.p, kTableBytes + (size_t)2 * M * sizeof(int), cudaMemcpyHostToDevice, st));
+  if (delta) memcpy(ids + 2 * M, delta, sizeof(float));
+  const size_t bytes = kTableBytes + (size_t)2 * M * sizeof(int) + (delta ? sizeof(float) : 0);
+  FP_CUDA_OK(cudaMemcpyAsync(c->args.p, set.args.p, bytes, cudaMemcpyHostToDevice, st));
   return 0;
 }
 
@@ -430,11 +439,14 @@ static int stage_track_call(fp_ctx* c, StagingSet& set, int C, const unsigned ch
 // Readback, so one graph serves every staging set.  Frames on the device are read in place through the camera table
 // (setup_cameras), so where a frame lives changes neither the graph nor its key.  poses_out_dev and poses_keep_dev
 // (fp_track's continuation pose) are optional and complete in stream order; *ticket receives the call's ticket.
+// delta (host, validated) makes it a call with a fit: the TrackObjectsFit graph zeroes the fit counts first and ends
+// with the fit pass at the returned poses; delta travels in the argument block, so a new delta replays the graph.  The
+// counts go to fit_out_dev (optional, stream order) and to the Readback right after the poses.
 static int track_cameras_submit(fp_ctx* c, const char* caller, int C, const unsigned char* const* rgb,
                                 const float* const* depth, const float* K, const int* H, const int* W, int M,
                                 const int* camera_of, const int* slots_host, const float* poses_in_dev, int iterations,
                                 float* poses_out_dev, cudaStream_t st, unsigned long long* ticket,
-                                float* poses_keep_dev = nullptr) {
+                                float* poses_keep_dev = nullptr, const float* delta = nullptr, int* fit_out_dev = nullptr) {
   FrameSources on_dev;
   FP_TRY(frame_sources(c, C, rgb, depth, on_dev, caller));  // refused before anything is enqueued
   StagingSet* set;
@@ -449,9 +461,15 @@ static int track_cameras_submit(fp_ctx* c, const char* caller, int C, const unsi
   }
   FP_TRY(ensure_capacity(c, M));
   FP_TRY(pinned_alloc(nullptr, rb->poses, (size_t)M * 64));
+  const size_t fit_bytes = (size_t)M * kFitCounts * sizeof(int);
+  if (delta) {
+    FP_TRY(dev_alloc(&c->epoch, c->fit, fit_bytes));
+    FP_TRY(pinned_alloc(nullptr, rb->fit, fit_bytes));
+  }
   c->has_frame = false;
   int H_max = 0, W_max = 0;
-  const int staged = stage_track_call(c, *set, C, rgb, depth, on_dev, K, H, W, M, camera_of, slots_host, st, H_max, W_max);
+  const int staged =
+      stage_track_call(c, *set, C, rgb, depth, on_dev, K, H, W, M, camera_of, slots_host, delta, st, H_max, W_max);
   // whatever was staged before a failure is still on its way out: the set stays busy until then
   FP_TRY(set_busy(*set, st));
   FP_TRY(staged);
@@ -465,43 +483,59 @@ static int track_cameras_submit(fp_ctx* c, const char* caller, int C, const unsi
   const CameraDev* cams_dev = reinterpret_cast<const CameraDev*>(c->args.p);
   const int* mesh_of = reinterpret_cast<const int*>(static_cast<const char*>(c->args.p) + kTableBytes);
   const int* cam_of = mesh_of + M;
+  const float* delta_dev = reinterpret_cast<const float*>(cam_of + M);
+  int* fit = reinterpret_cast<int*>(c->fit.p);
   float* pa = reinterpret_cast<float*>(c->poses_a.p);
   float* pb = reinterpret_cast<float*>(c->poses_b.p);
   FP_CUDA_OK(cudaMemcpyAsync(pa, poses_in_dev, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
   const float* fin = (iterations % 2 == 0) ? pa : pb;
   const int grid_h = c->cam_grid_h, grid_w = c->cam_grid_w;
   auto body = [&](cudaStream_t s2) -> int {
+    // the counts are zeroed at the head of the sequence, so the fit pass follows the last pose update by programmatic
+    // dependent launch like every other link of the chain
+    if (delta) FP_CUDA_OK(cudaMemsetAsync(fit, 0, fit_bytes, s2));
     // estimater.py:250-268 for every object of every camera at once: each camera's frame filtered once (erode +
     // bilateral, depth2xyzmap_batch(zfar = inf)), M hypotheses each rendering its own mesh and cropping its own
     // camera's frame
     FP_TRY(frame_prep_cameras_launch(cams_dev, C, grid_h, grid_w, INFINITY, s2));
     c->has_frame = true;
-    return refine_body(c, M, iterations, s2, mesh_of, cams_dev, cam_of);
+    FP_TRY(refine_body(c, M, iterations, s2, mesh_of, cams_dev, cam_of));
+    if (delta) FP_TRY(make_crops(c, fin, M, 0, nullptr, nullptr, nullptr, s2, mesh_of, cams_dev, cam_of, nullptr, fit, delta_dev));
+    return 0;
   };
-  FP_TRY(run_graphed(c, GraphKind::TrackObjects, M, iterations, st, body, C));
+  FP_TRY(run_graphed(c, delta ? GraphKind::TrackObjectsFit : GraphKind::TrackObjects, M, iterations, st, body, C));
   c->has_frame = true;
   if (poses_out_dev) FP_CUDA_OK(cudaMemcpyAsync(poses_out_dev, fin, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
+  if (fit_out_dev) FP_CUDA_OK(cudaMemcpyAsync(fit_out_dev, fit, fit_bytes, cudaMemcpyDeviceToDevice, st));
   if (poses_keep_dev) FP_CUDA_OK(cudaMemcpyAsync(poses_keep_dev, fin, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
   FP_CUDA_OK(cudaMemcpyAsync(rb->poses.p, fin, (size_t)M * 64, cudaMemcpyDeviceToHost, st));
+  if (delta) FP_CUDA_OK(cudaMemcpyAsync(rb->fit.p, fit, fit_bytes, cudaMemcpyDeviceToHost, st));
   FP_CUDA_OK(rb->done.record(st));
   c->last_done = rb->done.e;
   c->last_stream = st;
   rb->M = M;
+  rb->has_fit = delta != nullptr;
   rb->ticket = ++c->last_ticket;
   *ticket = rb->ticket;
   return 0;
 }
 
-// fp_track_wait: waits for ticket's read-back and copies its poses out (poses_out_host may be null: the result is
-// dropped).  The ticket is collected whatever the outcome, so an asynchronous error is reported once.
-static int track_wait(fp_ctx* c, unsigned long long ticket, float* poses_out_host) {
+// fp_track_wait / fp_track_fit_wait (fit): waits for ticket's read-back and copies its poses out, and its fit counts for
+// fp_track_fit_wait (either output may be null: that result is dropped).  fp_track_fit_wait refuses a ticket submitted
+// without a fit and leaves it uncollected.  Otherwise the ticket is collected whatever the outcome, so an asynchronous
+// error is reported once.
+static int track_wait(fp_ctx* c, unsigned long long ticket, float* poses_out_host, bool fit = false,
+                      int* fit_out_host = nullptr) {
+  const char* caller = fit ? "fp_track_fit_wait" : "fp_track_wait";
   Readback* rb = nullptr;
   for (auto& r : c->readbacks)
     if (ticket != 0 && r->ticket == ticket) rb = r.get();
-  FP_REQUIRE(rb, "fp_track_wait: ticket %llu is unknown or already collected", ticket);
+  FP_REQUIRE(rb, "%s: ticket %llu is unknown or already collected", caller, ticket);
+  FP_REQUIRE(!fit || rb->has_fit, "%s: ticket %llu was submitted without a fit: collect it with fp_track_wait", caller, ticket);
   rb->ticket = 0;
   FP_CUDA_OK(cudaEventSynchronize(rb->done.e));
   if (poses_out_host) memcpy(poses_out_host, rb->poses.p, (size_t)rb->M * 64);
+  if (fit_out_host) memcpy(fit_out_host, rb->fit.p, (size_t)rb->M * kFitCounts * sizeof(int));
   return 0;
 }
 
@@ -1099,6 +1133,14 @@ int fp_track_wait(fp_ctx* c, unsigned long long ticket, float* poses_out_host) {
   FP_API_END
 }
 
+int fp_track_fit_wait(fp_ctx* c, unsigned long long ticket, float* poses_out_host, int* fit_out_host) {
+  FP_API_BEGIN
+  FP_REQUIRE(c, "fp_track_fit_wait: null ctx");
+  DeviceGuard dg(c->device);
+  return track_wait(c, ticket, poses_out_host, /*fit=*/true, fit_out_host);
+  FP_API_END
+}
+
 int fp_vis_size(int kind, int N, int* hw_out) {
   FP_API_BEGIN
   FP_REQUIRE(hw_out, "fp_vis_size: null output");
@@ -1207,6 +1249,25 @@ int fp_track_cameras_submit(fp_ctx* c, int C, const unsigned char* const* rgb, c
   DeviceGuard dg(c->device);
   return track_cameras_submit(c, "fp_track_cameras", C, rgb, depth, K, H, W, M, camera_of, slots_host, poses_in_dev, iterations,
                               poses_out_dev, reinterpret_cast<cudaStream_t>(stream), ticket);
+  FP_API_END
+}
+
+int fp_track_cameras_fit_submit(fp_ctx* c, int C, const unsigned char* const* rgb, const float* const* depth,
+                                const float* K, const int* H, const int* W, int M, const int* camera_of,
+                                const int* slots_host, const float* poses_in_dev, int iterations, float delta,
+                                float* poses_out_dev, int* fit_out_dev, void* stream, unsigned long long* ticket) {
+  FP_API_BEGIN
+  FP_REQUIRE(c && rgb && depth && K && H && W && M > 0 && camera_of && slots_host && poses_in_dev && iterations >= 0 &&
+                 ticket,
+             "fp_track_cameras_fit: bad argument");
+  FP_REQUIRE(isfinite(delta) && delta >= 0.f, "fp_track_cameras_fit: delta %g must be finite and >= 0 (metres)", (double)delta);
+  FP_REQUIRE(c->net[0].loaded, "refiner weights not loaded");
+  FP_TRY(check_cameras(C, rgb, depth, H, W, M, camera_of, "fp_track_cameras_fit"));
+  FP_TRY(check_slots(c, M, slots_host, "fp_track_cameras_fit"));
+  DeviceGuard dg(c->device);
+  return track_cameras_submit(c, "fp_track_cameras_fit", C, rgb, depth, K, H, W, M, camera_of, slots_host, poses_in_dev,
+                              iterations, poses_out_dev, reinterpret_cast<cudaStream_t>(stream), ticket, nullptr, &delta,
+                              fit_out_dev);
   FP_API_END
 }
 

@@ -112,6 +112,7 @@ struct TileSmem {
   int stat[4];
   MeshSlotDev slot;  // mesh table entry of this CTA's hypothesis
   CameraDev cam;     // camera table entry of this CTA's hypothesis (kCams)
+  int fit[kFitCounts];  // kFit: this CTA's counts (after every member the other instantiations read)
 };
 static_assert(sizeof(MeshSlotDev) % 16 == 0 && sizeof(MeshSlotDev) / 16 <= 32, "table entry copied as uint4s by warp 0");
 
@@ -122,7 +123,15 @@ static_assert(sizeof(MeshSlotDev) % 16 == 0 && sizeof(MeshSlotDev) / 16 <= 32, "
 #define FRAME(f) (kCams ? sm.cam.f : p.frame.f)
 // kVis: also write the fp32 record of every crop pixel to p.vis (fp_vis, the debug canvases).  A template flag for the
 // same reason: the instantiations without it compile to the same code as before the record existed.
-template <int TILE, bool kStats, bool kCams, bool kVis>
+// kFit (with kCams only, mode 0): the tracking calls' fit pass at the returned poses.  Binning and raster as always;
+// the shade loop takes only the rendered camera z of the winning triangle (the Z the A side normalises) and the z of
+// the nearest xyz_map sample (what the B side reads at the same crop pixel), and counts, per pixel p with d = z_o - z_r:
+// covered, valid (covered and z_o >= 0.001), inlier (valid, |d| <= delta), occluded (valid, d < -delta) and behind
+// (valid, d > delta).  Per lane, per warp (__reduce_add_sync), per CTA in shared memory, one atomicAdd per counter per
+// CTA: integer counts, independent of the tile size and of the order of CTAs, hypotheses and cameras.  Nothing is
+// stored but the counts.  The A and B windows differ by the 159/160 scale of SURVEY F5; like the refiner, the counts
+// compare the same crop pixel on both sides.
+template <int TILE, bool kStats, bool kCams, bool kVis, bool kFit>
 __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(const CropParams p) {
   constexpr int TPR = S / TILE;
   extern __shared__ __align__(16) unsigned char crop_smem_raw[];
@@ -139,6 +148,7 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
     sm.next = 0;
     sm.stat[0] = sm.stat[1] = sm.stat[2] = sm.stat[3] = 0;
   }
+  if (kFit && tid < kFitCounts) sm.fit[tid] = 0;
   // The mesh table, the camera table and the slot and camera ids are written by copies that precede the whole launch
   // sequence, never by a kernel of it: they may be read before the programmatic-dependency wait.  The pixels the camera
   // entry points to come from frame_prep_kernel of the same sequence and are only read after it.
@@ -366,6 +376,9 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
   __half* outA = p.crops + (size_t)n * img_stride;
   __half* outB = p.crops + (size_t)(p.b_img0 + n) * img_stride;
   constexpr int kBlocksX = TILE / 8, kBlocks = kBlocksX * (TILE / 4);
+  float delta = 0.f;  // kFit: the threshold, written with the slot and camera ids (readable before the wait)
+  int fit_n[kFitCounts] = {0, 0, 0, 0, 0};  // kFit: this lane's counts
+  if constexpr (kFit) delta = __ldg(p.fit_delta);
 #pragma unroll 1
   for (int blk = warp; blk < kBlocks; blk += kWarps) {
     const int jl = (blk % kBlocksX) * 8 + (lane & 7), rl = (blk / kBlocksX) * 4 + (lane >> 3);
@@ -375,7 +388,7 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
     const int unc = sm.coln[jl], uzc = sm.colz[jl];
     // ---- A: rendered crop
     float ar = 0.f, ag = 0.f, ab = 0.f, ax = 0.f, ay = 0.f, az = 0.f;
-    float za = 0.f;  // kVis: rendered camera z
+    float za = 0.f;  // kVis, kFit: rendered camera z
     const unsigned long long key = sm.zt[rl * TILE + jl];
     if (key != 0ull) {
       const int f = (int)(0xFFFFFFFFu - (unsigned)(key & 0xFFFFFFFFull));
@@ -387,15 +400,19 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
 #pragma unroll
       for (int q = 0; q < 3; ++q) {
         const float4 pp = __ldg(M.vpos + vid[q]);
-        const float4 nn = __ldg(M.vnrm + vid[q]);
-        att[q] = __ldg(M.vatt + vid[q]);
-        xform_vertex(sm.P, pp.x, pp.y, pp.z, W, FRAME(fx), FRAME(fy), FRAME(cx), FRAME(cy), vs[q]);
-        // diffuse = clip(normalize(R n) . (0,0,-1), 0, 1)   (Utils.py:203-207)
-        const float cxn = sm.P[0] * nn.x + sm.P[1] * nn.y + sm.P[2] * nn.z;
-        const float cyn = sm.P[4] * nn.x + sm.P[5] * nn.y + sm.P[6] * nn.z;
-        const float czn = sm.P[8] * nn.x + sm.P[9] * nn.y + sm.P[10] * nn.z;
-        const float len = fmaxf(sqrtf(cxn * cxn + cyn * cyn + czn * czn), 1e-12f);
-        dif[q] = fminf(fmaxf(-czn / len, 0.f), 1.f);
+        if constexpr (kFit) {
+          xform_vertex(sm.P, pp.x, pp.y, pp.z, W, FRAME(fx), FRAME(fy), FRAME(cx), FRAME(cy), vs[q]);
+        } else {
+          const float4 nn = __ldg(M.vnrm + vid[q]);
+          att[q] = __ldg(M.vatt + vid[q]);
+          xform_vertex(sm.P, pp.x, pp.y, pp.z, W, FRAME(fx), FRAME(fy), FRAME(cx), FRAME(cy), vs[q]);
+          // diffuse = clip(normalize(R n) . (0,0,-1), 0, 1)   (Utils.py:203-207)
+          const float cxn = sm.P[0] * nn.x + sm.P[1] * nn.y + sm.P[2] * nn.z;
+          const float cyn = sm.P[4] * nn.x + sm.P[5] * nn.y + sm.P[6] * nn.z;
+          const float czn = sm.P[8] * nn.x + sm.P[9] * nn.y + sm.P[10] * nn.z;
+          const float len = fmaxf(sqrtf(cxn * cxn + cyn * cyn + czn * czn), 1e-12f);
+          dif[q] = fminf(fmaxf(-czn / len, 0.f), 1.f);
+        }
       }
       float w0, w1, w2;  // perspective-correct weights (nvdiffrast: barycentrics computed in clip space)
       if (vs[0].Z > p.znear && vs[1].Z > p.znear && vs[2].Z > p.znear) {
@@ -427,44 +444,61 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
       const float X = w0 * vs[0].X + w1 * vs[1].X + w2 * vs[2].X;
       const float Y = w0 * vs[0].Y + w1 * vs[1].Y + w2 * vs[2].Y;
       const float Z = w0 * vs[0].Z + w1 * vs[1].Z + w2 * vs[2].Z;
-      const float diffuse = w0 * dif[0] + w1 * dif[1] + w2 * dif[2];
-      float cr, cg, cb;
-      if (sm.slot.has_tex) {
-        const int Ht = sm.slot.Ht, Wt = sm.slot.Wt;
-        const uchar4* tex = sm.slot.tex;
-        const float tu = w0 * att[0].x + w1 * att[1].x + w2 * att[2].x;
-        const float tv = w0 * att[0].y + w1 * att[1].y + w2 * att[2].y;
-        // dr.texture(filter_mode='linear', boundary 'wrap'): texel centres at +0.5.  Interpolated uv of a mesh lie in
-        // (-1, 2): the wrap is two conditional adds; anything further out takes the general modulo.
-        const float xx = tu * Wt - 0.5f, yy = tv * Ht - 0.5f;
-        const float xf = floorf(xx), yf = floorf(yy);
-        const float ax1 = xx - xf, ay1 = yy - yf;
-        int x0 = (int)xf, y0 = (int)yf;
-        if ((unsigned)(x0 + Wt) >= (unsigned)(3 * Wt)) x0 %= Wt;
-        if ((unsigned)(y0 + Ht) >= (unsigned)(3 * Ht)) y0 %= Ht;
-        if (x0 < 0) x0 += Wt;
-        if (y0 < 0) y0 += Ht;
-        if (x0 >= Wt) x0 -= Wt;
-        if (y0 >= Ht) y0 -= Ht;
-        const int x1 = (x0 + 1 == Wt) ? 0 : x0 + 1, y1 = (y0 + 1 == Ht) ? 0 : y0 + 1;
-        const uchar4 t00 = __ldg(tex + (size_t)y0 * Wt + x0), t01 = __ldg(tex + (size_t)y0 * Wt + x1);
-        const uchar4 t10 = __ldg(tex + (size_t)y1 * Wt + x0), t11 = __ldg(tex + (size_t)y1 * Wt + x1);
-        const float w00 = (1.f - ax1) * (1.f - ay1), w01 = ax1 * (1.f - ay1), w10 = (1.f - ax1) * ay1, w11 = ax1 * ay1;
-        const float k255 = 1.f / 255.f;
-        cr = (w00 * t00.x + w01 * t01.x + w10 * t10.x + w11 * t11.x) * k255;
-        cg = (w00 * t00.y + w01 * t01.y + w10 * t10.y + w11 * t11.y) * k255;
-        cb = (w00 * t00.z + w01 * t01.z + w10 * t10.z + w11 * t11.z) * k255;
+      if constexpr (kFit) {
+        za = Z;
       } else {
-        cr = w0 * att[0].x + w1 * att[1].x + w2 * att[2].x;
-        cg = w0 * att[0].y + w1 * att[1].y + w2 * att[2].y;
-        cb = w0 * att[0].z + w1 * att[1].z + w2 * att[2].z;
+        const float diffuse = w0 * dif[0] + w1 * dif[1] + w2 * dif[2];
+        float cr, cg, cb;
+        if (sm.slot.has_tex) {
+          const int Ht = sm.slot.Ht, Wt = sm.slot.Wt;
+          const uchar4* tex = sm.slot.tex;
+          const float tu = w0 * att[0].x + w1 * att[1].x + w2 * att[2].x;
+          const float tv = w0 * att[0].y + w1 * att[1].y + w2 * att[2].y;
+          // dr.texture(filter_mode='linear', boundary 'wrap'): texel centres at +0.5.  Interpolated uv of a mesh lie in
+          // (-1, 2): the wrap is two conditional adds; anything further out takes the general modulo.
+          const float xx = tu * Wt - 0.5f, yy = tv * Ht - 0.5f;
+          const float xf = floorf(xx), yf = floorf(yy);
+          const float ax1 = xx - xf, ay1 = yy - yf;
+          int x0 = (int)xf, y0 = (int)yf;
+          if ((unsigned)(x0 + Wt) >= (unsigned)(3 * Wt)) x0 %= Wt;
+          if ((unsigned)(y0 + Ht) >= (unsigned)(3 * Ht)) y0 %= Ht;
+          if (x0 < 0) x0 += Wt;
+          if (y0 < 0) y0 += Ht;
+          if (x0 >= Wt) x0 -= Wt;
+          if (y0 >= Ht) y0 -= Ht;
+          const int x1 = (x0 + 1 == Wt) ? 0 : x0 + 1, y1 = (y0 + 1 == Ht) ? 0 : y0 + 1;
+          const uchar4 t00 = __ldg(tex + (size_t)y0 * Wt + x0), t01 = __ldg(tex + (size_t)y0 * Wt + x1);
+          const uchar4 t10 = __ldg(tex + (size_t)y1 * Wt + x0), t11 = __ldg(tex + (size_t)y1 * Wt + x1);
+          const float w00 = (1.f - ax1) * (1.f - ay1), w01 = ax1 * (1.f - ay1), w10 = (1.f - ax1) * ay1, w11 = ax1 * ay1;
+          const float k255 = 1.f / 255.f;
+          cr = (w00 * t00.x + w01 * t01.x + w10 * t10.x + w11 * t11.x) * k255;
+          cg = (w00 * t00.y + w01 * t01.y + w10 * t10.y + w11 * t11.y) * k255;
+          cb = (w00 * t00.z + w01 * t01.z + w10 * t10.z + w11 * t11.z) * k255;
+        } else {
+          cr = w0 * att[0].x + w1 * att[1].x + w2 * att[2].x;
+          cg = w0 * att[0].y + w1 * att[1].y + w2 * att[2].y;
+          cb = w0 * att[0].z + w1 * att[1].z + w2 * att[2].z;
+        }
+        // color*w_ambient + diffuse*color*w_diffuse, clip(0,1)   (Utils.py:211-213)
+        ar = fminf(fmaxf(cr * 0.8f + diffuse * cr * 0.5f, 0.f), 1.f);
+        ag = fminf(fmaxf(cg * 0.8f + diffuse * cg * 0.5f, 0.f), 1.f);
+        ab = fminf(fmaxf(cb * 0.8f + diffuse * cb * 0.5f, 0.f), 1.f);
+        normalise_xyz(X, Y, Z, tvec, inv_radius, tau, ax, ay, az);
+        if (kVis) za = Z;
       }
-      // color*w_ambient + diffuse*color*w_diffuse, clip(0,1)   (Utils.py:211-213)
-      ar = fminf(fmaxf(cr * 0.8f + diffuse * cr * 0.5f, 0.f), 1.f);
-      ag = fminf(fmaxf(cg * 0.8f + diffuse * cg * 0.5f, 0.f), 1.f);
-      ab = fminf(fmaxf(cb * 0.8f + diffuse * cb * 0.5f, 0.f), 1.f);
-      normalise_xyz(X, Y, Z, tvec, inv_radius, tau, ax, ay, az);
-      if (kVis) za = Z;
+    }
+    if constexpr (kFit) {
+      const int vn = sm.rown[rl];
+      float zo = 0.f;  // z of the nearest xyz_map sample: 0 outside the frame and where the filtered depth is invalid
+      if (unc >= 0 && vn >= 0) zo = __ldg(reinterpret_cast<const float*>(FRAME(xyz_map) + (size_t)vn * FRAME(W) + unc) + 2);
+      const float d = zo - za;
+      const bool covered = key != 0ull, valid = covered && zo >= 0.001f;
+      fit_n[0] += covered;
+      fit_n[1] += valid;
+      fit_n[2] += valid && fabsf(d) <= delta;
+      fit_n[3] += valid && d < -delta;
+      fit_n[4] += valid && d > delta;
+      continue;
     }
     // ---- B: observed crop
     float br = 0.f, bg = 0.f, bb = 0.f, bx = 0.f, by = 0.f, bz = 0.f;
@@ -530,6 +564,15 @@ __global__ void __launch_bounds__(kThreads, FP_CROP_MIN_CTAS) crop_tile_kernel(c
       v[S * S] = make_float4(br, bg, bb, p.mode == 0 ? bz : zb);
     }
   }
+  if constexpr (kFit) {
+#pragma unroll
+    for (int k = 0; k < kFitCounts; ++k) {
+      const int w = __reduce_add_sync(0xffffffffu, fit_n[k]);
+      if (lane == 0 && w) atomicAdd(&sm.fit[k], w);
+    }
+    __syncthreads();
+    if (tid < kFitCounts && sm.fit[tid]) atomicAdd(p.fit + (size_t)n * kFitCounts + tid, sm.fit[tid]);
+  }
 }
 
 #undef FRAME
@@ -546,21 +589,24 @@ static int launch_tile(const CropParams& p, cudaStream_t stream) {
   const size_t smem = sizeof(TileSmem<TILE>);
   static std::atomic<unsigned long long> attr_mask{0};  // per device
   if (!device_bit_test(attr_mask)) {
-    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, false, false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, true, false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, false, true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, false, false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    FP_CUDA_OK(cudaFuncSetAttribute(crop_tile_kernel<TILE, false, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     device_bit_set(attr_mask);
   }
   const dim3 grid(TPR * TPR, p.N);
-  if (p.cams) {
-    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, false, true, false>, grid, dim3(kThreads), smem, stream, 1, p));
+  if (p.fit) {
+    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, false, true, false, true>, grid, dim3(kThreads), smem, stream, 1, p));
+  } else if (p.cams) {
+    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, false, true, false, false>, grid, dim3(kThreads), smem, stream, 1, p));
   } else if (p.stats) {
-    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, true, false, false>, grid, dim3(kThreads), smem, stream, 1, p));
+    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, true, false, false, false>, grid, dim3(kThreads), smem, stream, 1, p));
   } else if (p.vis) {
-    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, false, false, true>, grid, dim3(kThreads), smem, stream, 1, p));
+    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, false, false, true, false>, grid, dim3(kThreads), smem, stream, 1, p));
   } else {
-    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, false, false, false>, grid, dim3(kThreads), smem, stream, 1, p));
+    FP_CUDA_OK(launch_pdl(crop_tile_kernel<TILE, false, false, false, false>, grid, dim3(kThreads), smem, stream, 1, p));
   }
   return 0;
 }
@@ -570,8 +616,11 @@ int crop_launch(const CropParams& p, cudaStream_t stream) {
   FP_REQUIRE(!p.cams == !p.camera_of, "crop_launch: the camera table and the camera ids go together");
   FP_REQUIRE(!(p.cams && p.stats), "crop_launch: work counters are collected on the single-camera path only");
   FP_REQUIRE(!(p.vis && (p.cams || p.stats)), "crop_launch: the vis record is written on the single-camera path only");
-  // algorithmic bytes: the two 6-channel fp16 crops each hypothesis produces (SURVEY.md §8d)
-  prof_mark_begin(1, (double)p.N * 2.0 * 6.0 * S * S * 2.0, stream);
+  FP_REQUIRE(!p.fit == !p.fit_delta, "crop_launch: the fit counts and their threshold go together");
+  FP_REQUIRE(!p.fit || (p.cams && p.mode == 0 && !p.dbg && !p.win_out),
+             "crop_launch: the fit pass runs on the camera-table path, in the refiner's window, and writes only its counts");
+  // algorithmic bytes: the two 6-channel fp16 crops each hypothesis produces (SURVEY.md §8d); the fit pass stores none
+  prof_mark_begin(1, p.fit ? 0.0 : (double)p.N * 2.0 * 6.0 * S * S * 2.0, stream);
   int tile = p.N >= 64 ? 80 : (p.N >= 4 ? 32 : 16);
   if (g_crop_tile_override) tile = g_crop_tile_override;
   if (p.tile_override == 16 || p.tile_override == 32 || p.tile_override == 80) tile = p.tile_override;

@@ -92,7 +92,13 @@ struct CropParams {
   // crops hold (0..1) and one depth value — mode 0 the normalised z of the xyz channels, mode 1 the raw depth in metres
   // (A: rendered camera z, 0 where nothing is covered; B: the nearest sample of the filtered depth, predict_score.py:90)
   float4* vis;
+  // optional, camera-table path only (the tracking calls' fit pass, mode 0): no crop, dbg or vis record is written;
+  // instead every hypothesis adds its kFitCounts agreement counts of rendered and observed depth at threshold
+  // *fit_delta (device, metres) to fit[n][kFitCounts], which the caller zeroes first.  Both null or both set.
+  int* fit;
+  const float* fit_delta;
 };
+constexpr int kFitCounts = 5;  // FP_FIT_COUNTS (include/fpose.h): covered, valid, inlier, occluded, behind
 
 int crop_launch(const CropParams& p, cudaStream_t stream);
 int rgb_to_rgba_launch(const unsigned char* rgb, uchar4* out, int npix, cudaStream_t stream);

@@ -138,6 +138,7 @@ inline int b_img0_of(int N) { return (N + 3) & ~3; }
 
 static_assert(kMaxMeshes == FP_MAX_MESHES, "fp_crop.cuh and fpose.h disagree on the number of mesh slots");
 static_assert(kMaxCameras == FP_MAX_CAMERAS, "fp_crop.cuh and fpose.h disagree on the number of cameras");
+static_assert(kFitCounts == FP_FIT_COUNTS, "fp_crop.cuh and fpose.h disagree on the number of fit counts");
 
 // One mesh of the context (fp_meshlet.cu layout).  Slot 0 is the mesh of every single-object entry point.
 struct MeshSlot {
@@ -173,14 +174,16 @@ struct StagingSet {
   bool busy = false;
 };
 
-// The pose read-back of one submitted tracking call: pinned [M][16] poses, complete once `done` has passed.  Owned by
-// the call's ticket until fp_track_wait collects it (ticket 0: free for the next submit).  A call's read-back outlives
-// its staging set, which the call after next may reuse before this result is collected.
+// The pose read-back of one submitted tracking call: pinned [M][16] poses, and with a fit (fp_track_cameras_fit_submit)
+// its [M][FP_FIT_COUNTS] counts, complete once `done` has passed.  Owned by the call's ticket until fp_track_wait or
+// fp_track_fit_wait collects it (ticket 0: free for the next submit).  A call's read-back outlives its staging set, which
+// the call after next may reuse before this result is collected.
 struct Readback {
-  PinnedBuf poses;
+  PinnedBuf poses, fit;
   OwnedEvent done;
   unsigned long long ticket = 0;
   int M = 0;
+  bool has_fit = false;
 };
 
 }  // namespace fp
@@ -240,8 +243,10 @@ struct fp_ctx {
   cudaStream_t last_stream = nullptr;
   cudaEvent_t last_done = nullptr;  // the last call's Readback::done (a Readback is reused only by a later call)
   // the arguments of a multi-object call or register pass, one device block at a fixed address (a graph holds it),
-  // staged through a StagingSet: the camera table (CameraDev [FP_MAX_CAMERAS]), the slot ids [n], the camera ids [n]
+  // staged through a StagingSet: the camera table (CameraDev [FP_MAX_CAMERAS]), the slot ids [n], the camera ids [n],
+  // and for a tracking call with a fit its threshold (one float)
   fp::DevBuf args;
+  fp::DevBuf fit;  // the fit counts of the last tracking call with a fit, [M][FP_FIT_COUNTS] int32 (a graph holds it)
   int cam_grid_h = 0, cam_grid_w = 0;  // the tracking calls' frame-preparation grid: the largest frame seen
   // fp_register_objects / _cameras: row offsets of the objects' hypotheses [M + 1] and the objects' camera ids [M], the
   // objects' feature rows [sum N][512], each object's byte offset into mask_buf

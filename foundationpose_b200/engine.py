@@ -42,6 +42,9 @@ def _proto():
     lib.fp_track_cameras_submit.argtypes = [vp, i, C.POINTER(vp), C.POINTER(vp), C.POINTER(f), C.POINTER(i), C.POINTER(i), i,
                                             C.POINTER(i), C.POINTER(i), vp, i, vp, vp, C.POINTER(C.c_ulonglong)]
     lib.fp_track_wait.argtypes = [vp, C.c_ulonglong, vp]
+    lib.fp_track_cameras_fit_submit.argtypes = [vp, i, C.POINTER(vp), C.POINTER(vp), C.POINTER(f), C.POINTER(i), C.POINTER(i), i,
+                                                C.POINTER(i), C.POINTER(i), vp, i, f, vp, vp, vp, C.POINTER(C.c_ulonglong)]
+    lib.fp_track_fit_wait.argtypes = [vp, C.c_ulonglong, vp, vp]
     lib.fp_graph_captures.argtypes = [vp]
     lib.fp_graph_captures.restype = C.c_ulonglong
     lib.fp_load_network.argtypes = [vp, i, C.POINTER(_FpTensor), i]
@@ -74,7 +77,7 @@ def _proto():
     lib.fp_vis_workspace_bytes.argtypes = [vp]
     lib.fp_vis_workspace_bytes.restype = C.c_ulonglong
     for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_track_cameras", "fp_track_submit", "fp_track_objects_submit",
-                 "fp_track_cameras_submit", "fp_track_wait", "fp_register_objects", "fp_register_cameras", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh",
+                 "fp_track_cameras_submit", "fp_track_wait", "fp_track_cameras_fit_submit", "fp_track_fit_wait", "fp_register_objects", "fp_register_cameras", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh",
                  "fp_set_mesh_slot", "fp_set_frame",
                  "fp_get_depth", "fp_make_crops", "fp_start_poses", "fp_refine", "fp_score", "fp_score_features", "fp_score_tail",
                  "fp_op_score_tail_segments", "fp_register", "fp_op_refine_net", "fp_op_score_feats", "fp_op_encoder_layer", "fp_op_depth_filter",
@@ -88,6 +91,7 @@ FRAME_ON_DEVICE = 1
 MAX_MESHES = 64  # FP_MAX_MESHES: mesh slots per context
 MAX_CAMERAS = 16  # FP_MAX_CAMERAS: camera streams per fp_track_cameras / fp_register_cameras call
 MAX_IN_FLIGHT = 2  # FP_TRACK_MAX_IN_FLIGHT: tracking calls in flight per context (its staging sets)
+FIT_COUNTS = 5  # FP_FIT_COUNTS: covered, valid, inlier, occluded, behind
 FRAME_FILTER_DEPTH = 2
 
 
@@ -260,20 +264,25 @@ def _mesh_args(vertices, normals, faces, uv=None, tex=None, vertex_colors=None):
 
 class PendingPoses:
     """The host poses of one tracking call submitted with wait=False.  result() waits for the call's read-back (once; later
-    calls return the same array) and returns what the blocking call returns as its host poses.  A handle dropped without
-    result() is collected by its engine at a later submit or at close, so its ticket never leaks.  It holds the call's
-    device frames until result() has collected the call."""
+    calls return the same result) and returns what the blocking call returns as its host poses: the poses array, or for a
+    call with a fit (track_cameras(..., fit_delta=)) the tuple (poses, fit counts (M, FIT_COUNTS) int32).  A handle
+    dropped without result() is collected by its engine at a later submit or at close, so its ticket never leaks.  It
+    holds the call's device frames until result() has collected the call."""
 
-    def __init__(self, engine, ticket, shape, held=()):
+    def __init__(self, engine, ticket, shape, held=(), fit=False):
         self._engine, self.ticket, self._shape, self._host, self._held = engine, ticket, shape, None, list(held)
+        self._fit = fit
         self._dropped = weakref.finalize(self, engine._dropped.append, ticket)
 
     def result(self):
         if self._host is None:
             self._dropped.detach()
             host = np.empty(self._shape, dtype=np.float32)
-            self._engine._wait(self.ticket, host)
-            self._host = host
+            if self._fit:
+                self._host = (host, self._engine._wait_fit(self.ticket, host))
+            else:
+                self._engine._wait(self.ticket, host)
+                self._host = host
             self._held = []
         return self._host
 
@@ -352,9 +361,10 @@ class Engine:
             self._dropped.remove(t)
             _lib.check(lib.fp_track_wait(self._h, t, None), "fp_track_wait")
 
-    def _submit(self, fn, args, what, out, shape, wait, bufs=()):
+    def _submit(self, fn, args, what, out, shape, wait, bufs=(), fit=False):
         """Submits one tracking call (`fn(ctx, *args, stream, &ticket)`) on the frame buffers `bufs`.  Returns (out, host
-        poses) with wait, else (out, PendingPoses), which holds the device buffers among `bufs` until it is collected."""
+        poses) with wait, else (out, PendingPoses), which holds the device buffers among `bufs` until it is collected.
+        fit: a call with a fit, whose host result is (poses, counts)."""
         if not getattr(self, "_h", None):
             raise _lib.FposeError(f"{what}: the engine is closed")
         self._collect_dropped(MAX_IN_FLIGHT)
@@ -362,8 +372,10 @@ class Engine:
         _lib.check(fn(self._h, *args, _stream(), C.byref(ticket)), what)
         self._last_ticket = ticket.value
         if not wait:
-            return out, PendingPoses(self, ticket.value, shape, _hold(bufs))
+            return out, PendingPoses(self, ticket.value, shape, _hold(bufs), fit)
         host = np.empty(shape, dtype=np.float32)
+        if fit:
+            return out, (host, self._wait_fit(ticket.value, host))
         self._wait(ticket.value, host)
         return out, host
 
@@ -371,6 +383,15 @@ class Engine:
         if not getattr(self, "_h", None):
             raise _lib.FposeError("fp_track_wait: the engine is closed")
         _lib.check(lib.fp_track_wait(self._h, ticket, C.c_void_p(host.ctypes.data)), "fp_track_wait")
+
+    def _wait_fit(self, ticket, host):
+        """fp_track_fit_wait: the poses into `host` (M,4,4); returns the counts (M, FIT_COUNTS) int32."""
+        if not getattr(self, "_h", None):
+            raise _lib.FposeError("fp_track_fit_wait: the engine is closed")
+        counts = np.empty((host.shape[0], FIT_COUNTS), dtype=np.int32)
+        _lib.check(lib.fp_track_fit_wait(self._h, ticket, C.c_void_p(host.ctypes.data), C.c_void_p(counts.ctypes.data)),
+                   "fp_track_fit_wait")
+        return counts
 
     def track(self, rgb, depth, K, pose_in, iterations, pose_out=None, wait=True):
         """fp_track: one CUDA-graph launch per frame (upload + depth filters + xyz map + refiner passes + read-back).
@@ -408,12 +429,17 @@ class Engine:
         self.frame_hw = (H, W)
         return res
 
-    def track_cameras(self, frames, poses_in, camera_of, slots, iterations, wait=True):
+    def track_cameras(self, frames, poses_in, camera_of, slots, iterations, wait=True, fit_delta=None):
         """fp_track_cameras: `track_objects` for M objects spread over C camera streams in ONE CUDA-graph launch.  frames: C
         tuples (rgb uint8 (H,W,3), depth float32 (H,W), K (3,3)), one per camera, each with its own size and intrinsics and
         each buffer a host array or a CUDA tensor, as `track` (one call may mix them); object i is seen by camera
         camera_of[i] and renders the mesh in slot slots[i]; poses_in (M,4,4) CUDA tensor.  Returns (poses CUDA (M,4,4),
-        poses host (M,4,4) float32 numpy); wait=False as `track`."""
+        poses host (M,4,4) float32 numpy); wait=False as `track`.
+
+        fit_delta (metres): also count, in the same launch, how well each returned pose's rendered depth agrees with the
+        observed depth (fp_track_cameras_fit_submit, include/fpose.h): returns (poses CUDA, poses host, fit) with fit an
+        int32 (M, FIT_COUNTS) numpy array of (covered, valid, inlier, occluded, behind) pixels; wait=False returns
+        (poses CUDA, PendingPoses) whose result() gives (poses host, fit).  The poses are those of the call without it."""
         frames = [(*_frame(rgb, depth, f"track_cameras: camera {c}")[:2], K) for c, (rgb, depth, K) in enumerate(frames)]
         n_cam = len(frames)
         poses_in = poses_in.reshape(-1, 4, 4).contiguous().float()
@@ -423,9 +449,15 @@ class Engine:
             raise ValueError(f"track_cameras: {M} poses, {len(camera_of)} camera ids and {len(slots)} slots")
         rgbs, depths, Ks, Hs, Ws = _camera_args(frames)
         out = torch.empty(M, 4, 4, dtype=torch.float32, device="cuda")
-        res = self._submit(lib.fp_track_cameras_submit, (n_cam, rgbs, depths, Ks, Hs, Ws, M, (C.c_int * M)(*camera_of),
-                                                         (C.c_int * M)(*slots), _p(poses_in), int(iterations), _p(out)),
-                           "fp_track_cameras", out, (M, 4, 4), wait, [b for rgb, depth, _ in frames for b in (rgb, depth)])
+        ids = (n_cam, rgbs, depths, Ks, Hs, Ws, M, (C.c_int * M)(*camera_of), (C.c_int * M)(*slots), _p(poses_in), int(iterations))
+        bufs = [b for rgb, depth, _ in frames for b in (rgb, depth)]
+        if fit_delta is None:
+            res = self._submit(lib.fp_track_cameras_submit, (*ids, _p(out)), "fp_track_cameras", out, (M, 4, 4), wait, bufs)
+        else:
+            res = self._submit(lib.fp_track_cameras_fit_submit, (*ids, float(fit_delta), _p(out), None), "fp_track_cameras_fit",
+                               out, (M, 4, 4), wait, bufs, fit=True)
+            if wait:
+                res = (res[0], *res[1])
         self.frame_hw = tuple(frames[0][1].shape)  # camera 0's frame is the context's frame
         return res
 

@@ -14,6 +14,7 @@ to debug_dir, and track_one() at debug >= 2 puts the refiner canvas in extra['vi
 per-call `mesh` / `mesh_tensors` / `mesh_diameter` / `xyz_map` arguments of the reference: a mesh that is not
 the one already in the context is uploaded first, a caller-supplied xyz map replaces the derived one.
 """
+import dataclasses
 import logging
 import os
 import weakref
@@ -23,6 +24,43 @@ import torch
 
 from . import hypotheses, meshprep, synth, weights
 from .engine import MAX_CAMERAS, MAX_MESHES, Engine
+
+
+@dataclasses.dataclass(frozen=True)
+class PoseFit:
+    """How well a tracked pose's rendered depth agrees with the observed depth, over the refiner's 160 x 160 crop window at
+    the returned pose (FP_FIT_COUNTS, include/fpose.h): pixels the mesh covers, those of them with a valid observed depth,
+    and the valid ones whose observed depth lies within delta of the rendered one (inlier), more than delta in front of
+    it (occluded: something hides the object) or more than delta behind it (behind: the camera sees through where the
+    object should be, the signature of a lost track).  inlier + occluded + behind == valid.
+
+    The ratios are 0.0 when their denominator is 0, so `ratio < threshold` also fires for an object that left the view."""
+
+    covered: int
+    valid: int
+    inlier: int
+    occluded: int
+    behind: int
+
+    @classmethod
+    def from_counts(cls, counts):
+        return cls(*(int(c) for c in counts))
+
+    @staticmethod
+    def _ratio(a, b):
+        return a / b if b else 0.0
+
+    @property
+    def inlier_ratio(self):
+        return self._ratio(self.inlier, self.valid)
+
+    @property
+    def behind_ratio(self):
+        return self._ratio(self.behind, self.valid)
+
+    @property
+    def visible_ratio(self):
+        return self._ratio(self.valid, self.covered)
 
 
 class _Cfg(dict):
@@ -219,6 +257,7 @@ class FoundationPose:
         self.scorer = scorer if scorer is not None else ScorePredictor(engine=self.engine)
         self.refiner = refiner if refiner is not None else PoseRefinePredictor(engine=self.engine)
         self.pose_last = None  # used for tracking; per the centred mesh
+        self.fit_last = None  # PoseFit of the last tracking call made with a fit_delta
         # True: read (tx, ty, tz, n_valid) back before the 252 x K loop so that an empty / depth-less mask returns
         # without running it (the reference's control flow, one extra sync); False: sync-free, the loop runs and its
         # result is discarded in that case
@@ -367,12 +406,26 @@ class FoundationPose:
         pcd.colors = o3d.utility.Vector3dVector(rgb[valid].astype(np.float64) / 255.0)
         o3d.io.write_point_cloud(f"{self.debug_dir}/{name}", pcd)
 
-    def track_one(self, rgb, depth, K, iteration, extra={}):
+    def track_one(self, rgb, depth, K, iteration, extra={}, fit_delta=None):
+        """estimater.py:250-268.  fit_delta (metres): also measure how well the returned pose fits the frame's depth, in
+        the same launch, into self.fit_last (a PoseFit); host and device frames then both go through one
+        fp_track_cameras_fit call, which returns the same pose as the call without it."""
         if self.pose_last is None:
             logging.info("Please init pose by register first")
             raise RuntimeError
         e = self.engine
         _sync_mesh(e, self.mesh, self.mesh_tensors, self.diameter)
+        if fit_delta is not None:
+            pose_in = self.pose_last.reshape(1, 4, 4)
+            pose_dev, pose_host, fit = e.track_cameras([(rgb, depth, K)], pose_in, [0], [0], iteration, fit_delta=fit_delta)
+            self.fit_last = PoseFit.from_counts(fit[0])
+            if self.debug >= 2:
+                from . import vis  # cv2: only the debug canvases need it
+
+                extra["vis"] = vis.refine_canvas(e, pose_in, pose_dev)
+            self.pose_last = pose_dev.reshape(1, 4, 4)
+            self.refiner.last_trans_update = self.refiner.last_rot_update = None
+            return _uncentre(pose_host[0], self.model_center)
         if torch.is_tensor(rgb) or torch.is_tensor(depth):
             # device-resident frame: enqueue the stages one by one (estimater.py:255-264)
             e.set_frame(rgb, depth, K, filter_depth=True, zfar=float("inf"))
@@ -455,7 +508,12 @@ class PendingTrack:
         return self._out
 
 
-def track_objects(estimators, rgb, depth, K, iteration=2, wait=True):
+def _set_fit(estimators, fit):
+    for est, row in zip(estimators, fit):
+        est.fit_last = PoseFit.from_counts(row)
+
+
+def track_objects(estimators, rgb, depth, K, iteration=2, wait=True, fit_delta=None):
     """`[est.track_one(rgb, depth, K, iteration) for est in estimators]` for several objects of one camera stream, as ONE
     CUDA-graph launch per frame (fp_track_objects): the frame is uploaded and filtered once and the objects' poses are
     refined as one batch, each rendering its own mesh.  Same poses as the per-object calls; updates every pose_last.
@@ -464,7 +522,10 @@ def track_objects(estimators, rgb, depth, K, iteration=2, wait=True):
     so alternating objects re-uploads nothing.  Host frames only (uint8 (H,W,3) rgb, float32 (H,W) depth).
     Returns a list of (4,4) float32 poses of the original meshes.  wait=False returns a PendingTrack as soon as the call
     is submitted (the frame arrays may then be reused) with every pose_last already set, so the next frame can be
-    submitted while the device tracks this one."""
+    submitted while the device tracks this one.
+
+    fit_delta (metres): also measure, in the same launch, how well each returned pose fits the frame's depth: each
+    estimator's fit_last receives its PoseFit (with wait=False, when result() collects the call).  Same poses."""
     estimators = list(estimators)
     if not estimators:
         return [] if wait else PendingTrack(None, lambda _: [])
@@ -476,6 +537,10 @@ def track_objects(estimators, rgb, depth, K, iteration=2, wait=True):
         raise RuntimeError
     slots = [_object_slot(est) for est in estimators]
     poses_in = torch.stack([est.pose_last.reshape(4, 4) for est in estimators])
+    if fit_delta is not None:
+        # fp_track_objects is fp_track_cameras with one camera: the fit goes through the camera call, same poses
+        return _track_fit(estimators, [(rgb, depth, K)], poses_in, [0] * len(estimators), slots, iteration, wait, fit_delta,
+                          lambda flat: flat)
     if wait:
         poses_dev, poses_host = e.track_objects(rgb, depth, K, poses_in, slots, iteration)
     else:
@@ -488,7 +553,26 @@ def track_objects(estimators, rgb, depth, K, iteration=2, wait=True):
     return finish(poses_host) if wait else PendingTrack(pending, finish)
 
 
-def track_cameras(views, iteration=2, wait=True):
+def _track_fit(estimators, frames, poses_in, camera_of, slots, iteration, wait, fit_delta, group):
+    """track_objects / track_cameras with a fit: one Engine.track_cameras call, every pose_last set at submit, every
+    fit_last set when the counts are collected.  group: the flat list of un-centred poses -> the caller's result."""
+    e = estimators[0].engine
+    res = e.track_cameras(frames, poses_in, camera_of, slots, iteration, wait=wait, fit_delta=fit_delta)
+    poses_dev = res[0]
+    for i, est in enumerate(estimators):
+        est.pose_last = poses_dev[i].reshape(1, 4, 4)
+        est.refiner.last_trans_update = est.refiner.last_rot_update = None
+    centers = [est.model_center for est in estimators]
+
+    def finish(host_fit):
+        host, fit = host_fit
+        _set_fit(estimators, fit)
+        return group([_uncentre(host[i], c) for i, c in enumerate(centers)])
+
+    return finish(res[1:]) if wait else PendingTrack(res[1], finish)
+
+
+def track_cameras(views, iteration=2, wait=True, fit_delta=None):
     """`[[est.track_one(rgb, depth, K, iteration) for est in ests] for ests, rgb, depth, K in views]` for objects seen by
     several camera streams (a multi-camera rig, or several recordings on one GPU), as ONE CUDA-graph launch per call
     (fp_track_cameras): every camera's frame is uploaded and filtered, and every (object, camera) pair is refined in one
@@ -500,7 +584,7 @@ def track_cameras(views, iteration=2, wait=True):
     MAX_CAMERAS cameras with objects.  A camera without estimators gives [] and its frame is not uploaded.  Each
     estimator keeps its mesh in the slot track_objects / register_objects use.  Host frames only (uint8 (H,W,3) rgb,
     float32 (H,W) depth).  Returns one list of (4,4) float32 poses of the original meshes per camera.  wait=False returns
-    a PendingTrack as track_objects does."""
+    a PendingTrack as track_objects does; fit_delta sets every estimator's fit_last as track_objects does."""
     views = [(list(ests), rgb, depth, K) for ests, rgb, depth, K in views]
     if any(torch.is_tensor(rgb) or torch.is_tensor(depth) for _, rgb, depth, _ in views):
         raise TypeError("track_cameras takes host frames (numpy); for device-resident frames call track_one per object")
@@ -519,6 +603,14 @@ def track_cameras(views, iteration=2, wait=True):
     camera_of = [c for c, (ests, _, _, _) in enumerate(used) for _ in ests]
     poses_in = torch.stack([est.pose_last.reshape(4, 4) for est in estimators])
     frames = [(rgb, depth, K) for _, rgb, depth, K in used]
+    counts = [len(ests) for ests, _, _, _ in views]
+
+    def group(flat):
+        flat = iter(flat)
+        return [[next(flat) for _ in range(n)] for n in counts]
+
+    if fit_delta is not None:
+        return _track_fit(estimators, frames, poses_in, camera_of, slots, iteration, wait, fit_delta, group)
     if wait:
         poses_dev, poses_host = e.track_cameras(frames, poses_in, camera_of, slots, iteration)
     else:
@@ -527,11 +619,9 @@ def track_cameras(views, iteration=2, wait=True):
         est.pose_last = poses_dev[i].reshape(1, 4, 4)
         est.refiner.last_trans_update = est.refiner.last_rot_update = None
     centers = [est.model_center for est in estimators]
-    counts = [len(ests) for ests, _, _, _ in views]
 
     def finish(host):
-        flat = iter(_uncentre(host[i], c) for i, c in enumerate(centers))
-        return [[next(flat) for _ in range(n)] for n in counts]
+        return group(_uncentre(host[i], c) for i, c in enumerate(centers))
 
     return finish(poses_host) if wait else PendingTrack(pending, finish)
 

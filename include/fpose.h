@@ -369,6 +369,33 @@ int fp_track_objects_submit(fp_ctx* ctx, const unsigned char* rgb, const float* 
 int fp_track_submit(fp_ctx* ctx, const unsigned char* rgb, const float* depth, const float* K, int H, int W,
                     const float* pose_in_dev, int iterations, float* pose_out_dev, void* stream, unsigned long long* ticket);
 int fp_track_wait(fp_ctx* ctx, unsigned long long ticket, float* poses_out_host);
+/* Tracking health: how well each returned pose's rendered depth agrees with the observed depth, counted in the same
+ * graph launch and read back with the poses.  For object i, at its OUTPUT pose, over the 160 x 160 pixels p of the
+ * refiner's crop window (the refiner's crop_ratio, the object's camera and mesh slot): z_r(p) is the camera-space Z of
+ * the mesh's nearest triangle at p (what the refiner's rendered crop normalises), z_o(p) the z of the nearest xyz-map
+ * sample of the filtered depth the refiner's observed crop reads at p (0 outside the frame or where the depth is
+ * invalid), d = z_o - z_r in fp32.  The counts, int32 [M][FP_FIT_COUNTS]:
+ *   [0] covered   the mesh covers p
+ *   [1] valid     covered and z_o >= 0.001
+ *   [2] inlier    valid and |d| <= delta
+ *   [3] occluded  valid and d < -delta: something is in front of the model (occlusion, not failure)
+ *   [4] behind    valid and d > delta: the camera sees past the model's surface (free space violated: a lost track)
+ * so inlier + occluded + behind = valid.  The rendered and observed windows differ by the refiner's 159/160 scale; the
+ * counts compare the same crop pixel on both sides, as the refiner does.  Integer counts: they do not depend on the
+ * number or order of objects and cameras, nor on the crop tile.  The poses are exactly those of the call without a fit. */
+#define FP_FIT_COUNTS 5
+/* fp_track_cameras_submit plus the counts above at every output pose.  delta: metres, finite and >= 0 (checked with the
+ * other arguments: a refused call enqueues nothing).  fit_out_dev: optional DEVICE int32 [M][5], complete in stream
+ * order.  delta travels with the slot and camera ids, so a new delta replays the cached graph.  A fit ticket may be
+ * collected with fp_track_wait, which drops its counts. */
+int fp_track_cameras_fit_submit(fp_ctx* ctx, int C, const unsigned char* const* rgb, const float* const* depth,
+                                const float* K, const int* H, const int* W, int M, const int* camera_of,
+                                const int* slots_host, const float* poses_in_dev, int iterations, float delta,
+                                float* poses_out_dev, int* fit_out_dev, void* stream, unsigned long long* ticket);
+/* fp_track_wait for a ticket of fp_track_cameras_fit_submit, also copying its counts to fit_out_host (HOST int32
+ * [M][5], may be NULL).  A ticket submitted without a fit is refused and left uncollected: fp_track_wait still collects
+ * it. */
+int fp_track_fit_wait(fp_ctx* ctx, unsigned long long ticket, float* poses_out_host, int* fit_out_host);
 /* FoundationPose.register (estimater.py:159-240) applied to M objects of the same frame in one call; object i gives
  * exactly what fp_set_frame + fp_start_poses + fp_refine + fp_score give for that object alone, bit for bit.
  *   1. Checks every argument before anything is enqueued: slots_host HOST [M] loaded slot ids (one slot may appear
