@@ -197,34 +197,102 @@ static int run_graphed(fp_ctx* c, GraphKind kind, int N, int iters, cudaStream_t
   return 0;
 }
 
-// camera 0's filtered frame from rgb_dev / depth_dev, with camera 0's record by value (fp_set_frame, fp_register_objects)
-static int set_frame_launches(fp_ctx* c, const unsigned char* rgb_dev, const float* depth_dev, int flags, float zfar,
-                              cudaStream_t st) {
+// camera 0's filtered frame from rgb_dev / depth_dev in format fmt, with camera 0's record by value (fp_set_frame,
+// fp_register_objects)
+static int set_frame_launches(fp_ctx* c, const unsigned char* rgb_dev, const float* depth_dev, const FrameFmtDev& fmt,
+                              int flags, float zfar, cudaStream_t st) {
   CameraDev one = camera_dev(c, 0);
   one.rgb_raw = rgb_dev;  // camera 0's upload buffers, or the caller's device frame (FP_FRAME_ON_DEVICE)
   one.depth_raw = depth_dev;
   if (flags & FP_FRAME_FILTER_DEPTH) {
     // estimater.py:173-174 erode_depth(radius=2), bilateral_filter_depth(radius=2); :214 depth2xyzmap: one launch
-    return frame_prep_launch(one, zfar, st);
+    return frame_prep_launch(one, fmt, zfar, st);
   }
   const size_t npix = (size_t)one.H * one.W;
-  FP_TRY(rgb_to_rgba_launch(rgb_dev, one.rgb, (int)npix, st));
-  FP_CUDA_OK(cudaMemcpyAsync(one.depth, depth_dev, npix * 4, cudaMemcpyDeviceToDevice, st));
+  // packed float32 depth is copied as it is; any other depth is converted by the colour kernel
+  const bool depth_as_is = !fmt.u16 && (size_t)fmt.depth_pitch == (size_t)one.W * 4;
+  FP_TRY(raw_frame_launch(one, fmt, !depth_as_is, st));
+  if (depth_as_is) FP_CUDA_OK(cudaMemcpyAsync(one.depth, depth_dev, npix * 4, cudaMemcpyDeviceToDevice, st));
   return depth_to_xyz_launch(one, zfar, st);
+}
+
+// A camera's raw frame of width W in format f: the one place that knows its bytes per pixel, row bytes and pitches.
+struct FrameLayout {
+  int rgb_bpp, depth_bpp;          // bytes per pixel
+  size_t rgb_row, depth_row;       // bytes per packed row
+  long long rgb_pitch, depth_pitch;  // bytes from one row of the caller's buffer to the next
+};
+static FrameLayout frame_layout(const fp_frame_format_t& f, int W) {
+  FrameLayout L;
+  L.rgb_bpp = (f.color == FP_COLOR_RGBA8 || f.color == FP_COLOR_BGRA8) ? 4 : 3;
+  L.depth_bpp = f.depth == FP_DEPTH_U16 ? 2 : 4;
+  L.rgb_row = (size_t)W * L.rgb_bpp;
+  L.depth_row = (size_t)W * L.depth_bpp;
+  L.rgb_pitch = f.rgb_pitch ? f.rgb_pitch : (long long)L.rgb_row;
+  L.depth_pitch = f.depth_pitch ? f.depth_pitch : (long long)L.depth_row;
+  return L;
+}
+
+// The kernels' record of a raw frame in format f: read in place with the caller's pitches, or from the context's upload
+// buffers, where it was staged packed
+static FrameFmtDev fmt_dev(const fp_frame_format_t& f, const FrameLayout& L, bool rgb_in_place, bool depth_in_place) {
+  FrameFmtDev d;
+  memset(&d, 0, sizeof d);
+  d.rgb_pitch = (int)(rgb_in_place ? L.rgb_pitch : (long long)L.rgb_row);
+  d.depth_pitch = (int)(depth_in_place ? L.depth_pitch : (long long)L.depth_row);
+  d.depth_scale = f.depth == FP_DEPTH_U16 ? f.depth_scale : 0.f;
+  d.bpp = (unsigned char)L.rgb_bpp;
+  d.bgr = (f.color == FP_COLOR_BGR8 || f.color == FP_COLOR_BGRA8) ? 1 : 0;
+  d.u16 = f.depth == FP_DEPTH_U16 ? 1 : 0;
+  d.packed = (d.bpp == 3 && !d.bgr && !d.u16 && (size_t)d.rgb_pitch == L.rgb_row && (size_t)d.depth_pitch == L.depth_row) ? 1 : 0;
+  return d;
+}
+
+// Camera i's frame (depth buffer `depth`, width W) against camera i's format: pitches no shorter than a packed row, the
+// depth pitch and pointer aligned to the depth element.  Checked before anything is enqueued.
+static int check_frame_format(const fp_ctx* c, int i, const void* depth, int W, const char* caller) {
+  const fp_frame_format_t& f = c->fmt[i];
+  const FrameLayout L = frame_layout(f, W);
+  FP_REQUIRE(L.rgb_pitch >= (long long)L.rgb_row, "%s: camera %d: rgb pitch %lld bytes is below the %zu bytes of a row", caller,
+             i, L.rgb_pitch, L.rgb_row);
+  FP_REQUIRE(L.depth_pitch >= (long long)L.depth_row, "%s: camera %d: depth pitch %lld bytes is below the %zu bytes of a row",
+             caller, i, L.depth_pitch, L.depth_row);
+  FP_REQUIRE(L.depth_pitch % L.depth_bpp == 0, "%s: camera %d: depth pitch %lld bytes is not a multiple of the %d-byte depth value",
+             caller, i, L.depth_pitch, L.depth_bpp);
+  FP_REQUIRE(reinterpret_cast<uintptr_t>(depth) % L.depth_bpp == 0,
+             "%s: camera %d: depth buffer %p is not aligned to its %d-byte depth value", caller, i, depth, L.depth_bpp);
+  return 0;
+}
+static int check_frame_formats(const fp_ctx* c, int C, const float* const* depth, const int* W, const char* caller) {
+  for (int i = 0; i < C; ++i) FP_TRY(check_frame_format(c, i, depth[i], W[i], caller));
+  return 0;
+}
+
+// Copies `rows` host rows of `row` bytes, `pitch` bytes apart at `src`, into `dst` (device) on `st`: one copy when the
+// rows are packed, a 2D copy otherwise
+static int copy_rows(void* dst, const void* src, size_t row, long long pitch, int rows, cudaStream_t st) {
+  if (pitch == (long long)row) {
+    FP_CUDA_OK(cudaMemcpyAsync(dst, src, row * rows, cudaMemcpyHostToDevice, st));
+  } else {
+    FP_CUDA_OK(cudaMemcpy2DAsync(dst, row, src, (size_t)pitch, row, rows, cudaMemcpyHostToDevice, st));
+  }
+  return 0;
 }
 
 // Sizes camera i's buffers for npix pixels: the filtered frame always, the raw upload if `raw`.  Camera 0's addresses
 // are held by the graphs that take the frame by value, so growing its buffers bumps the graph epoch.  Cameras 1.. are
 // reached only through the camera table, which every call rewrites: growing them invalidates no graph.
-static int alloc_camera(fp_ctx* c, int i, size_t npix, bool raw) {
+// The raw upload holds rgb_bpp / depth_bpp bytes per pixel (the frame format's); buffers only grow, so a camera that
+// alternates between formats of a size it has seen allocates nothing after the first time.
+static int alloc_camera(fp_ctx* c, int i, size_t npix, bool raw, int rgb_bpp = 3, int depth_bpp = 4) {
   CameraBufs& b = c->cam[i];
   unsigned long long* epoch = i == 0 ? &c->epoch : nullptr;
   FP_TRY(dev_alloc(epoch, b.rgba, npix * 4));
   FP_TRY(dev_alloc(epoch, b.depth, npix * 4));
   FP_TRY(dev_alloc(epoch, b.xyz, npix * 16));
   if (raw) {
-    FP_TRY(dev_alloc(epoch, b.rgb_raw, npix * 3));
-    FP_TRY(dev_alloc(epoch, b.depth_raw, npix * 4));
+    FP_TRY(dev_alloc(epoch, b.rgb_raw, npix * rgb_bpp));
+    FP_TRY(dev_alloc(epoch, b.depth_raw, npix * depth_bpp));
   }
   return 0;
 }
@@ -265,20 +333,30 @@ static int refine_body(fp_ctx* c, int N, int iterations, cudaStream_t s2, const 
 
 // Copies `bytes` of host memory `src` into the pinned `stage` (grown as needed) and enqueues its upload to `dst`: the
 // caller's memory is free again once this returns.
-static int stage_copy(void* dst, PinnedBuf& stage, const void* src, size_t bytes, cudaStream_t st) {
+// The same for `rows` rows of `row` bytes, `pitch` bytes apart at `src`: staged packed, in one copy when they are packed.
+static int stage_rows(void* dst, PinnedBuf& stage, const void* src, size_t row, long long pitch, int rows, cudaStream_t st) {
+  const size_t bytes = row * rows;
   FP_TRY(pinned_alloc(nullptr, stage, bytes));
-  memcpy(stage.p, src, bytes);
+  if (pitch == (long long)row) {
+    memcpy(stage.p, src, bytes);
+  } else {
+    for (int r = 0; r < rows; ++r)
+      memcpy(static_cast<char*>(stage.p) + r * row, static_cast<const char*>(src) + r * pitch, row);
+  }
   FP_CUDA_OK(cudaMemcpyAsync(dst, stage.p, bytes, cudaMemcpyHostToDevice, st));
   return 0;
 }
+static int stage_copy(void* dst, PinnedBuf& stage, const void* src, size_t bytes, cudaStream_t st) {
+  return stage_rows(dst, stage, src, bytes, (long long)bytes, 1, st);
+}
 
-// Uploads one camera's frame through its staging (free: the set is not busy).  The two uploads are issued as soon as
-// their staging copy is done — the depth DMA runs under the host's rgb copy, the rgb DMA under the next camera's copies
-// or the graph launch — instead of being nodes of the graph (measured: -40 us per frame)
+// Uploads one camera's frame (H rows of layout L) through its staging (free: the set is not busy).  The two uploads are
+// issued as soon as their staging copy is done — the depth DMA runs under the host's rgb copy, the rgb DMA under the
+// next camera's copies or the graph launch — instead of being nodes of the graph (measured: -40 us per frame)
 static int upload_staged_frame(CameraBufs& b, PinnedBuf& stage_rgb, PinnedBuf& stage_depth, const unsigned char* rgb_host,
-                               const float* depth_host, size_t npix, cudaStream_t st) {
-  FP_TRY(stage_copy(b.depth_raw.p, stage_depth, depth_host, npix * 4, st));
-  return stage_copy(b.rgb_raw.p, stage_rgb, rgb_host, npix * 3, st);
+                               const void* depth_host, const FrameLayout& L, int H, cudaStream_t st) {
+  FP_TRY(stage_rows(b.depth_raw.p, stage_depth, depth_host, L.depth_row, L.depth_pitch, H, st));
+  return stage_rows(b.rgb_raw.p, stage_rgb, rgb_host, L.rgb_row, L.rgb_pitch, H, st);
 }
 
 // The one place that decides which staging set a call uses: the next one in turn, waited for first, if it is still
@@ -367,8 +445,10 @@ int order_after_track(fp_ctx* c, cudaStream_t st) {
 }
 
 constexpr size_t kTableBytes = sizeof(CameraDev) * kMaxCameras;  // the camera table at the head of fp_ctx::args
-// fp_ctx::args (and its staging) for `rows` slot and camera ids: the table, the ids, and a tracking call's fit threshold
-static size_t args_bytes(int rows) { return kTableBytes + (size_t)2 * rows * sizeof(int) + sizeof(float); }
+constexpr size_t kHeadBytes = kTableBytes + sizeof(FrameFmtDev) * kMaxCameras;  // then the cameras' frame formats
+// fp_ctx::args (and its staging) for `rows` slot and camera ids: the two tables, the ids, and a tracking call's fit
+// threshold
+static size_t args_bytes(int rows) { return kHeadBytes + (size_t)2 * rows * sizeof(int) + sizeof(float); }
 
 // The cameras of fp_track_cameras / _objects and fp_register_cameras / _objects, before anything reads a frame.  Every
 // camera's buffers are sized for the largest frame of the call (kept at the largest size seen, so a permutation of the
@@ -378,37 +458,45 @@ static size_t args_bytes(int rows) { return kTableBytes + (size_t)2 * rows * siz
 // uploaded through its camera's staging (camera i's DMA runs while camera i + 1 is copied on the host).  A frame buffer
 // on the device (on_dev) is read in place: its table entry points at the caller's buffer, and nothing is staged or
 // uploaded for it.  Every camera still gets its raw upload buffers, so where a frame lives never changes an allocation
-// or the graph epoch.  H_max / W_max: the largest frame height and width of the call.  `set`: the staging set the call
-// uploads through (not busy).
+// or the graph epoch.  Each camera's frame is read in its format (fp_ctx::fmt, copied into the format table beside the
+// camera table here): host frames are staged packed, at the format's bytes per pixel, device frames are read with their
+// pitch; the raw buffers are sized for the largest frame and the widest pixels of the call.  H_max / W_max: the largest
+// frame height and width of the call.  `set`: the staging set the call uploads through (not busy).
 static int setup_cameras(fp_ctx* c, StagingSet& set, int C, const unsigned char* const* rgb, const float* const* depth,
                          const FrameSources& on_dev, const float* K, const int* H, const int* W, int rows, int staged_rows,
                          cudaStream_t st, int& H_max, int& W_max) {
   size_t npix_max = 0;
+  int rgb_bpp = 0, depth_bpp = 0;
   H_max = W_max = 0;
   for (int i = 0; i < C; ++i) {
     npix_max = std::max(npix_max, (size_t)H[i] * W[i]);
     H_max = std::max(H_max, H[i]);
     W_max = std::max(W_max, W[i]);
+    const FrameLayout L = frame_layout(c->fmt[i], W[i]);
+    rgb_bpp = std::max(rgb_bpp, L.rgb_bpp);
+    depth_bpp = std::max(depth_bpp, L.depth_bpp);
   }
   for (int i = 0; i < C; ++i) {
-    FP_TRY(alloc_camera(c, i, npix_max, /*raw=*/true));
-    if (!on_dev.rgb[i]) FP_TRY(pinned_alloc(nullptr, set.rgb[i], npix_max * 3));
-    if (!on_dev.depth[i]) FP_TRY(pinned_alloc(nullptr, set.depth[i], npix_max * 4));
+    FP_TRY(alloc_camera(c, i, npix_max, /*raw=*/true, rgb_bpp, depth_bpp));
+    if (!on_dev.rgb[i]) FP_TRY(pinned_alloc(nullptr, set.rgb[i], npix_max * rgb_bpp));
+    if (!on_dev.depth[i]) FP_TRY(pinned_alloc(nullptr, set.depth[i], npix_max * depth_bpp));
   }
   c->n_frames = C;
   FP_TRY(dev_alloc(&c->epoch, c->args, args_bytes(rows)));
   FP_TRY(pinned_alloc(nullptr, set.args, args_bytes(staged_rows)));
   CameraDev* table = reinterpret_cast<CameraDev*>(set.args.p);
-  memset(table, 0, kTableBytes);
+  FrameFmtDev* fmts = reinterpret_cast<FrameFmtDev*>(static_cast<char*>(set.args.p) + kTableBytes);
+  memset(table, 0, kHeadBytes);
   for (int i = 0; i < C; ++i) {
     set_frame_geometry(c, i, K + 9 * i, H[i], W[i]);
     table[i] = camera_dev(c, i);
     if (on_dev.rgb[i]) table[i].rgb_raw = rgb[i];
     if (on_dev.depth[i]) table[i].depth_raw = depth[i];
+    const FrameLayout L = frame_layout(c->fmt[i], W[i]);
+    fmts[i] = fmt_dev(c->fmt[i], L, on_dev.rgb[i], on_dev.depth[i]);
     // the order of upload_staged_frame: depth, then rgb
-    const size_t npix = (size_t)H[i] * W[i];
-    if (!on_dev.depth[i]) FP_TRY(stage_copy(c->cam[i].depth_raw.p, set.depth[i], depth[i], npix * 4, st));
-    if (!on_dev.rgb[i]) FP_TRY(stage_copy(c->cam[i].rgb_raw.p, set.rgb[i], rgb[i], npix * 3, st));
+    if (!on_dev.depth[i]) FP_TRY(stage_rows(c->cam[i].depth_raw.p, set.depth[i], depth[i], L.depth_row, L.depth_pitch, H[i], st));
+    if (!on_dev.rgb[i]) FP_TRY(stage_rows(c->cam[i].rgb_raw.p, set.rgb[i], rgb[i], L.rgb_row, L.rgb_pitch, H[i], st));
   }
   return 0;
 }
@@ -420,11 +508,11 @@ static int stage_track_call(fp_ctx* c, StagingSet& set, int C, const unsigned ch
                             const int* camera_of, const int* slots_host, const float* delta, cudaStream_t st, int& H_max,
                             int& W_max) {
   FP_TRY(setup_cameras(c, set, C, rgb, depth, on_dev, K, H, W, M, M, st, H_max, W_max));
-  int* ids = reinterpret_cast<int*>(static_cast<char*>(set.args.p) + kTableBytes);
+  int* ids = reinterpret_cast<int*>(static_cast<char*>(set.args.p) + kHeadBytes);
   memcpy(ids, slots_host, (size_t)M * sizeof(int));
   memcpy(ids + M, camera_of, (size_t)M * sizeof(int));
   if (delta) memcpy(ids + 2 * M, delta, sizeof(float));
-  const size_t bytes = kTableBytes + (size_t)2 * M * sizeof(int) + (delta ? sizeof(float) : 0);
+  const size_t bytes = kHeadBytes + (size_t)2 * M * sizeof(int) + (delta ? sizeof(float) : 0);
   FP_CUDA_OK(cudaMemcpyAsync(c->args.p, set.args.p, bytes, cudaMemcpyHostToDevice, st));
   return 0;
 }
@@ -449,6 +537,7 @@ static int track_cameras_submit(fp_ctx* c, const char* caller, int C, const unsi
                                 float* poses_keep_dev = nullptr, const float* delta = nullptr, int* fit_out_dev = nullptr) {
   FrameSources on_dev;
   FP_TRY(frame_sources(c, C, rgb, depth, on_dev, caller));  // refused before anything is enqueued
+  FP_TRY(check_frame_formats(c, C, depth, W, caller));
   StagingSet* set;
   FP_TRY(take_set(c, set));
   FP_TRY(order_after_track(c, st));  // the context's device buffers are never used by two streams at once
@@ -481,7 +570,8 @@ static int track_cameras_submit(fp_ctx* c, const char* caller, int C, const unsi
     c->cam_grid_w = std::max(c->cam_grid_w, W_max);
   }
   const CameraDev* cams_dev = reinterpret_cast<const CameraDev*>(c->args.p);
-  const int* mesh_of = reinterpret_cast<const int*>(static_cast<const char*>(c->args.p) + kTableBytes);
+  const FrameFmtDev* fmts_dev = reinterpret_cast<const FrameFmtDev*>(static_cast<const char*>(c->args.p) + kTableBytes);
+  const int* mesh_of = reinterpret_cast<const int*>(static_cast<const char*>(c->args.p) + kHeadBytes);
   const int* cam_of = mesh_of + M;
   const float* delta_dev = reinterpret_cast<const float*>(cam_of + M);
   int* fit = reinterpret_cast<int*>(c->fit.p);
@@ -497,7 +587,7 @@ static int track_cameras_submit(fp_ctx* c, const char* caller, int C, const unsi
     // estimater.py:250-268 for every object of every camera at once: each camera's frame filtered once (erode +
     // bilateral, depth2xyzmap_batch(zfar = inf)), M hypotheses each rendering its own mesh and cropping its own
     // camera's frame
-    FP_TRY(frame_prep_cameras_launch(cams_dev, C, grid_h, grid_w, INFINITY, s2));
+    FP_TRY(frame_prep_cameras_launch(cams_dev, fmts_dev, C, grid_h, grid_w, INFINITY, s2));
     c->has_frame = true;
     FP_TRY(refine_body(c, M, iterations, s2, mesh_of, cams_dev, cam_of));
     if (delta) FP_TRY(make_crops(c, fin, M, 0, nullptr, nullptr, nullptr, s2, mesh_of, cams_dev, cam_of, nullptr, fit, delta_dev));
@@ -600,6 +690,7 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
   }
   FrameSources on_dev;
   FP_TRY(frame_sources(c, C, rgb, depth, on_dev, caller));
+  FP_TRY(check_frame_formats(c, C, depth, W, caller));
   std::vector<char> mask_on_dev(M, 0);
   for (int i = 0; i < M; ++i) {
     bool d = false;
@@ -653,7 +744,7 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
     if (!mask_on_dev[i])
       memcpy(static_cast<unsigned char*>(set->masks.p) + mask_at[i], masks[i], mask_at[i + 1] - mask_at[i]);
   // the ids of the pass starting at row r0 are staged at 2 * r0 after the table: its slot ids, then its camera ids
-  int* ids = reinterpret_cast<int*>(static_cast<char*>(set->args.p) + kTableBytes);
+  int* ids = reinterpret_cast<int*>(static_cast<char*>(set->args.p) + kHeadBytes);
   for (size_t p = 0; p + 1 < pass_obj.size(); ++p) {
     const int row0 = off[pass_obj[p]], n = off[pass_obj[p + 1]] - row0;
     for (int i = pass_obj[p]; i < pass_obj[p + 1]; ++i) {
@@ -682,11 +773,13 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
   if (by_value) {
     const unsigned char* rgb0 = on_dev.rgb[0] ? rgb[0] : static_cast<const unsigned char*>(c->cam[0].rgb_raw.p);
     const float* depth0 = on_dev.depth[0] ? depth[0] : static_cast<const float*>(c->cam[0].depth_raw.p);
-    FP_TRY(set_frame_launches(c, rgb0, depth0, FP_FRAME_FILTER_DEPTH, INFINITY, st));
+    const FrameFmtDev fmt0 = *reinterpret_cast<const FrameFmtDev*>(static_cast<const char*>(set->args.p) + kTableBytes);
+    FP_TRY(set_frame_launches(c, rgb0, depth0, fmt0, FP_FRAME_FILTER_DEPTH, INFINITY, st));
   } else {
-    FP_CUDA_OK(cudaMemcpyAsync(c->args.p, set->args.p, kTableBytes, cudaMemcpyHostToDevice, st));
+    const FrameFmtDev* fmts_dev = reinterpret_cast<const FrameFmtDev*>(static_cast<const char*>(c->args.p) + kTableBytes);
+    FP_CUDA_OK(cudaMemcpyAsync(c->args.p, set->args.p, kHeadBytes, cudaMemcpyHostToDevice, st));
     FP_CUDA_OK(cudaMemcpyAsync(c->mask_off.p, stage_mask_off, (size_t)M * sizeof(size_t), cudaMemcpyHostToDevice, st));
-    FP_TRY(frame_prep_cameras_launch(cams_dev, C, H_max, W_max, INFINITY, st));
+    FP_TRY(frame_prep_cameras_launch(cams_dev, fmts_dev, C, H_max, W_max, INFINITY, st));
   }
   c->has_frame = true;
   // estimater.py:137-156, :203-209 for every object in one launch pair; the start poses go to poses_out_dev and are
@@ -701,7 +794,7 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
   float* pb = reinterpret_cast<float*>(c->poses_b.p);
   float* ps = reinterpret_cast<float*>(c->pose_stage.p);
   float* fb = reinterpret_cast<float*>(c->feat_buf.p);
-  const int* mesh_of = reinterpret_cast<const int*>(static_cast<const char*>(c->args.p) + kTableBytes);
+  const int* mesh_of = reinterpret_cast<const int*>(static_cast<const char*>(c->args.p) + kHeadBytes);
   const float* fin = (iterations % 2 == 0) ? pa : pb;
   const int frame = by_value ? -1 : 0;  // from the table: prepared above, outside the graphs
   for (size_t p = 0; p + 1 < pass_obj.size(); ++p) {
@@ -709,7 +802,7 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
     const int* hyp_cam = by_value ? nullptr : mesh_of + n;
     // the pass's slot and camera ids and its start poses go to fixed context buffers and its outputs are copied out
     // after the replays: the graphs hold no per-pass address
-    FP_CUDA_OK(cudaMemcpyAsync(static_cast<char*>(c->args.p) + kTableBytes, ids + 2 * row0, (size_t)2 * n * sizeof(int),
+    FP_CUDA_OK(cudaMemcpyAsync(static_cast<char*>(c->args.p) + kHeadBytes, ids + 2 * row0, (size_t)2 * n * sizeof(int),
                                cudaMemcpyHostToDevice, st));
     FP_CUDA_OK(cudaMemcpyAsync(pa, poses_out_dev + (size_t)row0 * 16, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
     FP_TRY(run_graphed(
@@ -857,6 +950,26 @@ int fp_set_crop_tile(fp_ctx* c, int tile) {
   FP_API_END
 }
 
+int fp_set_camera_format(fp_ctx* c, int camera, const fp_frame_format_t* fmt) {
+  FP_API_BEGIN
+  FP_REQUIRE(c, "fp_set_camera_format: null ctx");
+  FP_REQUIRE(camera >= 0 && camera < kMaxCameras, "fp_set_camera_format: camera %d out of range [0, %d)", camera, kMaxCameras);
+  if (!fmt) {
+    c->fmt[camera] = fp_frame_format_t{};
+    return 0;
+  }
+  FP_REQUIRE(fmt->color >= FP_COLOR_RGB8 && fmt->color <= FP_COLOR_BGRA8, "fp_set_camera_format: camera %d: unknown colour format %d",
+             camera, fmt->color);
+  FP_REQUIRE(fmt->depth == FP_DEPTH_F32 || fmt->depth == FP_DEPTH_U16, "fp_set_camera_format: camera %d: unknown depth format %d",
+             camera, fmt->depth);
+  FP_REQUIRE(fmt->depth != FP_DEPTH_U16 || (isfinite(fmt->depth_scale) && fmt->depth_scale > 0.f),
+             "fp_set_camera_format: camera %d: uint16 depth scale %g must be finite and > 0 (metres per unit)", camera,
+             (double)fmt->depth_scale);
+  c->fmt[camera] = *fmt;
+  return 0;
+  FP_API_END
+}
+
 int fp_mesh_info(fp_ctx* c, int* info) {
   FP_API_BEGIN
   FP_REQUIRE(c && info && c->mesh[0].loaded, "fp_mesh_info: no mesh");
@@ -875,13 +988,15 @@ int fp_set_frame(fp_ctx* c, const unsigned char* rgb, const float* depth, const 
   FP_API_BEGIN
   FP_REQUIRE(c && rgb && depth && K, "fp_set_frame: null argument");
   FP_REQUIRE(H > 0 && W > 0, "fp_set_frame: empty frame");
+  FP_TRY(check_frame_format(c, 0, depth, W, "fp_set_frame"));
   DeviceGuard dg(c->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   FP_TRY(order_after_track(c, st));
   const size_t npix = (size_t)H * W;
   c->has_frame = false;
   const bool on_dev = (flags & FP_FRAME_ON_DEVICE) != 0;
-  FP_TRY(alloc_camera(c, 0, npix, /*raw=*/!on_dev));
+  const FrameLayout L = frame_layout(c->fmt[0], W);
+  FP_TRY(alloc_camera(c, 0, npix, /*raw=*/!on_dev, L.rgb_bpp, L.depth_bpp));
   set_frame_geometry(c, 0, K, H, W);
   c->n_frames = 1;
   const unsigned char* rgb_dev = rgb;
@@ -891,18 +1006,18 @@ int fp_set_frame(fp_ctx* c, const unsigned char* rgb, const float* depth, const 
     if (residence(c, rgb) == Residence::Pageable || residence(c, depth) == Residence::Pageable) {
       StagingSet* set;
       FP_TRY(take_set(c, set));
-      const int staged = upload_staged_frame(f, set->rgb[0], set->depth[0], rgb, depth, npix, st);
+      const int staged = upload_staged_frame(f, set->rgb[0], set->depth[0], rgb, depth, L, H, st);
       FP_TRY(set_busy(*set, st));
       FP_TRY(staged);
     } else {
       // page-locked frames, fp_group_register's among them, are read in place: one host copy fewer
-      FP_CUDA_OK(cudaMemcpyAsync(f.rgb_raw.p, rgb, npix * 3, cudaMemcpyHostToDevice, st));
-      FP_CUDA_OK(cudaMemcpyAsync(f.depth_raw.p, depth, npix * 4, cudaMemcpyHostToDevice, st));
+      FP_TRY(copy_rows(f.rgb_raw.p, rgb, L.rgb_row, L.rgb_pitch, H, st));
+      FP_TRY(copy_rows(f.depth_raw.p, depth, L.depth_row, L.depth_pitch, H, st));
     }
     rgb_dev = reinterpret_cast<const unsigned char*>(f.rgb_raw.p);
     depth_dev = reinterpret_cast<const float*>(f.depth_raw.p);
   }
-  FP_TRY(set_frame_launches(c, rgb_dev, depth_dev, flags, zfar, st));
+  FP_TRY(set_frame_launches(c, rgb_dev, depth_dev, fmt_dev(c->fmt[0], L, on_dev, on_dev), flags, zfar, st));
   c->has_frame = true;
   return 0;
   FP_API_END

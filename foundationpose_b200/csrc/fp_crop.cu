@@ -632,11 +632,15 @@ int crop_launch(const CropParams& p, cudaStream_t stream) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// frame preparation: uint8 RGB -> uchar4, depth -> xyz map (Utils.py:399-438)
+// frame preparation: the raw frame (camera format) -> uchar4 and float32 metres, depth -> xyz map (Utils.py:399-438)
 // ------------------------------------------------------------------------------------------------
-__global__ void rgb_to_rgba_kernel(const unsigned char* __restrict__ rgb, uchar4* __restrict__ out, int npix) {
+template <bool kDepth>
+__global__ void raw_frame_kernel(const CameraDev one, const FrameFmtDev f) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < npix) out[i] = make_uchar4(rgb[3 * i], rgb[3 * i + 1], rgb[3 * i + 2], 255);
+  if (i >= one.H * one.W) return;
+  const int v = i / one.W, u = i - v * one.W;
+  one.rgb[i] = raw_rgba_at(one.rgb_raw, f, v, u);
+  if (kDepth) one.depth[i] = raw_depth_at(one.depth_raw, f, v, u);
 }
 
 __global__ void depth_to_xyz_kernel(const CameraDev one, float zfar) {
@@ -653,8 +657,9 @@ __global__ void depth_to_xyz_kernel(const CameraDev one, float zfar) {
   one.xyz_map[i] = make_float4(X, Y, Z, 0.f);
 }
 
-int rgb_to_rgba_launch(const unsigned char* rgb, uchar4* out, int npix, cudaStream_t stream) {
-  rgb_to_rgba_kernel<<<(npix + 255) / 256, 256, 0, stream>>>(rgb, out, npix);
+int raw_frame_launch(const CameraDev& one, const FrameFmtDev& f, bool depth, cudaStream_t stream) {
+  const int npix = one.H * one.W;
+  (depth ? raw_frame_kernel<true> : raw_frame_kernel<false>)<<<(npix + 255) / 256, 256, 0, stream>>>(one, f);
   note_launches(1);
   FP_CUDA_OK(cudaGetLastError());
   return 0;

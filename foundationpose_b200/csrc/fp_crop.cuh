@@ -57,8 +57,8 @@ constexpr int kMaxCameras = 16;  // FP_MAX_CAMERAS (include/fpose.h)
 // frame) or read it from the camera table of the tracking calls and fp_register_cameras.  frame_prep_kernel reads the
 // raw frame and writes the filtered one; the crop producer and the start poses read the filtered one.
 struct __align__(16) CameraDev {
-  const unsigned char* rgb_raw;  // [H][W][3] uploaded frame
-  const float* depth_raw;        // [H][W]
+  const unsigned char* rgb_raw;  // [H][W] uploaded frame, in the camera's format (FrameFmtDev)
+  const float* depth_raw;        // [H][W], in the camera's format
   uchar4* rgb;                   // [H][W] RGBA8
   float* depth;                  // [H][W] eroded + bilateral-filtered depth
   float4* xyz_map;               // [H][W] (x, y, z, 0) back-projected filtered depth
@@ -66,6 +66,36 @@ struct __align__(16) CameraDev {
   int H, W;
 };
 static_assert(sizeof(CameraDev) == 64, "camera table entry: four uint4s");
+
+// How a camera's raw frame (CameraDev::rgb_raw / depth_raw) is laid out (fp_frame_format_t, resolved by the host for
+// where the frame is read: the caller's pitch in place, the packed row bytes once staged).  Only the frame preparation
+// reads it, by value or from the format table beside the camera table.
+struct __align__(16) FrameFmtDev {
+  int rgb_pitch;      // bytes per rgb row
+  int depth_pitch;    // bytes per depth row
+  float depth_scale;  // metres per unit (u16)
+  unsigned char bpp;  // rgb bytes per pixel: 3 or 4
+  unsigned char bgr;  // 1: channel order B, G, R
+  unsigned char u16;  // 1: uint16 depth * depth_scale, else float32 metres
+  unsigned char packed;  // 1: packed RGB8 + float32, the layout frames had before formats (read without the fields above)
+};
+static_assert(sizeof(FrameFmtDev) == 16, "format table entry: one uint4");
+
+#ifdef __CUDACC__
+// Pixel (v, u) of a raw depth frame in metres: float32 as stored, or uint16 * scale in one fp32 multiply rounded to
+// nearest (no contraction), numpy's v.astype(np.float32) * np.float32(scale)
+__device__ __forceinline__ float raw_depth_at(const float* base, const FrameFmtDev& f, int v, int u) {
+  const char* row = reinterpret_cast<const char*>(base) + (size_t)v * f.depth_pitch;
+  if (f.u16) return __fmul_rn((float)__ldg(reinterpret_cast<const unsigned short*>(row) + u), f.depth_scale);
+  return __ldg(reinterpret_cast<const float*>(row) + u);
+}
+// Pixel (v, u) of a raw colour frame as the context's RGBA8
+__device__ __forceinline__ uchar4 raw_rgba_at(const unsigned char* base, const FrameFmtDev& f, int v, int u) {
+  const unsigned char* p = base + (size_t)v * f.rgb_pitch + (size_t)u * f.bpp;
+  const unsigned char c0 = __ldg(p), c1 = __ldg(p + 1), c2 = __ldg(p + 2);
+  return f.bgr ? make_uchar4(c2, c1, c0, 255) : make_uchar4(c0, c1, c2, 255);
+}
+#endif
 
 struct CropParams {
   const float* poses;  // [N][16] row-major ob_in_cam
@@ -101,7 +131,9 @@ struct CropParams {
 constexpr int kFitCounts = 5;  // FP_FIT_COUNTS (include/fpose.h): covered, valid, inlier, occluded, behind
 
 int crop_launch(const CropParams& p, cudaStream_t stream);
-int rgb_to_rgba_launch(const unsigned char* rgb, uchar4* out, int npix, cudaStream_t stream);
+// the unfiltered frame of fp_set_frame: one.rgb from one.rgb_raw, and with `depth` one.depth from one.depth_raw (a
+// frame that is not packed float32), both read in format f
+int raw_frame_launch(const CameraDev& one, const FrameFmtDev& f, bool depth, cudaStream_t stream);
 // one.xyz_map from one.depth (invalid: z < 0.001 or z > zfar)
 int depth_to_xyz_launch(const CameraDev& one, float zfar, cudaStream_t stream);
 

@@ -202,6 +202,8 @@ struct fp_ctx {
   // frames: cam[0] is the context's frame, cameras 1.. those of the multi-camera calls
   fp::CameraBufs cam[fp::kMaxCameras];
   int n_frames = 0;  // the last call prepared the frames of cameras 0 .. n_frames - 1
+  // every camera's frame format (fp_set_camera_format; all zero = packed RGB8 + float32), read when a call is staged
+  fp_frame_format_t fmt[fp::kMaxCameras] = {};
   bool has_frame = false;
   // workspaces (sized for cap_n hypotheses)
   int cap_n = 0;

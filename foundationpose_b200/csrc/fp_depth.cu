@@ -105,18 +105,23 @@ __global__ void bilateral_depth_kernel(const float* __restrict__ depth, float* _
 // a second shared tile (halo pixels are recomputed by the neighbouring blocks, identically) and filters from there:
 // one read of the depth image instead of ~50 per pixel from L1 / L2, three launches fewer per frame (47 -> ~12 us of
 // a 0.97 ms tracked frame).  Same per-pixel code as the stand-alone kernels above: bit-identical.
-// kTable: one launch for several cameras (fp_track_objects / _cameras, fp_register_cameras).  blockIdx.z selects the camera's entry of the device table
-// `cams`; the grid covers the largest frame and the blocks outside a smaller one leave at once.  Otherwise the one frame
-// is `one`, passed by value.
+// kTable: one launch for several cameras (fp_track_objects / _cameras, fp_register_cameras).  blockIdx.z selects the
+// camera's entry of the device table `cams` and of the format table `fmts`; the grid covers the largest frame and the
+// blocks outside a smaller one leave at once.  Otherwise the one frame is `one` in format `fone`, passed by value.  The
+// raw frame is read in its camera's format (FrameFmtDev): depth converted to float32 metres as the tile is loaded,
+// colour repacked to RGBA8.  A frame in the default layout (FrameFmtDev::packed: packed RGB8 + float32) is read by the
+// body the kernel had before formats existed (kFmt = false), which never looks at the format: on default frames the
+// format-reading body measured 7.8 % slower by value (109.5 against 101.6 us per 1280x720 frame, H100 80GB HBM3 at
+// 700 W, torch.profiler, alternated).  By value the launch selects the body; from the table each block branches on its
+// camera's flag (block-uniform), so the tracking graphs replay whatever the formats and their key does not change.
 constexpr int kFpW = 32, kFpH = 8, kFpR = 2;
-template <bool kTable>
-__global__ void __launch_bounds__(kFpW* kFpH)
-    frame_prep_kernel(const CameraDev one, const CameraDev* __restrict__ cams, float zfar_xyz) {
-  constexpr int RW = kFpW + 4 * kFpR, RH = kFpH + 4 * kFpR;  // raw tile 40 x 16
-  constexpr int EW = kFpW + 2 * kFpR, EH = kFpH + 2 * kFpR;  // eroded tile 36 x 12
-  __shared__ float raw[RH * RW];
-  __shared__ float er[EH * EW];
-  const CameraDev cam = kTable ? cams[blockIdx.z] : one;
+constexpr int kFpRW = kFpW + 4 * kFpR, kFpRH = kFpH + 4 * kFpR;  // raw tile 40 x 16
+constexpr int kFpEW = kFpW + 2 * kFpR, kFpEH = kFpH + 2 * kFpR;  // eroded tile 36 x 12
+
+template <bool kTable, bool kFmt>
+__device__ __forceinline__ void frame_prep_body(const CameraDev& cam, const FrameFmtDev& fmt, float zfar_xyz, float* raw,
+                                                float* er) {
+  constexpr int RW = kFpRW, RH = kFpRH, EW = kFpEW, EH = kFpEH;
   const int H = cam.H, W = cam.W;
   const float fx = cam.fx, fy = cam.fy, cx = cam.cx, cy = cam.cy;
   const int w0 = blockIdx.x * kFpW, h0 = blockIdx.y * kFpH;
@@ -124,7 +129,8 @@ __global__ void __launch_bounds__(kFpW* kFpH)
   const int tid = threadIdx.y * kFpW + threadIdx.x;
   for (int i = tid; i < RH * RW; i += kFpW * kFpH) {
     const int v = h0 - 2 * kFpR + i / RW, u = w0 - 2 * kFpR + i % RW;
-    raw[i] = (v >= 0 && v < H && u >= 0 && u < W) ? __ldg(cam.depth_raw + v * W + u) : 0.f;  // out-of-image cells are never read
+    const bool in = v >= 0 && v < H && u >= 0 && u < W;  // out-of-image cells are never read
+    raw[i] = !in ? 0.f : kFmt ? raw_depth_at(cam.depth_raw, fmt, v, u) : __ldg(cam.depth_raw + v * W + u);
   }
   __syncthreads();
   const TileSrc rsrc{raw, h0 - 2 * kFpR, w0 - 2 * kFpR, RW};
@@ -145,20 +151,43 @@ __global__ void __launch_bounds__(kFpW* kFpH)
     Z = z;
   }
   cam.xyz_map[i] = make_float4(X, Y, Z, 0.f);
-  cam.rgb[i] = make_uchar4(__ldg(cam.rgb_raw + 3 * i), __ldg(cam.rgb_raw + 3 * i + 1), __ldg(cam.rgb_raw + 3 * i + 2), 255);
+  cam.rgb[i] = kFmt ? raw_rgba_at(cam.rgb_raw, fmt, h, w)
+                   : make_uchar4(__ldg(cam.rgb_raw + 3 * i), __ldg(cam.rgb_raw + 3 * i + 1), __ldg(cam.rgb_raw + 3 * i + 2), 255);
 }
 
-int frame_prep_launch(const CameraDev& one, float zfar_xyz, cudaStream_t stream) {
+// kFmt: the by-value body (ignored with kTable, where each block branches on its camera's FrameFmtDev::packed).  The
+// table kernel holds both bodies; six blocks per SM keep it at the occupancy it had with one (39 registers, no spills).
+template <bool kTable, bool kFmt>
+__global__ void __launch_bounds__(kFpW* kFpH, kTable ? 6 : 1)
+    frame_prep_kernel(const CameraDev one, const FrameFmtDev fone, const CameraDev* __restrict__ cams,
+                      const FrameFmtDev* __restrict__ fmts, float zfar_xyz) {
+  __shared__ float raw[kFpRH * kFpRW];
+  __shared__ float er[kFpEH * kFpEW];
+  if (!kTable) {
+    frame_prep_body<false, kFmt>(one, fone, zfar_xyz, raw, er);
+    return;
+  }
+  const CameraDev cam = cams[blockIdx.z];
+  const FrameFmtDev fmt = fmts[blockIdx.z];
+  if (fmt.packed)
+    frame_prep_body<true, false>(cam, fmt, zfar_xyz, raw, er);
+  else
+    frame_prep_body<true, true>(cam, fmt, zfar_xyz, raw, er);
+}
+
+int frame_prep_launch(const CameraDev& one, const FrameFmtDev& fmt, float zfar_xyz, cudaStream_t stream) {
   dim3 block(kFpW, kFpH), grid((one.W + kFpW - 1) / kFpW, (one.H + kFpH - 1) / kFpH);
-  frame_prep_kernel<false><<<grid, block, 0, stream>>>(one, nullptr, zfar_xyz);
+  (fmt.packed ? frame_prep_kernel<false, false> : frame_prep_kernel<false, true>)<<<grid, block, 0, stream>>>(
+      one, fmt, nullptr, nullptr, zfar_xyz);
   note_launches(1);
   FP_CUDA_OK(cudaGetLastError());
   return 0;
 }
 
-int frame_prep_cameras_launch(const CameraDev* cams, int C, int max_H, int max_W, float zfar_xyz, cudaStream_t stream) {
+int frame_prep_cameras_launch(const CameraDev* cams, const FrameFmtDev* fmts, int C, int max_H, int max_W, float zfar_xyz,
+                              cudaStream_t stream) {
   dim3 block(kFpW, kFpH), grid((max_W + kFpW - 1) / kFpW, (max_H + kFpH - 1) / kFpH, C);
-  frame_prep_kernel<true><<<grid, block, 0, stream>>>(CameraDev{}, cams, zfar_xyz);
+  frame_prep_kernel<true, true><<<grid, block, 0, stream>>>(CameraDev{}, FrameFmtDev{}, cams, fmts, zfar_xyz);
   note_launches(1);
   FP_CUDA_OK(cudaGetLastError());
   return 0;

@@ -10,10 +10,11 @@ int erode_depth_launch(const float* depth, float* out, int H, int W, int radius,
 int bilateral_depth_launch(const float* depth, float* out, int H, int W, int radius, float zfar, float sigmaD,
                            float sigmaR, cudaStream_t stream);
 // erode(2) -> bilateral(2) -> back-projection (invalid: z < 0.001 or z > zfar_xyz) + rgb -> rgba of one frame, one
-// launch (raw frame in, filtered frame out)
-int frame_prep_launch(const CameraDev& one, float zfar_xyz, cudaStream_t stream);
-// the same for C cameras in one launch: cams DEVICE [C]; max_H x max_W covers the largest of the frames
-int frame_prep_cameras_launch(const CameraDev* cams, int C, int max_H, int max_W, float zfar_xyz, cudaStream_t stream);
+// launch (raw frame in format fmt in, filtered frame out)
+int frame_prep_launch(const CameraDev& one, const FrameFmtDev& fmt, float zfar_xyz, cudaStream_t stream);
+// the same for C cameras in one launch: cams, fmts DEVICE [C]; max_H x max_W covers the largest of the frames
+int frame_prep_cameras_launch(const CameraDev* cams, const FrameFmtDev* fmts, int C, int max_H, int max_W, float zfar_xyz,
+                              cudaStream_t stream);
 // guess_translation + start poses of M objects in two launches; off [M + 1] device row offsets of each object in
 // rot_grid / poses_out ([off[M]][16]; null when M = 1 by value: rows [0, N)); stats: 6 M words of device scratch;
 // info [M][4] = {tx, ty, tz, n_valid}.  cams null: every object is seen in frame `one` (filtered depth, H x W,

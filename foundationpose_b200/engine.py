@@ -12,12 +12,18 @@ import torch
 
 from . import _lib, packing
 from ._lib import lib
+from .frames import DEFAULT_FORMAT, Color, Depth, frame_format
 
 CROP_SHAPE = (166, 2, 84, 8)  # padded fp16 crop image consumed by the stem convolution: rows x {even, odd cols} x pairs x ch
 
 
 class _FpTensor(C.Structure):
     _fields_ = [("name", C.c_char_p), ("data", C.c_void_p), ("dtype", C.c_int), ("numel", C.c_longlong)]
+
+
+class _FpFrameFormat(C.Structure):
+    _fields_ = [("color", C.c_int), ("depth", C.c_int), ("depth_scale", C.c_float), ("rgb_pitch", C.c_int),
+                ("depth_pitch", C.c_int)]
 
 
 def _proto():
@@ -27,6 +33,7 @@ def _proto():
     lib.fp_set_config.argtypes = [vp, i, f, f]
     lib.fp_mesh_info.argtypes = [vp, C.POINTER(i)]
     lib.fp_set_crop_tile.argtypes = [vp, i]
+    lib.fp_set_camera_format.argtypes = [vp, i, C.POINTER(_FpFrameFormat)]
     lib.fp_crop_stats.argtypes = [vp, vp, i, i, C.POINTER(i), vp]
     lib.fp_track.argtypes = [vp, vp, vp, C.POINTER(f), i, i, vp, i, vp, vp, vp]
     lib.fp_track_objects.argtypes = [vp, vp, vp, C.POINTER(f), i, i, i, C.POINTER(i), vp, i, vp, vp, vp]
@@ -76,7 +83,7 @@ def _proto():
     lib.fp_vis_crops.argtypes = [vp, vp, i, i, vp, vp]
     lib.fp_vis_workspace_bytes.argtypes = [vp]
     lib.fp_vis_workspace_bytes.restype = C.c_ulonglong
-    for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_track_cameras", "fp_track_submit", "fp_track_objects_submit",
+    for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_set_camera_format", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_track_cameras", "fp_track_submit", "fp_track_objects_submit",
                  "fp_track_cameras_submit", "fp_track_wait", "fp_track_cameras_fit_submit", "fp_track_fit_wait", "fp_register_objects", "fp_register_cameras", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh",
                  "fp_set_mesh_slot", "fp_set_frame",
                  "fp_get_depth", "fp_make_crops", "fp_start_poses", "fp_refine", "fp_score", "fp_score_features", "fp_score_tail",
@@ -112,18 +119,36 @@ def _ptr(x):
     return C.c_void_p(x.data_ptr() if torch.is_tensor(x) else x.ctypes.data)
 
 
-def _frame(rgb, depth, what):
-    """One camera's frame as the tracking and register calls take it: (rgb, depth, (H, W)).  Each buffer is a host array
-    (made a contiguous uint8 / float32 numpy array, staged by the library) or a CUDA tensor on the engine's device, read
-    in place in stream order: rgb uint8 (H,W,3), depth (H,W) converted to float32, both made contiguous."""
-    if _on_device(depth):
+def _check_wrapped_device(x, what, device):
+    if _on_device(x.img) and device is not None and x.img.device.index != device:
+        raise ValueError(f"{what}: {type(x).__name__} is a CUDA tensor on device {x.img.device.index}, the engine's is {device}")
+
+
+def _frame(rgb, depth, what, device=None):
+    """One camera's frame as the tracking and register calls take it: (rgb, depth, (H, W), format).  Each buffer is a
+    host array (made a contiguous uint8 / float32 numpy array, staged by the library) or a CUDA tensor on the engine's
+    device, read in place in stream order: rgb uint8 (H,W,3), depth (H,W) converted to float32, both made contiguous.  A
+    Color / Depth (frames.py) is taken as it is, in its own layout, wherever it lives; format is the camera format of
+    the pair (frames.frame_format)."""
+    fmt = frame_format(rgb, depth)
+    if isinstance(depth, Depth):
+        _check_wrapped_device(depth, what, device)
+        H, W = depth.H, depth.W
+        depth = depth.img
+    elif _on_device(depth):
         if depth.dim() != 2:
             raise ValueError(f"{what}: depth must be (H, W), got {tuple(depth.shape)}")
         depth = depth.contiguous().float()
+        H, W = depth.shape
     else:
         depth = np.ascontiguousarray(depth, dtype=np.float32)
-    H, W = depth.shape
-    if _on_device(rgb):
+        H, W = depth.shape
+    if isinstance(rgb, Color):
+        _check_wrapped_device(rgb, what, device)
+        if (rgb.H, rgb.W) != (H, W):
+            raise ValueError(f"{what}: the colour frame is {rgb.H} x {rgb.W}, the depth frame {H} x {W}")
+        rgb = rgb.img
+    elif _on_device(rgb):
         if rgb.dtype != torch.uint8:
             raise ValueError(f"{what}: a CUDA rgb frame must be uint8, got {rgb.dtype}")
         if tuple(rgb.shape) != (H, W, 3):
@@ -131,7 +156,7 @@ def _frame(rgb, depth, what):
         rgb = rgb.contiguous()
     else:
         rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
-    return rgb, depth, (int(H), int(W))
+    return rgb, depth, (int(H), int(W)), fmt
 
 
 def _device_mask(m):
@@ -151,7 +176,8 @@ def _hold(bufs):
 
 
 def _camera_args(frames):
-    """The (rgb pointers, depth pointers, K [C][9], H, W) arguments of the multi-camera calls for frames made by _frame."""
+    """The (rgb pointers, depth pointers, K [C][9], H, W) arguments of the multi-camera calls for (rgb, depth, K) frames
+    whose buffers _frame made."""
     n_cam = len(frames)
     rgbs = (C.c_void_p * n_cam)(*[_ptr(rgb).value for rgb, _, _ in frames])
     depths = (C.c_void_p * n_cam)(*[_ptr(depth).value for _, depth, _ in frames])
@@ -301,6 +327,7 @@ class Engine:
         self.frame_hw = None
         self._dropped = []  # tickets of PendingPoses dropped without result()
         self._last_ticket = 0
+        self._formats = [DEFAULT_FORMAT] * MAX_CAMERAS  # the frame format the context holds for each camera
 
     def close(self):
         if getattr(self, "_h", None):
@@ -354,6 +381,14 @@ class Engine:
         _lib.check(lib.fp_crop_stats(self._h, _p(poses), len(poses), mode, st, _stream()), "fp_crop_stats")
         return dict(meshlet_visits=st[0], triangles=st[1], fragments=st[2], near_plane_triangles=st[3])
 
+    def _set_formats(self, fmts):
+        """fp_set_camera_format for camera i = 0, 1, ... wherever fmts[i] differs from the format the context holds."""
+        for i, f in enumerate(fmts):
+            if self._formats[i] != f:
+                ff = _FpFrameFormat(*f)
+                _lib.check(lib.fp_set_camera_format(self._h, i, C.byref(ff)), "fp_set_camera_format")
+                self._formats[i] = f
+
     # ---- tracking: every call is a submit and, with wait=True, its fp_track_wait
     def _collect_dropped(self, keep):
         """Collects the dropped handles' tickets except those of the last `keep` submits (still running, most likely)."""
@@ -396,11 +431,13 @@ class Engine:
     def track(self, rgb, depth, K, pose_in, iterations, pose_out=None, wait=True):
         """fp_track: one CUDA-graph launch per frame (upload + depth filters + xyz map + refiner passes + read-back).
         rgb uint8 (H,W,3) / depth float32 (H,W): host arrays, or CUDA tensors on the engine's device, read in place in the
-        current stream's order (see _frame); pose_in (4,4) CUDA tensor or None (continue).
+        current stream's order (see _frame), or a Color / Depth (frames.py) in a sensor's own layout, host or device;
+        pose_in (4,4) CUDA tensor or None (continue).
         Returns (pose_out CUDA (4,4), pose host (4,4) float32 numpy).  wait=False returns as soon as the call is
         submitted (the host arrays may then be reused): (pose_out, PendingPoses), pose_out complete in stream order."""
-        rgb, depth, (H, W) = _frame(rgb, depth, "track")
+        rgb, depth, (H, W), fmt = _frame(rgb, depth, "track", self.device_index)
         Kf = (C.c_float * 9)(*[float(x) for x in np.asarray(K, dtype=np.float64).reshape(-1)])
+        self._set_formats([fmt])
         if pose_in is not None:
             pose_in = pose_in.reshape(4, 4).contiguous().float()
         if pose_out is None:
@@ -415,13 +452,14 @@ class Engine:
         slot slots[i] (loaded by set_mesh(..., slot=)).  rgb uint8 (H,W,3) / depth float32 (H,W): host arrays or CUDA
         tensors, as `track`; poses_in (M,4,4) CUDA tensor.  Returns (poses CUDA (M,4,4), poses host (M,4,4) float32
         numpy); wait=False as `track`."""
-        rgb, depth, (H, W) = _frame(rgb, depth, "track_objects")
+        rgb, depth, (H, W), fmt = _frame(rgb, depth, "track_objects", self.device_index)
         Kf = (C.c_float * 9)(*[float(x) for x in np.asarray(K, dtype=np.float64).reshape(-1)])
         poses_in = poses_in.reshape(-1, 4, 4).contiguous().float()
         M = len(poses_in)
         slots = [int(s) for s in slots]
         if len(slots) != M:
             raise ValueError(f"track_objects: {M} poses but {len(slots)} slots")
+        self._set_formats([fmt])
         out = torch.empty(M, 4, 4, dtype=torch.float32, device="cuda")
         res = self._submit(lib.fp_track_objects_submit, (_ptr(rgb), _ptr(depth), Kf, H, W, M, (C.c_int * M)(*slots), _p(poses_in),
                                                          int(iterations), _p(out)),
@@ -432,7 +470,8 @@ class Engine:
     def track_cameras(self, frames, poses_in, camera_of, slots, iterations, wait=True, fit_delta=None):
         """fp_track_cameras: `track_objects` for M objects spread over C camera streams in ONE CUDA-graph launch.  frames: C
         tuples (rgb uint8 (H,W,3), depth float32 (H,W), K (3,3)), one per camera, each with its own size and intrinsics and
-        each buffer a host array or a CUDA tensor, as `track` (one call may mix them); object i is seen by camera
+        each buffer a host array, a CUDA tensor or a Color / Depth, as `track` (one call may mix them, and each camera has
+        its own format); object i is seen by camera
         camera_of[i] and renders the mesh in slot slots[i]; poses_in (M,4,4) CUDA tensor.  Returns (poses CUDA (M,4,4),
         poses host (M,4,4) float32 numpy); wait=False as `track`.
 
@@ -440,13 +479,16 @@ class Engine:
         observed depth (fp_track_cameras_fit_submit, include/fpose.h): returns (poses CUDA, poses host, fit) with fit an
         int32 (M, FIT_COUNTS) numpy array of (covered, valid, inlier, occluded, behind) pixels; wait=False returns
         (poses CUDA, PendingPoses) whose result() gives (poses host, fit).  The poses are those of the call without it."""
-        frames = [(*_frame(rgb, depth, f"track_cameras: camera {c}")[:2], K) for c, (rgb, depth, K) in enumerate(frames)]
+        made = [(_frame(rgb, depth, f"track_cameras: camera {c}", self.device_index), K) for c, (rgb, depth, K) in enumerate(frames)]
+        frames = [(f[0], f[1], K) for f, K in made]
         n_cam = len(frames)
         poses_in = poses_in.reshape(-1, 4, 4).contiguous().float()
         M = len(poses_in)
         camera_of, slots = [int(c) for c in camera_of], [int(s) for s in slots]
         if len(camera_of) != M or len(slots) != M:
             raise ValueError(f"track_cameras: {M} poses, {len(camera_of)} camera ids and {len(slots)} slots")
+        if n_cam <= MAX_CAMERAS:  # more cameras: fp_track_cameras refuses the call
+            self._set_formats([f[3] for f, _ in made])
         rgbs, depths, Ks, Hs, Ws = _camera_args(frames)
         out = torch.empty(M, 4, 4, dtype=torch.float32, device="cuda")
         ids = (n_cam, rgbs, depths, Ks, Hs, Ws, M, (C.c_int * M)(*camera_of), (C.c_int * M)(*slots), _p(poses_in), int(iterations))
@@ -463,12 +505,13 @@ class Engine:
 
     def register_objects(self, rgb, depth, K, masks, rot_grids, slots, iterations):
         """fp_register_objects: the register() hot path for M objects of one frame in one call, object i rendering the mesh
-        in slot slots[i].  rgb uint8 (H,W,3) / depth float32 (H,W): host arrays or CUDA tensors, as `track`; masks
+        in slot slots[i].  rgb uint8 (H,W,3) / depth float32 (H,W): host arrays, CUDA tensors or a Color / Depth, as
+        `track`; masks
         (M,H,W) (nonzero = object): a host array, or a CUDA bool / uint8 / float tensor (or a sequence of M CUDA (H,W)
         masks) binarised on the device; rot_grids: M CUDA float32 (N_i,4,4) rotation grids.  Returns CUDA tensors: poses
         (sum N_i,4,4) refined, object-major and unranked; scores (sum N_i,); best (M,) int32, each object's first arg-max
         relative to its own rows; info (M,4) = (tx, ty, tz, n_valid) per object."""
-        rgb, depth, (H, W) = _frame(rgb, depth, "register_objects")
+        rgb, depth, (H, W), fmt = _frame(rgb, depth, "register_objects", self.device_index)
         if not _on_device(masks) and len(masks) and all(_on_device(m) for m in masks):
             masks = torch.stack(list(masks))
         masks = masks if _on_device(masks) else np.ascontiguousarray(masks)
@@ -491,6 +534,7 @@ class Engine:
         scores = torch.empty(total, dtype=torch.float32, device="cuda")
         best = torch.empty(M, dtype=torch.int32, device="cuda")
         info = torch.empty(M, 4, dtype=torch.float32, device="cuda")
+        self._set_formats([fmt])
         _lib.check(lib.fp_register_objects(self._h, _ptr(rgb), _ptr(depth), Kf, H, W, M, (C.c_int * M)(*slots), (C.c_int * M)(*n_hyp),
                                            _ptr(masks), _p(grids), int(iterations), _p(poses), _p(scores), _p(best), _p(info),
                                            _stream()),
@@ -501,11 +545,12 @@ class Engine:
     def register_cameras(self, frames, masks, rot_grids, camera_of, slots, iterations):
         """fp_register_cameras: `register_objects` for M objects spread over C camera streams in one call.  frames: C tuples
         (rgb uint8 (H,W,3), depth float32 (H,W), K (3,3)), one per camera, each with its own size and intrinsics and each
-        buffer a host array or a CUDA tensor, as `track`; object i is seen by camera camera_of[i], renders the mesh in slot
+        buffer a host array, a CUDA tensor or a Color / Depth, as `track_cameras`; object i is seen by camera camera_of[i], renders the mesh in slot
         slots[i] and has the mask masks[i] (nonzero = object) of its camera's frame size, a host array or a CUDA bool /
         uint8 / float tensor binarised on the device; rot_grids: M CUDA float32 (N_i,4,4) rotation grids.
         Returns the CUDA tensors of register_objects: poses (sum N_i,4,4), scores (sum N_i,), best (M,), info (M,4)."""
-        frames = [(*_frame(rgb, depth, f"register_cameras: camera {c}")[:2], K) for c, (rgb, depth, K) in enumerate(frames)]
+        made = [(_frame(rgb, depth, f"register_cameras: camera {c}", self.device_index), K) for c, (rgb, depth, K) in enumerate(frames)]
+        frames = [(f[0], f[1], K) for f, K in made]
         n_cam = len(frames)
         M = len(masks)
         camera_of, slots = [int(c) for c in camera_of], [int(s) for s in slots]
@@ -528,6 +573,8 @@ class Engine:
         scores = torch.empty(total, dtype=torch.float32, device="cuda")
         best = torch.empty(M, dtype=torch.int32, device="cuda")
         info = torch.empty(M, 4, dtype=torch.float32, device="cuda")
+        if n_cam <= MAX_CAMERAS:  # more cameras: fp_register_cameras refuses the call
+            self._set_formats([f[3] for f, _ in made])
         _lib.check(lib.fp_register_cameras(self._h, n_cam, rgbs, depths, Ks, Hs, Ws, M, (C.c_int * M)(*camera_of),
                                            (C.c_int * M)(*slots), (C.c_int * M)(*n_hyp), (C.c_void_p * M)(*[_ptr(m).value for m in masks]),
                                            _p(grids), int(iterations), _p(poses), _p(scores), _p(best), _p(info), _stream()),
@@ -536,11 +583,21 @@ class Engine:
         return poses, scores, best, info
 
     def set_frame(self, rgb, depth, K, filter_depth=True, zfar=float("inf")):
-        """rgb uint8 (H,W,3), depth float32 (H,W): numpy / CPU tensors or CUDA tensors.  Pageable host frames are staged
-        by the library and may be reused once this returns."""
+        """rgb uint8 (H,W,3), depth float32 (H,W): numpy / CPU tensors or CUDA tensors, or a Color / Depth (frames.py) in
+        a sensor's own layout, both on the host or both on the device.  Pageable host frames are staged by the library and
+        may be reused once this returns."""
         Kf = (C.c_float * 9)(*[float(x) for x in np.asarray(K, dtype=np.float64).reshape(-1)])
         flags = FRAME_FILTER_DEPTH if filter_depth else 0
-        if torch.is_tensor(rgb) and rgb.is_cuda:
+        fmt = DEFAULT_FORMAT
+        if isinstance(rgb, Color) or isinstance(depth, Depth):
+            rgb, depth, _, fmt = _frame(rgb, depth, "set_frame", self.device_index)
+            if _on_device(rgb) != _on_device(depth):
+                raise ValueError("set_frame: rgb and depth must both be CUDA tensors or both be on the host")
+            if _on_device(rgb):
+                flags |= FRAME_ON_DEVICE
+            else:
+                rgb, depth = (x if torch.is_tensor(x) else torch.from_numpy(x) for x in (rgb, depth))
+        elif torch.is_tensor(rgb) and rgb.is_cuda:
             assert torch.is_tensor(depth) and depth.is_cuda
             rgb = rgb.contiguous()
             depth = depth.contiguous().float()
@@ -556,6 +613,7 @@ class Engine:
         # device and page-locked frames are read in place after the call returns, in stream order: keep them until then
         in_place = rgb.is_cuda or (rgb.is_pinned() and depth.is_pinned())
         self._frame_keep = (rgb, depth) if in_place else None
+        self._set_formats([fmt])
         _lib.check(lib.fp_set_frame(self._h, _p(rgb), _p(depth), Kf, H, W, flags, float(zfar), _stream()), "fp_set_frame")
         self.frame_hw = (H, W)
 

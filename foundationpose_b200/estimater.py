@@ -24,6 +24,7 @@ import torch
 
 from . import hypotheses, meshprep, synth, weights
 from .engine import MAX_CAMERAS, MAX_MESHES, Engine
+from .frames import host_rgb, image, on_cuda
 
 
 @dataclasses.dataclass(frozen=True)
@@ -327,7 +328,8 @@ class FoundationPose:
         return hypotheses.guess_translation(depth, mask, K)
 
     def register(self, K, rgb, depth, ob_mask, ob_id=None, glctx=None, iteration=5):
-        """Compute the object pose in the frame (estimater.py:159-240). Returns (4,4) numpy."""
+        """Compute the object pose in the frame (estimater.py:159-240). Returns (4,4) numpy.  rgb / depth may be a Color /
+        Depth (frames.py), as in track_one."""
         e = self.engine
         # erode_depth + bilateral_filter_depth + depth2xyzmap on the device (estimater.py:173-174, :214), then the
         # translation guess and the start poses, also on the device: nothing synchronises until the result is read
@@ -340,7 +342,7 @@ class FoundationPose:
             # estimater.py:176-180: the filtered frame's cloud and the mask, before the early exit.  The frame may be
             # device-resident: the dumps take host copies
             depth_f, xyz = (t.cpu().numpy() for t in e.get_depth())
-            rgb_h = rgb.cpu().numpy() if torch.is_tensor(rgb) else np.asarray(rgb)
+            rgb_h = host_rgb(rgb)
             self._write_cloud("scene_raw.ply", xyz, rgb_h)
             m = ob_mask.cpu().numpy() if torch.is_tensor(ob_mask) else np.asarray(ob_mask)
             cv2.imwrite(f"{self.debug_dir}/ob_mask.png", (m * 255.0).clip(0, 255))
@@ -409,7 +411,8 @@ class FoundationPose:
     def track_one(self, rgb, depth, K, iteration, extra={}, fit_delta=None):
         """estimater.py:250-268.  fit_delta (metres): also measure how well the returned pose fits the frame's depth, in
         the same launch, into self.fit_last (a PoseFit); host and device frames then both go through one
-        fp_track_cameras_fit call, which returns the same pose as the call without it."""
+        fp_track_cameras_fit call, which returns the same pose as the call without it.  rgb / depth may be a Color / Depth
+        (frames.py) in a sensor's own layout, on the host or the device, as the plain arrays or tensors it wraps."""
         if self.pose_last is None:
             logging.info("Please init pose by register first")
             raise RuntimeError
@@ -426,7 +429,7 @@ class FoundationPose:
             self.pose_last = pose_dev.reshape(1, 4, 4)
             self.refiner.last_trans_update = self.refiner.last_rot_update = None
             return _uncentre(pose_host[0], self.model_center)
-        if torch.is_tensor(rgb) or torch.is_tensor(depth):
+        if torch.is_tensor(image(rgb)) or torch.is_tensor(image(depth)):
             # device-resident frame: enqueue the stages one by one (estimater.py:255-264)
             e.set_frame(rgb, depth, K, filter_depth=True, zfar=float("inf"))
             pose, canvas = self.refiner.predict(mesh=self.mesh, mesh_tensors=self.mesh_tensors, rgb=rgb, depth=depth, K=K,
@@ -519,7 +522,8 @@ def track_objects(estimators, rgb, depth, K, iteration=2, wait=True, fit_delta=N
     refined as one batch, each rendering its own mesh.  Same poses as the per-object calls; updates every pose_last.
 
     The estimators must share one engine (the default: get_engine()).  Each one keeps its mesh in a slot of that engine,
-    so alternating objects re-uploads nothing.  Host frames only (uint8 (H,W,3) rgb, float32 (H,W) depth).
+    so alternating objects re-uploads nothing.  Host frames only (uint8 (H,W,3) rgb, float32 (H,W) depth, or a
+    Color / Depth of frames.py around host memory).
     Returns a list of (4,4) float32 poses of the original meshes.  wait=False returns a PendingTrack as soon as the call
     is submitted (the frame arrays may then be reused) with every pose_last already set, so the next frame can be
     submitted while the device tracks this one.
@@ -529,7 +533,7 @@ def track_objects(estimators, rgb, depth, K, iteration=2, wait=True, fit_delta=N
     estimators = list(estimators)
     if not estimators:
         return [] if wait else PendingTrack(None, lambda _: [])
-    if torch.is_tensor(rgb) or torch.is_tensor(depth):
+    if torch.is_tensor(rgb) or torch.is_tensor(depth) or on_cuda(rgb) or on_cuda(depth):
         raise TypeError("track_objects takes host frames (numpy); for device-resident frames call track_one per object")
     e = _shared_engine_of(estimators, "track_objects")
     if any(est.pose_last is None for est in estimators):
@@ -583,10 +587,11 @@ def track_cameras(views, iteration=2, wait=True, fit_delta=None):
     estimators share one engine and none appears twice, across cameras or within one; at most MAX_MESHES - 1 objects and
     MAX_CAMERAS cameras with objects.  A camera without estimators gives [] and its frame is not uploaded.  Each
     estimator keeps its mesh in the slot track_objects / register_objects use.  Host frames only (uint8 (H,W,3) rgb,
-    float32 (H,W) depth).  Returns one list of (4,4) float32 poses of the original meshes per camera.  wait=False returns
+    float32 (H,W) depth, or a Color / Depth of frames.py around host memory).  Returns one list of (4,4) float32 poses of the original meshes per camera.  wait=False returns
     a PendingTrack as track_objects does; fit_delta sets every estimator's fit_last as track_objects does."""
     views = [(list(ests), rgb, depth, K) for ests, rgb, depth, K in views]
-    if any(torch.is_tensor(rgb) or torch.is_tensor(depth) for _, rgb, depth, _ in views):
+    if any(torch.is_tensor(rgb) or torch.is_tensor(depth) or on_cuda(rgb) or on_cuda(depth)
+           for _, rgb, depth, _ in views):
         raise TypeError("track_cameras takes host frames (numpy); for device-resident frames call track_one per object")
     used = [v for v in views if v[0]]
     if not used:
@@ -637,12 +642,14 @@ def register_objects(estimators, K, rgb, depth, ob_masks, ob_ids=None, iteration
     its previous state.  Everything comes back to the host in one read-back.
 
     The estimators must share one engine; each keeps its mesh in the same slot track_objects uses, so tracking them
-    afterwards uploads no mesh.  Host frames and masks only (uint8 (H,W,3) rgb, float32 (H,W) depth, (H,W) masks).
+    afterwards uploads no mesh.  Host frames and masks only (uint8 (H,W,3) rgb, float32 (H,W) depth, or a Color / Depth of
+    frames.py around host memory; (H,W) masks).
     Returns a list of (4,4) poses of the original meshes."""
     estimators = list(estimators)
     if not estimators:
         return []
-    if torch.is_tensor(rgb) or torch.is_tensor(depth) or any(torch.is_tensor(m) and m.is_cuda for m in ob_masks):
+    if (torch.is_tensor(rgb) or torch.is_tensor(depth) or on_cuda(rgb) or on_cuda(depth)
+            or any(torch.is_tensor(m) and m.is_cuda for m in ob_masks)):
         raise TypeError("register_objects takes host frames and masks (numpy); for device-resident frames call register per object")
     e = _shared_engine_of(estimators, "register_objects")
     ob_masks = list(ob_masks)
@@ -677,13 +684,13 @@ def register_cameras(views, ob_ids=None, iteration=5):
     one (H,W) mask of its frame per estimator.  ob_ids: None, or one list (or None) per view.  All estimators share one
     engine and none appears twice, across cameras or within one; at most MAX_MESHES - 1 objects and MAX_CAMERAS cameras
     with objects.  A camera without estimators gives [] and its frame is not uploaded.  Host frames and masks only
-    (uint8 (H,W,3) rgb, float32 (H,W) depth).  Returns one list of (4,4) poses of the original meshes per camera."""
+    (uint8 (H,W,3) rgb, float32 (H,W) depth, or a Color / Depth of frames.py around host memory).  Returns one list of (4,4) poses of the original meshes per camera."""
     views = [(list(ests), rgb, depth, K, list(ob_masks)) for ests, rgb, depth, K, ob_masks in views]
     ob_ids = [None] * len(views) if ob_ids is None else list(ob_ids)
     if len(ob_ids) != len(views):
         raise ValueError(f"register_cameras: {len(views)} views but {len(ob_ids)} ob_ids lists")
-    if any(torch.is_tensor(rgb) or torch.is_tensor(depth) or any(torch.is_tensor(m) and m.is_cuda for m in ms)
-           for _, rgb, depth, _, ms in views):
+    if any(torch.is_tensor(rgb) or torch.is_tensor(depth) or on_cuda(rgb) or on_cuda(depth)
+           or any(torch.is_tensor(m) and m.is_cuda for m in ms) for _, rgb, depth, _, ms in views):
         raise TypeError("register_cameras takes host frames and masks (numpy); for device-resident frames call register per object")
     used = [c for c, v in enumerate(views) if v[0]]
     if not used:

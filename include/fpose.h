@@ -235,6 +235,38 @@ int fp_mesh_info(fp_ctx* ctx, int* info);
  * INFINITY for register()).  Asynchronous on `stream`. */
 int fp_set_frame(fp_ctx* ctx, const unsigned char* rgb, const float* depth, const float* K, int H, int W, int flags,
                  float zfar, void* stream);
+/* Frames as sensors deliver them.  Each camera of a context has a frame format, the layout in which every later
+ * frame-taking call reads that camera's rgb and depth buffers: fp_set_frame, fp_track*, fp_track_objects* and
+ * fp_register_objects read camera 0; fp_track_cameras* and fp_register_cameras read camera i in camera i's format.
+ *   color:       FP_COLOR_RGB8 / BGR8 (3 bytes per pixel) or RGBA8 / BGRA8 (4 bytes per pixel, alpha ignored)
+ *   depth:       FP_DEPTH_F32 (float32 metres) or FP_DEPTH_U16 (uint16 units of depth_scale metres: the depth is
+ *                (float)v * depth_scale rounded to nearest in fp32, numpy's v.astype(np.float32) * np.float32(s));
+ *                0 stays invalid depth
+ *   depth_scale: metres per unit (FP_DEPTH_U16 only; finite and > 0)
+ *   rgb_pitch, depth_pitch: bytes from one row to the next (0 = packed rows); pixels within a row are packed
+ * The result of any call is bit-identical to the same call on the frame converted on the host to packed RGB8 and
+ * float32 metres by those expressions.  The default (all zero) is packed RGB8 + float32.  Host frames are staged
+ * packed in their own format (2 bytes per depth pixel for FP_DEPTH_U16); device frames are read in place with their
+ * pitch.  A call copies its cameras' formats when it is staged, so a call already submitted keeps the formats it was
+ * submitted with; this call only records the format (host state: it never waits and enqueues nothing) and refuses an
+ * unknown enum, a FP_DEPTH_U16 scale that is not finite and > 0, or a camera outside [0, FP_MAX_CAMERAS).  fmt = NULL
+ * restores the default.  A frame-taking call refuses, before anything is enqueued, a pitch below the packed row bytes
+ * and a depth pitch or depth pointer not aligned to the depth element size.  The cached graphs read the formats from
+ * the argument block (tracking calls, fp_register_cameras) or take them eagerly: a new format replays them. */
+#define FP_COLOR_RGB8 0
+#define FP_COLOR_BGR8 1
+#define FP_COLOR_RGBA8 2
+#define FP_COLOR_BGRA8 3
+#define FP_DEPTH_F32 0
+#define FP_DEPTH_U16 1
+typedef struct fp_frame_format {
+  int color;
+  int depth;
+  float depth_scale;
+  int rgb_pitch;
+  int depth_pitch;
+} fp_frame_format_t;
+int fp_set_camera_format(fp_ctx* ctx, int camera, const fp_frame_format_t* fmt);
 /* Replaces the xyz map derived by fp_set_frame with the caller's own (PoseRefinePredictor.predict's `xyz_map`
  * argument, predict_pose_refine.py:150,177): float32 [H][W][3], host or device pointer. */
 int fp_set_xyz_map(fp_ctx* ctx, const float* xyz, void* stream);
