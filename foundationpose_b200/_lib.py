@@ -28,6 +28,17 @@ def _load():
 lib = _load()
 
 
+class DepthSensor(C.Structure):
+    """struct fp_depth_sensor (include/fpose.h)."""
+
+    _fields_ = [("H", C.c_int), ("W", C.c_int), ("K", C.c_float * 9), ("T_color_from_depth", C.c_float * 16)]
+
+    @classmethod
+    def of(cls, H, W, K, T):
+        """The record of a depth image of H x W with intrinsics K (9 floats) and T_color_from_depth (16 floats), row-major."""
+        return cls(int(H), int(W), (C.c_float * 9)(*[float(x) for x in K]), (C.c_float * 16)(*[float(x) for x in T]))
+
+
 class GemmLayer(C.Structure):
     """struct fp_gemm_layer (include/fpose.h)."""
 

@@ -123,6 +123,8 @@ enum class GraphKind {
   RegisterRefine = 3,    // fp_register_objects / _cameras: one pass's refinement
   RegisterFeatures = 4,  // fp_register_objects / _cameras: one pass's scorer features
   TrackObjectsFit = 5,   // fp_track_cameras_fit_submit: TrackObjects, then the fit pass at the returned poses
+  TrackObjectsAligned = 6,     // TrackObjects with a camera's depth from its sensor: memset + align ahead of the filter
+  TrackObjectsFitAligned = 7,  // TrackObjectsFit likewise
 };
 
 // Runs `body(stream)` — a fixed sequence of kernel launches (and fixed-address copies) on ctx-owned buffers —
@@ -198,10 +200,15 @@ static int run_graphed(fp_ctx* c, GraphKind kind, int N, int iters, cudaStream_t
 }
 
 // camera 0's filtered frame from rgb_dev / depth_dev in format fmt, with camera 0's record by value (fp_set_frame,
-// fp_register_objects)
+// fp_register_objects).  sensor (non-null: camera 0 has a depth sensor, and depth_dev / fmt are then its aligned buffer
+// and aligned_fmt): the aligned buffer is zeroed and the sensor's depth aligned into it first.
 static int set_frame_launches(fp_ctx* c, const unsigned char* rgb_dev, const float* depth_dev, const FrameFmtDev& fmt,
-                              int flags, float zfar, cudaStream_t st) {
+                              int flags, float zfar, cudaStream_t st, const SensorDev* sensor = nullptr) {
   CameraDev one = camera_dev(c, 0);
+  if (sensor) {
+    FP_CUDA_OK(cudaMemsetAsync(sensor->aligned, 0, (size_t)one.H * one.W * 4, st));
+    FP_TRY(align_depth_launch(*sensor, one, st));
+  }
   one.rgb_raw = rgb_dev;  // camera 0's upload buffers, or the caller's device frame (FP_FRAME_ON_DEVICE)
   one.depth_raw = depth_dev;
   if (flags & FP_FRAME_FILTER_DEPTH) {
@@ -210,24 +217,25 @@ static int set_frame_launches(fp_ctx* c, const unsigned char* rgb_dev, const flo
   }
   const size_t npix = (size_t)one.H * one.W;
   // packed float32 depth is copied as it is; any other depth is converted by the colour kernel
-  const bool depth_as_is = !fmt.u16 && (size_t)fmt.depth_pitch == (size_t)one.W * 4;
+  const bool depth_as_is = fmt.depth_kind == kDepthF32 && (size_t)fmt.depth_pitch == (size_t)one.W * 4;
   FP_TRY(raw_frame_launch(one, fmt, !depth_as_is, st));
   if (depth_as_is) FP_CUDA_OK(cudaMemcpyAsync(one.depth, depth_dev, npix * 4, cudaMemcpyDeviceToDevice, st));
   return depth_to_xyz_launch(one, zfar, st);
 }
 
 // A camera's raw frame of width W in format f: the one place that knows its bytes per pixel, row bytes and pitches.
+// Wd: the width of its depth image, W's unless the camera has a depth sensor.
 struct FrameLayout {
   int rgb_bpp, depth_bpp;          // bytes per pixel
   size_t rgb_row, depth_row;       // bytes per packed row
   long long rgb_pitch, depth_pitch;  // bytes from one row of the caller's buffer to the next
 };
-static FrameLayout frame_layout(const fp_frame_format_t& f, int W) {
+static FrameLayout frame_layout(const fp_frame_format_t& f, int W, int Wd) {
   FrameLayout L;
   L.rgb_bpp = (f.color == FP_COLOR_RGBA8 || f.color == FP_COLOR_BGRA8) ? 4 : 3;
   L.depth_bpp = f.depth == FP_DEPTH_U16 ? 2 : 4;
   L.rgb_row = (size_t)W * L.rgb_bpp;
-  L.depth_row = (size_t)W * L.depth_bpp;
+  L.depth_row = (size_t)Wd * L.depth_bpp;
   L.rgb_pitch = f.rgb_pitch ? f.rgb_pitch : (long long)L.rgb_row;
   L.depth_pitch = f.depth_pitch ? f.depth_pitch : (long long)L.depth_row;
   return L;
@@ -243,16 +251,73 @@ static FrameFmtDev fmt_dev(const fp_frame_format_t& f, const FrameLayout& L, boo
   d.depth_scale = f.depth == FP_DEPTH_U16 ? f.depth_scale : 0.f;
   d.bpp = (unsigned char)L.rgb_bpp;
   d.bgr = (f.color == FP_COLOR_BGR8 || f.color == FP_COLOR_BGRA8) ? 1 : 0;
-  d.u16 = f.depth == FP_DEPTH_U16 ? 1 : 0;
-  d.packed = (d.bpp == 3 && !d.bgr && !d.u16 && (size_t)d.rgb_pitch == L.rgb_row && (size_t)d.depth_pitch == L.depth_row) ? 1 : 0;
+  d.depth_kind = f.depth == FP_DEPTH_U16 ? kDepthU16 : kDepthF32;
+  d.packed = (d.bpp == 3 && !d.bgr && d.depth_kind == kDepthF32 && (size_t)d.rgb_pitch == L.rgb_row &&
+              (size_t)d.depth_pitch == L.depth_row) ? 1 : 0;
   return d;
 }
 
-// Camera i's frame (depth buffer `depth`, width W) against camera i's format: pitches no shorter than a packed row, the
-// depth pitch and pointer aligned to the depth element.  Checked before anything is enqueued.
+// The size of camera i's depth image for a colour frame of H x W: its depth sensor's, or the colour frame's
+static void depth_size(const fp_ctx* c, int i, int H, int W, int& Hd, int& Wd) {
+  Hd = c->has_sensor[i] ? c->sensor[i].H : H;
+  Wd = c->has_sensor[i] ? c->sensor[i].W : W;
+}
+
+// Camera i's aligned buffer (fp_ctx::aligned)
+static unsigned int* aligned_buf(const fp_ctx* c, int i) {
+  return static_cast<unsigned int*>(c->aligned.p) + (size_t)i * c->aligned_stride;
+}
+
+// Sizes the aligned buffers of C cameras for frames of up to npix pixels.  A graph holds the block's address and its
+// memset's size, so growing either moves the epoch.
+static int ensure_aligned(fp_ctx* c, int C, size_t npix) {
+  if (npix > c->aligned_stride) {
+    ++c->epoch;
+    c->aligned_stride = npix;
+  }
+  return dev_alloc(&c->epoch, c->aligned, (size_t)C * c->aligned_stride * 4);
+}
+
+// Camera i's sensor record for the kernels, its raw depth read at `depth` with layout L (in place: the caller's pitch,
+// else the packed rows of the upload buffer); zero (aligned = null) when the camera has no sensor
+static SensorDev sensor_dev(const fp_ctx* c, int i, const void* depth, const FrameLayout& L, bool in_place) {
+  SensorDev d;
+  memset(&d, 0, sizeof d);
+  if (!c->has_sensor[i]) return d;
+  const fp_depth_sensor_t& s = c->sensor[i];
+  d.depth = depth;
+  d.aligned = aligned_buf(c, i);
+  d.pitch = (int)(in_place ? L.depth_pitch : (long long)L.depth_row);
+  d.u16 = c->fmt[i].depth == FP_DEPTH_U16 ? 1 : 0;
+  d.scale = d.u16 ? c->fmt[i].depth_scale : 0.f;
+  d.H = s.H;
+  d.W = s.W;
+  d.fx = s.K[0];
+  d.fy = s.K[4];
+  d.cx = s.K[2];
+  d.cy = s.K[5];
+  for (int k = 0; k < 12; ++k) d.T[k] = s.T_color_from_depth[k];
+  return d;
+}
+
+// The format record of a camera's aligned buffer (colour width W), which the frame filter reads in place of the raw
+// depth: the colour part of f stays, the depth becomes kDepthAligned rows of W slots
+static FrameFmtDev aligned_fmt(FrameFmtDev f, int W) {
+  f.depth_pitch = W * 4;
+  f.depth_scale = 0.f;
+  f.depth_kind = kDepthAligned;
+  f.packed = 0;
+  return f;
+}
+
+// Camera i's frame (depth buffer `depth`, colour width W) against camera i's format: pitches no shorter than a packed
+// row (of the depth sensor's width for the depth of a camera with one), the depth pitch and pointer aligned to the
+// depth element.  Checked before anything is enqueued.
 static int check_frame_format(const fp_ctx* c, int i, const void* depth, int W, const char* caller) {
   const fp_frame_format_t& f = c->fmt[i];
-  const FrameLayout L = frame_layout(f, W);
+  int Hd, Wd;
+  depth_size(c, i, 1, W, Hd, Wd);
+  const FrameLayout L = frame_layout(f, W, Wd);
   FP_REQUIRE(L.rgb_pitch >= (long long)L.rgb_row, "%s: camera %d: rgb pitch %lld bytes is below the %zu bytes of a row", caller,
              i, L.rgb_pitch, L.rgb_row);
   FP_REQUIRE(L.depth_pitch >= (long long)L.depth_row, "%s: camera %d: depth pitch %lld bytes is below the %zu bytes of a row",
@@ -282,9 +347,10 @@ static int copy_rows(void* dst, const void* src, size_t row, long long pitch, in
 // Sizes camera i's buffers for npix pixels: the filtered frame always, the raw upload if `raw`.  Camera 0's addresses
 // are held by the graphs that take the frame by value, so growing its buffers bumps the graph epoch.  Cameras 1.. are
 // reached only through the camera table, which every call rewrites: growing them invalidates no graph.
-// The raw upload holds rgb_bpp / depth_bpp bytes per pixel (the frame format's); buffers only grow, so a camera that
-// alternates between formats of a size it has seen allocates nothing after the first time.
-static int alloc_camera(fp_ctx* c, int i, size_t npix, bool raw, int rgb_bpp = 3, int depth_bpp = 4) {
+// The raw upload holds rgb_bpp / depth_bpp bytes per pixel (the frame format's), the depth one for depth_npix pixels
+// (0: npix; a depth sensor's image); buffers only grow, so a camera that alternates between formats of a size it has
+// seen allocates nothing after the first time.
+static int alloc_camera(fp_ctx* c, int i, size_t npix, bool raw, int rgb_bpp = 3, int depth_bpp = 4, size_t depth_npix = 0) {
   CameraBufs& b = c->cam[i];
   unsigned long long* epoch = i == 0 ? &c->epoch : nullptr;
   FP_TRY(dev_alloc(epoch, b.rgba, npix * 4));
@@ -292,7 +358,7 @@ static int alloc_camera(fp_ctx* c, int i, size_t npix, bool raw, int rgb_bpp = 3
   FP_TRY(dev_alloc(epoch, b.xyz, npix * 16));
   if (raw) {
     FP_TRY(dev_alloc(epoch, b.rgb_raw, npix * rgb_bpp));
-    FP_TRY(dev_alloc(epoch, b.depth_raw, npix * depth_bpp));
+    FP_TRY(dev_alloc(epoch, b.depth_raw, (depth_npix ? depth_npix : npix) * depth_bpp));
   }
   return 0;
 }
@@ -350,12 +416,13 @@ static int stage_copy(void* dst, PinnedBuf& stage, const void* src, size_t bytes
   return stage_rows(dst, stage, src, bytes, (long long)bytes, 1, st);
 }
 
-// Uploads one camera's frame (H rows of layout L) through its staging (free: the set is not busy).  The two uploads are
-// issued as soon as their staging copy is done — the depth DMA runs under the host's rgb copy, the rgb DMA under the
-// next camera's copies or the graph launch — instead of being nodes of the graph (measured: -40 us per frame)
+// Uploads one camera's frame (H rows of rgb and Hd rows of depth of layout L) through its staging (free: the set is not
+// busy).  The two uploads are issued as soon as their staging copy is done — the depth DMA runs under the host's rgb
+// copy, the rgb DMA under the next camera's copies or the graph launch — instead of being nodes of the graph (measured:
+// -40 us per frame)
 static int upload_staged_frame(CameraBufs& b, PinnedBuf& stage_rgb, PinnedBuf& stage_depth, const unsigned char* rgb_host,
-                               const void* depth_host, const FrameLayout& L, int H, cudaStream_t st) {
-  FP_TRY(stage_rows(b.depth_raw.p, stage_depth, depth_host, L.depth_row, L.depth_pitch, H, st));
+                               const void* depth_host, const FrameLayout& L, int H, int Hd, cudaStream_t st) {
+  FP_TRY(stage_rows(b.depth_raw.p, stage_depth, depth_host, L.depth_row, L.depth_pitch, Hd, st));
   return stage_rows(b.rgb_raw.p, stage_rgb, rgb_host, L.rgb_row, L.rgb_pitch, H, st);
 }
 
@@ -445,8 +512,9 @@ int order_after_track(fp_ctx* c, cudaStream_t st) {
 }
 
 constexpr size_t kTableBytes = sizeof(CameraDev) * kMaxCameras;  // the camera table at the head of fp_ctx::args
-constexpr size_t kHeadBytes = kTableBytes + sizeof(FrameFmtDev) * kMaxCameras;  // then the cameras' frame formats
-// fp_ctx::args (and its staging) for `rows` slot and camera ids: the two tables, the ids, and a tracking call's fit
+constexpr size_t kSensorsAt = kTableBytes + sizeof(FrameFmtDev) * kMaxCameras;  // then the cameras' frame formats
+constexpr size_t kHeadBytes = kSensorsAt + sizeof(SensorDev) * kMaxCameras;  // then the cameras' depth sensors
+// fp_ctx::args (and its staging) for `rows` slot and camera ids: the three tables, the ids, and a tracking call's fit
 // threshold
 static size_t args_bytes(int rows) { return kHeadBytes + (size_t)2 * rows * sizeof(int) + sizeof(float); }
 
@@ -460,54 +528,77 @@ static size_t args_bytes(int rows) { return kHeadBytes + (size_t)2 * rows * size
 // uploaded for it.  Every camera still gets its raw upload buffers, so where a frame lives never changes an allocation
 // or the graph epoch.  Each camera's frame is read in its format (fp_ctx::fmt, copied into the format table beside the
 // camera table here): host frames are staged packed, at the format's bytes per pixel, device frames are read with their
-// pitch; the raw buffers are sized for the largest frame and the widest pixels of the call.  H_max / W_max: the largest
-// frame height and width of the call.  `set`: the staging set the call uploads through (not busy).
+// pitch; the raw buffers are sized for the largest frame and the widest pixels of the call.  A camera with a depth
+// sensor (fp_ctx::sensor, copied into the sensor table here) has its raw depth staged or read at the sensor's size, its
+// table entry reads its aligned buffer as depth (aligned_fmt), and the call's aligned buffers are sized.
+// `set`: the staging set the call uploads through (not busy).
+struct CallFrames {
+  int H_max = 0, W_max = 0;    // the largest frame height and width of the call
+  bool aligned = false;        // some camera of the call has a depth sensor
+  int Hd_max = 0, Wd_max = 0;  // the largest depth image of those cameras
+};
 static int setup_cameras(fp_ctx* c, StagingSet& set, int C, const unsigned char* const* rgb, const float* const* depth,
                          const FrameSources& on_dev, const float* K, const int* H, const int* W, int rows, int staged_rows,
-                         cudaStream_t st, int& H_max, int& W_max) {
-  size_t npix_max = 0;
+                         cudaStream_t st, CallFrames& g) {
+  size_t npix_max = 0, depth_npix_max = 0;
   int rgb_bpp = 0, depth_bpp = 0;
-  H_max = W_max = 0;
+  g = CallFrames{};
   for (int i = 0; i < C; ++i) {
     npix_max = std::max(npix_max, (size_t)H[i] * W[i]);
-    H_max = std::max(H_max, H[i]);
-    W_max = std::max(W_max, W[i]);
-    const FrameLayout L = frame_layout(c->fmt[i], W[i]);
+    g.H_max = std::max(g.H_max, H[i]);
+    g.W_max = std::max(g.W_max, W[i]);
+    int Hd, Wd;
+    depth_size(c, i, H[i], W[i], Hd, Wd);
+    depth_npix_max = std::max(depth_npix_max, (size_t)Hd * Wd);
+    if (c->has_sensor[i]) {
+      g.aligned = true;
+      g.Hd_max = std::max(g.Hd_max, Hd);
+      g.Wd_max = std::max(g.Wd_max, Wd);
+    }
+    const FrameLayout L = frame_layout(c->fmt[i], W[i], Wd);
     rgb_bpp = std::max(rgb_bpp, L.rgb_bpp);
     depth_bpp = std::max(depth_bpp, L.depth_bpp);
   }
   for (int i = 0; i < C; ++i) {
-    FP_TRY(alloc_camera(c, i, npix_max, /*raw=*/true, rgb_bpp, depth_bpp));
+    FP_TRY(alloc_camera(c, i, npix_max, /*raw=*/true, rgb_bpp, depth_bpp, depth_npix_max));
     if (!on_dev.rgb[i]) FP_TRY(pinned_alloc(nullptr, set.rgb[i], npix_max * rgb_bpp));
-    if (!on_dev.depth[i]) FP_TRY(pinned_alloc(nullptr, set.depth[i], npix_max * depth_bpp));
+    if (!on_dev.depth[i]) FP_TRY(pinned_alloc(nullptr, set.depth[i], depth_npix_max * depth_bpp));
   }
+  if (g.aligned) FP_TRY(ensure_aligned(c, C, npix_max));
   c->n_frames = C;
   FP_TRY(dev_alloc(&c->epoch, c->args, args_bytes(rows)));
   FP_TRY(pinned_alloc(nullptr, set.args, args_bytes(staged_rows)));
   CameraDev* table = reinterpret_cast<CameraDev*>(set.args.p);
   FrameFmtDev* fmts = reinterpret_cast<FrameFmtDev*>(static_cast<char*>(set.args.p) + kTableBytes);
+  SensorDev* sensors = reinterpret_cast<SensorDev*>(static_cast<char*>(set.args.p) + kSensorsAt);
   memset(table, 0, kHeadBytes);
   for (int i = 0; i < C; ++i) {
     set_frame_geometry(c, i, K + 9 * i, H[i], W[i]);
     table[i] = camera_dev(c, i);
     if (on_dev.rgb[i]) table[i].rgb_raw = rgb[i];
     if (on_dev.depth[i]) table[i].depth_raw = depth[i];
-    const FrameLayout L = frame_layout(c->fmt[i], W[i]);
+    int Hd, Wd;
+    depth_size(c, i, H[i], W[i], Hd, Wd);
+    const FrameLayout L = frame_layout(c->fmt[i], W[i], Wd);
     fmts[i] = fmt_dev(c->fmt[i], L, on_dev.rgb[i], on_dev.depth[i]);
+    if (c->has_sensor[i]) {
+      sensors[i] = sensor_dev(c, i, table[i].depth_raw, L, on_dev.depth[i]);
+      table[i].depth_raw = reinterpret_cast<const float*>(sensors[i].aligned);
+      fmts[i] = aligned_fmt(fmts[i], W[i]);
+    }
     // the order of upload_staged_frame: depth, then rgb
-    if (!on_dev.depth[i]) FP_TRY(stage_rows(c->cam[i].depth_raw.p, set.depth[i], depth[i], L.depth_row, L.depth_pitch, H[i], st));
+    if (!on_dev.depth[i]) FP_TRY(stage_rows(c->cam[i].depth_raw.p, set.depth[i], depth[i], L.depth_row, L.depth_pitch, Hd, st));
     if (!on_dev.rgb[i]) FP_TRY(stage_rows(c->cam[i].rgb_raw.p, set.rgb[i], rgb[i], L.rgb_row, L.rgb_pitch, H[i], st));
   }
   return 0;
 }
 
 // The staging uploads of one tracking call: the frames, then the camera table, the slot ids, the camera ids and, with a
-// fit (delta non-null), its threshold in one copy to the argument block.  H_max / W_max as setup_cameras.
+// fit (delta non-null), its threshold in one copy to the argument block.  g as setup_cameras.
 static int stage_track_call(fp_ctx* c, StagingSet& set, int C, const unsigned char* const* rgb, const float* const* depth,
                             const FrameSources& on_dev, const float* K, const int* H, const int* W, int M,
-                            const int* camera_of, const int* slots_host, const float* delta, cudaStream_t st, int& H_max,
-                            int& W_max) {
-  FP_TRY(setup_cameras(c, set, C, rgb, depth, on_dev, K, H, W, M, M, st, H_max, W_max));
+                            const int* camera_of, const int* slots_host, const float* delta, cudaStream_t st, CallFrames& g) {
+  FP_TRY(setup_cameras(c, set, C, rgb, depth, on_dev, K, H, W, M, M, st, g));
   int* ids = reinterpret_cast<int*>(static_cast<char*>(set.args.p) + kHeadBytes);
   memcpy(ids, slots_host, (size_t)M * sizeof(int));
   memcpy(ids + M, camera_of, (size_t)M * sizeof(int));
@@ -556,21 +647,28 @@ static int track_cameras_submit(fp_ctx* c, const char* caller, int C, const unsi
     FP_TRY(pinned_alloc(nullptr, rb->fit, fit_bytes));
   }
   c->has_frame = false;
-  int H_max = 0, W_max = 0;
-  const int staged =
-      stage_track_call(c, *set, C, rgb, depth, on_dev, K, H, W, M, camera_of, slots_host, delta, st, H_max, W_max);
+  CallFrames g;
+  const int staged = stage_track_call(c, *set, C, rgb, depth, on_dev, K, H, W, M, camera_of, slots_host, delta, st, g);
   // whatever was staged before a failure is still on its way out: the set stays busy until then
   FP_TRY(set_busy(*set, st));
   FP_TRY(staged);
-  if (H_max > c->cam_grid_h || W_max > c->cam_grid_w) {
+  if (g.H_max > c->cam_grid_h || g.W_max > c->cam_grid_w) {
     // the frame-preparation grid is a by-value launch parameter: it covers the largest frame seen, the blocks outside
     // a smaller frame return at once
     ++c->epoch;
-    c->cam_grid_h = std::max(c->cam_grid_h, H_max);
-    c->cam_grid_w = std::max(c->cam_grid_w, W_max);
+    c->cam_grid_h = std::max(c->cam_grid_h, g.H_max);
+    c->cam_grid_w = std::max(c->cam_grid_w, g.W_max);
+  }
+  if (g.aligned && (g.Hd_max > c->sensor_grid_h || g.Wd_max > c->sensor_grid_w)) {
+    // the alignment grid likewise covers the largest depth image seen
+    ++c->epoch;
+    c->sensor_grid_h = std::max(c->sensor_grid_h, g.Hd_max);
+    c->sensor_grid_w = std::max(c->sensor_grid_w, g.Wd_max);
   }
   const CameraDev* cams_dev = reinterpret_cast<const CameraDev*>(c->args.p);
   const FrameFmtDev* fmts_dev = reinterpret_cast<const FrameFmtDev*>(static_cast<const char*>(c->args.p) + kTableBytes);
+  const SensorDev* sensors_dev = reinterpret_cast<const SensorDev*>(static_cast<const char*>(c->args.p) + kSensorsAt);
+  const size_t aligned_bytes = (size_t)C * c->aligned_stride * 4;
   const int* mesh_of = reinterpret_cast<const int*>(static_cast<const char*>(c->args.p) + kHeadBytes);
   const int* cam_of = mesh_of + M;
   const float* delta_dev = reinterpret_cast<const float*>(cam_of + M);
@@ -580,10 +678,17 @@ static int track_cameras_submit(fp_ctx* c, const char* caller, int C, const unsi
   FP_CUDA_OK(cudaMemcpyAsync(pa, poses_in_dev, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
   const float* fin = (iterations % 2 == 0) ? pa : pb;
   const int grid_h = c->cam_grid_h, grid_w = c->cam_grid_w;
+  const int sgrid_h = c->sensor_grid_h, sgrid_w = c->sensor_grid_w;
   auto body = [&](cudaStream_t s2) -> int {
     // the counts are zeroed at the head of the sequence, so the fit pass follows the last pose update by programmatic
     // dependent launch like every other link of the chain
     if (delta) FP_CUDA_OK(cudaMemsetAsync(fit, 0, fit_bytes, s2));
+    if (g.aligned) {
+      // the depth of the cameras with a sensor aligned into their zeroed aligned buffers, which the frame filter (an
+      // ordinary launch, after this one in stream order) reads as their depth
+      FP_CUDA_OK(cudaMemsetAsync(c->aligned.p, 0, aligned_bytes, s2));
+      FP_TRY(align_depth_cameras_launch(sensors_dev, cams_dev, C, sgrid_h, sgrid_w, s2));
+    }
     // estimater.py:250-268 for every object of every camera at once: each camera's frame filtered once (erode +
     // bilateral, depth2xyzmap_batch(zfar = inf)), M hypotheses each rendering its own mesh and cropping its own
     // camera's frame
@@ -593,7 +698,9 @@ static int track_cameras_submit(fp_ctx* c, const char* caller, int C, const unsi
     if (delta) FP_TRY(make_crops(c, fin, M, 0, nullptr, nullptr, nullptr, s2, mesh_of, cams_dev, cam_of, nullptr, fit, delta_dev));
     return 0;
   };
-  FP_TRY(run_graphed(c, delta ? GraphKind::TrackObjectsFit : GraphKind::TrackObjects, M, iterations, st, body, C));
+  const GraphKind kind = g.aligned ? (delta ? GraphKind::TrackObjectsFitAligned : GraphKind::TrackObjectsAligned)
+                                   : (delta ? GraphKind::TrackObjectsFit : GraphKind::TrackObjects);
+  FP_TRY(run_graphed(c, kind, M, iterations, st, body, C));
   c->has_frame = true;
   if (poses_out_dev) FP_CUDA_OK(cudaMemcpyAsync(poses_out_dev, fin, (size_t)M * 64, cudaMemcpyDeviceToDevice, st));
   if (fit_out_dev) FP_CUDA_OK(cudaMemcpyAsync(fit_out_dev, fit, fit_bytes, cudaMemcpyDeviceToDevice, st));
@@ -637,6 +744,20 @@ int check_slots(const fp_ctx* c, int M, const int* slots, const char* caller) {
                kMaxMeshes);
     FP_REQUIRE(c->mesh[slots[i]].loaded, "%s: object %d: slot %d holds no mesh", caller, i, slots[i]);
   }
+  return 0;
+}
+
+// A depth sensor's values (fp_set_camera_depth_sensor, fp_align_depth): a size the kernels index in int, finite
+// intrinsics and transform, and focal lengths > 0
+int check_depth_sensor(const fp_depth_sensor_t* s, const char* caller) {
+  FP_REQUIRE(s->H >= 1 && s->H <= FP_DEPTH_SENSOR_MAX_DIM && s->W >= 1 && s->W <= FP_DEPTH_SENSOR_MAX_DIM,
+             "%s: depth image %d x %d outside [1, %d]", caller, s->H, s->W, FP_DEPTH_SENSOR_MAX_DIM);
+  for (int k = 0; k < 9; ++k) FP_REQUIRE(isfinite(s->K[k]), "%s: K[%d] = %g is not finite", caller, k, (double)s->K[k]);
+  for (int k = 0; k < 16; ++k)
+    FP_REQUIRE(isfinite(s->T_color_from_depth[k]), "%s: T_color_from_depth[%d] = %g is not finite", caller, k,
+               (double)s->T_color_from_depth[k]);
+  FP_REQUIRE(s->K[0] > 0.f && s->K[4] > 0.f, "%s: focal lengths fx = %g, fy = %g must be > 0", caller, (double)s->K[0],
+             (double)s->K[4]);
   return 0;
 }
 
@@ -733,8 +854,8 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
   if (staged_masks) FP_TRY(pinned_alloc(nullptr, set->masks, mask_bytes));
   FP_TRY(pinned_alloc(nullptr, set->ints, (size_t)(2 * M + 2) * sizeof(int) + (size_t)M * sizeof(size_t)));
   c->has_frame = false;
-  int H_max, W_max;
-  FP_TRY(setup_cameras(c, *set, C, rgb, depth, on_dev, K, H, W, max_pass, total, st, H_max, W_max));
+  CallFrames g;
+  FP_TRY(setup_cameras(c, *set, C, rgb, depth, on_dev, K, H, W, max_pass, total, st, g));
   int* ints = reinterpret_cast<int*>(set->ints.p);
   size_t* stage_mask_off = reinterpret_cast<size_t*>(ints + 2 * M + 2);
   memcpy(ints, off.data(), (size_t)(M + 1) * sizeof(int));
@@ -774,12 +895,19 @@ static int register_cameras_body(fp_ctx* c, int C, const unsigned char* const* r
     const unsigned char* rgb0 = on_dev.rgb[0] ? rgb[0] : static_cast<const unsigned char*>(c->cam[0].rgb_raw.p);
     const float* depth0 = on_dev.depth[0] ? depth[0] : static_cast<const float*>(c->cam[0].depth_raw.p);
     const FrameFmtDev fmt0 = *reinterpret_cast<const FrameFmtDev*>(static_cast<const char*>(set->args.p) + kTableBytes);
-    FP_TRY(set_frame_launches(c, rgb0, depth0, fmt0, FP_FRAME_FILTER_DEPTH, INFINITY, st));
+    const SensorDev s0 = *reinterpret_cast<const SensorDev*>(static_cast<const char*>(set->args.p) + kSensorsAt);
+    if (s0.aligned) depth0 = reinterpret_cast<const float*>(s0.aligned);  // fmt0 is then aligned_fmt
+    FP_TRY(set_frame_launches(c, rgb0, depth0, fmt0, FP_FRAME_FILTER_DEPTH, INFINITY, st, s0.aligned ? &s0 : nullptr));
   } else {
     const FrameFmtDev* fmts_dev = reinterpret_cast<const FrameFmtDev*>(static_cast<const char*>(c->args.p) + kTableBytes);
     FP_CUDA_OK(cudaMemcpyAsync(c->args.p, set->args.p, kHeadBytes, cudaMemcpyHostToDevice, st));
     FP_CUDA_OK(cudaMemcpyAsync(c->mask_off.p, stage_mask_off, (size_t)M * sizeof(size_t), cudaMemcpyHostToDevice, st));
-    FP_TRY(frame_prep_cameras_launch(cams_dev, fmts_dev, C, H_max, W_max, INFINITY, st));
+    if (g.aligned) {
+      const SensorDev* sensors_dev = reinterpret_cast<const SensorDev*>(static_cast<const char*>(c->args.p) + kSensorsAt);
+      FP_CUDA_OK(cudaMemsetAsync(c->aligned.p, 0, (size_t)C * c->aligned_stride * 4, st));
+      FP_TRY(align_depth_cameras_launch(sensors_dev, cams_dev, C, g.Hd_max, g.Wd_max, st));
+    }
+    FP_TRY(frame_prep_cameras_launch(cams_dev, fmts_dev, C, g.H_max, g.W_max, INFINITY, st));
   }
   c->has_frame = true;
   // estimater.py:137-156, :203-209 for every object in one launch pair; the start poses go to poses_out_dev and are
@@ -970,6 +1098,23 @@ int fp_set_camera_format(fp_ctx* c, int camera, const fp_frame_format_t* fmt) {
   FP_API_END
 }
 
+int fp_set_camera_depth_sensor(fp_ctx* c, int camera, const fp_depth_sensor_t* s) {
+  FP_API_BEGIN
+  FP_REQUIRE(c, "fp_set_camera_depth_sensor: null ctx");
+  FP_REQUIRE(camera >= 0 && camera < kMaxCameras, "fp_set_camera_depth_sensor: camera %d out of range [0, %d)", camera,
+             kMaxCameras);
+  if (!s) {
+    c->has_sensor[camera] = false;
+    c->sensor[camera] = fp_depth_sensor_t{};
+    return 0;
+  }
+  FP_TRY(check_depth_sensor(s, "fp_set_camera_depth_sensor"));
+  c->sensor[camera] = *s;
+  c->has_sensor[camera] = true;
+  return 0;
+  FP_API_END
+}
+
 int fp_mesh_info(fp_ctx* c, int* info) {
   FP_API_BEGIN
   FP_REQUIRE(c && info && c->mesh[0].loaded, "fp_mesh_info: no mesh");
@@ -995,8 +1140,11 @@ int fp_set_frame(fp_ctx* c, const unsigned char* rgb, const float* depth, const 
   const size_t npix = (size_t)H * W;
   c->has_frame = false;
   const bool on_dev = (flags & FP_FRAME_ON_DEVICE) != 0;
-  const FrameLayout L = frame_layout(c->fmt[0], W);
-  FP_TRY(alloc_camera(c, 0, npix, /*raw=*/!on_dev, L.rgb_bpp, L.depth_bpp));
+  int Hd, Wd;  // the depth image: the colour frame's size, or its depth sensor's
+  depth_size(c, 0, H, W, Hd, Wd);
+  const FrameLayout L = frame_layout(c->fmt[0], W, Wd);
+  FP_TRY(alloc_camera(c, 0, npix, /*raw=*/!on_dev, L.rgb_bpp, L.depth_bpp, (size_t)Hd * Wd));
+  if (c->has_sensor[0]) FP_TRY(ensure_aligned(c, 1, npix));
   set_frame_geometry(c, 0, K, H, W);
   c->n_frames = 1;
   const unsigned char* rgb_dev = rgb;
@@ -1006,18 +1154,24 @@ int fp_set_frame(fp_ctx* c, const unsigned char* rgb, const float* depth, const 
     if (residence(c, rgb) == Residence::Pageable || residence(c, depth) == Residence::Pageable) {
       StagingSet* set;
       FP_TRY(take_set(c, set));
-      const int staged = upload_staged_frame(f, set->rgb[0], set->depth[0], rgb, depth, L, H, st);
+      const int staged = upload_staged_frame(f, set->rgb[0], set->depth[0], rgb, depth, L, H, Hd, st);
       FP_TRY(set_busy(*set, st));
       FP_TRY(staged);
     } else {
       // page-locked frames, fp_group_register's among them, are read in place: one host copy fewer
       FP_TRY(copy_rows(f.rgb_raw.p, rgb, L.rgb_row, L.rgb_pitch, H, st));
-      FP_TRY(copy_rows(f.depth_raw.p, depth, L.depth_row, L.depth_pitch, H, st));
+      FP_TRY(copy_rows(f.depth_raw.p, depth, L.depth_row, L.depth_pitch, Hd, st));
     }
     rgb_dev = reinterpret_cast<const unsigned char*>(f.rgb_raw.p);
     depth_dev = reinterpret_cast<const float*>(f.depth_raw.p);
   }
-  FP_TRY(set_frame_launches(c, rgb_dev, depth_dev, fmt_dev(c->fmt[0], L, on_dev, on_dev), flags, zfar, st));
+  FrameFmtDev fmt = fmt_dev(c->fmt[0], L, on_dev, on_dev);
+  if (c->has_sensor[0]) {
+    const SensorDev s = sensor_dev(c, 0, depth_dev, L, on_dev);
+    FP_TRY(set_frame_launches(c, rgb_dev, reinterpret_cast<const float*>(s.aligned), aligned_fmt(fmt, W), flags, zfar, st, &s));
+  } else {
+    FP_TRY(set_frame_launches(c, rgb_dev, depth_dev, fmt, flags, zfar, st));
+  }
   c->has_frame = true;
   return 0;
   FP_API_END

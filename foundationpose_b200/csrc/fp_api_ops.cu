@@ -8,6 +8,10 @@
 #include "fp_depth.cuh"
 #include "fp_gemm.cuh"
 
+#include <math.h>
+#include <stdint.h>
+#include <string.h>
+
 #include <vector>
 
 namespace fp {
@@ -279,6 +283,65 @@ int fp_pose_errors(const float* pts, int P, const float* pred, int N, const floa
   for (int i = 0; i < 5; ++i)
     if (ptrs[i] && check_device_ptr(ptrs[i], names[i])) return -1;
   return fp::pose_errors_launch(pts, P, pred, N, gt, n_gt, add_out, adds_out, reinterpret_cast<cudaStream_t>(stream));
+  FP_API_END
+}
+
+int fp_align_depth(const void* depth, int depth_format, float depth_scale, long long depth_pitch, const fp_depth_sensor_t* s,
+                   const float* K_color, int H, int W, float* out, void* stream) {
+  FP_API_BEGIN
+  const char* fn = "fp_align_depth";
+  FP_REQUIRE(depth && s && K_color && out, "%s: null argument", fn);
+  FP_TRY(check_depth_sensor(s, fn));
+  FP_REQUIRE(depth_format == FP_DEPTH_F32 || depth_format == FP_DEPTH_U16, "%s: unknown depth format %d", fn, depth_format);
+  FP_REQUIRE(depth_format != FP_DEPTH_U16 || (isfinite(depth_scale) && depth_scale > 0.f),
+             "%s: uint16 depth scale %g must be finite and > 0 (metres per unit)", fn, (double)depth_scale);
+  FP_REQUIRE(H >= 1 && W >= 1 && (long long)H * W <= 0x7fffffffLL, "%s: colour frame %d x %d is empty or too large", fn, H,
+             W);
+  {
+    // K_color is read on the host
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, K_color) != cudaSuccess)
+      cudaGetLastError();
+    else
+      FP_REQUIRE(a.type != cudaMemoryTypeDevice, "%s: K_color is device memory; it is read on the host", fn);
+  }
+  for (int k = 0; k < 9; ++k) FP_REQUIRE(isfinite(K_color[k]), "%s: K_color[%d] = %g is not finite", fn, k, (double)K_color[k]);
+  const int bpp = depth_format == FP_DEPTH_U16 ? 2 : 4;
+  const long long row = (long long)s->W * bpp, pitch = depth_pitch ? depth_pitch : row;
+  FP_REQUIRE(pitch >= row && pitch <= 0x7fffffffLL, "%s: depth pitch %lld bytes is below the %lld bytes of a row or too large", fn,
+             pitch, row);
+  FP_REQUIRE(pitch % bpp == 0, "%s: depth pitch %lld bytes is not a multiple of the %d-byte depth value", fn, pitch, bpp);
+  FP_REQUIRE(reinterpret_cast<uintptr_t>(depth) % bpp == 0, "%s: depth buffer %p is not aligned to its %d-byte depth value", fn,
+             depth, bpp);
+  FP_REQUIRE(reinterpret_cast<uintptr_t>(out) % 4 == 0, "%s: out %p is not aligned to 4 bytes", fn, (const void*)out);
+  if (check_device_ptr(depth, "depth", fn) || check_device_ptr(out, "out", fn)) return -1;
+  SensorDev d;
+  memset(&d, 0, sizeof d);
+  d.depth = depth;
+  d.aligned = reinterpret_cast<unsigned int*>(out);
+  d.pitch = (int)pitch;
+  d.u16 = depth_format == FP_DEPTH_U16 ? 1 : 0;
+  d.scale = d.u16 ? depth_scale : 0.f;
+  d.H = s->H;
+  d.W = s->W;
+  d.fx = s->K[0];
+  d.fy = s->K[4];
+  d.cx = s->K[2];
+  d.cy = s->K[5];
+  for (int k = 0; k < 12; ++k) d.T[k] = s->T_color_from_depth[k];
+  CameraDev colour;  // the colour frame's size and intrinsics, as a call's K gives them
+  memset(&colour, 0, sizeof colour);
+  colour.fx = K_color[0];
+  colour.fy = K_color[4];
+  colour.cx = K_color[2];
+  colour.cy = K_color[5];
+  colour.H = H;
+  colour.W = W;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const size_t npix = (size_t)H * W;
+  FP_CUDA_OK(cudaMemsetAsync(out, 0, npix * 4, st));
+  FP_TRY(align_depth_launch(d, colour, st));
+  return aligned_to_depth_launch(d.aligned, npix, st);
   FP_API_END
 }
 

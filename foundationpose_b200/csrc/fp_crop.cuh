@@ -70,23 +70,56 @@ static_assert(sizeof(CameraDev) == 64, "camera table entry: four uint4s");
 // How a camera's raw frame (CameraDev::rgb_raw / depth_raw) is laid out (fp_frame_format_t, resolved by the host for
 // where the frame is read: the caller's pitch in place, the packed row bytes once staged).  Only the frame preparation
 // reads it, by value or from the format table beside the camera table.
+// FrameFmtDev::depth_kind: how a raw depth frame stores its values
+constexpr unsigned char kDepthF32 = 0;      // float32 metres
+constexpr unsigned char kDepthU16 = 1;      // uint16 * depth_scale
+constexpr unsigned char kDepthAligned = 2;  // a camera's aligned buffer (align_depth_kernel): uint32 slots, 0 = no depth
 struct __align__(16) FrameFmtDev {
   int rgb_pitch;      // bytes per rgb row
   int depth_pitch;    // bytes per depth row
-  float depth_scale;  // metres per unit (u16)
+  float depth_scale;  // metres per unit (kDepthU16)
   unsigned char bpp;  // rgb bytes per pixel: 3 or 4
   unsigned char bgr;  // 1: channel order B, G, R
-  unsigned char u16;  // 1: uint16 depth * depth_scale, else float32 metres
+  unsigned char depth_kind;  // kDepthF32, kDepthU16 or kDepthAligned
   unsigned char packed;  // 1: packed RGB8 + float32, the layout frames had before formats (read without the fields above)
 };
 static_assert(sizeof(FrameFmtDev) == 16, "format table entry: one uint4");
 
+// A camera's depth sensor (fp_set_camera_depth_sensor) as align_depth_kernel reads it: the raw depth image of the
+// sensor, H x W, `pitch` bytes per row, float32 metres or uint16 * scale; its intrinsics; the top three rows of
+// T_color_from_depth; and the camera's aligned buffer ([H][W] of the colour frame, uint32 slots, zeroed before the
+// launch).  aligned = null: the camera has no sensor.  By value (camera 0) or from the sensor table beside the format
+// table.
+struct __align__(16) SensorDev {
+  const void* depth;
+  unsigned int* aligned;
+  int pitch, u16;
+  float scale;
+  int H, W;
+  float fx, fy, cx, cy;
+  float T[12];
+};
+static_assert(sizeof(SensorDev) == 112, "sensor table entry: seven uint4s");
+
 #ifdef __CUDACC__
-// Pixel (v, u) of a raw depth frame in metres: float32 as stored, or uint16 * scale in one fp32 multiply rounded to
-// nearest (no contraction), numpy's v.astype(np.float32) * np.float32(scale)
+// An aligned buffer's slot for depth z: the complement of an order key (unsigned order of the keys = float order of the
+// values, negative ones included), so an atomicMax over a zeroed buffer keeps the smallest z whatever the order of the
+// writes, and 0 (the key of a NaN, which is never stored) means no depth.
+__device__ __forceinline__ unsigned int aligned_slot_of(float z) {
+  const unsigned int b = __float_as_uint(z);
+  return ~((b & 0x80000000u) ? ~b : (b | 0x80000000u));
+}
+__device__ __forceinline__ float aligned_depth_of(unsigned int s) {
+  if (s == 0u) return 0.f;
+  const unsigned int key = ~s;
+  return __uint_as_float((key & 0x80000000u) ? (key & 0x7fffffffu) : ~key);
+}
+// Pixel (v, u) of a raw depth frame in metres: float32 as stored, uint16 * scale in one fp32 multiply rounded to
+// nearest (no contraction), numpy's v.astype(np.float32) * np.float32(scale), or an aligned buffer's slot
 __device__ __forceinline__ float raw_depth_at(const float* base, const FrameFmtDev& f, int v, int u) {
   const char* row = reinterpret_cast<const char*>(base) + (size_t)v * f.depth_pitch;
-  if (f.u16) return __fmul_rn((float)__ldg(reinterpret_cast<const unsigned short*>(row) + u), f.depth_scale);
+  if (f.depth_kind == kDepthU16) return __fmul_rn((float)__ldg(reinterpret_cast<const unsigned short*>(row) + u), f.depth_scale);
+  if (f.depth_kind == kDepthAligned) return aligned_depth_of(__ldg(reinterpret_cast<const unsigned int*>(row) + u));
   return __ldg(reinterpret_cast<const float*>(row) + u);
 }
 // Pixel (v, u) of a raw colour frame as the context's RGBA8

@@ -204,6 +204,14 @@ struct fp_ctx {
   int n_frames = 0;  // the last call prepared the frames of cameras 0 .. n_frames - 1
   // every camera's frame format (fp_set_camera_format; all zero = packed RGB8 + float32), read when a call is staged
   fp_frame_format_t fmt[fp::kMaxCameras] = {};
+  // every camera's depth sensor (fp_set_camera_depth_sensor), read when a call is staged; has_sensor false: the depth
+  // is in the colour frame's geometry
+  fp_depth_sensor_t sensor[fp::kMaxCameras] = {};
+  bool has_sensor[fp::kMaxCameras] = {};
+  // the aligned buffers of a call's cameras: camera i's [H][W] uint32 slots at slot i * aligned_stride, zeroed by one
+  // memset per call and scattered into by align_depth_kernel; aligned_stride only grows (and moves the graph epoch)
+  fp::DevBuf aligned;
+  size_t aligned_stride = 0;
   bool has_frame = false;
   // workspaces (sized for cap_n hypotheses)
   int cap_n = 0;
@@ -250,6 +258,7 @@ struct fp_ctx {
   fp::DevBuf args;
   fp::DevBuf fit;  // the fit counts of the last tracking call with a fit, [M][FP_FIT_COUNTS] int32 (a graph holds it)
   int cam_grid_h = 0, cam_grid_w = 0;  // the tracking calls' frame-preparation grid: the largest frame seen
+  int sensor_grid_h = 0, sensor_grid_w = 0;  // the tracking calls' alignment grid: the largest depth image seen
   // fp_register_objects / _cameras: row offsets of the objects' hypotheses [M + 1] and the objects' camera ids [M], the
   // objects' feature rows [sum N][512], each object's byte offset into mask_buf
   fp::DevBuf seg_off, reg_feats, mask_off;
@@ -311,6 +320,7 @@ int segmented_tail_params(fp_ctx* c, const float* feats, const int* off_host, in
 // fp_api.cu
 int order_after_track(fp_ctx* c, cudaStream_t st);
 int check_slots(const fp_ctx* c, int M, const int* slots, const char* caller);
+int check_depth_sensor(const fp_depth_sensor_t* s, const char* caller);
 
 }  // namespace fp
 

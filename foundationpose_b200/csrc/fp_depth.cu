@@ -193,6 +193,93 @@ int frame_prep_cameras_launch(const CameraDev* cams, const FrameFmtDev* fmts, in
   return 0;
 }
 
+// Depth from its own sensor aligned to the colour camera, librealsense's rs2::align rule for depth -> colour (the rule
+// is restated in include/fpose.h, fp_set_camera_depth_sensor): one thread per depth pixel deprojects the two corners of
+// its pixel at its depth, moves them into the colour camera, projects them and writes the slot of its z
+// (aligned_slot_of) into every colour pixel of the rectangle they span with an atomicMax, so each colour pixel keeps
+// the smallest z that covers it whatever the order of the threads.  Every operation is rounded on its own (no FMA
+// contraction), as numpy float32 computes it.  The caller zeroes the aligned buffer first.
+// kTable: blockIdx.z selects the camera's entries of the sensor table `sensors` and the camera table `cams` (colour
+// intrinsics and size); the grid covers the largest depth image, and a camera without a sensor or a block outside its
+// depth image leaves at once.  Otherwise the sensor `one` aligns to the colour frame `colour`, both by value.
+constexpr int kAlW = 32, kAlH = 8;
+
+template <bool kTable>
+__global__ void __launch_bounds__(kAlW* kAlH) align_depth_kernel(const SensorDev one, const CameraDev colour,
+                                                                 const SensorDev* __restrict__ sensors,
+                                                                 const CameraDev* __restrict__ cams) {
+  const SensorDev& s = kTable ? sensors[blockIdx.z] : one;
+  if (kTable && !s.aligned) return;
+  const int x = blockIdx.x * kAlW + threadIdx.x, y = blockIdx.y * kAlH + threadIdx.y;
+  if (x >= s.W || y >= s.H) return;
+  const char* row = static_cast<const char*>(s.depth) + (size_t)y * s.pitch;
+  float z;
+  if (s.u16) {
+    const unsigned short r = __ldg(reinterpret_cast<const unsigned short*>(row) + x);
+    if (r == 0) return;
+    z = __fmul_rn((float)r, s.scale);
+  } else {
+    z = __ldg(reinterpret_cast<const float*>(row) + x);
+    if (z == 0.f) return;
+  }
+  const CameraDev& c = kTable ? cams[blockIdx.z] : colour;
+  float xi[2], yi[2], zc[2];
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    const float px = __fadd_rn((float)x, k ? 0.5f : -0.5f), py = __fadd_rn((float)y, k ? 0.5f : -0.5f);
+    const float X = __fmul_rn(__fdiv_rn(__fsub_rn(px, s.cx), s.fx), z);
+    const float Y = __fmul_rn(__fdiv_rn(__fsub_rn(py, s.cy), s.fy), z);
+    float P[3];
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+      P[r] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(s.T[4 * r], X), __fmul_rn(s.T[4 * r + 1], Y)), __fmul_rn(s.T[4 * r + 2], z)),
+                       s.T[4 * r + 3]);
+    const float u = __fadd_rn(__fmul_rn(__fdiv_rn(P[0], P[2]), c.fx), c.cx);
+    const float v = __fadd_rn(__fmul_rn(__fdiv_rn(P[1], P[2]), c.fy), c.cy);
+    xi[k] = truncf(__fadd_rn(u, 0.5f));
+    yi[k] = truncf(__fadd_rn(v, 0.5f));
+    zc[k] = P[2];
+  }
+  // on the float values, so that NaN and values beyond int fail here
+  if (!(zc[0] > 0.f && zc[1] > 0.f)) return;
+  if (!(xi[0] >= 0.f && xi[0] <= xi[1] && xi[1] <= (float)(c.W - 1))) return;
+  if (!(yi[0] >= 0.f && yi[0] <= yi[1] && yi[1] <= (float)(c.H - 1))) return;
+  const unsigned int slot = aligned_slot_of(z);
+  const int x0 = (int)xi[0], x1 = (int)xi[1], y0 = (int)yi[0], y1 = (int)yi[1];
+  for (int yy = y0; yy <= y1; ++yy)
+    for (int xx = x0; xx <= x1; ++xx) atomicMax(s.aligned + (size_t)yy * c.W + xx, slot);
+}
+
+int align_depth_launch(const SensorDev& s, const CameraDev& colour, cudaStream_t stream) {
+  dim3 block(kAlW, kAlH), grid((s.W + kAlW - 1) / kAlW, (s.H + kAlH - 1) / kAlH);
+  align_depth_kernel<false><<<grid, block, 0, stream>>>(s, colour, nullptr, nullptr);
+  note_launches(1);
+  FP_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int align_depth_cameras_launch(const SensorDev* sensors, const CameraDev* cams, int C, int max_H, int max_W,
+                               cudaStream_t stream) {
+  dim3 block(kAlW, kAlH), grid((max_W + kAlW - 1) / kAlW, (max_H + kAlH - 1) / kAlH, C);
+  align_depth_kernel<true><<<grid, block, 0, stream>>>(SensorDev{}, CameraDev{}, sensors, cams);
+  note_launches(1);
+  FP_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// An aligned buffer of n slots to float32 metres in place (fp_align_depth)
+__global__ void aligned_to_depth_kernel(unsigned int* __restrict__ buf, size_t n) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) reinterpret_cast<float*>(buf)[i] = aligned_depth_of(buf[i]);
+}
+
+int aligned_to_depth_launch(unsigned int* buf, size_t n, cudaStream_t stream) {
+  aligned_to_depth_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(buf, n);
+  note_launches(1);
+  FP_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
 int erode_depth_launch(const float* depth, float* out, int H, int W, int radius, float diff_thres, float ratio_thres,
                        float zfar, cudaStream_t stream) {
   dim3 block(32, 8), grid((W + 31) / 32, (H + 7) / 8);

@@ -12,7 +12,7 @@ import torch
 
 from . import _lib, packing
 from ._lib import lib
-from .frames import DEFAULT_FORMAT, Color, Depth, frame_format
+from .frames import DEFAULT_FORMAT, Color, Depth, depth_sensor, frame_format
 
 CROP_SHAPE = (166, 2, 84, 8)  # padded fp16 crop image consumed by the stem convolution: rows x {even, odd cols} x pairs x ch
 
@@ -34,6 +34,7 @@ def _proto():
     lib.fp_mesh_info.argtypes = [vp, C.POINTER(i)]
     lib.fp_set_crop_tile.argtypes = [vp, i]
     lib.fp_set_camera_format.argtypes = [vp, i, C.POINTER(_FpFrameFormat)]
+    lib.fp_set_camera_depth_sensor.argtypes = [vp, i, C.POINTER(_lib.DepthSensor)]
     lib.fp_crop_stats.argtypes = [vp, vp, i, i, C.POINTER(i), vp]
     lib.fp_track.argtypes = [vp, vp, vp, C.POINTER(f), i, i, vp, i, vp, vp, vp]
     lib.fp_track_objects.argtypes = [vp, vp, vp, C.POINTER(f), i, i, i, C.POINTER(i), vp, i, vp, vp, vp]
@@ -83,7 +84,7 @@ def _proto():
     lib.fp_vis_crops.argtypes = [vp, vp, i, i, vp, vp]
     lib.fp_vis_workspace_bytes.argtypes = [vp]
     lib.fp_vis_workspace_bytes.restype = C.c_ulonglong
-    for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_set_camera_format", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_track_cameras", "fp_track_submit", "fp_track_objects_submit",
+    for name in ("fp_create", "fp_destroy", "fp_set_config", "fp_mesh_info", "fp_set_crop_tile", "fp_set_camera_format", "fp_set_camera_depth_sensor", "fp_crop_stats", "fp_track", "fp_track_objects", "fp_track_cameras", "fp_track_submit", "fp_track_objects_submit",
                  "fp_track_cameras_submit", "fp_track_wait", "fp_track_cameras_fit_submit", "fp_track_fit_wait", "fp_register_objects", "fp_register_cameras", "fp_set_xyz_map", "fp_load_network", "fp_set_mesh",
                  "fp_set_mesh_slot", "fp_set_frame",
                  "fp_get_depth", "fp_make_crops", "fp_start_poses", "fp_refine", "fp_score", "fp_score_features", "fp_score_tail",
@@ -125,16 +126,19 @@ def _check_wrapped_device(x, what, device):
 
 
 def _frame(rgb, depth, what, device=None):
-    """One camera's frame as the tracking and register calls take it: (rgb, depth, (H, W), format).  Each buffer is a
-    host array (made a contiguous uint8 / float32 numpy array, staged by the library) or a CUDA tensor on the engine's
-    device, read in place in stream order: rgb uint8 (H,W,3), depth (H,W) converted to float32, both made contiguous.  A
-    Color / Depth (frames.py) is taken as it is, in its own layout, wherever it lives; format is the camera format of
-    the pair (frames.frame_format)."""
-    fmt = frame_format(rgb, depth)
+    """One camera's frame as the tracking and register calls take it: (rgb, depth, (H, W), format, sensor).  Each buffer
+    is a host array (made a contiguous uint8 / float32 numpy array, staged by the library) or a CUDA tensor on the
+    engine's device, read in place in stream order: rgb uint8 (H,W,3), depth (H,W) converted to float32, both made
+    contiguous.  A Color / Depth (frames.py) is taken as it is, in its own layout, wherever it lives; format is the camera
+    format of the pair (frames.frame_format), sensor its depth sensor (frames.depth_sensor).  (H, W) is the colour
+    frame's: with a depth sensor the depth image has the sensor's own size."""
+    fmt, sensor = frame_format(rgb, depth), depth_sensor(depth)
     if isinstance(depth, Depth):
         _check_wrapped_device(depth, what, device)
         H, W = depth.H, depth.W
         depth = depth.img
+        if sensor is not None:  # the frame is the colour camera's
+            H, W = (rgb.H, rgb.W) if isinstance(rgb, Color) else tuple(rgb.shape if torch.is_tensor(rgb) else np.shape(rgb))[:2]
     elif _on_device(depth):
         if depth.dim() != 2:
             raise ValueError(f"{what}: depth must be (H, W), got {tuple(depth.shape)}")
@@ -145,7 +149,7 @@ def _frame(rgb, depth, what, device=None):
         H, W = depth.shape
     if isinstance(rgb, Color):
         _check_wrapped_device(rgb, what, device)
-        if (rgb.H, rgb.W) != (H, W):
+        if (rgb.H, rgb.W) != (H, W):  # with a sensor (H, W) is the colour frame's already
             raise ValueError(f"{what}: the colour frame is {rgb.H} x {rgb.W}, the depth frame {H} x {W}")
         rgb = rgb.img
     elif _on_device(rgb):
@@ -156,7 +160,7 @@ def _frame(rgb, depth, what, device=None):
         rgb = rgb.contiguous()
     else:
         rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
-    return rgb, depth, (int(H), int(W)), fmt
+    return rgb, depth, (int(H), int(W)), fmt, sensor
 
 
 def _device_mask(m):
@@ -175,15 +179,17 @@ def _hold(bufs):
     return held
 
 
-def _camera_args(frames):
+def _camera_args(frames, hw=None):
     """The (rgb pointers, depth pointers, K [C][9], H, W) arguments of the multi-camera calls for (rgb, depth, K) frames
-    whose buffers _frame made."""
+    whose buffers _frame made.  hw: each camera's colour frame size (H, W) as _frame gives it; None: the depth's shape
+    (no camera has a depth sensor)."""
     n_cam = len(frames)
+    hw = [tuple(depth.shape[:2]) for _, depth, _ in frames] if hw is None else hw
     rgbs = (C.c_void_p * n_cam)(*[_ptr(rgb).value for rgb, _, _ in frames])
     depths = (C.c_void_p * n_cam)(*[_ptr(depth).value for _, depth, _ in frames])
     Ks = (C.c_float * (9 * n_cam))(*[float(x) for _, _, K in frames for x in np.asarray(K, dtype=np.float64).reshape(-1)])
-    Hs = (C.c_int * n_cam)(*[int(depth.shape[0]) for _, depth, _ in frames])
-    Ws = (C.c_int * n_cam)(*[int(depth.shape[1]) for _, depth, _ in frames])
+    Hs = (C.c_int * n_cam)(*[int(h) for h, _ in hw])
+    Ws = (C.c_int * n_cam)(*[int(w) for _, w in hw])
     return rgbs, depths, Ks, Hs, Ws
 
 
@@ -328,6 +334,7 @@ class Engine:
         self._dropped = []  # tickets of PendingPoses dropped without result()
         self._last_ticket = 0
         self._formats = [DEFAULT_FORMAT] * MAX_CAMERAS  # the frame format the context holds for each camera
+        self._sensors = [None] * MAX_CAMERAS  # the depth sensor the context holds for each camera (frames.depth_sensor)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -381,13 +388,20 @@ class Engine:
         _lib.check(lib.fp_crop_stats(self._h, _p(poses), len(poses), mode, st, _stream()), "fp_crop_stats")
         return dict(meshlet_visits=st[0], triangles=st[1], fragments=st[2], near_plane_triangles=st[3])
 
-    def _set_formats(self, fmts):
-        """fp_set_camera_format for camera i = 0, 1, ... wherever fmts[i] differs from the format the context holds."""
+    def _set_formats(self, fmts, sensors=None):
+        """fp_set_camera_format for camera i = 0, 1, ... wherever fmts[i] differs from the format the context holds, and
+        fp_set_camera_depth_sensor wherever sensors[i] (frames.depth_sensor; None: every camera without) differs from
+        the sensor it holds."""
         for i, f in enumerate(fmts):
             if self._formats[i] != f:
                 ff = _FpFrameFormat(*f)
                 _lib.check(lib.fp_set_camera_format(self._h, i, C.byref(ff)), "fp_set_camera_format")
                 self._formats[i] = f
+        for i, sn in enumerate(sensors if sensors is not None else [None] * len(fmts)):
+            if self._sensors[i] != sn:
+                rec = None if sn is None else C.byref(_lib.DepthSensor.of(*sn))
+                _lib.check(lib.fp_set_camera_depth_sensor(self._h, i, rec), "fp_set_camera_depth_sensor")
+                self._sensors[i] = sn
 
     # ---- tracking: every call is a submit and, with wait=True, its fp_track_wait
     def _collect_dropped(self, keep):
@@ -435,9 +449,9 @@ class Engine:
         pose_in (4,4) CUDA tensor or None (continue).
         Returns (pose_out CUDA (4,4), pose host (4,4) float32 numpy).  wait=False returns as soon as the call is
         submitted (the host arrays may then be reused): (pose_out, PendingPoses), pose_out complete in stream order."""
-        rgb, depth, (H, W), fmt = _frame(rgb, depth, "track", self.device_index)
+        rgb, depth, (H, W), fmt, sensor = _frame(rgb, depth, "track", self.device_index)
         Kf = (C.c_float * 9)(*[float(x) for x in np.asarray(K, dtype=np.float64).reshape(-1)])
-        self._set_formats([fmt])
+        self._set_formats([fmt], [sensor])
         if pose_in is not None:
             pose_in = pose_in.reshape(4, 4).contiguous().float()
         if pose_out is None:
@@ -452,14 +466,14 @@ class Engine:
         slot slots[i] (loaded by set_mesh(..., slot=)).  rgb uint8 (H,W,3) / depth float32 (H,W): host arrays or CUDA
         tensors, as `track`; poses_in (M,4,4) CUDA tensor.  Returns (poses CUDA (M,4,4), poses host (M,4,4) float32
         numpy); wait=False as `track`."""
-        rgb, depth, (H, W), fmt = _frame(rgb, depth, "track_objects", self.device_index)
+        rgb, depth, (H, W), fmt, sensor = _frame(rgb, depth, "track_objects", self.device_index)
         Kf = (C.c_float * 9)(*[float(x) for x in np.asarray(K, dtype=np.float64).reshape(-1)])
         poses_in = poses_in.reshape(-1, 4, 4).contiguous().float()
         M = len(poses_in)
         slots = [int(s) for s in slots]
         if len(slots) != M:
             raise ValueError(f"track_objects: {M} poses but {len(slots)} slots")
-        self._set_formats([fmt])
+        self._set_formats([fmt], [sensor])
         out = torch.empty(M, 4, 4, dtype=torch.float32, device="cuda")
         res = self._submit(lib.fp_track_objects_submit, (_ptr(rgb), _ptr(depth), Kf, H, W, M, (C.c_int * M)(*slots), _p(poses_in),
                                                          int(iterations), _p(out)),
@@ -481,6 +495,7 @@ class Engine:
         (poses CUDA, PendingPoses) whose result() gives (poses host, fit).  The poses are those of the call without it."""
         made = [(_frame(rgb, depth, f"track_cameras: camera {c}", self.device_index), K) for c, (rgb, depth, K) in enumerate(frames)]
         frames = [(f[0], f[1], K) for f, K in made]
+        hw = [f[2] for f, _ in made]  # each camera's colour frame size
         n_cam = len(frames)
         poses_in = poses_in.reshape(-1, 4, 4).contiguous().float()
         M = len(poses_in)
@@ -488,8 +503,8 @@ class Engine:
         if len(camera_of) != M or len(slots) != M:
             raise ValueError(f"track_cameras: {M} poses, {len(camera_of)} camera ids and {len(slots)} slots")
         if n_cam <= MAX_CAMERAS:  # more cameras: fp_track_cameras refuses the call
-            self._set_formats([f[3] for f, _ in made])
-        rgbs, depths, Ks, Hs, Ws = _camera_args(frames)
+            self._set_formats([f[3] for f, _ in made], [f[4] for f, _ in made])
+        rgbs, depths, Ks, Hs, Ws = _camera_args(frames, hw)
         out = torch.empty(M, 4, 4, dtype=torch.float32, device="cuda")
         ids = (n_cam, rgbs, depths, Ks, Hs, Ws, M, (C.c_int * M)(*camera_of), (C.c_int * M)(*slots), _p(poses_in), int(iterations))
         bufs = [b for rgb, depth, _ in frames for b in (rgb, depth)]
@@ -500,7 +515,7 @@ class Engine:
                                out, (M, 4, 4), wait, bufs, fit=True)
             if wait:
                 res = (res[0], *res[1])
-        self.frame_hw = tuple(frames[0][1].shape)  # camera 0's frame is the context's frame
+        self.frame_hw = hw[0]  # camera 0's frame is the context's frame
         return res
 
     def register_objects(self, rgb, depth, K, masks, rot_grids, slots, iterations):
@@ -511,7 +526,7 @@ class Engine:
         masks) binarised on the device; rot_grids: M CUDA float32 (N_i,4,4) rotation grids.  Returns CUDA tensors: poses
         (sum N_i,4,4) refined, object-major and unranked; scores (sum N_i,); best (M,) int32, each object's first arg-max
         relative to its own rows; info (M,4) = (tx, ty, tz, n_valid) per object."""
-        rgb, depth, (H, W), fmt = _frame(rgb, depth, "register_objects", self.device_index)
+        rgb, depth, (H, W), fmt, sensor = _frame(rgb, depth, "register_objects", self.device_index)
         if not _on_device(masks) and len(masks) and all(_on_device(m) for m in masks):
             masks = torch.stack(list(masks))
         masks = masks if _on_device(masks) else np.ascontiguousarray(masks)
@@ -534,7 +549,7 @@ class Engine:
         scores = torch.empty(total, dtype=torch.float32, device="cuda")
         best = torch.empty(M, dtype=torch.int32, device="cuda")
         info = torch.empty(M, 4, dtype=torch.float32, device="cuda")
-        self._set_formats([fmt])
+        self._set_formats([fmt], [sensor])
         _lib.check(lib.fp_register_objects(self._h, _ptr(rgb), _ptr(depth), Kf, H, W, M, (C.c_int * M)(*slots), (C.c_int * M)(*n_hyp),
                                            _ptr(masks), _p(grids), int(iterations), _p(poses), _p(scores), _p(best), _p(info),
                                            _stream()),
@@ -551,6 +566,7 @@ class Engine:
         Returns the CUDA tensors of register_objects: poses (sum N_i,4,4), scores (sum N_i,), best (M,), info (M,4)."""
         made = [(_frame(rgb, depth, f"register_cameras: camera {c}", self.device_index), K) for c, (rgb, depth, K) in enumerate(frames)]
         frames = [(f[0], f[1], K) for f, K in made]
+        hw = [f[2] for f, _ in made]  # each camera's colour frame size
         n_cam = len(frames)
         M = len(masks)
         camera_of, slots = [int(c) for c in camera_of], [int(s) for s in slots]
@@ -560,26 +576,26 @@ class Engine:
                              f"{len(rot_grids)} rotation grids")
         masks = [m if _on_device(m) else np.asarray(m) for m in masks]
         for i, (m, c) in enumerate(zip(masks, camera_of)):
-            if 0 <= c < n_cam and tuple(m.shape) != tuple(frames[c][1].shape):
+            if 0 <= c < n_cam and tuple(m.shape) != hw[c]:
                 raise ValueError(f"register_cameras: mask {i} has shape {tuple(m.shape)}, camera {c}'s frame is "
-                                 f"{tuple(frames[c][1].shape)}")
+                                 f"{hw[c]}")
         # the reference tests `mask > 0` (estimater.py:138, :183)
         masks = [_device_mask(m) if _on_device(m) else np.ascontiguousarray(m > 0, dtype=np.uint8) for m in masks]
         n_hyp = [len(g) for g in rot_grids]
         grids = torch.cat(rot_grids).to(device="cuda", dtype=torch.float32).contiguous()
         total = len(grids)
-        rgbs, depths, Ks, Hs, Ws = _camera_args(frames)
+        rgbs, depths, Ks, Hs, Ws = _camera_args(frames, hw)
         poses = torch.empty(total, 4, 4, dtype=torch.float32, device="cuda")
         scores = torch.empty(total, dtype=torch.float32, device="cuda")
         best = torch.empty(M, dtype=torch.int32, device="cuda")
         info = torch.empty(M, 4, dtype=torch.float32, device="cuda")
         if n_cam <= MAX_CAMERAS:  # more cameras: fp_register_cameras refuses the call
-            self._set_formats([f[3] for f, _ in made])
+            self._set_formats([f[3] for f, _ in made], [f[4] for f, _ in made])
         _lib.check(lib.fp_register_cameras(self._h, n_cam, rgbs, depths, Ks, Hs, Ws, M, (C.c_int * M)(*camera_of),
                                            (C.c_int * M)(*slots), (C.c_int * M)(*n_hyp), (C.c_void_p * M)(*[_ptr(m).value for m in masks]),
                                            _p(grids), int(iterations), _p(poses), _p(scores), _p(best), _p(info), _stream()),
                    "fp_register_cameras")  # synchronises its stream: the device inputs are free again on return
-        self.frame_hw = tuple(frames[0][1].shape)  # camera 0's frame is the context's frame
+        self.frame_hw = hw[0]  # camera 0's frame is the context's frame
         return poses, scores, best, info
 
     def set_frame(self, rgb, depth, K, filter_depth=True, zfar=float("inf")):
@@ -588,9 +604,9 @@ class Engine:
         may be reused once this returns."""
         Kf = (C.c_float * 9)(*[float(x) for x in np.asarray(K, dtype=np.float64).reshape(-1)])
         flags = FRAME_FILTER_DEPTH if filter_depth else 0
-        fmt = DEFAULT_FORMAT
+        fmt, sensor = DEFAULT_FORMAT, None
         if isinstance(rgb, Color) or isinstance(depth, Depth):
-            rgb, depth, _, fmt = _frame(rgb, depth, "set_frame", self.device_index)
+            rgb, depth, (H, W), fmt, sensor = _frame(rgb, depth, "set_frame", self.device_index)
             if _on_device(rgb) != _on_device(depth):
                 raise ValueError("set_frame: rgb and depth must both be CUDA tensors or both be on the host")
             if _on_device(rgb):
@@ -609,11 +625,12 @@ class Engine:
             rgb = rgb.contiguous()
             depth = depth.contiguous()
             assert rgb.dtype == torch.uint8 and depth.dtype == torch.float32
-        H, W = depth.shape
+        if sensor is None:
+            H, W = depth.shape
         # device and page-locked frames are read in place after the call returns, in stream order: keep them until then
         in_place = rgb.is_cuda or (rgb.is_pinned() and depth.is_pinned())
         self._frame_keep = (rgb, depth) if in_place else None
-        self._set_formats([fmt])
+        self._set_formats([fmt], [sensor])
         _lib.check(lib.fp_set_frame(self._h, _p(rgb), _p(depth), Kf, H, W, flags, float(zfar), _stream()), "fp_set_frame")
         self.frame_hw = (H, W)
 

@@ -24,7 +24,7 @@ import torch
 
 from . import hypotheses, meshprep, synth, weights
 from .engine import MAX_CAMERAS, MAX_MESHES, Engine
-from .frames import host_rgb, image, on_cuda
+from .frames import frame_hw, host_rgb, image, on_cuda
 
 
 @dataclasses.dataclass(frozen=True)
@@ -360,7 +360,7 @@ class FoundationPose:
             cv2.imwrite(f"{self.debug_dir}/color.png", np.ascontiguousarray(rgb_h[..., ::-1]))
             cv2.imwrite(f"{self.debug_dir}/depth.png", (depth_f * 1000).astype(np.uint16))
             self._write_cloud("scene_complete.ply", xyz, rgb_h)
-        self.H, self.W = depth.shape[:2]
+        self.H, self.W = frame_hw(rgb, depth)
         self.K = K
         self.ob_id = ob_id
         self.ob_mask = ob_mask
@@ -657,7 +657,7 @@ def register_objects(estimators, K, rgb, depth, ob_masks, ob_ids=None, iteration
     M = len(estimators)
     if len(masks) != M:
         raise ValueError(f"register_objects: {M} estimators but {len(masks)} masks")
-    H, W = np.shape(depth)[:2]
+    H, W = frame_hw(rgb, depth)
     for i, m in enumerate(masks):
         if m.shape != (H, W):
             raise ValueError(f"register_objects: mask {i} has shape {m.shape}, the frame is {(H, W)}")
@@ -702,7 +702,7 @@ def register_cameras(views, ob_ids=None, iteration=5):
     masks, ob_masks, ids, frames, camera_of = [], [], [], [], []
     for j, c in enumerate(used):
         ests, rgb, depth, K, ms = views[c]
-        H, W = np.shape(depth)[:2]
+        H, W = frame_hw(rgb, depth)
         if len(ms) != len(ests):
             raise ValueError(f"register_cameras: camera {c}: {len(ests)} estimators but {len(ms)} masks")
         for i, m in enumerate(ms):

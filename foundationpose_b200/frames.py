@@ -11,7 +11,14 @@ are.  A uint16 depth becomes `np.float32(v) * np.float32(scale)` in metres, one 
 bit what the same call gives on that host-converted frame; 0 stays invalid.
 
 A plain uint16 array passed where depth is expected (no `Depth`) is cast to float32 as it always was: its values are
-then taken as metres.  Wrap it in `Depth(img, scale)` instead."""
+then taken as metres.  Wrap it in `Depth(img, scale)` instead.
+
+    Depth(img, scale, sensor=DepthSensor(K, T_color_from_depth))
+
+is depth from a depth imager of its own (fp_set_camera_depth_sensor, include/fpose.h): `img` is the depth sensor's
+(Hd, Wd) image, K its intrinsics and T_color_from_depth the rigid transform from the depth camera to the colour camera
+(4x4, metres).  The library aligns it to the colour frame on the GPU by librealsense's rs2::align rule, so the call's
+frame size, K and masks are the colour camera's."""
 import math
 
 import numpy as np
@@ -19,6 +26,7 @@ import torch
 
 COLOR_RGB8, COLOR_BGR8, COLOR_RGBA8, COLOR_BGRA8 = 0, 1, 2, 3  # FP_COLOR_* (include/fpose.h)
 DEPTH_F32, DEPTH_U16 = 0, 1  # FP_DEPTH_*
+DEPTH_SENSOR_MAX_DIM = 4096  # FP_DEPTH_SENSOR_MAX_DIM
 DEFAULT_FORMAT = (COLOR_RGB8, DEPTH_F32, 0.0, 0, 0)  # (color, depth, depth_scale, rgb_pitch, depth_pitch): packed RGB8 + float32
 
 _ORDERS = {"rgb": (COLOR_RGB8, 3), "bgr": (COLOR_BGR8, 3), "rgba": (COLOR_RGBA8, 4), "bgra": (COLOR_BGRA8, 4)}
@@ -71,11 +79,34 @@ class Color:
         return tuple(self.img.shape)
 
 
+class DepthSensor:
+    """A depth imager of its own (see the module docstring): K (3,3) its intrinsics (fx, fy > 0) and T_color_from_depth
+    (4,4) the rigid transform from the depth camera to the colour camera, in metres, both finite in float32.  From
+    pyrealsense2: T[:3, :3] = np.reshape(extr.rotation, (3, 3)).T, T[:3, 3] = extr.translation, with extr the depth
+    stream profile's get_extrinsics_to(colour profile)."""
+
+    def __init__(self, K, T_color_from_depth):
+        with np.errstate(over="ignore", invalid="ignore"):
+            K = np.asarray(K, dtype=np.float64).astype(np.float32)
+            T = np.asarray(T_color_from_depth, dtype=np.float64).astype(np.float32)
+        if K.shape != (3, 3) or T.shape != (4, 4):
+            raise ValueError(f"DepthSensor: K must be (3, 3) and T_color_from_depth (4, 4), got {K.shape} and {T.shape}")
+        if not (np.isfinite(K).all() and np.isfinite(T).all()):
+            raise ValueError("DepthSensor: K and T_color_from_depth must be finite in float32")
+        if not (K[0, 0] > 0 and K[1, 1] > 0):
+            raise ValueError(f"DepthSensor: focal lengths must be > 0, got fx = {K[0, 0]}, fy = {K[1, 1]}")
+        self.K, self.T = K, T
+
+
 class Depth:
     """A camera's depth frame as the sensor delivers it (see the module docstring): `img` float32 (H,W) metres with
-    scale=None, or uint16 (H,W) with `scale` metres per unit (finite and > 0 in float32)."""
+    scale=None, or uint16 (H,W) with `scale` metres per unit (finite and > 0 in float32).  sensor: a DepthSensor when
+    the image is a depth imager's own (H,W), aligned to the colour frame by the library."""
 
-    def __init__(self, img, scale=None):
+    def __init__(self, img, scale=None, sensor=None):
+        if sensor is not None and not isinstance(sensor, DepthSensor):
+            raise TypeError(f"Depth: sensor must be a DepthSensor or None, got {type(sensor).__name__}")
+        self.sensor = sensor
         if scale is None:
             self.code, self.scale = DEPTH_F32, 0.0
             what, np_dtype, torch_dtype = "Depth(scale=None)", np.float32, torch.float32
@@ -88,6 +119,8 @@ class Depth:
             what, np_dtype, torch_dtype = f"Depth(scale={scale!r})", np.uint16, torch.uint16
         self.img = img
         (self.H, self.W), self.pitch = _layout(img, what, 0, np_dtype, torch_dtype)
+        if sensor is not None and max(self.H, self.W) > DEPTH_SENSOR_MAX_DIM:
+            raise ValueError(f"Depth: a depth sensor's image is at most {DEPTH_SENSOR_MAX_DIM} pixels a side, got {self.H} x {self.W}")
 
     @property
     def shape(self):
@@ -97,6 +130,13 @@ class Depth:
 def image(x):
     """The array or tensor behind a frame argument: a wrapper's image, or the argument itself."""
     return x.img if isinstance(x, (Color, Depth)) else x
+
+
+def frame_hw(rgb, depth):
+    """The (H, W) of a camera's frame arguments: the depth's, or the colour's when the depth comes from a sensor of its
+    own (Depth(sensor=))."""
+    x = rgb if isinstance(depth, Depth) and depth.sensor is not None else depth
+    return tuple(int(n) for n in (x.shape if isinstance(x, (Color, Depth)) or torch.is_tensor(x) else np.shape(x))[:2])
 
 
 def on_cuda(x):
@@ -120,3 +160,12 @@ def frame_format(rgb, depth):
     c = (rgb.code, rgb.pitch) if isinstance(rgb, Color) else (COLOR_RGB8, 0)
     d = (depth.code, depth.scale, depth.pitch) if isinstance(depth, Depth) else (DEPTH_F32, 0.0, 0)
     return (c[0], d[0], d[1], c[1], d[2])
+
+
+def depth_sensor(depth):
+    """The (H, W, K, T) depth sensor of a depth frame argument for fp_set_camera_depth_sensor (K 9 and T 16 floats,
+    row-major), or None: plain arrays and a Depth without a sensor are in the colour frame's geometry."""
+    if not isinstance(depth, Depth) or depth.sensor is None:
+        return None
+    return (depth.H, depth.W, tuple(float(x) for x in depth.sensor.K.reshape(-1)),
+            tuple(float(x) for x in depth.sensor.T.reshape(-1)))

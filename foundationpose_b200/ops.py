@@ -135,3 +135,36 @@ def token_mean_proj(x, w, bias):
     _lib.check(lib.fp_op_token_mean_proj(_ptr(x), _ptr(w), _ptr(bias), _ptr(mean_ws), _ptr(out), B, _stream()),
                "fp_op_token_mean_proj")
     return out
+
+
+lib.fp_align_depth.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_longlong, C.POINTER(_lib.DepthSensor), C.POINTER(C.c_float),
+                               C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+lib.fp_align_depth.restype = C.c_int
+
+
+def align_depth(depth, sensor, K_color, H, W):
+    """Depth from its own sensor aligned to a colour frame of H x W with intrinsics K_color (3,3), by the rule of
+    fp_set_camera_depth_sensor (include/fpose.h, librealsense's rs2::align to colour): a CUDA float32 (H, W) tensor of
+    metres, 0 where no depth lands.  depth: a frames.Depth around a CUDA tensor (float32 metres or uint16 with a scale,
+    any row pitch) of the sensor's own size, or a plain CUDA float32 (Hd, Wd) tensor with `sensor` a frames.DepthSensor.
+    Runs on the current stream."""
+    from .frames import Depth, DepthSensor
+
+    if not isinstance(depth, Depth):
+        if not isinstance(sensor, DepthSensor):
+            raise TypeError("align_depth: a plain depth tensor needs a DepthSensor")
+        depth = Depth(depth, sensor=sensor)
+    elif sensor is not None and depth.sensor is not None and sensor is not depth.sensor:
+        raise ValueError("align_depth: the Depth has a sensor of its own; pass sensor=None")
+    sensor = depth.sensor if depth.sensor is not None else sensor
+    if not isinstance(sensor, DepthSensor):
+        raise TypeError("align_depth: needs a DepthSensor")
+    img = depth.img
+    if not (torch.is_tensor(img) and img.is_cuda):
+        raise _lib.FposeError("align_depth: the depth must be a CUDA tensor (there is no CPU path)")
+    rec = _lib.DepthSensor.of(depth.H, depth.W, sensor.K.reshape(-1), sensor.T.reshape(-1))
+    Kc = (C.c_float * 9)(*[float(x) for x in torch.as_tensor(K_color, dtype=torch.float64).reshape(-1)])
+    out = torch.empty(int(H), int(W), dtype=torch.float32, device=img.device)
+    _lib.check(lib.fp_align_depth(_ptr(img), depth.code, float(depth.scale), depth.pitch, C.byref(rec), Kc, int(H), int(W),
+                                  _ptr(out), _stream()), "fp_align_depth")
+    return out

@@ -267,6 +267,36 @@ typedef struct fp_frame_format {
   int depth_pitch;
 } fp_frame_format_t;
 int fp_set_camera_format(fp_ctx* ctx, int camera, const fp_frame_format_t* fmt);
+/* Depth from its own sensor.  A camera may be given a depth sensor: the depth image's size H x W, its intrinsics K
+ * (row-major 3x3; only fx = K[0], fy = K[4], cx = K[2], cy = K[5] are read) and the rigid transform from the depth
+ * camera to the colour camera T_color_from_depth (row-major 4x4, metres; only its top three rows are read).  Every
+ * later frame-taking call then reads that camera's depth buffer as the depth sensor's H x W image, in the camera's
+ * depth format and pitch (fp_set_camera_format), and aligns it to the colour frame on the device before the frame
+ * filter, by librealsense's rs2::align rule for depth to colour, in fp32 with every operation rounded on its own: for
+ * every depth pixel (x, y) whose raw value is not 0, with z its depth in metres, the corners (x - 0.5, y - 0.5) and
+ * (x + 0.5, y + 0.5) are deprojected with the depth intrinsics at z, moved by T and projected with the colour
+ * intrinsics (the call's K) to (u, v), rounded as (int)(u + 0.5), (int)(v + 0.5).  Unless Z > 0 at both corners and
+ * 0 <= x0 <= x1 <= W - 1, 0 <= y0 <= y1 <= H - 1 (colour W x H), the pixel is dropped; otherwise every colour pixel
+ * of [x0, x1] x [y0, y1] takes the smallest z of all depth pixels that cover it, and a pixel nothing covers is 0.
+ * The stored value is the depth sensor's z, as rs2::align stores it.  The call's H, W, K and masks stay the colour
+ * frame's.  Like fp_set_camera_format this is host state that a call copies when it is staged; it refuses a camera
+ * outside [0, FP_MAX_CAMERAS), H or W outside [1, FP_DEPTH_SENSOR_MAX_DIM], a K or T that is not finite, and fx <= 0 or
+ * fy <= 0.  s = NULL removes the camera's sensor.  Honoured by fp_set_frame, fp_track*, fp_register_objects (camera
+ * 0) and fp_register_cameras; a frame-taking call checks the depth pitch against the sensor's W.  A new sensor, depth
+ * size or depth address replays the cached graphs. */
+#define FP_DEPTH_SENSOR_MAX_DIM 4096
+typedef struct fp_depth_sensor {
+  int H, W;
+  float K[9];
+  float T_color_from_depth[16];
+} fp_depth_sensor_t;
+int fp_set_camera_depth_sensor(fp_ctx* ctx, int camera, const fp_depth_sensor_t* s);
+/* The alignment above as an operator, with no context: depth (device memory, s->H rows depth_pitch bytes apart, 0 =
+ * packed) in depth_format FP_DEPTH_F32 or FP_DEPTH_U16 (times depth_scale) is aligned to a colour frame of H x W with
+ * intrinsics K_color (host, row-major 3x3) into out (device, float32 [H][W] metres, 0 where nothing lands), on `stream`
+ * of the current device.  Every pointer is checked before anything is enqueued. */
+int fp_align_depth(const void* depth, int depth_format, float depth_scale, long long depth_pitch, const fp_depth_sensor_t* s,
+                   const float* K_color, int H, int W, float* out, void* stream);
 /* Replaces the xyz map derived by fp_set_frame with the caller's own (PoseRefinePredictor.predict's `xyz_map`
  * argument, predict_pose_refine.py:150,177): float32 [H][W][3], host or device pointer. */
 int fp_set_xyz_map(fp_ctx* ctx, const float* xyz, void* stream);
